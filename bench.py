@@ -146,7 +146,7 @@ def reference_main(args, rank):
 
 def torch_gpu_main(args, rank, local_rank):
     """BASELINE.md section 3: the same workload on stock PyTorch library kernels (cuDNN / cuBLAS / cuFFT, fp32, TF32 off,
-    cudnn.benchmark) on ONE B200 -- "the practical kernel to beat".  Informational: printed with impl = torch_gpu and the
+    cudnn.benchmark) on ONE GPU -- "the practical kernel to beat".  Informational: printed with impl = torch_gpu and the
     key gpu_library_baseline; never part of the product path."""
     if rank != 0:
         return
@@ -197,7 +197,7 @@ def side_workload_main(args, rank, local_rank):
     W = max(3, args.warmup)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    bf16 = json.load(open(peaks_path)).get("bf16_tflops_sustained", 1437.7) if os.path.exists(peaks_path) else 1400.0
+    bf16 = json.load(open(peaks_path)).get("bf16_tflops_sustained", 989.0) if os.path.exists(peaks_path) else 989.0   # H100 SXM data sheet, dense
     if args.workload == "c1":
         g = K.Generator(**G_PARAMS).to(dev).eval()
         g.remove_weight_norm()
@@ -322,6 +322,9 @@ def main():
     ap.add_argument("--graph", action="store_true", help="same as --launch graph")
     ap.add_argument("--graph-selftest", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--ncu", action="store_true", help="profiling mode: 1 warm-up + K steps, nothing else (not a bench number)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its losses, a fixed sample of every "
+                         "model's updated parameters) as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", 0))
@@ -380,7 +383,7 @@ def main():
     y_h, x_h = synth_batch(B_PER_GPU, 1234 + rank)
     y_h, x_h = y_h.pin_memory(), x_h.pin_memory()
     y_d, x_d = y_h.to(dev), x_h.to(dev)
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)   # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -446,13 +449,15 @@ def main():
         dist.all_reduce(t2, op=dist.ReduceOp.MAX)
     e2e_value = world * B_PER_GPU * T_WAV / (float(t2) / args.steps * 1e-3)
     clocks = sampler.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, log, model)
 
     line = {
         "metric": "hifigan_train_step_audio_samples_per_sec", "value": value, "unit": "samples/s",
         "n_gpus": world, "steps": args.steps, "warmup": W, "ms_per_step": ms_per_step, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "global_batch": B_PER_GPU * world, "segment": T_WAV, "parallelism": f"dp{world}",
-                   "precision": "fp32 storage; tcgen05 layers bf16x3 split (fp32-equivalent), others exact fp32 FFMA",
+                   "precision": "fp32 storage; tensor-core layers bf16x3 split (fp32-equivalent), others exact fp32 FFMA",
                    "l2": "explicit 256 MB flush write between timed iterations",
                    "launch": ("2 CUDA graphs per step (replay) + eager Adam / NCCL between them" if use_graph else
                               "eager launches; independent sub-discriminators / parallel resblocks on side streams") + launch_note,
@@ -478,6 +483,23 @@ def main():
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, log, model, param_sample=1 << 20):
+    """What the last timed step computed, for comparing two builds output for output: every tensor of the step's log
+    (the losses, float64) and a fixed, seeded sample of `param_sample` parameters of every model after that step's
+    optimizer update (float32; the generator and each discriminator, 4 MB each)."""
+    import re
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in log.items():
+        if torch.is_tensor(v):
+            np.save(os.path.join(out_dir, re.sub(r"[^A-Za-z0-9_.-]", "_", k) + ".npy"), v.detach().double().cpu().numpy())
+    mods = {"generator": model["generator"], **{f"discriminator_{k}": v for k, v in model["discriminator"].items()}}
+    for name, m in mods.items():
+        flat = torch.cat([p.detach().reshape(-1).float().cpu() for p in m.parameters()])
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:param_sample].sort().values
+        np.save(os.path.join(out_dir, f"{name}_params_sample.npy"), flat[idx].numpy())
+
+
 def graph_selftest(dev):
     """Child-process check: eager warm-up, capture, a few replays, finite losses."""
     import kantts_b200 as K
@@ -499,7 +521,7 @@ def graph_selftest(dev):
 def roofline_leg(step, batch, ops, ms_per_step):
     """One extra instrumented step: every conv library call is bracketed by CUDA events on the
     launching stream; the dominant kernel class's achieved algorithmic rate is reported against the
-    measured peak (MEASURED_PEAKS.json, else the B200_PROFILING.md fallback)."""
+    measured peak (MEASURED_PEAKS.json, else the H100 SXM data-sheet figures)."""
     from kantts_b200 import hifigan
     step.invalidate_weight_caches()        # eager launches after graph replays: prepared weights must be rebuilt
     # side streams OFF for this step: with concurrent streams an event pair around one launch also measures the
@@ -522,9 +544,9 @@ def roofline_leg(step, batch, ops, ms_per_step):
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(peaks_path):
         pk = json.load(open(peaks_path))
-        bf16, hbm, src = pk.get("bf16_tflops_sustained", 1437.7), pk.get("hbm_gbs", 6565.8), "measured"
+        bf16, hbm, src = pk.get("bf16_tflops_sustained", 989.0), pk.get("hbm_gbs", 3350.0), "measured"
     else:
-        bf16, hbm, src = 1400.0, 6650.0, "fallback"
+        bf16, hbm, src = 989.0, 3350.0, "H100 SXM data sheet (not reached)"
     total_ms = sum(v["ms"] for v in summ.values())
     shares = {k: {"calls": v["calls"], "ms": round(v["ms"], 3), "share_of_instrumented": round(v["ms"] / total_ms, 4),
                   "tflops_algorithmic": round(v["flops"] / (v["ms"] * 1e-3) / 1e12, 2) if v["ms"] > 0 else None,

@@ -1,5 +1,5 @@
 /*
- * kantts_b200.h -- C ABI of libkantts_b200.so, the sm_100a implementation of the
+ * kantts_b200.h -- C ABI of libkantts_b200.so, the sm_90a implementation of the
  * KAN-TTS HiFi-GAN hot path (generator / discriminator convolutions, DWT pooling,
  * mel-spectrogram loss).
  *
@@ -42,9 +42,9 @@ extern "C" {
 #define KT_ACT_TANH 2  /* output side only */
 
 /* compute paths */
-#define KT_PATH_AUTO 0  /* tcgen05 where the shape qualifies, FFMA otherwise */
+#define KT_PATH_AUTO 0  /* tensor-core where the shape qualifies, FFMA otherwise */
 #define KT_PATH_FFMA 1  /* exact-fp32 CUDA-core kernels */
-#define KT_PATH_TC 2    /* tcgen05 split-bf16 (bf16x3) tensor-core kernels; error if unsupported */
+#define KT_PATH_TC 2    /* tensor-core split-bf16 (bf16x3) tensor-core kernels; error if unsupported */
 
 /* One 1-D convolution layer (forward semantics; the backward entry points take the
  * SAME descriptor).  Replaces F.conv1d / F.conv_transpose1d / F.conv2d((k,1)) as
@@ -81,7 +81,7 @@ typedef struct KtConv1dDesc {
  * kt_weight_prepare from the reference parameter layout:
  *   conv       reference (Cout, Cin/g, k):  w_fwd[k][Cin/g][Cout]   w_bwd[k][Cout/g][Cin]
  *   transposed reference (Cin, Cout, k)  :  w_fwd[k][Cin][Cout]     w_bwd[k][Cout][Cin]
- * Both are fp32; kt_weight_pack_tc turns either into the split-bf16 tiles of the tcgen05 path. */
+ * Both are fp32; kt_weight_pack_tc turns either into the split-bf16 tiles of the tensor-core path. */
 
 /* Weight re-parametrisation + layout (replaces torch._weight_norm at layers.py:29,67,
  * 105,139 and hifigan.py:224,331; plain / spectral-normed weights use mode 0 with an
@@ -124,9 +124,9 @@ int kt_conv1d_bwd_data(const KtConv1dDesc* d, const float* dy, const float* y, c
 int kt_conv1d_bwd_weight(const KtConv1dDesc* d, const float* x, const float* dy, const float* y,
                          float* dw, float* dbias, void* stream);
 
-/* ---- tcgen05 (5th-gen tensor core) path: bf16x3 split-precision implicit GEMM, fp32 accumulation in TMEM ----
+/* ---- tensor-core (wgmma) path: bf16x3 split-precision implicit GEMM, fp32 accumulation in registers ----
  * kt_conv1d_tc_plan: returns the (padded) output-channel tile NT > 0 when direction `dir` (0 forward, 1 data
- * gradient) of the layer can run on the tcgen05 kernel, else 0.  Any stride / period / group count /
+ * gradient) of the layer can run on the tensor-core kernel, else 0.  Any stride / period / group count /
  * channel count qualifies (channels are zero-padded to 64-wide K chunks and 16-wide N tiles; a grouped
  * conv maps one group to one N tile); only the nearest-upsampled data gradient stays on the FFMA path.
  * kt_conv1d_tc_image_bytes / kt_weight_pack_tc: size of, and packing into, the hi/lo bf16 SWIZZLE_128B
@@ -141,7 +141,7 @@ int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, co
 int kt_conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
                           float* dx, void* stream);
 
-/* tcgen05 weight gradient (time is the contraction dimension; split-K partial tiles go to `workspace`,
+/* tensor-core weight gradient (time is the contraction dimension; split-K partial tiles go to `workspace`,
  * a second kernel reduces them -- a single split writes dw / dbias directly).  Plain convs with channel counts % 8 == 0
  * take the TMA-fed variant: `workspace` then also holds the two operands as hi / lo bf16 planes, written by one
  * elementwise pre-pass of the call (the planes are 16-byte aligned inside a 256-byte-aligned workspace).
@@ -281,8 +281,8 @@ int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, con
  *   h = conv(leaky_relu(x); w1, dilation d, pad_left1) + b1
  *   y = conv(leaky_relu(h); w2, dilation 1, pad_left2) + b2 + x
  * x, h, y: [B][T][C] channels-last fp32; C = 32 or 64, odd kernel <= 15; pad_left = (k-1)*dil for the causal variant
- * (layers.py:66), (k-1)*dil/2 otherwise; out-of-range taps read 0.  ONE launch on the tcgen05 path (bf16x3): the
- * intermediate stays in shared memory / TMEM.  kt_resblock_pack turns a conv's fp32 kernel-layout weight
+ * (layers.py:66), (k-1)*dil/2 otherwise; out-of-range taps read 0.  ONE launch on the tensor-core path (bf16x3): the
+ * intermediate stays in shared memory / registers.  kt_resblock_pack turns a conv's fp32 kernel-layout weight
  * ([k][C][C], kt_weight_prepare's w_fwd) into the kernel's weight image (kt_resblock_image_bytes bytes).
  * `h` (optional, may be NULL) receives the first conv's output for the backward pass. */
 typedef struct KtResblockDesc {
@@ -295,21 +295,17 @@ int64_t kt_resblock_image_bytes(const KtResblockDesc* d);      /* per conv; 0 = 
 int kt_resblock_pack(const KtResblockDesc* d, const float* w_fwd, void* img, void* stream);
 int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
                     const float* b2, float* h, float* y, void* stream);
-/* Backward of the unit from the saved (x, h): the data gradients of both convs (tcgen05 kernels, derivative masks and
+/* Backward of the unit from the saved (x, h): the data gradients of both convs (tensor-core kernels, derivative masks and
  * the residual path fused) -- dh = c2^T(dy) * lrelu'(h) is written to `dh` (the weight-gradient kernels of c1 need it),
  * dx = dy + c1^T(dh) * lrelu'(x).  wimg*_bwd: kt_weight_pack_tc(dir = 1) images of the two convs' descriptors d1 / d2
  * (the per-conv descriptors the weight-gradient entry points also take). */
 int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float* x, const float* h, const float* dy,
                     const void* wimg1_bwd, const void* wimg2_bwd, float* dh, float* dx, void* stream);
 
-/* Development aid: when dev_buf is non-NULL, CTA 0 of every following kt_conv1d_{fwd,bwd_data}_tc launch records
- * clock64() timestamps per role / tile / event into it (int64 [4 roles][16 tiles][4 events]; scripts/tc_trace.py).
- * Process-global and not thread-safe; pass NULL to switch it off (the default). */
+/* Development aid, kept for ABI compatibility: the tensor-core kernels record no per-role timelines; any dev_buf is ignored. */
 int kt_debug_set_trace(void* dev_buf);
-/* Development aid: ablation switches for timing experiments.  tcgen05 conv kernel: bit 0 no residual / mask loads, 1 no
- * global stores, 2 no transposition, 3 no TMEM loads (register epilogue), 4 no weight copies after the first ring pass, 5 no
- * image staging after the first ring pass, 6 no MMAs; weight-gradient chain: 8 no operand split, 9 no MMA kernel, 10 no
- * split-K reduce, 11 no weight-norm backward.  RESULTS ARE WRONG while non-zero. */
+/* Development aid: ablation switches for timing experiments of the weight-gradient chain: bit 8 no operand split, 9 no MMA
+ * kernel, 10 no split-K reduce, 11 no weight-norm backward.  RESULTS ARE WRONG while non-zero. */
 int kt_debug_set_flags(int32_t flags);
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
@@ -319,7 +315,7 @@ int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out12);
 /* library info */
 const char* kt_last_error(void);
 int kt_version(void);
-/* 1 when the library was built with the tcgen05 (sm_100a) conv path */
+/* 1 when the library was built with the tensor-core (sm_90a) conv path */
 int kt_has_tc(void);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-"""kantts_b200 -- B200-native (sm_100a) implementation of KAN-TTS's HiFi-GAN hot path.
+"""kantts_b200 -- H100-native (sm_90a) implementation of KAN-TTS's HiFi-GAN hot path.
 
 Public surface = the reference's own module API for this path:
   hifigan.Generator / MultiPeriodDiscriminator / MultiScaleDiscriminator   (kantts.models)

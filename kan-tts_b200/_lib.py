@@ -1,7 +1,7 @@
 """ctypes binding of libkantts_b200.so (the C ABI declared in include/kantts_b200.h).
 
 The library is built in-tree by ``__graft_entry__.build()`` / ``kantts_b200.build_library()``
-(nvcc, sm_100a).  There is NO fallback: if the shared object is missing or a call fails, a
+(nvcc, sm_90a).  There is NO fallback: if the shared object is missing or a call fails, a
 RuntimeError is raised -- the product path never routes through PyTorch library kernels or
 the CPU oracle.
 """
@@ -103,14 +103,14 @@ _lib = None
 
 def nvcc_command(out_path=LIB_PATH):
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    return ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    return ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
             "-Xcompiler", "-fPIC", "-shared", "-o", out_path] + srcs + ["-lcuda"]
 
 
 def build_library(force=False, verbose=False):
-    """Compile libkantts_b200.so in-tree for sm_100a (cross-compiles without a GPU)."""
+    """Compile libkantts_b200.so in-tree for sm_90a (cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tc_common.cuh"),
+    deps = srcs + [os.path.join(CSRC, h) for h in ("common.cuh", "tc_common.cuh", "tma.cuh", "wgmma.cuh")] + [
                    os.path.join(os.path.dirname(_HERE), "include", "kantts_b200.h")]
     deps = [d for d in deps if os.path.exists(d)]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
@@ -132,7 +132,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). kantts_b200 has no CPU / PyTorch fallback.")
+            "(nvcc, sm_90a). kantts_b200 has no CPU / PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, argtypes in PROTOTYPES.items():
         fn = getattr(lib, name)            # AttributeError here = header / library mismatch
@@ -151,7 +151,7 @@ def check(rc, what):
 
 
 _PTR_DTYPES = (torch.float32,)
-_AUX_DTYPES = (torch.uint8, torch.int32, torch.bfloat16)   # masks / keep-masks, gather indices, packed tcgen05 weight tiles
+_AUX_DTYPES = (torch.uint8, torch.int32, torch.bfloat16)   # masks / keep-masks, gather indices, packed tensor-core weight tiles
 
 
 def ptr(t, aux=False):

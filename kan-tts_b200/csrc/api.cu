@@ -79,7 +79,7 @@ int kt_conv1d_fwd(const KtConv1dDesc* d, const float* x, const float* w_fwd, con
   int rc = kt::validate_conv(d);
   if (rc) return rc;
   KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd: null pointer");
-  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_fwd: tcgen05 path not available for this shape");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_fwd: tensor-core path not available for this shape");
   return kt::conv1d_fwd_ffma(d, x, w_fwd, bias, resid, y, ST(stream));
 }
 
@@ -88,7 +88,7 @@ int kt_conv1d_bwd_data(const KtConv1dDesc* d, const float* dy, const float* y, c
   int rc = kt::validate_conv(d);
   if (rc) return rc;
   KT_REQUIRE(dy && w_bwd && dx, "kt_conv1d_bwd_data: null pointer");
-  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_data: tcgen05 path not available for this shape");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_data: tensor-core path not available for this shape");
   return kt::conv1d_bwd_data_ffma(d, dy, y, w_bwd, x, dx, ST(stream));
 }
 
@@ -97,7 +97,7 @@ int kt_conv1d_bwd_weight(const KtConv1dDesc* d, const float* x, const float* dy,
   int rc = kt::validate_conv(d);
   if (rc) return rc;
   KT_REQUIRE(x && dy && dw, "kt_conv1d_bwd_weight: null pointer");
-  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_weight: tcgen05 path not available for this shape");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_weight: tensor-core path not available for this shape");
   return kt::conv1d_bwd_weight_ffma(d, x, dy, y, dw, dbias, ST(stream));
 }
 

@@ -1,4 +1,4 @@
-// Shared helpers for libkantts_b200 (sm_100a).
+// Shared helpers for libkantts_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -55,8 +55,17 @@ __device__ __forceinline__ float side_apply(float v, float aux, int mode, float 
   }
 }
 
+// Deterministic reductions.  Float atomics from many blocks add in scheduling order, so two runs on the same inputs
+// would differ in the last bits (and a training run amplifies that).  Instead every block writes its partial sums to its
+// own slot of stream-ordered scratch memory (cudaMallocAsync / cudaFreeAsync on the launch stream: safe with concurrent
+// streams and inside CUDA-graph capture) and split_sum adds the slots in a fixed order.
+int scratch_alloc(float** p, long long floats, cudaStream_t st);
+int scratch_free(float* p, cudaStream_t st);
+// out[i] = (accumulate ? out[i] : 0) + sum_{s = 0, 1, ..., nsplit - 1} part[s * stride + i]   for i < n
+int split_sum(const float* part, long long n, int nsplit, long long stride, float* out, bool accumulate, cudaStream_t st);
+
 constexpr int kMaxTaps = 64;
-constexpr int kMaxDynSmem = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_100
+constexpr int kMaxDynSmem = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_90
 
 // One "phase" of a generalised 1-D convolution (see conv_ffma.cu for the decomposition):
 //   out[bb][o_off + o_step*m][co] (+)= epi( sum_n sum_ci W[tap_j[n]][ci][co] * in[bb][ floor((m*i_step + tap_ioff[n]) / up) ][ci] )

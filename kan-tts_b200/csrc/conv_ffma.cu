@@ -1,4 +1,4 @@
-// Exact-fp32 (FFMA) generalised Conv1d kernels, channels-last rows, sm_100a.
+// Exact-fp32 (FFMA) generalised Conv1d kernels, channels-last rows, sm_90a.
 //
 // Every layer-level operation of the HiFi-GAN hot path (conv / transposed conv /
 // nearest-upsampled conv; forward, data gradient, weight gradient; strided, dilated,
@@ -20,7 +20,7 @@
 // (4 x kk) step costs RM + 4*RN/... shared wavefronts for 4*RM*RN FFMAs per lane.
 //
 // These kernels are the exact-fp32 path (and the only path for thin layers: C_in/g < 32, C_out = 1).
-// The tcgen05 kernels in conv_tc.cu take over the GEMM-shaped layers.
+// The tensor-core kernels in conv_tc.cu take over the GEMM-shaped layers.
 #include <stdarg.h>
 #include <string.h>
 
@@ -249,7 +249,7 @@ static int run_core(CoreParams p, cudaStream_t st) {
   if (p.ph.M <= 0 || p.ph.ntaps <= 0) return KT_OK;
   const int RN = p.cout_g > 64 ? 4 : (p.cout_g > 32 ? 2 : 1);
   const int TN = 32 * RN;
-  // biggest row tile that still fills the machine (>= 2 CTAs per SM on 148 SMs)
+  // biggest row tile that still fills the machine (>= 2 CTAs per SM on 132 SMs)
   int RM = 16;
   auto ctas = [&](int rm) { return (long long)ceil_div(p.ph.M, 8 * rm) * p.groups * ceil_div(p.cout_g, TN) * p.batch; };
   while (RM > 4 && (ctas(RM) < 296 || p.ph.M <= 4 * RM)) RM >>= 1;
@@ -275,10 +275,12 @@ static int run_core(CoreParams p, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 struct WgradParams {
   Side a, b;
-  float* g;  // [k][ca_g][cb_total]
+  float* g;  // [k][ca_g][cb_total]; split s accumulates into g + s * g_stride (g_stride = 0: one split)
+  long long g_stride;
   int batch, nsub, t_a, t_b, ca_total, cb_total, groups, ca_g, cb_g;
   int rmax;
   int nsplit, npass;
+  long long g_size;   // floats of g
   Phase ph;
 };
 
@@ -432,6 +434,24 @@ __global__ void __launch_bounds__(256, 2) conv_wgrad_kernel(const __grid_constan
     }
   }
 
+  // ---- with SPLITM the eight warps hold partials of the same elements (they split the rows): fold them into warp 0 in
+  // warp order through shared memory (3 * RMA * RN * 32 floats <= the TK x TN B tile), so that below every element of the
+  // split's zeroed slice of G receives exactly one add -- the result does not depend on scheduling
+  if constexpr (SPLITM) {
+    float* red = smem;
+    for (int w = 1; w < 8; ++w) {
+      __syncthreads();
+      if (warp == w)
+#pragma unroll
+        for (int e = 0; e < NTW * RMA * RN; ++e) red[e * 32 + lane] = (&acc[0][0][0])[e];
+      __syncthreads();
+      if (warp == 0)
+#pragma unroll
+        for (int e = 0; e < NTW * RMA * RN; ++e) (&acc[0][0][0])[e] += red[e * 32 + lane];
+    }
+    if (warp != 0) return;
+  }
+
   // ---- reduce into G ----
   const int a_col = SPLITM ? 0 : warp * RMA;
 #pragma unroll
@@ -446,7 +466,7 @@ __global__ void __launch_bounds__(256, 2) conv_wgrad_kernel(const __grid_constan
       for (int j = 0; j < RN; ++j) {
         const int cb = cb0 + lane * RN + j;
         if (cb >= p.cb_g) continue;
-        atomicAdd(p.g + ((long long)j_tap * p.ca_g + ca) * p.cb_total + (long long)g * p.cb_g + cb, acc[n][i][j]);
+        atomicAdd(p.g + split * p.g_stride + ((long long)j_tap * p.ca_g + ca) * p.cb_total + (long long)g * p.cb_g + cb, acc[n][i][j]);
       }
     }
   }
@@ -459,9 +479,13 @@ static int launch_wgrad(WgradParams p, cudaStream_t st) {
   p.npass = ceil_div(p.ph.ntaps, NTW);
   const long long units = (long long)p.batch * ceil_div(p.ph.M, TK);
   const long long base = (long long)ceil_div(p.ca_g, TCA) * p.groups * ceil_div(p.cb_g, TN) * p.npass;
-  long long nsplit = std::max<long long>(1, (148 * 4) / std::max<long long>(1, base));
+  long long nsplit = std::max<long long>(1, (132 * 4) / std::max<long long>(1, base));
   nsplit = std::min<long long>(nsplit, std::max<long long>(1, units / 4));
   nsplit = std::min<long long>(nsplit, 4096);
+  // every split accumulates into its own zeroed slice of scratch (each element of a slice is added to by one CTA, in a
+  // fixed order); the slices are summed in order into g
+  const long long g_size = p.g_size;
+  nsplit = std::max<long long>(1, std::min<long long>(nsplit, (1LL << 25) / std::max<long long>(1, g_size)));
   p.nsplit = (int)nsplit;
   const size_t smem = ((size_t)p.rmax * TCA + (size_t)TK * TN) * sizeof(float);
   KT_REQUIRE(smem <= 200 * 1024, "conv_wgrad: tile too large (%zu bytes shared)", smem);
@@ -471,8 +495,23 @@ static int launch_wgrad(WgradParams p, cudaStream_t st) {
     configured.store(true, std::memory_order_release);
   }
   dim3 grid(ceil_div(p.ca_g, TCA), p.groups * ceil_div(p.cb_g, TN), p.npass * p.nsplit);
+  float* out = p.g;
+  float* part = nullptr;
+  p.g_stride = 0;
+  if (p.nsplit > 1) {
+    int rc = scratch_alloc(&part, (long long)p.nsplit * g_size, st);
+    if (rc) return rc;
+    KT_CHECK_CUDA(cudaMemsetAsync(part, 0, (size_t)p.nsplit * g_size * sizeof(float), st));
+    p.g = part;
+    p.g_stride = g_size;
+  }
   conv_wgrad_kernel<RN, RMA, SPLITM><<<grid, 256, smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
+  if (part) {
+    int rc = split_sum(part, g_size, p.nsplit, g_size, out, true, st);
+    if (rc) return rc;
+    return scratch_free(part, st);
+  }
   return KT_OK;
 }
 
@@ -499,8 +538,8 @@ static int run_wgrad(const WgradParams& p, cudaStream_t st) {
   return launch_wgrad<1, 8, false>(p, st);
 }
 
-// column sums: out[c] = sum_rows f(v[row][c])   (bias gradient)
-__global__ void colsum_kernel(Side s, long long rows, int c, float* out) {
+// column sums of one row range: part[blockIdx.y][c] = sum_rows f(v[row][c])   (bias gradient, see colsum_bias)
+__global__ void colsum_kernel(Side s, long long rows, int c, float* part) {
   const int ch = blockIdx.x * 32 + (threadIdx.x & 31);
   const int rlane = threadIdx.x >> 5;  // 8 row lanes
   float acc = 0.f;
@@ -517,7 +556,7 @@ __global__ void colsum_kernel(Side s, long long rows, int c, float* out) {
   if (rlane == 0 && ch < c) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x & 31];
-    atomicAdd(out + ch, t);
+    part[(long long)blockIdx.y * c + ch] = t;
   }
 }
 
@@ -659,6 +698,8 @@ int conv1d_bwd_data_ffma(const KtConv1dDesc* d, const float* dy, const float* y,
   return KT_OK;
 }
 
+int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t st);
+
 int conv1d_bwd_weight_ffma(const KtConv1dDesc* d, const float* x, const float* dy, const float* y,
                            float* dw, float* dbias, cudaStream_t st) {
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_weight: y required when act_out != NONE");
@@ -668,7 +709,7 @@ int conv1d_bwd_weight_ffma(const KtConv1dDesc* d, const float* x, const float* d
   const Side sx = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   const Side sdy = make_side(dy, y, d->act_out, d->act_out_slope, true);
   WgradParams p{};
-  p.g = dw; p.batch = d->batch * d->nsub; p.nsub = d->nsub; p.groups = d->groups;
+  p.g = dw; p.g_size = (long long)wn; p.batch = d->batch * d->nsub; p.nsub = d->nsub; p.groups = d->groups;
   if (!d->transposed) {
     // dW[j][ci][co] = sum x[(to*stride + j*dil - pad)/up][ci] * dpre[to][co]
     p.a = sx; p.b = sdy;
@@ -686,22 +727,20 @@ int conv1d_bwd_weight_ffma(const KtConv1dDesc* d, const float* x, const float* d
   }
   int rc = run_wgrad(p, st);
   if (rc) return rc;
-  if (dbias) {
-    KT_CHECK_CUDA(cudaMemsetAsync(dbias, 0, (size_t)d->c_out * sizeof(float), st));
-    const long long rows = (long long)d->batch * d->nsub * d->t_out;
-    dim3 grid(ceil_div(d->c_out, 32), (unsigned)std::min<long long>(std::max<long long>(1, rows / 256), 512));
-    colsum_kernel<<<grid, 256, 0, st>>>(sdy, rows, d->c_out, dbias);
-    KT_CHECK_CUDA(cudaGetLastError());
-  }
+  if (dbias) return colsum_bias(sdy, (long long)d->batch * d->nsub * d->t_out, d->c_out, dbias, st);
   return KT_OK;
 }
 
 int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t st) {
-  KT_CHECK_CUDA(cudaMemsetAsync(out, 0, (size_t)c * sizeof(float), st));
-  dim3 grid(ceil_div(c, 32), (unsigned)std::min<long long>(std::max<long long>(1, rows / 256), 512));
-  colsum_kernel<<<grid, 256, 0, st>>>(s, rows, c, out);
+  const int ny = (int)std::min<long long>(std::max<long long>(1, rows / 256), 512);
+  float* part = nullptr;
+  int rc = scratch_alloc(&part, (long long)ny * c, st);
+  if (rc) return rc;
+  colsum_kernel<<<dim3(ceil_div(c, 32), ny), 256, 0, st>>>(s, rows, c, part);
   KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
+  rc = split_sum(part, c, ny, c, out, false, st);
+  if (rc) return rc;
+  return scratch_free(part, st);
 }
 
 int validate_conv(const KtConv1dDesc* d) { return validate(d); }

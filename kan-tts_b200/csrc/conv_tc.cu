@@ -1,25 +1,24 @@
-// tcgen05 implicit-GEMM Conv1d (forward / data-gradient) for the GEMM-shaped HiFi-GAN layers.
+// wgmma implicit-GEMM Conv1d (forward / data-gradient) for the GEMM-shaped HiFi-GAN layers.
 //
 // Precision: "bf16x3".  Every fp32 operand is split x = hi + lo (two bf16, |x - hi - lo| <~ 2^-17 |x|)
-// and the product is accumulated in fp32 TMEM as hi*hi + hi*lo + lo*hi (the dropped lo*lo term is
+// and the product is accumulated in fp32 registers as hi*hi + hi*lo + lo*hi (the dropped lo*lo term is
 // ~2^-18 relative).  A single-pass TF32/BF16 MMA does not meet the path's tolerance (mel-L1 <= 1e-4,
 // SURVEY.md "hard parts"); three bf16 MMAs do, at twice the rate of 3xTF32.
 //
-// Tile = 128 consecutive FLATTENED outputs (time m, sub-sequence w) of one batch item x NT channels.
+// Tile = 128 consecutive FLATTENED outputs (time m, sub-sequence w) of one batch item x NT (<= 128) channels.
 // Data flow per CTA:
-//   warps 0-3  stage the channels-last fp32 activation rows (fused pre-activation / activation
+//   warpgroup 0  stages the channels-last fp32 activation rows (fused pre-activation / activation
 //              derivative), split them into hi / lo bf16 planes and store SWIZZLE_128B shared-memory
 //              images (rows = flattened (time, sub-sequence) positions of ONE input residue class).
-//              im2col-free: tap j = residue image rho_j read through a UMMA descriptor whose start
+//              im2col-free: tap j = residue image rho_j read through a wgmma descriptor whose start
 //              address is shifted by q_j * nsub rows (the 128-byte swizzle is a function of absolute
 //              smem address bits, so a row shift needs no re-phasing).  Stride s convs stage s residue
 //              images per 64-channel chunk; the period discriminator's (k,1) Conv2d needs nothing extra.
-//   warp 4     streams the pre-swizzled bf16 weight tiles (hi + lo, one tap x 64 input channels) with
+//   warp 12    streams the pre-swizzled bf16 weight tiles (hi + lo, one tap x 64 input channels) with
 //              cp.async.bulk (TMA engine) into a ring of shared-memory stages, mbarrier complete_tx.
-//   warp 5     one elected thread issues tcgen05.mma (M=128, N=NT, K=16) x 4 k-slices x 3 products per
-//              (chunk, tap); tcgen05.commit releases weight stages / activation images / signals the epilogue.
-//   warps 0-3  epilogue: tcgen05.ld the fp32 accumulators (thread = output row), bias / activation /
-//              residual (or act' mask for the data gradient), 16-byte stores to the channels-last output.
+//   warpgroups 1 / 2  wgmma (M = 64 rows each, N = NT, K = 16) x 4 k-slices x 3 products per (chunk, tap) into
+//              register accumulators, then the epilogue of their 64 rows: bias / activation / residual (or act'
+//              mask for the data gradient), stores to the channels-last output.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -100,17 +99,11 @@ struct TcParams {
   int batch, nsub, t_in, t_out, c_in, c_out;
   int out_act;
   float out_slope;
-  int NT, ntiles, kchunks, rows, na_stages, nb_stages, tmem_cols;
+  int NT, ntiles, kchunks, rows, na_stages, nb_stages;
   // 1: every (K chunk, tap) weight tile of the layer has its own shared-memory slot (slot = c * ntaps + n), loaded
   // ONCE per CTA and reused by all of its tiles -- thin layers otherwise re-stream all taps per 128-row tile through
-  // a ring whose refill round trip (commit -> empty -> bulk copy -> full) bounds the MMA issue rate (measured
-  // 0.6-0.8 us per tap, profiles/r02_tc_trace.md)
+  // a ring whose refill round trip (release -> empty -> bulk copy -> full) bounds the MMA issue rate
   int w_resident;
-  // 1 (NT <= 128, NT % 32 == 0): the hi*hi and hi*lo products of a K slice are ONE tcgen05.mma -- the weight tile
-  // [hi rows | lo rows] is read as a single N = 2*NT operand, accumulator columns [0, NT) and [NT, 2*NT) -- plus one
-  // N = NT instruction for lo*hi; the epilogue adds the two column ranges.  A tcgen05.mma of this kernel costs
-  // ~130 cycles whatever N is (shared-memory A operand), so 2 instructions per slice instead of 3 is -1/3 MMA time.
-  int fuse2;
   int kg;        // contraction channels per tile (C_in, or C_in / groups)
   int grouped;   // 1: N tile nt = group nt (input channels [nt * kg, +kg), outputs [nt * n_stride, +n_stride))
   int n_stride;  // output channels advanced per N tile
@@ -129,233 +122,53 @@ struct TcParams {
   int ntaps;
   int tap_j[kMaxTaps];                // weight tap index, ordered by group
   int tap_shift[kMaxTaps];            // image row shift (q_n - q_lo) * nsub
-  // development aid (kt_debug_set_trace): CTA 0 records clock64() per role / tile / event, see scripts/tc_trace.py
-  long long* trace;
-  int dbg;      // development aid (kt_debug_set_flags): ablation switches for timing experiments, results are WRONG when non-zero
-  // TMA epilogue (plain single-phase layers, see epilogue_tma): output / side (residual or activation-derivative operand)
-  // tensors as 3-D maps (channels, rows of one item, items), boxes of 16 channels x 32 rows, SWIZZLE_64B
-  int epi_tma;
-  int epi_split;   // 1: both epilogue groups drain EVERY tile (half of its columns each) instead of alternate tiles
-  int epi_alias;   // 1: every CTA has at most one tile -- its epilogue boxes reuse the (then idle) operand stages
-  alignas(64) CUtensorMap map_out;
-  alignas(64) CUtensorMap map_side;
 };
 
-constexpr int kEpiBufBytes = 32 * 16 * 4;   // one 32-row x 16-column fp32 box
-constexpr int kEpiBufs = 3;                 // per epilogue warp: (side load ->) combine -> store, three boxes in rotation
+// Warp roles (416 threads): warpgroup 0 stages activations; warpgroups 1 and 2 are the consumers -- each runs the wgmma
+// of one 64-row half of the 128-row tile into its registers and that half's epilogue; warp 12 streams weights.  (Warps
+// hold registers in groups of four: 13 warps keep the 128 registers per thread the consumers' accumulators need.)
+constexpr int kTcThreads = 416;
+constexpr int kTcConsumerArrivals = 8;   // one per consumer warp
 
-constexpr int kTraceTiles = 16, kTraceEvents = 4;
-__device__ __forceinline__ void trace_ev(const TcParams& p, int role, int tile_i, int ev) {
-  if (p.trace != nullptr && blockIdx.x == 0 && tile_i < kTraceTiles)
-    p.trace[(role * kTraceTiles + tile_i) * kTraceEvents + ev] = clock64();
-}
-
-// Epilogue through the TMA unit.  The register-path epilogue below spends ~2.7 us per 32-column chunk of a warp on a chain of
-// dependent shared / global memory instructions (transposition tile -> coalesced 16-byte stores, residual loads from
-// L2): 11 us per 128 x 128 tile, 25 us per 128 x 256 tile, fully exposed on the last (or only) tile of a CTA (in-kernel
-// timeline, call r2ae).  Here a warp writes its 32 rows x 16 columns straight from the tcgen05.ld layout (thread = row)
-// into a SWIZZLE_64B box -- the XOR the transposition tile already used, so the stores are conflict-free -- and one
-// elected lane hands the box to cp.async.bulk.tensor (store): coalescing, row clipping at the end of the item and
-// the global write itself are the TMA unit's.  A residual / derivative-mask operand is PREFETCHED into the same box two
-// boxes ahead (bulk tensor load on a per-box mbarrier) and combined in place.  Three boxes per warp rotate.
-template <bool SIMPLE>
-__device__ __forceinline__ void epilogue_tma(const TcParams& p, uint32_t tmem_acc, uint32_t buf_cols, uint64_t* tmem_full, uint64_t* tmem_empty,
-                                             uint8_t* ebuf, uint64_t* ebar, float* sbias, int quarter, int egrp, int lane, int total_tiles,
-                                             int mtiles, bool tracer) {
-  const bool split = p.epi_split != 0;
-  const int halves_tile = p.NT >> 4;                       // 16-column boxes per tile row block
-  const int h_begin = split ? egrp * (halves_tile >> 1) : 0;
-  const int h_end = split ? h_begin + (halves_tile >> 1) : halves_tile;
-  const int side_kind = p.resid ? 1 : (p.mask.p ? 2 : 0);  // 0 none, 1 residual add, 2 LeakyReLU-derivative mask
-  const uint32_t sw = (uint32_t)((lane >> 1) & 3);          // SWIZZLE_64B: 16-byte chunk index ^= address bits [7, 9) = (row >> 1) & 3
-  uint32_t k = 0;                                           // boxes this warp has handled so far (buffer rotation / barrier phases)
-  int ti = 0;
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-    if (!split && (ti & 1) != egrp) continue;
-    const int mt = tile % mtiles, nt = (tile / mtiles) % p.ntiles, bb = tile / (mtiles * p.ntiles);
-    const int buf = ti & 1;
-    const int r0 = mt * kTcM + quarter * 32;               // this warp's first row inside the item (flattened (time, sub-sequence))
-    const int c_tile = nt * p.n_stride;
-    const int n_valid = min(p.n_stride, p.c_out - c_tile);
-    if (tracer) trace_ev(p, 3, ti, 0);
-    auto side_prefetch = [&]() {    // side boxes of the first two column blocks (their buffers: last read by stores k-3 and k-2)
-      if (side_kind && lane == 0) {
-        bulk_wait_group_read<1>();
-        for (int j = 0; j < 2; ++j)
-          if (h_begin + j < h_end) {
-            const uint32_t b = (k + j) % kEpiBufs;
-            mbar_arrive_expect_tx(&ebar[b], (uint32_t)kEpiBufBytes);
-            tma_load_3d(ebuf + b * kEpiBufBytes, &p.map_side, c_tile + (h_begin + j) * 16, r0, bb, &ebar[b]);
-          }
-      }
-    };
-    if (!p.epi_alias) side_prefetch();   // (aliased boxes ARE operand stages: nothing may land there before the tile's MMAs are done)
-    if (p.bias) {
-      __syncwarp();
-      for (int e = lane; e < p.NT; e += 32) sbias[e] = e < n_valid ? __ldg(p.bias + c_tile + e) : 0.f;
-      __syncwarp();
-    }
-    mbar_wait(&tmem_full[buf], (ti >> 1) & 1);
-    tc_fence_after();
-    if (p.epi_alias) side_prefetch();
-    if (tracer) trace_ev(p, 3, ti, 1);
-    const uint32_t t_lane = tmem_acc + (uint32_t)buf * buf_cols + ((uint32_t)(quarter * 32) << 16);
-    for (int hh = h_begin; hh < h_end; hh += 2) {
-      const int n0 = hh * 16;
-      const int nh = min(2, h_end - hh);
-      uint32_t rr[32];
-      if (nh == 2) {
-        tmem_ld32(t_lane + (uint32_t)n0, rr);
-      } else {
-        uint32_t r16[16];
-        tmem_ld16(t_lane + (uint32_t)n0, r16);
-#pragma unroll
-        for (int e = 0; e < 16; ++e) { rr[e] = r16[e]; rr[16 + e] = 0u; }
-      }
-      tmem_ld_wait();
-      if (p.fuse2) {   // + the hi*lo products (columns [NT, 2*NT))
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (h < nh) {
-            uint32_t t2[16];
-            tmem_ld16(t_lane + (uint32_t)(p.NT + n0 + 16 * h), t2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) rr[16 * h + e] = __float_as_uint(__uint_as_float(rr[16 * h + e]) + __uint_as_float(t2[e]));
-          }
-        }
-      }
-      if (hh + 2 >= h_end) {   // last TMEM read of this warp for this tile: hand the buffer back to the MMA issuer
-        tc_fence_before();
-        mbar_arrive(&tmem_empty[buf]);
-        if (tracer) trace_ev(p, 3, ti, 2);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (h < nh) {
-          const uint32_t b = k % kEpiBufs;
-          uint8_t* box = ebuf + b * kEpiBufBytes;
-          if (side_kind) {
-            mbar_wait(&ebar[b], (k / kEpiBufs) & 1);       // the side operand of this box has landed
-          } else {
-            if (lane == 0) bulk_wait_group_read<2>();        // the store that last used this box (k - 3) has read it
-            __syncwarp();
-          }
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            const int e = h * 16 + e4 * 4;
-            float v[4] = {__uint_as_float(rr[e]), __uint_as_float(rr[e + 1]), __uint_as_float(rr[e + 2]), __uint_as_float(rr[e + 3])};
-            if (p.bias) {
-              const float4 bv = *reinterpret_cast<const float4*>(sbias + n0 + e);
-              v[0] += bv.x; v[1] += bv.y; v[2] += bv.z; v[3] += bv.w;
-            }
-            if (p.out_act == KT_ACT_LRELU) {
-#pragma unroll
-              for (int z = 0; z < 4; ++z) v[z] = v[z] > 0.f ? v[z] : v[z] * p.out_slope;
-            } else if (!SIMPLE && p.out_act == KT_ACT_TANH) {
-#pragma unroll
-              for (int z = 0; z < 4; ++z) v[z] = tanhf(v[z]);
-            }
-            float4* cell = reinterpret_cast<float4*>(box + lane * 64 + (((uint32_t)e4 ^ sw) << 4));
-            if (side_kind == 1) {
-              const float4 a = *cell;
-              v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w;
-            } else if (side_kind == 2) {
-              const float4 a = *cell;
-              v[0] = a.x > 0.f ? v[0] : v[0] * p.mask.slope; v[1] = a.y > 0.f ? v[1] : v[1] * p.mask.slope;
-              v[2] = a.z > 0.f ? v[2] : v[2] * p.mask.slope; v[3] = a.w > 0.f ? v[3] : v[3] * p.mask.slope;
-            }
-            *cell = make_float4(v[0], v[1], v[2], v[3]);
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_3d(&p.map_out, box, c_tile + n0 + h * 16, r0, bb);
-            bulk_commit_group();
-            if (side_kind && hh + h + 2 < h_end) {   // side operand of the box after next -> the buffer store k-1 used
-              bulk_wait_group_read<1>();
-              const uint32_t b2 = (k + 2) % kEpiBufs;
-              mbar_arrive_expect_tx(&ebar[b2], (uint32_t)kEpiBufBytes);
-              tma_load_3d(ebuf + b2 * kEpiBufBytes, &p.map_side, c_tile + n0 + (h + 2) * 16, r0, bb, &ebar[b2]);
-            }
-          }
-          ++k;
-        }
-      }
-    }
-    if (tracer) trace_ev(p, 3, ti, 3);
-  }
-  if (lane == 0) bulk_wait_group_read<0>();   // the boxes must outlive their stores' reads
-  __syncwarp();
-}
-
-// warps 0-3 and 10-13 stage activations (two producer groups filling ALTERNATE pipeline stages, so two images'
-// worth of global loads are in flight), 4 streams weights, 5 issues MMAs, 6-9 and 14-17 epilogue (two groups
-// draining ALTERNATE tiles = TMEM accumulator buffers)
-constexpr int kTcThreads = 576;
-
-// Persistent: gridDim.x = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  The three
-// pipelines (activation images, weight tiles, TMEM accumulators: 2 buffers) run continuously ACROSS tiles,
-// so staging of tile i+1, the MMAs of tile i and the epilogue of tile i-1 overlap.
+// Persistent: gridDim.x = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  The activation and
+// weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
 // SIMPLE = true: nsub == 1, up == 1, vectorisable channel counts, no tanh / accumulate -- the generator's resblock
 // convs, the scale discriminator and every SAM-BERT linear / conv (see stage_rows).  false: everything else.
 template <bool SIMPLE>
 __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve-up (all image / tile bases 1024-byte aligned)
-  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space --
-  //  with the cast it emitted GENERIC ld / st for every image / staging access of the producers and the epilogue)
+  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space)
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   const int img_bytes = p.rows * 128;                 // one plane of one activation stage
   const int a_stage_bytes = 2 * img_bytes;            // hi + lo
   const int b_stage_bytes = 2 * p.NT * 128;           // hi + lo weight tile
   uint8_t* a_base = smem;
   uint8_t* b_base = a_base + (size_t)p.na_stages * a_stage_bytes;
-  // epilogue boxes (1024-byte aligned: the TMA path's SWIZZLE_64B pattern is a function of address bits):
-  // register path 8 warps x one 2 KB transposition tile, TMA path 8 warps x kEpiBufs boxes
-  uint8_t* s_end = b_base + (size_t)p.nb_stages * b_stage_bytes;
-  uint8_t* e_base = p.epi_alias ? a_base : s_end;
-  const int e_bytes = p.epi_alias ? 0 : (p.epi_tma ? 8 * kEpiBufs * kEpiBufBytes : 8 * 2048);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_end + e_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(b_base + (size_t)p.nb_stages * b_stage_bytes);
   uint64_t* full_a = bars;                         // [na]
   uint64_t* empty_a = full_a + p.na_stages;        // [na]
   uint64_t* full_b = empty_a + p.na_stages;        // [nb]
   uint64_t* empty_b = full_b + p.nb_stages;        // [nb]
-  uint64_t* tmem_full = empty_b + p.nb_stages;     // [2]
-  uint64_t* tmem_empty = tmem_full + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  // per-tap image row shift in descriptor units (16 bytes): the MMA issuer reads it with one LDS per tap instead of a
-  // dynamically indexed kernel-parameter load (constant-bank miss + address arithmetic on the issuing thread)
-  uint32_t* s_tapshift = tmem_slot + 4;          // [kMaxTaps]
-  float* epi_stage = reinterpret_cast<float*>(e_base);                  // 8 epilogue warps x (32 rows x 16 fp32)
-  float* epi_bias = reinterpret_cast<float*>(s_tapshift + kMaxTaps);    // 8 epilogue warps x 256 floats, 16-byte aligned
-  uint64_t* epi_bar = reinterpret_cast<uint64_t*>(epi_bias + 8 * 256);  // TMA path: 8 warps x kEpiBufs side-operand barriers
+  // per-tap image row shift in descriptor units (16 bytes)
+  uint32_t* s_tapshift = reinterpret_cast<uint32_t*>(empty_b + p.nb_stages);   // [kMaxTaps]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mtiles = p.ph_mt0[p.nphases];   // m-tiles of all phases (each: 128 flattened outputs m * nsub + w)
   const int total_tiles = mtiles * p.ntiles * p.batch;
 
   if (tid == 0) {
-    for (int s = 0; s < p.na_stages; ++s) { mbar_init(&full_a[s], 128); mbar_init(&empty_a[s], 1); }
-    for (int s = 0; s < p.nb_stages; ++s) { mbar_init(&full_b[s], 1); mbar_init(&empty_b[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], (p.epi_tma && p.epi_split) ? 256 : 128); }
-    if (p.epi_tma)
-      for (int s = 0; s < 8 * kEpiBufs; ++s) mbar_init(&epi_bar[s], 1);
+    for (int s = 0; s < p.na_stages; ++s) { mbar_init(&full_a[s], 128); mbar_init(&empty_a[s], kTcConsumerArrivals); }
+    for (int s = 0; s < p.nb_stages; ++s) { mbar_init(&full_b[s], 1); mbar_init(&empty_b[s], kTcConsumerArrivals); }
     mbar_fence_init();
     fence_proxy_async();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  if (tid >= 192 && tid < 192 + kMaxTaps) s_tapshift[tid - 192] = (uint32_t)p.tap_shift[tid - 192] * 8u;
-  tc_fence_before();
+  if (tid < kMaxTaps) s_tapshift[tid] = (uint32_t)p.tap_shift[tid] * 8u;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
-  const uint32_t buf_cols = (uint32_t)(p.tmem_cols / 2);
 
-  if (warp < 4 || (warp >= 10 && warp < 14)) {
+  if (warp < 4) {
     // ===================== activation producers =====================
-    const int pg = warp < 4 ? 0 : 1;                 // producer group: stages it = pg, pg + 2, ...
-    const int ptid = warp < 4 ? tid : tid - 320;     // 0..127 inside the group
+    const int ptid = tid;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int gm = tile % mtiles, bb = tile / (mtiles * p.ntiles);
@@ -365,25 +178,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       const int f0 = (gm - p.ph_mt0[ph]) * kTcM;
       for (int c = 0; c < p.kchunks; ++c) {
         for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ++it) {
-          if ((it & 1) != pg) continue;
           const int s = it % p.na_stages;
           mbar_wait(&empty_a[s], ((it / p.na_stages) & 1) ^ 1);
-          if (ptid == 0) trace_ev(p, pg, it >> 1, 0);
           uint8_t* img_hi = a_base + (size_t)s * a_stage_bytes;
           RowMap rm;
           rm.base_row = (long long)bb * p.t_in * p.nsub;
           rm.fv0 = f0 + p.grp_qlo[g] * p.nsub;
           rm.nsub = p.nsub; rm.step = p.i_step; rm.rho = p.grp_rho[g]; rm.up = p.up; rm.t_lim = p.t_in * p.up;
-          if (!(p.dbg & 32) || it < p.na_stages)   // (ablation 32: images staged only on the first ring pass)
           stage_rows<5, SIMPLE, 3>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
-                                min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
+                                   min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
           fence_proxy_async();
           mbar_arrive(&full_a[s]);
-          if (ptid == 0) trace_ev(p, pg, it >> 1, 1);
         }
       }
     }
-  } else if (warp == 4) {
+  } else if (warp == 12) {
     // ===================== weight stream (bulk async copies) =====================
     const bool leader = elect_one();
     if (leader && p.w_resident) {
@@ -396,6 +205,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
             mbar_arrive_expect_tx(&full_b[s], (uint32_t)b_stage_bytes);
             bulk_g2s(b_base + (size_t)s * b_stage_bytes, src, (uint32_t)b_stage_bytes, &full_b[s]);
           }
+        for (int s = 0; s < p.nb_stages; ++s) mbar_wait(&full_b[s], 0);   // no bulk copy may outlive the CTA
       }
     } else if (leader) {
       int it = 0;
@@ -405,12 +215,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         while ((tile % mtiles) >= p.ph_mt0[ph + 1]) ++ph;
         const int n_begin = p.grp_first[p.ph_g0[ph]], n_end = p.grp_first[p.ph_g0[ph + 1]];
         for (int c = 0; c < p.kchunks; ++c) {
-          for (int n = n_begin; n < n_end; ++n, ++it) {  // taps are ordered by group: same order as the MMA issuer
+          for (int n = n_begin; n < n_end; ++n, ++it) {  // taps are ordered by group: same order as the consumers
             const int s = it % p.nb_stages;
             mbar_wait(&empty_b[s], ((it / p.nb_stages) & 1) ^ 1);
             const long long block = ((long long)p.tap_j[n] * p.kchunks + c) * p.ntiles + nt;
             const uint8_t* src = reinterpret_cast<const uint8_t*>(p.wimg) + block * (long long)b_stage_bytes;
-            if ((p.dbg & 16) && it >= p.nb_stages) { mbar_arrive(&full_b[s]); continue; }   // ablation: no weight traffic after the first ring pass
             mbar_arrive_expect_tx(&full_b[s], (uint32_t)b_stage_bytes);
             bulk_g2s(b_base + (size_t)s * b_stage_bytes, src, (uint32_t)b_stage_bytes, &full_b[s]);
           }
@@ -418,280 +227,113 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    // One elected thread.  Everything it touches per MMA is a 32-bit add: the UMMA shared-memory descriptors are kept as
-    // (lo word, constant hi word) pairs -- lo = (address >> 4) | LBO field, so a tap's row shift, the K = 16 slice offset
-    // (32 bytes = 2 units) and the hi -> lo plane distance are plain integer adds on the lo word (shared-memory addresses
-    // are < 2^18, so the 14-bit address field never carries into the LBO field).  Resident weight slots are waited for
-    // once per CTA (their single phase completes once and stays complete); ring stages once per (chunk, tap).
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(kTcM, p.NT, 0, 0);
-      const uint32_t idesc2 = make_idesc_bf16(kTcM, 2 * p.NT, 0, 0);
-      const uint32_t a_base16 = (smem_u32(a_base) >> 4) | 0x10000u;     // descriptor lo word of stage 0, hi plane
-      const uint32_t b_base16 = (smem_u32(b_base) >> 4) | 0x10000u;
-      const uint32_t a_stage16 = (uint32_t)a_stage_bytes >> 4, img16 = (uint32_t)img_bytes >> 4;
-      const uint32_t b_stage16 = (uint32_t)b_stage_bytes >> 4, bplane16 = (uint32_t)(p.NT * 128) >> 4;
-      const bool resident = p.w_resident != 0, fuse2 = p.fuse2 != 0;
-      int it_a = 0, it_b = 0, ti = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-        const int buf = ti & 1;
-        trace_ev(p, 2, ti, 0);
-        mbar_wait(&tmem_empty[buf], ((ti >> 1) & 1) ^ 1);   // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        trace_ev(p, 2, ti, 1);
-        const uint32_t d_tmem = tmem_acc + (uint32_t)buf * buf_cols;
-        uint32_t acc = 0;
-        const bool tr_on = p.trace != nullptr && blockIdx.x == 0 && ti < kTraceTiles;   // role 6: cycles this tile's issuer waited
-        long long w_a = 0, w_b = 0, t_w = 0;
-        int ph = 0;
-        while ((tile % mtiles) >= p.ph_mt0[ph + 1]) ++ph;
-        const int g_begin = p.ph_g0[ph], g_end = p.ph_g0[ph + 1];
-        for (int c = 0; c < p.kchunks; ++c) {
-          const int kslices = (min(kTcKC, p.kg - c * kTcKC) + 15) >> 4;   // K = 16 slices holding real channels
-          for (int g = g_begin; g < g_end; ++g, ++it_a) {
-            const int sa = it_a % p.na_stages;
-            // (no tcgen05.fence here or after the weight wait: the producers' fence.proxy.async + mbarrier release
-            //  / the bulk copy's complete_tx make the data visible to the MMA's async-proxy reads)
-            if (tr_on) t_w = clock64();
-            mbar_wait(&full_a[sa], (it_a / p.na_stages) & 1);
-            if (tr_on) w_a += clock64() - t_w;
-            if (c == 0 && g == g_begin) trace_ev(p, 2, ti, 2);
-            const uint32_t a16 = a_base16 + (uint32_t)sa * a_stage16;
-            const int n_begin = p.grp_first[g], n_end = p.grp_first[g + 1];
-            uint32_t sh = s_tapshift[n_begin];
-            for (int n = n_begin; n < n_end; ++n, ++it_b) {
-              const uint32_t a_hi = a16 + sh;
-              if (n + 1 < n_end) sh = s_tapshift[n + 1];          // next tap's shift: its LDS latency hides behind this tap's MMAs
-              int sb;
-              if (resident) {
-                sb = c * p.ntaps + n;
-                if (ti == 0) mbar_wait(&full_b[sb], 0u);
-              } else {
-                sb = it_b % p.nb_stages;
-                if (tr_on) t_w = clock64();
-                mbar_wait(&full_b[sb], (uint32_t)((it_b / p.nb_stages) & 1));
-                if (tr_on) w_b += clock64() - t_w;
-              }
-              const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
-              if (p.dbg & 64) {
-                // ablation: no MMAs (pipelines and commits only)
-              } else if (fuse2) {
-                umma_step_fuse2(d_tmem, a_hi, img16, b_hi, idesc2, idesc, acc, (uint32_t)kslices);
-                acc = 1;
-              } else {
-                umma_step_x3(d_tmem, a_hi, img16, b_hi, bplane16, idesc, acc, (uint32_t)kslices);
-                acc = 1;
-              }
-              if (!resident) umma_commit(&empty_b[sb]);
-            }
-            umma_commit(&empty_a[sa]);
-          }
-        }
-        umma_commit(&tmem_full[buf]);
-        trace_ev(p, 2, ti, 3);
-        if (tr_on) {
-          long long* t6 = p.trace + (6 * kTraceTiles + ti) * kTraceEvents;
-          t6[0] = w_a; t6[1] = w_b; t6[2] = it_b; t6[3] = p.na_stages * 100 + p.nb_stages;
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 6-9 and 14-17; TMEM lane quarter = warp & 3) =====================
-    // Two groups of four warps: group e owns the tiles with (ti & 1) == e, i.e. TMEM accumulator buffer e -- a tile's
-    // epilogue is a long, latency-bound instruction stream per warp (~1.7 us per 32-column chunk measured with one
-    // group), so two tiles are drained concurrently.
-    // tcgen05.ld hands every thread ONE output row.  Writing rows straight from that layout makes each 16-byte warp
-    // store touch 32 different 128-byte lines, so every warp transposes 32 rows x 16 columns at a time through a private
-    // 2 KB shared-memory tile (16-byte chunks XOR-swizzled: conflict-free both ways): 4 consecutive lanes then cover one
-    // 64-byte row segment, 8 rows per warp instruction -- residual / mask loads, the read-modify-write of `accumulate`
-    // and the stores are whole 32-byte sectors.  Bias and the output activation are applied before the transposition
-    // (per column), residual / derivative masks after it (per element).
-    const int quarter = warp & 3;
-    const int egrp = warp >= 14 ? 1 : 0;
-    const int ewarp = egrp * 4 + quarter;
-    float* stg = epi_stage + (size_t)ewarp * (32 * 16);
-    float* sbias = epi_bias + ewarp * 256;          // this warp's copy of the tile's bias (NT <= 256 floats)
-    const bool tracer = (tid == 192 || tid == 448);
-    if (p.epi_tma) {
-      epilogue_tma<SIMPLE>(p, tmem_acc, buf_cols, tmem_full, tmem_empty, e_base + (size_t)ewarp * (kEpiBufs * kEpiBufBytes),
-                           epi_bar + ewarp * kEpiBufs, sbias, quarter, egrp, lane, total_tiles, mtiles, tracer);
-    } else {
-    int ti = 0;
+  } else if (warp >= 4 && warp < 12) {
+    // ===================== consumers: wgmma + epilogue, one 64-row half of the tile per warpgroup =====================
+    // Descriptor low words + 32-bit adds only: a tap's row shift, the K = 16 slice offset (32 bytes = 2 units), the hi -> lo
+    // plane distance and this warpgroup's 64-row offset (8 KB = 512 units) are integer adds on the low word.
+    const int cw = (warp - 4) >> 2;                  // 0: rows 0-63, 1: rows 64-127
+    const int wq = warp & 3;                         // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of the half
+    const uint32_t a_base16 = (smem_u32(a_base) >> 4) + (uint32_t)cw * 512u;
+    const uint32_t b_base16 = smem_u32(b_base) >> 4;
+    const uint32_t a_stage16 = (uint32_t)a_stage_bytes >> 4, img16 = (uint32_t)img_bytes >> 4;
+    const uint32_t b_stage16 = (uint32_t)b_stage_bytes >> 4, bplane16 = (uint32_t)(p.NT * 128) >> 4;
+    const bool resident = p.w_resident != 0;
+    const int NT = p.NT;
+    float acc[kWgmmaMaxRegs];
+#pragma unroll
+    for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
+    int it_a = 0, it_b = 0, ti = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-      if ((ti & 1) != egrp) continue;
       const int gm = tile % mtiles, nt = (tile / mtiles) % p.ntiles, bb = tile / (mtiles * p.ntiles);
       int ph = 0;
       while (gm >= p.ph_mt0[ph + 1]) ++ph;
+      const int g_begin = p.ph_g0[ph], g_end = p.ph_g0[ph + 1];
+      uint32_t scale_d = 0;
+      for (int c = 0; c < p.kchunks; ++c) {
+        const int kslices = (min(kTcKC, p.kg - c * kTcKC) + 15) >> 4;   // K = 16 slices holding real channels
+        for (int g = g_begin; g < g_end; ++g, ++it_a) {
+          const int sa = it_a % p.na_stages;
+          mbar_wait(&full_a[sa], (it_a / p.na_stages) & 1);
+          const uint32_t a16 = a_base16 + (uint32_t)sa * a_stage16;
+          for (int n = p.grp_first[g]; n < p.grp_first[g + 1]; ++n, ++it_b) {
+            int sb;
+            if (resident) {
+              sb = c * p.ntaps + n;
+              if (ti == 0) mbar_wait(&full_b[sb], 0u);
+            } else {
+              sb = it_b % p.nb_stages;
+              mbar_wait(&full_b[sb], (uint32_t)((it_b / p.nb_stages) & 1));
+            }
+            const uint32_t a_hi = a16 + s_tapshift[n];
+            const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
+            wgmma_fence();
+            for (int ks = 0; ks < kslices; ++ks) {
+              wgmma_x3<0, 0>(NT, acc, a_hi + 2u * ks, img16, b_hi + 2u * ks, bplane16, scale_d);
+              scale_d = 1;
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(acc);
+            if (!resident && lane == 0) mbar_arrive(&empty_b[sb]);
+          }
+          if (lane == 0) mbar_arrive(&empty_a[sa]);
+        }
+      }
+      // ---- epilogue: registers -> bias / activation / residual (or act' mask for the data gradient) -> output rows
       const int mt = gm - p.ph_mt0[ph];
       const int F = p.ph_M[ph] * p.nsub;
-      const int buf = ti & 1;
-      if (tracer) trace_ev(p, 3, ti, 0);
-      mbar_wait(&tmem_full[buf], (ti >> 1) & 1);
-      tc_fence_after();
-      if (tracer) trace_ev(p, 3, ti, 1);
-      const int f = mt * kTcM + quarter * 32 + lane;
-      const bool valid = f < F;
-      const int m = valid ? (p.nsub == 1 ? f : f / p.nsub) : 0;
-      const int w = valid ? f - m * p.nsub : 0;
-      const int to = p.ph_ooff[ph] + p.o_step * m;
-      const int orow = (bb * p.t_out + to) * p.nsub + w;                  // output row (flattened), < 2^31
-      const long long obase = (long long)orow * p.c_out + (long long)nt * p.n_stride;
-      const int n_valid = min(p.n_stride, p.c_out - nt * p.n_stride);   // real output channels of this tile
-      const bool vec_out = SIMPLE || ((n_valid | p.c_out | p.n_stride) & 3) == 0;
-      const uint32_t t_lane = tmem_acc + (uint32_t)buf * buf_cols + ((uint32_t)(quarter * 32) << 16);
-      // forward: residual add; data gradient: act_in' mask -- never both (the scalar path handles the general case)
-      const float* side_p = p.resid ? p.resid : p.mask.p;
-      const bool side_is_mask = p.resid == nullptr;
-      const bool coalesced = vec_out && !(p.resid && p.mask.p);          // warp-uniform
-      if (coalesced && p.bias) {   // per-tile bias -> shared memory once: the chunk loop reads it with broadcast LDS.128
-        __syncwarp();
-        for (int e = lane; e < p.NT; e += 32) sbias[e] = e < n_valid ? __ldg(p.bias + nt * p.n_stride + e) : 0.f;
-        __syncwarp();
-      }
-      // rows this lane serves in the coalesced phase: row_i = 8 * i + lane / 4 (i = 0..3), 16-byte chunk cq = lane % 4
-      const int cq = lane & 3;
-      float* rptr[4];                      // &out[row_i][first column of this lane's 16-byte chunk in this tile]
-      uint32_t rok = 0;
-      if (coalesced) {
+      const int c_tile = nt * p.n_stride;
+      const int n_valid = min(p.n_stride, p.c_out - c_tile);   // real output channels of this tile
+      const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int src = i * 8 + (lane >> 2);
-          rptr[i] = p.out + ((long long)__shfl_sync(0xffffffffu, orow, src) * p.c_out + (long long)nt * p.n_stride + cq * 4);
-          rok |= (uint32_t)__shfl_sync(0xffffffffu, (int)valid, src) << i;
-        }
-      }
-      // residual / mask tensors are indexed like the output: one pointer difference serves every element
-      const long long side_delta = side_p ? side_p - p.out : 0;
-      const int side_kind = !side_p ? 0 : (!side_is_mask ? 1 : 2);          // 0 none, 1 residual add, 2 act' mask
-      for (int n0 = 0; n0 < p.NT; n0 += 32) {
-        uint32_t rr[32];
-        if (tracer && ti < 2) trace_ev(p, 4 + ti, n0 >> 5, 0);   // roles 4 / 5: per-chunk stamps, tiles 0 / 1
-        if (p.dbg & 8) {
+      for (int h = 0; h < 2; ++h) {
+        const int f = mt * kTcM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        if (f >= F) continue;
+        const int m = p.nsub == 1 ? f : f / p.nsub;
+        const int w = f - m * p.nsub;
+        const int to = p.ph_ooff[ph] + p.o_step * m;
+        const long long obase = ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
 #pragma unroll
-          for (int e = 0; e < 32; ++e) rr[e] = (uint32_t)(e + lane);
-        } else if (p.NT - n0 >= 32) {
-          tmem_ld32(t_lane + (uint32_t)n0, rr);
-        } else {  // NT % 32 == 16
-          uint32_t r16[16];
-          tmem_ld16(t_lane + (uint32_t)n0, r16);
+        for (int i = 0; i < kWgmmaMaxN / 8; ++i) {
+          const int col = i * 8 + 2 * (lane & 3);
+          if (i * 8 >= NT || col >= n_valid) continue;
+          float v[2] = {acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]};
+          const bool pair = vec2 && col + 1 < n_valid;
+          const int ne = col + 1 < n_valid ? 2 : 1;
+          float bia[2] = {0.f, 0.f}, sd[2] = {0.f, 0.f}, md[2] = {0.f, 0.f}, od[2] = {0.f, 0.f};
+          const long long o = obase + col;
+          if (pair) {
+            if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + c_tile + col)); bia[0] = t.x; bia[1] = t.y; }
+            if (p.mask.p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.mask.p + o)); md[0] = t.x; md[1] = t.y; }
+            if (p.resid) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.resid + o)); sd[0] = t.x; sd[1] = t.y; }
+            if (!SIMPLE && p.accumulate) { const float2 t = *reinterpret_cast<const float2*>(p.out + o); od[0] = t.x; od[1] = t.y; }
+          } else {
 #pragma unroll
-          for (int e = 0; e < 16; ++e) { rr[e] = r16[e]; rr[16 + e] = 0u; }
-        }
-        const int ncols_t = min(32, n_valid - n0);       // real columns of this chunk (tile-uniform, may be <= 0)
-        // side-tensor loads of the first 16-column half are issued before the TMEM load is waited for; those of the
-        // second half while the first half is being transposed (volatile asm: the compiler must not sink them to their
-        // uses -- that serialised the store loop on one L2 round trip per row group)
-        float4 sd[2][4];
-        auto side_load = [&](int h) {
-          const bool col_ok = h * 16 + cq * 4 < ncols_t;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float* a = (col_ok && ((rok >> i) & 1u)) ? rptr[i] + side_delta + (n0 + h * 16) : side_p;
-            asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];"
-                         : "=f"(sd[h][i].x), "=f"(sd[h][i].y), "=f"(sd[h][i].z), "=f"(sd[h][i].w) : "l"(a));
-          }
-        };
-        if (coalesced && side_p && !(p.dbg & 1)) side_load(0);
-        tmem_ld_wait();
-        if (p.fuse2 && !(p.dbg & 8)) {   // + the hi*lo products (columns [NT, 2*NT)), 16 columns at a time (registers)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t t2[16];
-            tmem_ld16(t_lane + (uint32_t)(p.NT + n0 + 16 * h), t2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) rr[16 * h + e] = __float_as_uint(__uint_as_float(rr[16 * h + e]) + __uint_as_float(t2[e]));
-          }
-        }
-        if (n0 + 32 >= p.NT) {   // last TMEM read of this tile: hand the buffer back to the MMA issuer
-          tc_fence_before();
-          mbar_arrive(&tmem_empty[buf]);
-          if (tracer) trace_ev(p, 3, ti, 2);
-        }
-        if (tracer && ti < 2) trace_ev(p, 4 + ti, n0 >> 5, 1);
-        if (coalesced && !(p.dbg & 4)) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (h == 0 && side_p && !(p.dbg & 1)) side_load(1);
-            // ---- row-owner layout: bias + output activation, then into the transposition tile
-#pragma unroll
-            for (int e4 = 0; e4 < 4; ++e4) {
-              const int e = h * 16 + e4 * 4;
-              float v[4] = {__uint_as_float(rr[e]), __uint_as_float(rr[e + 1]), __uint_as_float(rr[e + 2]), __uint_as_float(rr[e + 3])};
-              if (p.bias) {
-                const float4 b = *reinterpret_cast<const float4*>(sbias + n0 + e);
-                v[0] += b.x; v[1] += b.y; v[2] += b.z; v[3] += b.w;
-              }
-              if (p.out_act == KT_ACT_LRELU) {
-#pragma unroll
-                for (int z = 0; z < 4; ++z) v[z] = v[z] > 0.f ? v[z] : v[z] * p.out_slope;
-              } else if (!SIMPLE && p.out_act == KT_ACT_TANH) {
-#pragma unroll
-                for (int z = 0; z < 4; ++z) v[z] = tanhf(v[z]);
-              }
-              *reinterpret_cast<float4*>(stg + lane * 16 + ((e4 ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[0], v[1], v[2], v[3]);
+            for (int e = 0; e < 2; ++e) {
+              if (e >= ne) break;
+              if (p.bias) bia[e] = __ldg(p.bias + c_tile + col + e);
+              if (p.mask.p) md[e] = __ldg(p.mask.p + o + e);
+              if (p.resid) sd[e] = __ldg(p.resid + o + e);
+              if (!SIMPLE && p.accumulate) od[e] = p.out[o + e];
             }
-            __syncwarp();
-            // ---- coalesced layout: 4 lanes = one 64-byte row segment, 8 rows per instruction
-            const bool col_ok = h * 16 + cq * 4 < ncols_t;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int row = i * 8 + (lane >> 2);
-              float4 t = *reinterpret_cast<const float4*>(stg + row * 16 + ((cq ^ ((row >> 1) & 3)) << 2));
-              const float4 a = sd[h][i];
-              if (side_kind == 1) {
-                t.x += a.x; t.y += a.y; t.z += a.z; t.w += a.w;
-              } else if (side_kind == 2) {
-                if (p.mask.mode == SIDE_DLRELU) {
-                  t.x = a.x > 0.f ? t.x : t.x * p.mask.slope; t.y = a.y > 0.f ? t.y : t.y * p.mask.slope;
-                  t.z = a.z > 0.f ? t.z : t.z * p.mask.slope; t.w = a.w > 0.f ? t.w : t.w * p.mask.slope;
-                } else {
-                  t.x = side_apply(t.x, a.x, p.mask.mode, p.mask.slope); t.y = side_apply(t.y, a.y, p.mask.mode, p.mask.slope);
-                  t.z = side_apply(t.z, a.z, p.mask.mode, p.mask.slope); t.w = side_apply(t.w, a.w, p.mask.mode, p.mask.slope);
-                }
-              }
-              if (col_ok && ((rok >> i) & 1u) && !(p.dbg & 2)) {
-                float* o = rptr[i] + (n0 + h * 16);
-                if (!SIMPLE && p.accumulate) {
-                  const float4 c = *reinterpret_cast<const float4*>(o);
-                  t.x += c.x; t.y += c.y; t.z += c.z; t.w += c.w;
-                }
-                *reinterpret_cast<float4*>(o) = t;
-              }
-            }
-            __syncwarp();      // the tile is rewritten by the next half
           }
-          if (tracer && ti < 2) trace_ev(p, 4 + ti, n0 >> 5, 3);
-        } else if (!SIMPLE && valid) {
-          // thin / unaligned tiles (C_out = 1, ...): scalar epilogue
-          const int ncols = max(ncols_t, 0);
-          for (int e = 0; e < ncols; ++e) {
-            const long long o = obase + n0 + e;
-            float v = __uint_as_float(rr[e]);
-            if (p.bias) v += __ldg(p.bias + nt * p.n_stride + n0 + e);
-            if (p.out_act == KT_ACT_LRELU) v = v > 0.f ? v : v * p.out_slope;
-            else if (p.out_act == KT_ACT_TANH) v = tanhf(v);
-            if (p.mask.p) v = side_apply(v, __ldg(p.mask.p + o), p.mask.mode, p.mask.slope);
-            if (p.resid) v += __ldg(p.resid + o);
-            if (p.accumulate) v += p.out[o];
-            p.out[o] = v;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float x = v[e] + bia[e];
+            if (p.out_act == KT_ACT_LRELU) x = x > 0.f ? x : x * p.out_slope;
+            else if (!SIMPLE && p.out_act == KT_ACT_TANH) x = tanhf(x);
+            if (p.mask.p) x = side_apply(x, md[e], p.mask.mode, p.mask.slope);
+            x += sd[e] + od[e];
+            v[e] = x;
+          }
+          if (pair) *reinterpret_cast<float2*>(p.out + o) = make_float2(v[0], v[1]);
+          else {
+            p.out[o] = v[0];
+            if (ne == 2) p.out[o + 1] = v[1];
           }
         }
       }
-      if (tracer) trace_ev(p, 3, ti, 3);
     }
-    }
-  }
-
-  if (warp == 4 && lane == 0 && p.w_resident && (int)blockIdx.x < total_tiles)
-    for (int s = 0; s < p.nb_stages; ++s) mbar_wait(&full_b[s], 0);   // no bulk copy may outlive the CTA
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -704,40 +346,18 @@ struct TcLayerPlan {
   int kg;        // contraction channels per tile
   int n_total;   // produced channels (tensor width)
   int n_stride;  // produced channels per N tile
-  int NT;        // padded N tile (multiple of 16, <= 256)
+  int NT;        // padded N tile (multiple of 16, <= 128: the accumulators live in registers)
   int ntiles, kchunks, grouped;
   int kin_g, pout_g;   // grouped: channels of ONE group on the contraction / produced side (kg = gt * kin_g)
 };
 
 std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir);  // conv_ffma.cu
 struct TcParams;
-static int plan_max_rows(const KtConv1dDesc* d, int dir);
 
-// shared memory outside the activation / weight stages: barriers, TMEM slot, tap-shift table, epilogue transposition
-// + bias tiles (see the carve-up in conv_tc_kernel)
-static int tc_fixed_smem(int slots, bool epi_tma = false, bool epi_alias = false) {
-  return (2 * 3 + 2 * std::max(6, slots) + 4) * 8 + 16 + kMaxTaps * 4 + (epi_alias ? 0 : (epi_tma ? 8 * kEpiBufs * kEpiBufBytes : 8 * 2048)) +
-         8 * 1024 + 8 * kEpiBufs * 8;
-}
-static bool epi_tma_enabled() {
-  static const bool on = [] {
-    const char* e = std::getenv("KANTTS_B200_EPI_TMA");
-    return !(e && e[0] == '0') && encode_tiled_fn() != nullptr;
-  }();
-  return on;
-}
-// can a (rows, NT) tiling run with at least two activation and two weight stages?
-static bool tc_ring_fits(int rows, int NT) {
-  return 2 * (2 * rows * 128) + 2 * (2 * NT * 128) <= kMaxDynSmem - 1024 - tc_fixed_smem(0);
-}
+// shared memory outside the activation / weight stages: barriers and the tap-shift table (see the carve-up in conv_tc_kernel)
+static int tc_fixed_smem(int slots) { return (2 * 3 + 2 * std::max(6, slots)) * 8 + kMaxTaps * 4; }
 
 static int sm_count();
-
-// one phase writing consecutive output rows from row 0 (every forward of a plain conv, the data gradient of a stride-1 conv)
-static bool plain_single_phase(const KtConv1dDesc* d, int dir) {
-  const std::vector<Phase> ph = conv_phases(d, dir);
-  return ph.size() == 1 && ph[0].o_step == 1 && ph[0].o_off == 0 && !ph[0].accumulate;
-}
 
 static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
   TcLayerPlan L{};
@@ -749,7 +369,7 @@ static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
   L.kchunks = ceil_div(kin, kTcKC);
   L.grouped = g > 1;
   if (g > 1) {
-    if (pout > 256) return L;
+    if (pout > kWgmmaMaxN) return L;
     // groups per tile: fill one 64-channel K chunk, keep the N tile <= 128 (block-diagonal tile, see tc_pack_weights_kernel)
     int gt = 1;
     while (gt * 2 <= g && g % (gt * 2) == 0 && kin * gt * 2 <= kTcKC && pout * gt * 2 <= 128) gt *= 2;
@@ -757,22 +377,18 @@ static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
     L.kg = gt * kin;
     L.kchunks = ceil_div(L.kg, kTcKC);
     L.n_stride = gt * pout; L.NT = (L.n_stride + 15) & ~15; L.ntiles = g / gt;
-  } else if (pout <= 256) {
-    L.n_stride = pout; L.NT = (pout + 15) & ~15; L.ntiles = 1;
+  } else if (pout <= 2 * kWgmmaMaxN) {
+    // N tiles of <= 128 channels (a 64-row half tile's accumulators are 64 registers per thread at N = 128)
+    L.ntiles = ceil_div(pout, kWgmmaMaxN);
+    L.n_stride = (ceil_div(pout, L.ntiles) + 15) & ~15; L.NT = L.n_stride;
     // under-filled grids (short sequences x wide layers): split N so that >= ~1 tile per SM exists
     const long long mtiles = (long long)ceil_div((dir == 0 ? d->t_out : d->t_in) * d->nsub, kTcM) * d->batch;
     while (mtiles * L.ntiles < 120 && L.NT >= 128 && L.NT % 32 == 0 && pout % (L.NT / 2) == 0) {
       L.NT /= 2; L.n_stride = L.NT; L.ntiles = pout / L.NT;
     }
   } else {
-    L.NT = pout % 256 == 0 ? 256 : (pout % 128 == 0 ? 128 : 0);
+    L.NT = pout % 128 == 0 ? 128 : 0;
     if (L.NT == 0) return L;
-    const long long mtiles = (long long)ceil_div((dir == 0 ? d->t_out : d->t_in) * d->nsub, kTcM) * d->batch;
-    if (L.NT == 256 && mtiles * (pout / 256) < 120) L.NT = 128;
-    if (L.NT == 256 && !tc_ring_fits(plan_max_rows(d, dir), 256)) L.NT = 128;   // long-halo (strided) layers: 64 KB weight stages do not fit
-    // TMA epilogue: its boxes take the room of one 64 KB stage -- unless every CTA gets at most one tile (the boxes then
-    // reuse the idle operand stages, epi_alias)
-    if (L.NT == 256 && epi_tma_enabled() && plain_single_phase(d, dir) && mtiles * (pout / 256) > sm_count()) L.NT = 128;
     L.n_stride = L.NT; L.ntiles = pout / L.NT;
   }
   L.ok = true;
@@ -846,16 +462,7 @@ static bool plan_launches(const std::vector<Phase>& phases, int nsub, std::vecto
   return true;
 }
 
-// image rows (128 + halo) the layer's phases need (0: the phases do not fit the kernel's limits)
-static int plan_max_rows(const KtConv1dDesc* d, int dir) {
-  std::vector<TcParams> launches;
-  if (!plan_launches(conv_phases(d, dir), d->nsub, launches, TcParams{})) return 0;
-  int rows = 0;
-  for (const TcParams& lp : launches) rows = std::max(rows, lp.rows);
-  return rows;
-}
-
-// Is (direction dir: 0 fwd, 1 bwd_data) of this layer runnable on the tcgen05 kernel?  -> N tile or 0
+// Is (direction dir: 0 fwd, 1 bwd_data) of this layer runnable on the tensor-core kernel?  -> N tile or 0
 bool thin_cin1_ok(const KtConv1dDesc* d);   // thin.cu
 
 int tc_plan(const KtConv1dDesc* d, int dir) {
@@ -877,7 +484,7 @@ long long tc_image_bytes(const KtConv1dDesc* d, int dir) {
 
 // w = the fp32 kernel-layout weight of this direction (w_fwd for dir 0, w_bwd for dir 1): [taps][K][N]
 int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cudaStream_t st) {
-  KT_REQUIRE(w && out && tc_plan(d, dir) > 0, "tc_pack_layer: layer not supported by the tcgen05 path");
+  KT_REQUIRE(w && out && tc_plan(d, dir) > 0, "tc_pack_layer: layer not supported by the tensor-core path");
   const TcLayerPlan L = layer_plan(d, dir);
   const dim3 grid((unsigned)(d->kernel * L.kchunks * L.ntiles), (unsigned)ceil_div(L.NT * 8, 256));
   tc_pack_weights_kernel<<<grid, 256, 0, st>>>(w, d->kernel, L.kg, L.n_total, L.NT, L.n_stride, L.ntiles,
@@ -890,78 +497,34 @@ static int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
 
-static long long* g_trace = nullptr;   // development aid, not thread-safe: set by kt_debug_set_trace
-static int g_dbg = 0;
+static int g_dbg = 0;   // development aid (kt_debug_set_flags): ablation switches of the weight-gradient chain, see wgrad_tc.cu
 void debug_set_flags(int f) { g_dbg = f; }
 int debug_flags() { return g_dbg; }
-void debug_set_trace(long long* dev_buf) { g_trace = dev_buf; }
-
-static bool tc_env_flag(const char* name) {
-  const char* e = std::getenv(name);
-  return e && e[0] == '1';
-}
+void debug_set_trace(long long*) {}   // (the per-role timelines belonged to the previous tensor-core kernels)
 
 static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned by plan_launches
-  p.trace = g_trace;
-  p.dbg = g_dbg;
-  p.fuse2 = (p.NT <= 128 && p.NT % 32 == 0) ? 1 : 0;   // [a_hi*b_hi | a_hi*b_lo] as one N = 2*NT MMA: A is read from shared memory once for both products
-  p.tmem_cols = 32;
-  while (p.tmem_cols < (p.fuse2 ? 2 : 1) * p.NT) p.tmem_cols <<= 1;
-  p.tmem_cols *= 2;                                   // two accumulator buffers
   const int a_stage = 2 * p.rows * 128;
   const int b_stage = 2 * p.NT * 128;
   const int slots = p.ntaps * p.kchunks;                                      // weight tiles of the whole layer
-  // TMA epilogue: one phase of consecutive output rows, whole 16-column boxes inside this tile's channel range (or past the
-  // tensor's last channel, where the TMA unit clips), at most one side operand, room for two image + two weight stages
-  const float* side_ptr = p.resid ? p.resid : p.mask.p;
   const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
-  const bool one_tile = tiles <= sm_count();
-  p.epi_tma = (epi_tma_enabled() && p.nphases == 1 && p.o_step == 1 && p.ph_ooff[0] == 0 && !p.accumulate && p.ph_M[0] == p.t_out &&
-               (p.c_out & 3) == 0 && (p.ntiles == 1 || p.n_stride == p.NT) && !(p.resid && p.mask.p) &&
-               (!p.mask.p || p.mask.mode == SIDE_DLRELU) && (p.NT & 15) == 0 &&
-               2 * a_stage + 2 * b_stage <= kMaxDynSmem - 1024 - tc_fixed_smem(slots, true, one_tile) &&
-               (!one_tile || 2 * a_stage + 2 * b_stage >= 8 * kEpiBufs * kEpiBufBytes)) ? 1 : 0;
-  p.epi_split = (p.epi_tma && (p.NT & 31) == 0) ? 1 : 0;
-  p.epi_alias = (p.epi_tma && one_tile) ? 1 : 0;
-  const int bar_bytes = tc_fixed_smem(slots, p.epi_tma != 0, p.epi_alias != 0);
+  const int bar_bytes = tc_fixed_smem(slots);
   const int budget = kMaxDynSmem - 1024 /*align slack*/ - bar_bytes;
-  if (p.epi_tma) {
-    // (cuTensorMapEncodeTiled is a driver call: it needs the primary context bound to THIS thread -- backward launches come from
-    //  autograd engine threads that may not have made a runtime call yet; any runtime call binds it, this one is capture-safe)
-    cudaStreamCaptureStatus cap;
-    KT_CHECK_CUDA(cudaStreamIsCapturing(st, &cap));
-    const cuuint64_t rows_item = (cuuint64_t)p.t_out * p.nsub;
-    const cuuint64_t gdim[3] = {(cuuint64_t)p.c_out, rows_item, (cuuint64_t)p.batch};
-    const cuuint64_t gstr[2] = {(cuuint64_t)p.c_out * 4, rows_item * p.c_out * 4};
-    const cuuint32_t box[3] = {16, 32, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = encode_tiled_fn()(&p.map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, p.out, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r == CUDA_SUCCESS && side_ptr)
-      r = encode_tiled_fn()(&p.map_side, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(side_ptr), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    KT_REQUIRE(r == CUDA_SUCCESS, "conv_tc: cuTensorMapEncodeTiled (epilogue) failed (%d)", (int)r);
-  }
   p.w_resident = 0;
   if (p.ntiles == 1 && slots <= 160 && 2 * a_stage + slots * b_stage <= budget) {
     p.w_resident = 1;
     p.nb_stages = slots;
     p.na_stages = (budget - slots * b_stage) / a_stage >= 3 ? 3 : 2;
   } else {
-    // The weight ring is what bounds wide layers: a stage (32 KB at N = 128) arrives ~0.65 us after its copy is issued, so a
-    // ring of two stages paces every (tap, chunk) step at ~0.65 us against 0.4 us of MMAs (call r2y: removing the MMAs, the
-    // producers or the copies one at a time changed nothing).  Layers with >= 4 taps per activation image spend long enough
-    // on one image for its successor to be staged meanwhile: they give the third image stage to the weight ring.
+    // Layers with >= 4 taps per activation image spend long enough on one image for its successor to be staged meanwhile:
+    // when three image and three weight stages do not fit, they give the third image stage to the weight ring.
     int min_taps = kMaxTaps;
     for (int g = 0; g < p.ngroups; ++g) min_taps = std::min(min_taps, p.grp_first[g + 1] - p.grp_first[g]);
-    // (three of each when they fit -- single-tile launches, whose epilogue boxes reuse the stages)
-    p.na_stages = (3 * a_stage + 3 * b_stage <= budget) ? 3 : ((min_taps >= 4 && !tc_env_flag("KANTTS_B200_TC_NA3")) ? 2 : 3);
+    p.na_stages = (3 * a_stage + 3 * b_stage <= budget) ? 3 : (min_taps >= 4 ? 2 : 3);
     if (3 * a_stage + 2 * b_stage > budget) p.na_stages = 2;
     p.nb_stages = std::min(6, (budget - p.na_stages * a_stage) / b_stage);
   }
@@ -993,7 +556,7 @@ static Side make_side_tc(const float* p, const float* aux, int act, float slope,
 
 int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
                   float* y, cudaStream_t st) {
-  KT_REQUIRE(tc_plan(d, 0) > 0, "conv1d_fwd_tc: layer not supported by the tcgen05 path");
+  KT_REQUIRE(tc_plan(d, 0) > 0, "conv1d_fwd_tc: layer not supported by the tensor-core path");
   const TcLayerPlan L = layer_plan(d, 0);
   TcParams p{};
   p.NT = L.NT; p.ntiles = L.ntiles; p.kchunks = L.kchunks; p.kg = L.kg; p.grouped = L.grouped; p.n_stride = L.n_stride;
@@ -1013,7 +576,7 @@ int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const
 
 int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
                        float* dx, cudaStream_t st) {
-  KT_REQUIRE(tc_plan(d, 1) > 0, "conv1d_bwd_data_tc: layer not supported by the tcgen05 path");
+  KT_REQUIRE(tc_plan(d, 1) > 0, "conv1d_bwd_data_tc: layer not supported by the tensor-core path");
   const TcLayerPlan L = layer_plan(d, 1);
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_data: y required when act_out != NONE");
   KT_REQUIRE(d->act_in == KT_ACT_NONE || x != nullptr, "bwd_data: x required when act_in != NONE");

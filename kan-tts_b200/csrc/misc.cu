@@ -1,13 +1,15 @@
 // Small HBM-bound kernels of the HiFi-GAN hot path: sin(x)+x, resblock mean, db3 DWT pooling,
 // L1 reduction.  All are pure streaming kernels (one read / one write per element, float4 where
-// the shape allows), grid sized to a multiple of the 148 SMs.
+// the shape allows), grid sized to a multiple of the 132 SMs.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace kt {
 
 static inline int stream_grid(long long n_items, int threads) {
   long long blocks = (n_items + threads - 1) / threads;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
@@ -51,7 +53,7 @@ __global__ void add3_scale_kernel(const float* __restrict__ a, const float* __re
 }
 
 // Data gradient of `nn.Upsample(nearest, scale) -> LeakyReLU -> conv` (hifigan.py:82-97) in two steps: the plain
-// conv data gradient wrt the (never materialised in forward) up-sampled rows runs on the tcgen05 kernel, then
+// conv data gradient wrt the (never materialised in forward) up-sampled rows runs on the tensor-core kernel, then
 //   dx[r][c] = act_in'(x[r][c]) * sum_{u < up} dxu[r*up + u][c]
 // folds the `up` replicated rows back (bound: HBM, reads up*rows*C + rows*C floats once).
 __global__ void upsample_grad_reduce_kernel(const float* __restrict__ dxu, const float* __restrict__ x, int act,
@@ -128,7 +130,55 @@ __global__ void dwt_bwd_kernel(const float* __restrict__ dy, float* __restrict__
   }
 }
 
-__global__ void l1_sum_kernel(const float* __restrict__ a, const float* __restrict__ b, long long n, float scale, float* out) {
+// one thread per output, slots in ascending order
+__global__ void split_sum_kernel(const float* __restrict__ part, long long n, int nsplit, long long stride, float* __restrict__ out,
+                                 int accumulate) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int s = 0; s < nsplit; ++s) acc += __ldg(part + (long long)s * stride + i);
+    out[i] = accumulate ? out[i] + acc : acc;
+  }
+}
+
+// few outputs, many slots: one block per output; thread t sums the slots t, t + 256, ... in order, then a fixed tree
+__global__ void split_sum_wide_kernel(const float* __restrict__ part, long long n, int nsplit, long long stride, float* __restrict__ out,
+                                      int accumulate) {
+  __shared__ float red[256];
+  for (long long i = blockIdx.x; i < n; i += gridDim.x) {
+    float acc = 0.f;
+    for (int s = threadIdx.x; s < nsplit; s += 256) acc += __ldg(part + (long long)s * stride + i);
+    red[threadIdx.x] = acc;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+      if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) out[i] = accumulate ? out[i] + red[0] : red[0];
+    __syncthreads();
+  }
+}
+
+int scratch_alloc(float** p, long long floats, cudaStream_t st) {
+  KT_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(p), (size_t)std::max<long long>(floats, 1) * sizeof(float), st));
+  return KT_OK;
+}
+int scratch_free(float* p, cudaStream_t st) {
+  KT_CHECK_CUDA(cudaFreeAsync(p, st));
+  return KT_OK;
+}
+
+int split_sum(const float* part, long long n, int nsplit, long long stride, float* out, bool accumulate, cudaStream_t st) {
+  if (n <= 0) return KT_OK;
+  if (nsplit >= 64 && n <= 4096)
+    split_sum_wide_kernel<<<(int)std::min<long long>(n, 132LL * 8), 256, 0, st>>>(part, n, nsplit, stride, out, accumulate ? 1 : 0);
+  else
+    split_sum_kernel<<<stream_grid(n, 256), 256, 0, st>>>(part, n, nsplit, stride, out, accumulate ? 1 : 0);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+// per-block partial sums of scale * |a - b| -> part[blockIdx.x] (summed in order by split_sum)
+__global__ void l1_sum_kernel(const float* __restrict__ a, const float* __restrict__ b, long long n, float scale, float* part) {
   float acc = 0.f;
   const long long gtid = blockIdx.x * (long long)blockDim.x + threadIdx.x, gsz = (long long)gridDim.x * blockDim.x;
   const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0;
@@ -146,7 +196,7 @@ __global__ void l1_sum_kernel(const float* __restrict__ a, const float* __restri
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    atomicAdd(out, t * scale);
+    part[blockIdx.x] = t * scale;
   }
 }
 
@@ -187,11 +237,19 @@ int dwt_bwd(const float* dy, float* dx, int batch, int t, cudaStream_t st) {
 }
 int l1_sum(const float* a, const float* b, long long n, float scale, float* out, cudaStream_t st, bool accumulate) {
   KT_REQUIRE(a && b && out && n >= 0, "l1_sum: bad arguments");
-  if (!accumulate) KT_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
-  if (n == 0) return KT_OK;
-  l1_sum_kernel<<<stream_grid(n / 4 + 1, 256), 256, 0, st>>>(a, b, n, scale, out);
+  if (n == 0) {
+    if (!accumulate) KT_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
+    return KT_OK;
+  }
+  const int blocks = stream_grid(n / 4 + 1, 256);
+  float* part = nullptr;
+  int rc = scratch_alloc(&part, blocks, st);
+  if (rc) return rc;
+  l1_sum_kernel<<<blocks, 256, 0, st>>>(a, b, n, scale, part);
   KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
+  rc = split_sum(part, 1, blocks, 1, out, accumulate, st);
+  if (rc) return rc;
+  return scratch_free(part, st);
 }
 
 }  // namespace kt

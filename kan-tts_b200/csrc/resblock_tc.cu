@@ -5,8 +5,8 @@
 //
 // in ONE launch for the thin stages (C = 32 / 64 channels) -- unfused, each of the two convs re-stages its input
 // (global fp32 -> split bf16 shared-memory image) and writes / re-reads the intermediate; the pair is bound by that
-// staging and by the epilogue, not by the tensor pipe (profiles/r02_notes.md).  Here the intermediate never leaves the
-// SM: epilogue 1 turns the c1 accumulator (TMEM) straight into the split-bf16 shared-memory image c2's MMAs read.
+// staging and by the epilogue, not by the tensor pipe.  Here the intermediate never leaves the
+// SM: epilogue 1 turns the c1 accumulators (registers) straight into the split-bf16 shared-memory image c2's MMAs read.
 //
 // Tile = TO = 128 - (k - 1) consecutive outputs of one batch item.  c2 needs h on the 128 rows [H0, H0 + 128),
 // H0 = i * TO - p2 (one M = 128 MMA block; rows outside [0, T) are c2's zero padding); c1 needs x on
@@ -14,10 +14,7 @@
 // conv_tc.cu.  C = 32 packs TWO taps per 64-wide K chunk: image row r holds [act(x[r]) | act(x[r + d])], so a tap pair is
 // one dense K = 64 step and the resident weights halve (k = 11: 96 KB for both convs).
 //
-// Warp roles (576 threads): 0-3 / 10-13 producers of x images (alternate tiles), 4 weight stream (bulk async copies),
-// 5 MMA issuer, 6-9 epilogue 1 (TMEM -> +b1 -> [h to global] -> lrelu -> split -> H image), 14-17 epilogue 2
-// (TMEM -> +b2 -> transposition -> +x -> y).  The MMA issuer software-pipelines  c1(i+1) | c2(i)  so that the tensor
-// pipe runs the next tile's first conv while epilogue 1 builds this tile's H image.
+// Warp roles: see resblock_tc_kernel.
 
 #include <algorithm>
 #include <atomic>
@@ -31,7 +28,7 @@ namespace kt {
 
 using namespace tc;
 
-constexpr int kRbThreads = 576;
+constexpr int kRbThreads = 416;
 constexpr int kRbM = 128;
 
 struct RbParams {
@@ -118,46 +115,6 @@ __device__ __forceinline__ void rb_stage_pair(uint8_t* img_hi, uint8_t* img_lo, 
   }
 }
 
-// ---- coalesced store of one 32-row x 32-column chunk held row-per-thread (see conv_tc.cu's epilogue) ----------------
-// v: this thread's row, 32 columns.  Two 16-column halves through the warp's 2 KB transposition tile; 4 consecutive
-// lanes then own one 64-byte row segment (rows 8 i + lane / 4).  RESID: += side tensor (same indexing as the output).
-template <bool RESID>
-__device__ __forceinline__ void rb_store32(float* stg, int lane, const float (&v)[32], float* const (&rptr)[4], uint32_t rok,
-                                           int n0, int ncols, long long side_delta, const float* safe) {
-  const int cq = lane & 3;
-  float4 sd[2][4];
-  if (RESID) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const bool col_ok = h * 16 + cq * 4 < ncols;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float* a = (col_ok && ((rok >> i) & 1u)) ? rptr[i] + side_delta + (n0 + h * 16) : safe;   // always readable
-        asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];"
-                     : "=f"(sd[h][i].x), "=f"(sd[h][i].y), "=f"(sd[h][i].z), "=f"(sd[h][i].w) : "l"(a));
-      }
-    }
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-#pragma unroll
-    for (int e4 = 0; e4 < 4; ++e4) {
-      const int e = h * 16 + e4 * 4;
-      *reinterpret_cast<float4*>(stg + lane * 16 + ((e4 ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[e], v[e + 1], v[e + 2], v[e + 3]);
-    }
-    __syncwarp();
-    const bool col_ok = h * 16 + cq * 4 < ncols;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int row = i * 8 + (lane >> 2);
-      float4 t = *reinterpret_cast<const float4*>(stg + row * 16 + ((cq ^ ((row >> 1) & 3)) << 2));
-      if (RESID) { t.x += sd[h][i].x; t.y += sd[h][i].y; t.z += sd[h][i].z; t.w += sd[h][i].w; }
-      if (col_ok && ((rok >> i) & 1u)) *reinterpret_cast<float4*>(rptr[i] + (n0 + h * 16)) = t;
-    }
-    __syncwarp();
-  }
-}
-
 // ---- TMA: one box (32 channels x rows) of the 3-D tensor (C, T, B) -> shared memory, completion on an mbarrier (SASS UTMALDG)
 __device__ __forceinline__ void tma_load_box(void* dst_smem, const CUtensorMap* map, int c0, int t0, int b, uint64_t* bar) {
   asm volatile(
@@ -190,6 +147,16 @@ __device__ __forceinline__ void rb_convert_tile(uint8_t* img_hi, uint8_t* img_lo
   }
 }
 
+// Warp roles (416 threads): warpgroup 0 produces the x images, warpgroups 1 / 2 are the consumers (each: the 64-row half
+// of both convs' wgmma and of both epilogues), warp 12 streams weights (bulk async copies).  (Warps hold registers in
+// groups of four: 13 warps keep the 128 registers per thread the consumers' accumulators need.)
+// Per tile a consumer runs c1 (x image -> registers), epilogue 1 (+b1 -> [h to global] -> lrelu -> split -> its half of
+// the H image), a named barrier of both consumers, c2 (H image -> registers) and epilogue 2 (+b2 + x -> y).
+constexpr int kRbConsumerArrivals = 8;   // one per consumer warp
+constexpr int kRbConsumerBar = 1;        // named barrier of the 256 consumer threads
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync %0, 256;" ::"n"(kRbConsumerBar) : "memory"); }
+
 __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -203,56 +170,37 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
   uint64_t* bars = reinterpret_cast<uint64_t*>(f_base + (p.tma ? (size_t)p.nx * p.fstage_bytes : 0));
   uint64_t* x_full = bars;                 // [2]
   uint64_t* x_empty = x_full + 2;          // [2]
-  uint64_t* a1_full = x_empty + 2;         // [2]
-  uint64_t* a1_empty = a1_full + 2;        // [2]
-  uint64_t* a2_full = a1_empty + 2;        // [2]
-  uint64_t* a2_empty = a2_full + 2;        // [2]
-  uint64_t* h_full = a2_empty + 2;         // [1]
-  uint64_t* h_empty = h_full + 1;          // [1]
-  uint64_t* w_full = h_empty + 1;          // [nslots]
+  uint64_t* w_full = x_empty + 2;          // [nslots]
   uint64_t* w_empty = w_full + nslots;     // [nslots] (ring only)
   uint64_t* f_full = w_empty + nslots;     // [2] (tma only): the x tile has landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(f_full + 2);
-  float* epi_stage = reinterpret_cast<float*>(tmem_slot + 4);        // 8 warps x 32 rows x 16 fp32
-  float* s_bias = epi_stage + 8 * 32 * 16;                           // b1 | b2 (2 * NT floats)
+  float* s_bias = reinterpret_cast<float*>(f_full + 2);              // b1 | b2 (2 * NT floats)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile_cta = ((int)blockIdx.x < p.total_tiles) ? (p.total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const uint32_t acc_cols = 2u * (uint32_t)NT;                       // fuse2: [hi*hi | hi*lo] column ranges
-  const uint32_t tmem_cols = 4u * acc_cols < 32u ? 32u : 4u * acc_cols;   // acc1[2], acc2[2]: 256 (C = 32) / 512 (C = 64)
 
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
-      mbar_init(&x_full[s], p.tma ? 256 : 128); mbar_init(&x_empty[s], 1);
+      mbar_init(&x_full[s], 128); mbar_init(&x_empty[s], kRbConsumerArrivals);
       mbar_init(&f_full[s], 1);
-      mbar_init(&a1_full[s], 1); mbar_init(&a1_empty[s], 128);
-      mbar_init(&a2_full[s], 1); mbar_init(&a2_empty[s], 128);
     }
-    mbar_init(h_full, 128); mbar_init(h_empty, 1);
-    for (int s = 0; s < nslots; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
+    for (int s = 0; s < nslots; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], kRbConsumerArrivals); }
     mbar_fence_init();
     fence_proxy_async();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
   // the H image starts as zeros: rows >= 128 (read only by discarded output rows) and, in the paired layout, the
   // second half of row 127 are never written
   for (int i = tid; i < 2 * himg / 16; i += kRbThreads) reinterpret_cast<uint4*>(h_base)[i] = make_uint4(0u, 0u, 0u, 0u);
   for (int i = tid; i < 2 * NT; i += kRbThreads) s_bias[i] = i < NT ? (p.b1 ? p.b1[i] : 0.f) : (p.b2 ? p.b2[i - NT] : 0.f);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
 
-  if (warp < 4 || (warp >= 10 && warp < 14)) {
+  if (warp < 4) {
     // ===================== producers: x images (fused input LeakyReLU) =====================
-    const int pg = warp < 4 ? 0 : 1;
-    const int ptid = warp < 4 ? tid : tid - 320;
+    const int ptid = tid;
     if (p.tma) {
-      // TMA-staged: both groups convert the landed fp32 tile cooperatively (upper / lower half of the image rows); thread 0
-      // of group 0 issues the loads, `nx` tiles ahead, as soon as the landing stage has been read
-      const int split = ((p.rows_x / 2) + 15) & ~15;
-      const int r0 = pg ? min(split, p.rows_x) : 0, r1 = pg ? p.rows_x : min(split, p.rows_x);
+      // TMA-staged: the producers convert the landed fp32 tile; thread 0 issues the loads, `nx` tiles ahead, as soon as the
+      // landing stage has been read
+      const int r0 = 0, r1 = p.rows_x;
       const int nbox = p.c / 32, box_floats = p.rows_box * 32;
       auto issue = [&](int ti) {
         const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
@@ -263,7 +211,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
         for (int bx = 0; bx < nbox; ++bx)
           tma_load_box(f_base + (size_t)s * p.fstage_bytes + (size_t)bx * box_floats * 4, &p.tmx, bx * 32, x0, bb, &f_full[s]);
       };
-      if (pg == 0 && ptid == 0)
+      if (ptid == 0)
         for (int ti = 0; ti < min(p.nx, ntile_cta); ++ti) issue(ti);
       for (int ti = 0; ti < ntile_cta; ++ti) {
         const int s = ti % p.nx, n = ti / p.nx;
@@ -275,15 +223,12 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
         else rb_convert_tile<false>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
         fence_proxy_async();
         mbar_arrive(&x_full[s]);
-        asm volatile("bar.sync 1, 256;" ::: "memory");          // every producer thread has read the landing stage
-        if (pg == 0 && ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx);
+        asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
+        if (ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx);
       }
     } else {
     const Side sx{p.x, nullptr, SIDE_LRELU, p.slope};
     for (int ti = 0; ti < ntile_cta; ++ti) {
-      // two stages: the groups own one stage each (alternate tiles).  One stage: group 0 alone -- two groups waiting on the
-      // SAME barrier for consecutive phases could overtake each other (parity waits alias phases mod 2)
-      if (p.nx == 2 ? ((ti & 1) != pg) : (pg != 0)) continue;
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
       const int x0 = it * p.to - p.p2 - p.p1;
@@ -301,7 +246,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
       mbar_arrive(&x_full[s]);
     }
     }
-  } else if (warp == 4) {
+  } else if (warp == 12) {
     // ===================== weight stream =====================
     if (elect_one() && ntile_cta > 0) {
       if (p.resident) {
@@ -310,8 +255,9 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
           mbar_arrive_expect_tx(&w_full[s], (uint32_t)p.tile_bytes);
           bulk_g2s(w_base + (size_t)s * p.tile_bytes, src, (uint32_t)p.tile_bytes, &w_full[s]);
         }
+        for (int s = 0; s < 2 * p.nsteps; ++s) mbar_wait(&w_full[s], 0);   // no bulk copy may outlive the CTA
       } else {
-        // same job order as the MMA issuer: c1(0); then per tile: c1(ti + 1), c2(ti)
+        // same job order as the consumers: per tile c1, c2
         int it = 0;
         auto stream_conv = [&](const __nv_bfloat16* w) {
           for (int s = 0; s < p.nsteps; ++s, ++it) {
@@ -322,210 +268,128 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
                      (uint32_t)p.tile_bytes, &w_full[slot]);
           }
         };
-        stream_conv(p.w1);
         for (int ti = 0; ti < ntile_cta; ++ti) {
-          if (ti + 1 < ntile_cta) stream_conv(p.w1);
+          stream_conv(p.w1);
           stream_conv(p.w2);
         }
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    if (elect_one() && ntile_cta > 0) {
-      const uint32_t idesc = make_idesc_bf16(kRbM, NT, 0, 0);
-      const uint32_t idesc2 = make_idesc_bf16(kRbM, 2 * NT, 0, 0);
-      const uint32_t x16 = (smem_u32(x_base) >> 4) | 0x10000u, h16 = (smem_u32(h_base) >> 4) | 0x10000u;
-      const uint32_t w16 = (smem_u32(w_base) >> 4) | 0x10000u;
-      const uint32_t ximg16 = (uint32_t)ximg >> 4, himg16 = (uint32_t)himg >> 4, tile16 = (uint32_t)p.tile_bytes >> 4;
-      const uint32_t step1 = (uint32_t)((p.pair ? 2 : 1) * p.d1) * 8u;      // row shift per MMA step, 16-byte units
-      const uint32_t step2 = (uint32_t)(p.pair ? 2 : 1) * 8u;
-      int it_w = 0;
-      // one conv of one tile: A = image (hi plane at a16, lo plane a16 + plane16), taps = descriptor row shifts
-      auto run_conv = [&](int cv, uint32_t a16, uint32_t plane16, uint32_t astep, uint32_t d_tmem, bool first_pass) {
-        uint32_t acc = 0;
-        for (int s = 0; s < p.nsteps; ++s, ++it_w) {
-          int slot;
-          if (p.resident) {
-            slot = cv * p.nsteps + s;
-            if (first_pass) mbar_wait(&w_full[slot], 0u);
-          } else {
-            slot = it_w % p.nb;
-            mbar_wait(&w_full[slot], (uint32_t)((it_w / p.nb) & 1));
-          }
-          const uint32_t a_hi = a16 + (uint32_t)s * astep;
-          const uint32_t b_hi = w16 + (uint32_t)slot * tile16;
-          const int ks = (s == p.nsteps - 1) ? p.last_kslices : 4;
-          umma_step_fuse2(d_tmem, a_hi, plane16, b_hi, idesc2, idesc, acc, (uint32_t)ks);   // per slice: [a_hi*b_hi | a_hi*b_lo], a_lo*b_hi
-          acc = 1;
-          if (!p.resident) umma_commit(&w_empty[slot]);
+  } else if (warp >= 4 && warp < 12) {
+    // ===================== consumers =====================
+    const int cw = (warp - 4) >> 2;                  // 0: accumulator rows 0-63, 1: rows 64-127
+    const int wq = warp & 3;
+    const uint32_t x16 = smem_u32(x_base) >> 4, h16 = smem_u32(h_base) >> 4, w16 = smem_u32(w_base) >> 4;
+    const uint32_t half16 = (uint32_t)cw * 512u;                      // 64 rows x 128 B
+    const uint32_t ximg16 = (uint32_t)ximg >> 4, himg16 = (uint32_t)himg >> 4, tile16 = (uint32_t)p.tile_bytes >> 4;
+    const uint32_t bplane16 = (uint32_t)(NT * 128) >> 4;
+    const uint32_t step1 = (uint32_t)((p.pair ? 2 : 1) * p.d1) * 8u;      // row shift per MMA step, 16-byte units
+    const uint32_t step2 = (uint32_t)(p.pair ? 2 : 1) * 8u;
+    float acc[kWgmmaMaxRegs];
+#pragma unroll
+    for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
+    int it_w = 0;
+    // one conv of one tile: A = image (hi plane at a16, lo plane a16 + plane16), taps = descriptor row shifts
+    auto run_conv = [&](int cv, uint32_t a16, uint32_t plane16, uint32_t astep, bool first_pass) {
+      uint32_t scale_d = 0;
+      for (int s = 0; s < p.nsteps; ++s, ++it_w) {
+        int slot;
+        if (p.resident) {
+          slot = cv * p.nsteps + s;
+          if (first_pass) mbar_wait(&w_full[slot], 0u);
+        } else {
+          slot = it_w % p.nb;
+          mbar_wait(&w_full[slot], (uint32_t)((it_w / p.nb) & 1));
         }
-      };
-      auto conv1 = [&](int ti) {
-        const int s = ti % p.nx, n = ti / p.nx, b = ti & 1;
-        mbar_wait(&x_full[s], (uint32_t)(n & 1));
-        mbar_wait(&a1_empty[b], (uint32_t)(((ti >> 1) & 1) ^ 1));
-        tc_fence_after();
-        run_conv(0, x16 + (uint32_t)s * 2u * ximg16, ximg16, step1, tmem_acc + (uint32_t)b * acc_cols, ti == 0);
-        umma_commit(&x_empty[s]);
-        umma_commit(&a1_full[b]);
-      };
-      auto conv2 = [&](int ti) {
-        const int b = ti & 1;
-        mbar_wait(h_full, (uint32_t)(ti & 1));
-        mbar_wait(&a2_empty[b], (uint32_t)(((ti >> 1) & 1) ^ 1));
-        tc_fence_after();
-        run_conv(1, h16, himg16, step2, tmem_acc + (uint32_t)(2 + b) * acc_cols, ti == 0);
-        umma_commit(h_empty);
-        umma_commit(&a2_full[b]);
-      };
-      conv1(0);
-      for (int ti = 0; ti < ntile_cta; ++ti) {
-        if (ti + 1 < ntile_cta) conv1(ti + 1);
-        conv2(ti);
+        const uint32_t a_hi = a16 + (uint32_t)s * astep;
+        const uint32_t b_hi = w16 + (uint32_t)slot * tile16;
+        const int ks = (s == p.nsteps - 1) ? p.last_kslices : 4;
+        wgmma_fence();
+        for (int k = 0; k < ks; ++k) {
+          wgmma_x3<0, 0>(NT, acc, a_hi + 2u * k, plane16, b_hi + 2u * k, bplane16, scale_d);
+          scale_d = 1;
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(acc);
+        if (!p.resident && lane == 0) mbar_arrive(&w_empty[slot]);
       }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogues =====================
-    const int quarter = warp & 3;
-    const bool second = warp >= 14;
-    const int ewarp = (second ? 4 : 0) + quarter;
-    float* stg = epi_stage + (size_t)ewarp * (32 * 16);
-    const int r = quarter * 32 + lane;                  // accumulator row of this thread
-    const int cq = lane & 3;
-    if (!second) {
-      // ---------- epilogue 1: acc1 -> h = acc + b1 -> [global] -> lrelu -> split -> H image ----------
-      for (int ti = 0; ti < ntile_cta; ++ti) {
-        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-        const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
-        const int h0 = it * p.to - p.p2;
+    };
+    for (int ti = 0; ti < ntile_cta; ++ti) {
+      const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+      const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
+      const int s = ti % p.nx, n = ti / p.nx;
+      // ---------- c1 ----------
+      mbar_wait(&x_full[s], (uint32_t)(n & 1));
+      run_conv(0, x16 + (uint32_t)s * 2u * ximg16 + half16, ximg16, step1, ti == 0);
+      if (lane == 0) mbar_arrive(&x_empty[s]);
+      // ---------- epilogue 1: h = acc + b1 -> [global] -> lrelu -> split -> H image ----------
+      const int h0 = it * p.to - p.p2;
+#pragma unroll
+      for (int i = 0; i < kWgmmaMaxRegs; ++i)
+        if ((i >> 2) * 8 < NT) acc[i] += s_bias[(i >> 2) * 8 + 2 * (lane & 3) + (i & 1)];
+      if (p.h) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+          const int t = h0 + r;
+          if (!(r >= p.p2 && r < p.p2 + p.to && t < p.t)) continue;
+          float* dst = p.h + ((long long)bb * p.t + t) * p.c + 2 * (lane & 3);
+#pragma unroll
+          for (int i = 0; i < kWgmmaMaxRegs / 4; ++i)
+            if (i * 8 < NT) *reinterpret_cast<float2*>(dst + i * 8) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+        }
+      }
+      consumer_sync();   // both consumers have finished c2 of the previous tile: the H image may be rewritten
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
         const int t = h0 + r;
         const bool in_range = t >= 0 && t < p.t;                       // else: c2's zero padding
-        const bool own = p.h != nullptr && r >= p.p2 && r < p.p2 + p.to && t < p.t;
-        const int b = ti & 1;
-        float* rptr[4];
-        uint32_t rok = 0;
-        if (p.h) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int src = i * 8 + (lane >> 2);
-            const long long orow = (long long)bb * p.t + __shfl_sync(0xffffffffu, t, src);
-            rptr[i] = p.h + orow * p.c + cq * 4;
-            rok |= (uint32_t)__shfl_sync(0xffffffffu, (int)own, src) << i;
+        for (int i = 0; i < kWgmmaMaxRegs / 4; ++i) {
+          if (i * 8 >= NT) continue;
+          float e2[2];
+#pragma unroll
+          for (int z = 0; z < 2; ++z) {
+            const float hv = acc[4 * i + 2 * hh + z];
+            e2[z] = in_range ? (hv > 0.f ? hv : hv * p.slope) : 0.f;
+          }
+          const __nv_bfloat162 hb = __floats2bfloat162_rn(e2[0], e2[1]);
+          const float2 hf = __bfloat1622float2(hb);
+          const __nv_bfloat162 lb = __floats2bfloat162_rn(e2[0] - hf.x, e2[1] - hf.y);
+          const uint32_t bo = 4u * (uint32_t)(lane & 3);                // byte offset of this thread's 2 channels in the 16-byte chunk
+          const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)i) + bo;
+          *reinterpret_cast<__nv_bfloat162*>(h_base + o) = hb;
+          *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o) = lb;
+          if (p.pair && r > 0) {   // second half of the previous row: act(h[r]) = "row r - 1, + 1"
+            const uint32_t o2 = sw128_offset((uint32_t)(r - 1), (uint32_t)i + 4u) + bo;
+            *reinterpret_cast<__nv_bfloat162*>(h_base + o2) = hb;
+            *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o2) = lb;
           }
         }
-        mbar_wait(&a1_full[b], (uint32_t)((ti >> 1) & 1));
-        tc_fence_after();
-        const uint32_t t_lane = tmem_acc + (uint32_t)b * acc_cols + ((uint32_t)(quarter * 32) << 16);
-        bool h_waited = false;
-        for (int n0 = 0; n0 < NT; n0 += 32) {
-          uint32_t rr[32];
-          tmem_ld32(t_lane + (uint32_t)n0, rr);
-          tmem_ld_wait();
-          float v[32];
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t t2[16];
-            tmem_ld16(t_lane + (uint32_t)(NT + n0 + 16 * hh), t2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[16 * hh + e] = __uint_as_float(rr[16 * hh + e]) + __uint_as_float(t2[e]);
-          }
-          if (n0 + 32 >= NT) {     // accumulator drained
-            tc_fence_before();
-            mbar_arrive(&a1_empty[b]);
-          }
-#pragma unroll
-          for (int e = 0; e < 32; e += 4) {
-            const float4 bv = *reinterpret_cast<const float4*>(s_bias + n0 + e);
-            v[e] += bv.x; v[e + 1] += bv.y; v[e + 2] += bv.z; v[e + 3] += bv.w;
-          }
-          if (p.h) rb_store32<false>(stg, lane, v, rptr, rok, n0, 32, 0, p.x);
-          if (!h_waited) {         // c2 of the previous tile must have consumed the H image
-            mbar_wait(h_empty, (uint32_t)((ti & 1) ^ 1));
-            h_waited = true;
-          }
-#pragma unroll
-          for (int c8 = 0; c8 < 4; ++c8) {
-            float e8[8];
-#pragma unroll
-            for (int z = 0; z < 8; ++z) {
-              const float hv = v[c8 * 8 + z];
-              e8[z] = in_range ? (hv > 0.f ? hv : hv * p.slope) : 0.f;
-            }
-            uint4 hi, lo;
-            split8(e8, hi, lo);
-            const uint32_t q = (uint32_t)(n0 >> 3) + (uint32_t)c8;
-            const uint32_t o = sw128_offset((uint32_t)r, q);
-            *reinterpret_cast<uint4*>(h_base + o) = hi;
-            *reinterpret_cast<uint4*>(h_base + himg + o) = lo;
-            if (p.pair && r > 0) {   // second half of the previous row: act(h[r]) = "row r - 1, + 1"
-              const uint32_t o2 = sw128_offset((uint32_t)(r - 1), q + 4u);
-              *reinterpret_cast<uint4*>(h_base + o2) = hi;
-              *reinterpret_cast<uint4*>(h_base + himg + o2) = lo;
-            }
-          }
-        }
-        fence_proxy_async();
-        mbar_arrive(h_full);
       }
-    } else {
-      // ---------- epilogue 2: acc2 -> + b2 -> transposition -> + x -> y ----------
-      const long long side_delta = p.x - p.y;
-      for (int ti = 0; ti < ntile_cta; ++ti) {
-        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-        const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
+      fence_proxy_async();
+      consumer_sync();   // the whole H image is written
+      // ---------- c2 ----------
+      run_conv(1, h16 + half16, himg16, step2, ti == 0);
+      // ---------- epilogue 2: y = acc + b2 + x ----------
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
         const int t = it * p.to + r;
-        const bool valid = r < p.to && t < p.t;
-        const int b = ti & 1;
-        float* rptr[4];
-        uint32_t rok = 0;
+        if (!(r < p.to && t < p.t)) continue;
+        const long long o = ((long long)bb * p.t + t) * p.c + 2 * (lane & 3);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int src = i * 8 + (lane >> 2);
-          const long long orow = (long long)bb * p.t + __shfl_sync(0xffffffffu, t, src);
-          rptr[i] = p.y + orow * p.c + cq * 4;
-          rok |= (uint32_t)__shfl_sync(0xffffffffu, (int)valid, src) << i;
-        }
-        mbar_wait(&a2_full[b], (uint32_t)((ti >> 1) & 1));
-        tc_fence_after();
-        const uint32_t t_lane = tmem_acc + (uint32_t)(2 + b) * acc_cols + ((uint32_t)(quarter * 32) << 16);
-        for (int n0 = 0; n0 < NT; n0 += 32) {
-          uint32_t rr[32];
-          tmem_ld32(t_lane + (uint32_t)n0, rr);
-          tmem_ld_wait();
-          float v[32];
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t t2[16];
-            tmem_ld16(t_lane + (uint32_t)(NT + n0 + 16 * hh), t2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[16 * hh + e] = __uint_as_float(rr[16 * hh + e]) + __uint_as_float(t2[e]);
-          }
-          if (n0 + 32 >= NT) {
-            tc_fence_before();
-            mbar_arrive(&a2_empty[b]);
-          }
-#pragma unroll
-          for (int e = 0; e < 32; e += 4) {
-            const float4 bv = *reinterpret_cast<const float4*>(s_bias + NT + n0 + e);
-            v[e] += bv.x; v[e + 1] += bv.y; v[e + 2] += bv.z; v[e + 3] += bv.w;
-          }
-          rb_store32<true>(stg, lane, v, rptr, rok, n0, 32, side_delta, p.x);
+        for (int i = 0; i < kWgmmaMaxRegs / 4; ++i) {
+          if (i * 8 >= NT) continue;
+          const int col = i * 8 + 2 * (lane & 3);
+          const float2 xv = __ldg(reinterpret_cast<const float2*>(p.x + o + i * 8));
+          *reinterpret_cast<float2*>(p.y + o + i * 8) =
+              make_float2(acc[4 * i + 2 * hh] + s_bias[NT + col] + xv.x, acc[4 * i + 2 * hh + 1] + s_bias[NT + col + 1] + xv.y);
         }
       }
     }
-  }
-
-  if (warp == 4 && lane == 0 && p.resident && ntile_cta > 0)
-    for (int s = 0; s < 2 * p.nsteps; ++s) mbar_wait(&w_full[s], 0);   // no bulk copy may outlive the CTA
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, tmem_cols);
   }
 }
 
@@ -538,7 +402,7 @@ struct RbPlan {
   size_t smem;
 };
 
-static int rb_fixed_smem(int nslots) { return (16 + 2 * nslots) * 8 + 16 + 8 * 2048 + 2 * 64 * 4; }
+static int rb_fixed_smem(int nslots) { return (6 + 2 * nslots) * 8 + 2 * 64 * 4; }
 
 // KANTTS_B200_RB_TMA=0 keeps the producer warps on global loads (A/B testing); default: TMA-staged x tiles when they fit
 static bool rb_want_tma() {
@@ -604,7 +468,7 @@ int resblock_pack(const KtResblockDesc* d, const float* w, void* img, cudaStream
   KT_REQUIRE(pl.ok && w && img, "resblock_pack: shape not supported by the fused kernel");
   if (pl.p.pair) {
     const int total = pl.p.nsteps * 32 * 64;
-    rb_pack_pair_kernel<<<std::min((total + 255) / 256, 148 * 4), 256, 0, st>>>(w, d->kernel, pl.p.nsteps,
+    rb_pack_pair_kernel<<<std::min((total + 255) / 256, 132 * 4), 256, 0, st>>>(w, d->kernel, pl.p.nsteps,
                                                                                 reinterpret_cast<__nv_bfloat16*>(img));
     KT_CHECK_CUDA(cudaGetLastError());
     return KT_OK;
@@ -642,9 +506,9 @@ int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, cons
     KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
     cfg.store(true, std::memory_order_release);
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = std::min(p.total_tiles, sms > 0 ? sms : 148);
+  const int grid = std::min(p.total_tiles, sms > 0 ? sms : 132);
   resblock_tc_kernel<<<grid, kRbThreads, pl.smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;

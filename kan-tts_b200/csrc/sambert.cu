@@ -5,7 +5,7 @@
 // conv kernels (conv_tc.cu / conv_ffma.cu) as kernel-size-1/3 convolutions over the same (B, L, C) rows.
 //
 // Everything here is exact fp32 on CUDA cores: with d_head = 16 (sambert_24k.yaml) one attention head is a
-// K=16 contraction -- a single tcgen05 k-step -- and the kernels are bound by the probability-matrix
+// K=16 contraction -- a single wgmma k-step -- and the kernels are bound by the probability-matrix
 // traffic (B*H*Lq*Lk*4 bytes written in forward, read twice in backward), not by math.
 #include <atomic>
 

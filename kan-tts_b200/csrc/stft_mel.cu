@@ -10,6 +10,8 @@
 // optional saved spectrum and the 80 mel values ever touch HBM.
 // The backward runs the same FFT with conjugated twiddles on Z_k = d re_k + i d im_k and
 // overlap-adds win[n] * Re(ifft) into d wav.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace kt {
@@ -96,7 +98,7 @@ __global__ void __launch_bounds__(256) stft_mel_bwd_kernel(MelParams p, const fl
                                                            const float* __restrict__ spec,
                                                            const float* __restrict__ window,
                                                            const float* __restrict__ melmat,
-                                                           float* __restrict__ dwav) {
+                                                           float* __restrict__ frame_grad) {
   extern __shared__ __align__(16) float smem_f[];
   float2* s = reinterpret_cast<float2*>(smem_f);          // [n_fft]
   float* amp = smem_f + 2 * p.n_fft;                      // [nb]
@@ -143,11 +145,29 @@ __global__ void __launch_bounds__(256) stft_mel_bwd_kernel(MelParams p, const fl
     s[bitrev(i, p.logn)] = zk;
   }
   fft_inplace(s, n, p.logn, +1.f);
-  float* dw = dwav + (long long)b * p.t;
-  const int start = f * p.hop - n / 2;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const int si = src_index(start + i, p.t, p.pad_mode);
-    if (si >= 0) atomicAdd(dw + si, s[i].x * __ldg(window + i));
+  // windowed frame gradient; ola_gather_kernel overlap-adds the frames (a fixed summation order, unlike float atomics)
+  float* fg = frame_grad + fb * n;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) fg[i] = s[i].x * __ldg(window + i);
+}
+
+// dwav[b][t] = sum over the padded positions q that src_index maps to t (q = t, its left and right reflections), and over
+// the frames f covering q (ascending), of frame_grad[b][f][q - f * hop + n / 2]
+__global__ void ola_gather_kernel(const MelParams p, const float* __restrict__ frame_grad, float* __restrict__ dwav) {
+  const int n = p.n_fft, half = n / 2;
+  const long long total = (long long)p.batch * p.t;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int b = (int)(idx / p.t), t = (int)(idx - (long long)b * p.t);
+    const int cand[3] = {t, -t, 2 * (p.t - 1) - t};
+    float acc = 0.f;
+    for (int c = 0; c < 3; ++c) {
+      const int q = cand[c];
+      if ((c == 1 && q == cand[0]) || (c == 2 && (q == cand[0] || q == cand[1]))) continue;
+      if (src_index(q, p.t, p.pad_mode) != t) continue;
+      // frames f with 0 <= q - f * hop + half < n
+      const int f_lo = max(0, fdiv(q + half - n, p.hop) + 1), f_hi = min(p.frames - 1, fdiv(q + half, p.hop));
+      for (int f = f_lo; f <= f_hi; ++f) acc += __ldg(frame_grad + ((long long)b * p.frames + f) * n + (q - f * p.hop + half));
+    }
+    dwav[idx] = acc;
   }
 }
 
@@ -187,13 +207,18 @@ int stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, const
   int rc = fill(p, d);
   if (rc) return rc;
   KT_REQUIRE(spec && window && dwav && (dmel || damp) && (!dmel || melmat), "stft_mel_bwd: null argument");
-  KT_CHECK_CUDA(cudaMemsetAsync(dwav, 0, (size_t)p.batch * p.t * sizeof(float), st));
   const size_t smem = (2 * (size_t)p.n_fft + p.n_fft / 2 + 1 + p.n_mels) * sizeof(float);
   static bool cfg = false;
   if (!cfg) { KT_CHECK_CUDA(cudaFuncSetAttribute(stft_mel_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); cfg = true; }
-  stft_mel_bwd_kernel<<<p.batch * p.frames, 256, smem, st>>>(p, dmel, damp, spec, window, melmat, dwav);
+  float* frame_grad = nullptr;
+  rc = scratch_alloc(&frame_grad, (long long)p.batch * p.frames * p.n_fft, st);
+  if (rc) return rc;
+  stft_mel_bwd_kernel<<<p.batch * p.frames, 256, smem, st>>>(p, dmel, damp, spec, window, melmat, frame_grad);
   KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
+  const long long total = (long long)p.batch * p.t;
+  ola_gather_kernel<<<(int)std::min<long long>((total + 255) / 256, 132LL * 16), 256, 0, st>>>(p, frame_grad, dwav);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return scratch_free(frame_grad, st);
 }
 
 }  // namespace kt

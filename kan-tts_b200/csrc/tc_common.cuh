@@ -1,12 +1,12 @@
-// sm_100a primitives used by the tcgen05 kernels: mbarrier, bulk async copy (TMA engine, UBLKCP),
-// tcgen05 alloc / mma / commit / ld, UMMA shared-memory + instruction descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor" tables (the same fields
-// CUTLASS's cute/arch/mma_sm100_desc.hpp encodes); everything here is hand-written inline PTX.
+// sm_90a primitives used by the tensor-core kernels: mbarrier, bulk async copy (TMA engine, UBLKCP),
+// wgmma shared-memory descriptors and warpgroup synchronisation.  Bit layouts follow the PTX ISA "matrix descriptor"
+// table of wgmma; everything here is hand-written inline PTX.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace kt {
 namespace tc {
@@ -14,8 +14,7 @@ namespace tc {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // One elected lane of a fully converged warp (elect.sync).  Unlike `if (lane == 0)`, the compiler knows that exactly
-// one thread runs the guarded region, so tcgen05.mma / bulk-copy operands move to uniform registers directly; with
-// the lane test every tcgen05.mma was wrapped in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall loop.
+// one thread runs the guarded region, so bulk-copy operands move to uniform registers directly.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -53,7 +52,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // Bounded wait: a protocol bug must surface as a trap (launch error), never as a hung GPU.  The try_wait carries CUTLASS's
 // suspend-time hint (the hardware parks the warp instead of polling) and the loop must NOT be unrolled: nvcc unrolled it
 // 64x at every call site (~2 KB of SASS each, ~15 sites per kernel), and four concurrently running warp roles were
-// thrashing the instruction cache (stall_no_inst, profiles/r02_notes.md).
+// thrashing the instruction cache (stall_no_inst).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
   uint32_t ok = 0;
@@ -71,7 +70,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   __trap();
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (tcgen05.mma / bulk copies)
+// generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- bulk async copy global -> shared, completion on an mbarrier (TMA engine; SASS UBLKCP) ----
@@ -82,158 +81,40 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                : "memory");
 }
 
-// ---- tensor memory ----
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate; issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, with the two shared-memory descriptors given by their LOW words only.  Every operand of this library is a
-// SWIZZLE_128B image with 128-byte rows: the high word (SBO = 1024 B -> 0x40, descriptor version 1 -> bit 14, layout
-// SWIZZLE_128B = 2 -> bits 29-31) is the constant 0x40004040; the low word is (address >> 4) | (LBO >> 4) << 16.
-constexpr uint32_t kDescHiSw128 = 0x40004040u;
-__device__ __forceinline__ void umma_bf16_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-// All MMAs of one (tap, K chunk) step in ONE asm block: `ks` (1..4) K = 16 slices, the descriptor low words advance by 2 (32 bytes)
-// per slice.  Issued one by one through umma_bf16_lo the compiler kept the step's loop-invariant operands in vector registers
-// and re-converted them for every slice (5 R2UR + ~9 UMOV / UIADD3 per pair of UTCHMMA, ~115 cycles per MMA measured on the
-// 32-channel layers whose MMAs take 16-32 cycles); here they enter the uniform datapath once per step.
-// fuse2 form, per slice: [a_hi*b_hi | a_hi*b_lo] (idesc2, N = 2*NT, accumulate flag `acc` on the first slice), a_lo*b_hi (idesc).
-__device__ __forceinline__ void umma_step_fuse2(uint32_t d_tmem, uint32_t a_hi, uint32_t img16, uint32_t b_hi, uint32_t idesc2,
-                                                uint32_t idesc, uint32_t acc, uint32_t ks) {
-  asm volatile(
-      "{\n\t.reg .pred pacc, pt, q1, q2, q3;\n\t.reg .b32 a1, a2, b1;\n\t.reg .b64 da, db, dc;\n\t"
-      "setp.ne.b32 pacc, %6, 0;\n\tsetp.eq.u32 pt, %7, %7;\n\t"
-      "setp.gt.u32 q1, %7, 1;\n\tsetp.gt.u32 q2, %7, 2;\n\tsetp.gt.u32 q3, %7, 3;\n\t"
-      "add.u32 a2, %1, %2;\n\t"
-      "mov.b64 da, {%1, %8};\n\tmov.b64 db, {%3, %8};\n\tmov.b64 dc, {a2, %8};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 2;\n\tadd.u32 b1, %3, 2;\n\tadd.u32 a2, a2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\t"
-      "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, pt;\n\t"
-      "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 4;\n\tadd.u32 b1, %3, 4;\n\tadd.u32 a2, a2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\t"
-      "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, pt;\n\t"
-      "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 6;\n\tadd.u32 b1, %3, 6;\n\tadd.u32 a2, a2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\t"
-      "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, pt;\n\t"
-      "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t}"
-      ::"r"(d_tmem), "r"(a_hi), "r"(img16), "r"(b_hi), "r"(idesc2), "r"(idesc), "r"(acc), "r"(ks), "r"(kDescHiSw128)
-      : "memory");
-}
-// plain form, per slice: a_lo*b_hi (accumulate flag `acc` on the first slice), a_hi*b_lo (b_lo = b_hi + bplane16), a_hi*b_hi
-__device__ __forceinline__ void umma_step_x3(uint32_t d_tmem, uint32_t a_hi, uint32_t img16, uint32_t b_hi, uint32_t bplane16, uint32_t idesc,
-                                             uint32_t acc, uint32_t ks) {
-  asm volatile(
-      "{\n\t.reg .pred pacc, pt, q1, q2, q3;\n\t.reg .b32 a1, a2, b1, b2;\n\t.reg .b64 da, db, dc, dd;\n\t"
-      "setp.ne.b32 pacc, %6, 0;\n\tsetp.eq.u32 pt, %7, %7;\n\t"
-      "setp.gt.u32 q1, %7, 1;\n\tsetp.gt.u32 q2, %7, 2;\n\tsetp.gt.u32 q3, %7, 3;\n\t"
-      "add.u32 a2, %1, %2;\n\tadd.u32 b2, %3, %4;\n\t"
-      "mov.b64 da, {%1, %8};\n\tmov.b64 db, {%3, %8};\n\tmov.b64 dc, {a2, %8};\n\tmov.b64 dd, {b2, %8};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, dd, %5, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 2;\n\tadd.u32 b1, %3, 2;\n\tadd.u32 a2, a2, 2;\n\tadd.u32 b2, b2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\tmov.b64 dd, {b2, %8};\n\t"
-      "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], da, dd, %5, pt;\n\t"
-      "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 4;\n\tadd.u32 b1, %3, 4;\n\tadd.u32 a2, a2, 2;\n\tadd.u32 b2, b2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\tmov.b64 dd, {b2, %8};\n\t"
-      "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], da, dd, %5, pt;\n\t"
-      "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-      "add.u32 a1, %1, 6;\n\tadd.u32 b1, %3, 6;\n\tadd.u32 a2, a2, 2;\n\tadd.u32 b2, b2, 2;\n\t"
-      "mov.b64 da, {a1, %8};\n\tmov.b64 db, {b1, %8};\n\tmov.b64 dc, {a2, %8};\n\tmov.b64 dd, {b2, %8};\n\t"
-      "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], dc, db, %5, pt;\n\t"
-      "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], da, dd, %5, pt;\n\t"
-      "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t}"
-      ::"r"(d_tmem), "r"(a_hi), "r"(img16), "r"(b_hi), "r"(bplane16), "r"(idesc), "r"(acc), "r"(ks), "r"(kDescHiSw128)
-      : "memory");
-}
-// all previously issued MMAs of this thread complete -> arrive on the mbarrier (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors ----
-// Shared-memory matrix descriptor, 128-byte swizzle, rows of 128 bytes (64 bf16) spaced 128 bytes:
+// ---- warpgroup MMA (wgmma) ----
+// Every operand of this library is a SWIZZLE_128B image with 128-byte rows (64 bf16).  Shared-memory matrix descriptor:
 //   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4     bits [46,48) version = 1 (sm_100)
-//   bits [49,52) matrix base offset          bits [61,64) layout: 2 = SWIZZLE_128B
-// K-major operand  (rows = M/N index, K contiguous):  SBO = 1024 (8 rows), LBO unused (1)
-// MN-major operand (rows = K index, M/N contiguous):  SBO = 1024 (8 K-rows), LBO = stride between
-//                                                     64-element M/N groups
-// The swizzle XOR acts on absolute shared-memory address bits [4,7) ^= [7,10) (measured on B200), so a
-// start address advanced by whole 128-byte rows reads a ROW-SHIFTED view of the same staged image --
-// this is what makes a conv tap a descriptor offset.  `use_base_offset` (matrix base offset =
-// (start >> 7) & 7) must stay false for that; it is kept only to document the failed variant.
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t start_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                    bool use_base_offset) {
-  uint64_t d = 0;
-  d |= (uint64_t)((start_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  if (use_base_offset) d |= (uint64_t)((start_addr >> 7) & 7) << 49;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
+//   bits [32,46) stride byte offset >> 4     bits [49,52) matrix base offset (0)     bits [62,64) layout: 1 = SWIZZLE_128B
+// K-major operand  (rows = M/N index, K contiguous):  SBO = 1024 (8 rows), LBO unused
+// MN-major operand (rows = K index, M/N contiguous):  SBO = 1024 (8 K-rows), LBO = stride between 64-element M/N groups
+// The high word (SBO = 1024 -> 0x40, SWIZZLE_128B -> bit 30) is a constant; the kernels keep the low word
+// (address >> 4) | (LBO >> 4) << 16 and move through an image with 32-bit adds: +2 per K = 16 slice of a K-major operand,
+// +128 per 16 rows of an MN-major one, +8 per 128-byte row.  The swizzle XOR acts on absolute shared-memory address bits
+// [4,7) ^= [7,10), so a start address advanced by whole rows reads a ROW-SHIFTED view of the same staged image -- this is
+// what makes a conv tap a descriptor offset (all image bases are 1024-byte aligned, base offset 0).
+constexpr uint32_t kDescHiSw128 = 0x40000040u;
+__device__ __forceinline__ uint64_t desc_lo(uint32_t lo) { return ((uint64_t)kDescHiSw128 << 32) | lo; }
 
-// Instruction descriptor, kind::f16: fp32 accumulate (bits[4,6)=1), A/B = bf16 (bits[7,10)=1, [10,13)=1),
-// a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major), N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[kWgmmaMaxRegs]) {
+#pragma unroll
+  for (int i = 0; i < kWgmmaMaxRegs; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// accumulator element i of thread `lane` of warp `w` (0..3) of the warpgroup: row 16 w + lane / 4 + 8 ((i >> 1) & 1),
+// column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
+
+// split-bf16 ("bf16x3") product of one K = 16 slice: lo * hi + hi * lo + hi * hi into the accumulators
+// (a_hi / b_hi: descriptor low words of the hi planes, a_pl / b_pl: plane distances in 16-byte units)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_x3(int n, float (&d)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t a_pl, uint32_t b_hi, uint32_t b_pl,
+                                         uint32_t scale_d) {
+  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi + a_pl), desc_lo(b_hi), scale_d);
+  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi), desc_lo(b_hi + b_pl), 1u);
+  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi), desc_lo(b_hi), 1u);
 }
 
 // byte offset of 16-byte chunk `q` (0..7) of row `r` inside a 1024-byte-aligned SWIZZLE_128B image
@@ -259,7 +140,7 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo
 // Stage `rows` time steps x 64 channels of a channels-last fp32 tensor into a hi / lo bf16
 // SWIZZLE_128B image pair.  128 threads: thread -> (row = tid/8 + 16*i, 16-byte chunk q = tid%8).
 // Loads are issued in batches of NB rows per thread BEFORE any conversion so that each thread keeps
-// 2*NB (4*NB with an aux tensor) 16-byte loads in flight: with one 192-thread CTA per SM the
+// 2*NB (4*NB with an aux tensor) 16-byte loads in flight: with one CTA per SM the
 // staging loop is otherwise pure DRAM/L2 latency.
 //
 // RowMap: image row r -> source row of the channels-last tensor.  The rows of a tile are the
@@ -295,7 +176,7 @@ struct RowMap {
 // 32 bytes, x2 with an aux tensor) back to back with no dependent instruction in between; phase 2
 // converts and stores.  The two phases are separate fully-unrolled loops without early exits: with one
 // CTA per SM the staging loop is pure DRAM/L2 latency, and a fused load->convert->store loop measured
-// ~1 load in flight per thread (profiles/r01_notes.md).
+// ~1 load in flight per thread.
 template <int NB, bool VEC, bool AUX, bool SIMPLE = false>
 __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                                 const float* aux_base, int c_total, int ch0, int nv, const RowMap& rm,
@@ -379,7 +260,7 @@ __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, con
   if (nv <= 0) {
     // pure padding chunk (thin layers with fill_all): zeros, no loads.  Without this exit such lanes fell into the scalar
     // (non-vector) staging path, and every warp executed BOTH paths: ncu counted ~265 instructions per 8-element chunk for
-    // the 32-channel weight gradients against ~80 for full chunks (profiles/r02_notes.md)
+    // the 32-channel weight gradients against ~80 for full chunks
     const uint4 z = make_uint4(0u, 0u, 0u, 0u);
     for (int r = r_begin + (tid >> 3); r < rows; r += 16) {
       const uint32_t o = tc::sw128_offset((uint32_t)r, (uint32_t)q);

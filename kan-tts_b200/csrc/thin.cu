@@ -26,6 +26,9 @@ struct ThinParams {
   const float* y;    // forward output (act' of the fused output LeakyReLU)
   float* out;        // forward: y;  weight gradient: dw [k][c_out]
   float* dbias;
+  // weight gradient: CTA b writes its partial sums to part + b * (k + 1) * c_out ([k][c_out] dw, then [c_out] dbias),
+  // summed in CTA order afterwards (deterministic, unlike float atomics)
+  float* part;
   int batch, nsub, t_in, t_out, c_out, k, stride, dil, pad, act;
   float slope;
 };
@@ -76,7 +79,7 @@ __global__ void __launch_bounds__(256) thin_cin1_fwd_kernel(const ThinParams p) 
 // dW[j][co] = sum_rows x[row -> tap j] * dpre[row][co],  dbias[co] = sum_rows dpre[row][co],  dpre = dy * act'(y).
 // thread = (channel c = tid % C_out, row slot = tid / C_out); a CTA walks a contiguous row range, a warp reads
 // 128 contiguous bytes of dy per row; the k input samples of a row are warp-uniform loads.  Per-CTA partial sums
-// are reduced in shared memory and added to dw / dbias with (k+1)*C_out atomics per CTA.
+// are reduced in shared memory and written to the CTA's slot of p.part ((k+1)*C_out floats).
 __global__ void __launch_bounds__(256) thin_cin1_wgrad_kernel(const ThinParams p, long long rows_per_cta) {
   __shared__ float red[256 * (kThinMaxK + 1)];
   const int c = threadIdx.x % p.c_out, slot = threadIdx.x / p.c_out, nslots = 256 / p.c_out;
@@ -125,8 +128,7 @@ __global__ void __launch_bounds__(256) thin_cin1_wgrad_kernel(const ThinParams p
     const int jj = j < p.k ? j : kThinMaxK;
     float s = 0.f;
     for (int q = 0; q < nslots; ++q) s += red[jj * 256 + q * p.c_out + cc];
-    if (j < p.k) atomicAdd(p.out + j * p.c_out + cc, s);
-    else if (p.dbias) atomicAdd(p.dbias + cc, s);
+    p.part[(long long)blockIdx.x * (p.k + 1) * p.c_out + i] = s;
   }
 }
 
@@ -182,7 +184,7 @@ __global__ void __launch_bounds__(256) thin_c128_fwd_kernel(const ThinParams p) 
 
 template <int K>
 __global__ void __launch_bounds__(256) thin_c128_wgrad_kernel(const ThinParams p) {
-  __shared__ float4 red[4][K + 1][32];   // two rounds: warps 4-7 -> 0-3, then 0-3 -> the atomics
+  __shared__ float4 red[4][K + 1][32];   // two rounds: warps 4-7 -> 0-3, then 0-3 -> the CTA's slot of p.part
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = lane * 4;
   const int gwarp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), nwarps = (int)((gridDim.x * blockDim.x) >> 5);
   float4 acc[K + 1];
@@ -246,8 +248,7 @@ __global__ void __launch_bounds__(256) thin_c128_wgrad_kernel(const ThinParams p
     float s = 0.f;
 #pragma unroll
     for (int q = 0; q < 4; ++q) s += reinterpret_cast<const float*>(&red[q][j][0])[cc];
-    if (j < K) atomicAdd(p.out + j * 128 + cc, s);
-    else if (p.dbias) atomicAdd(p.dbias + cc, s);
+    p.part[(long long)blockIdx.x * (K + 1) * 128 + i] = s;
   }
 }
 
@@ -285,25 +286,33 @@ int thin_cin1_wgrad(const KtConv1dDesc* d, const float* x, const float* dy, cons
   p.batch = d->batch; p.nsub = d->nsub; p.t_in = d->t_in; p.t_out = d->t_out; p.c_out = d->c_out; p.k = d->kernel;
   p.stride = d->stride; p.dil = d->dilation; p.pad = d->pad_left; p.act = d->act_out; p.slope = d->act_out_slope;
   KT_REQUIRE((long long)d->batch * d->t_out * d->nsub < (1LL << 31), "thin_cin1_wgrad: tensor too large for 32-bit row indexing");
-  KT_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)d->kernel * d->c_out * sizeof(float), st));
-  if (dbias) KT_CHECK_CUDA(cudaMemsetAsync(dbias, 0, (size_t)d->c_out * sizeof(float), st));
-  if (thin_c128_ok(d)) {
+  const long long slot = (long long)(d->kernel + 1) * d->c_out;
+  const bool c128 = thin_c128_ok(d);
+  long long ctas, rows_per_cta = 0;
+  if (c128) {
     const long long tasks = (long long)d->batch * ((d->t_out + kThinRW - 1) / kThinRW);
-    const int blocks = (int)std::max<long long>(1, std::min<long long>((tasks + 7) / 8, 148LL));
-    if (d->kernel == 15) thin_c128_wgrad_kernel<15><<<blocks, 256, 0, st>>>(p);
-    else if (d->kernel == 5) thin_c128_wgrad_kernel<5><<<blocks, 256, 0, st>>>(p);
-    else thin_c128_wgrad_kernel<3><<<blocks, 256, 0, st>>>(p);
-    KT_CHECK_CUDA(cudaGetLastError());
-    return KT_OK;
+    ctas = std::max<long long>(1, std::min<long long>((tasks + 7) / 8, 132LL));
+  } else {
+    const long long rows = (long long)d->batch * d->t_out * d->nsub;
+    const int nslots = 256 / d->c_out;
+    ctas = std::min<long long>(132LL * 4, std::max<long long>(1, rows / (nslots * 32LL)));
+    rows_per_cta = (rows + ctas - 1) / ctas;
+    ctas = (rows + rows_per_cta - 1) / rows_per_cta;
   }
-  const long long rows = (long long)d->batch * d->t_out * d->nsub;
-  const int nslots = 256 / d->c_out;
-  long long ctas = std::min<long long>(148LL * 4, std::max<long long>(1, rows / (nslots * 32LL)));
-  const long long rows_per_cta = (rows + ctas - 1) / ctas;
-  ctas = (rows + rows_per_cta - 1) / rows_per_cta;
-  thin_cin1_wgrad_kernel<<<(int)ctas, 256, 0, st>>>(p, rows_per_cta);
+  int rc = scratch_alloc(&p.part, ctas * slot, st);
+  if (rc) return rc;
+  if (c128) {
+    if (d->kernel == 15) thin_c128_wgrad_kernel<15><<<(int)ctas, 256, 0, st>>>(p);
+    else if (d->kernel == 5) thin_c128_wgrad_kernel<5><<<(int)ctas, 256, 0, st>>>(p);
+    else thin_c128_wgrad_kernel<3><<<(int)ctas, 256, 0, st>>>(p);
+  } else {
+    thin_cin1_wgrad_kernel<<<(int)ctas, 256, 0, st>>>(p, rows_per_cta);
+  }
   KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
+  rc = split_sum(p.part, (long long)d->kernel * d->c_out, (int)ctas, slot, dw, false, st);
+  if (!rc && dbias) rc = split_sum(p.part + (long long)d->kernel * d->c_out, d->c_out, (int)ctas, slot, dbias, false, st);
+  if (rc) return rc;
+  return scratch_free(p.part, st);
 }
 
 }  // namespace kt

@@ -1,4 +1,4 @@
-// tcgen05 weight-gradient kernel (bf16x3 split precision, fp32 accumulation in TMEM).
+// wgmma weight-gradient kernel (bf16x3 split precision, fp32 accumulation in registers).
 //
 //   G[tap j][ca][cb] = sum_{batch, w, m}  fa(A[b][(m*step + ioff_j)/up, w][ca]) * fb(Bm[b][m, w][cb])
 //   conv layer      : A = act_in(x)  (ca = C_in),  Bm = dy * act_out'(y) (cb = C_out), step = stride
@@ -6,14 +6,14 @@
 //
 // The contraction runs over the flattened (time, sub-sequence) index, so both MMA operands are
 // "MN-major" views of the same kind of shared-memory image the forward kernel uses ([flattened rows]
-// [64 channels] bf16, SWIZZLE_128B): K = 16 consecutive rows per tcgen05.mma, M / N = channels
+// [64 channels] bf16, SWIZZLE_128B): K = 16 consecutive rows per wgmma, M / N = channels
 // (64-element groups, LBO apart).  A conv tap (q, rho) is again a pure descriptor row shift (q * nsub)
-// of the staged residue image rho.  Two ways to fill M = 128:
-//   mode 0 (ca % 128 == 0): two 64-channel images of one tap (LBO = image stride)
-//   mode 1 (ca == 64)     : ONE image, two taps of the same residue: LBO = (q_{n+1} - q_n) * nsub * 128 B
-// Each CTA owns (ca tile, cb tile, a group of <= U "units" of one residue class = U*NT TMEM columns
-// <= 512) for a slice of the (batch, flattened time) range (split-K); partial tiles go to a workspace
-// with plain 16-byte stores and a second kernel reduces over the splits (cheaper than ~10^7 atomics).
+// of the staged residue image rho.  Two ways to fill M = 128 (two warpgroups of M = 64):
+//   mode 0 (ca % 128 == 0): two 64-channel images of one tap
+//   mode 1 (ca == 64)     : ONE image, two taps of the same residue, (q_{n+1} - q_n) * nsub rows apart
+// Each CTA owns (ca tile, cb tile, a group of <= U "units" of one residue class = U*NT <= 128 accumulator
+// columns) for a slice of the (batch, flattened time) range (split-K); partial tiles go to a workspace
+// with plain stores and a second kernel reduces over the splits in order (deterministic, and cheaper than ~10^7 atomics).
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -28,11 +28,6 @@ namespace kt {
 using namespace tc;
 
 constexpr int kWgTK = 64;        // flattened rows per staged chunk
-// warps 0-3 / 10-13: producers of the even chunks (upper / lower half of every image's rows; 0-3 also run the epilogue);
-// 6-9 / 14-17: producers of the odd chunks; 4: TMEM alloc; 5: MMA issuer.  The kernel is bound by the ISSUE rate of the
-// fp32 -> split-bf16 staging (~80 instructions per 8 elements, ncu: issue slots 23-30 % busy with 8 producer warps), so the
-// producers are 16 warps: two groups per pipeline stage.
-constexpr int kWgThreads = 576;
 constexpr int kWgMaxUnits = 8;
 constexpr int kWgMaxGroups = 24;
 
@@ -50,7 +45,6 @@ struct WgTcParams {
   int nsplit, chunks_per_batch;
   int a_groups, b_groups;      // 64-channel images per stage on each side
   int rows_a;                  // A image rows (max over unit groups), multiple of 8
-  int tmem_cols;
   int ngroups;                 // unit groups (grid.y)
   int grp_rho[kWgMaxGroups], grp_qlo[kWgMaxGroups];
   int grp_first_unit[kWgMaxGroups + 1];
@@ -58,84 +52,111 @@ struct WgTcParams {
   int unit_ntaps[kMaxTaps];    // 1 or 2
   int tap_j[kMaxTaps];
   int tap_q[kMaxTaps];
-  // bias gradient as one more accumulator unit of unit group `bias_grp` (-1: none): D[m][n] += sum_rows 1 * B[row][n] with an
-  // all-ones A operand -- every accumulator row is the column sum of the (masked) output gradient over this CTA's rows, row 0
-  // goes to the split's slice of the workspace at `bias_off` and wgrad_reduce sums the splits like any other element
+  // bias gradient in the split-K workspace at `bias_off` (bias_grp >= 0) -- not produced by these kernels (bias_grp = -1): the
+  // bias gradient is the column-sum kernel's
   int bias_grp;
   long long bias_off, split_stride;
   float* bias_direct;   // nsplit == 1: the kernel writes dw / dbias itself (ws = dw, no reduce pass); else nullptr
 };
 
-// TMEM -> workspace partial tiles (warps 0-3 of either kernel; thread = accumulator row)
-__device__ __forceinline__ void wg_epilogue(const WgTcParams& p, uint64_t* tmem_full, uint32_t tmem_acc, int warp, int lane, int cb_tile,
-                                            int ca_tile, int cgrp, int u0, int nu, int split, bool has_bias) {
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int row = warp * 32 + lane;  // M index inside the unit
-    const uint32_t t_lane = tmem_acc + ((uint32_t)(warp * 32) << 16);
-    for (int u = 0; u < nu; ++u) {
+// Consumers: two warpgroups, warpgroup cw owns rows [64 cw, 64 cw + 64) of the M = 128 accumulator block of every unit (U =
+// 128 / NT units of NT columns: 64 fp32 registers per thread).  Mode 0: rows = channels [128 ca_tile + 64 cw, +64) -- the
+// second 64-channel image; mode 1: rows = channels of tap 2u + cw of the unit -- the image row-shifted by the tap distance.
+constexpr int kWgConsumerArrivals = 8;   // one per consumer warp
+
+// MMAs of one staged chunk for one unit (accumulators acc[OFF, OFF + NT / 2)): A (M = 64 channels x K rows) and B (K rows x
+// NT channels) are MN-major images, the hi / lo planes img16 apart, K = 16 rows = 128 descriptor units per slice
+template <int NT, int OFF>
+__device__ __forceinline__ void wg_unit_mma(float (&acc)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t img_a16, uint32_t b_hi, uint32_t img_b16,
+                                            int kslices) {
+  for (int ks = 0; ks < kslices; ++ks) {
+    const uint32_t ko = (uint32_t)ks * 128u;
+    wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko + img_a16), desc_lo(b_hi + ko), 1u);
+    wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko), desc_lo(b_hi + ko + img_b16), 1u);
+    wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko), desc_lo(b_hi + ko), 1u);
+  }
+}
+
+// all units of one staged chunk, then wait for the MMAs (the stage is released by the caller)
+template <int NT>
+__device__ __forceinline__ void wg_chunk_mma(float (&acc)[kWgmmaMaxRegs], uint32_t sbase16, uint32_t b_hi, uint32_t img_a16, uint32_t img_b16,
+                                             const uint32_t* s_shift, const uint32_t* s_half, int nu, int cw, int kslices) {
+  wgmma_fence();
+  wg_unit_mma<NT, 0>(acc, sbase16 + s_shift[0] + (cw ? s_half[0] : 0u), img_a16, b_hi, img_b16, kslices);
+  if constexpr (kWgmmaMaxN / NT > 1) {
+    if (nu > 1) wg_unit_mma<NT, NT / 2>(acc, sbase16 + s_shift[1] + (cw ? s_half[1] : 0u), img_a16, b_hi, img_b16, kslices);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+}
+
+// registers -> workspace partial tiles (or dw itself when there is one split)
+template <int NT>
+__device__ __forceinline__ void wg_store(const WgTcParams& p, const float (&acc)[kWgmmaMaxRegs], int cw, int wq, int lane, int cb_tile,
+                                         int ca_tile, int cgrp, int u0, int nu, int split) {
+  const bool vec = ((p.cb | p.cb_g0) & 1) == 0;
+#pragma unroll
+  for (int u = 0; u < kWgmmaMaxN / NT; ++u) {
+    if (u >= nu) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;   // M index inside the unit
       int tap_n, ca_idx;
       bool valid;
       if (p.mode == 0) { tap_n = p.unit_tap0[u0 + u]; ca_idx = ca_tile * 128 + row; valid = true; }
       else { tap_n = p.unit_tap0[u0 + u] + (row >> 6); ca_idx = row & 63; valid = (row >> 6) < p.unit_ntaps[u0 + u]; }
       valid = valid && ca_idx < p.ca_g;
-      const int col0 = cb_tile * p.NT;                                    // first column inside the (super-)group
+      if (!valid) continue;
+      const int col0 = cb_tile * NT;                                      // first column inside the (super-)group
       // columns [c_lo, c_hi) of this tile are stored, column n at obase + n
-      int c_lo = 0, c_hi = min(p.NT, p.cb_g - col0);
-      long long obase = 0;
-      if (valid) {
-        if (p.gt > 1) {   // block diagonal: row of conv group gl keeps only that group's cb_g0 columns
-          const int gl = ca_idx / p.ca_g0, ci_l = ca_idx - gl * p.ca_g0;
-          c_lo = gl * p.cb_g0; c_hi = c_lo + p.cb_g0;
-          obase = (long long)split * p.split_stride + (((long long)p.tap_j[tap_n]) * p.ca_g0 + ci_l) * p.cb +
-                  ((long long)cgrp * p.gt + gl) * p.cb_g0 - c_lo;
+      int c_lo = 0, c_hi = min(NT, p.cb_g - col0);
+      long long obase;
+      if (p.gt > 1) {   // block diagonal: row of conv group gl keeps only that group's cb_g0 columns
+        const int gl = ca_idx / p.ca_g0, ci_l = ca_idx - gl * p.ca_g0;
+        c_lo = gl * p.cb_g0; c_hi = c_lo + p.cb_g0;
+        obase = (long long)split * p.split_stride + (((long long)p.tap_j[tap_n]) * p.ca_g0 + ci_l) * p.cb +
+                ((long long)cgrp * p.gt + gl) * p.cb_g0 - c_lo;
+      } else {
+        obase = (long long)split * p.split_stride + (((long long)p.tap_j[tap_n]) * p.ca_g + ca_idx) * p.cb + (long long)cgrp * p.cb_g + col0;
+      }
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int n = i * 8 + 2 * (lane & 3);
+        const float v0 = acc[u * (NT / 2) + 4 * i + 2 * h], v1 = acc[u * (NT / 2) + 4 * i + 2 * h + 1];
+        const bool ok0 = n >= c_lo && n < c_hi, ok1 = n + 1 >= c_lo && n + 1 < c_hi;
+        if (vec && ok0 && ok1) {
+          *reinterpret_cast<float2*>(p.ws + obase + n) = make_float2(v0, v1);
         } else {
-          obase = (long long)split * p.split_stride + (((long long)p.tap_j[tap_n]) * p.ca_g + ca_idx) * p.cb + (long long)cgrp * p.cb_g + col0;
-        }
-      }
-      const bool vec = ((p.cb | p.cb_g0) & 3) == 0;
-      for (int n0 = 0; n0 < p.NT; n0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(t_lane + (uint32_t)(u * p.NT + n0), rr);
-        tmem_ld_wait();
-        if (valid) {
-          const int e0 = max(0, c_lo - n0), e1 = min(32, c_hi - n0);
-          if (vec) {   // (fully unrolled with predicates: rr[] must stay in registers)
-#pragma unroll
-            for (int e = 0; e < 32; e += 4)
-              if (e >= e0 && e < e1)
-                *reinterpret_cast<float4*>(p.ws + obase + n0 + e) =
-                    make_float4(__uint_as_float(rr[e]), __uint_as_float(rr[e + 1]), __uint_as_float(rr[e + 2]), __uint_as_float(rr[e + 3]));
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (e >= e0 && e < e1) p.ws[obase + n0 + e] = __uint_as_float(rr[e]);
-          }
+          if (ok0) p.ws[obase + n] = v0;
+          if (ok1) p.ws[obase + n + 1] = v1;
         }
       }
     }
-    if (has_bias && warp == 0) {   // accumulator unit `nu`: every row = column sums; row 0 (lane 0) stores them
-      const int col0 = cb_tile * p.NT;
-      const int ncol = min(p.NT, p.cb_g - col0);
-      float* dst = p.bias_direct ? p.bias_direct + (long long)cgrp * p.cb_g + col0
-                                 : p.ws + (long long)split * p.split_stride + p.bias_off + (long long)cgrp * p.cb_g + col0;
-      for (int n0 = 0; n0 < p.NT; n0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(tmem_acc + (uint32_t)(nu * p.NT + n0), rr);
-        tmem_ld_wait();
-        if (lane == 0) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e)
-            if (n0 + e < ncol) dst[n0 + e] = __uint_as_float(rr[e]);
-        }
-      }
-    }
+  }
 }
 
+// per unit of this CTA: A-side row shift and the offset of the second warpgroup's 64 rows, in 16-byte descriptor units
+__device__ __forceinline__ void wg_unit_table(const WgTcParams& p, int u0, int nu, int qlo, int img_a, uint32_t* s_shift, uint32_t* s_half) {
+  for (int u = threadIdx.x; u < nu; u += blockDim.x) {
+    const int n_a = p.unit_tap0[u0 + u];
+    uint32_t half;
+    if (p.mode == 0) half = 2u * (uint32_t)img_a;
+    // mode 1: second half of M = the next tap of the same residue (rows 64..127 are discarded when the unit has one tap)
+    else half = p.unit_ntaps[u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
+    s_shift[u] = ((uint32_t)((p.tap_q[n_a] - qlo) * p.nsub) * 128u) >> 4;
+    s_half[u] = half >> 4;
+  }
+}
+
+// warpgroups 0 / 3: producers of the even / odd chunks; warpgroups 1 / 2: consumers (MMAs + epilogue).  The kernel is bound
+// by the ISSUE rate of the fp32 -> split-bf16 staging (~80 instructions per 8 elements), so the producers are 8 warps.
+constexpr int kWgThreads = 512;
+
+template <int NT>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space --
-  //  with the cast it emitted GENERIC ld / st for every image / staging access of the producers and the epilogue)
+  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space)
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   const int img_a = p.rows_a * 128;            // one plane of one A image
   const int img_b = kWgTK * 128;               // one plane of one B image
@@ -144,10 +165,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * (size_t)stage_bytes);
   uint64_t* full = bars;        // [2] producers -> MMA
   uint64_t* empty = bars + 2;   // [2] MMA -> producers
-  uint64_t* tmem_full = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
-  uint32_t* s_unit = tmem_slot + 2;     // [kWgMaxUnits] per unit of this CTA: A-side row shift (16-byte units) | LBO field
-  uint8_t* ones_img = reinterpret_cast<uint8_t*>(bars) + 128;   // (kWgTK + 8) rows x 128 B of bf16 1.0 (only when bias_grp >= 0)
+  uint32_t* s_shift = reinterpret_cast<uint32_t*>(bars + 4);   // [kWgMaxUnits]
+  uint32_t* s_half = s_shift + kWgMaxUnits;                    // [kWgMaxUnits]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cb_tile = blockIdx.x % p.n_cb_tiles;
@@ -158,46 +177,22 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   const int nu = p.grp_first_unit[grp + 1] - u0;
   const int qlo = p.grp_qlo[grp];
   const int split = blockIdx.z;
-
-  const bool has_bias = p.bias_grp == (int)blockIdx.y && ca_tile == 0;
   const long long units = (long long)p.batch * p.chunks_per_batch;
   const long long c_begin = units * split / p.nsplit;
   const long long c_end = units * (split + 1) / p.nsplit;
 
   if (tid == 0) {
-    for (int s = 0; s < 2; ++s) { mbar_init(&full[s], 256); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(&full[s], 128); mbar_init(&empty[s], kWgConsumerArrivals); }
     mbar_fence_init();
     fence_proxy_async();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  if (has_bias) {   // uniform data: invariant under the 128-byte swizzle, any 16-byte-aligned start address works
-    for (int i = tid; i < (kWgTK + 8) * 128 / 16; i += kWgThreads) reinterpret_cast<uint4*>(ones_img)[i] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
-    fence_proxy_async();
-  }
-  if (tid >= 160 && tid < 160 + nu) {
-    const int u = tid - 160;
-    const int n_a = p.unit_tap0[u0 + u];
-    uint32_t lbo_a;
-    if (p.mode == 0) lbo_a = 2u * (uint32_t)img_a;
-    // mode 1: second half of M = the next tap of the same residue (rows 64..127 are discarded when the unit has one tap)
-    else lbo_a = p.unit_ntaps[u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
-    const uint32_t shift = (uint32_t)((p.tap_q[n_a] - qlo) * p.nsub) * 128u;
-    s_unit[u] = (shift >> 4) + ((lbo_a >> 4) << 16);
-  }
-  tc_fence_before();
+  wg_unit_table(p, u0, nu, qlo, img_a, s_shift, s_half);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
 
-  if (warp < 4 || warp >= 6) {
+  if (warp < 4 || warp >= 12) {
     // ===================== producers =====================
-    const int pg = (warp < 4 || (warp >= 10 && warp < 14)) ? 0 : 1;      // pipeline stage this group fills
-    const int half = warp >= 10 ? 1 : 0;                                   // which half of every image's rows
-    const int ptid = tid & 127;                                            // 0..127 inside the group (each value once)
-    const int a_split = ((p.rows_a / 2) + 15) & ~15, b_split = kWgTK / 2;  // row ranges of the two halves
-    const int a_r0 = half ? a_split : 0, a_r1 = half ? p.rows_a : min(a_split, p.rows_a);
-    const int b_r0 = half ? b_split : 0, b_r1 = half ? kWgTK : b_split;
+    const int pg = warp < 4 ? 0 : 1;                                       // pipeline stage this group fills
+    const int ptid = tid & 127;
     int it = 0;
     for (long long c = c_begin; c < c_end; ++c, ++it) {
       const int s = it & 1;
@@ -214,7 +209,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
         uint8_t* hi = st + (size_t)g * 2 * img_a;
         const int c_lo = ca_tile * (p.mode == 0 ? 128 : 64) + g * 64;           // channel offset inside the group
         stage_rows<4, false, 2>(hi, hi + img_a, p.a, p.a.p, p.a.aux, p.ca, cgrp * p.ca_g + c_lo, min(64, p.ca_g - c_lo), true, ra,
-                                a_r1, ptid, a_r0);
+                                p.rows_a, ptid);
       }
       RowMap rb;  // base side: rows m (flattened with w), zero beyond M
       rb.base_row = (long long)bb * p.t_b * p.nsub;
@@ -222,68 +217,31 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       uint8_t* bst = st + (size_t)p.a_groups * 2 * img_a;
       for (int g = 0; g < p.b_groups; ++g) {
         uint8_t* hi = bst + (size_t)g * 2 * img_b;
-        const int c_lo = cb_tile * p.NT + g * 64;
+        const int c_lo = cb_tile * NT + g * 64;
         stage_rows<2, false, 2>(hi, hi + img_b, p.b, p.b.p, p.b.aux, p.cb, cgrp * p.cb_g + c_lo, min(64, p.cb_g - c_lo), true, rb,
-                                b_r1, ptid, b_r0);
+                                kWgTK, ptid);
       }
       fence_proxy_async();
       mbar_arrive(&full[s]);
     }
-
-    // ===================== epilogue (warps 0-3): TMEM -> workspace partial tiles =====================
-    if (warp < 4) wg_epilogue(p, tmem_full, tmem_acc, warp, lane, cb_tile, ca_tile, cgrp, u0, nu, split, has_bias);
-    tc_fence_before();
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    // (descriptor low words + 32-bit adds only, see conv_tc.cu; tap shifts / LBO fields of the units come from a
-    //  shared-memory table filled at kernel start)
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(128, p.NT, 1, 1);
-      const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
-      const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
-      const uint32_t st16[2] = {smem_u32(stage0) >> 4, smem_u32(stage0 + stage_bytes) >> 4};
-      const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
-      const uint32_t ones16 = (smem_u32(ones_img) >> 4) | ((128u >> 4) << 16);   // second 64-channel half of M: one row further (all ones)
-      int it = 0;
-      for (long long c = c_begin; c < c_end; ++c, ++it) {
-        const int s = it & 1;
-        mbar_wait(&full[s], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t b_hi = (st16[s] + boff16) | lbo_b16;
-        uint32_t ua = s_unit[0];
-        for (int u = 0; u < nu; ++u) {
-          const uint32_t a_hi = st16[s] + ua;                 // ua = row shift (16-byte units) | LBO field
-          if (u + 1 < nu) ua = s_unit[u + 1];
-          const uint32_t d = tmem_acc + (uint32_t)(u * p.NT);
+  } else {
+    // ===================== consumers =====================
+    const int cw = (warp - 4) >> 2, wq = warp & 3;
+    const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
+    const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
+    const uint32_t st16[2] = {smem_u32(stage0) >> 4, smem_u32(stage0 + stage_bytes) >> 4};
+    const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
+    float acc[kWgmmaMaxRegs];
 #pragma unroll
-          for (int ks = 0; ks < kWgTK / 16; ++ks) {
-            const uint32_t ko = (uint32_t)ks * 128u;            // 16 rows x 128 bytes, in 16-byte units
-            const uint32_t acc = (it > 0 || ks > 0) ? 1u : 0u;
-            umma_bf16_lo(d, a_hi + img_a16 + ko, b_hi + ko, idesc, acc);
-            umma_bf16_lo(d, a_hi + ko, b_hi + img_b16 + ko, idesc, 1u);
-            umma_bf16_lo(d, a_hi + ko, b_hi + ko, idesc, 1u);
-          }
-        }
-        if (has_bias) {   // ones^T x (b_hi + b_lo): two MMAs per K slice into accumulator unit `nu`
-          const uint32_t d = tmem_acc + (uint32_t)(nu * p.NT);
-#pragma unroll
-          for (int ks = 0; ks < kWgTK / 16; ++ks) {
-            const uint32_t ko = (uint32_t)ks * 128u;
-            umma_bf16_lo(d, ones16 + ko, b_hi + ko, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-            umma_bf16_lo(d, ones16 + ko, b_hi + img_b16 + ko, idesc, 1u);
-          }
-        }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(tmem_full);
+    for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
+    int it = 0;
+    for (long long c = c_begin; c < c_end; ++c, ++it) {
+      const int s = it & 1;
+      mbar_wait(&full[s], (it >> 1) & 1);
+      wg_chunk_mma<NT>(acc, st16[s], (st16[s] + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, nu, cw, kWgTK / 16);
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-    __syncwarp();
-  }
-
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, (uint32_t)p.tmem_cols);
+    wg_store<NT>(p, acc, cw, wq, lane, cb_tile, ca_tile, cgrp, u0, nu, split);
   }
 }
 
@@ -294,11 +252,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
 // each operand ONCE as hi / lo bf16 planes ([plane][batch][time][sub-sequence][channel], the activation layout), and the
 // weight-gradient CTAs pull their tiles with cp.async.bulk.tensor (SWIZZLE_128B boxes of 64 channels x `nsub` x `tt`
 // time steps land as exactly the MN-major images the MMAs read; rows outside [0, T) are the TMA unit's zero fill), so the
-// main loop is one elected producer thread, one elected MMA thread and an `nstages`-deep mbarrier ring.
+// main loop is one elected producer thread, two consumer warpgroups and an `nstages`-deep mbarrier ring.
 // A chunk = `tt` base time steps x all sub-sequences = R rows, padded to Rp = ceil16(R) (K = 16 per MMA) with rows that
 // are zeroed once and never written again.  A strided conv reads one residue class of the input per unit group: each
 // residue rho has its own tensor map (base + rho rows, time stride = step), so no element strides are needed.
-constexpr int kWgTmaThreads = 192;   // warps 0-3 epilogue, 4 TMEM alloc + TMA producer, 5 MMA issuer
+constexpr int kWgTmaThreads = 288;   // warpgroups 0 / 1 consumers (MMAs + epilogue), warp 8 TMA producer
 constexpr int kWgTmaMaxStages = 4;
 
 struct WgTmaExtra {
@@ -340,6 +298,7 @@ __global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16* __res
   }
 }
 
+template <int NT>
 __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __grid_constant__ WgTcParams p, const __grid_constant__ WgTmaExtra x) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -350,10 +309,8 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)x.nstages * stage_bytes);
   uint64_t* full = bars;                        // [nstages] TMA -> MMA
   uint64_t* empty = bars + kWgTmaMaxStages;     // [nstages] MMA -> TMA
-  uint64_t* tmem_full = bars + 2 * kWgTmaMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kWgTmaMaxStages + 1);
-  uint32_t* s_unit = tmem_slot + 2;             // [kWgMaxUnits]
-  uint8_t* ones_img = reinterpret_cast<uint8_t*>(bars) + 128;   // (Rp + 8) rows x 128 B of bf16 1.0 (only when bias_grp >= 0)
+  uint32_t* s_shift = reinterpret_cast<uint32_t*>(bars + 2 * kWgTmaMaxStages);   // [kWgMaxUnits]
+  uint32_t* s_half = s_shift + kWgMaxUnits;                                     // [kWgMaxUnits]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cb_tile = blockIdx.x % p.n_cb_tiles;
@@ -364,17 +321,14 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   const int nu = p.grp_first_unit[grp + 1] - u0;
   const int qlo = p.grp_qlo[grp];
   const int split = blockIdx.z;
-  const bool has_bias = p.bias_grp == (int)blockIdx.y && ca_tile == 0;
   const long long units = (long long)p.batch * x.chunks_per_batch;
   const long long c_begin = units * split / p.nsplit;
   const long long c_end = units * (split + 1) / p.nsplit;
 
   if (tid == 0) {
-    for (int s = 0; s < x.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < x.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kWgConsumerArrivals); }
     mbar_fence_init();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   {  // padding rows of every image (never written by the TMA boxes): zero, so that a partial last K slice contributes nothing
     const int a_box_rows = x.a_box_t * p.nsub;
     const int n_img = 2 * (p.a_groups + p.b_groups);
@@ -386,30 +340,17 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
         for (int o = r0 * 128 + tid * 16; o < r1 * 128; o += kWgTmaThreads * 16) *reinterpret_cast<uint4*>(img + o) = make_uint4(0u, 0u, 0u, 0u);
       }
   }
-  if (has_bias)
-    for (int i = tid; i < (x.Rp + 8) * 128 / 16; i += kWgTmaThreads) reinterpret_cast<uint4*>(ones_img)[i] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
-  if (tid >= 160 && tid < 160 + nu) {
-    const int u = tid - 160;
-    const int n_a = p.unit_tap0[u0 + u];
-    uint32_t lbo_a;
-    if (p.mode == 0) lbo_a = 2u * (uint32_t)img_a;
-    else lbo_a = p.unit_ntaps[u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
-    const uint32_t shift = (uint32_t)((p.tap_q[n_a] - qlo) * p.nsub) * 128u;
-    s_unit[u] = (shift >> 4) + ((lbo_a >> 4) << 16);
-  }
+  wg_unit_table(p, u0, nu, qlo, img_a, s_shift, s_half);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       const uint32_t tx = 2u * (uint32_t)(p.a_groups * x.a_box_t * p.nsub + p.b_groups * x.R) * 128u;
       const CUtensorMap* ma = &x.map_a[p.grp_rho[grp]];
       const int ca0 = cgrp * p.ca_g + ca_tile * (p.mode == 0 ? 128 : 64);
-      const int cb0 = cgrp * p.cb_g + cb_tile * p.NT;
+      const int cb0 = cgrp * p.cb_g + cb_tile * NT;
       int it = 0;
       for (long long c = c_begin; c < c_end; ++c, ++it) {
         const int s = it % x.nstages;
@@ -426,65 +367,29 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
           for (int pl = 0; pl < 2; ++pl)
             tma_load_5d(bst + (size_t)(2 * g + pl) * img_b, &x.map_b, cb0 + g * 64, 0, m0, bb, pl, &full[s]);
       }
-    }
-    __syncwarp();
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(128, p.NT, 1, 1);
-      const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
-      const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
-      const uint32_t st0_16 = smem_u32(stage0) >> 4, stage16 = (uint32_t)stage_bytes >> 4;
-      const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
-      const uint32_t ones16 = (smem_u32(ones_img) >> 4) | ((128u >> 4) << 16);
-      const int kslices = x.Rp >> 4;
-      int it = 0;
-      for (long long c = c_begin; c < c_end; ++c, ++it) {
-        const int s = it % x.nstages;
-        mbar_wait(&full[s], (it / x.nstages) & 1);
-        tc_fence_after();
-        const uint32_t sbase = st0_16 + (uint32_t)s * stage16;
-        const uint32_t b_hi = (sbase + boff16) | lbo_b16;
-        uint32_t ua = s_unit[0];
-        for (int u = 0; u < nu; ++u) {
-          const uint32_t a_hi = sbase + ua;
-          if (u + 1 < nu) ua = s_unit[u + 1];
-          const uint32_t d = tmem_acc + (uint32_t)(u * p.NT);
-          // (fully unrolled with a uniform predicate per slice: the rolled loop re-materialised its loop-invariant descriptor
-          //  words every iteration -- 2 R2UR + 4 ULEA + 4 UMOV per 3 UTCHMMA, ~97 cycles per MMA measured on N = 64 tiles)
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            if (ks < kslices) {
-              const uint32_t ko = (uint32_t)ks * 128u;            // 16 rows x 128 bytes, in 16-byte units
-              const uint32_t acc = (it > 0 || ks > 0) ? 1u : 0u;
-              umma_bf16_lo(d, a_hi + img_a16 + ko, b_hi + ko, idesc, acc);
-              umma_bf16_lo(d, a_hi + ko, b_hi + img_b16 + ko, idesc, 1u);
-              umma_bf16_lo(d, a_hi + ko, b_hi + ko, idesc, 1u);
-            }
-          }
-        }
-        if (has_bias) {
-          const uint32_t d = tmem_acc + (uint32_t)(nu * p.NT);
-#pragma unroll 1
-          for (int ks = 0; ks < kslices; ++ks) {
-            const uint32_t ko = (uint32_t)ks * 128u;
-            umma_bf16_lo(d, ones16 + ko, b_hi + ko, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-            umma_bf16_lo(d, ones16 + ko, b_hi + img_b16 + ko, idesc, 1u);
-          }
-        }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(tmem_full);
+      // every issued box has landed before the CTA may exit: the consumers waited for all of them
     }
     __syncwarp();
   } else {
-    wg_epilogue(p, tmem_full, tmem_acc, warp, lane, cb_tile, ca_tile, cgrp, u0, nu, split, has_bias);
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, (uint32_t)p.tmem_cols);
+    // ===================== consumers =====================
+    const int cw = warp >> 2, wq = warp & 3;
+    const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
+    const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
+    const uint32_t st0_16 = smem_u32(stage0) >> 4, stage16 = (uint32_t)stage_bytes >> 4;
+    const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
+    const int kslices = x.Rp >> 4;
+    float acc[kWgmmaMaxRegs];
+#pragma unroll
+    for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
+    int it = 0;
+    for (long long c = c_begin; c < c_end; ++c, ++it) {
+      const int s = it % x.nstages;
+      mbar_wait(&full[s], (it / x.nstages) & 1);
+      const uint32_t sbase = st0_16 + (uint32_t)s * stage16;
+      wg_chunk_mma<NT>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, nu, cw, kslices);
+      if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    wg_store<NT>(p, acc, cw, wq, lane, cb_tile, ca_tile, cgrp, u0, nu, split);
   }
 }
 
@@ -573,6 +478,19 @@ struct WgPlan {
 
 int debug_flags();   // conv_tc.cu (kt_debug_set_flags): 256 skip the operand split, 512 skip the MMA kernel, 1024 skip the split-K reduce
 
+// SMs of the current device (132 without one: the host-logic tests plan for an H100)
+static int wg_sm_count() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) {
+      cudaGetLastError();
+      v = 132;
+    }
+    return v;
+  }();
+  return n;
+}
+
 static bool wg_want_tma() {
   static const bool on = [] { const char* e = std::getenv("KANTTS_B200_WG_TMA"); return !(e && e[0] == '0'); }();
   return on;
@@ -601,18 +519,15 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   // channels are zero-padded to 64-wide images: thin / grouped layers use the same kernel
   p.mode = p.ca_g <= 64 ? 1 : 0;
   // TMA variant (see wgrad_tma_kernel): plain convs whose box coordinates (multiples of the (super-)group widths) are 16-byte
-  // aligned.  Its tiles are N = 128 wide: a stage is then ~70 KB and the ring holds three -- the N = 256 tiles of the
-  // register-staged kernel leave room for two 100 KB stages only, and the loads of one chunk (~3 us of L2 latency +
-  // transfer) could not hide behind the 1.6 us of MMAs of the other (measured 260 cycles per N = 256 MMA against 77 per
-  // N = 128 MMA with three stages, call r2ab).
+  // aligned.  Tiles are at most N = 128 wide (the accumulators of all units of a CTA are 64 registers per consumer thread).
   const bool tma_ok = allow_tma && !tr && p.up == 1 && (ca % 8) == 0 && (cb % 8) == 0 && (p.ca_g % 8) == 0 && (p.cb_g % 8) == 0 &&
                       (plan_only || (wg_want_tma() && encode_tiled_fn() != nullptr));   // plan_only: host-logic tests without a driver
-  p.NT = std::min(tma_ok ? 128 : 256, (p.cb_g + 63) & ~63);
+  p.NT = std::min(kWgmmaMaxN, (p.cb_g + 63) & ~63);
   p.n_cb_tiles = ceil_div(p.cb_g, p.NT);
   p.n_ca_tiles = p.mode == 0 ? ceil_div(p.ca_g, 128) : 1;
   p.a_groups = p.mode == 0 ? 2 : 1;
   p.b_groups = p.NT / 64;
-  const int U = std::min(kWgMaxUnits, 512 / p.NT);
+  const int U = std::min(kWgMaxUnits, kWgmmaMaxN / p.NT);
   const int taps_per_unit = p.mode == 1 ? 2 : 1;
   // taps sorted by (residue, q)
   int ntap = 0, nunit = 0;
@@ -660,28 +575,18 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   const size_t stage = 2 * ((size_t)p.a_groups * p.rows_a * 128 + (size_t)p.b_groups * kWgTK * 128);
   pl.smem = 1024 + 2 * stage + 128;
   if (pl.smem > (size_t)kMaxDynSmem) return pl;   // (a smaller U would shrink the halo; not needed for the shipped shapes)
-  // bias gradient: one spare accumulator unit in some unit group (the LAST group with fewer than U units) + the ones image.
-  // Only for a plain conv (the bias belongs to the B side = output gradient); transposed convs keep the column-sum kernel.
-  p.bias_grp = -1;
-  if (!tr) {
-    for (int g = p.ngroups - 1; g >= 0; --g)
-      if (p.grp_first_unit[g + 1] - p.grp_first_unit[g] < U) { p.bias_grp = g; break; }
-    if (p.bias_grp >= 0 && pl.smem + (kWgTK + 8) * 128 > (size_t)kMaxDynSmem) p.bias_grp = -1;
-    if (p.bias_grp >= 0) pl.smem += (kWgTK + 8) * 128;
-  }
-  p.tmem_cols = 32;
-  while (p.tmem_cols < U * p.NT) p.tmem_cols <<= 1;
-  if (p.tmem_cols > 512) return pl;
+  p.bias_grp = -1;   // the bias gradient is the column-sum kernel's (conv1d_bwd_weight_tc)
   p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
   const long long units = (long long)p.batch * p.chunks_per_batch;
   const long long base = (long long)p.groups * p.n_ca_tiles * p.n_cb_tiles * p.ngroups;
-  // split-K factor: CTAs run one per SM in waves of ~148; minimise (waves x chunks per CTA) plus the cost of writing
+  const int sms = wg_sm_count();
+  // split-K factor: CTAs run one per SM in waves of one per SM; minimise (waves x chunks per CTA) plus the cost of writing
   // and re-reading one more partial copy of the gradient (in units of one chunk ~ 10 us; ~4 TB/s effective)
   const double out_chunks = (double)p.taps_total * p.ca_g0 * cb * 8.0 / 4e12 / 10e-6;
   long long nsplit = 1;
   double best = 1e30;
   for (long long ns = 1; ns <= std::min<long long>(units, 296); ++ns) {
-    const long long waves = (base * ns + 147) / 148;
+    const long long waves = (base * ns + sms - 1) / sms;
     const double cost = (double)waves * (double)((units + ns - 1) / ns) + (double)ns * out_chunks;
     if (cost < best - 1e-9) { best = cost; nsplit = ns; }
   }
@@ -736,7 +641,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
     long long ns_best = 1;
     double cbest = 1e30;
     for (long long ns = 1; ns <= std::min<long long>(units_t, 296); ++ns) {
-      const long long waves = (base * ns + 147) / 148;
+      const long long waves = (base * ns + sms - 1) / sms;
       const double cost = (double)waves * (double)((units_t + ns - 1) / ns) * chunk_us + (ns > 1 ? 5.0 + (double)ns * out_us : 0.0);
       if (cost < cbest - 1e-9) { cbest = cost; ns_best = ns; }
     }
@@ -774,7 +679,7 @@ int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t s
 int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw,
                          float* dbias, float* ws, long long ws_floats, cudaStream_t st) {
   WgPlan pl = make_plan(d);
-  KT_REQUIRE(pl.ok, "conv1d_bwd_weight_tc: layer not supported by the tcgen05 path");
+  KT_REQUIRE(pl.ok, "conv1d_bwd_weight_tc: layer not supported by the tensor-core path");
   KT_REQUIRE(ws && ws_floats >= pl.ws_floats, "conv1d_bwd_weight_tc: workspace too small (%lld < %lld floats)", ws_floats, pl.ws_floats);
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_weight: y required when act_out != NONE");
   WgTcParams& p = pl.p;
@@ -796,7 +701,7 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
     __nv_bfloat16* pa = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_a_off);
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
-    auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 148LL * 16)); };
+    auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 132LL * 16)); };
     if (!(debug_flags() & 256)) {
       const int ba = blocks_for(na / 8), bb = blocks_for(nb / 8);
       split_planes_kernel<<<ba + bb, 256, 0, st>>>(p.a, na / 8, pa, p.b, nb / 8, pb, ba);
@@ -822,30 +727,36 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
     }
     static std::atomic<bool> cfg_t{false};
     if (!cfg_t.load(std::memory_order_acquire)) {
-      KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+      KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+      KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
       cfg_t.store(true, std::memory_order_release);
     }
     dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
-    if (!(debug_flags() & 512)) wgrad_tma_kernel<<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
+    if (!(debug_flags() & 512)) {
+      if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
+      else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
+    }
     KT_CHECK_CUDA(cudaGetLastError());
   } else {
   static std::atomic<bool> cfg{false};
   if (!cfg.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
     cfg.store(true, std::memory_order_release);
   }
   dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
-  wgrad_tc_kernel<<<grid, kWgThreads, pl.smem, st>>>(p);
+  if (p.NT == 64) wgrad_tc_kernel<64><<<grid, kWgThreads, pl.smem, st>>>(p);
+  else wgrad_tc_kernel<128><<<grid, kWgThreads, pl.smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   }
   const long long n = (long long)p.taps_total * p.ca_g0 * p.cb;
-  const int blocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 255) / 256, 148LL * 8));
+  const int blocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 255) / 256, 132LL * 8));
   const bool fused_bias = dbias != nullptr && p.bias_grp >= 0;
   if (direct || (debug_flags() & 1024)) {
     // nothing to reduce (or ablation)
   } else if (p.nsplit >= 16) {
     const long long warps = n / 4 + d->c_out;
-    const int wblocks = (int)std::max<long long>(1, std::min<long long>((warps + 7) / 8, 148LL * 8));
+    const int wblocks = (int)std::max<long long>(1, std::min<long long>((warps + 7) / 8, 132LL * 8));
     wgrad_reduce_wide_kernel<<<wblocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride, fused_bias ? dbias : nullptr, p.bias_off, d->c_out);
   } else {
     wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride, fused_bias ? dbias : nullptr, p.bias_off, d->c_out);

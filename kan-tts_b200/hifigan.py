@@ -1,4 +1,4 @@
-"""B200-native HiFi-GAN modules with the reference's module API.
+"""H100-native HiFi-GAN modules with the reference's module API.
 
 Drop-in replacements for ``kantts.models.hifigan.hifigan.{Generator, MultiPeriodDiscriminator,
 MultiScaleDiscriminator}`` (KAN-TTS kantts/models/hifigan/hifigan.py:22-478, layers.py:15-226):
@@ -6,7 +6,7 @@ same class names, constructor kwargs (yaml ``params``), forward signatures / ret
 ``state_dict`` keys and shapes, ``remove_weight_norm()`` and ``nsf_enable``; parameters are plain
 leaf ``nn.Parameter``s so ``torch.optim.Adam`` / ``DistributedDataParallel`` work unchanged.
 
-Every tensor op of the forward and backward runs in libkantts_b200.so (hand-written sm_100a
+Every tensor op of the forward and backward runs in libkantts_b200.so (hand-written sm_90a
 kernels) through ``ops.py``; activations are channels-last rows internally and are converted only
 at the module boundary (feature maps are returned as zero-copy permuted views).
 The NSF branch (``nsf_params``) is module plumbing over the same kernels and has NOT run on a GPU yet (round 1 ran out
@@ -523,7 +523,7 @@ class MultiPeriodDiscriminator(nn.Module):
             self.discriminators += [PeriodDiscriminator(**params)]
 
     def forward(self, y):
-        # The period discriminators are independent and their late layers are too small to fill 148 SMs:
+        # The period discriminators are independent and their late layers are too small to fill 132 SMs:
         # run them on side streams (fork / join around the loop; autograd replays the same streams in
         # backward, and CUDA-graph capture records the branches as parallel graph paths).
         y_d_rs, fmap_rs = [], []
@@ -742,7 +742,7 @@ class MultiScaleDiscriminator(nn.Module):
         for i, d in enumerate(self.discriminators):
             # a spectral-normed scale stays on the calling stream: its parameters receive their gradients through autograd
             # (w / sigma is recomputed per forward), and with that chain on a side stream the gradient of the first layer's
-            # weight_orig was intermittently lost when the scale is used twice in one backward (profiles/r02_notes.md)
+            # weight_orig was intermittently lost when the scale is used twice in one backward
             side = par and not (_SPECTRAL_ON_MAIN and any(getattr(l[0], "norm", "") == "spectral" for l in d.convs))
             if side:
                 streams[i].wait_stream(cur)

@@ -1,4 +1,4 @@
-"""Patch the B200-native classes into an importable KAN-TTS checkout so that its unchanged
+"""Patch the H100-native classes into an importable KAN-TTS checkout so that its unchanged
 ``kantts/bin/train_hifigan.py`` / ``kantts.train.trainer.GAN_Trainer`` run on them
 (see INTEGRATION.md).  ``model_builder`` looks classes up by name in ``kantts.models``' globals
 (kantts/models/__init__.py:38,51) and ``criterion_builder`` in ``loss_dict`` (loss.py:512-544)."""

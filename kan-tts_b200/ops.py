@@ -154,7 +154,7 @@ class ConvSpec:
 
     def without_upsample(self):
         """The same conv over the already up-sampled rows (upsample = 1, no fused pre-activation): its data
-        gradient on the tcgen05 kernel + kt_upsample_grad_reduce replaces the FFMA data gradient of the
+        gradient on the tensor-core kernel + kt_upsample_grad_reduce replaces the FFMA data gradient of the
         nearest-upsampled conv."""
         s = self.__dict__.get("_noup")
         if s is None:
@@ -176,11 +176,11 @@ class PreparedWeight:
         self.key = None
         self.last_reuse = None   # (d, nt_fwd) of the latest pair_reuse forward (a second forward shape per step)
         self.last = None       # (d, nt_fwd, d_bwd, nt_bwd) of the latest forward: what prefetch() re-prepares
-        self.img = {}          # (dir, n_tile) -> packed split-bf16 tcgen05 weight tiles
+        self.img = {}          # (dir, n_tile) -> packed split-bf16 tensor-core weight tiles
         self.img_stale = set()
 
     def tc_image(self, spec, d, direction, n_tile):
-        """hi/lo bf16 SWIZZLE_128B weight tiles for the tcgen05 kernels (kt_weight_pack_tc).  The tiling
+        """hi/lo bf16 SWIZZLE_128B weight tiles for the tensor-core kernels (kt_weight_pack_tc).  The tiling
         (N tile, padding) can depend on the sequence length, hence the key on n_tile."""
         k = (direction, n_tile)
         img = self.img.get(k)
@@ -199,7 +199,7 @@ class PreparedWeight:
 
 
 def prefetch_weight(cache, spec, v, g):
-    """Re-prepare (weight norm + layouts + tcgen05 tiles) a layer's weights ahead of its next forward, for the
+    """Re-prepare (weight norm + layouts + tensor-core tiles) a layer's weights ahead of its next forward, for the
     shapes its latest forward used -- a no-op when nothing changed.  train.GanStep runs this for a whole model on
     side streams right after that model's optimizer step, off the critical path of the other model's forward."""
     if cache.last is None:
@@ -254,7 +254,7 @@ def prepare_weight(cache, spec, v, g):
           "kt_weight_prepare")
     _count()
     cache.key = key
-    cache.img_stale = set(cache.img)      # packed tcgen05 tiles are re-packed (in place) on next use
+    cache.img_stale = set(cache.img)      # packed tensor-core tiles are re-packed (in place) on next use
     return cache
 
 
@@ -356,7 +356,7 @@ def tc_launch_count():
 
 
 def set_force_ffma(flag):
-    """Route every conv through the exact-fp32 FFMA kernels (A/B testing of the tcgen05 path)."""
+    """Route every conv through the exact-fp32 FFMA kernels (A/B testing of the tensor-core path)."""
     global _FORCE_FFMA
     _FORCE_FFMA = bool(flag)
 
@@ -365,7 +365,7 @@ _WGRAD_TC = os.environ.get("KANTTS_B200_WGRAD_TC", "1") != "0"
 
 
 def _wgrad_tc_workspace(lib, spec, d):
-    """fp32 workspace floats for the tcgen05 weight-gradient kernel, 0 = use the FFMA kernel."""
+    """fp32 workspace floats for the tensor-core weight-gradient kernel, 0 = use the FFMA kernel."""
     if _FORCE_FFMA or not _WGRAD_TC or spec.path == KT_PATH_FFMA:
         return 0
     key = ("wg", d.batch, d.nsub, d.t_in)
@@ -385,7 +385,7 @@ def _tc_tile(lib, spec, d, direction):
         nt = lib.kt_conv1d_tc_plan(ctypes.byref(d), direction)
         spec._descs[key] = nt
     if nt == 0 and spec.path == KT_PATH_TC:
-        raise RuntimeError(f"kantts_b200: layer {spec} cannot run on the tcgen05 path")
+        raise RuntimeError(f"kantts_b200: layer {spec} cannot run on the tensor-core path")
     return nt
 
 
@@ -507,7 +507,7 @@ class ConvFn(torch.autograd.Function):
         nt_b = _tc_tile(lib, spec, db, 1) if x.requires_grad else 0
         ctx.d_up = None
         if x.requires_grad and nt_b == 0 and spec.upsample > 1 and spec.c_in % 4 == 0 and not spec.transposed:
-            # data gradient wrt the up-sampled rows on the tcgen05 kernel, folded back by kt_upsample_grad_reduce
+            # data gradient wrt the up-sampled rows on the tensor-core kernel, folded back by kt_upsample_grad_reduce
             s2 = spec.without_upsample()
             d2 = s2.desc(nb, nsub, t_in * spec.upsample)
             nt2 = _tc_tile(lib, s2, d2, 1) if d2.t_out == d.t_out else 0
@@ -571,7 +571,7 @@ class ConvFn(torch.autograd.Function):
             # `dy_full` is still being read -- by this layer's weight-gradient chain on its side stream and, when it is the
             # shared output of Mean3Fn.backward, by the other parallel resblocks on THEIR streams.  Returning the alias let
             # the engine overwrite it under those readers: parameter gradients of the generator were off by ~5 % with the
-            # (slow) exact-fp32 kernels and side streams on (profiles/r02_notes.md, scripts/diag_fullsize.py).
+            # (slow) exact-fp32 kernels and side streams on (scripts/diag_fullsize.py).
             dres = dy_full.clone()
         dbias, dv, dg = _weight_backward(spec, d, x_, dy, y_, v, g, ctx.params, ctx.norm, ctx.needs_input_grad[3],
                                          ctx.has_g and ctx.needs_input_grad[4], ctx.has_bias and ctx.needs_input_grad[2])
@@ -656,7 +656,7 @@ def resblock_desc(spec1, spec2, batch, t):
 
 
 def _rb_image(pw, rd):
-    """the fused kernel's weight image of one conv (kt_resblock_pack), cached beside the tcgen05 tile images"""
+    """the fused kernel's weight image of one conv (kt_resblock_pack), cached beside the tensor-core tile images"""
     k = ("rb", rd.channels, rd.kernel)
     img = pw.img.get(k)
     if img is None or k in pw.img_stale:
@@ -697,7 +697,7 @@ class ResblockFn(torch.autograd.Function):
             d1, d2 = spec1.desc(nb, 1, T), spec2.desc(nb, 1, T)
             ctx.nb, ctx.d1, ctx.d2, ctx.specs = nb, d1, d2, (spec1, spec2)
             nt1, nt2 = _tc_tile(lib, spec1, d1, 1), _tc_tile(lib, spec2, d2, 1)
-            assert nt1 and nt2, "fused resblock: the data gradients run on the tcgen05 kernels"
+            assert nt1 and nt2, "fused resblock: the data gradients run on the tensor-core kernels"
             ctx.img_bwd = (pw1.tc_image(spec1, d1, 1, nt1), pw2.tc_image(spec2, d2, 1, nt2))
             ctx.norms = (pw1.norm, pw2.norm)
             ctx.params = ((v1, g1, b1), (v2, g2, b2))

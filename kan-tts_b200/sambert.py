@@ -1,4 +1,4 @@
-"""B200-native SAM-BERT acoustic model with the reference's module API.
+"""H100-native SAM-BERT acoustic model with the reference's module API.
 
 Drop-in for ``kantts.models.sambert.kantts_sambert.KanTtsSAMBERT`` (KAN-TTS
 kantts/models/sambert/kantts_sambert.py:652-1044 and the blocks it is built from: sambert/__init__.py,
@@ -9,7 +9,7 @@ the same torch initialisers).
 
 Where the arithmetic runs:
   * every Linear / Conv1d (QKV and output projections, conv feed-forward, prenets, FSMN feed-forward,
-    pitch / energy embeddings) -> the conv kernels of libkantts_b200.so (tcgen05 split-bf16 or exact fp32 FFMA)
+    pitch / energy embeddings) -> the conv kernels of libkantts_b200.so (tensor-core split-bf16 or exact fp32 FFMA)
     through ops.ConvFn, on the model's native (B, L, C) rows, with bias / ReLU / residual fused;
   * LayerNorm, multi-head attention (both PNCA attentions, probabilities materialised like the reference),
     the FSMN memory block and the LengthRegulator expansion -> the kernels in csrc/sambert.cu;

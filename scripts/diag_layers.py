@@ -1,4 +1,4 @@
-"""Full-size per-layer parity sweep of the generator's layer shapes: tcgen05 (default) and FFMA (exact) paths vs the CPU layer
+"""Full-size per-layer parity sweep of the generator's layer shapes: tensor-core (default) and FFMA (exact) paths vs the CPU layer
 oracle -- y, dx, dv, dg, db (development aid for the full-size train-step parity test)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

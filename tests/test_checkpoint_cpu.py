@@ -1,11 +1,9 @@
 """Checkpoint format round trip (SURVEY.md 8f-4; kantts/train/trainer.py:591-674): a checkpoint written in the trainer's layout
-from the B200-native modules loads -- strict -- into fresh native modules AND (where a KAN-TTS checkout is importable: this
-container, not the GPU box) into the unmodified reference classes, and the other way round; optimizer / scheduler states
-of the reference's `torch.optim.Adam` / `MultiStepLR` restore onto the native parameters (same parameter order)."""
+from the native modules loads -- strict -- into fresh native modules; a checkpoint written by the unmodified reference classes
+(stored under tests/golden) loads into the native modules, and a native checkpoint has the reference's layout; optimizer /
+scheduler states of the reference's `torch.optim.Adam` / `MultiStepLR` restore onto the native parameters (same order)."""
 import os
-import sys
 
-import pytest
 import torch
 
 import kantts_b200 as K
@@ -23,11 +21,18 @@ MPD_CFG = dict(periods=[2, 3], discriminator_params=dict(in_channels=1, out_chan
                                                          nonlinear_activation_params={"negative_slope": 0.1}, use_spectral_norm=False))
 
 
-def _build(mod):
+# smaller still for the stored reference checkpoint (tests/golden/checkpoint_reference.pth, kept under 1 MB)
+TINY = (dict(G_CFG, channels=8, resblock_kernel_sizes=[3], resblock_dilations=[[1, 3]]),
+        dict(MSD_CFG, discriminator_params=dict(MSD_CFG["discriminator_params"], channels=4, max_downsample_channels=16)),
+        dict(MPD_CFG, discriminator_params=dict(MPD_CFG["discriminator_params"], channels=2, max_downsample_channels=16)))
+
+
+def _build(mod, cfgs=(G_CFG, MSD_CFG, MPD_CFG)):
     torch.manual_seed(3)
-    model = {"generator": mod.Generator(**G_CFG),
-             "discriminator": {"MultiScaleDiscriminator": mod.MultiScaleDiscriminator(**MSD_CFG),
-                               "MultiPeriodDiscriminator": mod.MultiPeriodDiscriminator(**MPD_CFG)}}
+    g_cfg, msd_cfg, mpd_cfg = cfgs
+    model = {"generator": mod.Generator(**g_cfg),
+             "discriminator": {"MultiScaleDiscriminator": mod.MultiScaleDiscriminator(**msd_cfg),
+                               "MultiPeriodDiscriminator": mod.MultiPeriodDiscriminator(**mpd_cfg)}}
     mk = lambda m: torch.optim.Adam(m.parameters(), lr=2e-4, betas=(0.5, 0.9))
     opt = {"generator": mk(model["generator"]), "discriminator": {k: mk(m) for k, m in model["discriminator"].items()}}
     sch = {"generator": torch.optim.lr_scheduler.MultiStepLR(opt["generator"], milestones=[10], gamma=0.5),
@@ -88,25 +93,32 @@ def test_native_checkpoint_round_trip(tmp_path):
     assert a.keys() == b.keys() and all(torch.equal(a[i]["exp_avg"], b[i]["exp_avg"]) for i in a)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/kantts"), reason="needs an importable KAN-TTS checkout (not present on the GPU box)")
+def _layout(sd):
+    return [(k, tuple(v.shape)) for k, v in sd.items()]
+
+
 def test_checkpoints_interchange_with_the_reference_classes(tmp_path):
-    from oracle import ref_shims
-    ref_shims.import_reference()
-    import kantts.models.hifigan.hifigan as R
-    model, opt, sch = _build(K)
+    """tests/golden/checkpoint_reference.pth was written by the unmodified reference classes (make_golden_checkpoint.py): it
+    loads strict into native modules / optimizers / schedulers, and a native checkpoint has exactly its layout."""
+    ref = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "checkpoint_reference.pth")
+    rsd = torch.load(ref, map_location="cpu")
+    m3, o3, s3 = _build(K, TINY)
+    assert _load(m3, o3, s3, ref) == 4            # reference checkpoint -> native trainer objects, strict
+    _same(rsd["model"]["generator"], m3["generator"].state_dict())
+    for k in m3["discriminator"]:
+        _same(rsd["model"]["discriminator"][k], m3["discriminator"][k].state_dict())
+    a, b = rsd["optimizer"]["generator"]["state"], o3["generator"].state_dict()["state"]
+    assert a.keys() == b.keys() and all(torch.equal(a[i]["exp_avg_sq"], b[i]["exp_avg_sq"]) for i in a)
+    model, opt, sch = _build(K, TINY)             # and the other way: a native checkpoint in the reference's layout
     _fake_train(model, opt)
     p1 = os.path.join(tmp_path, "native.pth")
     _save(model, opt, sch, 3, p1)
-    rm, ro, rs = _build(R)                       # reference classes, reference-side Adam / MultiStepLR
-    assert _load(rm, ro, rs, p1) == 3            # native checkpoint -> reference trainer objects, strict
-    _same(model["generator"].state_dict(), rm["generator"].state_dict())
-    for k in model["discriminator"]:
-        _same(model["discriminator"][k].state_dict(), rm["discriminator"][k].state_dict())
-    _fake_train(rm, ro)
-    p2 = os.path.join(tmp_path, "reference.pth")
-    _save(rm, ro, rs, 4, p2)
-    m3, o3, s3 = _build(K)
-    assert _load(m3, o3, s3, p2) == 4            # and back
-    _same(rm["generator"].state_dict(), m3["generator"].state_dict())
-    a, b = ro["generator"].state_dict()["state"], o3["generator"].state_dict()["state"]
-    assert a.keys() == b.keys() and all(torch.equal(a[i]["exp_avg_sq"], b[i]["exp_avg_sq"]) for i in a)
+    nsd = torch.load(p1, map_location="cpu")
+    assert _layout(nsd["model"]["generator"]) == _layout(rsd["model"]["generator"])
+    for k in rsd["model"]["discriminator"]:
+        assert _layout(nsd["model"]["discriminator"][k]) == _layout(rsd["model"]["discriminator"][k]), k
+    for n, r in [(nsd["optimizer"]["generator"], rsd["optimizer"]["generator"])] + \
+            [(nsd["optimizer"]["discriminator"][k], rsd["optimizer"]["discriminator"][k]) for k in rsd["optimizer"]["discriminator"]]:
+        assert [g["params"] for g in n["param_groups"]] == [g["params"] for g in r["param_groups"]]
+        assert all(n["state"][i]["exp_avg"].shape == r["state"][i]["exp_avg"].shape for i in r["state"])
+    assert nsd["scheduler"]["generator"].keys() == rsd["scheduler"]["generator"].keys()

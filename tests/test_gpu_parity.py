@@ -1,7 +1,7 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Every check goes through the C ABI
+"""GPU parity tests (``pytest -m gpu``).  Every check goes through the C ABI
 (ctypes -> libkantts_b200.so) and compares against the CPU oracle / golden vectors from the
 unmodified reference.  Tolerances (north_star): waveform RMS <= 1e-3, mel-L1 <= 1e-4; we hold the
-exact-fp32 (FFMA) kernels to ~1e-5 relative and the tcgen05 bf16x3 kernels to 1e-4 relative."""
+exact-fp32 (FFMA) kernels to ~1e-5 relative and the tensor-core (wgmma) bf16x3 kernels to 1e-4 relative."""
 import math
 import os
 import zlib
@@ -148,8 +148,8 @@ def test_conv_layer_ffma_vs_oracle(name):
 @pytest.mark.parametrize("name", list(CASES))
 def test_conv_layer_tcgen05_vs_oracle(name):
     """default dispatch: every layer shape (thin, grouped, strided, period, transposed, upsampled) runs on
-    the tcgen05 kernels (channels zero-padded to 64-wide K chunks / 16-wide N tiles)."""
-    assert _run_case(name, force_ffma=False), "expected the tcgen05 path to be taken"
+    the tensor-core kernels (channels zero-padded to 64-wide K chunks / 16-wide N tiles)."""
+    assert _run_case(name, force_ffma=False), "expected the tensor-core path to be taken"
 
 
 def _check_param_grads(m, refg, exact, tol=(5e-4, 1e-3, 1e-2)):
@@ -416,7 +416,7 @@ def test_full_size_properties():
     (y * r).sum().backward()
     x2 = torch.randn(B, T, device=DEV)
     assert abs(float((ops.DwtFn.apply(x2) * r).sum()) - float((x2 * x.grad).sum())) < 1e-2 * float(r.norm() * x2.norm()) * 1e-3 + 1e-2
-    # conv linearity + adjointness on the heaviest resblock shape (C=128, T=2048, k=11, d=5), tcgen05 path
+    # conv linearity + adjointness on the heaviest resblock shape (C=128, T=2048, k=11, d=5), tensor-core path
     spec = ops.ConvSpec(c_in=128, c_out=128, kernel=11, dilation=5, pad_left=50)
     v = torch.randn(128, 128, 11, device=DEV) * 0.05
     cache = ops.PreparedWeight()

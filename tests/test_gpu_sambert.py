@@ -244,7 +244,7 @@ def test_sambert_medium_matches_oracle(path):
     tensor-core path the forward carries ~1e-5 relative error, which flips the sign of the ~1e-5 fraction of the
     34 ReLU layers' pre-activations that lie that close to zero; each flipped unit changes the (discontinuous)
     gradient by O(1), i.e. a relative gradient difference of ~sqrt(1e-5) = 3e-3 that is not an arithmetic error
-    (measured: median 3.2e-3, max 9e-3; profiles/r01_notes.md).  That path is therefore held to a direction
+    (measured: median 3.2e-3, max 9e-3).  That path is therefore held to a direction
     test (cosine similarity of the whole gradient) plus a loose per-tensor bound."""
     import kantts_b200
     from kantts_b200 import sambert

@@ -1,4 +1,4 @@
-"""CPU: host-side planning logic of the C ABI (no kernel is launched): tcgen05 tile plans, packed-weight image sizes,
+"""CPU: host-side planning logic of the C ABI (no kernel is launched): tensor-core tile plans, packed-weight image sizes,
 split-K workspaces and the dispatch rules added for thin / grouped / waveform-input layers."""
 import ctypes
 
@@ -20,11 +20,11 @@ def _desc(B, t_in, nsub=1, **kw):
 
 
 def test_dense_layer_tiles(lib):
-    # 1024 -> 1024 k5 (period discriminator): N tiles of 256, 16 K chunks of 64
+    # 1024 -> 1024 k5 (period discriminator): N tiles of 128 (register accumulators), 16 K chunks of 64
     _, d = _desc(32, 34, nsub=3, c_in=1024, c_out=1024, kernel=5, pad_left=2, pad_right=2)
-    assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) == 256 and lib.kt_conv1d_tc_plan(ctypes.byref(d), 1) == 256
+    assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) == 128 and lib.kt_conv1d_tc_plan(ctypes.byref(d), 1) == 128
     # image = taps x K chunks x N tiles x (hi + lo) x NT x 64 bf16
-    assert lib.kt_conv1d_tc_image_bytes(ctypes.byref(d), 0) == 5 * 16 * 4 * 2 * 256 * 64 * 2
+    assert lib.kt_conv1d_tc_image_bytes(ctypes.byref(d), 0) == 5 * 16 * 8 * 2 * 128 * 64 * 2
     # generator resblock conv: one N tile of the layer's width
     _, d = _desc(16, 8192, c_in=32, c_out=32, kernel=7, pad_left=6)
     assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) == 32
@@ -47,7 +47,7 @@ def test_waveform_input_layers_leave_the_tensor_path(lib):
     _, d = _desc(32, 2731, nsub=3, **kw)
     assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) == 0            # forward: FIR kernel (thin.cu)
     assert lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d)) == 0
-    assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 1) > 0             # its data gradient stays on tcgen05
+    assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 1) > 0             # its data gradient stays on the tensor cores
     _, d = _desc(32, 2731, nsub=3, path=KT_PATH_TC, **kw)            # explicitly requested: still available
     assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) > 0 and lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d)) > 0
 
@@ -71,8 +71,18 @@ def test_split_k_workspace_is_whole_slices_of_the_gradient(lib):
         # one slice per split: the weight gradient + (when the bias gradient rides along as an all-ones MMA unit) the
         # bias gradient padded to a multiple of 4 floats
         per = spec.w_numel + ((spec.c_out + 3) & ~3)
-        assert ws > 0 and (ws % spec.w_numel == 0 or ws % per == 0)
-        nsplit = ws // per if ws % per == 0 else ws // spec.w_numel
+        out = (ctypes.c_int32 * 12)()
+        assert lib.kt_debug_wgrad_plan(ctypes.byref(d), out) == 0
+        if out[1] and ws % spec.w_numel and ws % per:
+            # TMA variant (a driver is present): the slices, padded to 64 floats, then the hi / lo bf16 operand planes of
+            # both operands (one float per element each, padded to 64 floats)
+            r64 = lambda n: (n + 63) & ~63
+            planes = r64(d.batch * d.t_in * d.nsub * d.c_in) + r64(d.batch * d.t_out * d.nsub * d.c_out)
+            assert ws - planes in (r64(out[7] * spec.w_numel), r64(out[7] * per)), (ws, planes, out[7])
+            nsplit = out[7]
+        else:
+            assert ws > 0 and (ws % spec.w_numel == 0 or ws % per == 0)
+            nsplit = ws // per if ws % per == 0 else ws // spec.w_numel
         assert 1 <= nsplit <= 296
 
 
