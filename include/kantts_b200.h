@@ -290,7 +290,9 @@ typedef struct KtResblockDesc {
   float slope;   /* LeakyReLU negative slope of both pre-activations */
   int32_t path;  /* KT_PATH_* (FFMA: the fused kernel is not available) */
 } KtResblockDesc;
-int kt_resblock_plan(const KtResblockDesc* d);                 /* 1: the fused kernel supports this shape */
+/* 1: the fused kernel supports this shape (no GPU needed).  The x tile arrives as one TMA box of
+ * ceil8(128 + (k-1)*dilation) rows (+ dilation when C = 32), at most 256: e.g. C = 32, k = 15, dilation 11 is not fused. */
+int kt_resblock_plan(const KtResblockDesc* d);
 int64_t kt_resblock_image_bytes(const KtResblockDesc* d);      /* per conv; 0 = unsupported */
 int kt_resblock_pack(const KtResblockDesc* d, const float* w_fwd, void* img, void* stream);
 int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
@@ -302,11 +304,6 @@ int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, c
 int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float* x, const float* h, const float* dy,
                     const void* wimg1_bwd, const void* wimg2_bwd, float* dh, float* dx, void* stream);
 
-/* Development aid, kept for ABI compatibility: the tensor-core kernels record no per-role timelines; any dev_buf is ignored. */
-int kt_debug_set_trace(void* dev_buf);
-/* Development aid: ablation switches for timing experiments of the weight-gradient chain: bit 8 no operand split, 9 no MMA
- * kernel, 10 no split-K reduce, 11 no weight-norm backward.  RESULTS ARE WRONG while non-zero. */
-int kt_debug_set_flags(int32_t flags);
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

@@ -91,8 +91,6 @@ PROTOTYPES = {
     "kt_fsmn_bwd": [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "kt_rows_gather_fwd": [_P, _P, _P, _I, _I, _I, _I, _P],
     "kt_rows_gather_bwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
-    "kt_debug_set_trace": [_P],
-    "kt_debug_set_flags": [_I],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_version": [],
     "kt_has_tc": [],

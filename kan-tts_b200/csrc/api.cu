@@ -22,8 +22,6 @@ int stft_mel_bwd(const KtMelDesc*, const float*, const float*, const float*, con
 long long wgrad_tc_workspace(const KtConv1dDesc*);
 int conv1d_bwd_weight_tc(const KtConv1dDesc*, const float*, const float*, const float*, float*, float*, float*, long long, cudaStream_t);
 int tc_plan(const KtConv1dDesc*, int);
-void debug_set_trace(long long*);
-void debug_set_flags(int);
 void debug_wgrad_plan(const KtConv1dDesc*, int*);
 long long tc_image_bytes(const KtConv1dDesc*, int);
 int tc_pack_layer(const KtConv1dDesc*, int, const float*, void*, cudaStream_t);
@@ -106,17 +104,9 @@ int kt_sinadd_bwd(const float* x, const float* dy, float* dx, int64_t n, void* s
 int kt_add3_scale(const float* a, const float* b, const float* c, float scale, float* y, int64_t n, void* stream) {
   return kt::add3_scale(a, b, c, scale, y, n, ST(stream));
 }
-int kt_debug_set_trace(void* dev_buf) {
-  kt::debug_set_trace(reinterpret_cast<long long*>(dev_buf));
-  return KT_OK;
-}
 int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out12) {
   KT_REQUIRE(d && out12, "kt_debug_wgrad_plan: null pointer");
   kt::debug_wgrad_plan(d, out12);
-  return KT_OK;
-}
-int kt_debug_set_flags(int32_t flags) {
-  kt::debug_set_flags(flags);
   return KT_OK;
 }
 int kt_upsample_grad_reduce(const float* dxu, const float* x, int32_t act_in, float act_in_slope, float* dx, int64_t rows,
@@ -141,7 +131,7 @@ int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float*
 }
 
 const char* kt_last_error(void) { return kt::last_error(); }
-int kt_version(void) { return 1; }
+int kt_version(void) { return 2; }
 int kt_has_tc(void) { return 1; }
 
 int kt_conv1d_tc_plan(const KtConv1dDesc* d, int32_t dir) {

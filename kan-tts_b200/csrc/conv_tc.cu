@@ -502,11 +502,6 @@ static int sm_count() {
   return n;
 }
 
-static int g_dbg = 0;   // development aid (kt_debug_set_flags): ablation switches of the weight-gradient chain, see wgrad_tc.cu
-void debug_set_flags(int f) { g_dbg = f; }
-int debug_flags() { return g_dbg; }
-void debug_set_trace(long long*) {}   // (the per-role timelines belonged to the previous tensor-core kernels)
-
 static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned by plan_launches
   const int a_stage = 2 * p.rows * 128;
   const int b_stage = 2 * p.NT * 128;

@@ -50,12 +50,11 @@ struct RbParams {
   int last_kslices;                 // K = 16 slices of the last step (pair with odd k: 2, else 4)
   int resident, nb;                 // weights: all tiles resident | ring of nb stages
   int tile_bytes;                   // one weight tile: [hi NT rows | lo NT rows] x 128 B
-  // TMA-staged input (north_star: "TMA-staged input tiles"): the fp32 x tile [rows_box][C] of every tile -- halo included,
-  // rows outside [0, T) zero-filled by the TMA unit itself -- is brought into shared memory with cp.async.bulk.tensor (one
-  // box of 32 channels x rows_box rows per 32 channels); the producer warps then only CONVERT shared -> shared
-  // (LeakyReLU, hi / lo split, swizzled image): no global-load latency, no address arithmetic, no bounds tests.
-  int tma;                          // 1: x tiles arrive by TMA (f stages = nx); 0: producer warps load them (LDG)
-  int rows_box;                     // rows of one TMA box (rows_x, + d1 for the paired layout)
+  // TMA-staged input: the fp32 x tile [rows_box][C] of every tile -- halo included, rows outside [0, T) zero-filled by the
+  // TMA unit itself -- is brought into shared memory with cp.async.bulk.tensor (one box of 32 channels x rows_box rows per
+  // 32 channels, nx landing stages); the producer warps then only CONVERT shared -> shared (LeakyReLU, hi / lo split,
+  // swizzled image): no global-load latency, no address arithmetic, no bounds tests.
+  int rows_box;                     // rows of one TMA box (rows_x, + d1 for the paired layout): at most 256
   int fstage_bytes;                 // one fp32 landing stage: (C / 32) boxes x rows_box x 128 B
   alignas(64) CUtensorMap tmx;      // 3-D map of x: (C, T, B), box (32, rows_box, 1), no swizzle, zero OOB fill
 };
@@ -75,43 +74,6 @@ __global__ void rb_pack_pair_kernel(const float* __restrict__ w, int k, int npai
     const uint32_t off = (sw128_offset((uint32_t)n, (uint32_t)(c >> 3)) >> 1) + (uint32_t)(c & 7);
     out[base + off] = hi;
     out[base + 32 * 64 + off] = lo;
-  }
-}
-
-// ---- paired staging (C = 32): image row r = [act(x[X0 + r]) (32 ch) | act(x[X0 + r + d]) (32 ch)] ------------------
-// 128 threads: thread -> (row = tid / 8 + 16 * i, chunk q = tid % 8); q < 4: channels 8q.. of source row r, q >= 4:
-// channels 8(q-4).. of source row r + d.  NB rows per thread are loaded back to back before any conversion.
-template <int NB>
-__device__ __forceinline__ void rb_stage_pair(uint8_t* img_hi, uint8_t* img_lo, const float* x, long long base_row, int x0,
-                                              int d, int t_lim, float slope, int rows, int tid) {
-  const int q = tid & 7;
-  const int ch = (q & 3) * 8, dsh = (q >> 2) * d;
-  for (int r0 = tid >> 3; r0 < rows; r0 += 16 * NB) {
-    float4 v[NB][2];
-    bool ok[NB];
-#pragma unroll
-    for (int i = 0; i < NB; ++i) {
-      const int r = r0 + 16 * i;
-      const int tv = x0 + r + dsh;
-      ok[i] = r < rows && tv >= 0 && tv < t_lim;
-      const float* src = ok[i] ? x + (base_row + tv) * 32 + ch : x;
-      v[i][0] = __ldg(reinterpret_cast<const float4*>(src));
-      v[i][1] = __ldg(reinterpret_cast<const float4*>(src) + 1);
-    }
-#pragma unroll
-    for (int i = 0; i < NB; ++i) {
-      const int r = r0 + 16 * i;
-      float e[8] = {v[i][0].x, v[i][0].y, v[i][0].z, v[i][0].w, v[i][1].x, v[i][1].y, v[i][1].z, v[i][1].w};
-#pragma unroll
-      for (int z = 0; z < 8; ++z) e[z] = ok[i] ? (e[z] > 0.f ? e[z] : e[z] * slope) : 0.f;
-      uint4 hi, lo;
-      split8(e, hi, lo);
-      if (r < rows) {
-        const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)q);
-        *reinterpret_cast<uint4*>(img_hi + o) = hi;
-        *reinterpret_cast<uint4*>(img_lo + o) = lo;
-      }
-    }
   }
 }
 
@@ -166,13 +128,13 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
   uint8_t* x_base = smem;                                            // nx stages x (hi | lo)
   uint8_t* h_base = x_base + (size_t)p.nx * 2 * ximg;                // (hi | lo)
   uint8_t* w_base = h_base + 2 * (size_t)himg;
-  uint8_t* f_base = w_base + (size_t)nslots * p.tile_bytes;          // fp32 landing stages of the TMA-staged x tiles (tma only)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(f_base + (p.tma ? (size_t)p.nx * p.fstage_bytes : 0));
+  uint8_t* f_base = w_base + (size_t)nslots * p.tile_bytes;          // nx fp32 landing stages of the TMA-staged x tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(f_base + (size_t)p.nx * p.fstage_bytes);
   uint64_t* x_full = bars;                 // [2]
   uint64_t* x_empty = x_full + 2;          // [2]
   uint64_t* w_full = x_empty + 2;          // [nslots]
   uint64_t* w_empty = w_full + nslots;     // [nslots] (ring only)
-  uint64_t* f_full = w_empty + nslots;     // [2] (tma only): the x tile has landed
+  uint64_t* f_full = w_empty + nslots;     // [2] the x tile has landed
   float* s_bias = reinterpret_cast<float*>(f_full + 2);              // b1 | b2 (2 * NT floats)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -196,55 +158,34 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
 
   if (warp < 4) {
     // ===================== producers: x images (fused input LeakyReLU) =====================
+    // the producers convert the landed fp32 tile; thread 0 issues the TMA loads, `nx` tiles ahead, as soon as the landing
+    // stage has been read
     const int ptid = tid;
-    if (p.tma) {
-      // TMA-staged: the producers convert the landed fp32 tile; thread 0 issues the loads, `nx` tiles ahead, as soon as the
-      // landing stage has been read
-      const int r0 = 0, r1 = p.rows_x;
-      const int nbox = p.c / 32, box_floats = p.rows_box * 32;
-      auto issue = [&](int ti) {
-        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-        const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
-        const int x0 = it * p.to - p.p2 - p.p1;
-        const int s = ti % p.nx;
-        mbar_arrive_expect_tx(&f_full[s], (uint32_t)p.fstage_bytes);
-        for (int bx = 0; bx < nbox; ++bx)
-          tma_load_box(f_base + (size_t)s * p.fstage_bytes + (size_t)bx * box_floats * 4, &p.tmx, bx * 32, x0, bb, &f_full[s]);
-      };
-      if (ptid == 0)
-        for (int ti = 0; ti < min(p.nx, ntile_cta); ++ti) issue(ti);
-      for (int ti = 0; ti < ntile_cta; ++ti) {
-        const int s = ti % p.nx, n = ti / p.nx;
-        mbar_wait(&x_empty[s], (uint32_t)((n & 1) ^ 1));
-        mbar_wait(&f_full[s], (uint32_t)(n & 1));
-        uint8_t* img_hi = x_base + (size_t)s * 2 * ximg;
-        const float* ft = reinterpret_cast<const float*>(f_base + (size_t)s * p.fstage_bytes);
-        if (p.pair) rb_convert_tile<true>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
-        else rb_convert_tile<false>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
-        fence_proxy_async();
-        mbar_arrive(&x_full[s]);
-        asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
-        if (ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx);
-      }
-    } else {
-    const Side sx{p.x, nullptr, SIDE_LRELU, p.slope};
-    for (int ti = 0; ti < ntile_cta; ++ti) {
+    const int r0 = 0, r1 = p.rows_x;
+    const int nbox = p.c / 32, box_floats = p.rows_box * 32;
+    auto issue = [&](int ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
       const int x0 = it * p.to - p.p2 - p.p1;
+      const int s = ti % p.nx;
+      mbar_arrive_expect_tx(&f_full[s], (uint32_t)p.fstage_bytes);
+      for (int bx = 0; bx < nbox; ++bx)
+        tma_load_box(f_base + (size_t)s * p.fstage_bytes + (size_t)bx * box_floats * 4, &p.tmx, bx * 32, x0, bb, &f_full[s]);
+    };
+    if (ptid == 0)
+      for (int ti = 0; ti < min(p.nx, ntile_cta); ++ti) issue(ti);
+    for (int ti = 0; ti < ntile_cta; ++ti) {
       const int s = ti % p.nx, n = ti / p.nx;
       mbar_wait(&x_empty[s], (uint32_t)((n & 1) ^ 1));
+      mbar_wait(&f_full[s], (uint32_t)(n & 1));
       uint8_t* img_hi = x_base + (size_t)s * 2 * ximg;
-      if (p.pair) {
-        rb_stage_pair<4>(img_hi, img_hi + ximg, p.x, (long long)bb * p.t, x0, p.d1, p.t, p.slope, p.rows_x, ptid);
-      } else {
-        RowMap rm;
-        rm.base_row = (long long)bb * p.t; rm.fv0 = x0; rm.nsub = 1; rm.step = 1; rm.rho = 0; rm.up = 1; rm.t_lim = p.t;
-        stage_rows<4, true, 4>(img_hi, img_hi + ximg, sx, p.x, nullptr, p.c, 0, p.c, false, rm, p.rows_x, ptid);
-      }
+      const float* ft = reinterpret_cast<const float*>(f_base + (size_t)s * p.fstage_bytes);
+      if (p.pair) rb_convert_tile<true>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+      else rb_convert_tile<false>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
       fence_proxy_async();
       mbar_arrive(&x_full[s]);
-    }
+      asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
+      if (ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx);
     }
   } else if (warp == 12) {
     // ===================== weight stream =====================
@@ -404,13 +345,8 @@ struct RbPlan {
 
 static int rb_fixed_smem(int nslots) { return (6 + 2 * nslots) * 8 + 2 * 64 * 4; }
 
-// KANTTS_B200_RB_TMA=0 keeps the producer warps on global loads (A/B testing); default: TMA-staged x tiles when they fit
-static bool rb_want_tma() {
-  static const bool v = [] { const char* e = getenv("KANTTS_B200_RB_TMA"); return !(e && e[0] == '0'); }();
-  return v;
-}
-
-static RbPlan rb_plan(const KtResblockDesc* d, bool tma = false) {
+// geometry only (no device query): kt_resblock_plan answers without a GPU
+static RbPlan rb_plan(const KtResblockDesc* d) {
   RbPlan pl{};
   RbParams& p = pl.p;
   if (d->path == KT_PATH_FFMA) return pl;
@@ -432,9 +368,8 @@ static RbPlan rb_plan(const KtResblockDesc* d, bool tma = false) {
   const int himg2 = 2 * p.rows_h * 128;
   p.rows_box = p.rows_x + (p.pair ? p.d1 : 0);
   p.fstage_bytes = (p.c / 32) * p.rows_box * 128;
-  if (tma && p.rows_box > 256) return pl;          // TMA box limit
-  p.tma = tma ? 1 : 0;
-  const int ximg2 = 2 * p.rows_x * 128 + (tma ? p.fstage_bytes : 0);   // one x stage: (hi | lo) image (+ its fp32 landing stage)
+  if (p.rows_box > 256) return pl;                 // TMA box limit (k >= 13 with dilation >= 9): the pair runs as two convs
+  const int ximg2 = 2 * p.rows_x * 128 + p.fstage_bytes;   // one x stage: (hi | lo) image + its fp32 landing stage
   const int cap = kMaxDynSmem - 1024;
   // preference: resident weights + 2 x stages; resident + 1; ring (>= 3 stages) + 2 x stages; ring + 1
   const int res_bytes = 2 * p.nsteps * p.tile_bytes;
@@ -483,24 +418,22 @@ int resblock_pack(const KtResblockDesc* d, const float* w, void* img, cudaStream
 
 int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2, const float* b2,
                  float* h, float* y, cudaStream_t st) {
-  RbPlan pl = rb_plan(d, rb_want_tma() && encode_tiled_fn() != nullptr);
-  if (!pl.ok) pl = rb_plan(d, false);
-  KT_REQUIRE(pl.ok, "resblock_fwd: shape not supported by the fused kernel (channels 32 / 64, odd kernel)");
+  RbPlan pl = rb_plan(d);
+  KT_REQUIRE(pl.ok, "resblock_fwd: shape not supported by the fused kernel (see kt_resblock_plan)");
   KT_REQUIRE(x && img1 && img2 && y, "resblock_fwd: null pointer");
+  KT_REQUIRE(encode_tiled_fn() != nullptr, "resblock_fwd: the driver provides no cuTensorMapEncodeTiled");
   RbParams& p = pl.p;
   p.x = x; p.y = y; p.h = h;
   p.w1 = reinterpret_cast<const __nv_bfloat16*>(img1); p.w2 = reinterpret_cast<const __nv_bfloat16*>(img2);
   p.b1 = b1; p.b2 = b2;
-  if (p.tma) {
-    const cuuint64_t gdim[3] = {(cuuint64_t)p.c, (cuuint64_t)p.t, (cuuint64_t)p.batch};
-    const cuuint64_t gstr[2] = {(cuuint64_t)p.c * 4, (cuuint64_t)p.t * p.c * 4};
-    const cuuint32_t box[3] = {32, (cuuint32_t)p.rows_box, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    const CUresult r = encode_tiled_fn()(&p.tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
-                                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    KT_REQUIRE(r == CUDA_SUCCESS, "resblock_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
-  }
+  const cuuint64_t gdim[3] = {(cuuint64_t)p.c, (cuuint64_t)p.t, (cuuint64_t)p.batch};
+  const cuuint64_t gstr[2] = {(cuuint64_t)p.c * 4, (cuuint64_t)p.t * p.c * 4};
+  const cuuint32_t box[3] = {32, (cuuint32_t)p.rows_box, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = encode_tiled_fn()(&p.tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
+                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  KT_REQUIRE(r == CUDA_SUCCESS, "resblock_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
   static std::atomic<bool> cfg{false};
   if (!cfg.load(std::memory_order_acquire)) {
     KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));

@@ -2,7 +2,6 @@
 // the reference parameter layout to the kernel layouts of conv_ffma.cu / conv_tc.cu.
 // Replaces torch._weight_norm + its backward (kantts/models/hifigan/layers.py:29,67,105,139).
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -275,8 +274,7 @@ __global__ void __launch_bounds__(256) weight_grad_tiled_kernel(const float* __r
 
 // tiled kernels for layers of >= 256 K elements with rows of >= 256 elements; -> (row blocks, b slices, b per slice)
 static bool weight_tiled_plan(int d0, int d1, int k, int& nblk, int& nsl, int& b_slice) {
-  static const bool off = [] { const char* e = std::getenv("KANTTS_B200_WEIGHT_TILED"); return e && e[0] == '0'; }();
-  if (off || (long long)d0 * d1 * k < 262144 || d1 * k < 256 || k > kWTile) return false;
+  if ((long long)d0 * d1 * k < 262144 || d1 * k < 256 || k > kWTile) return false;
   nblk = (d0 + kWA - 1) / kWA;
   nsl = std::max(1, std::min(std::max(1, d1 / 32), (296 + nblk - 1) / nblk));
   b_slice = ((d1 + nsl - 1) / nsl + 31) & ~31;
@@ -301,8 +299,6 @@ int weight_prepare(const float* v, const float* g, const float* inv_sigma, int m
   return KT_OK;
 }
 
-int debug_flags();   // 2048: skip the weight-norm backward kernel (ablation)
-
 int weight_grad(const float* dw, const float* v, const float* g, const float* norm, const float* inv_sigma,
                 int mode, int d0, int d1, int k, int transposed, int groups, float* dv, float* dg, int accumulate,
                 const float* dbias_src, float* dbias_dst, int nbias, cudaStream_t st) {
@@ -311,9 +307,7 @@ int weight_grad(const float* dw, const float* v, const float* g, const float* no
   WLayout L{d0, d1, k, transposed, groups};
   KT_REQUIRE((dbias_dst == nullptr) == (dbias_src == nullptr) && nbias >= 0, "weight_grad: dbias_src / dbias_dst must come together");
   int nblk, nsl, b_slice;
-  if (debug_flags() & 2048) {
-    // ablation: no weight-norm backward
-  } else if (weight_tiled_plan(d0, d1, k, nblk, nsl, b_slice)) {
+  if (weight_tiled_plan(d0, d1, k, nblk, nsl, b_slice)) {
     weight_grad_tiled_kernel<<<dim3(nblk, nsl), 256, 0, st>>>(dw, v, g, norm, inv_sigma, mode, L, make_forms(L), dv, dg, accumulate, dbias_src,
                                                                dbias_dst, nbias, b_slice);
   } else {

@@ -16,7 +16,6 @@
 // with plain stores and a second kernel reduces over the splits in order (deterministic, and cheaper than ~10^7 atomics).
 #include <algorithm>
 #include <atomic>
-#include <cstdlib>
 #include <vector>
 
 #include "common.cuh"
@@ -52,11 +51,7 @@ struct WgTcParams {
   int unit_ntaps[kMaxTaps];    // 1 or 2
   int tap_j[kMaxTaps];
   int tap_q[kMaxTaps];
-  // bias gradient in the split-K workspace at `bias_off` (bias_grp >= 0) -- not produced by these kernels (bias_grp = -1): the
-  // bias gradient is the column-sum kernel's
-  int bias_grp;
-  long long bias_off, split_stride;
-  float* bias_direct;   // nsplit == 1: the kernel writes dw / dbias itself (ws = dw, no reduce pass); else nullptr
+  long long split_stride;      // floats between two splits' partial gradients in ws
 };
 
 // Consumers: two warpgroups, warpgroup cw owns rows [64 cw, 64 cw + 64) of the M = 128 accumulator block of every unit (U =
@@ -393,17 +388,9 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   }
 }
 
-// sums the split-K partials: ws = [nsplit][stride] with stride >= n + nb; elements [0, n) -> dw, [bias_off, bias_off + nb) -> dbias
-__global__ void wgrad_reduce_kernel(const float* __restrict__ ws, float* __restrict__ dw, long long n, int nsplit, long long stride,
-                                    float* __restrict__ dbias, long long bias_off, int nb) {
+// sums the split-K partials: ws = [nsplit][stride] with stride >= n; elements [0, n) -> dw
+__global__ void wgrad_reduce_kernel(const float* __restrict__ ws, float* __restrict__ dw, long long n, int nsplit, long long stride) {
   const long long gtid = blockIdx.x * (long long)blockDim.x + threadIdx.x, gsz = (long long)gridDim.x * blockDim.x;
-  if (dbias) {
-    for (long long i = gtid; i < nb; i += gsz) {
-      float acc = 0.f;
-      for (int s = 0; s < nsplit; ++s) acc += ws[(long long)s * stride + bias_off + i];
-      dbias[i] = acc;
-    }
-  }
   if ((n & 3) || (stride & 3)) {  // thin layers: split slices are not 16-byte aligned
     for (long long i = gtid; i < n; i += gsz) {
       float acc = ws[i];
@@ -425,26 +412,20 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ ws, float* __restr
 
 // Many splits of a small gradient (thin layers: 147 splits of 7 K floats): one WARP per output float4, lanes stride over the splits
 // and combine with shuffles -- the kernel above walks the splits serially per thread (47 us for that shape with 7 CTAs).
-__global__ void wgrad_reduce_wide_kernel(const float* __restrict__ ws, float* __restrict__ dw, long long n, int nsplit, long long stride,
-                                         float* __restrict__ dbias, long long bias_off, int nb) {
+__global__ void wgrad_reduce_wide_kernel(const float* __restrict__ ws, float* __restrict__ dw, long long n, int nsplit, long long stride) {
   const int lane = threadIdx.x & 31;
   const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   const bool vec = ((n | stride) & 3) == 0;
   const long long items = vec ? n / 4 : n;
-  const long long items_b = dbias ? nb : 0;
-  for (long long i = warp; i < items + items_b; i += nwarps) {
+  for (long long i = warp; i < items; i += nwarps) {
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (i < items) {
-      if (vec) {
-        for (int s = lane; s < nsplit; s += 32) {
-          const float4 v = __ldg(reinterpret_cast<const float4*>(ws + (long long)s * stride) + i);
-          acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        }
-      } else {
-        for (int s = lane; s < nsplit; s += 32) acc.x += ws[(long long)s * stride + i];
+    if (vec) {
+      for (int s = lane; s < nsplit; s += 32) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(ws + (long long)s * stride) + i);
+        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
       }
     } else {
-      for (int s = lane; s < nsplit; s += 32) acc.x += ws[(long long)s * stride + bias_off + (i - items)];
+      for (int s = lane; s < nsplit; s += 32) acc.x += ws[(long long)s * stride + i];
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -452,8 +433,7 @@ __global__ void wgrad_reduce_wide_kernel(const float* __restrict__ ws, float* __
       acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o); acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
     }
     if (lane == 0) {
-      if (i >= items) dbias[i - items] = acc.x;
-      else if (vec) reinterpret_cast<float4*>(dw)[i] = acc;
+      if (vec) reinterpret_cast<float4*>(dw)[i] = acc;
       else dw[i] = acc.x;
     }
   }
@@ -476,8 +456,6 @@ struct WgPlan {
   int max_span_q;
 };
 
-int debug_flags();   // conv_tc.cu (kt_debug_set_flags): 256 skip the operand split, 512 skip the MMA kernel, 1024 skip the split-K reduce
-
 // SMs of the current device (132 without one: the host-logic tests plan for an H100)
 static int wg_sm_count() {
   static const int n = [] {
@@ -489,11 +467,6 @@ static int wg_sm_count() {
     return v;
   }();
   return n;
-}
-
-static bool wg_want_tma() {
-  static const bool on = [] { const char* e = std::getenv("KANTTS_B200_WG_TMA"); return !(e && e[0] == '0'); }();
-  return on;
 }
 
 static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_only = false) {
@@ -521,7 +494,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   // TMA variant (see wgrad_tma_kernel): plain convs whose box coordinates (multiples of the (super-)group widths) are 16-byte
   // aligned.  Tiles are at most N = 128 wide (the accumulators of all units of a CTA are 64 registers per consumer thread).
   const bool tma_ok = allow_tma && !tr && p.up == 1 && (ca % 8) == 0 && (cb % 8) == 0 && (p.ca_g % 8) == 0 && (p.cb_g % 8) == 0 &&
-                      (plan_only || (wg_want_tma() && encode_tiled_fn() != nullptr));   // plan_only: host-logic tests without a driver
+                      (plan_only || encode_tiled_fn() != nullptr);   // plan_only: host-logic tests without a driver
   p.NT = std::min(kWgmmaMaxN, (p.cb_g + 63) & ~63);
   p.n_cb_tiles = ceil_div(p.cb_g, p.NT);
   p.n_ca_tiles = p.mode == 0 ? ceil_div(p.ca_g, 128) : 1;
@@ -575,7 +548,6 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   const size_t stage = 2 * ((size_t)p.a_groups * p.rows_a * 128 + (size_t)p.b_groups * kWgTK * 128);
   pl.smem = 1024 + 2 * stage + 128;
   if (pl.smem > (size_t)kMaxDynSmem) return pl;   // (a smaller U would shrink the halo; not needed for the shipped shapes)
-  p.bias_grp = -1;   // the bias gradient is the column-sum kernel's (conv1d_bwd_weight_tc)
   p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
   const long long units = (long long)p.batch * p.chunks_per_batch;
   const long long base = (long long)p.groups * p.n_ca_tiles * p.n_cb_tiles * p.ngroups;
@@ -591,9 +563,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
     if (cost < best - 1e-9) { best = cost; nsplit = ns; }
   }
   p.nsplit = (int)nsplit;
-  const long long n_main = (long long)p.taps_total * p.ca_g0 * cb;
-  p.bias_off = n_main;
-  p.split_stride = n_main + (p.bias_grp >= 0 ? ((cb + 3) & ~3) : 0);
+  p.split_stride = (long long)p.taps_total * p.ca_g0 * cb;
   pl.ws_floats = nsplit * p.split_stride;
   pl.ok = true;
 
@@ -611,7 +581,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
       if (tt + pl.max_span_q > 256 || R > 256 || (tt > 1 && R * 5 < Rp * 4)) continue;
       const int rows_a_p = (Rp + pl.max_span_q * p.nsub + 7) & ~7;
       const size_t stage = 2 * ((size_t)p.a_groups * rows_a_p * 128 + (size_t)p.b_groups * Rp * 128);
-      const size_t fixed = 1024 + 128 + (p.bias_grp >= 0 ? (size_t)(Rp + 8) * 128 : 0);
+      const size_t fixed = 1024 + 128;
       if (fixed + stage > (size_t)kMaxDynSmem) continue;
       const int ns = (int)std::min<size_t>(kWgTmaMaxStages, ((size_t)kMaxDynSmem - fixed) / stage);
       if (ns > best_ns) { best_ns = ns; best_tt = tt; }
@@ -624,7 +594,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
     x.nstages = best_ns;
     {
       const size_t stage = 2 * ((size_t)p.a_groups * x.rows_a_p * 128 + (size_t)p.b_groups * x.Rp * 128);
-      pl.smem_tma = 1024 + 128 + (p.bias_grp >= 0 ? (size_t)(x.Rp + 8) * 128 : 0) + (size_t)best_ns * stage;
+      pl.smem_tma = 1024 + 128 + (size_t)best_ns * stage;
     }
     pl.tma = true;
     x.chunks_per_batch = ceil_div(p.M, x.tt);
@@ -690,22 +660,17 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
   else sdy.aux = nullptr;
   if (d->transposed) { p.a = sdy; p.b = sx; }
   else { p.a = sx; p.b = sdy; }
-  p.ws = ws;
-  p.bias_direct = nullptr;
   if (pl.tma) p.nsplit = pl.nsplit_tma;
-  if (dbias == nullptr) p.bias_grp = -1;
   const bool direct = p.nsplit == 1;      // one split: the partial tile IS the gradient
-  if (direct) { p.ws = dw; p.bias_direct = dbias; }
+  p.ws = direct ? dw : ws;
   if (pl.tma) {
     WgTmaExtra& x = pl.x;
     __nv_bfloat16* pa = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_a_off);
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
     auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 132LL * 16)); };
-    if (!(debug_flags() & 256)) {
-      const int ba = blocks_for(na / 8), bb = blocks_for(nb / 8);
-      split_planes_kernel<<<ba + bb, 256, 0, st>>>(p.a, na / 8, pa, p.b, nb / 8, pb, ba);
-    }
+    const int ba = blocks_for(na / 8), bb = blocks_for(nb / 8);
+    split_planes_kernel<<<ba + bb, 256, 0, st>>>(p.a, na / 8, pa, p.b, nb / 8, pb, ba);
     KT_CHECK_CUDA(cudaGetLastError());
     const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     {
@@ -732,10 +697,8 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
       cfg_t.store(true, std::memory_order_release);
     }
     dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
-    if (!(debug_flags() & 512)) {
-      if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
-      else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
-    }
+    if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
+    else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
     KT_CHECK_CUDA(cudaGetLastError());
   } else {
   static std::atomic<bool> cfg{false};
@@ -750,19 +713,15 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
   KT_CHECK_CUDA(cudaGetLastError());
   }
   const long long n = (long long)p.taps_total * p.ca_g0 * p.cb;
-  const int blocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 255) / 256, 132LL * 8));
-  const bool fused_bias = dbias != nullptr && p.bias_grp >= 0;
-  if (direct || (debug_flags() & 1024)) {
-    // nothing to reduce (or ablation)
-  } else if (p.nsplit >= 16) {
-    const long long warps = n / 4 + d->c_out;
-    const int wblocks = (int)std::max<long long>(1, std::min<long long>((warps + 7) / 8, 132LL * 8));
-    wgrad_reduce_wide_kernel<<<wblocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride, fused_bias ? dbias : nullptr, p.bias_off, d->c_out);
-  } else {
-    wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride, fused_bias ? dbias : nullptr, p.bias_off, d->c_out);
+  if (p.nsplit >= 16) {
+    const int wblocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 7) / 8, 132LL * 8));
+    wgrad_reduce_wide_kernel<<<wblocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride);
+  } else if (!direct) {
+    const int blocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 255) / 256, 132LL * 8));
+    wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(ws, dw, n, p.nsplit, p.split_stride);
   }
   KT_CHECK_CUDA(cudaGetLastError());
-  if (dbias && !fused_bias) {
+  if (dbias) {
     const long long rows = (long long)d->batch * d->nsub * d->t_out;
     int rc = colsum_bias(sdy, rows, d->c_out, dbias, st);
     if (rc) return rc;

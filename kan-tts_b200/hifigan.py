@@ -14,7 +14,6 @@ of GPU budget: tests/test_gpu_pipeline.py is opt-in).  Out of scope (SURVEY.md s
 """
 import copy
 import math
-import os
 
 import numpy as np
 import torch
@@ -29,8 +28,7 @@ from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO
 # --------------------------------------------------------------------------------------------
 
 
-_PARALLEL_STREAMS = os.environ.get("KANTTS_B200_STREAMS", "1") != "0"
-_SPECTRAL_ON_MAIN = os.environ.get("KANTTS_B200_SPECTRAL_ON_MAIN", "1") != "0"
+_PARALLEL_STREAMS = True   # False: every sub-discriminator on the calling stream (bench.py's per-launch event timings)
 _STREAMS = {}
 
 
@@ -257,7 +255,7 @@ class ResidualBlock(nn.Module):
         for c1, c2 in zip(self.convs1, self.convs2):
             n1, n2 = c1.conv1d, c2.conv1d
             rd = ops.resblock_desc(n1.spec, n2.spec, x.shape[0], x.shape[1]) \
-                if (ops._FUSE_RESBLOCK and not ops._FORCE_FFMA and x.dim() == 3 and n1.norm != "spectral" and n2.norm != "spectral") else None
+                if (not ops._FORCE_FFMA and x.dim() == 3 and n1.norm != "spectral" and n2.norm != "spectral") else None
             if rd is not None:
                 # thin stages (32 / 64 channels): the pair is ONE launch, the intermediate stays on the SM (kt_resblock_fwd)
                 v1, g1 = n1.effective_weight()
@@ -743,7 +741,7 @@ class MultiScaleDiscriminator(nn.Module):
             # a spectral-normed scale stays on the calling stream: its parameters receive their gradients through autograd
             # (w / sigma is recomputed per forward), and with that chain on a side stream the gradient of the first layer's
             # weight_orig was intermittently lost when the scale is used twice in one backward
-            side = par and not (_SPECTRAL_ON_MAIN and any(getattr(l[0], "norm", "") == "spectral" for l in d.convs))
+            side = par and not any(getattr(l[0], "norm", "") == "spectral" for l in d.convs)
             if side:
                 streams[i].wait_stream(cur)
                 with torch.cuda.stream(streams[i]):

@@ -6,7 +6,6 @@ Backward functions run on the autograd engine thread; every call passes the thre
 stream explicitly and the library keeps no global state.
 """
 import ctypes
-import os
 from dataclasses import dataclass, field
 
 import torch
@@ -304,7 +303,7 @@ def mark_direct_grad(param, flag=True):
     param._kt_direct = bool(flag)
 
 
-_WGRAD_ASYNC = os.environ.get("KANTTS_B200_WGRAD_STREAMS", "1") != "0"
+_WGRAD_ASYNC = True   # False: the chains stay on the calling stream (bench.py's per-launch event timings)
 _WG_POOL = {}
 _wg_next = 0
 
@@ -347,7 +346,7 @@ def _is_direct(p):
     return p is None or (getattr(p, "_kt_direct", False) and p.grad is not None and p.grad.is_contiguous())
 
 
-_FORCE_FFMA = os.environ.get("KANTTS_B200_PATH", "").lower() == "ffma"
+_FORCE_FFMA = False
 _tc_launches = 0
 
 
@@ -356,17 +355,14 @@ def tc_launch_count():
 
 
 def set_force_ffma(flag):
-    """Route every conv through the exact-fp32 FFMA kernels (A/B testing of the tensor-core path)."""
+    """Route every conv through the exact-fp32 FFMA kernels (the reference the tensor-core path is tested against)."""
     global _FORCE_FFMA
     _FORCE_FFMA = bool(flag)
 
 
-_WGRAD_TC = os.environ.get("KANTTS_B200_WGRAD_TC", "1") != "0"
-
-
 def _wgrad_tc_workspace(lib, spec, d):
     """fp32 workspace floats for the tensor-core weight-gradient kernel, 0 = use the FFMA kernel."""
-    if _FORCE_FFMA or not _WGRAD_TC or spec.path == KT_PATH_FFMA:
+    if _FORCE_FFMA or spec.path == KT_PATH_FFMA:
         return 0
     key = ("wg", d.batch, d.nsub, d.t_in)
     n = spec._descs.get(key)
@@ -571,7 +567,7 @@ class ConvFn(torch.autograd.Function):
             # `dy_full` is still being read -- by this layer's weight-gradient chain on its side stream and, when it is the
             # shared output of Mean3Fn.backward, by the other parallel resblocks on THEIR streams.  Returning the alias let
             # the engine overwrite it under those readers: parameter gradients of the generator were off by ~5 % with the
-            # (slow) exact-fp32 kernels and side streams on (scripts/diag_fullsize.py).
+            # (slow) exact-fp32 kernels and side streams on (test_full_size_c2_train_step_matches_oracle).
             dres = dy_full.clone()
         dbias, dv, dg = _weight_backward(spec, d, x_, dy, y_, v, g, ctx.params, ctx.norm, ctx.needs_input_grad[3],
                                          ctx.has_g and ctx.needs_input_grad[4], ctx.has_bias and ctx.needs_input_grad[2])
@@ -623,16 +619,6 @@ def pair_conv(owner, x, spec, cache, v, g, bias, resid=None):
 
 
 # ---- fused ResidualBlock unit (csrc/resblock_tc.cu) -------------------------------------------------------------------
-_FUSE_RESBLOCK = os.environ.get("KANTTS_B200_FUSE_RESBLOCK", "1") != "0"
-
-
-def set_fuse_resblock(flag):
-    """Route the (convs1[i], convs2[i]) pairs of the thin generator stages through the fused kernel (default) or through
-    two conv launches (A/B testing)."""
-    global _FUSE_RESBLOCK
-    _FUSE_RESBLOCK = bool(flag)
-
-
 def resblock_desc(spec1, spec2, batch, t):
     """-> KtResblockDesc when the pair (dilated conv, dilation-1 conv; same channels / kernel; fused input LeakyReLU, no
     output activation) can run on the fused kernel for this shape, else None.  Cached per shape on spec1."""

@@ -60,7 +60,7 @@ class GanStep:
     shape and ``criterion`` as built by the reference's builders (or this package's)."""
 
     def __init__(self, model, optimizer, scheduler, criterion, config, skip_unused_d_grads=True, cuda_graph=False,
-                 graph_warmup=3, pair_discriminators=True, reuse_real_half=None):
+                 graph_warmup=3, pair_discriminators=True, reuse_real_half=True):
         self.model, self.optimizer, self.scheduler = model, optimizer, scheduler
         self.criterion, self.config = criterion, config
         self.skip_unused_d_grads = skip_unused_d_grads
@@ -68,7 +68,7 @@ class GanStep:
         self.pair_discriminators = pair_discriminators
         # the discriminators' forward on the REAL waveforms is the same computation in both phases (same weights, same input):
         # the generator phase records it, the discriminator phase reuses it (ops.pair_state); spectral-normed scales excluded
-        self.reuse_real_half = (os.environ.get("KANTTS_B200_REUSE_REAL", "1") != "0") if reuse_real_half is None else reuse_real_half
+        self.reuse_real_half = reuse_real_half
         self._pair_recorded = False
         self.g_grads = FlatGrads(model["generator"])
         self.d_grads = {k: FlatGrads(m) for k, m in model["discriminator"].items()}
@@ -336,7 +336,7 @@ def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None
     reference's foreach Adam, ~4 launches per model instead of ~12 multi-tensor passes; ablation: the three Adam steps
     cost 1.4 ms of a 36 ms step)."""
     if fused_optimizer is None:
-        fused_optimizer = torch.device(device).type == "cuda" and os.environ.get("KANTTS_B200_FUSED_ADAM", "1") != "0"
+        fused_optimizer = torch.device(device).type == "cuda"
     from . import hifigan
     model = {"discriminator": {}}
     optimizer = {"discriminator": {}}

@@ -56,12 +56,7 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--only", default=None)
-    ap.add_argument("--flags", type=int, default=0, help="kt_debug_set_flags ablation bits (timing experiments; results are wrong)")
     a = ap.parse_args()
-    if a.flags:
-        from kantts_b200 import _lib
-        _lib.load().kt_debug_set_flags(a.flags)
-        print(f"# ablation flags {a.flags}")
     only = None if a.only is None else a.only.split(",")
     for n in LAYERS:
         if only is None or n in only:

@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol(lib):
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in kantts_b200.h but not exported"
     assert declared == set(_lib.PROTOTYPES) | {"kt_last_error"}
-    assert lib.kt_version() >= 1
+    assert lib.kt_version() >= 2
 
 
 def test_descriptor_struct_sizes_match_header():

@@ -5,7 +5,7 @@ import ctypes
 import pytest
 
 from kantts_b200 import _lib, ops
-from kantts_b200._lib import KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC
+from kantts_b200._lib import KT_ACT_LRELU, KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC
 
 
 @pytest.fixture(scope="module")
@@ -68,22 +68,45 @@ def test_split_k_workspace_is_whole_slices_of_the_gradient(lib):
                            (dict(c_in=128, c_out=256, kernel=41, stride=4, pad_left=20, pad_right=20, groups=16), 16, 2048, 1)):
         spec, d = _desc(B, T, nsub=nsub, **kw)
         ws = lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d))
-        # one slice per split: the weight gradient + (when the bias gradient rides along as an all-ones MMA unit) the
-        # bias gradient padded to a multiple of 4 floats
-        per = spec.w_numel + ((spec.c_out + 3) & ~3)
+        # one slice of the weight gradient per split (the bias gradient is the column-sum kernel's)
         out = (ctypes.c_int32 * 12)()
         assert lib.kt_debug_wgrad_plan(ctypes.byref(d), out) == 0
-        if out[1] and ws % spec.w_numel and ws % per:
+        if out[1] and ws % spec.w_numel:
             # TMA variant (a driver is present): the slices, padded to 64 floats, then the hi / lo bf16 operand planes of
             # both operands (one float per element each, padded to 64 floats)
             r64 = lambda n: (n + 63) & ~63
             planes = r64(d.batch * d.t_in * d.nsub * d.c_in) + r64(d.batch * d.t_out * d.nsub * d.c_out)
-            assert ws - planes in (r64(out[7] * spec.w_numel), r64(out[7] * per)), (ws, planes, out[7])
+            assert ws - planes == r64(out[7] * spec.w_numel), (ws, planes, out[7])
             nsplit = out[7]
         else:
-            assert ws > 0 and (ws % spec.w_numel == 0 or ws % per == 0)
-            nsplit = ws // per if ws % per == 0 else ws // spec.w_numel
+            assert ws > 0 and ws % spec.w_numel == 0
+            nsplit = ws // spec.w_numel
         assert 1 <= nsplit <= 296
+
+
+def _resblock_specs(C, k, d, causal):
+    p1 = (k - 1) * d if causal else (k - 1) * d // 2
+    p2 = (k - 1) if causal else (k - 1) // 2
+    s1 = ops.ConvSpec(c_in=C, c_out=C, kernel=k, dilation=d, pad_left=p1, pad_right=(k - 1) * d - p1, act_in=KT_ACT_LRELU, act_in_slope=0.1)
+    s2 = ops.ConvSpec(c_in=C, c_out=C, kernel=k, dilation=1, pad_left=p2, pad_right=(k - 1) - p2, act_in=KT_ACT_LRELU, act_in_slope=0.1)
+    return s1, s2
+
+
+def test_resblock_plan_fuses_the_shipped_pairs_and_rejects_boxes_over_256_rows(lib):
+    """kt_resblock_plan (geometry only, no GPU): every pair of the fused-resblock parity tests and of the shipped generator
+    stages (C = 32 / 64, k = 3 / 7 / 11, dilation 1 / 3 / 5) runs on the fused kernel.  Its x tile is one TMA box of
+    ceil8(128 + (k - 1) * dilation) (+ dilation when C = 32) rows, at most 256: C = 32, k = 15, dilation 11 needs 282, so
+    that pair runs as two conv launches."""
+    from test_gpu_parity import RB_CASES
+    shapes = [(C, k, d, causal, B, T) for C, k, d, causal, B, T in RB_CASES.values()]
+    shapes += [(C, k, d, causal, 16, 8192) for C in (32, 64) for k in (3, 7, 11) for d in (1, 3, 5) for causal in (True, False)]
+    for C, k, d, causal, B, T in shapes:
+        s1, s2 = _resblock_specs(C, k, d, causal)
+        rd = ops.resblock_desc(s1, s2, B, T)
+        assert rd is not None and lib.kt_resblock_plan(ctypes.byref(rd)) == 1, (C, k, d, causal, B, T)
+        assert lib.kt_resblock_image_bytes(ctypes.byref(rd)) > 0
+    s1, s2 = _resblock_specs(32, 15, 11, True)
+    assert ops.resblock_desc(s1, s2, 2, 1000) is None
 
 
 def test_grad_items_context_restores_state():
