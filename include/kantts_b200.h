@@ -265,6 +265,30 @@ int kt_rows_gather_fwd(const float* in, const int32_t* idx, float* out, int32_t 
 int kt_rows_gather_bwd(const float* dout, const int32_t* idx, const int32_t* start, const int32_t* count, float* din,
                        int32_t batch, int32_t t_out, int32_t t_in, int32_t c, void* stream);
 
+/* Filled-pause insertion (KanTtsSAMBERT.insert_fp, kantts_sambert.py:766-860).  Row t of utterance b of the output is
+ * row t of the stream: for j = 0 .. length-1, the 3 rows of filled pause k_j (when k_j > 0) then text_hid[b][j]; after
+ * that text_hid[b][q % length] for q = 0, 1, ...
+ * kt_fp_insert_plan: one CTA per utterance.  Either fp_label [batch][length] (label_bytes 4 = int32, 8 = int64;
+ * k_j = label when it is 1..3, n_b counts every label > 0 over all positions) or, with label_bytes 0, the softmax output
+ * fp_p [batch][length][4] (16-byte aligned): on positions j < input_lengths[b] the flags are (p == max over the 4
+ * classes) for classes 1..3, k_j is the first set flag and n_b counts every set flag.  Writes
+ *   codes [batch][t_cap]: >= 0 a text_hid row; -(1 + 3 (k-1) + m) row m of filled pause k (rows past t_cap are dropped),
+ *   rows [batch][length]: the stream row of text_hid[b][j],
+ *   inter_lengths [batch] = input_lengths[b] + 3 n_b.
+ * t_ins = length + max(inter_lengths) - max(input_lengths) rows are valid; t_cap >= t_ins is the caller's bound
+ * (4 * length for labels, 10 * length for predictions).
+ * kt_fp_insert_fwd: out [batch][t_ins][c] from text_hid [batch][length][c] and fp_enc [3][3][c].
+ * kt_fp_insert_bwd: d_text_hid [batch][length][c] and / or d_fp_enc [3][3][c] (either may be NULL), each a fixed-order
+ * sum (d_fp_enc: per-utterance sums into `partials`, at least 9 * batch * c floats, then a sum over b in order). */
+int kt_fp_insert_plan(const void* fp_label, int32_t label_bytes, const float* fp_p, const int32_t* input_lengths,
+                      int32_t batch, int32_t length, int32_t t_cap, int32_t* codes, int32_t* rows, int32_t* inter_lengths,
+                      void* stream);
+int kt_fp_insert_fwd(const float* text_hid, const float* fp_enc, const int32_t* codes, float* out, int32_t batch,
+                     int32_t length, int32_t t_cap, int32_t t_ins, int32_t c, void* stream);
+int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* rows, float* d_text_hid, float* d_fp_enc,
+                     float* partials, int64_t partial_floats, int32_t batch, int32_t length, int32_t t_cap, int32_t t_ins,
+                     int32_t c, void* stream);
+
 /* Autoregressive duration predictor, free-running inference (VarRnnARPredictor.infer, kantts/models/sambert/adaptors.py:67-83):
  * the whole per-symbol recurrence  x -> Prenet(1 -> p1 -> p2, ReLU) -> cat(cond) -> 2-layer LSTM(hidden) -> Linear(hidden, 1) ->
  * ReLU -> next x  in ONE launch (one CTA per batch item) instead of ~10 library launches per symbol from Python.

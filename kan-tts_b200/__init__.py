@@ -14,7 +14,7 @@ All tensor math runs in libkantts_b200.so (C ABI: include/kantts_b200.h); there 
 from . import _lib  # noqa: F401
 from ._lib import build_library  # noqa: F401
 from . import ops, hifigan, audio, loss, sambert_ops, sambert, train, infer, install as _install  # noqa: F401
-from .sambert import KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss  # noqa: F401
+from .sambert import KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss  # noqa: F401
 from .hifigan import Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator  # noqa: F401
 from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401
@@ -39,6 +39,12 @@ def sambert_24k_config():
         postnet_fsmn_num_layers=4, postnet_num_memory_units=256, postnet_ffn_inner_dim=512, postnet_dropout=0.1,
         postnet_shift=17, postnet_lstm_units=128, MAS=False,
         sy=147, tone=10, syllable_flag=8, word_segment=8, emotion=36, speaker=4)
+
+
+def sambert_fp_8k_config():
+    """``Model.KanTtsSAMBERT.params`` of kantts/configs/sambert_fp_8k.yaml: the sambert_24k.yaml network with the
+    filled-pause predictor (``FP: True``) and the yaml's six speakers."""
+    return dict(sambert_24k_config(), FP=True, speaker=6)
 
 
 install = _install.install

@@ -91,6 +91,9 @@ PROTOTYPES = {
     "kt_fsmn_bwd": [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "kt_rows_gather_fwd": [_P, _P, _P, _I, _I, _I, _I, _P],
     "kt_rows_gather_bwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "kt_fp_insert_plan": [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P],
+    "kt_fp_insert_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    "kt_fp_insert_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_version": [],
     "kt_has_tc": [],
@@ -149,7 +152,7 @@ def check(rc, what):
 
 
 _PTR_DTYPES = (torch.float32,)
-_AUX_DTYPES = (torch.uint8, torch.int32, torch.bfloat16)   # masks / keep-masks, gather indices, packed tensor-core weight tiles
+_AUX_DTYPES = (torch.uint8, torch.int32, torch.int64, torch.bfloat16)   # masks / keep-masks, gather indices, filled-pause labels, packed tensor-core weight tiles
 
 
 def ptr(t, aux=False):

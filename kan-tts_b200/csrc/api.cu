@@ -47,6 +47,10 @@ int fsmn_bwd(const float*, const float*, const float*, const unsigned char*, flo
              int, int, int, cudaStream_t);
 int rows_gather_fwd(const float*, const int*, float*, int, int, int, int, cudaStream_t);
 int rows_gather_bwd(const float*, const int*, const int*, const int*, float*, int, int, int, int, cudaStream_t);
+int fp_insert_plan(const void*, int, const float*, const int*, int, int, int, int*, int*, int*, cudaStream_t);
+int fp_insert_fwd(const float*, const float*, const int*, float*, int, int, int, int, int, cudaStream_t);
+int fp_insert_bwd(const float*, const int*, const int*, float*, float*, float*, long long, int, int, int, int, int,
+                  cudaStream_t);
 }  // namespace kt
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -131,7 +135,7 @@ int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float*
 }
 
 const char* kt_last_error(void) { return kt::last_error(); }
-int kt_version(void) { return 2; }
+int kt_version(void) { return 3; }
 int kt_has_tc(void) { return 1; }
 
 int kt_conv1d_tc_plan(const KtConv1dDesc* d, int32_t dir) {
@@ -244,6 +248,22 @@ int kt_rows_gather_fwd(const float* in, const int32_t* idx, float* out, int32_t 
 int kt_rows_gather_bwd(const float* dout, const int32_t* idx, const int32_t* start, const int32_t* count, float* din,
                        int32_t batch, int32_t t_out, int32_t t_in, int32_t c, void* stream) {
   return kt::rows_gather_bwd(dout, idx, start, count, din, batch, t_out, t_in, c, ST(stream));
+}
+int kt_fp_insert_plan(const void* fp_label, int32_t label_bytes, const float* fp_p, const int32_t* input_lengths,
+                      int32_t batch, int32_t length, int32_t t_cap, int32_t* codes, int32_t* rows, int32_t* inter_lengths,
+                      void* stream) {
+  return kt::fp_insert_plan(fp_label, label_bytes, fp_p, input_lengths, batch, length, t_cap, codes, rows, inter_lengths,
+                            ST(stream));
+}
+int kt_fp_insert_fwd(const float* text_hid, const float* fp_enc, const int32_t* codes, float* out, int32_t batch,
+                     int32_t length, int32_t t_cap, int32_t t_ins, int32_t c, void* stream) {
+  return kt::fp_insert_fwd(text_hid, fp_enc, codes, out, batch, length, t_cap, t_ins, c, ST(stream));
+}
+int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* rows, float* d_text_hid, float* d_fp_enc,
+                     float* partials, int64_t partial_floats, int32_t batch, int32_t length, int32_t t_cap, int32_t t_ins,
+                     int32_t c, void* stream) {
+  return kt::fp_insert_bwd(dout, codes, rows, d_text_hid, d_fp_enc, partials, partial_floats, batch, length, t_cap, t_ins, c,
+                           ST(stream));
 }
 
 }  // extern "C"

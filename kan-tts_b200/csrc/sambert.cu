@@ -8,6 +8,7 @@
 // K=16 contraction -- a single wgmma k-step -- and the kernels are bound by the probability-matrix
 // traffic (B*H*Lq*Lk*4 bytes written in forward, read twice in backward), not by math.
 #include <atomic>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -894,6 +895,196 @@ int rows_gather_bwd(const float* dout, const int* idx, const int* start, const i
   rows_gather_bwd_kernel<<<grid_for((long long)B * T_in * C, 256), 256, 0, st>>>(dout, idx, start, count, din, B, T_out,
                                                                                  T_in, C);
   KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Filled-pause insertion (KanTtsSAMBERT.insert_fp, kantts_sambert.py:766-860) as an index plan plus a row
+// gather.  Row t of utterance b is row t of the stream: for j = 0 .. L-1, the 3 rows of filled pause k_j (if
+// k_j > 0) then text_hid[b, j]; then the tail rows text_hid[b, q mod L], q = 0, 1, ...  A row code >= 0 is a
+// text_hid row; code = -(1 + 3 (k-1) + m) is row m of filled pause k (fp_enc is [3][3][C]).
+//   training  (labels):  k_j = label if 1 <= label <= 3, n_b counts every label > 0 over all L positions;
+//   inference (FP_p):    flags = (p == max over the 4 classes)[1:] on valid positions, k_j = first set flag,
+//                        n_b counts every set flag (an exact tie counts twice but inserts once).
+// inter_lengths[b] = input_lengths[b] + 3 n_b.  rows[b, j] = the stream row of text_hid[b, j].
+// ------------------------------------------------------------------------------------------------
+constexpr int kFpPlanThreads = 256;
+
+__global__ void __launch_bounds__(kFpPlanThreads) fp_plan_kernel(const void* __restrict__ labels, int label_bytes,
+                                                                 const float* __restrict__ fp_p, const int* __restrict__ in_len,
+                                                                 int L, int T_cap, int* __restrict__ codes,
+                                                                 int* __restrict__ rows, int* __restrict__ inter) {
+  __shared__ int s_w[kFpPlanThreads / 32], s_n[kFpPlanThreads / 32];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int len = __ldg(in_len + b);
+  int* code = codes + (long long)b * T_cap;
+  int carry_w = 0, carry_n = 0;
+  for (int base = 0; base < L; base += kFpPlanThreads) {
+    const int j = base + tid;
+    int k = 0, cnt = 0;
+    if (j < L) {
+      const long long bj = (long long)b * L + j;
+      if (label_bytes) {
+        const long long v = label_bytes == 8 ? __ldg((const long long*)labels + bj) : (long long)__ldg((const int*)labels + bj);
+        cnt = v > 0;
+        k = (v >= 1 && v <= 3) ? (int)v : 0;
+      } else if (j < len) {
+        const float4 p = __ldg((const float4*)fp_p + bj);
+        const float mx = fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w));
+        const int f1 = p.y == mx, f2 = p.z == mx, f3 = p.w == mx;
+        cnt = f1 + f2 + f3;
+        k = f1 ? 1 : (f2 ? 2 : (f3 ? 3 : 0));
+      }
+    }
+    const int w = j < L ? (k ? 4 : 1) : 0;
+    int iw = w, in = cnt;                                  // inclusive block scan of the widths, block sum of the counts
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int a = __shfl_up_sync(0xffffffffu, iw, o);
+      if (lane >= o) iw += a;
+    }
+    in = __reduce_add_sync(0xffffffffu, in);
+    if (lane == 31) s_w[warp] = iw;
+    if (lane == 0) s_n[warp] = in;
+    __syncthreads();
+    int before = 0, tot_w = 0, tot_n = 0;
+#pragma unroll
+    for (int i = 0; i < kFpPlanThreads / 32; ++i) {
+      if (i < warp) before += s_w[i];
+      tot_w += s_w[i];
+      tot_n += s_n[i];
+    }
+    if (j < L) {
+      const int off = carry_w + before + iw - w;
+      for (int m = 0; m < 3 && k; ++m)
+        if (off + m < T_cap) code[off + m] = -(1 + 3 * (k - 1) + m);
+      const int r = off + w - 1;
+      rows[(long long)b * L + j] = r;
+      if (r < T_cap) code[r] = j;
+    }
+    carry_w += tot_w;
+    carry_n += tot_n;
+    __syncthreads();
+  }
+  for (int t = carry_w + tid; t < T_cap; t += kFpPlanThreads) code[t] = (t - carry_w) % L;
+  if (tid == 0) inter[b] = len + 3 * carry_n;
+}
+
+template <int V>
+__global__ void fp_insert_fwd_kernel(const float* __restrict__ text, const float* __restrict__ fp_enc,
+                                     const int* __restrict__ codes, float* __restrict__ out, int B, int L, int T_cap,
+                                     int T_ins, int C) {
+  using vec = typename std::conditional<V == 4, float4, float>::type;
+  const int cv = C / V;
+  const long long total = (long long)B * T_ins * cv;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cv);
+    const long long bt = i / cv;
+    const int b = (int)(bt / T_ins), t = (int)(bt % T_ins);
+    const int code = __ldg(codes + (long long)b * T_cap + t);
+    const float* src = code >= 0 ? text + ((long long)b * L + code) * C : fp_enc + (long long)(-code - 1) * C;
+    reinterpret_cast<vec*>(out)[i] = __ldg(reinterpret_cast<const vec*>(src) + c);
+  }
+}
+
+// d text_hid[b, s] = the interleaved row rows[b, s] (when it is < T_ins) + the tail rows S_b + s + q L, ascending
+template <int V>
+__global__ void fp_insert_bwd_text_kernel(const float* __restrict__ dout, const int* __restrict__ rows,
+                                          float* __restrict__ dtext, int B, int L, int T_ins, int C) {
+  using vec = typename std::conditional<V == 4, float4, float>::type;
+  const int cv = C / V;
+  const long long total = (long long)B * L * cv;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cv);
+    const long long bs = i / cv;
+    const int b = (int)(bs / L), s = (int)(bs % L);
+    const int S = __ldg(rows + (long long)b * L + L - 1) + 1;
+    const vec* d = reinterpret_cast<const vec*>(dout) + (long long)b * T_ins * cv + c;
+    vec acc;
+    float* a = reinterpret_cast<float*>(&acc);
+#pragma unroll
+    for (int v = 0; v < V; ++v) a[v] = 0.f;
+    const int r = __ldg(rows + bs);
+    for (int t = r; t < T_ins; t = (t == r) ? S + s : t + L) {
+      const vec x = __ldg(d + (long long)t * cv);
+      const float* xv = reinterpret_cast<const float*>(&x);
+#pragma unroll
+      for (int v = 0; v < V; ++v) a[v] += xv[v];
+    }
+    reinterpret_cast<vec*>(dtext)[i] = acc;
+  }
+}
+
+// per-utterance partial d fp_enc: partial[b][km][c] = sum over t ascending of dout[b, t, c] where code = -(km + 1)
+__global__ void fp_insert_bwd_fp_partial_kernel(const float* __restrict__ dout, const int* __restrict__ codes,
+                                                float* __restrict__ partial, int T_cap, int T_ins, int C) {
+  const int b = blockIdx.x;
+  const int* code = codes + (long long)b * T_cap;
+  const float* d = dout + (long long)b * T_ins * C;
+  for (int i = threadIdx.x; i < 9 * C; i += blockDim.x) {
+    const int km = i / C, c = i % C;
+    float acc = 0.f;
+    for (int t = 0; t < T_ins; ++t)
+      if (__ldg(code + t) == -(km + 1)) acc += __ldg(d + (long long)t * C + c);
+    partial[(long long)b * 9 * C + i] = acc;
+  }
+}
+
+__global__ void fp_insert_bwd_fp_reduce_kernel(const float* __restrict__ partial, float* __restrict__ dfp, int B, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int b = 0; b < B; ++b) acc += partial[(long long)b * n + i];
+    dfp[i] = acc;
+  }
+}
+
+int fp_insert_plan(const void* labels, int label_bytes, const float* fp_p, const int* in_len, int B, int L, int T_cap,
+                   int* codes, int* rows, int* inter, cudaStream_t st) {
+  KT_REQUIRE(in_len && codes && rows && inter && B >= 1 && L >= 1 && T_cap >= L, "fp_insert_plan: bad arguments");
+  KT_REQUIRE(label_bytes ? (labels && (label_bytes == 4 || label_bytes == 8)) : (label_bytes == 0 && fp_p != nullptr),
+             "fp_insert_plan: give int32 / int64 labels or the (B, L, 4) predictions");
+  KT_REQUIRE(label_bytes || (reinterpret_cast<uintptr_t>(fp_p) & 15) == 0, "fp_insert_plan: predictions not 16-byte aligned");
+  fp_plan_kernel<<<B, kFpPlanThreads, 0, st>>>(labels, label_bytes, fp_p, in_len, L, T_cap, codes, rows, inter);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+static bool fp_vec4(int C, const void* a, const void* b, const void* c) {
+  return C % 4 == 0 && ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
+}
+
+int fp_insert_fwd(const float* text, const float* fp_enc, const int* codes, float* out, int B, int L, int T_cap, int T_ins,
+                  int C, cudaStream_t st) {
+  KT_REQUIRE(text && fp_enc && codes && out && B >= 1 && L >= 1 && C >= 1 && T_ins >= L && T_ins <= T_cap,
+             "fp_insert_fwd: bad arguments");
+  if (fp_vec4(C, text, fp_enc, out))
+    fp_insert_fwd_kernel<4><<<grid_for((long long)B * T_ins * C / 4, 256), 256, 0, st>>>(text, fp_enc, codes, out, B, L, T_cap,
+                                                                                        T_ins, C);
+  else
+    fp_insert_fwd_kernel<1><<<grid_for((long long)B * T_ins * C, 256), 256, 0, st>>>(text, fp_enc, codes, out, B, L, T_cap,
+                                                                                    T_ins, C);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+int fp_insert_bwd(const float* dout, const int* codes, const int* rows, float* dtext, float* dfp, float* partial,
+                  long long partial_floats, int B, int L, int T_cap, int T_ins, int C, cudaStream_t st) {
+  KT_REQUIRE(dout && codes && rows && B >= 1 && L >= 1 && C >= 1 && T_ins >= L && T_ins <= T_cap,
+             "fp_insert_bwd: bad arguments");
+  KT_REQUIRE(!dfp || (partial && partial_floats >= 9LL * B * C), "fp_insert_bwd: partials need 9 * batch * c floats");
+  if (dtext) {
+    if (fp_vec4(C, dout, dtext, dtext))
+      fp_insert_bwd_text_kernel<4><<<grid_for((long long)B * L * C / 4, 256), 256, 0, st>>>(dout, rows, dtext, B, L, T_ins, C);
+    else
+      fp_insert_bwd_text_kernel<1><<<grid_for((long long)B * L * C, 256), 256, 0, st>>>(dout, rows, dtext, B, L, T_ins, C);
+    KT_CHECK_CUDA(cudaGetLastError());
+  }
+  if (dfp) {
+    fp_insert_bwd_fp_partial_kernel<<<B, 288, 0, st>>>(dout, codes, partial, T_cap, T_ins, C);
+    KT_CHECK_CUDA(cudaGetLastError());
+    fp_insert_bwd_fp_reduce_kernel<<<grid_for(9LL * C, 256), 256, 0, st>>>(partial, dfp, B, 9 * C);
+    KT_CHECK_CUDA(cudaGetLastError());
+  }
   return KT_OK;
 }
 

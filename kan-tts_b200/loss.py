@@ -11,6 +11,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .audio import MelSpectrogram, stft
+from .sambert import FpCELoss
 
 
 def _as_list(outputs):
@@ -230,6 +231,7 @@ loss_dict = {
     "mel_loss": MelSpectrogramLoss,
     "subband_stft_loss": MultiResolutionSTFTLoss,
     "feat_match_loss": FeatureMatchLoss,
+    "FpCELoss": FpCELoss,
 }
 
 

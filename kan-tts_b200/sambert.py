@@ -16,8 +16,10 @@ Where the arithmetic runs:
   * the four LSTMs stay on cuDNN (``nn.LSTM``) -- SURVEY.md section 2c rules them out of scope for custom
     kernels -- and the remaining glue (embedding lookups, concatenations, padding masks, sinusoid tables,
     dropout) is torch elementwise / indexing code, as in the reference.
-Not built: MAS alignment (``MAS: True``), the filled-pause predictor (``FP``) and speaker-encoder (``SE``)
-variants -- the shipped sambert_24k.yaml disables all three.
+The filled-pause variant (``FP: True``, sambert_fp_8k.yaml) is built: FP_Predictor on the same conv / LayerNorm
+kernels, and the splice of the predicted or labelled pauses into the text encoding as an index plan plus one
+gather each way (kt_fp_insert_*).  Not built: MAS alignment (``MAS: True``) and the speaker-encoder (``SE``)
+variant -- the shipped sambert_24k.yaml and sambert_fp_8k.yaml disable both.
 """
 import numpy as np
 import torch
@@ -747,12 +749,35 @@ class PostNet(nn.Module):
         return self.fc(h, resid=resid)
 
 
-class KanTtsSAMBERT(nn.Module):
-    """kantts_sambert.py:652-1044."""
+class FP_Predictor(nn.Module):
+    """kantts_sambert.py:677-710: filled-pause class probabilities (none / en / a / e) per symbol.  The two ReLUs are
+    fused into the convs; the 4-class softmax stays a torch op."""
 
     def __init__(self, config):
         super().__init__()
-        for flag in ("SE", "MAS", "FP"):
+        d_proj, d_hid = config["encoder_projection_units"], config["embedding_dim"] // 2
+        self.w_1 = RowConv1d(d_proj, d_hid, 3, padding=1, relu=True)
+        self.w_2 = RowConv1d(d_hid, d_proj, 1, relu=True)
+        self.layer_norm1 = LayerNorm(d_hid, eps=1e-6)
+        self.layer_norm2 = LayerNorm(d_proj, eps=1e-6)
+        self.dropout_inner = nn.Dropout(0.1)
+        self.dropout = nn.Dropout(0.1)
+        self.fc = Linear(d_proj, 4)
+
+    def forward(self, x):
+        x = self.dropout_inner(self.layer_norm1(self.w_1(x)))
+        x = self.dropout(self.layer_norm2(self.w_2(x)))
+        return F.softmax(self.fc(x), dim=2)
+
+
+class KanTtsSAMBERT(nn.Module):
+    """kantts_sambert.py:652-1044.  With ``FP: True`` the model builder must set ``fp_dict`` ({1: en, 2: a, 3: e},
+    each a (1, 3, 4) long tensor of linguistic ids) before the first forward, as kantts/models/__init__.py:99-105
+    does."""
+
+    def __init__(self, config):
+        super().__init__()
+        for flag in ("SE", "MAS"):
             if config.get(flag, False):
                 raise NotImplementedError(f"KanTtsSAMBERT variant {flag}=True is not built (see module docstring)")
         self.text_encoder = TextFftEncoder(config)
@@ -763,7 +788,25 @@ class KanTtsSAMBERT(nn.Module):
         self.mel_decoder = MelPNCADecoder(config)
         self.mel_postnet = PostNet(config)
         self.MAS = False
-        self.fp_enable = False
+        self.fp_enable = bool(config.get("FP", False))
+        if self.fp_enable:
+            self.FP_predictor = FP_Predictor(config)
+        self.fp_dict = None
+
+    def insert_fp(self, text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths):
+        """kantts_sambert.py:766-860: splice the encodings of the filled pauses (labelled, or predicted when
+        ``fp_label`` is None) in front of their symbols.  The three pause sequences go through the text encoder as one
+        unmasked batch; the emotion / speaker ids are only extended (row t takes row t mod L)."""
+        if self.fp_dict is None:
+            raise RuntimeError("KanTtsSAMBERT(FP=True) needs model.fp_dict = {1: en, 2: a, 3: e} (each a (1, 3, 4) "
+                               "long tensor of linguistic ids) before the forward, as the reference model builder sets")
+        seqs = torch.cat([self.fp_dict[k].reshape(1, 3, -1) for k in (1, 2, 3)], 0).to(text_hid.device)
+        fp_enc, _, _ = self.text_encoder(seqs)
+        L = text_hid.size(1)
+        codes, rows, inter_lengths, t_ins = sops.fp_insert_plan(input_lengths, L, fp_label=fp_label, fp_p=fp_p)
+        text_hid = sops.FpInsertFn.apply(text_hid, fp_enc, codes, rows, t_ins)
+        ext = torch.arange(t_ins, device=text_hid.device) % L
+        return text_hid, inputs_emotion[:, ext], inputs_speaker[:, ext], inter_lengths
 
     def get_lfr_mask_from_lengths(self, lengths, max_len):
         """kantts_sambert.py:681-695 without the per-item host loop: ceil(len / r) frames are valid."""
@@ -778,6 +821,11 @@ class KanTtsSAMBERT(nn.Module):
         input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
         text_hid, enc_attns, _ = self.text_encoder(inputs_ling, input_masks, return_attns=True)
         inter_lengths = input_lengths
+        fp_p = None
+        if self.fp_enable:
+            fp_p = self.FP_predictor(text_hid)
+            text_hid, inputs_emotion, inputs_speaker, inter_lengths = self.insert_fp(
+                text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths)
         emo_hid = self.emo_tokenizer(inputs_emotion)
         spk_hid = self.spk_tokenizer(inputs_speaker)
         inter_masks = get_mask_from_lengths(inter_lengths, max_len=text_hid.size(1))
@@ -816,7 +864,7 @@ class KanTtsSAMBERT(nn.Module):
             "postnet_outputs": postnet_outputs, "LR_length_rounded": lr_len,
             "log_duration_predictions": log_dur_p, "pitch_predictions": pitch_p, "energy_predictions": energy_p,
             "duration_targets": duration_targets, "pitch_targets": pitch_targets, "energy_targets": energy_targets,
-            "fp_predictions": None, "valid_inter_lengths": inter_lengths,
+            "fp_predictions": fp_p, "valid_inter_lengths": inter_lengths,
             "LR_text_outputs": lr_text, "LR_emo_outputs": lr_emo, "LR_spk_outputs": lr_spk,
         }
 
@@ -868,3 +916,19 @@ class ProsodyReconLoss(nn.Module):
         pitch_loss = torch.sum(self._err(pitch_targets, pitch_predictions) * valid) / n
         energy_loss = torch.sum(self._err(energy_targets, energy_predictions) * valid) / n
         return dur_loss, pitch_loss, energy_loss
+
+
+class FpCELoss(nn.Module):
+    """train/loss.py:88-105: class-weighted cross entropy of the filled-pause predictions over the valid symbols.
+    ``fp_pd`` is already a softmax output and the cross entropy applies log_softmax to it again, as the reference does.
+    The class weights are a buffer, so ``.to(device)`` moves them."""
+
+    def __init__(self, loss_type="ce", weight=[1, 4, 4, 8]):
+        super().__init__()
+        self.loss_type = loss_type
+        self.register_buffer("weight", torch.tensor(weight, dtype=torch.float32))
+
+    def forward(self, input_lengths, fp_pd, fp_label):
+        valid = ~get_mask_from_lengths(input_lengths, max_len=fp_label.size(1))
+        ce = F.cross_entropy(fp_pd.transpose(2, 1), fp_label, weight=self.weight, reduction="none")
+        return torch.sum(ce * valid) / valid.sum()

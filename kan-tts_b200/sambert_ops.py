@@ -1,5 +1,5 @@
 """autograd wrappers of the SAM-BERT entry points of libkantts_b200.so (LayerNorm, multi-head attention,
-FSMN memory block, LengthRegulator gather).  Same contract as ops.py: CUDA fp32 tensors only, explicit
+FSMN memory block, LengthRegulator gather, filled-pause insertion).  Same contract as ops.py: CUDA fp32 tensors only, explicit
 stream, RuntimeError on any failure -- no PyTorch / CPU fallback."""
 import ctypes
 
@@ -277,3 +277,60 @@ class RowsGatherFn(torch.autograd.Function):
                                      stream_ptr()), "kt_rows_gather_bwd")
         _count()
         return din, None, None, None
+
+
+def fp_insert_plan(input_lengths, length, fp_label=None, fp_p=None):
+    """Index plan of KanTtsSAMBERT.insert_fp (kantts_sambert.py:766-860, kt_fp_insert_plan): from ``fp_label`` (B, L)
+    integer labels (training) or the (B, L, 4) predictions ``fp_p`` (inference).  -> codes (B, t_cap) int32,
+    rows (B, L) int32, inter_lengths (B,) int64, t_ins.  Reading t_ins is the one host synchronisation."""
+    lib = _lib.load()
+    B = input_lengths.shape[0]
+    lens = input_lengths.to(torch.int32).contiguous()
+    if fp_label is not None:
+        lab = fp_label if fp_label.dtype in (torch.int32, torch.int64) else fp_label.long()
+        lab, nbytes, p, t_cap = lab.contiguous(), lab.element_size(), None, 4 * length
+    else:
+        lab, nbytes, p, t_cap = None, 0, fp_p.detach().contiguous(), 10 * length
+    codes = torch.empty(B, t_cap, device=lens.device, dtype=torch.int32)
+    rows = torch.empty(B, length, device=lens.device, dtype=torch.int32)
+    inter = torch.empty(B, device=lens.device, dtype=torch.int32)
+    check(lib.kt_fp_insert_plan(ptr(lab, True), nbytes, ptr(p), ptr(lens, True), B, length, t_cap, ptr(codes, True),
+                                ptr(rows, True), ptr(inter, True), stream_ptr()), "kt_fp_insert_plan")
+    _count()
+    t_ins = length + int(inter.max() - lens.max())
+    return codes, rows, inter.to(input_lengths.dtype), t_ins
+
+
+class FpInsertFn(torch.autograd.Function):
+    """Filled-pause splice of KanTtsSAMBERT.insert_fp as a row gather (kt_fp_insert_fwd / _bwd): text_hid (B, L, C)
+    and fp_enc (3, 3, C), the text encoder's output for the three filled-pause symbol sequences, -> (B, t_ins, C)."""
+
+    @staticmethod
+    def forward(ctx, text_hid, fp_enc, codes, rows, t_ins):
+        lib = _lib.load()
+        text_hid, fp_enc = text_hid.contiguous(), fp_enc.contiguous()
+        B, L, C = text_hid.shape
+        assert fp_enc.shape == (3, 3, C), fp_enc.shape
+        out = torch.empty(B, t_ins, C, device=text_hid.device, dtype=torch.float32)
+        check(lib.kt_fp_insert_fwd(ptr(text_hid), ptr(fp_enc), ptr(codes, True), ptr(out), B, L, codes.shape[1], t_ins, C,
+                                   stream_ptr()), "kt_fp_insert_fwd")
+        _count()
+        ctx.save_for_backward(codes, rows)
+        ctx.shape = (B, L, C)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = _lib.load()
+        codes, rows = ctx.saved_tensors
+        B, L, C = ctx.shape
+        dout = dout.contiguous()
+        dev = dout.device
+        dtext = torch.empty(B, L, C, device=dev, dtype=torch.float32) if ctx.needs_input_grad[0] else None
+        dfp = torch.empty(3, 3, C, device=dev, dtype=torch.float32) if ctx.needs_input_grad[1] else None
+        part = torch.empty(9 * B * C, device=dev, dtype=torch.float32) if dfp is not None else None
+        check(lib.kt_fp_insert_bwd(ptr(dout), ptr(codes, True), ptr(rows, True), ptr(dtext), ptr(dfp), ptr(part),
+                                   0 if part is None else part.numel(), B, L, codes.shape[1], dout.shape[1], C,
+                                   stream_ptr()), "kt_fp_insert_bwd")
+        _count(1 + 2 * (dfp is not None))
+        return dtext, dfp, None, None, None

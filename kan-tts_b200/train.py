@@ -396,18 +396,24 @@ class SambertStep:
     def step(self, batch):
         """batch: dict with the reference collate keys (input_lings, input_emotions, input_speakers,
         valid_input_lengths, valid_output_lengths, mel_targets, durations, pitch_contours, energy_contours),
-        tensors already on the model's device."""
+        tensors already on the model's device; plus ``fp_label`` for a filled-pause (FP) model, whose durations /
+        pitch / energy contours are padded to the length with the pauses inserted."""
+        fp_label = batch.get("fp_label")
         res = self.model(
             batch["input_lings"], batch["input_emotions"], batch["input_speakers"], batch["valid_input_lengths"],
             output_lengths=batch["valid_output_lengths"], mel_targets=batch["mel_targets"],
             duration_targets=batch["durations"], pitch_targets=batch["pitch_contours"],
-            energy_targets=batch["energy_contours"])
+            energy_targets=batch["energy_contours"], fp_label=fp_label)
         mel_loss_, mel_loss = self.criterion["MelReconLoss"](
             batch["valid_output_lengths"], batch["mel_targets"], res["dec_outputs"], res["postnet_outputs"])
         dur_loss, pitch_loss, energy_loss = self.criterion["ProsodyReconLoss"](
             res["valid_inter_lengths"], res["duration_targets"], res["pitch_targets"], res["energy_targets"],
             res["log_duration_predictions"], res["pitch_predictions"], res["energy_predictions"])
         loss_total = mel_loss_ + mel_loss + dur_loss + pitch_loss + energy_loss
+        fp_loss = None
+        if "FpCELoss" in self.criterion:
+            fp_loss = self.criterion["FpCELoss"](batch["valid_input_lengths"], res["fp_predictions"], fp_label)
+            loss_total = loss_total + fp_loss
         self.grads.zero()
         loss_total.backward()
         ops.join_wgrad_streams(loss_total.device if loss_total.is_cuda else None)
@@ -417,18 +423,24 @@ class SambertStep:
         self.optimizer.step()
         self.scheduler.step()
         self.steps += 1
-        return {"TotalLoss": loss_total.detach(), "mel_loss_": mel_loss_.detach(), "mel_loss": mel_loss.detach(),
-                "dur_loss": dur_loss.detach(), "pitch_loss": pitch_loss.detach(),
-                "energy_loss": energy_loss.detach(), "x_band_width": res["x_band_width"],
-                "h_band_width": res["h_band_width"]}
+        out = {"TotalLoss": loss_total.detach(), "mel_loss_": mel_loss_.detach(), "mel_loss": mel_loss.detach(),
+               "dur_loss": dur_loss.detach(), "pitch_loss": pitch_loss.detach(),
+               "energy_loss": energy_loss.detach(), "x_band_width": res["x_band_width"],
+               "h_band_width": res["h_band_width"]}
+        if fp_loss is not None:
+            out["fp_loss"] = fp_loss.detach()
+        return out
 
 
-def sambert_model_builder(config, device):
+def sambert_model_builder(config, device, fp_dict=None):
     """kantts/models/__init__.py:89-129 without the DDP wrapper: ``config`` is the whole yaml dict with the
-    linguistic-unit sizes already merged into ``Model.KanTtsSAMBERT.params`` (bin/train_sambert.py:144-146)."""
+    linguistic-unit sizes already merged into ``Model.KanTtsSAMBERT.params`` (bin/train_sambert.py:144-146).
+    ``fp_dict`` ({1: en, 2: a, 3: e} linguistic-id tensors) is attached to a filled-pause (FP) model."""
     from . import sambert
     sect = config["Model"]["KanTtsSAMBERT"]
     model = sambert.KanTtsSAMBERT(sect["params"]).to(device)
+    if fp_dict is not None:
+        model.fp_dict = {k: v.to(device) for k, v in fp_dict.items()}
     opt = optimizer_builder(model.parameters(), sect["optimizer"].get("type", "Adam"),
                             dict(sect["optimizer"].get("params", {})))
     sch_t = sect["scheduler"].get("type", "NoamLR")
