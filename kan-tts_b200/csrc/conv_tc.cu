@@ -238,102 +238,105 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     const uint32_t a_stage16 = (uint32_t)a_stage_bytes >> 4, img16 = (uint32_t)img_bytes >> 4;
     const uint32_t b_stage16 = (uint32_t)b_stage_bytes >> 4, bplane16 = (uint32_t)(p.NT * 128) >> 4;
     const bool resident = p.w_resident != 0;
-    const int NT = p.NT;
-    float acc[kWgmmaMaxRegs];
+    // one consumer path per MMA width (see with_wgmma_n)
+    with_wgmma_n(p.NT, [&](auto nt) {
+      constexpr int NT = decltype(nt)::value;
+      float acc[kWgmmaMaxRegs];
 #pragma unroll
-    for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
-    int it_a = 0, it_b = 0, ti = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-      const int gm = tile % mtiles, nt = (tile / mtiles) % p.ntiles, bb = tile / (mtiles * p.ntiles);
-      int ph = 0;
-      while (gm >= p.ph_mt0[ph + 1]) ++ph;
-      const int g_begin = p.ph_g0[ph], g_end = p.ph_g0[ph + 1];
-      uint32_t scale_d = 0;
-      for (int c = 0; c < p.kchunks; ++c) {
-        const int kslices = (min(kTcKC, p.kg - c * kTcKC) + 15) >> 4;   // K = 16 slices holding real channels
-        for (int g = g_begin; g < g_end; ++g, ++it_a) {
-          const int sa = it_a % p.na_stages;
-          mbar_wait(&full_a[sa], (it_a / p.na_stages) & 1);
-          const uint32_t a16 = a_base16 + (uint32_t)sa * a_stage16;
-          for (int n = p.grp_first[g]; n < p.grp_first[g + 1]; ++n, ++it_b) {
-            int sb;
-            if (resident) {
-              sb = c * p.ntaps + n;
-              if (ti == 0) mbar_wait(&full_b[sb], 0u);
-            } else {
-              sb = it_b % p.nb_stages;
-              mbar_wait(&full_b[sb], (uint32_t)((it_b / p.nb_stages) & 1));
+      for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
+      int it_a = 0, it_b = 0, ti = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
+        const int gm = tile % mtiles, nt = (tile / mtiles) % p.ntiles, bb = tile / (mtiles * p.ntiles);
+        int ph = 0;
+        while (gm >= p.ph_mt0[ph + 1]) ++ph;
+        const int g_begin = p.ph_g0[ph], g_end = p.ph_g0[ph + 1];
+        uint32_t scale_d = 0;
+        for (int c = 0; c < p.kchunks; ++c) {
+          const int kslices = warp_uniform((min(kTcKC, p.kg - c * kTcKC) + 15) >> 4);   // K = 16 slices holding real channels
+          for (int g = g_begin; g < g_end; ++g, ++it_a) {
+            const int sa = it_a % p.na_stages;
+            mbar_wait(&full_a[sa], (it_a / p.na_stages) & 1);
+            const uint32_t a16 = a_base16 + (uint32_t)sa * a_stage16;
+            for (int n = p.grp_first[g]; n < p.grp_first[g + 1]; ++n, ++it_b) {
+              int sb;
+              if (resident) {
+                sb = c * p.ntaps + n;
+                if (ti == 0) mbar_wait(&full_b[sb], 0u);
+              } else {
+                sb = it_b % p.nb_stages;
+                mbar_wait(&full_b[sb], (uint32_t)((it_b / p.nb_stages) & 1));
+              }
+              const uint32_t a_hi = a16 + s_tapshift[n];
+              const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
+              wgmma_fence();
+              for (int ks = 0; ks < kslices; ++ks) {
+                wgmma_x3<NT, 0, 0>(acc, a_hi + 2u * ks, img16, b_hi + 2u * ks, bplane16, scale_d);
+                scale_d = 1;
+              }
+              wgmma_commit();
+              wgmma_wait<0>();
+              acc_fence(acc);
+              if (!resident && lane == 0) mbar_arrive(&empty_b[sb]);
             }
-            const uint32_t a_hi = a16 + s_tapshift[n];
-            const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
-            wgmma_fence();
-            for (int ks = 0; ks < kslices; ++ks) {
-              wgmma_x3<0, 0>(NT, acc, a_hi + 2u * ks, img16, b_hi + 2u * ks, bplane16, scale_d);
-              scale_d = 1;
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            acc_fence(acc);
-            if (!resident && lane == 0) mbar_arrive(&empty_b[sb]);
+            if (lane == 0) mbar_arrive(&empty_a[sa]);
           }
-          if (lane == 0) mbar_arrive(&empty_a[sa]);
         }
-      }
-      // ---- epilogue: registers -> bias / activation / residual (or act' mask for the data gradient) -> output rows
-      const int mt = gm - p.ph_mt0[ph];
-      const int F = p.ph_M[ph] * p.nsub;
-      const int c_tile = nt * p.n_stride;
-      const int n_valid = min(p.n_stride, p.c_out - c_tile);   // real output channels of this tile
-      const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
+        // ---- epilogue: registers -> bias / activation / residual (or act' mask for the data gradient) -> output rows
+        const int mt = gm - p.ph_mt0[ph];
+        const int F = p.ph_M[ph] * p.nsub;
+        const int c_tile = nt * p.n_stride;
+        const int n_valid = min(p.n_stride, p.c_out - c_tile);   // real output channels of this tile
+        const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int f = mt * kTcM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
-        if (f >= F) continue;
-        const int m = p.nsub == 1 ? f : f / p.nsub;
-        const int w = f - m * p.nsub;
-        const int to = p.ph_ooff[ph] + p.o_step * m;
-        const long long obase = ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
+        for (int h = 0; h < 2; ++h) {
+          const int f = mt * kTcM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+          if (f >= F) continue;
+          const int m = p.nsub == 1 ? f : f / p.nsub;
+          const int w = f - m * p.nsub;
+          const int to = p.ph_ooff[ph] + p.o_step * m;
+          const long long obase = ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
 #pragma unroll
-        for (int i = 0; i < kWgmmaMaxN / 8; ++i) {
-          const int col = i * 8 + 2 * (lane & 3);
-          if (i * 8 >= NT || col >= n_valid) continue;
-          float v[2] = {acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]};
-          const bool pair = vec2 && col + 1 < n_valid;
-          const int ne = col + 1 < n_valid ? 2 : 1;
-          float bia[2] = {0.f, 0.f}, sd[2] = {0.f, 0.f}, md[2] = {0.f, 0.f}, od[2] = {0.f, 0.f};
-          const long long o = obase + col;
-          if (pair) {
-            if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + c_tile + col)); bia[0] = t.x; bia[1] = t.y; }
-            if (p.mask.p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.mask.p + o)); md[0] = t.x; md[1] = t.y; }
-            if (p.resid) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.resid + o)); sd[0] = t.x; sd[1] = t.y; }
-            if (!SIMPLE && p.accumulate) { const float2 t = *reinterpret_cast<const float2*>(p.out + o); od[0] = t.x; od[1] = t.y; }
-          } else {
+          for (int i = 0; i < NT / 8; ++i) {
+            const int col = i * 8 + 2 * (lane & 3);
+            if (col >= n_valid) continue;
+            float v[2] = {acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]};
+            const bool pair = vec2 && col + 1 < n_valid;
+            const int ne = col + 1 < n_valid ? 2 : 1;
+            float bia[2] = {0.f, 0.f}, sd[2] = {0.f, 0.f}, md[2] = {0.f, 0.f}, od[2] = {0.f, 0.f};
+            const long long o = obase + col;
+            if (pair) {
+              if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + c_tile + col)); bia[0] = t.x; bia[1] = t.y; }
+              if (p.mask.p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.mask.p + o)); md[0] = t.x; md[1] = t.y; }
+              if (p.resid) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.resid + o)); sd[0] = t.x; sd[1] = t.y; }
+              if (!SIMPLE && p.accumulate) { const float2 t = *reinterpret_cast<const float2*>(p.out + o); od[0] = t.x; od[1] = t.y; }
+            } else {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                if (e >= ne) break;
+                if (p.bias) bia[e] = __ldg(p.bias + c_tile + col + e);
+                if (p.mask.p) md[e] = __ldg(p.mask.p + o + e);
+                if (p.resid) sd[e] = __ldg(p.resid + o + e);
+                if (!SIMPLE && p.accumulate) od[e] = p.out[o + e];
+              }
+            }
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              if (e >= ne) break;
-              if (p.bias) bia[e] = __ldg(p.bias + c_tile + col + e);
-              if (p.mask.p) md[e] = __ldg(p.mask.p + o + e);
-              if (p.resid) sd[e] = __ldg(p.resid + o + e);
-              if (!SIMPLE && p.accumulate) od[e] = p.out[o + e];
+              float x = v[e] + bia[e];
+              if (p.out_act == KT_ACT_LRELU) x = x > 0.f ? x : x * p.out_slope;
+              else if (!SIMPLE && p.out_act == KT_ACT_TANH) x = tanhf(x);
+              if (p.mask.p) x = side_apply(x, md[e], p.mask.mode, p.mask.slope);
+              x += sd[e] + od[e];
+              v[e] = x;
             }
-          }
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float x = v[e] + bia[e];
-            if (p.out_act == KT_ACT_LRELU) x = x > 0.f ? x : x * p.out_slope;
-            else if (!SIMPLE && p.out_act == KT_ACT_TANH) x = tanhf(x);
-            if (p.mask.p) x = side_apply(x, md[e], p.mask.mode, p.mask.slope);
-            x += sd[e] + od[e];
-            v[e] = x;
-          }
-          if (pair) *reinterpret_cast<float2*>(p.out + o) = make_float2(v[0], v[1]);
-          else {
-            p.out[o] = v[0];
-            if (ne == 2) p.out[o + 1] = v[1];
+            if (pair) *reinterpret_cast<float2*>(p.out + o) = make_float2(v[0], v[1]);
+            else {
+              p.out[o] = v[0];
+              if (ne == 2) p.out[o + 1] = v[1];
+            }
           }
         }
       }
-    }
+    });
   }
 }
 

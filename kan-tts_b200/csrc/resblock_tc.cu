@@ -119,10 +119,11 @@ constexpr int kRbConsumerBar = 1;        // named barrier of the 256 consumer th
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync %0, 256;" ::"n"(kRbConsumerBar) : "memory"); }
 
+// NT = C (32 or 64): the MMA width is a compile-time constant of each instance
+template <int NT>
 __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int NT = p.c;
   const int ximg = p.rows_x * 128, himg = p.rows_h * 128;            // one plane
   const int nslots = p.resident ? 2 * p.nsteps : p.nb;
   uint8_t* x_base = smem;                                            // nx stages x (hi | lo)
@@ -231,8 +232,11 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
     int it_w = 0;
     // one conv of one tile: A = image (hi plane at a16, lo plane a16 + plane16), taps = descriptor row shifts
+    // One MMA group stays in flight: a step's wait retires the PREVIOUS step, whose ring slot is then released.  (Draining
+    // every step instead -- wait<0> between the steps' wgmmas -- makes ptxas serialise every wgmma of the kernel, C7515.)
     auto run_conv = [&](int cv, uint32_t a16, uint32_t plane16, uint32_t astep, bool first_pass) {
       uint32_t scale_d = 0;
+      int held = -1;   // ring slot read by the group in flight
       for (int s = 0; s < p.nsteps; ++s, ++it_w) {
         int slot;
         if (p.resident) {
@@ -244,17 +248,20 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
         }
         const uint32_t a_hi = a16 + (uint32_t)s * astep;
         const uint32_t b_hi = w16 + (uint32_t)slot * tile16;
-        const int ks = (s == p.nsteps - 1) ? p.last_kslices : 4;
+        const int ks = warp_uniform((s == p.nsteps - 1) ? p.last_kslices : 4);
         wgmma_fence();
         for (int k = 0; k < ks; ++k) {
-          wgmma_x3<0, 0>(NT, acc, a_hi + 2u * k, plane16, b_hi + 2u * k, bplane16, scale_d);
+          wgmma_x3<NT, 0, 0>(acc, a_hi + 2u * k, plane16, b_hi + 2u * k, bplane16, scale_d);
           scale_d = 1;
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        acc_fence(acc);
-        if (!p.resident && lane == 0) mbar_arrive(&w_empty[slot]);
+        wgmma_wait<1>();
+        if (held >= 0 && lane == 0) mbar_arrive(&w_empty[held]);
+        held = p.resident ? -1 : slot;
       }
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (held >= 0 && lane == 0) mbar_arrive(&w_empty[held]);
     };
     for (int ti = 0; ti < ntile_cta; ++ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
@@ -436,13 +443,15 @@ int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, cons
   KT_REQUIRE(r == CUDA_SUCCESS, "resblock_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
   static std::atomic<bool> cfg{false};
   if (!cfg.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
     cfg.store(true, std::memory_order_release);
   }
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = std::min(p.total_tiles, sms > 0 ? sms : 132);
-  resblock_tc_kernel<<<grid, kRbThreads, pl.smem, st>>>(p);
+  if (p.c == 32) resblock_tc_kernel<32><<<grid, kRbThreads, pl.smem, st>>>(p);
+  else resblock_tc_kernel<64><<<grid, kRbThreads, pl.smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }

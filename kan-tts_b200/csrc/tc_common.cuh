@@ -109,13 +109,19 @@ __device__ __forceinline__ void acc_fence(float (&d)[kWgmmaMaxRegs]) {
 
 // split-bf16 ("bf16x3") product of one K = 16 slice: lo * hi + hi * lo + hi * hi into the accumulators
 // (a_hi / b_hi: descriptor low words of the hi planes, a_pl / b_pl: plane distances in 16-byte units)
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_x3(int n, float (&d)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t a_pl, uint32_t b_hi, uint32_t b_pl,
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_x3(float (&d)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t a_pl, uint32_t b_hi, uint32_t b_pl,
                                          uint32_t scale_d) {
-  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi + a_pl), desc_lo(b_hi), scale_d);
-  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi), desc_lo(b_hi + b_pl), 1u);
-  wgmma_bf16<TA, TB>(n, d, desc_lo(a_hi), desc_lo(b_hi), 1u);
+  wgmma_bf16_n<N, TA, TB>(d, desc_lo(a_hi + a_pl), desc_lo(b_hi), scale_d);
+  wgmma_bf16_n<N, TA, TB>(d, desc_lo(a_hi), desc_lo(b_hi + b_pl), 1u);
+  wgmma_bf16_n<N, TA, TB>(d, desc_lo(a_hi), desc_lo(b_hi), 1u);
 }
+
+// A value every lane of the warp already holds, in a form ptxas can prove warp-uniform.  ptxas serialises EVERY wgmma of a
+// kernel (a wait for completion after each one; ptxas info C7520) when it cannot prove that all threads run the same
+// number of them, and it cannot for a loop bound derived from the counter of a loop that waits on an mbarrier: the MMA
+// loops take such trip counts through this.
+__device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // byte offset of 16-byte chunk `q` (0..7) of row `r` inside a 1024-byte-aligned SWIZZLE_128B image
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t q) { return r * 128u + ((q ^ (r & 7u)) << 4); }

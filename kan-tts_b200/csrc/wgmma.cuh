@@ -4,6 +4,8 @@
 #pragma once
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace kt {
 namespace tc {
 
@@ -72,18 +74,19 @@ __device__ __forceinline__ void wgmma_bf16_n(float (&d)[kWgmmaMaxRegs], uint64_t
   else wgmma_n128<TA, TB, O>(d, da, db, scale_d);
 }
 
-// N = 16, 32, ..., 128 chosen at run time; the accumulator array is always indexed with constants (registers)
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_bf16(int n, float (&d)[kWgmmaMaxRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+// f(std::integral_constant<int, N>{}) for the run-time tile width n = 16, 32, ..., 128: a kernel selects N ONCE and runs
+// a main loop compiled for that N (a switch over N around every wgmma costs a warpgroup.arrive per wgmma)
+template <typename F>
+__device__ __forceinline__ void with_wgmma_n(int n, F&& f) {
   switch (n) {
-    case 16: wgmma_n16<TA, TB>(d, da, db, scale_d); break;
-    case 32: wgmma_n32<TA, TB>(d, da, db, scale_d); break;
-    case 48: wgmma_n48<TA, TB>(d, da, db, scale_d); break;
-    case 64: wgmma_n64<TA, TB>(d, da, db, scale_d); break;
-    case 80: wgmma_n80<TA, TB>(d, da, db, scale_d); break;
-    case 96: wgmma_n96<TA, TB>(d, da, db, scale_d); break;
-    case 112: wgmma_n112<TA, TB>(d, da, db, scale_d); break;
-    case 128: wgmma_n128<TA, TB>(d, da, db, scale_d); break;
+    case 16: f(std::integral_constant<int, 16>{}); break;
+    case 32: f(std::integral_constant<int, 32>{}); break;
+    case 48: f(std::integral_constant<int, 48>{}); break;
+    case 64: f(std::integral_constant<int, 64>{}); break;
+    case 80: f(std::integral_constant<int, 80>{}); break;
+    case 96: f(std::integral_constant<int, 96>{}); break;
+    case 112: f(std::integral_constant<int, 112>{}); break;
+    case 128: f(std::integral_constant<int, 128>{}); break;
     default: __trap();
   }
 }

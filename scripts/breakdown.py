@@ -26,5 +26,11 @@ by = prof.by_layer()
 ops.set_profiler(False)
 tot = sum(v[1] for v in by.values())
 print(f"instrumented total {tot:.2f} ms")
+classes = {}
+for (name, _), (calls, ms, flops) in by.items():
+    c = classes.setdefault(name, [0, 0.0, 0.0])
+    c[0] += calls; c[1] += ms; c[2] += flops
+for name, (calls, ms, flops) in sorted(classes.items(), key=lambda kv: -kv[1][1]):
+    print(f"class {name:16s} {ms:8.3f} ms {100*ms/tot:5.1f}% x{calls:4d} {flops/ms/1e9 if ms else 0:7.1f} TF/s")
 for (name, det), (calls, ms, flops) in sorted(by.items(), key=lambda kv: -kv[1][1])[:140]:
     print(f"{ms:8.3f} ms {100*ms/tot:5.1f}% x{calls:3d} {flops/ms/1e9 if ms else 0:7.1f} TF/s  {name:16s} {det}")

@@ -19,6 +19,13 @@ LAYERS = {
     "msd_1024_1024_k5": (dict(c_in=1024, c_out=1024, kernel=5, pad_left=2, pad_right=2), 16, 33, 0),
     "gen_128_128_k11": (dict(c_in=128, c_out=128, kernel=11, pad_left=10, pad_right=0), 16, 2048, 0),
     "gen_32_32_k7": (dict(c_in=32, c_out=32, kernel=7, pad_left=6, pad_right=0), 16, 8192, 0),
+    # one shape per MMA tile width N: 16 (single-channel output; the data gradient of a 1-channel input layer),
+    # 32 / 64 (generator stages 4 / 3), 64 (N split of a 256-channel layer with 32 M tiles; grouped k41), 128 (above)
+    "msd_post_1024_1_k3": (dict(c_in=1024, c_out=1, kernel=3, pad_left=1, pad_right=1), 16, 33, 0),
+    "msd_pre_1_128_k15": (dict(c_in=1, c_out=128, kernel=15, pad_left=7, pad_right=7), 16, 8192, 0),
+    "gen_64_64_k7": (dict(c_in=64, c_out=64, kernel=7, pad_left=6, pad_right=0), 16, 4096, 0),
+    "gen_256_256_k11": (dict(c_in=256, c_out=256, kernel=11, pad_left=10, pad_right=0), 16, 256, 0),
+    "msd_128_128_k41_g4_s4": (dict(c_in=128, c_out=128, kernel=41, stride=4, groups=4, pad_left=20, pad_right=20), 16, 8192, 0),
     "sambert_ffn_128_1024_k3": (dict(c_in=128, c_out=1024, kernel=3, pad_left=1, pad_right=1), 32, 256, 0),
     "sambert_ffn_1024_128_k1": (dict(c_in=1024, c_out=128, kernel=1), 32, 256, 0),
 }
