@@ -4,17 +4,20 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
+
 #include "../../include/kantts_b200.h"
 
 namespace kt {
 
 void set_error(const char* fmt, ...);
 
-#define KT_CHECK_CUDA(expr)                                                          \
+// variadic: the expression may contain a template-id with commas (allow_dyn_smem<kernel<A, B>>(...))
+#define KT_CHECK_CUDA(...)                                                           \
   do {                                                                               \
-    cudaError_t _e = (expr);                                                         \
+    cudaError_t _e = (__VA_ARGS__);                                                  \
     if (_e != cudaSuccess) {                                                         \
-      kt::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
+      kt::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #__VA_ARGS__, cudaGetErrorString(_e)); \
       return KT_ERR_CUDA;                                                            \
     }                                                                                \
   } while (0)
@@ -28,6 +31,33 @@ void set_error(const char* fmt, ...);
   } while (0)
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// SMs of the current device, queried once per process; 132 (an H100) without a device, so that the host-logic tests plan
+// for an H100.  A failed query's error is cleared: a later cudaGetLastError() must not report it as a launch failure.
+inline int device_sm_count() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) {
+      cudaGetLastError();
+      v = 132;
+    }
+    return v;
+  }();
+  return n;
+}
+
+// Allow launches of `Kernel` with up to `bytes` of dynamic shared memory (use: KT_CHECK_CUDA(allow_dyn_smem<k>(bytes))
+// before the launch).  The attribute belongs to the function, so it is set once per process per kernel instance and never
+// lowered later.  A caller returns only after the attribute is set (concurrent first callers each set the same value);
+// a failed call is returned and retried by the next caller.
+template <auto Kernel>
+cudaError_t allow_dyn_smem(int bytes) {
+  static std::atomic<bool> done{false};
+  if (done.load(std::memory_order_acquire)) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) done.store(true, std::memory_order_release);
+  return e;
+}
 
 // floor division for b > 0
 __host__ __device__ inline int fdiv(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }

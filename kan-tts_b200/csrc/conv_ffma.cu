@@ -25,7 +25,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <atomic>
 #include <vector>
 
 #include "common.cuh"
@@ -232,13 +231,7 @@ static int launch_core(const CoreParams& p, cudaStream_t st) {
   constexpr int TN = 32 * RN, TM = 8 * RM, NTC = 4;
   const size_t smem = ((size_t)p.rmax * KC + (size_t)NTC * KC * TN) * sizeof(float);
   KT_REQUIRE(smem <= 200 * 1024, "conv_core: activation tile too large (%zu bytes shared)", smem);
-  // opt in ONCE per process to the full 227 KB (the attribute is per function, not per thread: a
-  // smaller value set later from the autograd thread would make larger launches fail)
-  static std::atomic<bool> configured{false};
-  if (!configured.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(conv_core_kernel<RN, RM, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    configured.store(true, std::memory_order_release);
-  }
+  KT_CHECK_CUDA(allow_dyn_smem<conv_core_kernel<RN, RM, KC>>(kMaxDynSmem));
   dim3 grid(ceil_div(p.ph.M, TM), p.groups * ceil_div(p.cout_g, TN), p.batch);
   conv_core_kernel<RN, RM, KC><<<grid, 256, smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
@@ -489,11 +482,7 @@ static int launch_wgrad(WgradParams p, cudaStream_t st) {
   p.nsplit = (int)nsplit;
   const size_t smem = ((size_t)p.rmax * TCA + (size_t)TK * TN) * sizeof(float);
   KT_REQUIRE(smem <= 200 * 1024, "conv_wgrad: tile too large (%zu bytes shared)", smem);
-  static std::atomic<bool> configured{false};
-  if (!configured.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<RN, RMA, SPLITM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    configured.store(true, std::memory_order_release);
-  }
+  KT_CHECK_CUDA(allow_dyn_smem<conv_wgrad_kernel<RN, RMA, SPLITM>>(kMaxDynSmem));
   dim3 grid(ceil_div(p.ca_g, TCA), p.groups * ceil_div(p.cb_g, TN), p.npass * p.nsplit);
   float* out = p.g;
   float* part = nullptr;

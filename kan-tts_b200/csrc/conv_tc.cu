@@ -20,7 +20,6 @@
 //              register accumulators, then the epilogue of their 64 rows: bias / activation / residual (or act'
 //              mask for the data gradient), stores to the channels-last output.
 #include <algorithm>
-#include <atomic>
 #include <cstdlib>
 #include <vector>
 
@@ -137,9 +136,7 @@ constexpr int kTcConsumerArrivals = 8;   // one per consumer warp
 template <bool SIMPLE>
 __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve-up (all image / tile bases 1024-byte aligned)
-  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space)
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_align_1024(smem_raw);          // carve-up: all image / tile bases 1024-byte aligned
   const int img_bytes = p.rows * 128;                 // one plane of one activation stage
   const int a_stage_bytes = 2 * img_bytes;            // hi + lo
   const int b_stage_bytes = 2 * p.NT * 128;           // hi + lo weight tile
@@ -169,7 +166,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   if (warp < 4) {
     // ===================== activation producers =====================
     const int ptid = tid;
-    int it = 0;
+    RingPos ra;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int gm = tile % mtiles, bb = tile / (mtiles * p.ntiles);
       int ph = 0;
@@ -177,9 +174,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       const int ch_base = p.grouped ? ((tile / mtiles) % p.ntiles) * p.kg : 0;
       const int f0 = (gm - p.ph_mt0[ph]) * kTcM;
       for (int c = 0; c < p.kchunks; ++c) {
-        for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ++it) {
-          const int s = it % p.na_stages;
-          mbar_wait(&empty_a[s], ((it / p.na_stages) & 1) ^ 1);
+        for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ra.advance(p.na_stages)) {
+          const int s = ra.slot();
+          mbar_wait(&empty_a[s], ra.phase() ^ 1u);
           uint8_t* img_hi = a_base + (size_t)s * a_stage_bytes;
           RowMap rm;
           rm.base_row = (long long)bb * p.t_in * p.nsub;
@@ -208,16 +205,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         for (int s = 0; s < p.nb_stages; ++s) mbar_wait(&full_b[s], 0);   // no bulk copy may outlive the CTA
       }
     } else if (leader) {
-      int it = 0;
+      RingPos rb;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = (tile / mtiles) % p.ntiles;
         int ph = 0;
         while ((tile % mtiles) >= p.ph_mt0[ph + 1]) ++ph;
         const int n_begin = p.grp_first[p.ph_g0[ph]], n_end = p.grp_first[p.ph_g0[ph + 1]];
         for (int c = 0; c < p.kchunks; ++c) {
-          for (int n = n_begin; n < n_end; ++n, ++it) {  // taps are ordered by group: same order as the consumers
-            const int s = it % p.nb_stages;
-            mbar_wait(&empty_b[s], ((it / p.nb_stages) & 1) ^ 1);
+          for (int n = n_begin; n < n_end; ++n, rb.advance(p.nb_stages)) {  // taps are ordered by group: same order as the consumers
+            const int s = rb.slot();
+            mbar_wait(&empty_b[s], rb.phase() ^ 1u);
             const long long block = ((long long)p.tap_j[n] * p.kchunks + c) * p.ntiles + nt;
             const uint8_t* src = reinterpret_cast<const uint8_t*>(p.wimg) + block * (long long)b_stage_bytes;
             mbar_arrive_expect_tx(&full_b[s], (uint32_t)b_stage_bytes);
@@ -244,7 +241,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       float acc[kWgmmaMaxRegs];
 #pragma unroll
       for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
-      int it_a = 0, it_b = 0, ti = 0;
+      RingPos ra, rb;
+      int ti = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
         const int gm = tile % mtiles, nt = (tile / mtiles) % p.ntiles, bb = tile / (mtiles * p.ntiles);
         int ph = 0;
@@ -253,18 +251,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         uint32_t scale_d = 0;
         for (int c = 0; c < p.kchunks; ++c) {
           const int kslices = warp_uniform((min(kTcKC, p.kg - c * kTcKC) + 15) >> 4);   // K = 16 slices holding real channels
-          for (int g = g_begin; g < g_end; ++g, ++it_a) {
-            const int sa = it_a % p.na_stages;
-            mbar_wait(&full_a[sa], (it_a / p.na_stages) & 1);
+          for (int g = g_begin; g < g_end; ++g, ra.advance(p.na_stages)) {
+            const int sa = ra.slot();
+            mbar_wait(&full_a[sa], ra.phase());
             const uint32_t a16 = a_base16 + (uint32_t)sa * a_stage16;
-            for (int n = p.grp_first[g]; n < p.grp_first[g + 1]; ++n, ++it_b) {
+            for (int n = p.grp_first[g]; n < p.grp_first[g + 1]; ++n) {
               int sb;
               if (resident) {
                 sb = c * p.ntaps + n;
                 if (ti == 0) mbar_wait(&full_b[sb], 0u);
               } else {
-                sb = it_b % p.nb_stages;
-                mbar_wait(&full_b[sb], (uint32_t)((it_b / p.nb_stages) & 1));
+                sb = rb.slot();
+                mbar_wait(&full_b[sb], rb.phase());
+                rb.advance(p.nb_stages);
               }
               const uint32_t a_hi = a16 + s_tapshift[n];
               const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
@@ -359,8 +358,6 @@ struct TcParams;
 
 // shared memory outside the activation / weight stages: barriers and the tap-shift table (see the carve-up in conv_tc_kernel)
 static int tc_fixed_smem(int slots) { return (2 * 3 + 2 * std::max(6, slots)) * 8 + kMaxTaps * 4; }
-
-static int sm_count();
 
 static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
   TcLayerPlan L{};
@@ -496,15 +493,6 @@ int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cud
   return KT_OK;
 }
 
-static int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-  }
-  return n;
-}
-
 static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned by plan_launches
   const int a_stage = 2 * p.rows * 128;
   const int b_stage = 2 * p.NT * 128;
@@ -528,13 +516,9 @@ static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned 
   }
   KT_REQUIRE(p.nb_stages >= 2 || p.w_resident, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
   const size_t smem = 1024 + (size_t)p.na_stages * a_stage + (size_t)p.nb_stages * b_stage + bar_bytes;
-  static std::atomic<bool> cfg{false};
-  if (!cfg.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    KT_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    cfg.store(true, std::memory_order_release);
-  }
-  const int grid = (int)std::min<long long>(tiles, sm_count());
+  KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<true>>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<false>>(kMaxDynSmem));
+  const int grid = (int)std::min<long long>(tiles, device_sm_count());
   const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
                       (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
                       (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);

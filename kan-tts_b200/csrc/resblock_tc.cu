@@ -17,7 +17,6 @@
 // Warp roles: see resblock_tc_kernel.
 
 #include <algorithm>
-#include <atomic>
 #include <vector>
 
 #include "common.cuh"
@@ -77,15 +76,6 @@ __global__ void rb_pack_pair_kernel(const float* __restrict__ w, int k, int npai
   }
 }
 
-// ---- TMA: one box (32 channels x rows) of the 3-D tensor (C, T, B) -> shared memory, completion on an mbarrier (SASS UTMALDG)
-__device__ __forceinline__ void tma_load_box(void* dst_smem, const CUtensorMap* map, int c0, int t0, int b, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-          smem_u32(dst_smem)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(t0), "r"(b)
-      : "memory");
-}
-
 // ---- shared fp32 landing tile -> split-bf16 SWIZZLE_128B image (fused LeakyReLU), rows [r_begin, r_end), 128 threads.
 // ft: boxes of [rows_box][32 floats] (128-byte rows, linear).  PAIR (C = 32): image row r = [x[r] | x[r + d]];
 // else (C = 64): image row r = channels 0..63 of row r, box q / 4.  Rows outside [0, T) arrive as zeros.
@@ -123,7 +113,7 @@ __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync %0, 256
 template <int NT>
 __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_align_1024(smem_raw);
   const int ximg = p.rows_x * 128, himg = p.rows_h * 128;            // one plane
   const int nslots = p.resident ? 2 * p.nsteps : p.nb;
   uint8_t* x_base = smem;                                            // nx stages x (hi | lo)
@@ -164,21 +154,21 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
     const int ptid = tid;
     const int r0 = 0, r1 = p.rows_x;
     const int nbox = p.c / 32, box_floats = p.rows_box * 32;
-    auto issue = [&](int ti) {
+    auto issue = [&](int ti, int s) {   // tile ti of this CTA -> landing stage s
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
       const int x0 = it * p.to - p.p2 - p.p1;
-      const int s = ti % p.nx;
       mbar_arrive_expect_tx(&f_full[s], (uint32_t)p.fstage_bytes);
       for (int bx = 0; bx < nbox; ++bx)
-        tma_load_box(f_base + (size_t)s * p.fstage_bytes + (size_t)bx * box_floats * 4, &p.tmx, bx * 32, x0, bb, &f_full[s]);
+        tma_load_3d(f_base + (size_t)s * p.fstage_bytes + (size_t)bx * box_floats * 4, &p.tmx, bx * 32, x0, bb, &f_full[s]);
     };
     if (ptid == 0)
-      for (int ti = 0; ti < min(p.nx, ntile_cta); ++ti) issue(ti);
-    for (int ti = 0; ti < ntile_cta; ++ti) {
-      const int s = ti % p.nx, n = ti / p.nx;
-      mbar_wait(&x_empty[s], (uint32_t)((n & 1) ^ 1));
-      mbar_wait(&f_full[s], (uint32_t)(n & 1));
+      for (int ti = 0; ti < min(p.nx, ntile_cta); ++ti) issue(ti, ti);
+    RingPos rx;
+    for (int ti = 0; ti < ntile_cta; ++ti, rx.advance(p.nx)) {
+      const int s = rx.slot();
+      mbar_wait(&x_empty[s], rx.phase() ^ 1u);
+      mbar_wait(&f_full[s], rx.phase());
       uint8_t* img_hi = x_base + (size_t)s * 2 * ximg;
       const float* ft = reinterpret_cast<const float*>(f_base + (size_t)s * p.fstage_bytes);
       if (p.pair) rb_convert_tile<true>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
@@ -186,7 +176,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
       fence_proxy_async();
       mbar_arrive(&x_full[s]);
       asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
-      if (ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx);
+      if (ptid == 0 && ti + p.nx < ntile_cta) issue(ti + p.nx, s);
     }
   } else if (warp == 12) {
     // ===================== weight stream =====================
@@ -200,11 +190,11 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
         for (int s = 0; s < 2 * p.nsteps; ++s) mbar_wait(&w_full[s], 0);   // no bulk copy may outlive the CTA
       } else {
         // same job order as the consumers: per tile c1, c2
-        int it = 0;
+        RingPos rw;
         auto stream_conv = [&](const __nv_bfloat16* w) {
-          for (int s = 0; s < p.nsteps; ++s, ++it) {
-            const int slot = it % p.nb;
-            mbar_wait(&w_empty[slot], (uint32_t)(((it / p.nb) & 1) ^ 1));
+          for (int s = 0; s < p.nsteps; ++s, rw.advance(p.nb)) {
+            const int slot = rw.slot();
+            mbar_wait(&w_empty[slot], rw.phase() ^ 1u);
             mbar_arrive_expect_tx(&w_full[slot], (uint32_t)p.tile_bytes);
             bulk_g2s(w_base + (size_t)slot * p.tile_bytes, reinterpret_cast<const uint8_t*>(w) + (size_t)s * p.tile_bytes,
                      (uint32_t)p.tile_bytes, &w_full[slot]);
@@ -230,21 +220,22 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
     float acc[kWgmmaMaxRegs];
 #pragma unroll
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
-    int it_w = 0;
+    RingPos rw;   // weight ring (not used with resident weights)
     // one conv of one tile: A = image (hi plane at a16, lo plane a16 + plane16), taps = descriptor row shifts
     // One MMA group stays in flight: a step's wait retires the PREVIOUS step, whose ring slot is then released.  (Draining
     // every step instead -- wait<0> between the steps' wgmmas -- makes ptxas serialise every wgmma of the kernel, C7515.)
     auto run_conv = [&](int cv, uint32_t a16, uint32_t plane16, uint32_t astep, bool first_pass) {
       uint32_t scale_d = 0;
       int held = -1;   // ring slot read by the group in flight
-      for (int s = 0; s < p.nsteps; ++s, ++it_w) {
+      for (int s = 0; s < p.nsteps; ++s) {
         int slot;
         if (p.resident) {
           slot = cv * p.nsteps + s;
           if (first_pass) mbar_wait(&w_full[slot], 0u);
         } else {
-          slot = it_w % p.nb;
-          mbar_wait(&w_full[slot], (uint32_t)((it_w / p.nb) & 1));
+          slot = rw.slot();
+          mbar_wait(&w_full[slot], rw.phase());
+          rw.advance(p.nb);
         }
         const uint32_t a_hi = a16 + (uint32_t)s * astep;
         const uint32_t b_hi = w16 + (uint32_t)slot * tile16;
@@ -263,12 +254,13 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
       acc_fence(acc);
       if (held >= 0 && lane == 0) mbar_arrive(&w_empty[held]);
     };
-    for (int ti = 0; ti < ntile_cta; ++ti) {
+    RingPos rx;
+    for (int ti = 0; ti < ntile_cta; ++ti, rx.advance(p.nx)) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
-      const int s = ti % p.nx, n = ti / p.nx;
+      const int s = rx.slot();
       // ---------- c1 ----------
-      mbar_wait(&x_full[s], (uint32_t)(n & 1));
+      mbar_wait(&x_full[s], rx.phase());
       run_conv(0, x16 + (uint32_t)s * 2u * ximg16 + half16, ximg16, step1, ti == 0);
       if (lane == 0) mbar_arrive(&x_empty[s]);
       // ---------- epilogue 1: h = acc + b1 -> [global] -> lrelu -> split -> H image ----------
@@ -428,7 +420,6 @@ int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, cons
   RbPlan pl = rb_plan(d);
   KT_REQUIRE(pl.ok, "resblock_fwd: shape not supported by the fused kernel (see kt_resblock_plan)");
   KT_REQUIRE(x && img1 && img2 && y, "resblock_fwd: null pointer");
-  KT_REQUIRE(encode_tiled_fn() != nullptr, "resblock_fwd: the driver provides no cuTensorMapEncodeTiled");
   RbParams& p = pl.p;
   p.x = x; p.y = y; p.h = h;
   p.w1 = reinterpret_cast<const __nv_bfloat16*>(img1); p.w2 = reinterpret_cast<const __nv_bfloat16*>(img2);
@@ -436,20 +427,12 @@ int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, cons
   const cuuint64_t gdim[3] = {(cuuint64_t)p.c, (cuuint64_t)p.t, (cuuint64_t)p.batch};
   const cuuint64_t gstr[2] = {(cuuint64_t)p.c * 4, (cuuint64_t)p.t * p.c * 4};
   const cuuint32_t box[3] = {32, (cuuint32_t)p.rows_box, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const CUresult r = encode_tiled_fn()(&p.tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
-                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  KT_REQUIRE(r == CUDA_SUCCESS, "resblock_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
-  static std::atomic<bool> cfg{false};
-  if (!cfg.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    KT_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    cfg.store(true, std::memory_order_release);
-  }
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = std::min(p.total_tiles, sms > 0 ? sms : 132);
+  const int rc = encode_tensor_map(&p.tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, x, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "resblock_fwd");
+  if (rc) return rc;
+  KT_CHECK_CUDA(allow_dyn_smem<resblock_tc_kernel<32>>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<resblock_tc_kernel<64>>(kMaxDynSmem));
+  const int grid = std::min(p.total_tiles, device_sm_count());
   if (p.c == 32) resblock_tc_kernel<32><<<grid, kRbThreads, pl.smem, st>>>(p);
   else resblock_tc_kernel<64><<<grid, kRbThreads, pl.smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());

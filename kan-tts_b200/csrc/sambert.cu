@@ -7,7 +7,6 @@
 // Everything here is exact fp32 on CUDA cores: with d_head = 16 (sambert_24k.yaml) one attention head is a
 // K=16 contraction -- a single wgmma k-step -- and the kernels are bound by the probability-matrix
 // traffic (B*H*Lq*Lk*4 bytes written in forward, read twice in backward), not by math.
-#include <atomic>
 #include <type_traits>
 
 #include "common.cuh"
@@ -173,9 +172,7 @@ template <int NC>
 static int ln_bwd_launch(const float* dy, const float* x, const float* g, const float* mean, const float* rstd,
                          float* dx, float* ws, int rows, int c, int grid, cudaStream_t st) {
   const size_t smem = (size_t)8 * 2 * c * sizeof(float);   // up to 64 KB at C = 1024: above the 48 KB default
-  static std::atomic<bool> attr_set{false};
-  if (smem > 48 * 1024 && !attr_set.exchange(true))
-    KT_CHECK_CUDA(cudaFuncSetAttribute(layernorm_bwd_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  if (smem > 48 * 1024) KT_CHECK_CUDA(allow_dyn_smem<layernorm_bwd_kernel<NC>>(64 * 1024));
   layernorm_bwd_kernel<NC><<<grid, 256, smem, st>>>(dy, x, g, mean, rstd, dx, ws, rows, c);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
@@ -593,9 +590,7 @@ static int attn_fwd_launch(const KtAttnDesc* d, const AttnArgs& a, cudaStream_t 
   constexpr int QT = 8 * RW;
   const size_t smem = ((size_t)QT * d->lk + (size_t)kKeyTile * (D + 4)) * sizeof(float);
   KT_REQUIRE(smem <= (size_t)kMaxDynSmem, "attention: shared memory budget exceeded (Lk too long)");
-  static std::atomic<bool> attr_set{false};
-  if (!attr_set.exchange(true))
-    KT_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, RW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<attn_fwd_kernel<D, RW>>(kMaxDynSmem));
   dim3 grid((d->lq + QT - 1) / QT, d->heads * d->batch);
   attn_fwd_kernel<D, RW><<<grid, 256, smem, st>>>(a);
   KT_CHECK_CUDA(cudaGetLastError());
@@ -630,9 +625,7 @@ static int attn_bwd_launch(const KtAttnDesc* d, const AttnBwdArgs& a, cudaStream
   constexpr int QT = 8 * RW;
   const size_t smem = ((size_t)QT * d->lk + (size_t)kKeyTile * (D + 4)) * sizeof(float);
   KT_REQUIRE(smem <= (size_t)kMaxDynSmem, "attention: shared memory budget exceeded (Lk too long)");
-  static std::atomic<bool> attr_set{false};
-  if (!attr_set.exchange(true))
-    KT_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_q_kernel<D, RW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<attn_bwd_q_kernel<D, RW>>(kMaxDynSmem));
   dim3 gq((d->lq + QT - 1) / QT, d->heads * d->batch);
   attn_bwd_q_kernel<D, RW><<<gq, 256, smem, st>>>(a);
   KT_CHECK_CUDA(cudaGetLastError());
@@ -792,9 +785,7 @@ static int fsmn_fir_launch(const float* x, const float* w, const unsigned char* 
                            int K, int lp, int reverse, cudaStream_t st) {
   const size_t smem = ((size_t)(kFsT + K - 1) * kFsC + (size_t)K * kFsC) * sizeof(float);
   KT_REQUIRE(K <= 256 && B <= 65535, "fsmn: need K <= 256, B <= 65535");
-  static std::atomic<bool> attr_set{false};
-  if (!attr_set.exchange(true))
-    KT_CHECK_CUDA(cudaFuncSetAttribute(fsmn_fir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<fsmn_fir_kernel>(kMaxDynSmem));
   dim3 grid((T + kFsT - 1) / kFsT, (C + kFsC - 1) / kFsC, B);
   fsmn_fir_kernel<<<grid, 256, smem, st>>>(x, w, mask, y, T, C, K, lp, reverse);
   KT_CHECK_CUDA(cudaGetLastError());
@@ -811,9 +802,7 @@ template <int TJ>
 static int fsmn_wgrad_launch(const float* x, const float* dy, const unsigned char* mask, float* ws, int B, int T, int C,
                              int K, int lp, int cpb, cudaStream_t st) {
   const size_t smem = ((size_t)(kFsT + 4 * TJ - 1) * kFsC + (size_t)kFsT * kFsC) * sizeof(float);
-  static std::atomic<bool> attr_set{false};
-  if (!attr_set.exchange(true))
-    KT_CHECK_CUDA(cudaFuncSetAttribute(fsmn_bwd_weight_kernel<TJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<fsmn_bwd_weight_kernel<TJ>>(kMaxDynSmem));
   fsmn_bwd_weight_kernel<TJ><<<dim3((C + kFsC - 1) / kFsC, B * cpb), 256, smem, st>>>(x, dy, mask, ws, T, C, K, lp, cpb);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;

@@ -194,8 +194,7 @@ int stft_mel_fwd(const KtMelDesc* d, const float* wav, const float* window, cons
   if (rc) return rc;
   KT_REQUIRE(wav && window && (!mel || melmat), "stft_mel_fwd: null argument");
   const size_t smem = (2 * (size_t)p.n_fft + p.n_fft / 2 + 1) * sizeof(float);
-  static bool cfg = false;
-  if (!cfg) { KT_CHECK_CUDA(cudaFuncSetAttribute(stft_mel_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); cfg = true; }
+  KT_CHECK_CUDA(allow_dyn_smem<stft_mel_fwd_kernel>(64 * 1024));
   stft_mel_fwd_kernel<<<p.batch * p.frames, 256, smem, st>>>(p, wav, window, melmat, mel, amp, spec);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
@@ -208,8 +207,7 @@ int stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, const
   if (rc) return rc;
   KT_REQUIRE(spec && window && dwav && (dmel || damp) && (!dmel || melmat), "stft_mel_bwd: null argument");
   const size_t smem = (2 * (size_t)p.n_fft + p.n_fft / 2 + 1 + p.n_mels) * sizeof(float);
-  static bool cfg = false;
-  if (!cfg) { KT_CHECK_CUDA(cudaFuncSetAttribute(stft_mel_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); cfg = true; }
+  KT_CHECK_CUDA(allow_dyn_smem<stft_mel_bwd_kernel>(64 * 1024));
   float* frame_grad = nullptr;
   rc = scratch_alloc(&frame_grad, (long long)p.batch * p.frames * p.n_fft, st);
   if (rc) return rc;

@@ -38,17 +38,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // Bounded wait: a protocol bug must surface as a trap (launch error), never as a hung GPU.  The try_wait carries CUTLASS's
 // suspend-time hint (the hardware parks the warp instead of polling) and the loop must NOT be unrolled: nvcc unrolled it
 // 64x at every call site (~2 KB of SASS each, ~15 sites per kernel), and four concurrently running warp roles were
@@ -68,6 +57,26 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (ok) return;
   }
   __trap();
+}
+
+// Position in a ring of `n` stages, each with a "full" and an "empty" mbarrier: the slot and the parity of its current
+// pass.  A consumer waits on full[slot()] with phase(), a producer on empty[slot()] with phase() ^ 1 (the first pass
+// finds every slot empty).  Stage counts are run-time values: advance() wraps without a division.  Both live in one
+// register, as the loop counter they replace did: conv_tc_kernel's consumers are at the 128-register cap.
+struct RingPos {
+  uint32_t v = 0;   // slot << 1 | phase
+  __device__ __forceinline__ int slot() const { return (int)(v >> 1); }
+  __device__ __forceinline__ uint32_t phase() const { return v & 1u; }
+  __device__ __forceinline__ void advance(int n) {
+    v += 2u;
+    if (v >> 1 == (uint32_t)n) v = (v & 1u) ^ 1u;
+  }
+};
+
+// The dynamic shared-memory base rounded up to 1024 bytes: every SWIZZLE_128B image and tile base must be 1024-byte aligned.
+// (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space)
+__device__ __forceinline__ uint8_t* smem_align_1024(uint8_t* smem_raw) {
+  return smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
 }
 
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / bulk copies)

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
+
 namespace kt {
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -19,6 +21,21 @@ inline EncodeTiledFn encode_tiled_fn() {
     return reinterpret_cast<EncodeTiledFn>(f);
   }();
   return fn;
+}
+
+// Tiled tensor map of a `rank`-D tensor (rank <= 5): dims and box innermost first, `strides` = byte strides of dims
+// 1 .. rank - 1, unit element strides, no interleave; elements outside the tensor arrive as zeros.  `what` prefixes the
+// error message.
+inline int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                             const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle,
+                             CUtensorMapL2promotion l2, const char* what) {
+  const EncodeTiledFn fn = encode_tiled_fn();
+  KT_REQUIRE(fn != nullptr, "%s: the driver provides no cuTensorMapEncodeTiled", what);
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  KT_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed (%d)", what, (int)r);
+  return KT_OK;
 }
 
 namespace tc {
@@ -39,16 +56,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst_smem, const CUtensorMap* m
                "l"(map), "r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
-// one 3-D box shared -> global (SASS UTMASTG), bulk async-group completion; elements outside the tensor are not written
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src_smem, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map),
-               "r"((uint32_t)__cvta_generic_to_shared(src_smem)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all but the N most recent bulk groups of this thread have finished READING their shared-memory source
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
 }  // namespace tc
 }  // namespace kt

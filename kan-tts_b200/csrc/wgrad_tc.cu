@@ -15,7 +15,6 @@
 // columns) for a slice of the (batch, flattened time) range (split-K); partial tiles go to a workspace
 // with plain stores and a second kernel reduces over the splits in order (deterministic, and cheaper than ~10^7 atomics).
 #include <algorithm>
-#include <atomic>
 #include <vector>
 
 #include "common.cuh"
@@ -151,8 +150,7 @@ constexpr int kWgThreads = 512;
 template <int NT>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // (pointer arithmetic on the __shared__ array, not integer casts: the compiler must keep the shared address space)
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_align_1024(smem_raw);
   const int img_a = p.rows_a * 128;            // one plane of one A image
   const int img_b = kWgTK * 128;               // one plane of one B image
   const int stage_bytes = 2 * (p.a_groups * img_a + p.b_groups * img_b);
@@ -296,7 +294,7 @@ __global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16* __res
 template <int NT>
 __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __grid_constant__ WgTcParams p, const __grid_constant__ WgTmaExtra x) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_align_1024(smem_raw);
   const int img_a = x.rows_a_p * 128;          // one plane of one A image
   const int img_b = x.Rp * 128;                // one plane of one B image
   const int stage_bytes = 2 * (p.a_groups * img_a + p.b_groups * img_b);
@@ -346,10 +344,10 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
       const CUtensorMap* ma = &x.map_a[p.grp_rho[grp]];
       const int ca0 = cgrp * p.ca_g + ca_tile * (p.mode == 0 ? 128 : 64);
       const int cb0 = cgrp * p.cb_g + cb_tile * NT;
-      int it = 0;
-      for (long long c = c_begin; c < c_end; ++c, ++it) {
-        const int s = it % x.nstages;
-        mbar_wait(&empty[s], ((it / x.nstages) & 1) ^ 1);
+      RingPos r;
+      for (long long c = c_begin; c < c_end; ++c, r.advance(x.nstages)) {
+        const int s = r.slot();
+        mbar_wait(&empty[s], r.phase() ^ 1u);
         const int bb = (int)(c / x.chunks_per_batch);
         const int m0 = (int)(c % x.chunks_per_batch) * x.tt;
         uint8_t* st = stage0 + (size_t)s * stage_bytes;
@@ -376,10 +374,10 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
     float acc[kWgmmaMaxRegs];
 #pragma unroll
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
-    int it = 0;
-    for (long long c = c_begin; c < c_end; ++c, ++it) {
-      const int s = it % x.nstages;
-      mbar_wait(&full[s], (it / x.nstages) & 1);
+    RingPos r;
+    for (long long c = c_begin; c < c_end; ++c, r.advance(x.nstages)) {
+      const int s = r.slot();
+      mbar_wait(&full[s], r.phase());
       const uint32_t sbase = st0_16 + (uint32_t)s * stage16;
       wg_chunk_mma<NT>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, nu, cw, kslices);
       if (lane == 0) mbar_arrive(&empty[s]);
@@ -455,19 +453,6 @@ struct WgPlan {
   int nsplit_tma;
   int max_span_q;
 };
-
-// SMs of the current device (132 without one: the host-logic tests plan for an H100)
-static int wg_sm_count() {
-  static const int n = [] {
-    int dev = 0, v = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) {
-      cudaGetLastError();
-      v = 132;
-    }
-    return v;
-  }();
-  return n;
-}
 
 static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_only = false) {
   WgPlan pl{};
@@ -551,7 +536,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
   const long long units = (long long)p.batch * p.chunks_per_batch;
   const long long base = (long long)p.groups * p.n_ca_tiles * p.n_cb_tiles * p.ngroups;
-  const int sms = wg_sm_count();
+  const int sms = device_sm_count();
   // split-K factor: CTAs run one per SM in waves of one per SM; minimise (waves x chunks per CTA) plus the cost of writing
   // and re-reading one more partial copy of the gradient (in units of one chunk ~ 10 us; ~4 TB/s effective)
   const double out_chunks = (double)p.taps_total * p.ca_g0 * cb * 8.0 / 4e12 / 10e-6;
@@ -672,45 +657,35 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
     const int ba = blocks_for(na / 8), bb = blocks_for(nb / 8);
     split_planes_kernel<<<ba + bb, 256, 0, st>>>(p.a, na / 8, pa, p.b, nb / 8, pb, ba);
     KT_CHECK_CUDA(cudaGetLastError());
-    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     {
       const cuuint64_t gdim[5] = {(cuuint64_t)p.cb, (cuuint64_t)p.nsub, (cuuint64_t)p.t_b, (cuuint64_t)p.batch, 2};
       const cuuint64_t gstr[4] = {(cuuint64_t)p.cb * 2, (cuuint64_t)p.nsub * p.cb * 2, (cuuint64_t)p.t_b * p.nsub * p.cb * 2, (cuuint64_t)nb * 2};
       const cuuint32_t box[5] = {64, (cuuint32_t)p.nsub, (cuuint32_t)x.tt, 1, 1};
-      const CUresult r = encode_tiled_fn()(&x.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pb, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      KT_REQUIRE(r == CUDA_SUCCESS, "conv1d_bwd_weight_tc: cuTensorMapEncodeTiled(B) failed (%d)", (int)r);
+      const int rc = encode_tensor_map(&x.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pb, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv1d_bwd_weight_tc (operand B)");
+      if (rc) return rc;
     }
     for (int rho = 0; rho < p.step; ++rho) {
       const cuuint64_t gdim[5] = {(cuuint64_t)p.ca, (cuuint64_t)p.nsub, (cuuint64_t)ceil_div(p.t_a - rho, p.step), (cuuint64_t)p.batch, 2};
       const cuuint64_t gstr[4] = {(cuuint64_t)p.ca * 2, (cuuint64_t)p.step * p.nsub * p.ca * 2, (cuuint64_t)p.t_a * p.nsub * p.ca * 2, (cuuint64_t)na * 2};
       const cuuint32_t box[5] = {64, (cuuint32_t)p.nsub, (cuuint32_t)x.a_box_t, 1, 1};
-      const CUresult r = encode_tiled_fn()(&x.map_a[rho], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pa + (long long)rho * p.nsub * p.ca, gdim, gstr, box, estr,
-                                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      KT_REQUIRE(r == CUDA_SUCCESS, "conv1d_bwd_weight_tc: cuTensorMapEncodeTiled(A, residue %d) failed (%d)", rho, (int)r);
+      const int rc = encode_tensor_map(&x.map_a[rho], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pa + (long long)rho * p.nsub * p.ca, gdim, gstr, box,
+                                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv1d_bwd_weight_tc (operand A)");
+      if (rc) return rc;
     }
-    static std::atomic<bool> cfg_t{false};
-    if (!cfg_t.load(std::memory_order_acquire)) {
-      KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-      KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-      cfg_t.store(true, std::memory_order_release);
-    }
+    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<64>>(kMaxDynSmem));
+    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<128>>(kMaxDynSmem));
     dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
     if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
     else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
     KT_CHECK_CUDA(cudaGetLastError());
   } else {
-  static std::atomic<bool> cfg{false};
-  if (!cfg.load(std::memory_order_acquire)) {
-    KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    KT_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    cfg.store(true, std::memory_order_release);
-  }
-  dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
-  if (p.NT == 64) wgrad_tc_kernel<64><<<grid, kWgThreads, pl.smem, st>>>(p);
-  else wgrad_tc_kernel<128><<<grid, kWgThreads, pl.smem, st>>>(p);
-  KT_CHECK_CUDA(cudaGetLastError());
+    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<64>>(kMaxDynSmem));
+    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<128>>(kMaxDynSmem));
+    dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
+    if (p.NT == 64) wgrad_tc_kernel<64><<<grid, kWgThreads, pl.smem, st>>>(p);
+    else wgrad_tc_kernel<128><<<grid, kWgThreads, pl.smem, st>>>(p);
+    KT_CHECK_CUDA(cudaGetLastError());
   }
   const long long n = (long long)p.taps_total * p.ca_g0 * p.cb;
   if (p.nsplit >= 16) {
