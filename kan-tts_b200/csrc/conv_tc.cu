@@ -467,7 +467,8 @@ bool thin_cin1_ok(const KtConv1dDesc* d);   // thin.cu
 
 int tc_plan(const KtConv1dDesc* d, int dir) {
   if (dir == 0 && d->path != KT_PATH_TC && thin_cin1_ok(d)) return 0;   // waveform-input layers: HBM-bound FIR kernel
-  if (dir == 1 && d->upsample > 1) return 0;          // `upsample` single-tap residue phases: staging-bound, stays FFMA
+  if (dir == 1 && d->upsample > 1) return 0;          // no direct plan: ops.ConvPlan runs it as the plain conv over
+                                                      // the up-sampled rows + kt_upsample_grad_reduce
   const TcLayerPlan L = layer_plan(d, dir);
   if (!L.ok) return 0;
   std::vector<TcParams> launches;

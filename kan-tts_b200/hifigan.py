@@ -55,10 +55,11 @@ def join_side_streams(device=None):
 
 
 def prefetch_weights(module, streams):
-    """Launch the weight preparation of every weight-normed / plain conv of ``module`` on ``streams`` (round-robin,
+    """Launch the weight preparation of every weight-normed / plain conv of ``module`` that has run through ConvFn
+    (convs that only run inside the fused resblock are left to their forward) on ``streams`` (round-robin,
     one contiguous share of the layers per stream).  The caller forks the streams off the current one before and
     joins them before the module's next forward.  Spectral-normed layers recompute their weight per forward."""
-    layers = [m for m in module.modules() if isinstance(m, _NormedConv) and m.norm != "spectral" and m._cache.last is not None]
+    layers = [m for m in module.modules() if isinstance(m, _NormedConv) and m.norm != "spectral" and m._cache.conv_used]
     n = len(streams)
     for i, s in enumerate(streams):
         share = layers[i::n]
@@ -255,7 +256,7 @@ class ResidualBlock(nn.Module):
         for c1, c2 in zip(self.convs1, self.convs2):
             n1, n2 = c1.conv1d, c2.conv1d
             rd = ops.resblock_desc(n1.spec, n2.spec, x.shape[0], x.shape[1]) \
-                if (not ops._FORCE_FFMA and x.dim() == 3 and n1.norm != "spectral" and n2.norm != "spectral") else None
+                if (x.dim() == 3 and n1.norm != "spectral" and n2.norm != "spectral") else None
             if rd is not None:
                 # thin stages (32 / 64 channels): the pair is ONE launch, the intermediate stays on the SM (kt_resblock_fwd)
                 v1, g1 = n1.effective_weight()

@@ -6,7 +6,7 @@ Backward functions run on the autograd engine thread; every call passes the thre
 stream explicitly and the library keeps no global state.
 """
 import ctypes
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 
 import torch
 
@@ -73,27 +73,24 @@ def _sig(spec, d):
             f" B{d.batch}x{d.nsub} t{d.t_in}")
 
 
-class _timed:
-    """Context manager around one library call; a no-op unless the profiler is on."""
-    __slots__ = ("name", "spec", "d", "e0")
-
-    def __init__(self, name, spec=None, d=None):
-        self.name, self.spec, self.d = name, spec, d
-
-    def __enter__(self):
-        if _profiler is not None:
-            self.e0 = torch.cuda.Event(enable_timing=True)
-            self.e0.record()
-        return self
-
-    def __exit__(self, *exc):
-        if _profiler is not None:
-            e1 = torch.cuda.Event(enable_timing=True)
-            e1.record()
-            flops, nbytes = _conv_work(self.spec, self.d) if self.spec is not None else (0.0, 0.0)
-            _profiler.records.append((self.name, self.e0, e1, flops, nbytes))
-            _profiler.details.append(_sig(self.spec, self.d) if self.spec is not None else "")
-        return False
+def _run(name, spec, d, launches, tc, *calls):
+    """Make the library calls ``(entry point, *args)`` as one unit of kernel class ``name``: timed by the profiler
+    (when on) against the work of layer ``spec`` at descriptor ``d``, each checked, and counted as ``launches``
+    kernel launches, ``tc`` of them on the tensor cores."""
+    global _tc_launches
+    lib = _lib.load()
+    if _profiler is not None:
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+    for fn, *args in calls:
+        check(getattr(lib, fn)(*args), fn)
+    if _profiler is not None:
+        e1 = torch.cuda.Event(enable_timing=True)
+        e1.record()
+        _profiler.records.append((name, e0, e1, *_conv_work(spec, d)))
+        _profiler.details.append(_sig(spec, d))
+    _count(launches)
+    _tc_launches += tc
 
 
 def _conv_work(spec, d):
@@ -127,7 +124,8 @@ class ConvSpec:
     act_out: int = KT_ACT_NONE
     act_out_slope: float = 0.0
     path: int = KT_PATH_AUTO
-    _descs: dict = field(default_factory=dict, repr=False)
+    _plans: dict = field(default_factory=dict, init=False, repr=False, compare=False)
+    _rb_cache: dict = field(default_factory=dict, init=False, repr=False, compare=False)
 
     def t_out(self, t_in):
         if self.transposed:
@@ -135,84 +133,113 @@ class ConvSpec:
         t = t_in * self.upsample
         return (t + self.pad_left + self.pad_right - self.dilation * (self.kernel - 1) - 1) // self.stride + 1
 
+    def plan(self, batch, nsub, t_in):
+        """-> the ConvPlan of this layer for one input shape, cached per shape and exact-path flag (the tests toggle
+        set_force_ffma at run time).  Every field of the spec must be set before its first plan."""
+        key = (batch, nsub, t_in, _exact(self))
+        p = self._plans.get(key)
+        if p is None:
+            p = self._plans[key] = ConvPlan(self, batch, nsub, t_in, key[3])
+        return p
+
     def desc(self, batch, nsub, t_in):
-        key = (batch, nsub, t_in)
-        d = self._descs.get(key)
-        if d is None:
-            d = KtConv1dDesc(batch=batch, nsub=nsub, t_in=t_in, t_out=self.t_out(t_in), c_in=self.c_in,
-                             c_out=self.c_out, groups=self.groups, kernel=self.kernel, stride=self.stride,
-                             dilation=self.dilation, pad_left=self.pad_left, transposed=int(self.transposed),
-                             upsample=self.upsample, act_in=self.act_in, act_in_slope=self.act_in_slope,
-                             act_out=self.act_out, act_out_slope=self.act_out_slope, path=self.path)
-            self._descs[key] = d
-        return d
+        """-> a new KtConv1dDesc of this layer for one input shape (the plan keeps the one the layer runs with)."""
+        return KtConv1dDesc(batch=batch, nsub=nsub, t_in=t_in, t_out=self.t_out(t_in), c_in=self.c_in, c_out=self.c_out,
+                            groups=self.groups, kernel=self.kernel, stride=self.stride, dilation=self.dilation,
+                            pad_left=self.pad_left, transposed=int(self.transposed), upsample=self.upsample,
+                            act_in=self.act_in, act_in_slope=self.act_in_slope, act_out=self.act_out,
+                            act_out_slope=self.act_out_slope, path=self.path)
 
     @property
     def w_numel(self):
         return self.kernel * (self.c_in // self.groups) * self.c_out
 
-    def without_upsample(self):
-        """The same conv over the already up-sampled rows (upsample = 1, no fused pre-activation): its data
-        gradient on the tensor-core kernel + kt_upsample_grad_reduce replaces the FFMA data gradient of the
-        nearest-upsampled conv."""
-        s = self.__dict__.get("_noup")
-        if s is None:
-            s = ConvSpec(c_in=self.c_in, c_out=self.c_out, kernel=self.kernel, stride=self.stride, dilation=self.dilation,
-                         pad_left=self.pad_left, pad_right=self.pad_right, groups=self.groups, act_out=self.act_out,
-                         act_out_slope=self.act_out_slope, path=self.path)
-            self.__dict__["_noup"] = s
-        return s
+
+class ConvPlan:
+    """Which kernel runs each pass of one conv layer for one input shape.  An N tile or workspace of 0 means the
+    exact-fp32 (FFMA) kernel.
+      d                        the layer's descriptor
+      nt_fwd                   forward N tile
+      d_bwd, nt_bwd, up_bwd    data gradient: descriptor, N tile, and whether it runs over the up-sampled rows
+      wg_ws                    tensor-core weight-gradient workspace, in floats"""
+
+    __slots__ = ("spec", "d", "nt_fwd", "d_bwd", "nt_bwd", "up_bwd", "wg_ws")
+
+    def __init__(self, spec, batch, nsub, t_in, exact):
+        self.spec = spec
+        self.d = self.d_bwd = d = spec.desc(batch, nsub, t_in)
+        self.nt_fwd = self.nt_bwd = self.wg_ws = 0
+        self.up_bwd = False
+        if exact:
+            return
+        lib = _lib.load()
+        self.nt_fwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 0)
+        self.nt_bwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 1)
+        if (not self.nt_bwd and spec.path == KT_PATH_AUTO and spec.upsample > 1 and spec.c_in % 4 == 0
+                and not spec.transposed):
+            # the nearest-upsampled conv has no tensor-core data gradient of its own: run the same conv over the
+            # up-sampled rows (upsample = 1, no fused pre-activation) and fold it back with kt_upsample_grad_reduce
+            d2 = replace(spec, upsample=1, act_in=KT_ACT_NONE, act_in_slope=0.0).desc(batch, nsub, t_in * spec.upsample)
+            nt2 = lib.kt_conv1d_tc_plan(ctypes.byref(d2), 1)
+            if nt2:
+                self.d_bwd, self.nt_bwd, self.up_bwd = d2, nt2, True
+        self.wg_ws = int(lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d)))
+
+    def tile(self, direction):
+        """N tile of direction 0 (forward) or 1 (data gradient), for a pass that runs: a KT_PATH_TC layer raises here
+        when the tensor cores cannot run it (unless set_force_ffma put every layer on the exact path)."""
+        nt = self.nt_bwd if direction else self.nt_fwd
+        if nt == 0 and self.spec.path == KT_PATH_TC and not _exact(self.spec):
+            raise RuntimeError(f"kantts_b200: layer {self.spec} cannot run on the tensor-core path")
+        return nt
 
 
 class PreparedWeight:
     """Kernel-layout copies of one layer's effective weight (w_fwd, w_bwd) + the weight-norm
     row norms, valid for one (parameter version) -- see kt_weight_prepare."""
 
-    __slots__ = ("w_fwd", "w_bwd", "norm", "key", "img", "img_stale", "last", "last_reuse")
+    __slots__ = ("w_fwd", "w_bwd", "norm", "key", "img", "img_stale", "conv_used")
 
     def __init__(self):
         self.w_fwd = self.w_bwd = self.norm = None
         self.key = None
-        self.last_reuse = None   # (d, nt_fwd) of the latest pair_reuse forward (a second forward shape per step)
-        self.last = None       # (d, nt_fwd, d_bwd, nt_bwd) of the latest forward: what prefetch() re-prepares
-        self.img = {}          # (dir, n_tile) -> packed split-bf16 tensor-core weight tiles
+        self.img = {}          # key -> (packed weight image, descriptor it is packed for), see image()
         self.img_stale = set()
+        self.conv_used = False  # a ConvFn forward ran on it: hifigan.prefetch_weights re-prepares it
 
-    def tc_image(self, spec, d, direction, n_tile):
-        """hi/lo bf16 SWIZZLE_128B weight tiles for the tensor-core kernels (kt_weight_pack_tc).  The tiling
-        (N tile, padding) can depend on the sequence length, hence the key on n_tile."""
-        k = (direction, n_tile)
-        img = self.img.get(k)
-        if img is None or k in self.img_stale:
-            lib = _lib.load()
-            src = self.w_fwd if direction == 0 else self.w_bwd
-            if img is None:
-                nbytes = int(lib.kt_conv1d_tc_image_bytes(ctypes.byref(d), direction))
-                img = torch.empty(nbytes // 2, device=src.device, dtype=torch.bfloat16)
-                self.img[k] = img
-            check(lib.kt_weight_pack_tc(ctypes.byref(d), direction, ptr(src), ptr(img, True), stream_ptr()),
-                  "kt_weight_pack_tc")
-            _count()
-            self.img_stale.discard(k)
+    def image(self, key, d):
+        """A packed split-bf16 weight image: hi/lo SWIZZLE_128B tiles for the tensor-core conv kernels
+        (kt_weight_pack_tc, key (direction, N tile): the tiling can depend on the sequence length, hence the key on the
+        N tile) or the fused resblock's (kt_resblock_pack, key ("rb", C, k), d a KtResblockDesc).  Packed for
+        descriptor d on first use and re-packed in place once the weights changed; the image depends on its key only,
+        so a re-pack reuses that first descriptor (prefetch_weight passes none)."""
+        img = self.img.get(key)
+        if img is not None and key not in self.img_stale:
+            return img[0]
+        lib = _lib.load()
+        rb = key[0] == "rb"
+        if img is None:
+            nbytes = lib.kt_resblock_image_bytes(ctypes.byref(d)) if rb else lib.kt_conv1d_tc_image_bytes(ctypes.byref(d), key[0])
+            img = (torch.empty(int(nbytes) // 2, device=self.w_fwd.device, dtype=torch.bfloat16), d)
+            self.img[key] = img
+        img, d = img
+        if rb:
+            check(lib.kt_resblock_pack(ctypes.byref(d), ptr(self.w_fwd), ptr(img, True), stream_ptr()), "kt_resblock_pack")
+        else:
+            src = self.w_fwd if key[0] == 0 else self.w_bwd
+            check(lib.kt_weight_pack_tc(ctypes.byref(d), key[0], ptr(src), ptr(img, True), stream_ptr()), "kt_weight_pack_tc")
+        _count()
+        self.img_stale.discard(key)
         return img
 
 
 def prefetch_weight(cache, spec, v, g):
-    """Re-prepare (weight norm + layouts + tensor-core tiles) a layer's weights ahead of its next forward, for the
-    shapes its latest forward used -- a no-op when nothing changed.  train.GanStep runs this for a whole model on
-    side streams right after that model's optimizer step, off the critical path of the other model's forward."""
-    if cache.last is None:
-        return
-    d, nt, db, nt_b = cache.last
+    """Re-prepare (weight norm + layouts + packed images) a layer's weights ahead of its next forward, for every image
+    it holds -- a no-op when nothing changed.  train.GanStep runs this for a whole model on side streams right after
+    that model's optimizer step, off the critical path of the other model's forward."""
     pw = prepare_weight(cache, spec, v, g)
-    if nt and not (_FORCE_FFMA or spec.path == KT_PATH_FFMA):
-        pw.tc_image(spec, d, 0, nt)
-    if nt_b and not (_FORCE_FFMA or spec.path == KT_PATH_FFMA):
-        pw.tc_image(spec, db, 1, nt_b)
-    if cache.last_reuse is not None and not (_FORCE_FFMA or spec.path == KT_PATH_FFMA):
-        d2, nt2 = cache.last_reuse
-        if nt2:
-            pw.tc_image(spec, d2, 0, nt2)
+    for key in [k for k in pw.img if k in pw.img_stale]:
+        pw.image(key, None)
 
 
 def prepare_weight(cache, spec, v, g):
@@ -360,37 +387,16 @@ def set_force_ffma(flag):
     _FORCE_FFMA = bool(flag)
 
 
-def _wgrad_tc_workspace(lib, spec, d):
-    """fp32 workspace floats for the tensor-core weight-gradient kernel, 0 = use the FFMA kernel."""
-    if _FORCE_FFMA or spec.path == KT_PATH_FFMA:
-        return 0
-    key = ("wg", d.batch, d.nsub, d.t_in)
-    n = spec._descs.get(key)
-    if n is None:
-        n = int(lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d)))
-        spec._descs[key] = n
-    return n
+def _exact(spec):
+    """Does this layer run on the exact-fp32 (FFMA) kernels only?"""
+    return _FORCE_FFMA or spec.path == KT_PATH_FFMA
 
 
-def _tc_tile(lib, spec, d, direction):
-    if _FORCE_FFMA or spec.path == KT_PATH_FFMA:
-        return 0
-    key = ("tc", direction, d.batch, d.nsub, d.t_in)
-    nt = spec._descs.get(key)
-    if nt is None:
-        nt = lib.kt_conv1d_tc_plan(ctypes.byref(d), direction)
-        spec._descs[key] = nt
-    if nt == 0 and spec.path == KT_PATH_TC:
-        raise RuntimeError(f"kantts_b200: layer {spec} cannot run on the tensor-core path")
-    return nt
-
-
-def _weight_backward(spec, d, x_, dy, y_, v, g, params, norm, need_v, need_g, need_b):
+def _weight_backward(spec, plan, x_, dy, y_, v, g, params, norm, need_v, need_g, need_b):
     """Weight-gradient chain of one conv layer (wgrad kernel -> split-K reduce -> bias column sums -> weight-norm backward),
     shared by ConvFn.backward and ResblockFn.backward.  x_, dy, y_: the layer's input, output gradient and (when it has a
-    fused output activation) output, already restricted to the batch items that carry gradient.  -> (dbias, dv, dg): the
+    fused output activation) output, already restricted to the batch items of `plan`.  -> (dbias, dv, dg): the
     gradients to hand to autograd, None for parameters whose .grad the kernels accumulated into directly (mark_direct_grad)."""
-    global _tc_launches
     dbias = dv = dg = None
     need_w = need_v or need_g
     if not (need_w or need_b):
@@ -416,18 +422,14 @@ def _weight_backward(spec, d, x_, dy, y_, v, g, params, norm, need_v, need_g, ne
         dw = torch.empty(spec.w_numel, device=x_.device, dtype=torch.float32)
         if need_b:
             dbias = torch.empty(spec.c_out, device=x_.device, dtype=torch.float32)
-        ws_floats = _wgrad_tc_workspace(lib, spec, d)
+        d, ws_floats, n = plan.d, plan.wg_ws, 4 if need_b else 2
         if ws_floats:
             ws = torch.empty(ws_floats, device=x_.device, dtype=torch.float32)
-            with _timed("conv_wgrad_tc", spec, d):
-                check(lib.kt_conv1d_bwd_weight_tc(ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_), ptr(dw), ptr(dbias),
-                                                  ptr(ws), ws_floats, st), "kt_conv1d_bwd_weight_tc")
-            _tc_launches += 1
+            _run("conv_wgrad_tc", spec, d, n, 1, ("kt_conv1d_bwd_weight_tc", ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_),
+                                                  ptr(dw), ptr(dbias), ptr(ws), ws_floats, st))
         else:
-            with _timed("conv_wgrad_ffma", spec, d):
-                check(lib.kt_conv1d_bwd_weight(ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_), ptr(dw), ptr(dbias), st),
-                      "kt_conv1d_bwd_weight")
-        _count(4 if need_b else 2)
+            _run("conv_wgrad_ffma", spec, d, n, 0, ("kt_conv1d_bwd_weight", ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_),
+                                                    ptr(dw), ptr(dbias), st))
         if need_w:
             vd = v.detach().contiguous()
             gd = None if g is None else g.detach().contiguous()
@@ -460,74 +462,52 @@ class ConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, resid, bias, v, g, spec, cache, reuse=None):
-        lib = _lib.load()
         x = x.contiguous()
         nsub = x.shape[2] if x.dim() == 4 else 1
         B, t_in = x.shape[0], x.shape[1]
         assert x.shape[-1] == spec.c_in, (x.shape, spec)
-        d_full = spec.desc(B, nsub, t_in)
+        full = spec.plan(B, nsub, t_in)
         pw = prepare_weight(cache, spec, v, g)
-        shape = (B, d_full.t_out, nsub, spec.c_out) if x.dim() == 4 else (B, d_full.t_out, spec.c_out)
+        shape = (B, full.d.t_out, nsub, spec.c_out) if x.dim() == 4 else (B, full.d.t_out, spec.c_out)
         if reuse is not None:
             # pair_reuse: the output of this layer for the batch items [nb_run, B) is already in `y_buf` (same weights, same
             # inputs, computed earlier in the step); only the first nb_run items are computed, in place
             y_buf, nb_run = reuse
             assert tuple(y_buf.shape) == tuple(shape) and y_buf.is_contiguous() and resid is None, (y_buf.shape, shape)
             y = y_buf.detach()
-            d = spec.desc(nb_run, nsub, t_in)
+            run = spec.plan(nb_run, nsub, t_in)
         else:
             y = torch.empty(shape, device=x.device, dtype=torch.float32)
-            d = d_full
+            run = full
         if resid is not None:
             resid = resid.contiguous()
             assert resid.shape == y.shape, (resid.shape, y.shape)
         bd = None if bias is None else bias.detach()
-        nt = _tc_tile(lib, spec, d, 0)
+        d, nt, n = run.d, run.tile(0), (spec.stride if spec.transposed else 1)
         if nt:
-            global _tc_launches
-            img = pw.tc_image(spec, d, 0, nt)
-            with _timed("conv_fwd_tc", spec, d):
-                check(lib.kt_conv1d_fwd_tc(ctypes.byref(d), ptr(x), ptr(img, True), ptr(bd), ptr(resid),
-                                           ptr(y), stream_ptr()), "kt_conv1d_fwd_tc")
-            _tc_launches += spec.stride if spec.transposed else 1
+            img = pw.image((0, nt), d)
+            _run("conv_fwd_tc", spec, d, n, n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True), ptr(bd),
+                                                ptr(resid), ptr(y), stream_ptr()))
         else:
-            with _timed("conv_fwd_ffma", spec, d):
-                check(lib.kt_conv1d_fwd(ctypes.byref(d), ptr(x), ptr(pw.w_fwd), ptr(bd), ptr(resid), ptr(y),
-                                        stream_ptr()), "kt_conv1d_fwd")
-        _count(spec.stride if spec.transposed else 1)
+            _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd", ctypes.byref(d), ptr(x), ptr(pw.w_fwd), ptr(bd),
+                                                  ptr(resid), ptr(y), stream_ptr()))
+        pw.conv_used = True
         nb = B if _grad_items is None else min(_grad_items, B)     # batch items that carry gradient
-        d = d_full
-        db = d if nb == B else spec.desc(nb, nsub, t_in)
-        ctx.spec, ctx.d, ctx.nb = spec, db, nb
+        ctx.spec, ctx.nb = spec, nb
+        ctx.plan = full if nb == B else spec.plan(nb, nsub, t_in)
         ctx.w_bwd, ctx.norm = pw.w_bwd, pw.norm
-        nt_b = _tc_tile(lib, spec, db, 1) if x.requires_grad else 0
-        ctx.d_up = None
-        if x.requires_grad and nt_b == 0 and spec.upsample > 1 and spec.c_in % 4 == 0 and not spec.transposed:
-            # data gradient wrt the up-sampled rows on the tensor-core kernel, folded back by kt_upsample_grad_reduce
-            s2 = spec.without_upsample()
-            d2 = s2.desc(nb, nsub, t_in * spec.upsample)
-            nt2 = _tc_tile(lib, s2, d2, 1) if d2.t_out == d.t_out else 0
-            if nt2:
-                ctx.d_up, nt_b = d2, nt2
-        ctx.nt_bwd = nt_b
-        ctx.img_bwd = pw.tc_image(spec, ctx.d_up or db, 1, nt_b) if nt_b else None
+        nt_b = ctx.plan.tile(1) if x.requires_grad else 0
+        ctx.img_bwd = pw.image((1, nt_b), ctx.plan.d_bwd) if nt_b else None
         ctx.has_resid, ctx.has_bias, ctx.has_g = resid is not None, bias is not None, g is not None
         ctx.params = (v, g, bias)
-        prev = cache.last
-        if reuse is not None and prev is not None:
-            cache.last_reuse = (spec.desc(reuse[1], nsub, t_in), nt)   # keep the full-batch shapes for the prefetch, add this one
-        elif nt_b == 0 and prev is not None and prev[3]:   # a no-grad forward keeps the data-gradient plan to prefetch
-            cache.last = (d, nt, prev[2], prev[3])
-        else:
-            cache.last = (d, nt, ctx.d_up or db, nt_b)
         ctx.save_for_backward(x, y if spec.act_out != KT_ACT_NONE else None, v, g)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        lib = _lib.load()
         x, y, v, g = ctx.saved_tensors
-        spec, d = ctx.spec, ctx.d
+        spec, plan = ctx.spec, ctx.plan
+        d = plan.d
         dy = dy.contiguous()
         st = stream_ptr()
         dx = dres = dbias = dv = dg = None
@@ -539,28 +519,22 @@ class ConvFn(torch.autograd.Function):
             x_, y_ = x, y
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)     # items >= nb stay unwritten: nothing differentiable consumes them
-            if ctx.d_up is not None:
-                global _tc_launches
-                d2 = ctx.d_up
+            n = max(spec.stride if not spec.transposed else 1, spec.upsample)
+            # the forward packs the plan's tensor-core image only when its x requires grad; a non-contiguous x is copied
+            # there without grad, and its data gradient then runs on the exact kernel
+            if ctx.img_bwd is None:
+                _run("conv_dgrad_ffma", spec, d, n, 0, ("kt_conv1d_bwd_data", ctypes.byref(d), ptr(dy), ptr(y_),
+                                                        ptr(ctx.w_bwd), ptr(x_), ptr(dx), st))
+            elif plan.up_bwd:
+                d2 = plan.d_bwd
                 dxu = torch.empty((ctx.nb, d2.t_in * d2.nsub, spec.c_in), device=x.device, dtype=torch.float32)
-                with _timed("conv_dgrad_tc", spec, d):
-                    check(lib.kt_conv1d_bwd_data_tc(ctypes.byref(d2), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), None,
-                                                    ptr(dxu), st), "kt_conv1d_bwd_data_tc")
-                    check(lib.kt_upsample_grad_reduce(ptr(dxu), ptr(x_), spec.act_in, spec.act_in_slope, ptr(dx),
-                                                      ctx.nb * d.t_in * d.nsub, spec.upsample, spec.c_in, st),
-                          "kt_upsample_grad_reduce")
-                _tc_launches += 1
-                _count()
-            elif ctx.nt_bwd:
-                with _timed("conv_dgrad_tc", spec, d):
-                    check(lib.kt_conv1d_bwd_data_tc(ctypes.byref(d), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), ptr(x_),
-                                                    ptr(dx), st), "kt_conv1d_bwd_data_tc")
-                _tc_launches += 1
+                _run("conv_dgrad_tc", spec, d, n + 1, 1,
+                     ("kt_conv1d_bwd_data_tc", ctypes.byref(d2), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), None, ptr(dxu), st),
+                     ("kt_upsample_grad_reduce", ptr(dxu), ptr(x_), spec.act_in, spec.act_in_slope, ptr(dx),
+                      ctx.nb * d.t_in * d.nsub, spec.upsample, spec.c_in, st))
             else:
-                with _timed("conv_dgrad_ffma", spec, d):
-                    check(lib.kt_conv1d_bwd_data(ctypes.byref(d), ptr(dy), ptr(y_), ptr(ctx.w_bwd), ptr(x_), ptr(dx),
-                                                 st), "kt_conv1d_bwd_data")
-            _count(max(spec.stride if not spec.transposed else 1, spec.upsample))
+                _run("conv_dgrad_tc", spec, d, n, 1, ("kt_conv1d_bwd_data_tc", ctypes.byref(d), ptr(dy), ptr(y_),
+                                                      ptr(ctx.img_bwd, True), ptr(x_), ptr(dx), st))
         if ctx.has_resid and ctx.needs_input_grad[1]:
             # NOT the incoming tensor itself: the autograd engine accumulates gradients arriving at the same input IN PLACE
             # into the first arrival when it holds the last reference (input_buffer.cpp: can_accumulate_inplace), and
@@ -569,7 +543,7 @@ class ConvFn(torch.autograd.Function):
             # the engine overwrite it under those readers: parameter gradients of the generator were off by ~5 % with the
             # (slow) exact-fp32 kernels and side streams on (test_full_size_c2_train_step_matches_oracle).
             dres = dy_full.clone()
-        dbias, dv, dg = _weight_backward(spec, d, x_, dy, y_, v, g, ctx.params, ctx.norm, ctx.needs_input_grad[3],
+        dbias, dv, dg = _weight_backward(spec, plan, x_, dy, y_, v, g, ctx.params, ctx.norm, ctx.needs_input_grad[3],
                                          ctx.has_g and ctx.needs_input_grad[4], ctx.has_bias and ctx.needs_input_grad[2])
         return dx, dres, dbias, dv, dg, None, None, None
 
@@ -621,9 +595,12 @@ def pair_conv(owner, x, spec, cache, v, g, bias, resid=None):
 # ---- fused ResidualBlock unit (csrc/resblock_tc.cu) -------------------------------------------------------------------
 def resblock_desc(spec1, spec2, batch, t):
     """-> KtResblockDesc when the pair (dilated conv, dilation-1 conv; same channels / kernel; fused input LeakyReLU, no
-    output activation) can run on the fused kernel for this shape, else None.  Cached per shape on spec1."""
-    key = ("rb", batch, t)
-    d = spec1._descs.get(key, False)
+    output activation) can run on the fused kernel for this shape, else None (also on the exact path).  Cached per
+    shape on spec1."""
+    if _exact(spec1) or _exact(spec2):
+        return None
+    key = (batch, t)
+    d = spec1._rb_cache.get(key, False)
     if d is not False:
         return d
     d = None
@@ -631,29 +608,14 @@ def resblock_desc(spec1, spec2, batch, t):
           and spec1.stride == spec2.stride == 1 and spec1.groups == spec2.groups == 1 and not spec1.transposed
           and not spec2.transposed and spec1.upsample == spec2.upsample == 1 and spec1.act_in == spec2.act_in == KT_ACT_LRELU
           and spec1.act_in_slope == spec2.act_in_slope and spec1.act_out == spec2.act_out == KT_ACT_NONE
-          and spec1.t_out(t) == t and spec2.t_out(t) == t and spec1.path != KT_PATH_FFMA and spec2.path != KT_PATH_FFMA)
+          and spec1.t_out(t) == t and spec2.t_out(t) == t)
     if ok:
         cand = KtResblockDesc(batch=batch, t=t, channels=spec1.c_in, kernel=spec1.kernel, dilation=spec1.dilation,
                               pad_left1=spec1.pad_left, pad_left2=spec2.pad_left, slope=spec1.act_in_slope, path=KT_PATH_AUTO)
         if _lib.load().kt_resblock_plan(ctypes.byref(cand)) == 1:
             d = cand
-    spec1._descs[key] = d
+    spec1._rb_cache[key] = d
     return d
-
-
-def _rb_image(pw, rd):
-    """the fused kernel's weight image of one conv (kt_resblock_pack), cached beside the tensor-core tile images"""
-    k = ("rb", rd.channels, rd.kernel)
-    img = pw.img.get(k)
-    if img is None or k in pw.img_stale:
-        lib = _lib.load()
-        if img is None:
-            img = torch.empty(int(lib.kt_resblock_image_bytes(ctypes.byref(rd))) // 2, device=pw.w_fwd.device, dtype=torch.bfloat16)
-            pw.img[k] = img
-        check(lib.kt_resblock_pack(ctypes.byref(rd), ptr(pw.w_fwd), ptr(img, True), stream_ptr()), "kt_resblock_pack")
-        _count()
-        pw.img_stale.discard(k)
-    return img
 
 
 class ResblockFn(torch.autograd.Function):
@@ -662,29 +624,25 @@ class ResblockFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, b1, v1, g1, b2, v2, g2, spec1, cache1, spec2, cache2, rd):
-        global _tc_launches
-        lib = _lib.load()
         x = x.contiguous()
         B, T = x.shape[0], x.shape[1]
         pw1 = prepare_weight(cache1, spec1, v1, g1)
         pw2 = prepare_weight(cache2, spec2, v2, g2)
-        img1, img2 = _rb_image(pw1, rd), _rb_image(pw2, rd)
+        key = ("rb", rd.channels, rd.kernel)
+        img1, img2 = pw1.image(key, rd), pw2.image(key, rd)
         need_grad = any(ctx.needs_input_grad[:7])
         y = torch.empty_like(x)
         h = torch.empty_like(x) if need_grad else None
-        with _timed("resblock_fwd_tc", spec1, spec1.desc(B, 1, T)):
-            check(lib.kt_resblock_fwd(ctypes.byref(rd), ptr(x), ptr(img1, True), ptr(None if b1 is None else b1.detach()),
-                                      ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h), ptr(y), stream_ptr()),
-                  "kt_resblock_fwd")
-        _tc_launches += 1
-        _count()
+        _run("resblock_fwd_tc", spec1, spec1.plan(B, 1, T).d, 1, 1,
+             ("kt_resblock_fwd", ctypes.byref(rd), ptr(x), ptr(img1, True), ptr(None if b1 is None else b1.detach()),
+              ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h), ptr(y), stream_ptr()))
         if need_grad:
             nb = B if _grad_items is None else min(_grad_items, B)
-            d1, d2 = spec1.desc(nb, 1, T), spec2.desc(nb, 1, T)
-            ctx.nb, ctx.d1, ctx.d2, ctx.specs = nb, d1, d2, (spec1, spec2)
-            nt1, nt2 = _tc_tile(lib, spec1, d1, 1), _tc_tile(lib, spec2, d2, 1)
+            p1, p2 = spec1.plan(nb, 1, T), spec2.plan(nb, 1, T)
+            ctx.nb, ctx.plans, ctx.specs = nb, (p1, p2), (spec1, spec2)
+            nt1, nt2 = p1.tile(1), p2.tile(1)
             assert nt1 and nt2, "fused resblock: the data gradients run on the tensor-core kernels"
-            ctx.img_bwd = (pw1.tc_image(spec1, d1, 1, nt1), pw2.tc_image(spec2, d2, 1, nt2))
+            ctx.img_bwd = (pw1.image((1, nt1), p1.d), pw2.image((1, nt2), p2.d))
             ctx.norms = (pw1.norm, pw2.norm)
             ctx.params = ((v1, g1, b1), (v2, g2, b2))
             ctx.save_for_backward(x, h, v1, g1, v2, g2)
@@ -692,10 +650,9 @@ class ResblockFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        global _tc_launches
-        lib = _lib.load()
         x, h, v1, g1, v2, g2 = ctx.saved_tensors
         spec1, spec2 = ctx.specs
+        p1, p2 = ctx.plans
         dy = dy.contiguous()
         dy_full = dy
         if ctx.nb < x.shape[0]:
@@ -704,17 +661,14 @@ class ResblockFn(torch.autograd.Function):
             x_, h_ = x, h
         dh = torch.empty_like(x_)
         dx = torch.empty_like(x)
-        with _timed("conv_dgrad_tc", spec1, ctx.d1):
-            check(lib.kt_resblock_bwd(ctypes.byref(ctx.d1), ctypes.byref(ctx.d2), ptr(x_), ptr(h_), ptr(dy), ptr(ctx.img_bwd[0], True),
-                                      ptr(ctx.img_bwd[1], True), ptr(dh), ptr(dx if ctx.nb == x.shape[0] else dx[:ctx.nb]),
-                                      stream_ptr()), "kt_resblock_bwd")
-        _tc_launches += 2
-        _count(3)
+        _run("conv_dgrad_tc", spec1, p1.d, 3, 2,
+             ("kt_resblock_bwd", ctypes.byref(p1.d), ctypes.byref(p2.d), ptr(x_), ptr(h_), ptr(dy), ptr(ctx.img_bwd[0], True),
+              ptr(ctx.img_bwd[1], True), ptr(dh), ptr(dx if ctx.nb == x.shape[0] else dx[:ctx.nb]), stream_ptr()))
         ni = ctx.needs_input_grad
         (pv1, pg1, pb1), (pv2, pg2, pb2) = ctx.params
-        db2, dv2, dg2 = _weight_backward(spec2, ctx.d2, h_, dy, None, v2, g2, (pv2, pg2, pb2), ctx.norms[1], ni[5],
+        db2, dv2, dg2 = _weight_backward(spec2, p2, h_, dy, None, v2, g2, (pv2, pg2, pb2), ctx.norms[1], ni[5],
                                          g2 is not None and ni[6], pb2 is not None and ni[4])
-        db1, dv1, dg1 = _weight_backward(spec1, ctx.d1, x_, dh, None, v1, g1, (pv1, pg1, pb1), ctx.norms[0], ni[2],
+        db1, dv1, dg1 = _weight_backward(spec1, p1, x_, dh, None, v1, g1, (pv1, pg1, pb1), ctx.norms[0], ni[2],
                                          g1 is not None and ni[3], pb1 is not None and ni[1])
         return (dx if ni[0] else None), db1, dv1, dg1, db2, dv2, dg2, None, None, None, None, None
 

@@ -56,10 +56,21 @@ def test_upsampled_conv_data_gradient_plan(lib):
     spec, d = _desc(16, 32, c_in=512, c_out=256, kernel=7, pad_left=6, upsample=8, act_in=1, act_in_slope=0.1)
     assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 0) > 0
     assert lib.kt_conv1d_tc_plan(ctypes.byref(d), 1) == 0            # not directly ...
-    s2 = spec.without_upsample()
-    d2 = s2.desc(16, 1, 32 * 8)
-    assert d2.t_out == d.t_out and s2.act_in == 0 and s2.upsample == 1
-    assert lib.kt_conv1d_tc_plan(ctypes.byref(d2), 1) > 0            # ... but as the plain conv over the up-sampled rows
+    p = spec.plan(16, 1, 32)
+    d2 = p.d_bwd
+    assert p.up_bwd and d2.t_in == 32 * 8 and d2.t_out == d.t_out and d2.act_in == 0 and d2.upsample == 1
+    assert lib.kt_conv1d_tc_plan(ctypes.byref(d2), 1) == p.nt_bwd > 0   # ... but as the plain conv over the up-sampled rows
+    # a layer that insists on the tensor cores gets no detour: its forward runs, its data gradient raises when it runs
+    spec = ops.ConvSpec(c_in=512, c_out=256, kernel=7, pad_left=6, upsample=8, act_in=1, act_in_slope=0.1, path=KT_PATH_TC)
+    p = spec.plan(16, 1, 32)
+    assert p.tile(0) > 0 and not p.up_bwd
+    with pytest.raises(RuntimeError, match="cannot run on the tensor-core path"):
+        p.tile(1)
+    ops.set_force_ffma(True)
+    try:
+        assert _no_tensor_routes(spec.plan(16, 1, 32))              # set_force_ffma overrides KT_PATH_TC
+    finally:
+        ops.set_force_ffma(False)
 
 
 def test_split_k_workspace_is_whole_slices_of_the_gradient(lib):
@@ -119,10 +130,31 @@ def test_grad_items_context_restores_state():
     assert ops._grad_items is None
 
 
+def _no_tensor_routes(p):
+    return p.tile(0) == p.tile(1) == p.wg_ws == 0 and not p.up_bwd and p.d_bwd is p.d
+
+
 def test_ffma_path_has_no_tensor_plan(lib):
-    _, d = _desc(2, 100, c_in=64, c_out=64, kernel=3, pad_left=2, path=KT_PATH_FFMA)
-    spec = ops.ConvSpec(c_in=64, c_out=64, kernel=3, pad_left=2, path=KT_PATH_FFMA)
-    assert ops._tc_tile(lib, spec, d, 0) == 0 and ops._wgrad_tc_workspace(lib, spec, d) == 0
+    for kw in (dict(c_in=64, c_out=64, kernel=3, pad_left=2),
+               dict(c_in=512, c_out=256, kernel=7, pad_left=6, upsample=8, act_in=1, act_in_slope=0.1)):
+        assert _no_tensor_routes(ops.ConvSpec(path=KT_PATH_FFMA, **kw).plan(2, 1, 100)), kw
+
+
+def test_plan_cache_follows_the_exact_path_flag(lib):
+    spec = ops.ConvSpec(c_in=64, c_out=64, kernel=3, pad_left=2)
+    p = spec.plan(2, 1, 100)
+    assert p.tile(0) > 0 and p.tile(1) > 0 and p.wg_ws > 0
+    s1, s2 = _resblock_specs(32, 7, 3, True)
+    assert ops.resblock_desc(s1, s2, 16, 8192) is not None
+    ops.set_force_ffma(True)
+    try:
+        assert _no_tensor_routes(spec.plan(2, 1, 100))
+        assert ops.resblock_desc(s1, s2, 16, 8192) is None
+    finally:
+        ops.set_force_ffma(False)
+    assert spec.plan(2, 1, 100) is p and ops.resblock_desc(s1, s2, 16, 8192) is not None
+    s1, s2 = _resblock_specs(32, 15, 11, True)                       # 282 rows: over the 256-row TMA box
+    assert ops.resblock_desc(s1, s2, 2, 1000) is None
 
 
 def test_tma_weight_gradient_plans_respect_the_hardware_limits():
