@@ -136,10 +136,15 @@ int kt_conv1d_bwd_weight(const KtConv1dDesc* d, const float* x, const float* dy,
 int kt_conv1d_tc_plan(const KtConv1dDesc* d, int32_t dir);
 int64_t kt_conv1d_tc_image_bytes(const KtConv1dDesc* d, int32_t dir);
 int kt_weight_pack_tc(const KtConv1dDesc* d, int32_t dir, const float* w, void* out, void* stream);
+/* Workspace: channel counts % 8 == 0 without nearest-upsampling may take the TMA-fed route, which first writes the
+ * gathered operand (forward: act_in(x); data gradient: dy * act_out'(y)) into `workspace` as hi / lo bf16 planes
+ * ([plane][B][T][nsub][C], 16-byte aligned).  kt_conv1d_tc_workspace: floats of workspace direction `dir` needs, 0 for
+ * the register-staged route (then workspace may be NULL); a smaller workspace returns KT_ERR_WORKSPACE. */
+int64_t kt_conv1d_tc_workspace(const KtConv1dDesc* d, int32_t dir);
 int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
-                     float* y, void* stream);
+                     float* y, float* workspace, int64_t workspace_floats, void* stream);
 int kt_conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
-                          float* dx, void* stream);
+                          float* dx, float* workspace, int64_t workspace_floats, void* stream);
 
 /* tensor-core weight gradient (time is the contraction dimension; split-K partial tiles go to `workspace`,
  * a second kernel reduces them -- a single split writes dw / dbias directly).  Plain convs with channel counts % 8 == 0
@@ -332,6 +337,10 @@ int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float*
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */
 int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out12);
+/* Test aid (no GPU needed): the plan kt_conv1d_{fwd,bwd_data}_tc would make for direction `dir` on a GPU box.
+ * out9 = {N tile (0: not on the tensor cores), TMA route, time steps per M tile, rows per M tile, time steps per image box,
+ * image stages, weight stages, shared-memory bytes, workspace floats}; tile and stage entries describe the first launch. */
+int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t* out9);
 
 /* library info */
 const char* kt_last_error(void);

@@ -71,8 +71,9 @@ PROTOTYPES = {
     "kt_conv1d_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_conv1d_tc_image_bytes": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_weight_pack_tc": [ctypes.POINTER(KtConv1dDesc), _I, _P, _P, _P],
-    "kt_conv1d_fwd_tc": [ctypes.POINTER(KtConv1dDesc), _P, _P, _P, _P, _P, _P],
-    "kt_conv1d_bwd_data_tc": [ctypes.POINTER(KtConv1dDesc), _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_tc_workspace": [ctypes.POINTER(KtConv1dDesc), _I],
+    "kt_conv1d_fwd_tc": [ctypes.POINTER(KtConv1dDesc), _P, _P, _P, _P, _P, _P, _L, _P],
+    "kt_conv1d_bwd_data_tc": [ctypes.POINTER(KtConv1dDesc), _P, _P, _P, _P, _P, _P, _L, _P],
     "kt_conv1d_bwd_weight_tc_workspace": [ctypes.POINTER(KtConv1dDesc)],
     "kt_conv1d_bwd_weight_tc": [ctypes.POINTER(KtConv1dDesc), _P, _P, _P, _P, _P, _P, _L, _P],
     "kt_ar_duration_infer": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _P],
@@ -95,6 +96,7 @@ PROTOTYPES = {
     "kt_fp_insert_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_fp_insert_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
+    "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_version": [],
     "kt_has_tc": [],
 }

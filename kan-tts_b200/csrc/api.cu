@@ -25,8 +25,11 @@ int tc_plan(const KtConv1dDesc*, int);
 void debug_wgrad_plan(const KtConv1dDesc*, int*);
 long long tc_image_bytes(const KtConv1dDesc*, int);
 int tc_pack_layer(const KtConv1dDesc*, int, const float*, void*, cudaStream_t);
-int conv1d_fwd_tc(const KtConv1dDesc*, const float*, const void*, const float*, const float*, float*, cudaStream_t);
-int conv1d_bwd_data_tc(const KtConv1dDesc*, const float*, const float*, const void*, const float*, float*, cudaStream_t);
+long long conv_tc_workspace(const KtConv1dDesc*, int);
+void debug_conv_tc_plan(const KtConv1dDesc*, int, long long*);
+int conv1d_fwd_tc(const KtConv1dDesc*, const float*, const void*, const float*, const float*, float*, float*, long long, cudaStream_t);
+int conv1d_bwd_data_tc(const KtConv1dDesc*, const float*, const float*, const void*, const float*, float*, float*, long long, cudaStream_t,
+                       bool allow_tma = true);
 int ar_duration_infer(const float*, const float*, const float*, const float*, const float*, const float*, const float*, const float*,
                       const float*, const float*, const float*, float, float*, int, int, int, int, int, cudaStream_t);
 int resblock_plan(const KtResblockDesc*);
@@ -113,6 +116,13 @@ int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out12) {
   kt::debug_wgrad_plan(d, out12);
   return KT_OK;
 }
+int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t* out9) {
+  KT_REQUIRE(d && out9, "kt_debug_conv_tc_plan: null pointer");
+  long long v[9];
+  kt::debug_conv_tc_plan(d, dir, v);
+  for (int i = 0; i < 9; ++i) out9[i] = v[i];
+  return KT_OK;
+}
 int kt_upsample_grad_reduce(const float* dxu, const float* x, int32_t act_in, float act_in_slope, float* dx, int64_t rows,
                             int32_t up, int32_t c, void* stream) {
   return kt::upsample_grad_reduce(dxu, x, act_in, act_in_slope, dx, rows, up, c, ST(stream));
@@ -135,7 +145,7 @@ int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float*
 }
 
 const char* kt_last_error(void) { return kt::last_error(); }
-int kt_version(void) { return 3; }
+int kt_version(void) { return 4; }
 int kt_has_tc(void) { return 1; }
 
 int kt_conv1d_tc_plan(const KtConv1dDesc* d, int32_t dir) {
@@ -151,12 +161,16 @@ int kt_weight_pack_tc(const KtConv1dDesc* d, int32_t dir, const float* w, void* 
   if (rc) return rc;
   return kt::tc_pack_layer(d, dir, w, out, ST(stream));
 }
+int64_t kt_conv1d_tc_workspace(const KtConv1dDesc* d, int32_t dir) {
+  if (kt::validate_conv(d)) return 0;
+  return kt::conv_tc_workspace(d, dir);
+}
 int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
-                     float* y, void* stream) {
+                     float* y, float* workspace, int64_t workspace_floats, void* stream) {
   int rc = kt::validate_conv(d);
   if (rc) return rc;
   KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc: null pointer");
-  return kt::conv1d_fwd_tc(d, x, wimg, bias, resid, y, ST(stream));
+  return kt::conv1d_fwd_tc(d, x, wimg, bias, resid, y, workspace, workspace_floats, ST(stream));
 }
 int64_t kt_conv1d_bwd_weight_tc_workspace(const KtConv1dDesc* d) {
   if (kt::validate_conv(d)) return 0;
@@ -170,11 +184,11 @@ int kt_conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* 
   return kt::conv1d_bwd_weight_tc(d, x, dy, y, dw, dbias, workspace, workspace_floats, ST(stream));
 }
 int kt_conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
-                          float* dx, void* stream) {
+                          float* dx, float* workspace, int64_t workspace_floats, void* stream) {
   int rc = kt::validate_conv(d);
   if (rc) return rc;
   KT_REQUIRE(dy && wimg && dx, "kt_conv1d_bwd_data_tc: null pointer");
-  return kt::conv1d_bwd_data_tc(d, dy, y, wimg, x, dx, ST(stream));
+  return kt::conv1d_bwd_data_tc(d, dy, y, wimg, x, dx, workspace, workspace_floats, ST(stream));
 }
 
 int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, const float* w2t, const float* b2, const float* wih0t,
@@ -202,9 +216,10 @@ int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float*
                  d2->t_out == d2->t_in && d1->batch == d2->batch && d1->nsub == 1 && d2->nsub == 1,
              "kt_resblock_bwd: descriptors are not a (convs1[i], convs2[i]) pair of a ResidualBlock");
   // dh = c2^T(dy) * lrelu'(h);  dx = c1^T(dh) * lrelu'(x) + dy   (the residual path, layers.py:219)
-  int rc = kt::conv1d_bwd_data_tc(d2, dy, nullptr, wimg2_bwd, h, dh, ST(stream));
+  // (register-staged route: this entry point takes no workspace)
+  int rc = kt::conv1d_bwd_data_tc(d2, dy, nullptr, wimg2_bwd, h, dh, nullptr, 0, ST(stream), false);
   if (rc) return rc;
-  rc = kt::conv1d_bwd_data_tc(d1, dh, nullptr, wimg1_bwd, x, dx, ST(stream));
+  rc = kt::conv1d_bwd_data_tc(d1, dh, nullptr, wimg1_bwd, x, dx, nullptr, 0, ST(stream), false);
   if (rc) return rc;
   const long long n = (long long)d1->batch * d1->t_in * d1->c_in;
   return kt::add3_scale(dx, dy, nullptr, 1.f, dx, n, ST(stream));

@@ -19,6 +19,13 @@
 //   warpgroups 1 / 2  wgmma (M = 64 rows each, N = NT, K = 16) x 4 k-slices x 3 products per (chunk, tap) into
 //              register accumulators, then the epilogue of their 64 rows: bias / activation / residual (or act'
 //              mask for the data gradient), stores to the channels-last output.
+//
+// TMA-fed route (plain convs, channel counts % 8 == 0, see make_tc_plan): warpgroup 0 is the bound of the layers with
+// few taps per image -- every CTA converts its own copy of each image, once per N tile -- so the call first writes the
+// transformed gathered operand ONCE as hi / lo bf16 planes (split_planes, the weight gradient's layout) and one elected
+// thread pulls each image as two SWIZZLE_128B boxes (64 channels x nsub x a_box_t time steps, one per plane) straight into
+// the stage the consumers read.  A box starts at a whole time step, so an M tile is tt whole time steps x nsub rows
+// (R = tt * nsub <= 128); the consumers still issue M = 128 and the epilogue discards rows r >= R.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -121,20 +128,44 @@ struct TcParams {
   int ntaps;
   int tap_j[kMaxTaps];                // weight tap index, ordered by group
   int tap_shift[kMaxTaps];            // image row shift (q_n - q_lo) * nsub
+  int span_q;                         // largest tap span (q_hi - q_lo) of a residue group
+  // output rows per m-tile: kTcM on the register-staged route; tt whole time steps x nsub on the TMA route
+  int R, tt;
+  int a_box_t;                        // TMA route: time steps per image box = tt + span_q
 };
 
-// Warp roles (416 threads): warpgroup 0 stages activations; warpgroups 1 and 2 are the consumers -- each runs the wgmma
-// of one 64-row half of the 128-row tile into its registers and that half's epilogue; warp 12 streams weights.  (Warps
-// hold registers in groups of four: 13 warps keep the 128 registers per thread the consumers' accumulators need.)
+// TMA route: one tensor map of the gathered operand's planes per input residue class rho (base + rho rows, time stride
+// i_step), as wgrad_tma_kernel's map_a[]
+struct TcTmaMaps {
+  alignas(64) CUtensorMap map[kTcMaxGroups];
+};
+
+// Warp roles, register-staged route (416 threads): warpgroup 0 stages activations; warpgroups 1 and 2 are the consumers --
+// each runs the wgmma of one 64-row half of the 128-row tile into its registers and that half's epilogue; warp 12 streams
+// weights.  (Warps hold registers in groups of four: 13 warps keep the 128 registers per thread the consumers'
+// accumulators need.)  TMA route (320 threads): warpgroups 0 and 1 are the consumers, warp 8 issues the image boxes,
+// warp 9 streams weights.
 constexpr int kTcThreads = 416;
+constexpr int kTcTmaThreads = 320;
 constexpr int kTcConsumerArrivals = 8;   // one per consumer warp
+
+// Kernel instances.  REG_SIMPLE: register-staged, nsub == 1, up == 1, vectorisable channel counts, no tanh / accumulate --
+// the generator's resblock convs, the scale discriminator and every SAM-BERT linear / conv (see stage_rows); it exists
+// because the generic staging code made one kernel too large for the instruction cache.  REG: every other
+// register-staged layer.  TMA: the TMA-fed route (no staging code, one instance).
+enum TcRoute { kTcRegSimple = 0, kTcReg = 1, kTcTma = 2 };
 
 // Persistent: gridDim.x = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  The activation and
 // weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
-// SIMPLE = true: nsub == 1, up == 1, vectorisable channel counts, no tanh / accumulate -- the generator's resblock
-// convs, the scale discriminator and every SAM-BERT linear / conv (see stage_rows).  false: everything else.
-template <bool SIMPLE>
-__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ TcParams p) {
+template <int ROUTE>
+__global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
+    conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
+  constexpr bool SIMPLE = ROUTE == kTcRegSimple;
+  constexpr bool TMA = ROUTE == kTcTma;
+  constexpr int kConsumer0 = TMA ? 0 : 4;     // first consumer warp
+  constexpr int kWeightWarp = TMA ? 9 : 12;
+  // rows per m-tile: a compile-time 128 on the register-staged route (those instances are at their 128-register cap)
+  const int R = TMA ? p.R : kTcM;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);          // carve-up: all image / tile bases 1024-byte aligned
   const int img_bytes = p.rows * 128;                 // one plane of one activation stage
@@ -151,11 +182,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   uint32_t* s_tapshift = reinterpret_cast<uint32_t*>(empty_b + p.nb_stages);   // [kMaxTaps]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mtiles = p.ph_mt0[p.nphases];   // m-tiles of all phases (each: 128 flattened outputs m * nsub + w)
+  const int mtiles = p.ph_mt0[p.nphases];   // m-tiles of all phases (each: R flattened outputs m * nsub + w)
   const int total_tiles = mtiles * p.ntiles * p.batch;
 
   if (tid == 0) {
-    for (int s = 0; s < p.na_stages; ++s) { mbar_init(&full_a[s], 128); mbar_init(&empty_a[s], kTcConsumerArrivals); }
+    for (int s = 0; s < p.na_stages; ++s) { mbar_init(&full_a[s], TMA ? 1 : 128); mbar_init(&empty_a[s], kTcConsumerArrivals); }
     for (int s = 0; s < p.nb_stages; ++s) { mbar_init(&full_b[s], 1); mbar_init(&empty_b[s], kTcConsumerArrivals); }
     mbar_fence_init();
     fence_proxy_async();
@@ -163,8 +194,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   if (tid < kMaxTaps) s_tapshift[tid] = (uint32_t)p.tap_shift[tid] * 8u;
   __syncthreads();
 
-  if (warp < 4) {
-    // ===================== activation producers =====================
+  if (!TMA && warp < 4) {
+    // ===================== activation producers (register-staged) =====================
     const int ptid = tid;
     RingPos ra;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -189,7 +220,39 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 12) {
+  } else if (TMA && warp == 8) {
+    // ===================== activation producer (TMA) =====================
+    // Image row r = (time step m0 + qlo + r / nsub of residue class rho, sub-sequence r % nsub): the register-staged row map
+    // with f0 = mt * R.  Time steps outside [0, T) -- left padding included -- and channels past c_in arrive as the TMA
+    // unit's zeros.  In a block-diagonal grouped tile (kg < 64) the box also brings the next tile's real channels: they meet
+    // zero weight rows, and kslices stops the MMAs at the last K = 16 slice holding this tile's channels.  Rows past the box
+    // keep whatever an earlier image left there: they feed only the discarded output rows r >= R, and the stage holds
+    // p.rows >= 128 + span_q * nsub rows, so every row an MMA reads lies inside it.
+    if (elect_one()) {
+      const uint32_t box_bytes = (uint32_t)(p.a_box_t * p.nsub) * 128u;
+      RingPos ra;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int gm = tile % mtiles, bb = tile / (mtiles * p.ntiles);
+        int ph = 0;
+        while (gm >= p.ph_mt0[ph + 1]) ++ph;
+        const int ch_base = p.grouped ? ((tile / mtiles) % p.ntiles) * p.kg : 0;
+        const int m0 = (gm - p.ph_mt0[ph]) * p.tt;
+        for (int c = 0; c < p.kchunks; ++c) {
+          for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ra.advance(p.na_stages)) {
+            const int s = ra.slot();
+            mbar_wait(&empty_a[s], ra.phase() ^ 1u);
+            uint8_t* img_hi = a_base + (size_t)s * a_stage_bytes;
+            const CUtensorMap* map = &maps.map[p.grp_rho[g]];
+            mbar_arrive_expect_tx(&full_a[s], 2u * box_bytes);
+            tma_load_5d(img_hi, map, ch_base + c * kTcKC, 0, m0 + p.grp_qlo[g], bb, 0, &full_a[s]);
+            tma_load_5d(img_hi + img_bytes, map, ch_base + c * kTcKC, 0, m0 + p.grp_qlo[g], bb, 1, &full_a[s]);
+          }
+        }
+      }
+      // every issued box has landed before the CTA may exit: the consumers waited for all of them
+    }
+    __syncwarp();
+  } else if (warp == kWeightWarp) {
     // ===================== weight stream (bulk async copies) =====================
     const bool leader = elect_one();
     if (leader && p.w_resident) {
@@ -224,11 +287,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       }
     }
     __syncwarp();
-  } else if (warp >= 4 && warp < 12) {
+  } else if (warp >= kConsumer0 && warp < kConsumer0 + 8) {
     // ===================== consumers: wgmma + epilogue, one 64-row half of the tile per warpgroup =====================
     // Descriptor low words + 32-bit adds only: a tap's row shift, the K = 16 slice offset (32 bytes = 2 units), the hi -> lo
     // plane distance and this warpgroup's 64-row offset (8 KB = 512 units) are integer adds on the low word.
-    const int cw = (warp - 4) >> 2;                  // 0: rows 0-63, 1: rows 64-127
+    const int cw = (warp - kConsumer0) >> 2;         // 0: rows 0-63, 1: rows 64-127
     const int wq = warp & 3;                         // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of the half
     const uint32_t a_base16 = (smem_u32(a_base) >> 4) + (uint32_t)cw * 512u;
     const uint32_t b_base16 = smem_u32(b_base) >> 4;
@@ -288,8 +351,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int f = mt * kTcM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
-          if (f >= F) continue;
+          const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;   // row of the M = 128 accumulator tile
+          const int f = mt * R + r;
+          if ((TMA && r >= R) || f >= F) continue;
           const int m = p.nsub == 1 ? f : f / p.nsub;
           const int w = f - m * p.nsub;
           const int to = p.ph_ooff[ph] + p.o_step * m;
@@ -398,7 +462,7 @@ static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
 // Append one phase (its residue groups and taps) to the launch parameters.  Returns false when the
 // phase does not fit the kernel's limits.  Call reset_phases() first.
 static void reset_phases(TcParams& p) {
-  p.nphases = 0; p.ngroups = 0; p.ntaps = 0; p.rows = 0;
+  p.nphases = 0; p.ngroups = 0; p.ntaps = 0; p.rows = 0; p.span_q = 0;
   p.ph_mt0[0] = 0; p.ph_g0[0] = 0; p.grp_first[0] = 0;
 }
 
@@ -434,10 +498,11 @@ static bool add_phase(TcParams& p, const Phase& ph, int nsub) {
       }
     p.grp_first[p.ngroups] = p.ntaps;
     max_span = std::max(max_span, (qhi - qlo) * nsub);
+    p.span_q = std::max(p.span_q, qhi - qlo);
   }
   const int i = p.nphases++;
   p.ph_M[i] = ph.M; p.ph_ooff[i] = ph.o_off;
-  p.ph_mt0[i + 1] = p.ph_mt0[i] + ceil_div(ph.M * nsub, kTcM);
+  p.ph_mt0[i + 1] = p.ph_mt0[i] + ceil_div(ph.M * nsub, p.R);
   p.ph_g0[i + 1] = p.ngroups;
   p.rows = std::max(p.rows, (kTcM + max_span + 7) & ~7);
   return p.rows <= kTcMaxRows;
@@ -462,19 +527,78 @@ static bool plan_launches(const std::vector<Phase>& phases, int nsub, std::vecto
   return true;
 }
 
-// Is (direction dir: 0 fwd, 1 bwd_data) of this layer runnable on the tensor-core kernel?  -> N tile or 0
 bool thin_cin1_ok(const KtConv1dDesc* d);   // thin.cu
 
-int tc_plan(const KtConv1dDesc* d, int dir) {
-  if (dir == 0 && d->path != KT_PATH_TC && thin_cin1_ok(d)) return 0;   // waveform-input layers: HBM-bound FIR kernel
-  if (dir == 1 && d->upsample > 1) return 0;          // no direct plan: ops.ConvPlan runs it as the plain conv over
-                                                      // the up-sampled rows + kt_upsample_grad_reduce
-  const TcLayerPlan L = layer_plan(d, dir);
-  if (!L.ok) return 0;
+// What a call of direction dir (0 forward, 1 data gradient) of a layer runs: the tiling, the launches (phases planned,
+// pointers filled in by the caller) and the route.  The gathered operand is x (c_in channels, t_in rows) for the forward
+// and dy (c_out channels, t_out rows) for the data gradient.
+struct TcPlan {
+  bool ok;                          // the tensor-core kernel runs this direction
+  bool tma;                         // TMA-fed route, else register-staged
+  TcLayerPlan L;
   std::vector<TcParams> launches;
-  if (!plan_launches(conv_phases(d, dir), d->nsub, launches, TcParams{})) return 0;
-  return L.NT;
+  long long ws_floats;              // TMA route: hi / lo bf16 planes of the gathered operand (one float per element)
+};
+
+// Does the split pass pay for itself?  It moves ~12 bytes per gathered element through HBM (read fp32, write and re-read
+// two bf16 planes) to take the staging off the CTAs.  Measured per layer in the C2 step (H100 SXM, 700 W, both routes):
+//   wins  dense layers with >= 2 N tiles (the staging was repeated per N tile): MPD 1024 -> 1024 k5 fwd / dgrad 0.29-0.38
+//         -> 0.24 ms, MPD 512 -> 1024 s3 dgrad 0.41 -> 0.17 ms, 256 -> 256 k3 dgrad 0.44 -> 0.21 ms; and small gathered
+//         tensors, whose planes stay in L2 (MSD 1024 -> 1 k3 fwd 0.33 -> 0.20 ms, MPD 1 -> 32 s3 dgrad 0.65 -> 0.26 ms)
+//   losses one N tile over >= 4 M elements (generator 128 -> 128 k3 fwd 0.55 -> 0.78 ms, MPD 128 -> 512 s3 dgrad at
+//         15 M elements 0.22 -> 0.55 ms: HBM-bound already), and grouped layers on balance (MSD g16 dgrads 0.29 -> 0.59,
+//         0.61 -> 0.83, 0.29 -> 0.50 ms against g4 / g16 dgrad wins of 0.34 and 0.32 ms)
+// Below 512 K gathered elements no producer is the bound (the C2 step's 1024-channel layers at 9 time steps: 0.20 vs 0.21 ms)
+// and the split pass is one more launch, plus the tensor maps encoded on the host, in latency-bound calls (batch-1 inference).
+static bool tma_pays(const TcParams& lp) {
+  const long long elems = (long long)lp.batch * lp.t_in * lp.nsub * lp.c_in;   // gathered operand
+  return !lp.grouped && elems >= (1LL << 19) && (lp.ntiles >= 2 || elems < (1LL << 22));
 }
+
+static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true, bool plan_only = false) {
+  TcPlan P{};
+  if (dir == 0 && d->path != KT_PATH_TC && thin_cin1_ok(d)) return P;   // waveform-input layers: HBM-bound FIR kernel
+  if (dir == 1 && d->upsample > 1) return P;   // no direct plan: ops.ConvPlan runs it as the plain conv over the
+                                               // up-sampled rows + kt_upsample_grad_reduce
+  P.L = layer_plan(d, dir);
+  const TcLayerPlan& L = P.L;
+  if (!L.ok) return P;
+  TcParams base{};
+  base.NT = L.NT; base.ntiles = L.ntiles; base.kchunks = L.kchunks; base.kg = L.kg; base.grouped = L.grouped; base.n_stride = L.n_stride;
+  base.batch = d->batch; base.nsub = d->nsub;
+  // roles swap for the data gradient: the gathered tensor is dy, the product is dx
+  base.t_in = dir == 0 ? d->t_in : d->t_out; base.t_out = dir == 0 ? d->t_out : d->t_in;
+  base.c_in = dir == 0 ? d->c_in : d->c_out; base.c_out = dir == 0 ? d->c_out : d->c_in;
+  const std::vector<Phase> phases = conv_phases(d, dir);
+  // TMA route: no nearest-upsampling (the planes hold the tensor as stored), 16-byte aligned box coordinates and strides
+  // (the gathered width and the channels per tile % 8), box extents <= 256 and a time step in every residue class
+  bool tma = allow_tma && d->upsample == 1 && base.c_in % 8 == 0 && L.kg % 8 == 0 && d->nsub <= kTcM &&
+             (plan_only || encode_tiled_fn() != nullptr);
+  if (tma) {
+    base.tt = kTcM / d->nsub; base.R = base.tt * d->nsub;
+    tma = plan_launches(phases, d->nsub, P.launches, base);
+    for (TcParams& lp : P.launches) {
+      lp.a_box_t = lp.tt + lp.span_q;
+      tma = tma && lp.up == 1 && lp.a_box_t <= 256 && lp.t_in >= lp.i_step && tma_pays(lp);
+    }
+  }
+  if (!tma) {
+    P.launches.clear();
+    base.tt = 0; base.R = kTcM;
+    if (!plan_launches(phases, d->nsub, P.launches, base)) return P;
+  }
+  P.ok = true;
+  P.tma = tma;
+  P.ws_floats = tma ? ((long long)base.batch * base.t_in * base.nsub * base.c_in + 63) & ~63LL : 0;
+  return P;
+}
+
+int tc_plan(const KtConv1dDesc* d, int dir) {
+  const TcPlan P = make_tc_plan(d, dir);
+  return P.ok ? P.L.NT : 0;
+}
+
+long long conv_tc_workspace(const KtConv1dDesc* d, int dir) { return make_tc_plan(d, dir).ws_floats; }
 
 // bytes of the packed split-bf16 weight image of direction `dir` (0 when unsupported)
 long long tc_image_bytes(const KtConv1dDesc* d, int dir) {
@@ -494,11 +618,11 @@ int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cud
   return KT_OK;
 }
 
-static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned by plan_launches
+// Ring sizes of one launch -> its shared-memory bytes (0: the stages do not fit)
+static size_t size_stages(TcParams& p) {
   const int a_stage = 2 * p.rows * 128;
   const int b_stage = 2 * p.NT * 128;
   const int slots = p.ntaps * p.kchunks;                                      // weight tiles of the whole layer
-  const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
   const int bar_bytes = tc_fixed_smem(slots);
   const int budget = kMaxDynSmem - 1024 /*align slack*/ - bar_bytes;
   p.w_resident = 0;
@@ -515,16 +639,43 @@ static int run_tc(TcParams p, cudaStream_t st) {   // p: phases already planned 
     if (3 * a_stage + 2 * b_stage > budget) p.na_stages = 2;
     p.nb_stages = std::min(6, (budget - p.na_stages * a_stage) / b_stage);
   }
-  KT_REQUIRE(p.nb_stages >= 2 || p.w_resident, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
-  const size_t smem = 1024 + (size_t)p.na_stages * a_stage + (size_t)p.nb_stages * b_stage + bar_bytes;
-  KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<true>>(kMaxDynSmem));
-  KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<false>>(kMaxDynSmem));
+  if (p.nb_stages < 2 && !p.w_resident) return 0;
+  return 1024 + (size_t)p.na_stages * a_stage + (size_t)p.nb_stages * b_stage + bar_bytes;
+}
+
+// development / test aid (kt_debug_conv_tc_plan): the plan of direction dir as it would be made on a GPU box
+// out = {N tile (0: not on the tensor cores), TMA route, tt, R, a_box_t, image stages, weight stages, shared-memory bytes,
+// workspace floats}, the launch-dependent entries for the first launch
+void debug_conv_tc_plan(const KtConv1dDesc* d, int dir, long long* out) {
+  TcPlan P = make_tc_plan(d, dir, true, true);
+  for (int i = 0; i < 9; ++i) out[i] = 0;
+  if (!P.ok) return;
+  TcParams& lp = P.launches[0];
+  const size_t smem = size_stages(lp);
+  out[0] = P.L.NT; out[1] = P.tma; out[2] = lp.tt; out[3] = lp.R; out[4] = lp.a_box_t;
+  out[5] = lp.na_stages; out[6] = lp.nb_stages; out[7] = (long long)smem; out[8] = P.ws_floats;
+}
+
+static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, cudaStream_t st) {   // p: phases already planned
+  const size_t smem = size_stages(p);
+  KT_REQUIRE(smem > 0, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
+  const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
   const int grid = (int)std::min<long long>(tiles, device_sm_count());
-  const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
-                      (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
-                      (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
-  if (simple) conv_tc_kernel<true><<<grid, kTcThreads, smem, st>>>(p);
-  else conv_tc_kernel<false><<<grid, kTcThreads, smem, st>>>(p);
+  if (tma) {
+    KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcTma>>(kMaxDynSmem));
+    conv_tc_kernel<kTcTma><<<grid, kTcTmaThreads, smem, st>>>(p, maps);
+  } else {
+    const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
+                        (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
+                        (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
+    if (simple) {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple>>(kMaxDynSmem));
+      conv_tc_kernel<kTcRegSimple><<<grid, kTcThreads, smem, st>>>(p, maps);
+    } else {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg>>(kMaxDynSmem));
+      conv_tc_kernel<kTcReg><<<grid, kTcThreads, smem, st>>>(p, maps);
+    }
+  }
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
@@ -537,48 +688,69 @@ static Side make_side_tc(const float* p, const float* aux, int act, float slope,
   return s;
 }
 
-int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
-                  float* y, cudaStream_t st) {
-  KT_REQUIRE(tc_plan(d, 0) > 0, "conv1d_fwd_tc: layer not supported by the tensor-core path");
-  const TcLayerPlan L = layer_plan(d, 0);
-  TcParams p{};
-  p.NT = L.NT; p.ntiles = L.ntiles; p.kchunks = L.kchunks; p.kg = L.kg; p.grouped = L.grouped; p.n_stride = L.n_stride;
-  p.in = make_side_tc(x, nullptr, d->act_in, d->act_in_slope, false);
-  p.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
-  p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
-  p.batch = d->batch; p.nsub = d->nsub; p.t_in = d->t_in; p.t_out = d->t_out; p.c_in = d->c_in; p.c_out = d->c_out;
-  p.out_act = d->act_out; p.out_slope = d->act_out_slope;
-  std::vector<TcParams> launches;
-  KT_REQUIRE(plan_launches(conv_phases(d, 0), d->nsub, launches, p), "conv1d_fwd_tc: phases exceed kernel limits");
-  for (const TcParams& lp : launches) {
-    int rc = run_tc(lp, st);
+// Every launch of plan P with the operands of `io` (in, wimg, bias, resid, mask, out, out_act, out_slope).  The TMA route
+// first writes the gathered operand's planes into ws.
+static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws_floats, const char* what, cudaStream_t st) {
+  TcTmaMaps maps{};
+  __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(ws);
+  if (P.tma) {
+    if (ws == nullptr || ws_floats < P.ws_floats) {
+      set_error("%s: workspace too small (%lld < %lld floats)", what, ws_floats, P.ws_floats);
+      return KT_ERR_WORKSPACE;
+    }
+    const TcParams& g = P.launches[0];
+    KT_CHECK_CUDA(split_planes(io.in, (long long)g.batch * g.t_in * g.nsub * g.c_in, planes, Side{nullptr, nullptr, 0, 0.f}, 0,
+                               nullptr, st));
+  }
+  for (TcParams lp : P.launches) {
+    lp.in = io.in; lp.wimg = io.wimg; lp.bias = io.bias; lp.resid = io.resid; lp.mask = io.mask; lp.out = io.out;
+    lp.out_act = io.out_act; lp.out_slope = io.out_slope;
+    if (P.tma) {
+      // planes [hi | lo][batch][time][sub-sequence][channel]; residue class rho = time steps rho, rho + i_step, ...
+      const long long n = (long long)lp.batch * lp.t_in * lp.nsub * lp.c_in;
+      for (int rho = 0; rho < lp.i_step; ++rho) {
+        const cuuint64_t gdim[5] = {(cuuint64_t)lp.c_in, (cuuint64_t)lp.nsub, (cuuint64_t)ceil_div(lp.t_in - rho, lp.i_step),
+                                    (cuuint64_t)lp.batch, 2};
+        const cuuint64_t gstr[4] = {(cuuint64_t)lp.c_in * 2, (cuuint64_t)lp.i_step * lp.nsub * lp.c_in * 2,
+                                    (cuuint64_t)lp.t_in * lp.nsub * lp.c_in * 2, (cuuint64_t)n * 2};
+        const cuuint32_t box[5] = {kTcKC, (cuuint32_t)lp.nsub, (cuuint32_t)lp.a_box_t, 1, 1};
+        const int rc = encode_tensor_map(&maps.map[rho], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, planes + (long long)rho * lp.nsub * lp.c_in,
+                                         gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
+        if (rc) return rc;
+      }
+    }
+    const int rc = run_tc(lp, maps, P.tma, st);
     if (rc) return rc;
   }
   return KT_OK;
 }
 
+int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
+                  float* y, float* ws, long long ws_floats, cudaStream_t st) {
+  const TcPlan P = make_tc_plan(d, 0);
+  KT_REQUIRE(P.ok, "conv1d_fwd_tc: layer not supported by the tensor-core path");
+  TcParams io{};
+  io.in = make_side_tc(x, nullptr, d->act_in, d->act_in_slope, false);
+  io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
+  io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
+  io.out_act = d->act_out; io.out_slope = d->act_out_slope;
+  return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", st);
+}
+
+// allow_tma = false: the register-staged route, which needs no workspace (kt_resblock_bwd)
 int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
-                       float* dx, cudaStream_t st) {
-  KT_REQUIRE(tc_plan(d, 1) > 0, "conv1d_bwd_data_tc: layer not supported by the tensor-core path");
-  const TcLayerPlan L = layer_plan(d, 1);
+                       float* dx, float* ws, long long ws_floats, cudaStream_t st, bool allow_tma) {
+  const TcPlan P = make_tc_plan(d, 1, allow_tma);
+  KT_REQUIRE(P.ok, "conv1d_bwd_data_tc: layer not supported by the tensor-core path");
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_data: y required when act_out != NONE");
   KT_REQUIRE(d->act_in == KT_ACT_NONE || x != nullptr, "bwd_data: x required when act_in != NONE");
-  TcParams p{};
-  p.NT = L.NT; p.ntiles = L.ntiles; p.kchunks = L.kchunks; p.kg = L.kg; p.grouped = L.grouped; p.n_stride = L.n_stride;
-  p.in = make_side_tc(dy, y, d->act_out, d->act_out_slope, true);
-  p.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
-  p.bias = nullptr; p.resid = nullptr; p.out = dx;
-  p.mask = d->act_in == KT_ACT_LRELU ? Side{x, nullptr, SIDE_DLRELU, d->act_in_slope} : Side{nullptr, nullptr, 0, 0.f};
-  // roles swap: the gathered tensor is dy (c_out channels, t_out rows), the product is dx
-  p.batch = d->batch; p.nsub = d->nsub; p.t_in = d->t_out; p.t_out = d->t_in; p.c_in = d->c_out; p.c_out = d->c_in;
-  p.out_act = KT_ACT_NONE; p.out_slope = 0.f;
-  std::vector<TcParams> launches;
-  KT_REQUIRE(plan_launches(conv_phases(d, 1), d->nsub, launches, p), "conv1d_bwd_data_tc: phases exceed kernel limits");
-  for (const TcParams& lp : launches) {
-    int rc = run_tc(lp, st);
-    if (rc) return rc;
-  }
-  return KT_OK;
+  TcParams io{};
+  io.in = make_side_tc(dy, y, d->act_out, d->act_out_slope, true);
+  io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
+  io.bias = nullptr; io.resid = nullptr; io.out = dx;
+  io.mask = d->act_in == KT_ACT_LRELU ? Side{x, nullptr, SIDE_DLRELU, d->act_in_slope} : Side{nullptr, nullptr, 0, 0.f};
+  io.out_act = KT_ACT_NONE; io.out_slope = 0.f;
+  return run_plan(P, io, ws, ws_floats, "conv1d_bwd_data_tc", st);
 }
 
 }  // namespace kt

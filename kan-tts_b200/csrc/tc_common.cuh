@@ -5,6 +5,8 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -148,6 +150,49 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo
   }
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
+// fp32 operand -> hi / lo bf16 planes ([plane][batch][time][sub-sequence][channel], the activation layout), with the
+// operand's fused transform (pre-activation / activation-derivative mask) -- the same arithmetic as stage_rows, so a tile
+// pulled from the planes by the TMA unit holds the bits a register-staged tile would.  Two operands in ONE launch: CTAs
+// [0, blocks_a) convert operand A, the rest operand B (n8b = 0: none).  Static: every kernel file that feeds its tiles
+// from planes compiles its own instance of this one definition.
+static __global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16* __restrict__ hia, Side sb, long long n8b,
+                                           __nv_bfloat16* __restrict__ hib, int blocks_a) {
+  const bool first = (int)blockIdx.x < blocks_a;
+  const Side s = first ? sa : sb;
+  const long long n8 = first ? n8a : n8b;
+  __nv_bfloat16* hi = first ? hia : hib;
+  __nv_bfloat16* lo = hi + n8 * 8;
+  const long long b0 = first ? blockIdx.x : blockIdx.x - blocks_a, nb = first ? blocks_a : (long long)gridDim.x - blocks_a;
+  const bool has_aux = s.mode >= SIDE_DLRELU;
+  for (long long i = b0 * (long long)blockDim.x + threadIdx.x; i < n8; i += nb * blockDim.x) {
+    const float4 v0 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i), v1 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i + 1);
+    float x[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+    if (has_aux) {
+      const float4 a0 = __ldg(reinterpret_cast<const float4*>(s.aux) + 2 * i), a1 = __ldg(reinterpret_cast<const float4*>(s.aux) + 2 * i + 1);
+      const float ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[e] = side_apply(x[e], ax[e], s.mode, s.slope);
+    } else if (s.mode == SIDE_LRELU) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : x[e] * s.slope;
+    }
+    uint4 h, l;
+    split8(x, h, l);
+    reinterpret_cast<uint4*>(hi)[i] = h;
+    reinterpret_cast<uint4*>(lo)[i] = l;
+  }
+}
+
+// Launch split_planes_kernel over na elements of operand a into the planes at pa and nb elements of b into pb (na, nb
+// multiples of 8; nb = 0: one operand).
+static inline cudaError_t split_planes(const Side& a, long long na, __nv_bfloat16* pa, const Side& b, long long nb,
+                                       __nv_bfloat16* pb, cudaStream_t st) {
+  auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 132LL * 16)); };
+  const int ba = blocks_for(na / 8), bb = nb > 0 ? blocks_for(nb / 8) : 0;
+  split_planes_kernel<<<ba + bb, 256, 0, st>>>(a, na / 8, pa, b, nb / 8, pb, ba);
+  return cudaGetLastError();
 }
 
 }  // namespace tc

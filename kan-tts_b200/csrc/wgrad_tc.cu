@@ -261,36 +261,7 @@ struct WgTmaExtra {
   alignas(64) CUtensorMap map_a[8];   // one per residue class of the input
 };
 
-// fp32 operand -> hi / lo bf16 planes, with the operand's fused transform (pre-activation / activation-derivative mask)
-// (both operands of a layer in ONE launch: CTAs [0, blocks_a) convert operand A, the rest operand B)
-__global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16* __restrict__ hia, Side sb, long long n8b,
-                                    __nv_bfloat16* __restrict__ hib, int blocks_a) {
-  const bool first = (int)blockIdx.x < blocks_a;
-  const Side s = first ? sa : sb;
-  const long long n8 = first ? n8a : n8b;
-  __nv_bfloat16* hi = first ? hia : hib;
-  __nv_bfloat16* lo = hi + n8 * 8;
-  const long long b0 = first ? blockIdx.x : blockIdx.x - blocks_a, nb = first ? blocks_a : (long long)gridDim.x - blocks_a;
-  const bool has_aux = s.mode >= SIDE_DLRELU;
-  for (long long i = b0 * (long long)blockDim.x + threadIdx.x; i < n8; i += nb * blockDim.x) {
-    const float4 v0 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i), v1 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i + 1);
-    float x[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-    if (has_aux) {
-      const float4 a0 = __ldg(reinterpret_cast<const float4*>(s.aux) + 2 * i), a1 = __ldg(reinterpret_cast<const float4*>(s.aux) + 2 * i + 1);
-      const float ax[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-#pragma unroll
-      for (int e = 0; e < 8; ++e) x[e] = side_apply(x[e], ax[e], s.mode, s.slope);
-    } else if (s.mode == SIDE_LRELU) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : x[e] * s.slope;
-    }
-    uint4 h, l;
-    split8(x, h, l);
-    reinterpret_cast<uint4*>(hi)[i] = h;
-    reinterpret_cast<uint4*>(lo)[i] = l;
-  }
-}
-
+// (the operand planes are written by split_planes, tc_common.cuh)
 template <int NT>
 __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __grid_constant__ WgTcParams p, const __grid_constant__ WgTmaExtra x) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -653,10 +624,7 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
     __nv_bfloat16* pa = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_a_off);
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
-    auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 132LL * 16)); };
-    const int ba = blocks_for(na / 8), bb = blocks_for(nb / 8);
-    split_planes_kernel<<<ba + bb, 256, 0, st>>>(p.a, na / 8, pa, p.b, nb / 8, pb, ba);
-    KT_CHECK_CUDA(cudaGetLastError());
+    KT_CHECK_CUDA(split_planes(p.a, na, pa, p.b, nb, pb, st));
     {
       const cuuint64_t gdim[5] = {(cuuint64_t)p.cb, (cuuint64_t)p.nsub, (cuuint64_t)p.t_b, (cuuint64_t)p.batch, 2};
       const cuuint64_t gstr[4] = {(cuuint64_t)p.cb * 2, (cuuint64_t)p.nsub * p.cb * 2, (cuuint64_t)p.t_b * p.nsub * p.cb * 2, (cuuint64_t)nb * 2};

@@ -161,14 +161,15 @@ class ConvPlan:
       d                        the layer's descriptor
       nt_fwd                   forward N tile
       d_bwd, nt_bwd, up_bwd    data gradient: descriptor, N tile, and whether it runs over the up-sampled rows
+      ws_fwd, ws_bwd           tensor-core forward / data-gradient workspace (operand planes of the TMA-fed route), in floats
       wg_ws                    tensor-core weight-gradient workspace, in floats"""
 
-    __slots__ = ("spec", "d", "nt_fwd", "d_bwd", "nt_bwd", "up_bwd", "wg_ws")
+    __slots__ = ("spec", "d", "nt_fwd", "d_bwd", "nt_bwd", "up_bwd", "ws_fwd", "ws_bwd", "wg_ws")
 
     def __init__(self, spec, batch, nsub, t_in, exact):
         self.spec = spec
         self.d = self.d_bwd = d = spec.desc(batch, nsub, t_in)
-        self.nt_fwd = self.nt_bwd = self.wg_ws = 0
+        self.nt_fwd = self.nt_bwd = self.ws_fwd = self.ws_bwd = self.wg_ws = 0
         self.up_bwd = False
         if exact:
             return
@@ -183,6 +184,10 @@ class ConvPlan:
             nt2 = lib.kt_conv1d_tc_plan(ctypes.byref(d2), 1)
             if nt2:
                 self.d_bwd, self.nt_bwd, self.up_bwd = d2, nt2, True
+        if self.nt_fwd:
+            self.ws_fwd = int(lib.kt_conv1d_tc_workspace(ctypes.byref(d), 0))
+        if self.nt_bwd:
+            self.ws_bwd = int(lib.kt_conv1d_tc_workspace(ctypes.byref(self.d_bwd), 1))
         self.wg_ws = int(lib.kt_conv1d_bwd_weight_tc_workspace(ctypes.byref(d)))
 
     def tile(self, direction):
@@ -457,6 +462,13 @@ def _weight_backward(spec, plan, x_, dy, y_, v, g, params, norm, need_v, need_g,
     return dbias, dv, dg
 
 
+def _workspace(floats, device):
+    """Scratch of a tensor-core conv call (None when it needs none), from the caching allocator on the launching stream: it is
+    free again for later work on that stream once the call's kernels ran (and under graph capture it comes from the graph's
+    pool)."""
+    return torch.empty(floats, device=device, dtype=torch.float32) if floats else None
+
+
 class ConvFn(torch.autograd.Function):
     """y = act_out(conv(act_in(x)) + bias) + resid   on channels-last rows."""
 
@@ -486,8 +498,9 @@ class ConvFn(torch.autograd.Function):
         d, nt, n = run.d, run.tile(0), (spec.stride if spec.transposed else 1)
         if nt:
             img = pw.image((0, nt), d)
-            _run("conv_fwd_tc", spec, d, n, n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True), ptr(bd),
-                                                ptr(resid), ptr(y), stream_ptr()))
+            ws = _workspace(run.ws_fwd, x.device)
+            _run("conv_fwd_tc", spec, d, n + (ws is not None), n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True),
+                                                                   ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd, stream_ptr()))
         else:
             _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd", ctypes.byref(d), ptr(x), ptr(pw.w_fwd), ptr(bd),
                                                   ptr(resid), ptr(y), stream_ptr()))
@@ -528,13 +541,17 @@ class ConvFn(torch.autograd.Function):
             elif plan.up_bwd:
                 d2 = plan.d_bwd
                 dxu = torch.empty((ctx.nb, d2.t_in * d2.nsub, spec.c_in), device=x.device, dtype=torch.float32)
-                _run("conv_dgrad_tc", spec, d, n + 1, 1,
-                     ("kt_conv1d_bwd_data_tc", ctypes.byref(d2), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), None, ptr(dxu), st),
+                ws = _workspace(plan.ws_bwd, x.device)
+                _run("conv_dgrad_tc", spec, d, n + 1 + (ws is not None), 1,
+                     ("kt_conv1d_bwd_data_tc", ctypes.byref(d2), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), None, ptr(dxu),
+                      ptr(ws), plan.ws_bwd, st),
                      ("kt_upsample_grad_reduce", ptr(dxu), ptr(x_), spec.act_in, spec.act_in_slope, ptr(dx),
                       ctx.nb * d.t_in * d.nsub, spec.upsample, spec.c_in, st))
             else:
-                _run("conv_dgrad_tc", spec, d, n, 1, ("kt_conv1d_bwd_data_tc", ctypes.byref(d), ptr(dy), ptr(y_),
-                                                      ptr(ctx.img_bwd, True), ptr(x_), ptr(dx), st))
+                ws = _workspace(plan.ws_bwd, x.device)
+                _run("conv_dgrad_tc", spec, d, n + (ws is not None), 1,
+                     ("kt_conv1d_bwd_data_tc", ctypes.byref(d), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), ptr(x_), ptr(dx),
+                      ptr(ws), plan.ws_bwd, st))
         if ctx.has_resid and ctx.needs_input_grad[1]:
             # NOT the incoming tensor itself: the autograd engine accumulates gradients arriving at the same input IN PLACE
             # into the first arrival when it holds the last reference (input_buffer.cpp: can_accumulate_inplace), and
