@@ -76,6 +76,21 @@ struct Side {
   float slope;
 };
 
+// The Side of a tensor with a fused activation `act`: the pre-activation applied to the layer input (derivative = false, aux
+// unused), or the activation's derivative at aux applied to a gradient (derivative = true, aux = the activation's output)
+inline Side make_side(const float* p, const float* aux, int act, float slope, bool derivative) {
+  Side s{p, aux, SIDE_PLAIN, slope};
+  if (act == KT_ACT_LRELU) s.mode = derivative ? SIDE_DLRELU : SIDE_LRELU;
+  else if (act == KT_ACT_TANH) s.mode = derivative ? SIDE_DTANH : SIDE_PLAIN;
+  if (s.mode < SIDE_DLRELU) s.aux = nullptr;
+  return s;
+}
+
+// The data gradient's output mask: leaky_relu'(x) of a fused input LeakyReLU, else none
+inline Side dgrad_mask(const KtConv1dDesc* d, const float* x) {
+  return d->act_in == KT_ACT_LRELU ? Side{x, nullptr, SIDE_DLRELU, d->act_in_slope} : Side{nullptr, nullptr, 0, 0.f};
+}
+
 __device__ __forceinline__ float side_apply(float v, float aux, int mode, float slope) {
   switch (mode) {
     case SIDE_LRELU: return v > 0.f ? v : v * slope;
@@ -107,5 +122,31 @@ struct Phase {
   int min_ioff, max_ioff;
   int accumulate;
 };
+
+// The taps of a phase split into the residue classes of an input step (<= kMaxResidues): tap n reads time
+// q * step + rho of the input, with q = floor(tap_ioff[n] / step) and rho = tap_ioff[n] - q * step.  Class rho holds taps
+// [first[rho], first[rho + 1]) in phase order, so in a gather phase (tap_ioff increasing with j) by increasing (q, j).
+// The placeholder tap of an output residue no real tap reaches goes to class 0 at a q far outside every tensor: it
+// reads only zeros.
+constexpr int kMaxResidues = 8;
+struct ResidueTaps {
+  int first[kMaxResidues + 1];
+  int q[kMaxTaps], j[kMaxTaps];
+};
+
+inline ResidueTaps residue_taps(const Phase& ph, int step) {
+  ResidueTaps rt;
+  int n = 0;
+  for (int r = 0; r < step; ++r) {
+    rt.first[r] = n;
+    for (int t = 0; t < ph.ntaps; ++t) {
+      const bool placeholder = ph.tap_ioff[t] < -(1 << 24);
+      const int q = placeholder ? -(1 << 20) : fdiv(ph.tap_ioff[t], step);
+      if ((placeholder ? 0 : ph.tap_ioff[t] - q * step) == r) { rt.q[n] = q; rt.j[n] = ph.tap_j[t]; ++n; }
+    }
+  }
+  rt.first[step] = n;
+  return rt;
+}
 
 }  // namespace kt

@@ -575,7 +575,7 @@ static void finish_phase(Phase& ph) {
 
 // forward of a conv / data-gradient of a transposed conv: one gather phase
 //   out[to] = sum_j W_j in[(to*stride + j*dil - pad) / up]
-static Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up) {
+Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up) {
   Phase ph{};
   ph.M = t_out; ph.o_off = 0; ph.o_step = 1; ph.i_step = stride; ph.up = up; ph.accumulate = 0;
   ph.ntaps = kernel;
@@ -606,14 +606,6 @@ static std::vector<Phase> scatter_phases(int t_out, int kernel, int stride, int 
     v.push_back(ph);
   }
   return v;
-}
-
-static Side make_side(const float* p, const float* aux, int act, float slope, bool derivative) {
-  Side s{p, aux, SIDE_PLAIN, slope};
-  if (act == KT_ACT_LRELU) s.mode = derivative ? SIDE_DLRELU : SIDE_LRELU;
-  else if (act == KT_ACT_TANH) s.mode = derivative ? SIDE_DTANH : SIDE_PLAIN;
-  if (s.mode < SIDE_DLRELU) s.aux = nullptr;
-  return s;
 }
 
 // Phases of a layer: dir 0 = forward, dir 1 = data gradient (roles of t_in / t_out swapped by the caller).
@@ -673,7 +665,7 @@ int conv1d_bwd_data_ffma(const KtConv1dDesc* d, const float* dy, const float* y,
   KT_REQUIRE(d->act_in == KT_ACT_NONE || x != nullptr, "bwd_data: x required when act_in != NONE");
   p.in = make_side(dy, y, d->act_out, d->act_out_slope, true);
   p.w = w_bwd; p.bias = nullptr; p.resid = nullptr; p.out = dx;
-  p.mask = d->act_in == KT_ACT_LRELU ? Side{x, nullptr, SIDE_DLRELU, d->act_in_slope} : Side{nullptr, nullptr, 0, 0.f};
+  p.mask = dgrad_mask(d, x);
   // roles swap: "in" = dy (c_out channels, t_out rows), "out" = dx (c_in channels, t_in rows)
   p.batch = d->batch * d->nsub; p.nsub = d->nsub; p.t_in = d->t_out; p.t_out = d->t_in;
   p.c_in = d->c_out; p.c_out = d->c_in; p.groups = d->groups; p.cin_g = d->c_out / d->groups; p.cout_g = d->c_in / d->groups;

@@ -472,30 +472,20 @@ static bool add_phase(TcParams& p, const Phase& ph, int nsub) {
   if (s < 1 || s > kTcMaxGroups || p.nphases >= kTcMaxGroups) return false;
   if (p.nphases > 0 && (p.o_step != ph.o_step || p.i_step != ph.i_step || p.up != ph.up)) return false;
   p.o_step = ph.o_step; p.i_step = ph.i_step; p.up = ph.up; p.accumulate = ph.accumulate;
-  int q[kMaxTaps], rho[kMaxTaps];
-  for (int n = 0; n < ph.ntaps; ++n) {
-    if (ph.tap_ioff[n] < -(1 << 24)) {  // placeholder tap of an output residue no real tap reaches
-      q[n] = -(1 << 20); rho[n] = 0;
-      continue;
-    }
-    q[n] = fdiv(ph.tap_ioff[n], s);
-    rho[n] = ph.tap_ioff[n] - q[n] * s;
-  }
+  const ResidueTaps rt = residue_taps(ph, s);
   int max_span = 0;
   for (int r = 0; r < s; ++r) {
-    int qlo = 1 << 30, qhi = -(1 << 30), cnt = 0;
-    for (int n = 0; n < ph.ntaps; ++n)
-      if (rho[n] == r) { qlo = std::min(qlo, q[n]); qhi = std::max(qhi, q[n]); ++cnt; }
+    const int n0 = rt.first[r], cnt = rt.first[r + 1] - n0;
     if (!cnt) continue;
+    int qlo = 1 << 30, qhi = -(1 << 30);
+    for (int n = n0; n < n0 + cnt; ++n) { qlo = std::min(qlo, rt.q[n]); qhi = std::max(qhi, rt.q[n]); }
     if (p.ngroups >= kTcMaxGroups || p.ntaps + cnt > kMaxTaps) return false;
     const int g = p.ngroups++;
     p.grp_rho[g] = r; p.grp_qlo[g] = qlo; p.grp_first[g] = p.ntaps;
-    for (int n = 0; n < ph.ntaps; ++n)
-      if (rho[n] == r) {
-        p.tap_j[p.ntaps] = ph.tap_j[n];
-        p.tap_shift[p.ntaps] = (q[n] - qlo) * nsub;
-        ++p.ntaps;
-      }
+    for (int n = n0; n < n0 + cnt; ++n, ++p.ntaps) {
+      p.tap_j[p.ntaps] = rt.j[n];
+      p.tap_shift[p.ntaps] = (rt.q[n] - qlo) * nsub;
+    }
     p.grp_first[p.ngroups] = p.ntaps;
     max_span = std::max(max_span, (qhi - qlo) * nsub);
     p.span_q = std::max(p.span_q, qhi - qlo);
@@ -589,7 +579,7 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   }
   P.ok = true;
   P.tma = tma;
-  P.ws_floats = tma ? ((long long)base.batch * base.t_in * base.nsub * base.c_in + 63) & ~63LL : 0;
+  P.ws_floats = tma ? plane_floats(base.batch, base.t_in, base.nsub, base.c_in) : 0;
   return P;
 }
 
@@ -680,14 +670,6 @@ static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, cudaStream_t st) 
   return KT_OK;
 }
 
-static Side make_side_tc(const float* p, const float* aux, int act, float slope, bool derivative) {
-  Side s{p, aux, SIDE_PLAIN, slope};
-  if (act == KT_ACT_LRELU) s.mode = derivative ? SIDE_DLRELU : SIDE_LRELU;
-  else if (act == KT_ACT_TANH) s.mode = derivative ? SIDE_DTANH : SIDE_PLAIN;
-  if (s.mode < SIDE_DLRELU) s.aux = nullptr;
-  return s;
-}
-
 // Every launch of plan P with the operands of `io` (in, wimg, bias, resid, mask, out, out_act, out_slope).  The TMA route
 // first writes the gathered operand's planes into ws.
 static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws_floats, const char* what, cudaStream_t st) {
@@ -705,19 +687,9 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
   for (TcParams lp : P.launches) {
     lp.in = io.in; lp.wimg = io.wimg; lp.bias = io.bias; lp.resid = io.resid; lp.mask = io.mask; lp.out = io.out;
     lp.out_act = io.out_act; lp.out_slope = io.out_slope;
-    if (P.tma) {
-      // planes [hi | lo][batch][time][sub-sequence][channel]; residue class rho = time steps rho, rho + i_step, ...
-      const long long n = (long long)lp.batch * lp.t_in * lp.nsub * lp.c_in;
-      for (int rho = 0; rho < lp.i_step; ++rho) {
-        const cuuint64_t gdim[5] = {(cuuint64_t)lp.c_in, (cuuint64_t)lp.nsub, (cuuint64_t)ceil_div(lp.t_in - rho, lp.i_step),
-                                    (cuuint64_t)lp.batch, 2};
-        const cuuint64_t gstr[4] = {(cuuint64_t)lp.c_in * 2, (cuuint64_t)lp.i_step * lp.nsub * lp.c_in * 2,
-                                    (cuuint64_t)lp.t_in * lp.nsub * lp.c_in * 2, (cuuint64_t)n * 2};
-        const cuuint32_t box[5] = {kTcKC, (cuuint32_t)lp.nsub, (cuuint32_t)lp.a_box_t, 1, 1};
-        const int rc = encode_tensor_map(&maps.map[rho], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, planes + (long long)rho * lp.nsub * lp.c_in,
-                                         gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
-        if (rc) return rc;
-      }
+    for (int rho = 0; P.tma && rho < lp.i_step; ++rho) {
+      const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what);
+      if (rc) return rc;
     }
     const int rc = run_tc(lp, maps, P.tma, st);
     if (rc) return rc;
@@ -730,7 +702,7 @@ int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const
   const TcPlan P = make_tc_plan(d, 0);
   KT_REQUIRE(P.ok, "conv1d_fwd_tc: layer not supported by the tensor-core path");
   TcParams io{};
-  io.in = make_side_tc(x, nullptr, d->act_in, d->act_in_slope, false);
+  io.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
   io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
@@ -745,10 +717,10 @@ int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, c
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_data: y required when act_out != NONE");
   KT_REQUIRE(d->act_in == KT_ACT_NONE || x != nullptr, "bwd_data: x required when act_in != NONE");
   TcParams io{};
-  io.in = make_side_tc(dy, y, d->act_out, d->act_out_slope, true);
+  io.in = make_side(dy, y, d->act_out, d->act_out_slope, true);
   io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
   io.bias = nullptr; io.resid = nullptr; io.out = dx;
-  io.mask = d->act_in == KT_ACT_LRELU ? Side{x, nullptr, SIDE_DLRELU, d->act_in_slope} : Side{nullptr, nullptr, 0, 0.f};
+  io.mask = dgrad_mask(d, x);
   io.out_act = KT_ACT_NONE; io.out_slope = 0.f;
   return run_plan(P, io, ws, ws_floats, "conv1d_bwd_data_tc", st);
 }

@@ -1,6 +1,7 @@
 // Tensor-map (TMA descriptor) helpers shared by the kernels that stage tiles with cp.async.bulk.tensor.
 #pragma once
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (resolved at run time, no link dependency)
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -36,6 +37,22 @@ inline int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int ra
                         swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   KT_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed (%d)", what, (int)r);
   return KT_OK;
+}
+
+// Split-bf16 planes of a [batch][t][nsub][c] fp32 tensor (split_planes, tc_common.cuh): [hi | lo][batch][t][nsub][c] bf16.
+// plane_floats: workspace floats they occupy (one per element), rounded up to 256 bytes.
+inline long long plane_floats(long long batch, long long t, long long nsub, long long c) { return (batch * t * nsub * c + 63) & ~63LL; }
+
+// Tensor map of residue class rho of such planes, time steps rho, rho + step, ...: 5-D boxes of box_c channels x nsub x box_t
+// of those steps, SWIZZLE_128B; coordinates (channel, sub-sequence, step of the class, batch, plane)
+inline int encode_plane_map(CUtensorMap* map, const __nv_bfloat16* planes, int batch, int t, int nsub, int c, int step, int rho,
+                            int box_c, int box_t, const char* what) {
+  const long long n = (long long)batch * t * nsub * c;
+  const cuuint64_t dims[5] = {(cuuint64_t)c, (cuuint64_t)nsub, (cuuint64_t)ceil_div(t - rho, step), (cuuint64_t)batch, 2};
+  const cuuint64_t strides[4] = {(cuuint64_t)c * 2, (cuuint64_t)step * nsub * c * 2, (cuuint64_t)t * nsub * c * 2, (cuuint64_t)n * 2};
+  const cuuint32_t box[5] = {(cuuint32_t)box_c, (cuuint32_t)nsub, (cuuint32_t)box_t, 1, 1};
+  return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, planes + (long long)rho * nsub * c, dims, strides, box,
+                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 namespace tc {

@@ -15,7 +15,6 @@
 // columns) for a slice of the (batch, flattened time) range (split-K); partial tiles go to a workspace
 // with plain stores and a second kernel reduces over the splits in order (deterministic, and cheaper than ~10^7 atomics).
 #include <algorithm>
-#include <vector>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -40,9 +39,9 @@ struct WgTcParams {
   int M;                       // base rows m per sub-sequence
   int step, up;
   int mode, NT, n_cb_tiles, n_ca_tiles;
-  int nsplit, chunks_per_batch;
+  int nsplit, chunks_per_batch;   // chunk = kWgTK flattened rows (register-staged) or tt base time steps (TMA)
   int a_groups, b_groups;      // 64-channel images per stage on each side
-  int rows_a;                  // A image rows (max over unit groups), multiple of 8
+  int rows_a;                  // register-staged route: A image rows (max over unit groups), multiple of 8
   int ngroups;                 // unit groups (grid.y)
   int grp_rho[kWgMaxGroups], grp_qlo[kWgMaxGroups];
   int grp_first_unit[kWgMaxGroups + 1];
@@ -51,6 +50,26 @@ struct WgTcParams {
   int tap_j[kMaxTaps];
   int tap_q[kMaxTaps];
   long long split_stride;      // floats between two splits' partial gradients in ws
+};
+
+// The work of one CTA: (conv group cgrp, ca tile, cb tile) = blockIdx.x, unit group grp = blockIdx.y (units [u0, u0 + nu) of one
+// residue class, lowest tap shift qlo), split-K slice split = blockIdx.z: chunks [c_begin, c_end) of the (batch, chunk) range
+struct WgCta {
+  int cb_tile, ca_tile, cgrp, grp, u0, nu, qlo, split;
+  long long c_begin, c_end;
+  __device__ __forceinline__ explicit WgCta(const WgTcParams& p) {
+    cb_tile = blockIdx.x % p.n_cb_tiles;
+    ca_tile = (blockIdx.x / p.n_cb_tiles) % p.n_ca_tiles;
+    cgrp = blockIdx.x / (p.n_cb_tiles * p.n_ca_tiles);
+    grp = blockIdx.y;
+    u0 = p.grp_first_unit[grp];
+    nu = p.grp_first_unit[grp + 1] - u0;
+    qlo = p.grp_qlo[grp];
+    split = blockIdx.z;
+    const long long units = (long long)p.batch * p.chunks_per_batch;
+    c_begin = units * split / p.nsplit;
+    c_end = units * (split + 1) / p.nsplit;
+  }
 };
 
 // Consumers: two warpgroups, warpgroup cw owns rows [64 cw, 64 cw + 64) of the M = 128 accumulator block of every unit (U =
@@ -87,8 +106,9 @@ __device__ __forceinline__ void wg_chunk_mma(float (&acc)[kWgmmaMaxRegs], uint32
 
 // registers -> workspace partial tiles (or dw itself when there is one split)
 template <int NT>
-__device__ __forceinline__ void wg_store(const WgTcParams& p, const float (&acc)[kWgmmaMaxRegs], int cw, int wq, int lane, int cb_tile,
-                                         int ca_tile, int cgrp, int u0, int nu, int split) {
+__device__ __forceinline__ void wg_store(const WgTcParams& p, const WgCta& cta, const float (&acc)[kWgmmaMaxRegs], int cw, int wq,
+                                         int lane) {
+  const int cb_tile = cta.cb_tile, ca_tile = cta.ca_tile, cgrp = cta.cgrp, u0 = cta.u0, nu = cta.nu, split = cta.split;
   const bool vec = ((p.cb | p.cb_g0) & 1) == 0;
 #pragma unroll
   for (int u = 0; u < kWgmmaMaxN / NT; ++u) {
@@ -131,14 +151,14 @@ __device__ __forceinline__ void wg_store(const WgTcParams& p, const float (&acc)
 }
 
 // per unit of this CTA: A-side row shift and the offset of the second warpgroup's 64 rows, in 16-byte descriptor units
-__device__ __forceinline__ void wg_unit_table(const WgTcParams& p, int u0, int nu, int qlo, int img_a, uint32_t* s_shift, uint32_t* s_half) {
-  for (int u = threadIdx.x; u < nu; u += blockDim.x) {
-    const int n_a = p.unit_tap0[u0 + u];
+__device__ __forceinline__ void wg_unit_table(const WgTcParams& p, const WgCta& cta, int img_a, uint32_t* s_shift, uint32_t* s_half) {
+  for (int u = threadIdx.x; u < cta.nu; u += blockDim.x) {
+    const int n_a = p.unit_tap0[cta.u0 + u];
     uint32_t half;
     if (p.mode == 0) half = 2u * (uint32_t)img_a;
     // mode 1: second half of M = the next tap of the same residue (rows 64..127 are discarded when the unit has one tap)
-    else half = p.unit_ntaps[u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
-    s_shift[u] = ((uint32_t)((p.tap_q[n_a] - qlo) * p.nsub) * 128u) >> 4;
+    else half = p.unit_ntaps[cta.u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
+    s_shift[u] = ((uint32_t)((p.tap_q[n_a] - cta.qlo) * p.nsub) * 128u) >> 4;
     s_half[u] = half >> 4;
   }
 }
@@ -162,24 +182,14 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   uint32_t* s_half = s_shift + kWgMaxUnits;                    // [kWgMaxUnits]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cb_tile = blockIdx.x % p.n_cb_tiles;
-  const int ca_tile = (blockIdx.x / p.n_cb_tiles) % p.n_ca_tiles;
-  const int cgrp = blockIdx.x / (p.n_cb_tiles * p.n_ca_tiles);   // conv group
-  const int grp = blockIdx.y;
-  const int u0 = p.grp_first_unit[grp];
-  const int nu = p.grp_first_unit[grp + 1] - u0;
-  const int qlo = p.grp_qlo[grp];
-  const int split = blockIdx.z;
-  const long long units = (long long)p.batch * p.chunks_per_batch;
-  const long long c_begin = units * split / p.nsplit;
-  const long long c_end = units * (split + 1) / p.nsplit;
+  const WgCta cta(p);
 
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) { mbar_init(&full[s], 128); mbar_init(&empty[s], kWgConsumerArrivals); }
     mbar_fence_init();
     fence_proxy_async();
   }
-  wg_unit_table(p, u0, nu, qlo, img_a, s_shift, s_half);
+  wg_unit_table(p, cta, img_a, s_shift, s_half);
   __syncthreads();
 
   if (warp < 4 || warp >= 12) {
@@ -187,7 +197,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     const int pg = warp < 4 ? 0 : 1;                                       // pipeline stage this group fills
     const int ptid = tid & 127;
     int it = 0;
-    for (long long c = c_begin; c < c_end; ++c, ++it) {
+    for (long long c = cta.c_begin; c < cta.c_end; ++c, ++it) {
       const int s = it & 1;
       if (s != pg) continue;
       mbar_wait(&empty[s], ((it >> 1) & 1) ^ 1);
@@ -196,12 +206,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       uint8_t* st = stage0 + (size_t)s * stage_bytes;
       RowMap ra;  // gathered side: residue image of this unit group
       ra.base_row = (long long)bb * p.t_a * p.nsub;
-      ra.fv0 = f0 + qlo * p.nsub;
-      ra.nsub = p.nsub; ra.step = p.step; ra.rho = p.grp_rho[grp]; ra.up = p.up; ra.t_lim = p.t_a * p.up;
+      ra.fv0 = f0 + cta.qlo * p.nsub;
+      ra.nsub = p.nsub; ra.step = p.step; ra.rho = p.grp_rho[cta.grp]; ra.up = p.up; ra.t_lim = p.t_a * p.up;
       for (int g = 0; g < p.a_groups; ++g) {
         uint8_t* hi = st + (size_t)g * 2 * img_a;
-        const int c_lo = ca_tile * (p.mode == 0 ? 128 : 64) + g * 64;           // channel offset inside the group
-        stage_rows<4, false, 2>(hi, hi + img_a, p.a, p.a.p, p.a.aux, p.ca, cgrp * p.ca_g + c_lo, min(64, p.ca_g - c_lo), true, ra,
+        const int c_lo = cta.ca_tile * (p.mode == 0 ? 128 : 64) + g * 64;           // channel offset inside the group
+        stage_rows<4, false, 2>(hi, hi + img_a, p.a, p.a.p, p.a.aux, p.ca, cta.cgrp * p.ca_g + c_lo, min(64, p.ca_g - c_lo), true, ra,
                                 p.rows_a, ptid);
       }
       RowMap rb;  // base side: rows m (flattened with w), zero beyond M
@@ -210,8 +220,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       uint8_t* bst = st + (size_t)p.a_groups * 2 * img_a;
       for (int g = 0; g < p.b_groups; ++g) {
         uint8_t* hi = bst + (size_t)g * 2 * img_b;
-        const int c_lo = cb_tile * NT + g * 64;
-        stage_rows<2, false, 2>(hi, hi + img_b, p.b, p.b.p, p.b.aux, p.cb, cgrp * p.cb_g + c_lo, min(64, p.cb_g - c_lo), true, rb,
+        const int c_lo = cta.cb_tile * NT + g * 64;
+        stage_rows<2, false, 2>(hi, hi + img_b, p.b, p.b.p, p.b.aux, p.cb, cta.cgrp * p.cb_g + c_lo, min(64, p.cb_g - c_lo), true, rb,
                                 kWgTK, ptid);
       }
       fence_proxy_async();
@@ -228,13 +238,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
 #pragma unroll
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
     int it = 0;
-    for (long long c = c_begin; c < c_end; ++c, ++it) {
+    for (long long c = cta.c_begin; c < cta.c_end; ++c, ++it) {
       const int s = it & 1;
       mbar_wait(&full[s], (it >> 1) & 1);
-      wg_chunk_mma<NT>(acc, st16[s], (st16[s] + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, nu, cw, kWgTK / 16);
+      wg_chunk_mma<NT>(acc, st16[s], (st16[s] + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kWgTK / 16);
       if (lane == 0) mbar_arrive(&empty[s]);
     }
-    wg_store<NT>(p, acc, cw, wq, lane, cb_tile, ca_tile, cgrp, u0, nu, split);
+    wg_store<NT>(p, cta, acc, cw, wq, lane);
   }
 }
 
@@ -256,7 +266,6 @@ struct WgTmaExtra {
   int tt, R, Rp, nstages;
   int rows_a_p;        // rows of one A image plane (multiple of 8): Rp + tap span
   int a_box_t;         // time steps per A box = tt + (largest tap span of a unit group)
-  int chunks_per_batch;
   alignas(64) CUtensorMap map_b;
   alignas(64) CUtensorMap map_a[8];   // one per residue class of the input
 };
@@ -277,17 +286,7 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   uint32_t* s_half = s_shift + kWgMaxUnits;                                     // [kWgMaxUnits]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cb_tile = blockIdx.x % p.n_cb_tiles;
-  const int ca_tile = (blockIdx.x / p.n_cb_tiles) % p.n_ca_tiles;
-  const int cgrp = blockIdx.x / (p.n_cb_tiles * p.n_ca_tiles);
-  const int grp = blockIdx.y;
-  const int u0 = p.grp_first_unit[grp];
-  const int nu = p.grp_first_unit[grp + 1] - u0;
-  const int qlo = p.grp_qlo[grp];
-  const int split = blockIdx.z;
-  const long long units = (long long)p.batch * x.chunks_per_batch;
-  const long long c_begin = units * split / p.nsplit;
-  const long long c_end = units * (split + 1) / p.nsplit;
+  const WgCta cta(p);
 
   if (tid == 0) {
     for (int s = 0; s < x.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kWgConsumerArrivals); }
@@ -304,7 +303,7 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
         for (int o = r0 * 128 + tid * 16; o < r1 * 128; o += kWgTmaThreads * 16) *reinterpret_cast<uint4*>(img + o) = make_uint4(0u, 0u, 0u, 0u);
       }
   }
-  wg_unit_table(p, u0, nu, qlo, img_a, s_shift, s_half);
+  wg_unit_table(p, cta, img_a, s_shift, s_half);
   fence_proxy_async();
   __syncthreads();
 
@@ -312,20 +311,20 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
     // ===================== TMA producer =====================
     if (elect_one()) {
       const uint32_t tx = 2u * (uint32_t)(p.a_groups * x.a_box_t * p.nsub + p.b_groups * x.R) * 128u;
-      const CUtensorMap* ma = &x.map_a[p.grp_rho[grp]];
-      const int ca0 = cgrp * p.ca_g + ca_tile * (p.mode == 0 ? 128 : 64);
-      const int cb0 = cgrp * p.cb_g + cb_tile * NT;
+      const CUtensorMap* ma = &x.map_a[p.grp_rho[cta.grp]];
+      const int ca0 = cta.cgrp * p.ca_g + cta.ca_tile * (p.mode == 0 ? 128 : 64);
+      const int cb0 = cta.cgrp * p.cb_g + cta.cb_tile * NT;
       RingPos r;
-      for (long long c = c_begin; c < c_end; ++c, r.advance(x.nstages)) {
+      for (long long c = cta.c_begin; c < cta.c_end; ++c, r.advance(x.nstages)) {
         const int s = r.slot();
         mbar_wait(&empty[s], r.phase() ^ 1u);
-        const int bb = (int)(c / x.chunks_per_batch);
-        const int m0 = (int)(c % x.chunks_per_batch) * x.tt;
+        const int bb = (int)(c / p.chunks_per_batch);
+        const int m0 = (int)(c % p.chunks_per_batch) * x.tt;
         uint8_t* st = stage0 + (size_t)s * stage_bytes;
         mbar_arrive_expect_tx(&full[s], tx);
         for (int g = 0; g < p.a_groups; ++g)
           for (int pl = 0; pl < 2; ++pl)
-            tma_load_5d(st + (size_t)(2 * g + pl) * img_a, ma, ca0 + g * 64, 0, m0 + qlo, bb, pl, &full[s]);
+            tma_load_5d(st + (size_t)(2 * g + pl) * img_a, ma, ca0 + g * 64, 0, m0 + cta.qlo, bb, pl, &full[s]);
         uint8_t* bst = st + (size_t)p.a_groups * 2 * img_a;
         for (int g = 0; g < p.b_groups; ++g)
           for (int pl = 0; pl < 2; ++pl)
@@ -346,14 +345,14 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
 #pragma unroll
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
     RingPos r;
-    for (long long c = c_begin; c < c_end; ++c, r.advance(x.nstages)) {
+    for (long long c = cta.c_begin; c < cta.c_end; ++c, r.advance(x.nstages)) {
       const int s = r.slot();
       mbar_wait(&full[s], r.phase());
       const uint32_t sbase = st0_16 + (uint32_t)s * stage16;
-      wg_chunk_mma<NT>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, nu, cw, kslices);
+      wg_chunk_mma<NT>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kslices);
       if (lane == 0) mbar_arrive(&empty[s]);
     }
-    wg_store<NT>(p, acc, cw, wq, lane, cb_tile, ca_tile, cgrp, u0, nu, split);
+    wg_store<NT>(p, cta, acc, cw, wq, lane);
   }
 }
 
@@ -413,21 +412,38 @@ __global__ void wgrad_reduce_wide_kernel(const float* __restrict__ ws, float* __
 // ---------------------------------------------------------------------------------------------
 struct WgPlan {
   bool ok;
+  bool tma;                  // TMA-fed kernel (x filled in), else register-staged
   WgTcParams p;
-  size_t smem;
-  long long ws_floats;       // whole workspace: split-K partials (+ the bf16 operand planes of the TMA variant)
-  // TMA variant (tma == true): x, its shared-memory size, offsets (floats) of the operand planes inside the workspace
-  bool tma;
   WgTmaExtra x;
-  size_t smem_tma;
-  long long part_floats, planes_a_off, planes_b_off;
-  int nsplit_tma;
-  int max_span_q;
+  size_t smem;
+  long long ws_floats;       // whole workspace: split-K partials, then on the TMA route the bf16 planes of both operands
+  long long planes_a_off, planes_b_off;   // TMA route: offsets (floats) of the operand planes inside the workspace
 };
 
-static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_only = false) {
+Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up);   // conv_ffma.cu
+
+// bytes of one ring stage: the hi / lo planes of the A images (rows_a rows) and of the B images (rows_b rows)
+static size_t wg_stage_bytes(const WgTcParams& p, int rows_a, int rows_b) {
+  return 2 * ((size_t)p.a_groups * rows_a * 128 + (size_t)p.b_groups * rows_b * 128);
+}
+
+// split-K factor: the ns in [1, min(units, 296)] of least cost(waves, chunks per CTA, ns), the smaller on a tie.  `ctas`
+// CTAs per split run one per SM in waves of one per SM.
+template <class Cost>
+static int split_k(long long units, long long ctas, Cost cost) {
+  const int sms = device_sm_count();
+  long long best_ns = 1;
+  double best = 1e30;
+  for (long long ns = 1; ns <= std::min<long long>(units, 296); ++ns) {
+    const long long waves = (ctas * ns + sms - 1) / sms;
+    const double c = cost((double)waves, (double)((units + ns - 1) / ns), ns);
+    if (c < best - 1e-9) { best = c; best_ns = ns; }
+  }
+  return (int)best_ns;
+}
+
+static WgPlan make_plan(const KtConv1dDesc* d, bool plan_only = false) {
   WgPlan pl{};
-  pl.ok = false;
   WgTcParams& p = pl.p;
   // gathered (A) side / base (B) side, see conv_ffma.cu: conv1d_bwd_weight_ffma
   const bool tr = d->transposed != 0;
@@ -444,13 +460,9 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   p.M = p.t_b;
   p.step = d->stride;
   p.up = tr ? 1 : d->upsample;
-  if (p.step > 8) return pl;
+  if (p.step > kMaxResidues) return pl;
   // channels are zero-padded to 64-wide images: thin / grouped layers use the same kernel
   p.mode = p.ca_g <= 64 ? 1 : 0;
-  // TMA variant (see wgrad_tma_kernel): plain convs whose box coordinates (multiples of the (super-)group widths) are 16-byte
-  // aligned.  Tiles are at most N = 128 wide (the accumulators of all units of a CTA are 64 registers per consumer thread).
-  const bool tma_ok = allow_tma && !tr && p.up == 1 && (ca % 8) == 0 && (cb % 8) == 0 && (p.ca_g % 8) == 0 && (p.cb_g % 8) == 0 &&
-                      (plan_only || encode_tiled_fn() != nullptr);   // plan_only: host-logic tests without a driver
   p.NT = std::min(kWgmmaMaxN, (p.cb_g + 63) & ~63);
   p.n_cb_tiles = ceil_div(p.cb_g, p.NT);
   p.n_ca_tiles = p.mode == 0 ? ceil_div(p.ca_g, 128) : 1;
@@ -458,136 +470,105 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool allow_tma = true, bool plan_
   p.b_groups = p.NT / 64;
   const int U = std::min(kWgMaxUnits, kWgmmaMaxN / p.NT);
   const int taps_per_unit = p.mode == 1 ? 2 : 1;
-  // taps sorted by (residue, q)
-  int ntap = 0, nunit = 0;
-  p.ngroups = 0;
-  int max_span = 0;
+  // taps by (residue, q, j): the gather phase of the gradient's contraction, as conv1d_bwd_weight_ffma runs it
+  const ResidueTaps rt = residue_taps(gather_phase(p.M, d->kernel, p.step, d->dilation, d->pad_left, p.up), p.step);
+  std::copy(rt.j, rt.j + rt.first[p.step], p.tap_j);
+  std::copy(rt.q, rt.q + rt.first[p.step], p.tap_q);
+  int nunit = 0, max_span_q = 0;
   for (int r = 0; r < p.step; ++r) {
-    std::vector<std::pair<int, int>> tq;  // (q, j)
-    for (int j = 0; j < d->kernel; ++j) {
-      const int ioff = j * d->dilation - d->pad_left;
-      const int q = fdiv(ioff, p.step);
-      if (ioff - q * p.step == r) tq.push_back({q, j});
-    }
-    std::sort(tq.begin(), tq.end());
-    size_t i = 0;
+    const int end = rt.first[r + 1];
     // the residue's units are spread EVENLY over its unit groups (5 taps, U = 4: groups of 3 + 2, not 4 + 1): every CTA loads
     // the same operand rows per chunk whatever its unit count, so the largest group sets the pace
-    const int units_r = ceil_div((int)tq.size(), taps_per_unit);
+    const int units_r = ceil_div(end - rt.first[r], taps_per_unit);
     const int groups_r = std::max(1, ceil_div(units_r, U));
     const int U_r = ceil_div(units_r, groups_r);
-    while (i < tq.size()) {
-      // one unit group: up to U units of this residue
+    for (int i = rt.first[r]; i < end;) {
+      // one unit group: up to U_r units of this residue
       if (p.ngroups >= kWgMaxGroups) return pl;
       const int g = p.ngroups++;
       p.grp_rho[g] = r;
-      p.grp_qlo[g] = tq[i].first;
+      p.grp_qlo[g] = rt.q[i];
       p.grp_first_unit[g] = nunit;
-      int qhi = tq[i].first;
-      for (int u = 0; u < U_r && i < tq.size(); ++u) {
-        p.unit_tap0[nunit] = ntap;
-        const int nt_u = (int)std::min<size_t>(taps_per_unit, tq.size() - i);
-        p.unit_ntaps[nunit] = nt_u;
-        for (int e = 0; e < nt_u; ++e, ++i, ++ntap) {
-          p.tap_j[ntap] = tq[i].second;
-          p.tap_q[ntap] = tq[i].first;
-          qhi = tq[i].first;
-        }
-        ++nunit;
+      for (int u = 0; u < U_r && i < end; ++u, ++nunit) {
+        p.unit_tap0[nunit] = i;
+        p.unit_ntaps[nunit] = std::min(taps_per_unit, end - i);
+        i += p.unit_ntaps[nunit];
       }
-      max_span = std::max(max_span, (qhi - p.grp_qlo[g]) * p.nsub);
-      pl.max_span_q = std::max(pl.max_span_q, qhi - p.grp_qlo[g]);
+      max_span_q = std::max(max_span_q, rt.q[i - 1] - p.grp_qlo[g]);
     }
   }
   p.grp_first_unit[p.ngroups] = nunit;
-  p.rows_a = (kWgTK + max_span + 7) & ~7;
-  const size_t stage = 2 * ((size_t)p.a_groups * p.rows_a * 128 + (size_t)p.b_groups * kWgTK * 128);
-  pl.smem = 1024 + 2 * stage + 128;
-  if (pl.smem > (size_t)kMaxDynSmem) return pl;   // (a smaller U would shrink the halo; not needed for the shipped shapes)
-  p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
-  const long long units = (long long)p.batch * p.chunks_per_batch;
-  const long long base = (long long)p.groups * p.n_ca_tiles * p.n_cb_tiles * p.ngroups;
-  const int sms = device_sm_count();
-  // split-K factor: CTAs run one per SM in waves of one per SM; minimise (waves x chunks per CTA) plus the cost of writing
-  // and re-reading one more partial copy of the gradient (in units of one chunk ~ 10 us; ~4 TB/s effective)
-  const double out_chunks = (double)p.taps_total * p.ca_g0 * cb * 8.0 / 4e12 / 10e-6;
-  long long nsplit = 1;
-  double best = 1e30;
-  for (long long ns = 1; ns <= std::min<long long>(units, 296); ++ns) {
-    const long long waves = (base * ns + sms - 1) / sms;
-    const double cost = (double)waves * (double)((units + ns - 1) / ns) + (double)ns * out_chunks;
-    if (cost < best - 1e-9) { best = cost; nsplit = ns; }
-  }
-  p.nsplit = (int)nsplit;
+  // Whether a layer runs on the tensor cores does not depend on the route (a driver without tensor-map encoding plans the
+  // same layers): the register-staged ring must fit on both.  (A smaller U would shrink the halo; not needed for the shipped
+  // shapes.)
+  const int rows_a = (kWgTK + max_span_q * p.nsub + 7) & ~7;
+  pl.smem = 1024 + 2 * wg_stage_bytes(p, rows_a, kWgTK) + 128;
+  if (pl.smem > (size_t)kMaxDynSmem) return pl;
   p.split_stride = (long long)p.taps_total * p.ca_g0 * cb;
-  pl.ws_floats = nsplit * p.split_stride;
-  pl.ok = true;
+  const double out_bytes = (double)p.taps_total * p.ca_g0 * cb * 8.0;   // one partial copy of the gradient, written and read
+  const long long ctas = (long long)p.groups * p.n_ca_tiles * p.n_cb_tiles * p.ngroups;
 
-  // ---- TMA variant: chunk = tt base time steps x nsub sub-sequences, padded to whole K = 16 slices
-  pl.tma = false;
-  if (tma_ok) {
-    WgTmaExtra& x = pl.x;
-    for (int r = 0; r < p.step; ++r)
-      if (p.t_a - r <= 0) return make_plan(d, false, plan_only);
-    // tt: the largest chunk (R = tt * nsub <= 128 rows, at most 20 % padding in the last K slice) that still leaves a ring of
-    // three stages; else the deepest ring
-    int best_tt = 0, best_ns = 0;
-    for (int tt = std::max(1, 128 / p.nsub); tt >= 1; --tt) {
-      const int R = tt * p.nsub, Rp = (R + 15) & ~15;
-      if (tt + pl.max_span_q > 256 || R > 256 || (tt > 1 && R * 5 < Rp * 4)) continue;
-      const int rows_a_p = (Rp + pl.max_span_q * p.nsub + 7) & ~7;
-      const size_t stage = 2 * ((size_t)p.a_groups * rows_a_p * 128 + (size_t)p.b_groups * Rp * 128);
-      const size_t fixed = 1024 + 128;
-      if (fixed + stage > (size_t)kMaxDynSmem) continue;
-      const int ns = (int)std::min<size_t>(kWgTmaMaxStages, ((size_t)kMaxDynSmem - fixed) / stage);
-      if (ns > best_ns) { best_ns = ns; best_tt = tt; }
+  // TMA route (see wgrad_tma_kernel): plain convs whose box coordinates (multiples of the (super-)group widths) are 16-byte
+  // aligned, with a time step in every residue class of the input.  Chunk = tt base time steps x nsub sub-sequences (R rows),
+  // padded to whole K = 16 slices (Rp rows).  tt: the largest chunk (R <= 128 rows, at most 20 % padding in the last K slice)
+  // that still leaves a ring of three stages; else the deepest ring, which must have two.
+  int tt = 0, nstages = 0;
+  if (!tr && p.up == 1 && (ca % 8) == 0 && (cb % 8) == 0 && (p.ca_g % 8) == 0 && (p.cb_g % 8) == 0 && p.t_a >= p.step &&
+      (plan_only || encode_tiled_fn() != nullptr)) {   // plan_only: host-logic tests without a driver
+    for (int t = std::max(1, 128 / p.nsub); t >= 1; --t) {
+      const int R = t * p.nsub, Rp = (R + 15) & ~15;
+      if (t + max_span_q > 256 || R > 256 || (t > 1 && R * 5 < Rp * 4)) continue;
+      const size_t stage = wg_stage_bytes(p, (Rp + max_span_q * p.nsub + 7) & ~7, Rp);
+      if (1024 + 128 + stage > (size_t)kMaxDynSmem) continue;
+      const int ns = (int)std::min<size_t>(kWgTmaMaxStages, ((size_t)kMaxDynSmem - 1024 - 128) / stage);
+      if (ns > nstages) { nstages = ns; tt = t; }
       if (ns >= 3) break;
     }
-    if (best_ns < 2) return make_plan(d, false, plan_only);
-    x.tt = best_tt; x.R = best_tt * p.nsub; x.Rp = (x.R + 15) & ~15;
-    x.a_box_t = best_tt + pl.max_span_q;
-    x.rows_a_p = (x.Rp + pl.max_span_q * p.nsub + 7) & ~7;
-    x.nstages = best_ns;
-    {
-      const size_t stage = 2 * ((size_t)p.a_groups * x.rows_a_p * 128 + (size_t)p.b_groups * x.Rp * 128);
-      pl.smem_tma = 1024 + 128 + (size_t)best_ns * stage;
-    }
-    pl.tma = true;
-    x.chunks_per_batch = ceil_div(p.M, x.tt);
-    const long long units_t = (long long)p.batch * x.chunks_per_batch;
-    // split-K: a chunk costs ~2 us here (TMA + MMAs), one more partial copy of the gradient out_bytes / ~4 TB/s twice
-    // (all in us) a chunk: the larger of its loads (~1.5 us per 70 KB at the observed ~45 GB/s per SM) and its MMAs (12 per unit
-    // and 64 rows, N / 2 cycles each); one split more: one more partial copy written and read back (~4 TB/s), and the
-    // reduce pass itself (~5 us) which a single split does not need at all (the kernel then writes dw directly)
+  }
+  pl.tma = nstages >= 2;
+  if (pl.tma) {
+    WgTmaExtra& x = pl.x;
+    x.tt = tt; x.R = tt * p.nsub; x.Rp = (x.R + 15) & ~15; x.nstages = nstages;
+    x.a_box_t = tt + max_span_q;
+    x.rows_a_p = (x.Rp + max_span_q * p.nsub + 7) & ~7;
+    pl.smem = 1024 + 128 + (size_t)nstages * wg_stage_bytes(p, x.rows_a_p, x.Rp);
+    p.chunks_per_batch = ceil_div(p.M, tt);
+    // split-K cost (in us) of a chunk: the larger of its loads (~1.5 us per 70 KB at the observed ~45 GB/s per SM) and its MMAs
+    // (12 per unit and 64 rows, N / 2 cycles each); of one split more: one more partial copy written and read back (~4 TB/s),
+    // and the reduce pass itself (~5 us) which a single split does not need at all (the kernel then writes dw directly)
     int u_max = 1;
     for (int g = 0; g < p.ngroups; ++g) u_max = std::max(u_max, p.grp_first_unit[g + 1] - p.grp_first_unit[g]);
     const double stage_kb = 2.0 * (p.a_groups * x.rows_a_p + p.b_groups * x.Rp) * 128 / 1024.0;
     const double chunk_us = std::max(stage_kb / 45.0, u_max * 3.0 * (x.Rp / 16) * (p.NT / 2) / 1900.0);
-    const double out_us = (double)p.taps_total * p.ca_g0 * cb * 8.0 / 4e12 * 1e6;
-    long long ns_best = 1;
-    double cbest = 1e30;
-    for (long long ns = 1; ns <= std::min<long long>(units_t, 296); ++ns) {
-      const long long waves = (base * ns + sms - 1) / sms;
-      const double cost = (double)waves * (double)((units_t + ns - 1) / ns) * chunk_us + (ns > 1 ? 5.0 + (double)ns * out_us : 0.0);
-      if (cost < cbest - 1e-9) { cbest = cost; ns_best = ns; }
-    }
-    pl.nsplit_tma = (int)ns_best;
-    pl.part_floats = (ns_best * p.split_stride + 63) & ~63LL;
-    const long long fa = ((long long)p.batch * p.t_a * p.nsub * ca + 63) & ~63LL;     // floats = 2 planes x bf16
-    const long long fb = ((long long)p.batch * p.t_b * p.nsub * cb + 63) & ~63LL;
-    pl.planes_a_off = pl.part_floats;
-    pl.planes_b_off = pl.part_floats + fa;
-    pl.ws_floats = pl.part_floats + fa + fb;
+    const double out_us = out_bytes / 4e12 * 1e6;
+    p.nsplit = split_k((long long)p.batch * p.chunks_per_batch, ctas, [&](double waves, double chunks, long long ns) {
+      return waves * chunks * chunk_us + (ns > 1 ? 5.0 + (double)ns * out_us : 0.0);
+    });
+    pl.planes_a_off = (p.nsplit * p.split_stride + 63) & ~63LL;
+    pl.planes_b_off = pl.planes_a_off + plane_floats(p.batch, p.t_a, p.nsub, ca);
+    pl.ws_floats = pl.planes_b_off + plane_floats(p.batch, p.t_b, p.nsub, cb);
+  } else {
+    p.rows_a = rows_a;
+    p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
+    // split-K: minimise (waves x chunks per CTA) plus the cost of writing and re-reading one more partial copy of the gradient
+    // (in units of one chunk ~ 10 us; ~4 TB/s effective)
+    const double out_chunks = out_bytes / 4e12 / 10e-6;
+    p.nsplit = split_k((long long)p.batch * p.chunks_per_batch, ctas, [&](double waves, double chunks, long long ns) {
+      return waves * chunks + (double)ns * out_chunks;
+    });
+    pl.ws_floats = p.nsplit * p.split_stride;
   }
+  pl.ok = true;
   return pl;
 }
 
-// development / test aid (kt_debug_wgrad_plan): the TMA variant's plan of a layer as it would be made on a GPU box
-// out = {ok, tma, tt, R, Rp, nstages, smem bytes, nsplit, NT, unit groups, a_box_t, rows_a_p}
+// development / test aid (kt_debug_wgrad_plan): the plan of a layer as it would be made on a GPU box
+// out = {ok, tma, tt, R, Rp, nstages, smem bytes, nsplit, NT, unit groups, a_box_t, rows_a_p} (TMA-only entries 0 on the
+// register-staged route)
 void debug_wgrad_plan(const KtConv1dDesc* d, int* out) {
-  const WgPlan pl = make_plan(d, true, true);
+  const WgPlan pl = make_plan(d, true);
   out[0] = pl.ok; out[1] = pl.tma; out[2] = pl.x.tt; out[3] = pl.x.R; out[4] = pl.x.Rp; out[5] = pl.x.nstages;
-  out[6] = (int)(pl.tma ? pl.smem_tma : pl.smem); out[7] = pl.tma ? pl.nsplit_tma : pl.p.nsplit; out[8] = pl.p.NT; out[9] = pl.p.ngroups;
+  out[6] = (int)pl.smem; out[7] = pl.p.nsplit; out[8] = pl.p.NT; out[9] = pl.p.ngroups;
   out[10] = pl.x.a_box_t; out[11] = pl.x.rows_a_p;
 }
 
@@ -609,52 +590,34 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
   KT_REQUIRE(ws && ws_floats >= pl.ws_floats, "conv1d_bwd_weight_tc: workspace too small (%lld < %lld floats)", ws_floats, pl.ws_floats);
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_weight: y required when act_out != NONE");
   WgTcParams& p = pl.p;
-  const Side sx{x, nullptr, d->act_in == KT_ACT_LRELU ? SIDE_LRELU : SIDE_PLAIN, d->act_in_slope};
-  Side sdy{dy, y, SIDE_PLAIN, d->act_out_slope};
-  if (d->act_out == KT_ACT_LRELU) sdy.mode = SIDE_DLRELU;
-  else if (d->act_out == KT_ACT_TANH) sdy.mode = SIDE_DTANH;
-  else sdy.aux = nullptr;
+  const Side sx = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
+  const Side sdy = make_side(dy, y, d->act_out, d->act_out_slope, true);
   if (d->transposed) { p.a = sdy; p.b = sx; }
   else { p.a = sx; p.b = sdy; }
-  if (pl.tma) p.nsplit = pl.nsplit_tma;
   const bool direct = p.nsplit == 1;      // one split: the partial tile IS the gradient
   p.ws = direct ? dw : ws;
+  const dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
   if (pl.tma) {
     WgTmaExtra& x = pl.x;
     __nv_bfloat16* pa = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_a_off);
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
     KT_CHECK_CUDA(split_planes(p.a, na, pa, p.b, nb, pb, st));
-    {
-      const cuuint64_t gdim[5] = {(cuuint64_t)p.cb, (cuuint64_t)p.nsub, (cuuint64_t)p.t_b, (cuuint64_t)p.batch, 2};
-      const cuuint64_t gstr[4] = {(cuuint64_t)p.cb * 2, (cuuint64_t)p.nsub * p.cb * 2, (cuuint64_t)p.t_b * p.nsub * p.cb * 2, (cuuint64_t)nb * 2};
-      const cuuint32_t box[5] = {64, (cuuint32_t)p.nsub, (cuuint32_t)x.tt, 1, 1};
-      const int rc = encode_tensor_map(&x.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pb, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv1d_bwd_weight_tc (operand B)");
-      if (rc) return rc;
-    }
-    for (int rho = 0; rho < p.step; ++rho) {
-      const cuuint64_t gdim[5] = {(cuuint64_t)p.ca, (cuuint64_t)p.nsub, (cuuint64_t)ceil_div(p.t_a - rho, p.step), (cuuint64_t)p.batch, 2};
-      const cuuint64_t gstr[4] = {(cuuint64_t)p.ca * 2, (cuuint64_t)p.step * p.nsub * p.ca * 2, (cuuint64_t)p.t_a * p.nsub * p.ca * 2, (cuuint64_t)na * 2};
-      const cuuint32_t box[5] = {64, (cuuint32_t)p.nsub, (cuuint32_t)x.a_box_t, 1, 1};
-      const int rc = encode_tensor_map(&x.map_a[rho], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, pa + (long long)rho * p.nsub * p.ca, gdim, gstr, box,
-                                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv1d_bwd_weight_tc (operand A)");
-      if (rc) return rc;
-    }
+    int rc = encode_plane_map(&x.map_b, pb, p.batch, p.t_b, p.nsub, p.cb, 1, 0, 64, x.tt, "conv1d_bwd_weight_tc (operand B)");
+    for (int rho = 0; rc == KT_OK && rho < p.step; ++rho)
+      rc = encode_plane_map(&x.map_a[rho], pa, p.batch, p.t_a, p.nsub, p.ca, p.step, rho, 64, x.a_box_t, "conv1d_bwd_weight_tc (operand A)");
+    if (rc) return rc;
     KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<64>>(kMaxDynSmem));
     KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<128>>(kMaxDynSmem));
-    dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
-    if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
-    else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem_tma, st>>>(p, x);
-    KT_CHECK_CUDA(cudaGetLastError());
+    if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem, st>>>(p, x);
+    else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem, st>>>(p, x);
   } else {
     KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<64>>(kMaxDynSmem));
     KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<128>>(kMaxDynSmem));
-    dim3 grid(p.groups * p.n_ca_tiles * p.n_cb_tiles, p.ngroups, p.nsplit);
     if (p.NT == 64) wgrad_tc_kernel<64><<<grid, kWgThreads, pl.smem, st>>>(p);
     else wgrad_tc_kernel<128><<<grid, kWgThreads, pl.smem, st>>>(p);
-    KT_CHECK_CUDA(cudaGetLastError());
   }
+  KT_CHECK_CUDA(cudaGetLastError());
   const long long n = (long long)p.taps_total * p.ca_g0 * p.cb;
   if (p.nsplit >= 16) {
     const int wblocks = (int)std::max<long long>(1, std::min<long long>((n / 4 + 7) / 8, 132LL * 8));
