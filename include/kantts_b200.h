@@ -333,6 +333,48 @@ int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, c
 int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float* x, const float* h, const float* dy,
                     const void* wimg1_bwd, const void* wimg2_bwd, float* dh, float* dx, void* stream);
 
+/* ---- streaming inference of causal layers (Generator.streamer: the waveform chunk by chunk) -------------------------
+ * A stream keeps each layer input of batch item b in a WINDOW of `pitch` rows x C channels, channels-last:
+ *   window row first + t  =  time step t of the current chunk (t >= 0),
+ *   rows [0, first)       =  the last `first` time steps of the earlier chunks (zeros at the start of an utterance).
+ * KtStreamWin places the three row tensors of one conv call: element (b, t, c) of x is
+ * x[((b * in_pitch + in_first + t) * c_in + c], likewise y (out_*) and resid (res_*; ignored when resid is NULL). */
+typedef struct KtStreamWin {
+  int32_t in_pitch, in_first;
+  int32_t out_pitch, out_first;
+  int32_t res_pitch, res_first;
+} KtStreamWin;
+/* Forward of one chunk.  The descriptor is the layer's with t_in / t_out = the chunk's rows (nsub == 1): a tap before the
+ * chunk reads the window's earlier rows, down to -in_first, where the whole-sequence forward reads its zero padding; a
+ * nearest-upsampled conv reads input row floor(t / upsample) of the same window.  The output goes to rows
+ * out_first + [0, t_out) of each item's output window.  _tc_stream: the register-staged tensor-core kernel
+ * (kt_conv1d_tc_plan(d, KT_PLAN_STREAM) != 0; no workspace), `wimg` = the forward image of that N tile. */
+int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd, const float* bias,
+                         const float* resid, float* y, void* stream);
+int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg, const float* bias,
+                            const float* resid, float* y, void* stream);
+/* kt_conv1d_tc_plan / kt_conv1d_tc_workspace / kt_debug_conv_tc_plan: direction flag of the stream forward (OR'd into dir 0):
+ * the plan of kt_conv1d_fwd_tc_stream, which always takes the register-staged route. */
+#define KT_PLAN_STREAM 16
+/* Elementwise stages into a window: row t of item b of x, a, b, c at x[((b * x_pitch + t) * ch], of y at
+ * y[((b * y_pitch + y_first + t) * ch], t < rows.  y = sin(x) + x;  y = scale * (a + b + c) (b, c optional). */
+int kt_sinadd_fwd_win(const float* x, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t x_pitch, int32_t y_pitch,
+                      int32_t y_first, void* stream);
+int kt_add3_scale_win(const float* a, const float* b, const float* c, float scale, float* y, int32_t batch, int32_t rows,
+                      int32_t ch, int32_t x_pitch, int32_t y_pitch, int32_t y_first, void* stream);
+/* One window of a stream: [batch][pitch][channels] fp32 at `base`, keeping `history` rows between chunks; a chunk of f
+ * frames writes f * rows_per_frame rows at row `history`. */
+typedef struct KtWindow {
+  float* base;
+  int32_t pitch, channels, history, rows_per_frame;
+} KtWindow;
+/* ONE launch over the device table `windows` [n]: after a chunk of `frames` frames, rows [0, history) of every window take
+ * the last `history` rows of (history | chunk), i.e. rows [r, r + history) with r = frames * rows_per_frame -- also when
+ * r < history and the two ranges overlap.  max_channels >= every window's channels. */
+int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t frames, int32_t max_channels, void* stream);
+/* ONE launch: rows [0, history) of every window are zeroed for the batch items b with slots[b] != 0 (device uint8 [batch]). */
+int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream);
+
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

@@ -19,6 +19,7 @@ SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.c
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
+KT_PLAN_STREAM = 16
 
 
 class KtConv1dDesc(ctypes.Structure):
@@ -32,6 +33,15 @@ class KtConv1dDesc(ctypes.Structure):
 class KtResblockDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("batch", "t", "channels", "kernel", "dilation", "pad_left1", "pad_left2")] + \
                [("slope", ctypes.c_float), ("path", ctypes.c_int32)]
+
+
+class KtStreamWin(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("in_pitch", "in_first", "out_pitch", "out_first", "res_pitch", "res_first")]
+
+
+class KtWindow(ctypes.Structure):
+    _fields_ = [("base", ctypes.c_void_p)] + \
+               [(n, ctypes.c_int32) for n in ("pitch", "channels", "history", "rows_per_frame")]
 
 
 class KtMelDesc(ctypes.Structure):
@@ -95,6 +105,12 @@ PROTOTYPES = {
     "kt_fp_insert_plan": [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P],
     "kt_fp_insert_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_fp_insert_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
+    "kt_conv1d_fwd_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_fwd_tc_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
+    "kt_sinadd_fwd_win": [_P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_add3_scale_win": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_stream_advance": [_P, _I, _I, _I, _I, _P],
+    "kt_stream_reset": [_P, _I, _I, _P, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_version": [],

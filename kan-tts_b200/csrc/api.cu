@@ -32,6 +32,14 @@ int conv1d_bwd_data_tc(const KtConv1dDesc*, const float*, const float*, const vo
                        bool allow_tma = true);
 int ar_duration_infer(const float*, const float*, const float*, const float*, const float*, const float*, const float*, const float*,
                       const float*, const float*, const float*, float, float*, int, int, int, int, int, cudaStream_t);
+int conv1d_fwd_ffma_stream(const KtConv1dDesc*, const KtStreamWin*, const float*, const float*, const float*, const float*, float*,
+                           cudaStream_t);
+int conv1d_fwd_tc_stream(const KtConv1dDesc*, const KtStreamWin*, const float*, const void*, const float*, const float*, float*,
+                         cudaStream_t);
+int sinadd_fwd_win(const float*, float*, int, int, int, int, int, int, cudaStream_t);
+int add3_scale_win(const float*, const float*, const float*, float, float*, int, int, int, int, int, int, cudaStream_t);
+int stream_advance(const KtWindow*, int, int, int, int, cudaStream_t);
+int stream_reset(const KtWindow*, int, int, const uint8_t*, int, cudaStream_t);
 int resblock_plan(const KtResblockDesc*);
 long long resblock_image_bytes(const KtResblockDesc*);
 int resblock_pack(const KtResblockDesc*, const float*, void*, cudaStream_t);
@@ -189,6 +197,46 @@ int kt_conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y
   if (rc) return rc;
   KT_REQUIRE(dy && wimg && dx, "kt_conv1d_bwd_data_tc: null pointer");
   return kt::conv1d_bwd_data_tc(d, dy, y, wimg, x, dx, workspace, workspace_floats, ST(stream));
+}
+
+static int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what) {
+  int rc = kt::validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(w != nullptr, "%s: null window descriptor", what);
+  KT_REQUIRE(d->nsub == 1, "%s: streams need nsub == 1", what);
+  KT_REQUIRE(w->in_first >= 0 && w->in_first + d->t_in <= w->in_pitch, "%s: the chunk does not fit its input window", what);
+  KT_REQUIRE(w->out_first >= 0 && w->out_first + d->t_out <= w->out_pitch, "%s: the chunk does not fit its output window", what);
+  KT_REQUIRE(!resid || (w->res_first >= 0 && w->res_first + d->t_out <= w->res_pitch),
+             "%s: the chunk does not fit its residual window", what);
+  return KT_OK;
+}
+int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd, const float* bias,
+                         const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
+  return kt::conv1d_fwd_ffma_stream(d, w, x, w_fwd, bias, resid, y, ST(stream));
+}
+int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg, const float* bias,
+                            const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
+  return kt::conv1d_fwd_tc_stream(d, w, x, wimg, bias, resid, y, ST(stream));
+}
+int kt_sinadd_fwd_win(const float* x, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t x_pitch, int32_t y_pitch,
+                      int32_t y_first, void* stream) {
+  return kt::sinadd_fwd_win(x, y, batch, rows, ch, x_pitch, y_pitch, y_first, ST(stream));
+}
+int kt_add3_scale_win(const float* a, const float* b, const float* c, float scale, float* y, int32_t batch, int32_t rows,
+                      int32_t ch, int32_t x_pitch, int32_t y_pitch, int32_t y_first, void* stream) {
+  return kt::add3_scale_win(a, b, c, scale, y, batch, rows, ch, x_pitch, y_pitch, y_first, ST(stream));
+}
+int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t frames, int32_t max_channels, void* stream) {
+  return kt::stream_advance(windows, n, batch, frames, max_channels, ST(stream));
+}
+int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream) {
+  return kt::stream_reset(windows, n, batch, slots, max_channels, ST(stream));
 }
 
 int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, const float* w2t, const float* b2, const float* wih0t,

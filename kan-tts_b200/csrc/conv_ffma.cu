@@ -58,13 +58,16 @@ struct CoreParams {
   float out_slope;
   int rmax;            // rows of the activation tile the host sized shared memory for
   Phase ph;
+  // stream instances (kt_conv1d_fwd_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
+  int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
 };
 
 __device__ __forceinline__ long long row_index(int bb, int t, int T, int nsub) {
   return ((long long)(bb / nsub) * T + t) * nsub + (bb % nsub);
 }
 
-template <int RN, int RM, int KC>
+// STREAM: rows are addressed in the windows of KtStreamWin, and input rows down to -in_first are real data
+template <int RN, int RM, int KC, bool STREAM = false>
 __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant__ CoreParams p) {
   constexpr int TN = 32 * RN;
   constexpr int TM = 8 * RM;
@@ -105,8 +108,9 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
       const int tin = row_lo + r;
       const int c = c0 + q * 4;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (tin >= 0 && tin < p.t_in && c < p.cin_g) {
-        const long long off = row_index(bb, tin, p.t_in, p.nsub) * p.c_in + (long long)g * p.cin_g + c;
+      if (tin >= (STREAM ? -p.in_first : 0) && tin < p.t_in && c < p.cin_g) {
+        const long long row = STREAM ? (long long)bb * p.in_pitch + p.in_first + tin : row_index(bb, tin, p.t_in, p.nsub);
+        const long long off = row * p.c_in + (long long)g * p.cin_g + c;
         if (vec_in && c + 3 < p.cin_g) {
           v = __ldg(reinterpret_cast<const float4*>(p.in.p + off));
           if (p.in.mode >= SIDE_DLRELU) {
@@ -208,7 +212,10 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
     const int m = m0 + warp * RM + i;
     if (m >= ph.M) continue;
     const int to = ph.o_off + ph.o_step * m;
-    const long long obase = row_index(bb, to, p.t_out, p.nsub) * p.c_out + (long long)g * p.cout_g;
+    const long long orow = STREAM ? (long long)bb * p.out_pitch + p.out_first + to : row_index(bb, to, p.t_out, p.nsub);
+    const long long obase = orow * p.c_out + (long long)g * p.cout_g;
+    // residual element = output element + rdelta (0 outside streams: the residual has the output's layout)
+    const long long rdelta = STREAM ? ((long long)bb * (p.res_pitch - p.out_pitch) + p.res_first - p.out_first) * p.c_out : 0;
 #pragma unroll
     for (int j = 0; j < RN; ++j) {
       const int co = co0 + lane * RN + j;
@@ -219,25 +226,26 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
       if (p.out_act == KT_ACT_LRELU) v = v > 0.f ? v : v * p.out_slope;
       else if (p.out_act == KT_ACT_TANH) v = tanhf(v);
       if (p.mask.p) v = side_apply(v, __ldg(p.mask.p + o), p.mask.mode, p.mask.slope);
-      if (p.resid) v += __ldg(p.resid + o);
+      if (p.resid) v += __ldg(p.resid + o + rdelta);
       if (ph.accumulate) v += p.out[o];
       p.out[o] = v;
     }
   }
 }
 
-template <int RN, int RM, int KC>
+template <int RN, int RM, int KC, bool STREAM>
 static int launch_core(const CoreParams& p, cudaStream_t st) {
   constexpr int TN = 32 * RN, TM = 8 * RM, NTC = 4;
   const size_t smem = ((size_t)p.rmax * KC + (size_t)NTC * KC * TN) * sizeof(float);
   KT_REQUIRE(smem <= 200 * 1024, "conv_core: activation tile too large (%zu bytes shared)", smem);
-  KT_CHECK_CUDA(allow_dyn_smem<conv_core_kernel<RN, RM, KC>>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<conv_core_kernel<RN, RM, KC, STREAM>>(kMaxDynSmem));
   dim3 grid(ceil_div(p.ph.M, TM), p.groups * ceil_div(p.cout_g, TN), p.batch);
-  conv_core_kernel<RN, RM, KC><<<grid, 256, smem, st>>>(p);
+  conv_core_kernel<RN, RM, KC, STREAM><<<grid, 256, smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
 
+template <bool STREAM = false>
 static int run_core(CoreParams p, cudaStream_t st) {
   if (p.ph.M <= 0 || p.ph.ntaps <= 0) return KT_OK;
   const int RN = p.cout_g > 64 ? 4 : (p.cout_g > 32 ? 2 : 1);
@@ -250,7 +258,7 @@ static int run_core(CoreParams p, cudaStream_t st) {
   p.rmax = fdiv((TM - 1) * p.ph.i_step + p.ph.max_ioff - p.ph.min_ioff, p.ph.up) + 2;
   const int KC = p.cin_g <= 4 ? 4 : 16;
 #define KT_CORE_CASE(rn, rm, kc) \
-  if (RN == rn && RM == rm && KC == kc) return launch_core<rn, rm, kc>(p, st);
+  if (RN == rn && RM == rm && KC == kc) return launch_core<rn, rm, kc, STREAM>(p, st);
   KT_CORE_CASE(4, 16, 16) KT_CORE_CASE(4, 8, 16) KT_CORE_CASE(4, 4, 16)
   KT_CORE_CASE(2, 16, 16) KT_CORE_CASE(2, 8, 16) KT_CORE_CASE(2, 4, 16)
   KT_CORE_CASE(1, 16, 16) KT_CORE_CASE(1, 8, 16) KT_CORE_CASE(1, 4, 16)
@@ -653,6 +661,25 @@ int conv1d_fwd_ffma(const KtConv1dDesc* d, const float* x, const float* w_fwd, c
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
     int rc = run_core(p, st);
+    if (rc) return rc;
+  }
+  return KT_OK;
+}
+
+// One chunk of a stream (KtStreamWin): the forward's phases over the windows
+int conv1d_fwd_ffma_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd, const float* bias,
+                           const float* resid, float* y, cudaStream_t st) {
+  CoreParams p{};
+  p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
+  p.w = w_fwd; p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
+  p.batch = d->batch; p.nsub = 1; p.t_in = d->t_in; p.t_out = d->t_out;
+  p.c_in = d->c_in; p.c_out = d->c_out; p.groups = d->groups; p.cin_g = d->c_in / d->groups; p.cout_g = d->c_out / d->groups;
+  p.out_act = d->act_out; p.out_slope = d->act_out_slope;
+  p.in_pitch = w->in_pitch; p.in_first = w->in_first; p.out_pitch = w->out_pitch; p.out_first = w->out_first;
+  p.res_pitch = w->res_pitch; p.res_first = w->res_first;
+  for (const Phase& ph : conv_phases(d, 0)) {
+    p.ph = ph;
+    int rc = run_core<true>(p, st);
     if (rc) return rc;
   }
   return KT_OK;

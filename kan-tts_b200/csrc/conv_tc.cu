@@ -132,6 +132,8 @@ struct TcParams {
   // output rows per m-tile: kTcM on the register-staged route; tt whole time steps x nsub on the TMA route
   int R, tt;
   int a_box_t;                        // TMA route: time steps per image box = tt + span_q
+  // stream instances (kt_conv1d_fwd_tc_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
+  int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
 };
 
 // TMA route: one tensor map of the gathered operand's planes per input residue class rho (base + rho rows, time stride
@@ -157,9 +159,12 @@ enum TcRoute { kTcRegSimple = 0, kTcReg = 1, kTcTma = 2 };
 
 // Persistent: gridDim.x = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  The activation and
 // weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
-template <int ROUTE>
+// STREAM (register-staged routes only): one chunk of a stream -- rows live in the windows of KtStreamWin, and the input
+// rows before the chunk (down to -in_first) are real data instead of zero padding.
+template <int ROUTE, bool STREAM = false>
 __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
     conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
+  static_assert(!(STREAM && ROUTE == kTcTma), "stream chunks take the register-staged route");
   constexpr bool SIMPLE = ROUTE == kTcRegSimple;
   constexpr bool TMA = ROUTE == kTcTma;
   constexpr int kConsumer0 = TMA ? 0 : 4;     // first consumer warp
@@ -210,10 +215,15 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
           mbar_wait(&empty_a[s], ra.phase() ^ 1u);
           uint8_t* img_hi = a_base + (size_t)s * a_stage_bytes;
           RowMap rm;
-          rm.base_row = (long long)bb * p.t_in * p.nsub;
+          if constexpr (STREAM) {
+            rm.base_row = (long long)bb * p.in_pitch + p.in_first;
+            rm.t_lo = -p.in_first * p.up;
+          } else {
+            rm.base_row = (long long)bb * p.t_in * p.nsub;
+          }
           rm.fv0 = f0 + p.grp_qlo[g] * p.nsub;
           rm.nsub = p.nsub; rm.step = p.i_step; rm.rho = p.grp_rho[g]; rm.up = p.up; rm.t_lim = p.t_in * p.up;
-          stage_rows<5, SIMPLE, 3>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
+          stage_rows<5, SIMPLE, 3, STREAM>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
                                    min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
           fence_proxy_async();
           mbar_arrive(&full_a[s]);
@@ -357,7 +367,10 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
           const int m = p.nsub == 1 ? f : f / p.nsub;
           const int w = f - m * p.nsub;
           const int to = p.ph_ooff[ph] + p.o_step * m;
-          const long long obase = ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
+          const long long obase = STREAM ? ((long long)bb * p.out_pitch + p.out_first + to) * p.c_out + c_tile
+                                         : ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
+          // residual element = output element + rdelta (0 outside streams: the residual has the output's layout)
+          const long long rdelta = STREAM ? ((long long)bb * (p.res_pitch - p.out_pitch) + p.res_first - p.out_first) * p.c_out : 0;
 #pragma unroll
           for (int i = 0; i < NT / 8; ++i) {
             const int col = i * 8 + 2 * (lane & 3);
@@ -370,7 +383,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
             if (pair) {
               if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + c_tile + col)); bia[0] = t.x; bia[1] = t.y; }
               if (p.mask.p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.mask.p + o)); md[0] = t.x; md[1] = t.y; }
-              if (p.resid) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.resid + o)); sd[0] = t.x; sd[1] = t.y; }
+              if (p.resid) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.resid + o + rdelta)); sd[0] = t.x; sd[1] = t.y; }
               if (!SIMPLE && p.accumulate) { const float2 t = *reinterpret_cast<const float2*>(p.out + o); od[0] = t.x; od[1] = t.y; }
             } else {
 #pragma unroll
@@ -378,7 +391,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
                 if (e >= ne) break;
                 if (p.bias) bia[e] = __ldg(p.bias + c_tile + col + e);
                 if (p.mask.p) md[e] = __ldg(p.mask.p + o + e);
-                if (p.resid) sd[e] = __ldg(p.resid + o + e);
+                if (p.resid) sd[e] = __ldg(p.resid + o + rdelta + e);
                 if (!SIMPLE && p.accumulate) od[e] = p.out[o + e];
               }
             }
@@ -583,15 +596,25 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   return P;
 }
 
+// dir: 0 / 1, or KT_PLAN_STREAM (the forward of a stream chunk: register-staged route, nsub == 1)
+static TcPlan make_tc_plan_flags(const KtConv1dDesc* d, int dir, bool plan_only = false) {
+  if (dir == KT_PLAN_STREAM) {
+    if (d->nsub != 1) return TcPlan{};
+    return make_tc_plan(d, 0, false, plan_only);
+  }
+  return make_tc_plan(d, dir, true, plan_only);
+}
+
 int tc_plan(const KtConv1dDesc* d, int dir) {
-  const TcPlan P = make_tc_plan(d, dir);
+  const TcPlan P = make_tc_plan_flags(d, dir);
   return P.ok ? P.L.NT : 0;
 }
 
-long long conv_tc_workspace(const KtConv1dDesc* d, int dir) { return make_tc_plan(d, dir).ws_floats; }
+long long conv_tc_workspace(const KtConv1dDesc* d, int dir) { return make_tc_plan_flags(d, dir).ws_floats; }
 
 // bytes of the packed split-bf16 weight image of direction `dir` (0 when unsupported)
 long long tc_image_bytes(const KtConv1dDesc* d, int dir) {
+  if (dir != 0 && dir != 1) return 0;
   if (tc_plan(d, dir) == 0) return 0;
   const TcLayerPlan L = layer_plan(d, dir);
   return (long long)d->kernel * L.kchunks * L.ntiles * 2LL * L.NT * kTcKC * 2LL;
@@ -637,7 +660,7 @@ static size_t size_stages(TcParams& p) {
 // out = {N tile (0: not on the tensor cores), TMA route, tt, R, a_box_t, image stages, weight stages, shared-memory bytes,
 // workspace floats}, the launch-dependent entries for the first launch
 void debug_conv_tc_plan(const KtConv1dDesc* d, int dir, long long* out) {
-  TcPlan P = make_tc_plan(d, dir, true, true);
+  TcPlan P = make_tc_plan_flags(d, dir, true);
   for (int i = 0; i < 9; ++i) out[i] = 0;
   if (!P.ok) return;
   TcParams& lp = P.launches[0];
@@ -646,7 +669,7 @@ void debug_conv_tc_plan(const KtConv1dDesc* d, int dir, long long* out) {
   out[5] = lp.na_stages; out[6] = lp.nb_stages; out[7] = (long long)smem; out[8] = P.ws_floats;
 }
 
-static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, cudaStream_t st) {   // p: phases already planned
+static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, cudaStream_t st) {   // p: phases already planned
   const size_t smem = size_stages(p);
   KT_REQUIRE(smem > 0, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
   const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
@@ -658,7 +681,13 @@ static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, cudaStream_t st) 
     const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
                         (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
                         (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
-    if (simple) {
+    if (stream && simple) {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple, true>>(kMaxDynSmem));
+      conv_tc_kernel<kTcRegSimple, true><<<grid, kTcThreads, smem, st>>>(p, maps);
+    } else if (stream) {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg, true>>(kMaxDynSmem));
+      conv_tc_kernel<kTcReg, true><<<grid, kTcThreads, smem, st>>>(p, maps);
+    } else if (simple) {
       KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple>>(kMaxDynSmem));
       conv_tc_kernel<kTcRegSimple><<<grid, kTcThreads, smem, st>>>(p, maps);
     } else {
@@ -687,11 +716,13 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
   for (TcParams lp : P.launches) {
     lp.in = io.in; lp.wimg = io.wimg; lp.bias = io.bias; lp.resid = io.resid; lp.mask = io.mask; lp.out = io.out;
     lp.out_act = io.out_act; lp.out_slope = io.out_slope;
+    lp.in_pitch = io.in_pitch; lp.in_first = io.in_first; lp.out_pitch = io.out_pitch; lp.out_first = io.out_first;
+    lp.res_pitch = io.res_pitch; lp.res_first = io.res_first;
     for (int rho = 0; P.tma && rho < lp.i_step; ++rho) {
       const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what);
       if (rc) return rc;
     }
-    const int rc = run_tc(lp, maps, P.tma, st);
+    const int rc = run_tc(lp, maps, P.tma, io.in_pitch > 0, st);
     if (rc) return rc;
   }
   return KT_OK;
@@ -707,6 +738,22 @@ int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const
   io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
   return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", st);
+}
+
+// One chunk of a stream (KtStreamWin): the register-staged route over the windows
+int conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg, const float* bias,
+                         const float* resid, float* y, cudaStream_t st) {
+  const TcPlan P = make_tc_plan_flags(d, KT_PLAN_STREAM);
+  KT_REQUIRE(P.ok && !P.tma, "conv1d_fwd_tc_stream: layer not supported by the tensor-core path");
+  KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "conv1d_fwd_tc_stream: bad window pitch");
+  TcParams io{};
+  io.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
+  io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
+  io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
+  io.out_act = d->act_out; io.out_slope = d->act_out_slope;
+  io.in_pitch = w->in_pitch; io.in_first = w->in_first; io.out_pitch = w->out_pitch; io.out_first = w->out_first;
+  io.res_pitch = w->res_pitch; io.res_first = w->res_first;
+  return run_plan(P, io, nullptr, 0, "conv1d_fwd_tc_stream", st);
 }
 
 // allow_tma = false: the register-staged route, which needs no workspace (kt_resblock_bwd)

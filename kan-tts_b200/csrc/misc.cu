@@ -221,6 +221,92 @@ int add3_scale(const float* a, const float* b, const float* c, float scale, floa
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
+// ---- streaming inference (Generator.streamer): elementwise stages that write into a window, window advance / reset ----
+// y[(b * y_pitch + y_first + t) * ch + c] = f(x[(b * x_pitch + t) * ch + c]),  t < rows
+__global__ void sinadd_win_kernel(const float* __restrict__ x, float* __restrict__ y, int rows, int ch, int x_pitch, int y_pitch,
+                                  int y_first, long long n) {
+  const long long per_item = (long long)rows * ch;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / per_item, e = i - b * per_item;
+    const float v = __ldg(x + b * x_pitch * ch + e);
+    y[(b * y_pitch + y_first) * ch + e] = v + sinf(v);
+  }
+}
+
+__global__ void add3_scale_win_kernel(const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ c,
+                                      float scale, float* __restrict__ y, int rows, int ch, int x_pitch, int y_pitch, int y_first,
+                                      long long n) {
+  const long long per_item = (long long)rows * ch;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long bi = i / per_item, e = i - bi * per_item, s = bi * x_pitch * ch + e;
+    y[(bi * y_pitch + y_first) * ch + e] = scale * (__ldg(a + s) + (b ? __ldg(b + s) : 0.f) + (c ? __ldg(c + s) : 0.f));
+  }
+}
+
+// grid (channel blocks, window, batch item); a thread owns one channel column of one window of one item.  Row r of the
+// history takes row r + n (n = the chunk's rows): in groups of g = min(n, 8) rows, all loads of a group before its stores --
+// the group's sources [r0 + n, r0 + n + g) and destinations [r0, r0 + g) are disjoint, and a later group reads only rows
+// >= r0 + g + n that no store has reached yet, so the move is right however n and the history compare.
+__global__ void stream_advance_kernel(const KtWindow* __restrict__ wins, int frames) {
+  const KtWindow w = wins[blockIdx.y];
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= w.channels) return;
+  const int n = frames * w.rows_per_frame;
+  const int g = min(n, 8);
+  float* col = w.base + (long long)blockIdx.z * w.pitch * w.channels + c;
+  for (int r0 = 0; r0 < w.history; r0 += g) {
+    float v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i < g && r0 + i < w.history) v[i] = col[(long long)(r0 + i + n) * w.channels];
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i < g && r0 + i < w.history) col[(long long)(r0 + i) * w.channels] = v[i];
+  }
+}
+
+__global__ void stream_reset_kernel(const KtWindow* __restrict__ wins, const uint8_t* __restrict__ slots) {
+  if (!slots[blockIdx.z]) return;
+  const KtWindow w = wins[blockIdx.y];
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= w.channels) return;
+  float* col = w.base + (long long)blockIdx.z * w.pitch * w.channels + c;
+  for (int r = 0; r < w.history; ++r) col[(long long)r * w.channels] = 0.f;
+}
+
+int sinadd_fwd_win(const float* x, float* y, int batch, int rows, int ch, int x_pitch, int y_pitch, int y_first, cudaStream_t st) {
+  KT_REQUIRE(x && y && batch > 0 && rows > 0 && ch > 0 && rows <= x_pitch && y_first >= 0 && y_first + rows <= y_pitch,
+             "sinadd_fwd_win: bad arguments");
+  const long long n = (long long)batch * rows * ch;
+  sinadd_win_kernel<<<stream_grid(n, 256), 256, 0, st>>>(x, y, rows, ch, x_pitch, y_pitch, y_first, n);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+int add3_scale_win(const float* a, const float* b, const float* c, float scale, float* y, int batch, int rows, int ch, int x_pitch,
+                   int y_pitch, int y_first, cudaStream_t st) {
+  KT_REQUIRE(a && y && batch > 0 && rows > 0 && ch > 0 && rows <= x_pitch && y_first >= 0 && y_first + rows <= y_pitch,
+             "add3_scale_win: bad arguments");
+  const long long n = (long long)batch * rows * ch;
+  add3_scale_win_kernel<<<stream_grid(n, 256), 256, 0, st>>>(a, b, c, scale, y, rows, ch, x_pitch, y_pitch, y_first, n);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+int stream_advance(const KtWindow* wins, int n, int batch, int frames, int max_c, cudaStream_t st) {
+  KT_REQUIRE(wins && n >= 0 && n <= 65535 && batch > 0 && batch <= 65535 && frames > 0 && max_c > 0,
+             "stream_advance: bad arguments");
+  if (n == 0) return KT_OK;
+  stream_advance_kernel<<<dim3(ceil_div(max_c, 128), n, batch), 128, 0, st>>>(wins, frames);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+int stream_reset(const KtWindow* wins, int n, int batch, const uint8_t* slots, int max_c, cudaStream_t st) {
+  KT_REQUIRE(wins && slots && n >= 0 && n <= 65535 && batch > 0 && batch <= 65535 && max_c > 0, "stream_reset: bad arguments");
+  if (n == 0) return KT_OK;
+  stream_reset_kernel<<<dim3(ceil_div(max_c, 128), n, batch), 128, 0, st>>>(wins, slots);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
 int dwt_fwd(const float* x, float* y, int batch, int t, cudaStream_t st) {
   KT_REQUIRE(x && y && batch > 0 && t > 0, "dwt_fwd: bad arguments");
   const int t2 = (t + 5) / 2;

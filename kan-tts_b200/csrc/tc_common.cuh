@@ -211,23 +211,28 @@ static inline cudaError_t split_planes(const Side& a, long long na, __nv_bfloat1
 //     source row = base_row + (tv / up) * nsub + w
 // With this map a conv tap (q, rho) is the row shift q * nsub of residue image rho for ANY stride and
 // period, so every M = 128 tile is a dense run of flattened outputs.
+// STREAM (a chunk of a stream, nsub == 1): base_row is the row of time step 0 in the item's window, and the rows before it
+// are real data down to tv >= t_lo (= -history * up); negative up-sampled times take the floor.
 struct RowMap {
   long long base_row;
   int fv0, nsub, step, rho, up, t_lim;
+  int t_lo;   // STREAM only
   // nsub == 1 && up == 1 (every layer but the period discriminator's and the nearest-upsampled convs): no divisions
+  template <bool STREAM = false>
   __device__ __forceinline__ bool map_simple(int r, long long& row) const {
     const int tv = (fv0 + r) * step + rho;
-    if (tv < 0 || tv >= t_lim) return false;
+    if (tv < (STREAM ? t_lo : 0) || tv >= t_lim) return false;
     row = base_row + tv;
     return true;
   }
+  template <bool STREAM = false>
   __device__ __forceinline__ bool map(int r, long long& row) const {
     const int fv = fv0 + r;
     const int mp = nsub == 1 ? fv : fdiv(fv, nsub);
     const int w = fv - mp * nsub;
     const int tv = mp * step + rho;
-    if (tv < 0 || tv >= t_lim) return false;
-    row = base_row + (long long)(up == 1 ? tv : tv / up) * nsub + w;
+    if (tv < (STREAM ? t_lo : 0) || tv >= t_lim) return false;
+    row = base_row + (long long)(up == 1 ? tv : (STREAM ? fdiv(tv, up) : tv / up)) * nsub + w;
     return true;
   }
 };
@@ -237,7 +242,7 @@ struct RowMap {
 // converts and stores.  The two phases are separate fully-unrolled loops without early exits: with one
 // CTA per SM the staging loop is pure DRAM/L2 latency, and a fused load->convert->store loop measured
 // ~1 load in flight per thread.
-template <int NB, bool VEC, bool AUX, bool SIMPLE = false>
+template <int NB, bool VEC, bool AUX, bool SIMPLE = false, bool STREAM = false>
 __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                                 const float* aux_base, int c_total, int ch0, int nv, const RowMap& rm,
                                                 int rows, int tid, int r_begin = 0) {
@@ -250,7 +255,7 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
     for (int i = 0; i < NB; ++i) {
       const int r = r0 + 16 * i;
       long long srow = 0;
-      ok[i] = r < rows && nv > 0 && (SIMPLE ? rm.map_simple(r, srow) : rm.map(r, srow));
+      ok[i] = r < rows && nv > 0 && (SIMPLE ? rm.template map_simple<STREAM>(r, srow) : rm.template map<STREAM>(r, srow));
       off[i] = ok[i] ? srow * c_total + ch0 + q * 8 : 0;   // offset 0 is always a readable address
     }
 #pragma unroll
@@ -305,7 +310,7 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
 // SIMPLE: the host guarantees nsub == 1, up == 1 and 16-byte-aligned 8-channel chunks (c_valid % 8 == 0, c_total % 4
 // == 0): only the vectorised instantiations exist in that kernel variant, which roughly halves its code size -- the
 // generic kernel (~140 KB of SASS shared by four concurrently running warp roles) does not fit the instruction cache.
-template <int NB, bool SIMPLE = false, int NB_AUX = NB>
+template <int NB, bool SIMPLE = false, int NB_AUX = NB, bool STREAM = false>
 __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                            const float* aux_base, int c_total, int ch0, int c_valid, bool fill_all,
                                            const RowMap& rm, int rows, int tid, int r_begin = 0) {
@@ -332,16 +337,16 @@ __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, con
   const bool vec = nv == 8 && (c_total & 3) == 0 && ((ch0 + q * 8) & 3) == 0;
   const bool has_aux = s.mode >= SIDE_DLRELU;
   if constexpr (SIMPLE) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true, true>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false, true>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, true, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, true, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
     return;
   }
   if (vec) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   } else {
-    if (has_aux) stage_rows_impl<2, false, true>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<2, false, false>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<2, false, true, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<2, false, false, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   }
 }
 

@@ -11,8 +11,8 @@ from dataclasses import dataclass, field, replace
 import torch
 
 from . import _lib
-from ._lib import (KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC, KtConv1dDesc, KtMelDesc,
-                   KtResblockDesc, check, ptr, stream_ptr)
+from ._lib import (KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC, KT_PLAN_STREAM, KtConv1dDesc,
+                   KtMelDesc, KtResblockDesc, check, ptr, stream_ptr)
 
 _launches = 0          # kernels-launched counter (bench.py reports it as gpu_launches)
 
@@ -133,13 +133,14 @@ class ConvSpec:
         t = t_in * self.upsample
         return (t + self.pad_left + self.pad_right - self.dilation * (self.kernel - 1) - 1) // self.stride + 1
 
-    def plan(self, batch, nsub, t_in):
-        """-> the ConvPlan of this layer for one input shape, cached per shape and exact-path flag (the tests toggle
-        set_force_ffma at run time).  Every field of the spec must be set before its first plan."""
-        key = (batch, nsub, t_in, _exact(self))
+    def plan(self, batch, nsub, t_in, stream=False):
+        """-> the ConvPlan of this layer for one input shape, cached per shape, exact-path flag (the tests toggle
+        set_force_ffma at run time) and stream flag (the forward of a stream chunk, see stream_conv).  Every field of the
+        spec must be set before its first plan."""
+        key = (batch, nsub, t_in, _exact(self), stream)
         p = self._plans.get(key)
         if p is None:
-            p = self._plans[key] = ConvPlan(self, batch, nsub, t_in, key[3])
+            p = self._plans[key] = ConvPlan(self, batch, nsub, t_in, key[3], stream)
         return p
 
     def desc(self, batch, nsub, t_in):
@@ -162,11 +163,12 @@ class ConvPlan:
       nt_fwd                   forward N tile
       d_bwd, nt_bwd, up_bwd    data gradient: descriptor, N tile, and whether it runs over the up-sampled rows
       ws_fwd, ws_bwd           tensor-core forward / data-gradient workspace (operand planes of the TMA-fed route), in floats
-      wg_ws                    tensor-core weight-gradient workspace, in floats"""
+      wg_ws                    tensor-core weight-gradient workspace, in floats
+    A stream plan (stream=True) plans the forward of a stream chunk only: the register-staged route, no workspace."""
 
     __slots__ = ("spec", "d", "nt_fwd", "d_bwd", "nt_bwd", "up_bwd", "ws_fwd", "ws_bwd", "wg_ws")
 
-    def __init__(self, spec, batch, nsub, t_in, exact):
+    def __init__(self, spec, batch, nsub, t_in, exact, stream=False):
         self.spec = spec
         self.d = self.d_bwd = d = spec.desc(batch, nsub, t_in)
         self.nt_fwd = self.nt_bwd = self.ws_fwd = self.ws_bwd = self.wg_ws = 0
@@ -174,6 +176,9 @@ class ConvPlan:
         if exact:
             return
         lib = _lib.load()
+        if stream:
+            self.nt_fwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), KT_PLAN_STREAM)
+            return
         self.nt_fwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 0)
         self.nt_bwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 1)
         if (not self.nt_bwd and spec.path == KT_PATH_AUTO and spec.upsample > 1 and spec.c_in % 4 == 0
@@ -567,6 +572,23 @@ class ConvFn(torch.autograd.Function):
 
 def conv(x, spec, cache, v, g=None, bias=None, resid=None, reuse=None):
     return ConvFn.apply(x, resid, bias, v, g, spec, cache, reuse)
+
+
+def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None):
+    """One chunk of a causal layer in a stream (no autograd): x, y and resid are the layer's (B, pitch, C) windows, placed
+    by ``win`` (a KtStreamWin), and ``t_in`` is the chunk's input rows; the taps before the chunk read the window's history.
+    ``pw``: the layer's PreparedWeight, prepared by the caller.  Planned once per chunk shape (ConvSpec.plan, stream=True);
+    the tensor-core image of the plan's N tile is packed from ``pw`` on its first use."""
+    plan = spec.plan(x.shape[0], 1, t_in, stream=True)
+    d, nt = plan.d, plan.tile(0)
+    if nt:
+        img = pw.image((0, nt), d)
+        _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(img, True),
+                                            ptr(bias), ptr(resid), ptr(y), stream_ptr()))
+    else:
+        n = spec.stride if spec.transposed else 1
+        _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(pw.w_fwd),
+                                              ptr(bias), ptr(resid), ptr(y), stream_ptr()))
 
 
 # ---- pair_reuse: one (generated, real) pair batch per phase, the real half computed once per step -----------------------

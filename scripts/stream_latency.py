@@ -1,0 +1,97 @@
+"""Per-chunk latency of streaming synthesis (Generator.streamer) on the GPU.
+
+For the class-default generator (hop 256 at 22.05 kHz) and the hifigan_v1_24k.yaml generator (hop 240 at 24 kHz), over
+B in {1, 16, 64} slots x F in {1, 4, 16} frames per chunk: the device time per graph-replayed chunk (CUDA events over
+--chunks chunks after warm-up), the host time to enqueue one push, the library launches per chunk, the real-time factor
+(audio seconds per chunk / chunk time; > 1 is faster than real time), and for comparison the whole-utterance forward of
+the same frames.  Prints the card and its power limit, read in the same run.
+
+    python scripts/stream_latency.py [--chunks 200] [--out DIR]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import kantts_b200 as K  # noqa: E402
+
+GENERATORS = {
+    "default_22k": (dict(), 22050),
+    "v1_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),
+}
+# the whole-utterance forward keeps every activation of the utterance: longer ones are timed at this many frames
+WHOLE_MAX_ROWS = 64 * 256
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+
+
+def measure(gen, sr, B, F, chunks):
+    st = gen.streamer(batch=B, max_frames=F)
+    mel = torch.randn(B, 80, F, device="cuda")
+    for _ in range(10):                                  # the first push captures the graph
+        st.push(mel)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    host = 0.0
+    e0.record()
+    for _ in range(chunks):
+        t0 = time.perf_counter()
+        st.push(mel)
+        host += time.perf_counter() - t0
+    e1.record()
+    torch.cuda.synchronize()
+    chunk_ms = e0.elapsed_time(e1) / chunks
+    # whole-utterance forward of the same frames (capped, see WHOLE_MAX_ROWS)
+    frames = min(chunks * F, max(F, WHOLE_MAX_ROWS // B))
+    whole = torch.randn(B, 80, frames, device="cuda")
+    with torch.no_grad():
+        gen(whole)
+        torch.cuda.synchronize()
+        w0, w1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        w0.record()
+        for _ in range(3):
+            gen(whole)
+        w1.record()
+        torch.cuda.synchronize()
+    whole_ms = w0.elapsed_time(w1) / 3
+    audio_s = F * st.hop / sr
+    return dict(B=B, F=F, chunk_ms=round(chunk_ms, 4), host_enqueue_ms=round(1e3 * host / chunks, 4),
+                launches_per_chunk=st.plan.launches_per_chunk, rtf=round(audio_s / (chunk_ms / 1e3), 2),
+                latency_audio_ms=round(1e3 * audio_s, 2), whole_frames=frames, whole_ms=round(whole_ms, 3),
+                whole_rtf=round(frames * st.hop / sr / (whole_ms / 1e3), 2))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--chunks", type=int, default=200)
+    ap.add_argument("--out", default=None, help="also write the rows as DIR/stream_latency.json")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("stream_latency: needs a CUDA device")
+    info = card()
+    print(f"card: {info}")
+    rows = []
+    for name, (cfg, sr) in GENERATORS.items():
+        torch.manual_seed(0)
+        gen = K.Generator(**cfg).cuda().eval()
+        for B in (1, 16, 64):
+            for F in (1, 4, 16):
+                r = dict(generator=name, **measure(gen, sr, B, F, args.chunks))
+                rows.append(r)
+                print(json.dumps(r), flush=True)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "stream_latency.json"), "w") as f:
+            json.dump(dict(card=info, rows=rows), f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
