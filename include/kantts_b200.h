@@ -375,6 +375,26 @@ int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t
 /* ONE launch: rows [0, history) of every window are zeroed for the batch items b with slots[b] != 0 (device uint8 [batch]). */
 int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream);
 
+/* ---- streaming SAM-BERT post-net (PostNet.streamer: decoder rows in, final post-net rows out, chunk by chunk) ---------------
+ * kt_fsmn_fwd_stream: one chunk of MemoryBlockV2 with FsmnEncoderV2's residual fused, seen as a causal depthwise FIR whose
+ * output lags its input by rp = k - 1 - pad_left rows.  x, y and resid are windows placed by `w` (KtStreamWin, c channels):
+ * input rows [-(k-1), rows) of the chunk are read (in_first >= k - 1), output rows [0, rows) are written.  Output row t is
+ * frame row0 + t of the utterance; its tap j reads input row t + j - (k-1), frame row0 + t + j - pad_left.  With
+ * keep(b, a) = (0 <= a < lengths[b]) (lengths: device int32 [batch]) and xm = keep * x:
+ *   y[t] = keep(row0 + t) * (xm[t - rp] + sum_j weight[c][j] * xm[t + j - (k-1)]) + resid[t]      (resid optional)
+ * Frames before 0 and from lengths[b] on read as zeros, so no chunk reads device data on the host.  The taps are summed in
+ * kt_fsmn_fwd's order: a streamed row equals the whole-sequence row bit for bit.  weight [c][k] as in kt_fsmn_fwd. */
+int kt_fsmn_fwd_stream(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths, const float* resid, float* y,
+                       int32_t batch, int32_t rows, int32_t c, int32_t k, int32_t pad_left, int32_t row0, void* stream);
+/* kt_lstm_stream: `rows` steps of a 1-layer unidirectional nn.LSTM (hidden <= 256), one CTA per batch item.
+ *   gx     row t of item b at gx[(b * gx_pitch + t) * 4 * hidden]: x . weight_ih^T + bias_ih + bias_hh (one k = 1 conv)
+ *   whh_t  [hidden][4 * hidden] = weight_hh^T
+ *   state  [batch][2][hidden]: (h, c) before the first step, overwritten with (h, c) after the last (zeros start an utterance)
+ *   h      row t of item b at h[(b * h_pitch + t) * hidden]: the LSTM output.
+ * PyTorch gate order (i, f, g, o); exact fp32. */
+int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t batch, int32_t rows, int32_t hidden,
+                   int32_t gx_pitch, int32_t h_pitch, void* stream);
+
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

@@ -111,6 +111,8 @@ PROTOTYPES = {
     "kt_add3_scale_win": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_stream_advance": [_P, _I, _I, _I, _I, _P],
     "kt_stream_reset": [_P, _I, _I, _P, _I, _P],
+    "kt_fsmn_fwd_stream": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_version": [],

@@ -62,6 +62,9 @@ int fp_insert_plan(const void*, int, const float*, const int*, int, int, int, in
 int fp_insert_fwd(const float*, const float*, const int*, float*, int, int, int, int, int, cudaStream_t);
 int fp_insert_bwd(const float*, const int*, const int*, float*, float*, float*, long long, int, int, int, int, int,
                   cudaStream_t);
+int fsmn_fwd_stream(const KtStreamWin*, const float*, const float*, const int*, const float*, float*, int, int, int, int, int, int,
+                    cudaStream_t);
+int lstm_stream(const float*, const float*, float*, float*, int, int, int, int, int, cudaStream_t);
 }  // namespace kt
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -327,6 +330,14 @@ int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* row
                      int32_t c, void* stream) {
   return kt::fp_insert_bwd(dout, codes, rows, d_text_hid, d_fp_enc, partials, partial_floats, batch, length, t_cap, t_ins, c,
                            ST(stream));
+}
+int kt_fsmn_fwd_stream(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths, const float* resid, float* y,
+                       int32_t batch, int32_t rows, int32_t c, int32_t k, int32_t pad_left, int32_t row0, void* stream) {
+  return kt::fsmn_fwd_stream(w, x, weight, lengths, resid, y, batch, rows, c, k, pad_left, row0, ST(stream));
+}
+int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t batch, int32_t rows, int32_t hidden,
+                   int32_t gx_pitch, int32_t h_pitch, void* stream) {
+  return kt::lstm_stream(gx, whh_t, state, h, batch, rows, hidden, gx_pitch, h_pitch, ST(stream));
 }
 
 }  // extern "C"

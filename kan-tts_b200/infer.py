@@ -4,9 +4,14 @@ symbols -> SAM-BERT free-running decode -> mel stays on the device -> HiFi-GAN g
 Reference flow: kantts/bin/infer_sambert.py:205-224 writes ``<utt>_mel.npy`` (the post-net mel, one utterance per
 forward because its decoder masks only support batch 1), kantts/bin/infer_hifigan.py:112-124 loads it, transposes to
 (1, C, T) and runs ``Generator`` with weight norm removed.  Here a whole batch of utterances goes through both models
-in one call; every utterance is cut at its own predicted length (frames x product of the up-sampling scales)."""
+in one call; every utterance is cut at its own predicted length (frames x product of the up-sampling scales).
+
+``stream_synthesize`` gives the same waveforms chunk by chunk while the decoder runs: decoder steps -> streamed post-net
+(PostNet.streamer) -> streamed causal vocoder (Generator.streamer)."""
 import numpy as np
 import torch
+
+from .hifigan import StreamPlan
 
 
 @torch.no_grad()
@@ -23,3 +28,82 @@ def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, 
     hop = int(np.prod(generator.upsample_scales))
     wavs = [wav[b, 0, : int(frames[b]) * hop] for b in range(wav.shape[0])]
     return wavs, res
+
+
+def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps=4):
+    """Streaming ``synthesize``: the encoder, the variance adaptor and the decoder memory run now, then iterating the
+    returned TtsStream decodes ``chunk_steps`` decoder steps at a time and yields their audio as soon as the post-net rows
+    are final.  The generator must be causal and without NSF.  For every slot b, the yielded chunks concatenated and cut
+    at ``lengths[b]`` are ``synthesize(...)[0][b]``."""
+    if sambert.training or generator.training:
+        raise RuntimeError("stream_synthesize() expects both models in eval() mode")
+    StreamPlan(generator)                                          # rejects non-causal and NSF generators
+    num_mels = sambert.mel_postnet.num_mels
+    if generator.conv_pre.conv1d.spec.c_in != num_mels:
+        raise ValueError(f"stream_synthesize(): the acoustic model makes {num_mels} mel channels, the generator takes "
+                         f"{generator.conv_pre.conv1d.spec.c_in}")
+    chunk_steps = int(chunk_steps)
+    if chunk_steps < 1:
+        raise ValueError(f"stream_synthesize(): chunk_steps must be >= 1, got {chunk_steps}")
+    return TtsStream(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps)
+
+
+class TtsStream:
+    """The audio of one batch of utterances, chunk by chunk (made by ``stream_synthesize``).
+
+    ``lengths``: per-slot sample counts, ``LR_length_rounded[b] * hop`` (read on the host once, before decoding).
+    Iterating yields ``(start_sample, wav)``, ``wav`` (B, 1, n) on the device, n > 0; slot b's audio ends at lengths[b] and
+    is padding after that.  From the first chunk to the last no device data is read on the host.  A stream is iterated
+    once."""
+
+    def __init__(self, sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps):
+        self.sambert, self.chunk_steps = sambert, chunk_steps
+        dec = sambert.mel_decoder
+        self.r, self.d_mel = dec.r, dec.d_mel
+        with torch.no_grad():
+            self._front = f = sambert.front_half(inputs_ling, inputs_emotion, inputs_speaker, input_lengths)
+        self.batch = B = f["memory"].shape[0]
+        self.hop = int(np.prod(generator.upsample_scales))
+        frames = f["lr_len"]
+        self.lengths = [int(n) * self.hop for n in frames.cpu()]
+        self.max_frames = F = self.r * chunk_steps
+        self._post = sambert.mel_postnet.streamer(B, F, frames)
+        self._voc = generator.streamer(batch=B, max_frames=F)
+        # capture the vocoder's graph now (a capture synchronises the device) rather than in the middle of the stream
+        self._voc.push(torch.zeros(B, self.d_mel, F, device=frames.device))
+        self._voc.reset(range(B))
+        self._used = False
+
+    def _vocode(self, rows, start):
+        """rows (B, n, num_mels) of final post-net output -> [(start sample, wav)] in pieces of at most max_frames frames."""
+        out = []
+        for piece in torch.split(rows, self.max_frames, dim=1):
+            if piece.shape[1]:
+                out.append((start, self._voc.push(piece.transpose(1, 2))))
+                start += piece.shape[1] * self.hop
+        return out, start
+
+    def __iter__(self):
+        if self._used:
+            raise RuntimeError("a TtsStream is iterated once")
+        self._used = True
+        f = self._front
+        steps, B, start, row = f["memory"].shape[1], self.batch, 0, 0
+        outs = []
+        with torch.no_grad():
+            for s, (out, _, _) in enumerate(self.sambert.mel_decoder.infer_steps(f["memory"], f["x_band_width"],
+                                                                                f["x_band_width"])):
+                outs.append(out)
+                last = s == steps - 1
+                if len(outs) < self.chunk_steps and not last:
+                    continue
+                dec = torch.cat(outs, 1).view(B, -1, self.d_mel)                 # de-LFR: r frames per step
+                outs = []
+                frames = torch.arange(row, row + dec.shape[1], device=dec.device)
+                dec = dec.masked_fill((frames[None, :] >= f["lr_len"][:, None]).unsqueeze(-1), 0)
+                row += dec.shape[1]
+                rows = self._post.push(dec)
+                if last:
+                    rows = torch.cat([rows, self._post.finish()], 1)
+                chunks, start = self._vocode(rows, start)
+                yield from chunks

@@ -21,6 +21,8 @@ kernels, and the splice of the predicted or labelled pauses into the text encodi
 gather each way (kt_fp_insert_*).  Not built: MAS alignment (``MAS: True``) and the speaker-encoder (``SE``)
 variant -- the shipped sambert_24k.yaml and sambert_fp_8k.yaml disable both.
 """
+import ctypes
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -28,7 +30,7 @@ import torch.nn.functional as F
 
 from . import ops
 from . import sambert_ops as sops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KtStreamWin, KtWindow
 
 
 def get_mask_from_lengths(lengths, max_len=None):
@@ -704,21 +706,27 @@ class MelPNCADecoder(nn.Module):
             config["decoder_ffn_inner_dim"], config["decoder_dropout"], config["decoder_attention_dropout"],
             config["decoder_relu_dropout"], self.d_mel * r)
 
-    def forward(self, memory, x_band_width, h_band_width, target=None, mask=None, return_attns=False):
+    def infer_steps(self, memory, x_band_width, h_band_width, mask=None, return_attns=False):
+        """Free-running decoding, one step at a time (kantts_sambert.py:567-612): yields (out, attn_x, attn_h) of every LFR
+        step, out (B, 1, r * d_mel); each step's last d_mel outputs feed the next step.  Step s depends only on earlier
+        steps, so a consumer can use a step's rows as soon as it is yielded."""
         go_frame = torch.zeros((memory.size(0), 1, self.d_mel), device=memory.device)
         self.mel_dec.reset_state()
+        inp = go_frame
+        for step in range(memory.size(1)):
+            out, ax, ah = self.mel_dec.infer(step, inp, memory, x_band_width, h_band_width, mask=mask,
+                                             return_attns=return_attns)
+            inp = out[:, :, -self.d_mel:]
+            yield out, ax, ah
+
+    def forward(self, memory, x_band_width, h_band_width, target=None, mask=None, return_attns=False):
         if target is None:
-            # free-running decoding (kantts_sambert.py:567-612): each step's last d_mel outputs feed the next step.
             # Attention rows come back at the full key length (masked keys are exact zeros), which is what the
             # reference builds by zero-padding every step's row before concatenating.
             outs = []
             ax_steps = [[] for _ in range(self.nb_layers)]
             ah_steps = [[] for _ in range(self.nb_layers)]
-            inp = go_frame
-            for step in range(memory.size(1)):
-                out, ax, ah = self.mel_dec.infer(step, inp, memory, x_band_width, h_band_width, mask=mask,
-                                                 return_attns=return_attns)
-                inp = out[:, :, -self.d_mel:]
+            for out, ax, ah in self.infer_steps(memory, x_band_width, h_band_width, mask, return_attns):
                 outs.append(out)
                 for i, (a, b) in enumerate(zip(ax, ah)):
                     ax_steps[i].append(a)
@@ -727,6 +735,8 @@ class MelPNCADecoder(nn.Module):
             if not return_attns:
                 return dec, [], []
             return dec, [torch.cat(a, dim=1) for a in ax_steps], [torch.cat(a, dim=1) for a in ah_steps]
+        go_frame = torch.zeros((memory.size(0), 1, self.d_mel), device=memory.device)
+        self.mel_dec.reset_state()
         inp = torch.cat([go_frame, target[:, self.r - 1:: self.r, :]], dim=1)[:, :-1, :]
         return self.mel_dec(inp, memory, x_band_width, h_band_width, mask=mask, return_attns=return_attns)
 
@@ -747,6 +757,217 @@ class PostNet(nn.Module):
     def forward(self, x, mask=None, resid=None):
         h, _ = self.lstm(self.fsmn(x, mask))
         return self.fc(h, resid=resid)
+
+    def streamer(self, batch, max_frames, lengths):
+        """-> a PostNetStreamer that runs this (eval-mode) post-net chunk by chunk over ``batch`` utterances of ``lengths``
+        (device tensor (batch,)) frames, at most ``max_frames`` decoder rows per chunk."""
+        return PostNetStreamer(self, batch, max_frames, lengths)
+
+
+class PostNetStreamPlan:
+    """What a PostNetStreamer runs per chunk, as data (no device needed).  The post-net is causal except for the right
+    padding of its memory blocks: output frame t is final once decoder row t + delay exists.
+      layers              per FSMN layer: {lp, rp, kernel, lag}: the memory block's left / right padding and filter size, and
+                          how many rows the layer's input lags the decoder rows (the sum of rp over the layers before it)
+      delay               D = the sum of rp: the post-net output of a chunk is its decoder rows shifted back by D rows
+      windows             one entry per tensor of a chunk: {name, channels, history}; a memory block's input keeps k - 1
+                          rows, a residual read lagging its tensor by n rows keeps n, the others keep none
+      steps               ("conv", module, input, output, residual or None) | ("fsmn", layer, input, output, residual or
+                          None) | ("lstm", input, output), in launch order; the LSTM's input projection is the conv step
+                          whose module is the post-net's nn.LSTM
+      launches_per_chunk  library calls of a steady chunk: one per step and one window advance; the copy of the decoder rows
+                          into their window and the output mask are not counted"""
+
+    def __init__(self, postnet):
+        if postnet.training:
+            raise ValueError("streaming runs a post-net in eval() mode")
+        fsmn = postnet.fsmn
+        self.windows, self.layers, self.steps = [], [], []
+        index = {}
+
+        def tensor(name, channels):
+            index[name] = len(self.windows)
+            self.windows.append(dict(name=name, channels=channels, history=0))
+            return name
+
+        def read(name, history):
+            w = self.windows[index[name]]
+            w["history"] = max(w["history"], history)
+
+        x, lag = tensor("dec", postnet.num_mels), 0
+        mid = tensor("mid", fsmn.ffn_inner_dim)
+        units = fsmn.num_memory_units
+        for i, (ffn, mb) in enumerate(zip(fsmn.ffn_lst, fsmn.memory_block_lst)):
+            k = mb.conv_dw.kernel_size[0]
+            if mb.rp < 0:
+                raise ValueError(f"streaming needs rp >= 0 in every memory block: layer {i} has shift > (filter_size - 1) / 2 "
+                                 f"(lp {mb.lp}, rp {mb.rp})")
+            self.layers.append(dict(lp=mb.lp, rp=mb.rp, kernel=k, lag=lag))
+            ctx = tensor(f"ctx{i}", units)
+            read(ctx, k - 1)
+            resid = x if ffn.w_1.in_channels == units else None
+            if resid is not None:
+                read(resid, mb.rp)
+            out = tensor(f"x{i + 1}", units)
+            self.steps += [("conv", ffn.w_1, x, mid, None), ("conv", ffn.w_2, mid, ctx, None), ("fsmn", i, ctx, out, resid)]
+            x, lag = out, lag + mb.rp
+        self.delay = lag
+        read("dec", self.delay)                            # the output Linear's residual: the decoder rows D rows back
+        gates = tensor("gates", 4 * postnet.lstm.hidden_size)
+        h = tensor("h", postnet.lstm.hidden_size)
+        self.steps += [("conv", postnet.lstm, x, gates, None), ("lstm", gates, h),
+                       ("conv", postnet.fc, h, tensor("out", postnet.num_mels), "dec")]
+        self.launches_per_chunk = len(self.steps) + any(w["history"] for w in self.windows)
+
+
+class PostNetStreamer:
+    """Chunk-by-chunk PostNet (PostNet.streamer) over decoder rows that arrive step by step.
+
+    ``push(dec_rows)`` takes the next (B, f, num_mels) decoder rows of every slot (de-LFR'd and masked, 1 <= f <=
+    max_frames) and returns the post-net output rows ``fc(lstm(fsmn(x))) + x``, masked beyond each slot's length, that have
+    become final: f rows in the steady state, fewer while the first ``delay`` rows are held back.  ``finish()`` pushes
+    ``delay`` all-padding rows and returns the rest; the rows returned in order are then the whole-sequence post-net output.
+    ``reset(lengths=None)`` starts a new batch.  No call reads device data on the host.
+
+    Each tensor a layer reads before the chunk lives in a persistent window of [history | chunk] rows per slot (see
+    PostNetStreamPlan); kt_fsmn_fwd_stream masks by each row's frame index against the slot lengths kept on the device, and
+    kt_lstm_stream carries the LSTM state.  The weights are prepared once, when the streamer is created."""
+
+    def __init__(self, postnet, batch, max_frames, lengths):
+        self.plan = plan = PostNetStreamPlan(postnet)
+        batch, max_frames = int(batch), int(max_frames)
+        if batch < 1 or max_frames < 1:
+            raise ValueError(f"streamer: batch ({batch}) and max_frames ({max_frames}) must be >= 1")
+        dev = next(postnet.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("kantts_b200: the post-net streamer runs on a CUDA device (no CPU fallback)")
+        self.batch, self.max_frames, self.delay, self.device = batch, max_frames, plan.delay, dev
+        self.num_mels, self.hidden = postnet.num_mels, postnet.lstm.hidden_size
+        self._hist = {w["name"]: w["history"] for w in plan.windows}
+        self._buf = {w["name"]: torch.zeros(batch, w["history"] + max_frames, w["channels"], device=dev) for w in plan.windows}
+        kept = [w for w in plan.windows if w["history"] > 0]
+        table = (KtWindow * len(kept))(*[KtWindow(base=self._buf[w["name"]].data_ptr(), pitch=self._buf[w["name"]].shape[1],
+                                                  channels=w["channels"], history=w["history"], rows_per_frame=1) for w in kept])
+        self._table = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(dev)
+        self._ntable, self._max_c = len(kept), max([w["channels"] for w in kept], default=1)
+        self._slots = torch.ones(batch, dtype=torch.uint8, device=dev)
+        self._state = torch.zeros(batch, 2, self.hidden, device=dev)
+        self._zeros = torch.zeros(batch, max_frames, self.num_mels, device=dev)
+        self._len = torch.empty(batch, dtype=torch.int32, device=dev)
+        self._weights = {}
+        self._ffn = {m for ffn in postnet.fsmn.ffn_lst for m in (ffn.w_1, ffn.w_2)}
+        with torch.no_grad(), torch.cuda.device(dev):
+            for st in plan.steps:
+                if st[0] == "conv":
+                    mod = st[1]
+                    if isinstance(mod, nn.LSTM):             # x . W_ih^T + b_ih + b_hh as one k = 1 conv
+                        spec = ops.ConvSpec(c_in=mod.input_size, c_out=4 * mod.hidden_size, kernel=1)
+                        w, b = mod.weight_ih_l0.unsqueeze(-1), mod.bias_ih_l0 + mod.bias_hh_l0
+                    else:
+                        spec, w, b = mod.spec, mod.weight, mod.bias
+                    pw = ops.prepare_weight(ops.PreparedWeight(), spec, w.detach().clone(), None)
+                    self._weights[mod] = (spec, pw, None if b is None else b.detach().clone())
+                elif st[0] == "fsmn":
+                    mb = postnet.fsmn.memory_block_lst[st[1]]
+                    self._weights[st[1]] = mb.conv_dw.weight.detach().reshape(mb.conv_dw.out_channels, -1).clone()
+            self._whh_t = postnet.lstm.weight_hh_l0.detach().t().contiguous()
+            self.reset(lengths)
+
+    def _win(self, src, dst, resid, in_skip=0, res_first=None):
+        b = self._buf
+        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=self._hist[src] + in_skip, out_pitch=b[dst].shape[1],
+                        out_first=self._hist[dst])
+        if resid is not None:
+            w.res_pitch = b[resid].shape[1]
+            w.res_first = self._hist[resid] if res_first is None else res_first
+        return w
+
+    def _chunk(self, f):
+        """Every launch of one chunk of f decoder rows (already in the "dec" window) -> the final output rows."""
+        from ._lib import load, check, ptr, stream_ptr
+        lib, b, B, a = load(), self._buf, self.batch, self._rows
+        first = a - self.delay                      # frame of the chunk's first output row
+        skip = max(0, -first)                       # output rows before frame 0 are not rows of the utterance
+        n = f - skip
+        for st in self.plan.steps:
+            kind = st[0]
+            if kind == "fsmn":
+                _, i, src, dst, resid = st
+                layer = self.plan.layers[i]
+                k = layer["kernel"]
+                win = self._win(src, dst, resid, res_first=None if resid is None else self._hist[resid] - layer["rp"])
+                check(lib.kt_fsmn_fwd_stream(ctypes.byref(win), ptr(b[src]), ptr(self._weights[i]), ptr(self._len, True),
+                                             ptr(None if resid is None else b[resid]), ptr(b[dst]), B, f, b[src].shape[2], k,
+                                             layer["lp"], a - layer["lag"] - layer["rp"], stream_ptr()), "kt_fsmn_fwd_stream")
+                ops._count()
+            elif kind == "conv" and st[1] in self._ffn:     # the FSMN feed-forward convs over the whole chunk
+                _, mod, src, dst, _ = st
+                spec, pw, bias = self._weights[mod]
+                ops.stream_conv(spec, pw, bias, b[src], b[dst], f, self._win(src, dst, None))
+            elif n <= 0:
+                continue                            # nothing of the utterance has reached the LSTM yet
+            elif kind == "lstm":
+                _, src, dst = st
+                check(lib.kt_lstm_stream(ptr(b[src]), ptr(self._whh_t), ptr(self._state), ptr(b[dst]), B, n, self.hidden,
+                                         b[src].shape[1], b[dst].shape[1], stream_ptr()), "kt_lstm_stream")
+                ops._count()
+            else:
+                _, mod, src, dst, resid = st
+                spec, pw, bias = self._weights[mod]
+                if resid is None:                   # the LSTM input projection: the chunk's rows from frame 0 on
+                    ops.stream_conv(spec, pw, bias, b[src], b[dst], n, self._win(src, dst, None, in_skip=skip))
+                else:                               # output Linear + the decoder rows D rows back
+                    win = self._win(src, dst, resid, res_first=self._hist[resid] - self.delay + skip)
+                    ops.stream_conv(spec, pw, bias, b[src], b[dst], n, win, b[resid])
+        if self._ntable:
+            check(lib.kt_stream_advance(ptr(self._table, True), self._ntable, B, f, self._max_c, stream_ptr()),
+                  "kt_stream_advance")
+            ops._count()
+        self._rows += f
+        if n <= 0:
+            return b["out"][:, :0].clone()
+        frames = torch.arange(first + skip, first + f, device=self.device)
+        pad = frames[None, :] >= self._len[:, None]
+        return b["out"][:, :n].masked_fill(pad.unsqueeze(-1), 0)
+
+    def push(self, dec_rows):
+        """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final."""
+        if dec_rows.dim() != 3 or dec_rows.shape[0] != self.batch or dec_rows.shape[2] != self.num_mels:
+            raise ValueError(f"push: expected ({self.batch}, f, {self.num_mels}) decoder rows, got {tuple(dec_rows.shape)}")
+        f = dec_rows.shape[1]
+        if not 1 <= f <= self.max_frames:
+            raise ValueError(f"push: a chunk holds 1 to {self.max_frames} rows, got {f}")
+        if dec_rows.device != self.device:
+            raise ValueError(f"push: the rows are on {dec_rows.device}, the streamer on {self.device}")
+        with torch.no_grad(), torch.cuda.device(self.device):
+            h = self._hist["dec"]
+            self._buf["dec"][:, h:h + f].copy_(dec_rows)
+            return self._chunk(f)
+
+    def finish(self):
+        """Push ``delay`` all-padding rows (the whole-sequence zero padding) -> the remaining (B, n, num_mels) output rows."""
+        outs, left = [], self.delay
+        while left > 0:
+            f = min(left, self.max_frames)
+            outs.append(self.push(self._zeros[:, :f]))
+            left -= f
+        return torch.cat(outs, 1) if outs else self._zeros[:, :0].clone()
+
+    def reset(self, lengths=None):
+        """Start a new batch: the carried windows and LSTM state return to zeros; ``lengths`` (device tensor (batch,)),
+        when given, replaces the slots' frame counts."""
+        from ._lib import load, check, ptr, stream_ptr
+        with torch.no_grad(), torch.cuda.device(self.device):
+            if lengths is not None:
+                if lengths.shape != (self.batch,):
+                    raise ValueError(f"reset: expected ({self.batch},) lengths, got {tuple(lengths.shape)}")
+                self._len.copy_(lengths)
+            if self._ntable:
+                check(load().kt_stream_reset(ptr(self._table, True), self._ntable, self.batch, ptr(self._slots, True),
+                                             self._max_c, stream_ptr()), "kt_stream_reset")
+                ops._count()
+            self._state.zero_()
+        self._rows = 0
 
 
 class FP_Predictor(nn.Module):
@@ -813,9 +1034,11 @@ class KanTtsSAMBERT(nn.Module):
         r = self.mel_decoder.r
         return get_mask_from_lengths((lengths + r - 1) // r, max_len=max_len // r)
 
-    def forward(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
-                mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, attn_priors=None,
-                fp_label=None):
+    def front_half(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
+                   mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, fp_label=None):
+        """Everything of ``forward`` before the decoder: text encoder, filled-pause insertion (``FP``), variance adaptor,
+        the decoder memory and the band width of its attentions.  -> dict of the intermediate results ``forward`` and
+        ``infer.stream_synthesize`` continue from."""
         batch_size = inputs_ling.size(0)
         r = self.mel_decoder.r
         input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
@@ -849,9 +1072,20 @@ class KanTtsSAMBERT(nn.Module):
             x_band_width = int(duration_targets.float().masked_fill(inter_masks, 0).max() / r + 0.5)
         else:
             x_band_width = int((torch.exp(log_dur_p) - 1).max() / r + 0.5)
-        h_band_width = x_band_width
-        dec, ax_lst, ah_lst = self.mel_decoder(memory, x_band_width, h_band_width, target=mel_targets,
-                                               mask=lfr_masks, return_attns=True)
+        return dict(enc_attns=enc_attns, fp_p=fp_p, inter_lengths=inter_lengths, output_masks=output_masks,
+                    lfr_masks=lfr_masks, lr_text=lr_text, lr_emo=lr_emo, lr_spk=lr_spk, lr_len=lr_len, log_dur_p=log_dur_p,
+                    pitch_p=pitch_p, energy_p=energy_p, memory=memory, x_band_width=x_band_width)
+
+    def forward(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
+                mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, attn_priors=None,
+                fp_label=None):
+        batch_size = inputs_ling.size(0)
+        f = self.front_half(inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths, mel_targets,
+                            duration_targets, pitch_targets, energy_targets, fp_label)
+        output_masks, lr_len, inter_lengths = f["output_masks"], f["lr_len"], f["inter_lengths"]
+        x_band_width = h_band_width = f["x_band_width"]
+        dec, ax_lst, ah_lst = self.mel_decoder(f["memory"], x_band_width, h_band_width, target=mel_targets,
+                                               mask=f["lfr_masks"], return_attns=True)
         dec_outputs = dec.contiguous().view(batch_size, -1, self.mel_decoder.d_mel)
         if output_masks is not None:
             dec_outputs = dec_outputs.masked_fill(output_masks.unsqueeze(-1), 0)
@@ -859,13 +1093,14 @@ class KanTtsSAMBERT(nn.Module):
         if output_masks is not None:
             postnet_outputs = postnet_outputs.masked_fill(output_masks.unsqueeze(-1), 0)
         return {
-            "x_band_width": x_band_width, "h_band_width": h_band_width, "enc_slf_attn_lst": enc_attns,
+            "x_band_width": x_band_width, "h_band_width": h_band_width, "enc_slf_attn_lst": f["enc_attns"],
             "pnca_x_attn_lst": ax_lst, "pnca_h_attn_lst": ah_lst, "dec_outputs": dec_outputs,
             "postnet_outputs": postnet_outputs, "LR_length_rounded": lr_len,
-            "log_duration_predictions": log_dur_p, "pitch_predictions": pitch_p, "energy_predictions": energy_p,
+            "log_duration_predictions": f["log_dur_p"], "pitch_predictions": f["pitch_p"],
+            "energy_predictions": f["energy_p"],
             "duration_targets": duration_targets, "pitch_targets": pitch_targets, "energy_targets": energy_targets,
-            "fp_predictions": fp_p, "valid_inter_lengths": inter_lengths,
-            "LR_text_outputs": lr_text, "LR_emo_outputs": lr_emo, "LR_spk_outputs": lr_spk,
+            "fp_predictions": f["fp_p"], "valid_inter_lengths": inter_lengths,
+            "LR_text_outputs": f["lr_text"], "LR_emo_outputs": f["lr_emo"], "LR_spk_outputs": f["lr_spk"],
         }
 
 
