@@ -14,6 +14,7 @@ of GPU budget: tests/test_gpu_pipeline.py is opt-in).  Out of scope (SURVEY.md s
 """
 import copy
 import math
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -22,7 +23,8 @@ import torch.nn.functional as F
 
 from . import ops
 from . import _lib
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtStreamWin, KtWindow, check, ptr, stream_ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, check, ptr, stream_ptr
+from .stream import Windows, WindowTable, own_weight
 
 # --------------------------------------------------------------------------------------------
 # parameter holders (names / shapes == the reference's weight_norm / spectral_norm wrapped convs)
@@ -469,6 +471,13 @@ def stream_history(spec):
     return -(-(spec.kernel - 1) * spec.dilation // spec.upsample)
 
 
+# The steps of a StreamPlan, over windows named by the plan: a conv of ``conv`` (a layer's conv1d or deconv) adding window
+# ``resid`` (or None), on side stream ``side`` of the parallel ResBlocks (None: the current stream); sin(x) + x; a mean.
+ConvStep = namedtuple("ConvStep", "conv src dst resid side")
+SinStep = namedtuple("SinStep", "src dst")
+MeanStep = namedtuple("MeanStep", "srcs dst scale")
+
+
 class StreamPlan:
     """What a GeneratorStreamer runs per chunk, as data (no device needed):
       windows             one entry per tensor of the chunk: {name, channels, rows_per_frame, history}; a tensor read by a
@@ -476,8 +485,7 @@ class StreamPlan:
       layer_history       {layer name (as in named_modules): input rows before the chunk it reads}
       launches_per_chunk  library calls of a full chunk: one per conv (one kernel each on the tensor-core path), one per
                           sin-add and per mean, one window advance; the mel chunk's copy into its window is not counted
-      steps               ("conv", side stream or None, _NormedConv, input, output, residual or None) | ("sin", input, output)
-                          | ("mean", inputs, output, scale), in launch order"""
+      steps               ConvStep | SinStep | MeanStep records, in launch order"""
 
     def __init__(self, gen):
         if gen.nsf_enable:
@@ -488,52 +496,46 @@ class StreamPlan:
         if gen.training:
             raise ValueError("streaming runs a generator in eval() mode")
         names = {m: n for n, m in gen.named_modules()}
-        self.windows, self.layer_history, self.steps = [], {}, []
-        index = {}
-
-        def tensor(name, channels, rate):
-            index[name] = len(self.windows)
-            self.windows.append(dict(name=name, channels=channels, rows_per_frame=rate, history=0))
-            return name
+        table = WindowTable()
+        self.windows, self.layer_history, self.steps = table.windows, {}, []
 
         def conv(mod, src, dst, resid=None, side=None):
             nc = mod.conv1d if hasattr(mod, "conv1d") else mod.deconv
             h = stream_history(nc.spec)
             self.layer_history[names[mod]] = h
-            w = self.windows[index[src]]
-            w["history"] = max(w["history"], h)
-            self.steps.append(("conv", side, nc, src, dst, resid))
+            table.read(src, h)
+            self.steps.append(ConvStep(nc, src, dst, resid, side))
 
         nk, ch, rate = gen.num_kernels, gen.conv_pre.conv1d.spec.c_out, 1
-        mel = tensor("mel", gen.conv_pre.conv1d.spec.c_in, 1)
-        x = tensor("x", ch, 1)
+        mel = table.add("mel", gen.conv_pre.conv1d.spec.c_in)
+        x = table.add("x", ch)
         conv(gen.conv_pre, mel, x)
         for i in range(gen.num_upsamples):
             cin, s = ch >> i, gen.upsample_scales[i]
             cout = cin // 2
-            sx = tensor(f"sin{i}", cin, rate)
-            self.steps.append(("sin", x, sx))
+            sx = table.add(f"sin{i}", cin, rate)
+            self.steps.append(SinStep(x, sx))
             rate *= s
-            rep = tensor(f"rep{i}", cout, rate)
+            rep = table.add(f"rep{i}", cout, rate)
             conv(gen.repeat_upsamples[i][2], sx, rep)
-            up = tensor(f"up{i}", cout, rate)
+            up = table.add(f"up{i}", cout, rate)
             conv(gen.transpose_upsamples[i][1], sx, up, resid=rep)
             outs = []
             for j in range(nk):
                 rb, xin = gen.conv_blocks[i * nk + j], up
                 side = j if nk > 1 else None
                 for p, (c1, c2) in enumerate(zip(rb.convs1, rb.convs2)):
-                    h = tensor(f"rb{i}.{j}.h{p}", cout, rate)
+                    h = table.add(f"rb{i}.{j}.h{p}", cout, rate)
                     conv(c1, xin, h, side=side)
-                    xo = tensor(f"rb{i}.{j}.x{p + 1}", cout, rate)
+                    xo = table.add(f"rb{i}.{j}.x{p + 1}", cout, rate)
                     conv(c2, h, xo, resid=xin, side=side)
                     xin = xo
                 outs.append(xin)
-            x = tensor(f"mean{i}", cout, rate)
-            self.steps.append(("mean", outs, x, 1.0 / nk))
-        conv(gen.conv_post, x, tensor("wav", 1, rate))
+            x = table.add(f"mean{i}", cout, rate)
+            self.steps.append(MeanStep(outs, x, 1.0 / nk))
+        conv(gen.conv_post, x, table.add("wav", 1, rate))
         self.hop = rate
-        self.launches_per_chunk = len(self.steps) + any(w["history"] for w in self.windows)
+        self.launches_per_chunk = table.launches_per_chunk(len(self.steps))
 
 
 class GeneratorStreamer:
@@ -544,139 +546,74 @@ class GeneratorStreamer:
     generator's forward on the whole mel.  Each batch slot is an independent stream; ``reset(slots)`` starts new utterances
     in the given slots.  ``push`` never waits for the device.
 
-    Every tensor a causal layer reads lives in a persistent window of [history | chunk] rows per slot: the producer writes
-    the chunk straight into its consumer's window, and one launch per chunk (kt_stream_advance) moves the last rows of
-    every window into its history.  A full-size chunk replays a CUDA graph, captured on the first one; a shorter chunk
-    runs the same kernels eagerly.
+    Every tensor a causal layer reads lives in a window (stream.py) that its producer writes straight into.  A full-size
+    chunk replays a CUDA graph; a shorter chunk runs the same kernels eagerly.
 
     The weights are prepared once, when the streamer is created: a generator whose parameters change later needs a new
-    streamer.  Creating one also runs a chunk of zeros through every kernel (then clears the state), so that the graph
-    capture finds every kernel loaded."""
+    streamer.  Creating one also runs a chunk of zeros through every kernel, so that every kernel is loaded, captures the
+    full-size chunk's graph, then clears the state; the capture synchronises the device once."""
 
     def __init__(self, gen, batch, max_frames):
         self.plan = plan = StreamPlan(gen)
-        batch, max_frames = int(batch), int(max_frames)
-        if batch < 1 or max_frames < 1:
-            raise ValueError(f"streamer: batch ({batch}) and max_frames ({max_frames}) must be >= 1")
-        dev = next(gen.parameters()).device
-        if dev.type != "cuda":
-            raise RuntimeError("kantts_b200: the streamer runs on a CUDA device (no CPU fallback)")
-        self.batch, self.max_frames, self.hop, self.device = batch, max_frames, plan.hop, dev
+        self._win = win = Windows(plan.windows, batch, max_frames, next(gen.parameters()).device, "streamer")
+        self.batch, self.max_frames, self.hop, self.device = win.batch, win.max_frames, plan.hop, win.device
         self.in_channels = plan.windows[0]["channels"]
-        self._buf = {w["name"]: torch.zeros(batch, w["history"] + max_frames * w["rows_per_frame"], w["channels"], device=dev)
-                     for w in plan.windows}
-        self._hist = {w["name"]: w["history"] for w in plan.windows}
-        self._rate = {w["name"]: w["rows_per_frame"] for w in plan.windows}
-        kept = [w for w in plan.windows if w["history"] > 0]
-        table = (KtWindow * len(kept))(*[KtWindow(base=self._buf[w["name"]].data_ptr(), pitch=self._buf[w["name"]].shape[1],
-                                                  channels=w["channels"], history=w["history"],
-                                                  rows_per_frame=w["rows_per_frame"]) for w in kept])
-        self._table = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(dev)
-        self._ntable, self._max_c = len(kept), max([w["channels"] for w in kept], default=1)
-        self._slots = torch.ones(batch, dtype=torch.uint8, device=dev)
-        self._wins = [self._win(*st[3:]) if st[0] == "conv" else None for st in plan.steps]
-        self._side = [torch.cuda.Stream(device=dev) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
-        # weights: own prepared copies (never the module's cache), biases copied
-        self._weights = {}
-        with torch.no_grad(), torch.cuda.device(dev):
-            for st in plan.steps:
-                if st[0] == "conv" and st[2] not in self._weights:
-                    nc = st[2]
-                    v, g = nc.effective_weight()
-                    pw = ops.prepare_weight(ops.PreparedWeight(), nc.spec, v.detach().clone(),
-                                            None if g is None else g.detach().clone())
-                    self._weights[nc] = (pw, None if nc.bias is None else nc.bias.detach().clone())
-            self._graph = None
-            self._run(max_frames)                    # warm-up: every kernel and weight image of a full chunk
-            self._reset_selected()
-
-    # -- per chunk ----------------------------------------------------------------------------------------------------
-    def _win(self, src, dst, resid):
-        b = self._buf
-        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=self._hist[src], out_pitch=b[dst].shape[1],
-                        out_first=self._hist[dst])
-        if resid is not None:
-            w.res_pitch, w.res_first = b[resid].shape[1], self._hist[resid]
-        return w
+        self._places = [win.place(st.src, st.dst, st.resid) if type(st) is ConvStep else None for st in plan.steps]
+        self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
+        with torch.no_grad(), torch.cuda.device(self.device):
+            self._weights = {st.conv: own_weight(st.conv.spec, *st.conv.effective_weight(), st.conv.bias)
+                             for st in plan.steps if type(st) is ConvStep}
+            self._run(self.max_frames)               # warm-up: every kernel and weight image of a full chunk
+            self._graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self._graph):
+                self._run(self.max_frames)
+            win.reset()
 
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
-        lib, b, B = _lib.load(), self._buf, self.batch
+        win = self._win
+        lib, b, B = _lib.load(), win.buf, self.batch
         cur = torch.cuda.current_stream()
         forked = False
-        for st, win in zip(self.plan.steps, self._wins):
-            side = st[1] if st[0] == "conv" else None
-            if side is not None and not forked:
+        for st, place in zip(self.plan.steps, self._places):
+            side = st.side if type(st) is ConvStep else None
+            if (side is not None) != forked:               # fork the side streams off the current one, or join them
+                forked = side is not None
                 for s in self._side:
-                    s.wait_stream(cur)
-                forked = True
-            elif side is None and forked:
-                for s in self._side:
-                    cur.wait_stream(s)
-                forked = False
-            if st[0] == "conv":
-                _, _, nc, src, dst, resid = st
-                pw, bias = self._weights[nc]
+                    s.wait_stream(cur) if forked else cur.wait_stream(s)
+            if type(st) is ConvStep:
+                pw, bias = self._weights[st.conv]
                 with torch.cuda.stream(self._side[side] if side is not None else cur):
-                    ops.stream_conv(nc.spec, pw, bias, b[src], b[dst], f * self._rate[src], win,
-                                    None if resid is None else b[resid])
-            elif st[0] == "sin":
-                _, src, dst = st
-                rows, c = f * self._rate[src], b[src].shape[2]
-                check(lib.kt_sinadd_fwd_win(ptr(b[src]), ptr(b[dst]), B, rows, c, b[src].shape[1], b[dst].shape[1],
-                                            self._hist[dst], stream_ptr()), "kt_sinadd_fwd_win")
+                    ops.stream_conv(st.conv.spec, pw, bias, b[st.src], b[st.dst], f * win.rate[st.src], place,
+                                    None if st.resid is None else b[st.resid])
+            elif type(st) is SinStep:
+                src, dst = b[st.src], b[st.dst]
+                check(lib.kt_sinadd_fwd_win(ptr(src), ptr(dst), B, f * win.rate[st.src], src.shape[2], src.shape[1],
+                                            dst.shape[1], win.first[st.dst], stream_ptr()), "kt_sinadd_fwd_win")
                 ops._count()
             else:
-                _, srcs, dst, scale = st
-                rows, c = f * self._rate[dst], b[dst].shape[2]
-                srcs = [b[s] for s in srcs] + [None] * (3 - len(srcs))
-                check(lib.kt_add3_scale_win(ptr(srcs[0]), ptr(srcs[1]), ptr(srcs[2]), scale, ptr(b[dst]), B, rows, c,
-                                            srcs[0].shape[1], b[dst].shape[1], self._hist[dst], stream_ptr()),
-                      "kt_add3_scale_win")
+                dst = b[st.dst]
+                srcs = [b[s] for s in st.srcs] + [None] * (3 - len(st.srcs))
+                check(lib.kt_add3_scale_win(ptr(srcs[0]), ptr(srcs[1]), ptr(srcs[2]), st.scale, ptr(dst), B,
+                                            f * win.rate[st.dst], dst.shape[2], srcs[0].shape[1], dst.shape[1],
+                                            win.first[st.dst], stream_ptr()), "kt_add3_scale_win")
                 ops._count()
-        if self._ntable:
-            check(lib.kt_stream_advance(ptr(self._table, True), self._ntable, B, f, self._max_c, stream_ptr()),
-                  "kt_stream_advance")
-            ops._count()
+        win.advance(f)
 
     def push(self, mel):
         """mel: (B, in_channels, f), 1 <= f <= max_frames, on the streamer's device -> the (B, 1, f * hop) waveform."""
-        if mel.dim() != 3 or mel.shape[0] != self.batch or mel.shape[1] != self.in_channels:
-            raise ValueError(f"push: expected a ({self.batch}, {self.in_channels}, f) mel, got {tuple(mel.shape)}")
-        f = mel.shape[2]
-        if not 1 <= f <= self.max_frames:
-            raise ValueError(f"push: a chunk holds 1 to {self.max_frames} frames, got {f}")
-        if mel.device != self.device:
-            raise ValueError(f"push: the mel is on {mel.device}, the streamer on {self.device}")
         with torch.no_grad(), torch.cuda.device(self.device):
-            h = self._hist["mel"]
-            self._buf["mel"][:, h:h + f].copy_(mel.transpose(1, 2))
+            f = self._win.push("mel", mel, 2, ("a {} mel", "frames", "the mel is"))
             if f == self.max_frames:
-                if self._graph is None:
-                    self._graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self._graph):
-                        self._run(f)
                 self._graph.replay()
             else:
                 self._run(f)
-            return self._buf["wav"][:, :f * self.hop, 0].unsqueeze(1).clone(memory_format=torch.contiguous_format)
+            return self._win.buf["wav"][:, :f * self.hop, 0].unsqueeze(1).clone(memory_format=torch.contiguous_format)
 
     def reset(self, slots):
         """The given batch slots start a new utterance: their carried state returns to zeros (one launch)."""
-        slots = sorted({int(s) for s in slots})
-        if any(not 0 <= s < self.batch for s in slots):
-            raise ValueError(f"reset: slots must lie in [0, {self.batch}), got {slots}")
-        mask = torch.zeros(self.batch, dtype=torch.uint8)
-        mask[slots] = 1
         with torch.cuda.device(self.device):
-            self._slots.copy_(mask)
-            self._reset_selected()
-
-    def _reset_selected(self):
-        if self._ntable:
-            check(_lib.load().kt_stream_reset(ptr(self._table, True), self._ntable, self.batch, ptr(self._slots, True),
-                                              self._max_c, stream_ptr()), "kt_stream_reset")
-            ops._count()
+            self._win.reset(slots)
 
 
 # --------------------------------------------------------------------------------------------

@@ -69,9 +69,6 @@ class TtsStream:
         self.max_frames = F = self.r * chunk_steps
         self._post = sambert.mel_postnet.streamer(B, F, frames)
         self._voc = generator.streamer(batch=B, max_frames=F)
-        # capture the vocoder's graph now (a capture synchronises the device) rather than in the middle of the stream
-        self._voc.push(torch.zeros(B, self.d_mel, F, device=frames.device))
-        self._voc.reset(range(B))
         self._used = False
 
     def _vocode(self, rows, start):

@@ -22,6 +22,7 @@ gather each way (kt_fp_insert_*).  Not built: MAS alignment (``MAS: True``) and 
 variant -- the shipped sambert_24k.yaml and sambert_fp_8k.yaml disable both.
 """
 import ctypes
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -30,7 +31,8 @@ import torch.nn.functional as F
 
 from . import ops
 from . import sambert_ops as sops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KtStreamWin, KtWindow
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, check, load, ptr, stream_ptr
+from .stream import Windows, WindowTable, own_weight
 
 
 def get_mask_from_lengths(lengths, max_len=None):
@@ -450,7 +452,6 @@ class VarRnnARPredictor(nn.Module):
         """adaptors.py:67-83: the per-symbol Python loop of the reference (prenet -> LSTM step -> fc, ~10 launches per symbol)
         is ONE kernel (kt_ar_duration_infer: one CTA per batch item walks the recurrence); the condition's share of the
         layer-0 input projection is one k = 1 conv over all symbols."""
-        from ._lib import load, check, ptr, stream_ptr
         lstm, B, L = self.lstm, cond.size(0), cond.size(1)
         H = lstm.hidden_size
         fc1, fc2 = [m for m in self.prenet.fcs if isinstance(m, nn.Linear)][:2]
@@ -764,17 +765,23 @@ class PostNet(nn.Module):
         return PostNetStreamer(self, batch, max_frames, lengths)
 
 
+# One launch of a post-net chunk over named windows.  kind "conv": a k = 1 conv of ``module`` (a Linear, or the nn.LSTM's
+# input projection); "fsmn": the memory block ``module`` of FSMN layer ``layer``; "lstm": the nn.LSTM's recurrence.
+# ``resid`` (or None) is added to the output from ``res_lag`` rows before the output's chunk rows.  A ``frame0`` step runs
+# over the chunk's rows of frame >= 0 only, written from row 0 of ``dst``; with ``in_skip`` its input holds every row.
+PostNetStep = namedtuple("PostNetStep", "kind module src dst resid res_lag frame0 in_skip layer",
+                         defaults=(None, 0, False, False, -1))
+
+
 class PostNetStreamPlan:
     """What a PostNetStreamer runs per chunk, as data (no device needed).  The post-net is causal except for the right
     padding of its memory blocks: output frame t is final once decoder row t + delay exists.
       layers              per FSMN layer: {lp, rp, kernel, lag}: the memory block's left / right padding and filter size, and
                           how many rows the layer's input lags the decoder rows (the sum of rp over the layers before it)
       delay               D = the sum of rp: the post-net output of a chunk is its decoder rows shifted back by D rows
-      windows             one entry per tensor of a chunk: {name, channels, history}; a memory block's input keeps k - 1
-                          rows, a residual read lagging its tensor by n rows keeps n, the others keep none
-      steps               ("conv", module, input, output, residual or None) | ("fsmn", layer, input, output, residual or
-                          None) | ("lstm", input, output), in launch order; the LSTM's input projection is the conv step
-                          whose module is the post-net's nn.LSTM
+      windows             one entry per tensor of a chunk: {name, channels, rows_per_frame (1), history}; a memory block's
+                          input keeps k - 1 rows, a residual read lagging its tensor by n rows keeps n, the others keep none
+      steps               PostNetStep records, in launch order
       launches_per_chunk  library calls of a steady chunk: one per step and one window advance; the copy of the decoder rows
                           into their window and the output mask are not counted"""
 
@@ -782,20 +789,10 @@ class PostNetStreamPlan:
         if postnet.training:
             raise ValueError("streaming runs a post-net in eval() mode")
         fsmn = postnet.fsmn
-        self.windows, self.layers, self.steps = [], [], []
-        index = {}
-
-        def tensor(name, channels):
-            index[name] = len(self.windows)
-            self.windows.append(dict(name=name, channels=channels, history=0))
-            return name
-
-        def read(name, history):
-            w = self.windows[index[name]]
-            w["history"] = max(w["history"], history)
-
-        x, lag = tensor("dec", postnet.num_mels), 0
-        mid = tensor("mid", fsmn.ffn_inner_dim)
+        table = WindowTable()
+        self.windows, self.layers, self.steps = table.windows, [], []
+        x, lag = table.add("dec", postnet.num_mels), 0
+        mid = table.add("mid", fsmn.ffn_inner_dim)
         units = fsmn.num_memory_units
         for i, (ffn, mb) in enumerate(zip(fsmn.ffn_lst, fsmn.memory_block_lst)):
             k = mb.conv_dw.kernel_size[0]
@@ -803,21 +800,24 @@ class PostNetStreamPlan:
                 raise ValueError(f"streaming needs rp >= 0 in every memory block: layer {i} has shift > (filter_size - 1) / 2 "
                                  f"(lp {mb.lp}, rp {mb.rp})")
             self.layers.append(dict(lp=mb.lp, rp=mb.rp, kernel=k, lag=lag))
-            ctx = tensor(f"ctx{i}", units)
-            read(ctx, k - 1)
+            ctx = table.add(f"ctx{i}", units)
+            table.read(ctx, k - 1)
             resid = x if ffn.w_1.in_channels == units else None
             if resid is not None:
-                read(resid, mb.rp)
-            out = tensor(f"x{i + 1}", units)
-            self.steps += [("conv", ffn.w_1, x, mid, None), ("conv", ffn.w_2, mid, ctx, None), ("fsmn", i, ctx, out, resid)]
+                table.read(resid, mb.rp)
+            out = table.add(f"x{i + 1}", units)
+            self.steps += [PostNetStep("conv", ffn.w_1, x, mid), PostNetStep("conv", ffn.w_2, mid, ctx),
+                           PostNetStep("fsmn", mb, ctx, out, resid, res_lag=mb.rp, layer=i)]
             x, lag = out, lag + mb.rp
         self.delay = lag
-        read("dec", self.delay)                            # the output Linear's residual: the decoder rows D rows back
-        gates = tensor("gates", 4 * postnet.lstm.hidden_size)
-        h = tensor("h", postnet.lstm.hidden_size)
-        self.steps += [("conv", postnet.lstm, x, gates, None), ("lstm", gates, h),
-                       ("conv", postnet.fc, h, tensor("out", postnet.num_mels), "dec")]
-        self.launches_per_chunk = len(self.steps) + any(w["history"] for w in self.windows)
+        table.read("dec", self.delay)                      # the output Linear's residual: the decoder rows D rows back
+        gates = table.add("gates", 4 * postnet.lstm.hidden_size)
+        h = table.add("h", postnet.lstm.hidden_size)
+        self.steps += [PostNetStep("conv", postnet.lstm, x, gates, frame0=True, in_skip=True),
+                       PostNetStep("lstm", postnet.lstm, gates, h, frame0=True),
+                       PostNetStep("conv", postnet.fc, h, table.add("out", postnet.num_mels), "dec", res_lag=self.delay,
+                                   frame0=True)]
+        self.launches_per_chunk = table.launches_per_chunk(len(self.steps))
 
 
 class PostNetStreamer:
@@ -829,100 +829,69 @@ class PostNetStreamer:
     ``delay`` all-padding rows and returns the rest; the rows returned in order are then the whole-sequence post-net output.
     ``reset(lengths=None)`` starts a new batch.  No call reads device data on the host.
 
-    Each tensor a layer reads before the chunk lives in a persistent window of [history | chunk] rows per slot (see
-    PostNetStreamPlan); kt_fsmn_fwd_stream masks by each row's frame index against the slot lengths kept on the device, and
-    kt_lstm_stream carries the LSTM state.  The weights are prepared once, when the streamer is created."""
+    A tensor a layer reads before the chunk lives in a window (stream.py); kt_fsmn_fwd_stream masks by each row's frame
+    index against the slot lengths kept on the device, and kt_lstm_stream carries the LSTM state.  The weights are
+    prepared once, when the streamer is created."""
 
     def __init__(self, postnet, batch, max_frames, lengths):
         self.plan = plan = PostNetStreamPlan(postnet)
-        batch, max_frames = int(batch), int(max_frames)
-        if batch < 1 or max_frames < 1:
-            raise ValueError(f"streamer: batch ({batch}) and max_frames ({max_frames}) must be >= 1")
-        dev = next(postnet.parameters()).device
-        if dev.type != "cuda":
-            raise RuntimeError("kantts_b200: the post-net streamer runs on a CUDA device (no CPU fallback)")
-        self.batch, self.max_frames, self.delay, self.device = batch, max_frames, plan.delay, dev
+        self._win = win = Windows(plan.windows, batch, max_frames, next(postnet.parameters()).device, "post-net streamer")
+        self.batch, self.max_frames, self.delay, self.device = win.batch, win.max_frames, plan.delay, win.device
         self.num_mels, self.hidden = postnet.num_mels, postnet.lstm.hidden_size
-        self._hist = {w["name"]: w["history"] for w in plan.windows}
-        self._buf = {w["name"]: torch.zeros(batch, w["history"] + max_frames, w["channels"], device=dev) for w in plan.windows}
-        kept = [w for w in plan.windows if w["history"] > 0]
-        table = (KtWindow * len(kept))(*[KtWindow(base=self._buf[w["name"]].data_ptr(), pitch=self._buf[w["name"]].shape[1],
-                                                  channels=w["channels"], history=w["history"], rows_per_frame=1) for w in kept])
-        self._table = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(dev)
-        self._ntable, self._max_c = len(kept), max([w["channels"] for w in kept], default=1)
-        self._slots = torch.ones(batch, dtype=torch.uint8, device=dev)
-        self._state = torch.zeros(batch, 2, self.hidden, device=dev)
-        self._zeros = torch.zeros(batch, max_frames, self.num_mels, device=dev)
-        self._len = torch.empty(batch, dtype=torch.int32, device=dev)
-        self._weights = {}
-        self._ffn = {m for ffn in postnet.fsmn.ffn_lst for m in (ffn.w_1, ffn.w_2)}
-        with torch.no_grad(), torch.cuda.device(dev):
-            for st in plan.steps:
-                if st[0] == "conv":
-                    mod = st[1]
-                    if isinstance(mod, nn.LSTM):             # x . W_ih^T + b_ih + b_hh as one k = 1 conv
-                        spec = ops.ConvSpec(c_in=mod.input_size, c_out=4 * mod.hidden_size, kernel=1)
-                        w, b = mod.weight_ih_l0.unsqueeze(-1), mod.bias_ih_l0 + mod.bias_hh_l0
-                    else:
-                        spec, w, b = mod.spec, mod.weight, mod.bias
-                    pw = ops.prepare_weight(ops.PreparedWeight(), spec, w.detach().clone(), None)
-                    self._weights[mod] = (spec, pw, None if b is None else b.detach().clone())
-                elif st[0] == "fsmn":
-                    mb = postnet.fsmn.memory_block_lst[st[1]]
-                    self._weights[st[1]] = mb.conv_dw.weight.detach().reshape(mb.conv_dw.out_channels, -1).clone()
-            self._whh_t = postnet.lstm.weight_hh_l0.detach().t().contiguous()
+        self._state = torch.zeros(self.batch, 2, self.hidden, device=self.device)
+        self._zeros = torch.zeros(self.batch, self.max_frames, self.num_mels, device=self.device)
+        self._len = torch.empty(self.batch, dtype=torch.int32, device=self.device)
+        self._steady = [self._place(st, 0) for st in plan.steps]
+        with torch.no_grad(), torch.cuda.device(self.device):
+            self._weights = [self._own_weight(st) for st in plan.steps]
             self.reset(lengths)
 
-    def _win(self, src, dst, resid, in_skip=0, res_first=None):
-        b = self._buf
-        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=self._hist[src] + in_skip, out_pitch=b[dst].shape[1],
-                        out_first=self._hist[dst])
-        if resid is not None:
-            w.res_pitch = b[resid].shape[1]
-            w.res_first = self._hist[resid] if res_first is None else res_first
-        return w
+    @staticmethod
+    def _own_weight(st):
+        """-> copies of what step st reads besides its windows: (spec, PreparedWeight, bias), the (C, k) taps or W_hh^T."""
+        mod = st.module
+        if st.kind == "fsmn":
+            return mod.conv_dw.weight.detach().reshape(mod.conv_dw.out_channels, -1).clone()
+        if st.kind == "lstm":
+            return mod.weight_hh_l0.detach().t().contiguous()
+        if isinstance(mod, nn.LSTM):                       # x . W_ih^T + b_ih + b_hh as one k = 1 conv
+            spec = ops.ConvSpec(c_in=mod.input_size, c_out=4 * mod.hidden_size, kernel=1)
+            return (spec, *own_weight(spec, mod.weight_ih_l0.unsqueeze(-1), None, mod.bias_ih_l0 + mod.bias_hh_l0))
+        return (mod.spec, *own_weight(mod.spec, mod.weight, None, mod.bias))
+
+    def _place(self, st, skip):
+        """-> the KtStreamWin of step st (None for the LSTM) in a chunk whose first ``skip`` rows lie before frame 0."""
+        if st.kind == "lstm":
+            return None
+        o = skip if st.frame0 else 0                    # the chunk row of the step's first output row
+        return self._win.place(st.src, st.dst, st.resid, in_offset=o if st.in_skip else 0, res_lag=st.res_lag - o)
 
     def _chunk(self, f):
         """Every launch of one chunk of f decoder rows (already in the "dec" window) -> the final output rows."""
-        from ._lib import load, check, ptr, stream_ptr
-        lib, b, B, a = load(), self._buf, self.batch, self._rows
+        lib, b, B, a = load(), self._win.buf, self.batch, self._rows
         first = a - self.delay                      # frame of the chunk's first output row
         skip = max(0, -first)                       # output rows before frame 0 are not rows of the utterance
         n = f - skip
-        for st in self.plan.steps:
-            kind = st[0]
-            if kind == "fsmn":
-                _, i, src, dst, resid = st
-                layer = self.plan.layers[i]
-                k = layer["kernel"]
-                win = self._win(src, dst, resid, res_first=None if resid is None else self._hist[resid] - layer["rp"])
-                check(lib.kt_fsmn_fwd_stream(ctypes.byref(win), ptr(b[src]), ptr(self._weights[i]), ptr(self._len, True),
-                                             ptr(None if resid is None else b[resid]), ptr(b[dst]), B, f, b[src].shape[2], k,
-                                             layer["lp"], a - layer["lag"] - layer["rp"], stream_ptr()), "kt_fsmn_fwd_stream")
-                ops._count()
-            elif kind == "conv" and st[1] in self._ffn:     # the FSMN feed-forward convs over the whole chunk
-                _, mod, src, dst, _ = st
-                spec, pw, bias = self._weights[mod]
-                ops.stream_conv(spec, pw, bias, b[src], b[dst], f, self._win(src, dst, None))
-            elif n <= 0:
-                continue                            # nothing of the utterance has reached the LSTM yet
-            elif kind == "lstm":
-                _, src, dst = st
-                check(lib.kt_lstm_stream(ptr(b[src]), ptr(self._whh_t), ptr(self._state), ptr(b[dst]), B, n, self.hidden,
-                                         b[src].shape[1], b[dst].shape[1], stream_ptr()), "kt_lstm_stream")
+        places = self._steady if skip == 0 else [self._place(st, skip) for st in self.plan.steps]
+        for st, w, place in zip(self.plan.steps, self._weights, places):
+            if st.frame0 and n <= 0:
+                continue                            # nothing of the utterance has reached this step yet
+            src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
+            rows = n if st.frame0 else f
+            if st.kind == "conv":
+                spec, pw, bias = w
+                ops.stream_conv(spec, pw, bias, src, dst, rows, place, resid)
+            elif st.kind == "fsmn":
+                layer = self.plan.layers[st.layer]
+                check(lib.kt_fsmn_fwd_stream(ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True), ptr(resid),
+                                             ptr(dst), B, rows, src.shape[2], layer["kernel"], layer["lp"],
+                                             a - layer["lag"] - layer["rp"], stream_ptr()), "kt_fsmn_fwd_stream")
                 ops._count()
             else:
-                _, mod, src, dst, resid = st
-                spec, pw, bias = self._weights[mod]
-                if resid is None:                   # the LSTM input projection: the chunk's rows from frame 0 on
-                    ops.stream_conv(spec, pw, bias, b[src], b[dst], n, self._win(src, dst, None, in_skip=skip))
-                else:                               # output Linear + the decoder rows D rows back
-                    win = self._win(src, dst, resid, res_first=self._hist[resid] - self.delay + skip)
-                    ops.stream_conv(spec, pw, bias, b[src], b[dst], n, win, b[resid])
-        if self._ntable:
-            check(lib.kt_stream_advance(ptr(self._table, True), self._ntable, B, f, self._max_c, stream_ptr()),
-                  "kt_stream_advance")
-            ops._count()
+                check(lib.kt_lstm_stream(ptr(src), ptr(w), ptr(self._state), ptr(dst), B, rows, self.hidden, src.shape[1],
+                                         dst.shape[1], stream_ptr()), "kt_lstm_stream")
+                ops._count()
+        self._win.advance(f)
         self._rows += f
         if n <= 0:
             return b["out"][:, :0].clone()
@@ -932,17 +901,8 @@ class PostNetStreamer:
 
     def push(self, dec_rows):
         """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final."""
-        if dec_rows.dim() != 3 or dec_rows.shape[0] != self.batch or dec_rows.shape[2] != self.num_mels:
-            raise ValueError(f"push: expected ({self.batch}, f, {self.num_mels}) decoder rows, got {tuple(dec_rows.shape)}")
-        f = dec_rows.shape[1]
-        if not 1 <= f <= self.max_frames:
-            raise ValueError(f"push: a chunk holds 1 to {self.max_frames} rows, got {f}")
-        if dec_rows.device != self.device:
-            raise ValueError(f"push: the rows are on {dec_rows.device}, the streamer on {self.device}")
         with torch.no_grad(), torch.cuda.device(self.device):
-            h = self._hist["dec"]
-            self._buf["dec"][:, h:h + f].copy_(dec_rows)
-            return self._chunk(f)
+            return self._chunk(self._win.push("dec", dec_rows, 1, ("{} decoder rows", "rows", "the rows are")))
 
     def finish(self):
         """Push ``delay`` all-padding rows (the whole-sequence zero padding) -> the remaining (B, n, num_mels) output rows."""
@@ -956,16 +916,12 @@ class PostNetStreamer:
     def reset(self, lengths=None):
         """Start a new batch: the carried windows and LSTM state return to zeros; ``lengths`` (device tensor (batch,)),
         when given, replaces the slots' frame counts."""
-        from ._lib import load, check, ptr, stream_ptr
         with torch.no_grad(), torch.cuda.device(self.device):
             if lengths is not None:
                 if lengths.shape != (self.batch,):
                     raise ValueError(f"reset: expected ({self.batch},) lengths, got {tuple(lengths.shape)}")
                 self._len.copy_(lengths)
-            if self._ntable:
-                check(load().kt_stream_reset(ptr(self._table, True), self._ntable, self.batch, ptr(self._slots, True),
-                                             self._max_c, stream_ptr()), "kt_stream_reset")
-                ops._count()
+            self._win.reset()
             self._state.zero_()
         self._rows = 0
 

@@ -1,0 +1,108 @@
+"""The stream window format of the streamed vocoder (hifigan.GeneratorStreamer) and post-net (sambert.PostNetStreamer),
+DESIGN.md §3.7.  A window is a persistent (B, H + F·rows_per_frame, C) buffer: rows [0, H) carry the last H rows of the
+earlier chunks (zeros after a reset: the causal padding), the chunk is written at row H, and H is the largest history
+any reader of the tensor needs."""
+import torch
+
+from . import ops
+from ._lib import KtStreamWin, KtWindow, check, load, ptr, stream_ptr
+
+
+class WindowTable:
+    """Plan-time list of a stream's windows: ``windows`` holds one {name, channels, rows_per_frame, history} dict per
+    tensor, in the order they were added."""
+
+    def __init__(self):
+        self.windows = []
+
+    def add(self, name, channels, rows_per_frame=1):
+        self.windows.append(dict(name=name, channels=channels, rows_per_frame=rows_per_frame, history=0))
+        return name
+
+    def read(self, name, history):
+        """A reader of ``name`` needs ``history`` rows before the chunk."""
+        w = next(w for w in self.windows if w["name"] == name)
+        w["history"] = max(w["history"], history)
+
+    def launches_per_chunk(self, steps):
+        """``steps`` launches, plus the window advance when any window keeps history."""
+        return steps + any(w["history"] for w in self.windows)
+
+
+class Windows:
+    """The buffers of a WindowTable's windows for ``batch`` slots and chunks of 1..max_frames frames, by name: ``buf``
+    (B, pitch, C), ``first`` (row H, where the chunk starts) and ``rate`` (rows per frame)."""
+
+    def __init__(self, windows, batch, max_frames, device, what):
+        batch, max_frames = int(batch), int(max_frames)
+        if batch < 1 or max_frames < 1:
+            raise ValueError(f"streamer: batch ({batch}) and max_frames ({max_frames}) must be >= 1")
+        if device.type != "cuda":
+            raise RuntimeError(f"kantts_b200: the {what} runs on a CUDA device (no CPU fallback)")
+        self.batch, self.max_frames, self.device = batch, max_frames, device
+        self.buf = {w["name"]: torch.zeros(batch, w["history"] + max_frames * w["rows_per_frame"], w["channels"], device=device)
+                    for w in windows}
+        self.first = {w["name"]: w["history"] for w in windows}
+        self.rate = {w["name"]: w["rows_per_frame"] for w in windows}
+        kept = [w for w in windows if w["history"] > 0]
+        table = (KtWindow * len(kept))(*[KtWindow(base=self.buf[w["name"]].data_ptr(), pitch=self.buf[w["name"]].shape[1],
+                                                  channels=w["channels"], history=w["history"],
+                                                  rows_per_frame=w["rows_per_frame"]) for w in kept])
+        self._table = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(device)
+        self._ntable, self._max_c = len(kept), max([w["channels"] for w in kept], default=1)
+        self._all = torch.ones(batch, dtype=torch.uint8, device=device)
+
+    def push(self, name, x, f_axis, what):
+        """Check the chunk x, (B, C, f) for f_axis 2 or (B, f, C) for f_axis 1, and write it into window ``name`` -> f.
+        ``what``: (x's description with {} for the shape, unit of f, "<x> is") for the errors."""
+        c = self.buf[name].shape[2]
+        if x.dim() != 3 or x.shape[0] != self.batch or x.shape[3 - f_axis] != c:
+            shape = (self.batch, c, "f") if f_axis == 2 else (self.batch, "f", c)
+            raise ValueError(f"push: expected {what[0].format('(%s, %s, %s)' % shape)}, got {tuple(x.shape)}")
+        f = x.shape[f_axis]
+        if not 1 <= f <= self.max_frames:
+            raise ValueError(f"push: a chunk holds 1 to {self.max_frames} {what[1]}, got {f}")
+        if x.device != self.device:
+            raise ValueError(f"push: {what[2]} on {x.device}, the streamer on {self.device}")
+        h = self.first[name]
+        self.buf[name][:, h:h + f].copy_(x if f_axis == 1 else x.transpose(1, 2))
+        return f
+
+    def place(self, src, dst, resid=None, in_offset=0, res_lag=0):
+        """-> the KtStreamWin of a layer reading ``src`` from ``in_offset`` rows into its chunk, writing the chunk of
+        ``dst`` and adding the rows of ``resid`` that lie ``res_lag`` rows before its chunk."""
+        b, first = self.buf, self.first
+        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=first[src] + in_offset, out_pitch=b[dst].shape[1],
+                        out_first=first[dst])
+        if resid is not None:
+            w.res_pitch, w.res_first = b[resid].shape[1], first[resid] - res_lag
+        return w
+
+    def advance(self, frames):
+        """After a chunk of ``frames`` frames, the last H rows of every window become its history (one launch)."""
+        if self._ntable:
+            check(load().kt_stream_advance(ptr(self._table, True), self._ntable, self.batch, frames, self._max_c,
+                                           stream_ptr()), "kt_stream_advance")
+            ops._count()
+
+    def reset(self, slots=None):
+        """The history of the given slots (None: all) returns to zeros in every window (one launch)."""
+        sel = self._all
+        if slots is not None:
+            slots = sorted({int(s) for s in slots})
+            if any(not 0 <= s < self.batch for s in slots):
+                raise ValueError(f"reset: slots must lie in [0, {self.batch}), got {slots}")
+            mask = torch.zeros(self.batch, dtype=torch.uint8)
+            mask[slots] = 1
+            sel = mask.to(self.device)
+        if self._ntable:
+            check(load().kt_stream_reset(ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c,
+                                         stream_ptr()), "kt_stream_reset")
+            ops._count()
+
+
+def own_weight(spec, v, g, bias):
+    """-> (a fresh PreparedWeight from copies of v and g, a copy of bias): a streamer's own weights, never the module's
+    cache.  g and bias may be None."""
+    copy = lambda t: None if t is None else t.detach().clone()
+    return ops.prepare_weight(ops.PreparedWeight(), spec, copy(v), copy(g)), copy(bias)
