@@ -5,11 +5,18 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <vector>
 
 #include "../../include/kantts_b200.h"
 
+// Each entry point of kantts_b200.h is defined as extern "C" inside namespace kt, in the file that holds its kernels.  A
+// C-linkage function is the same function whichever namespace declares it, so the compiler checks every definition against
+// its header declaration; inside a namespace a mismatch is only warning 338, so make it an error.
+#pragma nv_diag_error 338
+
 namespace kt {
 
+// The calling thread's error string, returned by kt_last_error (api.cu)
 void set_error(const char* fmt, ...);
 
 // variadic: the expression may contain a template-id with commas (allow_dyn_smem<kernel<A, B>>(...))
@@ -148,5 +155,25 @@ inline ResidueTaps residue_taps(const Phase& ph, int step) {
   rt.first[step] = n;
   return rt;
 }
+
+// ---- host functions shared between files ----
+// conv_ffma.cu
+int validate_conv(const KtConv1dDesc* d);
+// validate_conv plus the window placement of one stream chunk (kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream)
+int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what);
+Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up);
+std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir);
+// out[c] = the sum of the Side's values of channel c over `rows` rows, in a fixed order (the bias gradient)
+int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t st);
+// thin.cu: the single-input-channel layers
+bool thin_cin1_ok(const KtConv1dDesc* d);
+int thin_cin1_fwd(const KtConv1dDesc* d, const float* x, const float* w_fwd, const float* bias, float* y, cudaStream_t st);
+int thin_cin1_wgrad(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw, float* dbias,
+                    cudaStream_t st);
+// conv_tc.cu
+int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cudaStream_t st);
+// allow_tma = false: the register-staged route, which needs no workspace (kt_resblock_bwd)
+int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x, float* dx,
+                       float* ws, long long ws_floats, cudaStream_t st, bool allow_tma);
 
 }  // namespace kt

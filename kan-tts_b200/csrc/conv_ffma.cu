@@ -21,27 +21,12 @@
 //
 // These kernels are the exact-fp32 path (and the only path for thin layers: C_in/g < 32, C_out = 1).
 // The tensor-core kernels in conv_tc.cu take over the GEMM-shaped layers.
-#include <stdarg.h>
-#include <string.h>
-
 #include <algorithm>
 #include <vector>
 
 #include "common.cuh"
 
 namespace kt {
-
-// ---------------------------------------------------------------------------------------------
-// error string (thread-local: the ABI is re-entrant across forward / autograd threads)
-// ---------------------------------------------------------------------------------------------
-static thread_local char g_err[512] = "";
-void set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-}
-const char* last_error() { return g_err; }
 
 // ---------------------------------------------------------------------------------------------
 // core (forward-like) primitive
@@ -560,7 +545,7 @@ __global__ void colsum_kernel(Side s, long long rows, int c, float* part) {
 // ---------------------------------------------------------------------------------------------
 // host-side decomposition of a layer into phases
 // ---------------------------------------------------------------------------------------------
-static int validate(const KtConv1dDesc* d) {
+int validate_conv(const KtConv1dDesc* d) {
   KT_REQUIRE(d != nullptr, "null descriptor");
   KT_REQUIRE(d->batch > 0 && d->nsub > 0 && d->t_in > 0 && d->t_out > 0, "bad sizes B=%d nsub=%d t_in=%d t_out=%d", d->batch, d->nsub, d->t_in, d->t_out);
   KT_REQUIRE(d->c_in > 0 && d->c_out > 0 && d->groups > 0 && d->c_in % d->groups == 0 && d->c_out % d->groups == 0, "bad channels/groups %d %d %d", d->c_in, d->c_out, d->groups);
@@ -569,6 +554,18 @@ static int validate(const KtConv1dDesc* d) {
   KT_REQUIRE(!(d->transposed && (d->groups != 1 || d->upsample != 1)), "transposed conv: groups/upsample unsupported");
   KT_REQUIRE(!(d->upsample > 1 && d->stride != 1), "upsampled conv must have stride 1");
   KT_REQUIRE((long long)d->batch * d->nsub <= 65535, "batch*nsub too large");
+  return KT_OK;
+}
+
+int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what) {
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(w != nullptr, "%s: null window descriptor", what);
+  KT_REQUIRE(d->nsub == 1, "%s: streams need nsub == 1", what);
+  KT_REQUIRE(w->in_first >= 0 && w->in_first + d->t_in <= w->in_pitch, "%s: the chunk does not fit its input window", what);
+  KT_REQUIRE(w->out_first >= 0 && w->out_first + d->t_out <= w->out_pitch, "%s: the chunk does not fit its output window", what);
+  KT_REQUIRE(!resid || (w->res_first >= 0 && w->res_first + d->t_out <= w->res_pitch),
+             "%s: the chunk does not fit its residual window", what);
   return KT_OK;
 }
 
@@ -645,12 +642,13 @@ std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir) {
   return v;
 }
 
-bool thin_cin1_ok(const KtConv1dDesc* d);                                                                       // thin.cu
-int thin_cin1_fwd(const KtConv1dDesc*, const float*, const float*, const float*, float*, cudaStream_t);
-int thin_cin1_wgrad(const KtConv1dDesc*, const float*, const float*, const float*, float*, float*, cudaStream_t);
-
-int conv1d_fwd_ffma(const KtConv1dDesc* d, const float* x, const float* w_fwd, const float* bias,
-                    const float* resid, float* y, cudaStream_t st) {
+extern "C" int kt_conv1d_fwd(const KtConv1dDesc* d, const float* x, const float* w_fwd, const float* bias, const float* resid,
+                             float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd: null pointer");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_fwd: tensor-core path not available for this shape");
   if (thin_cin1_ok(d) && resid == nullptr) return thin_cin1_fwd(d, x, w_fwd, bias, y, st);   // waveform-input layers
   CoreParams p{};
   p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
@@ -660,15 +658,19 @@ int conv1d_fwd_ffma(const KtConv1dDesc* d, const float* x, const float* w_fwd, c
   p.out_act = d->act_out; p.out_slope = d->act_out_slope;
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
-    int rc = run_core(p, st);
+    rc = run_core(p, st);
     if (rc) return rc;
   }
   return KT_OK;
 }
 
 // One chunk of a stream (KtStreamWin): the forward's phases over the windows
-int conv1d_fwd_ffma_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd, const float* bias,
-                           const float* resid, float* y, cudaStream_t st) {
+extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd,
+                                    const float* bias, const float* resid, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
   CoreParams p{};
   p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   p.w = w_fwd; p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
@@ -679,17 +681,22 @@ int conv1d_fwd_ffma_stream(const KtConv1dDesc* d, const KtStreamWin* w, const fl
   p.res_pitch = w->res_pitch; p.res_first = w->res_first;
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
-    int rc = run_core<true>(p, st);
+    rc = run_core<true>(p, st);
     if (rc) return rc;
   }
   return KT_OK;
 }
 
-int conv1d_bwd_data_ffma(const KtConv1dDesc* d, const float* dy, const float* y, const float* w_bwd,
-                         const float* x, float* dx, cudaStream_t st) {
-  CoreParams p{};
+extern "C" int kt_conv1d_bwd_data(const KtConv1dDesc* d, const float* dy, const float* y, const float* w_bwd, const float* x,
+                                  float* dx, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(dy && w_bwd && dx, "kt_conv1d_bwd_data: null pointer");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_data: tensor-core path not available for this shape");
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_data: y required when act_out != NONE");
   KT_REQUIRE(d->act_in == KT_ACT_NONE || x != nullptr, "bwd_data: x required when act_in != NONE");
+  CoreParams p{};
   p.in = make_side(dy, y, d->act_out, d->act_out_slope, true);
   p.w = w_bwd; p.bias = nullptr; p.resid = nullptr; p.out = dx;
   p.mask = dgrad_mask(d, x);
@@ -700,16 +707,19 @@ int conv1d_bwd_data_ffma(const KtConv1dDesc* d, const float* dy, const float* y,
   // (a fused act_in' mask is multiplicative, so applying it in every accumulating phase is exact)
   for (const Phase& ph : conv_phases(d, 1)) {
     p.ph = ph;
-    int rc = run_core(p, st);
+    rc = run_core(p, st);
     if (rc) return rc;
   }
   return KT_OK;
 }
 
-int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t st);
-
-int conv1d_bwd_weight_ffma(const KtConv1dDesc* d, const float* x, const float* dy, const float* y,
-                           float* dw, float* dbias, cudaStream_t st) {
+extern "C" int kt_conv1d_bwd_weight(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw,
+                                    float* dbias, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(x && dy && dw, "kt_conv1d_bwd_weight: null pointer");
+  KT_REQUIRE(d->path != KT_PATH_TC, "kt_conv1d_bwd_weight: tensor-core path not available for this shape");
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_weight: y required when act_out != NONE");
   if (thin_cin1_ok(d)) return thin_cin1_wgrad(d, x, dy, y, dw, dbias, st);
   const size_t wn = (size_t)d->kernel * (d->c_in / d->groups) * d->c_out;
@@ -733,7 +743,7 @@ int conv1d_bwd_weight_ffma(const KtConv1dDesc* d, const float* x, const float* d
     p.ca_g = d->c_out; p.cb_g = d->c_in;
     p.ph = gather_phase(d->t_in, d->kernel, d->stride, d->dilation, d->pad_left, 1);
   }
-  int rc = run_wgrad(p, st);
+  rc = run_wgrad(p, st);
   if (rc) return rc;
   if (dbias) return colsum_bias(sdy, (long long)d->batch * d->nsub * d->t_out, d->c_out, dbias, st);
   return KT_OK;
@@ -750,7 +760,5 @@ int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t s
   if (rc) return rc;
   return scratch_free(part, st);
 }
-
-int validate_conv(const KtConv1dDesc* d) { return validate(d); }
 
 }  // namespace kt

@@ -430,7 +430,6 @@ struct TcLayerPlan {
   int kin_g, pout_g;   // grouped: channels of ONE group on the contraction / produced side (kg = gt * kin_g)
 };
 
-std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir);  // conv_ffma.cu
 struct TcParams;
 
 // shared memory outside the activation / weight stages: barriers and the tap-shift table (see the carve-up in conv_tc_kernel)
@@ -530,8 +529,6 @@ static bool plan_launches(const std::vector<Phase>& phases, int nsub, std::vecto
   return true;
 }
 
-bool thin_cin1_ok(const KtConv1dDesc* d);   // thin.cu
-
 // What a call of direction dir (0 forward, 1 data gradient) of a layer runs: the tiling, the launches (phases planned,
 // pointers filled in by the caller) and the route.  The gathered operand is x (c_in channels, t_in rows) for the forward
 // and dy (c_out channels, t_out rows) for the data gradient.
@@ -605,15 +602,24 @@ static TcPlan make_tc_plan_flags(const KtConv1dDesc* d, int dir, bool plan_only 
   return make_tc_plan(d, dir, true, plan_only);
 }
 
-int tc_plan(const KtConv1dDesc* d, int dir) {
+static int tc_plan(const KtConv1dDesc* d, int dir) {
   const TcPlan P = make_tc_plan_flags(d, dir);
   return P.ok ? P.L.NT : 0;
 }
 
-long long conv_tc_workspace(const KtConv1dDesc* d, int dir) { return make_tc_plan_flags(d, dir).ws_floats; }
+extern "C" int kt_conv1d_tc_plan(const KtConv1dDesc* d, int32_t dir) {
+  if (validate_conv(d)) return 0;
+  return tc_plan(d, dir);
+}
+
+extern "C" int64_t kt_conv1d_tc_workspace(const KtConv1dDesc* d, int32_t dir) {
+  if (validate_conv(d)) return 0;
+  return make_tc_plan_flags(d, dir).ws_floats;
+}
 
 // bytes of the packed split-bf16 weight image of direction `dir` (0 when unsupported)
-long long tc_image_bytes(const KtConv1dDesc* d, int dir) {
+extern "C" int64_t kt_conv1d_tc_image_bytes(const KtConv1dDesc* d, int32_t dir) {
+  if (validate_conv(d)) return 0;
   if (dir != 0 && dir != 1) return 0;
   if (tc_plan(d, dir) == 0) return 0;
   const TcLayerPlan L = layer_plan(d, dir);
@@ -629,6 +635,12 @@ int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cud
                                                L.grouped ? L.kin_g : 0, L.pout_g, reinterpret_cast<__nv_bfloat16*>(out));
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
+}
+
+extern "C" int kt_weight_pack_tc(const KtConv1dDesc* d, int32_t dir, const float* w, void* out, void* stream) {
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  return tc_pack_layer(d, dir, w, out, static_cast<cudaStream_t>(stream));
 }
 
 // Ring sizes of one launch -> its shared-memory bytes (0: the stages do not fit)
@@ -659,14 +671,16 @@ static size_t size_stages(TcParams& p) {
 // development / test aid (kt_debug_conv_tc_plan): the plan of direction dir as it would be made on a GPU box
 // out = {N tile (0: not on the tensor cores), TMA route, tt, R, a_box_t, image stages, weight stages, shared-memory bytes,
 // workspace floats}, the launch-dependent entries for the first launch
-void debug_conv_tc_plan(const KtConv1dDesc* d, int dir, long long* out) {
+extern "C" int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t* out) {
+  KT_REQUIRE(d && out, "kt_debug_conv_tc_plan: null pointer");
   TcPlan P = make_tc_plan_flags(d, dir, true);
   for (int i = 0; i < 9; ++i) out[i] = 0;
-  if (!P.ok) return;
+  if (!P.ok) return KT_OK;
   TcParams& lp = P.launches[0];
   const size_t smem = size_stages(lp);
   out[0] = P.L.NT; out[1] = P.tma; out[2] = lp.tt; out[3] = lp.R; out[4] = lp.a_box_t;
-  out[5] = lp.na_stages; out[6] = lp.nb_stages; out[7] = (long long)smem; out[8] = P.ws_floats;
+  out[5] = lp.na_stages; out[6] = lp.nb_stages; out[7] = (int64_t)smem; out[8] = P.ws_floats;
+  return KT_OK;
 }
 
 static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, cudaStream_t st) {   // p: phases already planned
@@ -728,8 +742,11 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
   return KT_OK;
 }
 
-int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
-                  float* y, float* ws, long long ws_floats, cudaStream_t st) {
+extern "C" int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const float* bias, const float* resid,
+                                float* y, float* ws, int64_t ws_floats, void* stream) {
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc: null pointer");
   const TcPlan P = make_tc_plan(d, 0);
   KT_REQUIRE(P.ok, "conv1d_fwd_tc: layer not supported by the tensor-core path");
   TcParams io{};
@@ -737,12 +754,15 @@ int conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const void* wimg, const
   io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
   io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
-  return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", st);
+  return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", static_cast<cudaStream_t>(stream));
 }
 
 // One chunk of a stream (KtStreamWin): the register-staged route over the windows
-int conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg, const float* bias,
-                         const float* resid, float* y, cudaStream_t st) {
+extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg,
+                                       const float* bias, const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
   const TcPlan P = make_tc_plan_flags(d, KT_PLAN_STREAM);
   KT_REQUIRE(P.ok && !P.tma, "conv1d_fwd_tc_stream: layer not supported by the tensor-core path");
   KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "conv1d_fwd_tc_stream: bad window pitch");
@@ -753,10 +773,9 @@ int conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const floa
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
   io.in_pitch = w->in_pitch; io.in_first = w->in_first; io.out_pitch = w->out_pitch; io.out_first = w->out_first;
   io.res_pitch = w->res_pitch; io.res_first = w->res_first;
-  return run_plan(P, io, nullptr, 0, "conv1d_fwd_tc_stream", st);
+  return run_plan(P, io, nullptr, 0, "conv1d_fwd_tc_stream", static_cast<cudaStream_t>(stream));
 }
 
-// allow_tma = false: the register-staged route, which needs no workspace (kt_resblock_bwd)
 int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
                        float* dx, float* ws, long long ws_floats, cudaStream_t st, bool allow_tma) {
   const TcPlan P = make_tc_plan(d, 1, allow_tma);
@@ -770,6 +789,14 @@ int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, c
   io.mask = dgrad_mask(d, x);
   io.out_act = KT_ACT_NONE; io.out_slope = 0.f;
   return run_plan(P, io, ws, ws_floats, "conv1d_bwd_data_tc", st);
+}
+
+extern "C" int kt_conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,
+                                     float* dx, float* ws, int64_t ws_floats, void* stream) {
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(dy && wimg && dx, "kt_conv1d_bwd_data_tc: null pointer");
+  return conv1d_bwd_data_tc(d, dy, y, wimg, x, dx, ws, ws_floats, static_cast<cudaStream_t>(stream), true);
 }
 
 }  // namespace kt

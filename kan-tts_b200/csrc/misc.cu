@@ -76,8 +76,9 @@ __global__ void upsample_grad_reduce_kernel(const float* __restrict__ dxu, const
   }
 }
 
-int upsample_grad_reduce(const float* dxu, const float* x, int act, float slope, float* dx, long long rows, int up, int c,
-                         cudaStream_t st) {
+extern "C" int kt_upsample_grad_reduce(const float* dxu, const float* x, int32_t act, float slope, float* dx, int64_t rows,
+                                       int32_t up, int32_t c, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dxu && dx && rows > 0 && up >= 1 && c > 0 && (c & 3) == 0, "upsample_grad_reduce: bad arguments (C %% 4 == 0 required)");
   KT_REQUIRE(act == KT_ACT_NONE || (act == KT_ACT_LRELU && x), "upsample_grad_reduce: act must be NONE or LRELU (with x)");
   upsample_grad_reduce_kernel<<<stream_grid(rows * (c / 4), 256), 256, 0, st>>>(dxu, x, act, slope, dx, rows, up, c / 4);
@@ -200,21 +201,24 @@ __global__ void l1_sum_kernel(const float* __restrict__ a, const float* __restri
   }
 }
 
-int sinadd_fwd(const float* x, float* y, long long n, cudaStream_t st) {
+extern "C" int kt_sinadd_fwd(const float* x, float* y, int64_t n, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && y && n >= 0, "sinadd_fwd: bad arguments");
   if (n == 0) return KT_OK;
   sinadd_fwd_kernel<<<stream_grid(n / 4 + 1, 256), 256, 0, st>>>(x, y, n);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int sinadd_bwd(const float* x, const float* dy, float* dx, long long n, cudaStream_t st) {
+extern "C" int kt_sinadd_bwd(const float* x, const float* dy, float* dx, int64_t n, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && dy && dx && n >= 0, "sinadd_bwd: bad arguments");
   if (n == 0) return KT_OK;
   sinadd_bwd_kernel<<<stream_grid(n / 4 + 1, 256), 256, 0, st>>>(x, dy, dx, n);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int add3_scale(const float* a, const float* b, const float* c, float scale, float* y, long long n, cudaStream_t st) {
+extern "C" int kt_add3_scale(const float* a, const float* b, const float* c, float scale, float* y, int64_t n, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(a && y && n >= 0, "add3_scale: bad arguments");
   if (n == 0) return KT_OK;
   add3_scale_kernel<<<stream_grid(n / 4 + 1, 256), 256, 0, st>>>(a, b, c, scale, y, n);
@@ -274,7 +278,9 @@ __global__ void stream_reset_kernel(const KtWindow* __restrict__ wins, const uin
   for (int r = 0; r < w.history; ++r) col[(long long)r * w.channels] = 0.f;
 }
 
-int sinadd_fwd_win(const float* x, float* y, int batch, int rows, int ch, int x_pitch, int y_pitch, int y_first, cudaStream_t st) {
+extern "C" int kt_sinadd_fwd_win(const float* x, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t x_pitch,
+                                 int32_t y_pitch, int32_t y_first, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && y && batch > 0 && rows > 0 && ch > 0 && rows <= x_pitch && y_first >= 0 && y_first + rows <= y_pitch,
              "sinadd_fwd_win: bad arguments");
   const long long n = (long long)batch * rows * ch;
@@ -282,8 +288,9 @@ int sinadd_fwd_win(const float* x, float* y, int batch, int rows, int ch, int x_
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int add3_scale_win(const float* a, const float* b, const float* c, float scale, float* y, int batch, int rows, int ch, int x_pitch,
-                   int y_pitch, int y_first, cudaStream_t st) {
+extern "C" int kt_add3_scale_win(const float* a, const float* b, const float* c, float scale, float* y, int32_t batch,
+                                 int32_t rows, int32_t ch, int32_t x_pitch, int32_t y_pitch, int32_t y_first, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(a && y && batch > 0 && rows > 0 && ch > 0 && rows <= x_pitch && y_first >= 0 && y_first + rows <= y_pitch,
              "add3_scale_win: bad arguments");
   const long long n = (long long)batch * rows * ch;
@@ -291,7 +298,8 @@ int add3_scale_win(const float* a, const float* b, const float* c, float scale, 
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int stream_advance(const KtWindow* wins, int n, int batch, int frames, int max_c, cudaStream_t st) {
+extern "C" int kt_stream_advance(const KtWindow* wins, int32_t n, int32_t batch, int32_t frames, int32_t max_c, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(wins && n >= 0 && n <= 65535 && batch > 0 && batch <= 65535 && frames > 0 && max_c > 0,
              "stream_advance: bad arguments");
   if (n == 0) return KT_OK;
@@ -299,7 +307,9 @@ int stream_advance(const KtWindow* wins, int n, int batch, int frames, int max_c
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int stream_reset(const KtWindow* wins, int n, int batch, const uint8_t* slots, int max_c, cudaStream_t st) {
+extern "C" int kt_stream_reset(const KtWindow* wins, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_c,
+                               void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(wins && slots && n >= 0 && n <= 65535 && batch > 0 && batch <= 65535 && max_c > 0, "stream_reset: bad arguments");
   if (n == 0) return KT_OK;
   stream_reset_kernel<<<dim3(ceil_div(max_c, 128), n, batch), 128, 0, st>>>(wins, slots);
@@ -307,21 +317,23 @@ int stream_reset(const KtWindow* wins, int n, int batch, const uint8_t* slots, i
   return KT_OK;
 }
 
-int dwt_fwd(const float* x, float* y, int batch, int t, cudaStream_t st) {
+extern "C" int kt_dwt_db3_fwd(const float* x, float* y, int32_t batch, int32_t t, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && y && batch > 0 && t > 0, "dwt_fwd: bad arguments");
   const int t2 = (t + 5) / 2;
   dwt_fwd_kernel<<<stream_grid((long long)batch * t2, 256), 256, 0, st>>>(x, y, batch, t, t2);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int dwt_bwd(const float* dy, float* dx, int batch, int t, cudaStream_t st) {
+extern "C" int kt_dwt_db3_bwd(const float* dy, float* dx, int32_t batch, int32_t t, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dy && dx && batch > 0 && t > 0, "dwt_bwd: bad arguments");
   const int t2 = (t + 5) / 2;
   dwt_bwd_kernel<<<stream_grid((long long)batch * t, 256), 256, 0, st>>>(dy, dx, batch, t, t2);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-int l1_sum(const float* a, const float* b, long long n, float scale, float* out, cudaStream_t st, bool accumulate) {
+static int l1_sum(const float* a, const float* b, long long n, float scale, float* out, cudaStream_t st, bool accumulate) {
   KT_REQUIRE(a && b && out && n >= 0, "l1_sum: bad arguments");
   if (n == 0) {
     if (!accumulate) KT_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
@@ -336,6 +348,12 @@ int l1_sum(const float* a, const float* b, long long n, float scale, float* out,
   rc = split_sum(part, 1, blocks, 1, out, accumulate, st);
   if (rc) return rc;
   return scratch_free(part, st);
+}
+extern "C" int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, void* stream) {
+  return l1_sum(a, b, n, scale, out, static_cast<cudaStream_t>(stream), false);
+}
+extern "C" int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float* out, void* stream) {
+  return l1_sum(a, b, n, scale, out, static_cast<cudaStream_t>(stream), true);
 }
 
 }  // namespace kt

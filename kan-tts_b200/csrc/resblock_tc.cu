@@ -389,15 +389,18 @@ static RbPlan rb_plan(const KtResblockDesc* d) {
   return pl;
 }
 
-int resblock_plan(const KtResblockDesc* d) { return rb_plan(d).ok ? 1 : 0; }
+extern "C" int kt_resblock_plan(const KtResblockDesc* d) { return d && rb_plan(d).ok ? 1 : 0; }
 
-long long resblock_image_bytes(const KtResblockDesc* d) {
+extern "C" int64_t kt_resblock_image_bytes(const KtResblockDesc* d) {
+  if (!d) return 0;
   const RbPlan pl = rb_plan(d);
-  return pl.ok ? (long long)pl.p.nsteps * pl.p.tile_bytes : 0;
+  return pl.ok ? (int64_t)pl.p.nsteps * pl.p.tile_bytes : 0;
 }
 
 // w: fp32 kernel-layout weight [k][C][C] of one of the two convs (kt_weight_prepare's w_fwd)
-int resblock_pack(const KtResblockDesc* d, const float* w, void* img, cudaStream_t st) {
+extern "C" int kt_resblock_pack(const KtResblockDesc* d, const float* w, void* img, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(d, "kt_resblock_pack: null descriptor");
   const RbPlan pl = rb_plan(d);
   KT_REQUIRE(pl.ok && w && img, "resblock_pack: shape not supported by the fused kernel");
   if (pl.p.pair) {
@@ -411,12 +414,13 @@ int resblock_pack(const KtResblockDesc* d, const float* w, void* img, cudaStream
   KtConv1dDesc cd{};
   cd.batch = d->batch; cd.nsub = 1; cd.t_in = d->t; cd.t_out = d->t; cd.c_in = 64; cd.c_out = 64; cd.groups = 1;
   cd.kernel = d->kernel; cd.stride = 1; cd.dilation = 1; cd.pad_left = d->kernel - 1; cd.upsample = 1; cd.path = KT_PATH_TC;
-  int tc_pack_layer(const KtConv1dDesc*, int, const float*, void*, cudaStream_t);
   return tc_pack_layer(&cd, 0, w, img, st);
 }
 
-int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2, const float* b2,
-                 float* h, float* y, cudaStream_t st) {
+extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
+                               const float* b2, float* h, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(d, "kt_resblock_fwd: null descriptor");
   RbPlan pl = rb_plan(d);
   KT_REQUIRE(pl.ok, "resblock_fwd: shape not supported by the fused kernel (see kt_resblock_plan)");
   KT_REQUIRE(x && img1 && img2 && y, "resblock_fwd: null pointer");
@@ -437,6 +441,23 @@ int resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, cons
   else resblock_tc_kernel<64><<<grid, kRbThreads, pl.smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
+}
+
+extern "C" int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float* x, const float* h, const float* dy,
+                               const void* wimg1_bwd, const void* wimg2_bwd, float* dh, float* dx, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(d1 && d2 && x && h && dy && wimg1_bwd && wimg2_bwd && dh && dx, "kt_resblock_bwd: null pointer");
+  KT_REQUIRE(d1->act_in == KT_ACT_LRELU && d2->act_in == KT_ACT_LRELU && d1->act_out == KT_ACT_NONE && d2->act_out == KT_ACT_NONE &&
+                 d1->c_in == d1->c_out && d2->c_in == d2->c_out && d1->c_in == d2->c_in && d1->t_in == d2->t_in && d1->t_out == d1->t_in &&
+                 d2->t_out == d2->t_in && d1->batch == d2->batch && d1->nsub == 1 && d2->nsub == 1,
+             "kt_resblock_bwd: descriptors are not a (convs1[i], convs2[i]) pair of a ResidualBlock");
+  // dh = c2^T(dy) * lrelu'(h);  dx = c1^T(dh) * lrelu'(x) + dy   (the residual path, layers.py:219)
+  // (register-staged route: this entry point takes no workspace)
+  int rc = conv1d_bwd_data_tc(d2, dy, nullptr, wimg2_bwd, h, dh, nullptr, 0, st, false);
+  if (rc) return rc;
+  rc = conv1d_bwd_data_tc(d1, dh, nullptr, wimg1_bwd, x, dx, nullptr, 0, st, false);
+  if (rc) return rc;
+  return kt_add3_scale(dx, dy, nullptr, 1.f, dx, (int64_t)d1->batch * d1->t_in * d1->c_in, stream);
 }
 
 }  // namespace kt

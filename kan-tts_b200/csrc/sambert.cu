@@ -144,7 +144,7 @@ static int ln_grid(int rows, int warps_per_block) {
   return want < 1 ? 1 : (want > 148 * 2 ? 148 * 2 : want);
 }
 
-long long layernorm_bwd_workspace(int rows, int c) { return (long long)ln_grid(rows, 8) * 2 * c; }
+extern "C" int64_t kt_layernorm_bwd_workspace(int32_t rows, int32_t c) { return (int64_t)ln_grid(rows, 8) * 2 * c; }
 
 template <int NC>
 static int ln_fwd_launch(const float* x, const float* g, const float* b, float* y, float* mean, float* rstd, int rows,
@@ -155,8 +155,9 @@ static int ln_fwd_launch(const float* x, const float* g, const float* b, float* 
   return KT_OK;
 }
 
-int layernorm_fwd(const float* x, const float* gamma, const float* beta, float* y, float* mean, float* rstd, int rows,
-                  int c, float eps, cudaStream_t st) {
+extern "C" int kt_layernorm_fwd(const float* x, const float* gamma, const float* beta, float* y, float* mean, float* rstd,
+                                int32_t rows, int32_t c, float eps, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && gamma && beta && y && mean && rstd, "layernorm_fwd: null pointer");
   KT_REQUIRE(rows >= 0 && c >= 1 && c <= 1024, "layernorm_fwd: need 1 <= C <= 1024 (got %d)", c);
   if (rows == 0) return KT_OK;
@@ -178,9 +179,10 @@ static int ln_bwd_launch(const float* dy, const float* x, const float* g, const 
   return KT_OK;
 }
 
-int layernorm_bwd(const float* dy, const float* x, const float* gamma, const float* mean, const float* rstd, float* dx,
-                  float* dgamma, float* dbeta, float* workspace, long long workspace_floats, int rows, int c,
-                  cudaStream_t st) {
+extern "C" int kt_layernorm_bwd(const float* dy, const float* x, const float* gamma, const float* mean, const float* rstd,
+                                float* dx, float* dgamma, float* dbeta, float* workspace, int64_t workspace_floats, int32_t rows,
+                                int32_t c, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dy && x && gamma && mean && rstd && dx && dgamma && dbeta && workspace, "layernorm_bwd: null pointer");
   KT_REQUIRE(rows >= 1 && c >= 1 && c <= 1024, "layernorm_bwd: need rows >= 1, 1 <= C <= 1024");
   const int grid = ln_grid(rows, 8);
@@ -597,8 +599,9 @@ static int attn_fwd_launch(const KtAttnDesc* d, const AttnArgs& a, cudaStream_t 
   return KT_OK;
 }
 
-int attention_fwd(const KtAttnDesc* d, const float* q, const float* k, const float* v, const unsigned char* mask,
-                  const unsigned char* keep, float* out, float* probs, float* probs_dropped, cudaStream_t st) {
+extern "C" int kt_attention_fwd(const KtAttnDesc* d, const float* q, const float* k, const float* v, const uint8_t* mask,
+                                const uint8_t* keep, float* out, float* probs, float* probs_dropped, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = attn_check(d);
   if (rc) return rc;
   KT_REQUIRE(q && k && v && out && probs, "attention_fwd: null pointer");
@@ -635,9 +638,10 @@ static int attn_bwd_launch(const KtAttnDesc* d, const AttnBwdArgs& a, cudaStream
   return KT_OK;
 }
 
-int attention_bwd(const KtAttnDesc* d, const float* q, const float* k, const float* v, const float* probs,
-                  const unsigned char* keep, const float* dout, float* dq, float* dk, float* dv, float* delta,
-                  int accum_dq, cudaStream_t st) {
+extern "C" int kt_attention_bwd(const KtAttnDesc* d, const float* q, const float* k, const float* v, const float* probs,
+                                const uint8_t* keep, const float* dout, float* dq, float* dk, float* dv, float* delta,
+                                int32_t accum_dq, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = attn_check(d);
   if (rc) return rc;
   KT_REQUIRE(q && k && v && probs && dout && dq && dk && dv && delta, "attention_bwd: null pointer");
@@ -771,8 +775,8 @@ __global__ void __launch_bounds__(256) fsmn_bwd_weight_kernel(const float* __res
   }
 }
 
-long long fsmn_bwd_workspace(int B, int T, int C, int K) {
-  return (long long)B * ((T + kFsmnChunk - 1) / kFsmnChunk) * C * K;
+extern "C" int64_t kt_fsmn_bwd_workspace(int32_t B, int32_t T, int32_t C, int32_t K) {
+  return (int64_t)B * ((T + kFsmnChunk - 1) / kFsmnChunk) * C * K;
 }
 
 static int grid_for(long long n, int threads) {
@@ -792,10 +796,10 @@ static int fsmn_fir_launch(const float* x, const float* w, const unsigned char* 
   return KT_OK;
 }
 
-int fsmn_fwd(const float* x, const float* w, const unsigned char* mask, float* y, int B, int T, int C, int K, int lp,
-             cudaStream_t st) {
+extern "C" int kt_fsmn_fwd(const float* x, const float* w, const uint8_t* mask, float* y, int32_t B, int32_t T, int32_t C,
+                           int32_t K, int32_t lp, void* stream) {
   KT_REQUIRE(x && w && y && B >= 1 && T >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_fwd: bad arguments");
-  return fsmn_fir_launch(x, w, mask, y, B, T, C, K, lp, 0, st);
+  return fsmn_fir_launch(x, w, mask, y, B, T, C, K, lp, 0, static_cast<cudaStream_t>(stream));
 }
 
 template <int TJ>
@@ -808,8 +812,10 @@ static int fsmn_wgrad_launch(const float* x, const float* dy, const unsigned cha
   return KT_OK;
 }
 
-int fsmn_bwd(const float* x, const float* dy, const float* w, const unsigned char* mask, float* dx, float* dw,
-             float* workspace, long long workspace_floats, int B, int T, int C, int K, int lp, cudaStream_t st) {
+extern "C" int kt_fsmn_bwd(const float* x, const float* dy, const float* w, const uint8_t* mask, float* dx, float* dw,
+                           float* workspace, int64_t workspace_floats, int32_t B, int32_t T, int32_t C, int32_t K, int32_t lp,
+                           void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && dy && w && B >= 1 && T >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_bwd: bad arguments");
   if (dx) {
     int rc = fsmn_fir_launch(dy, w, mask, dx, B, T, C, K, K - 1 - lp, 1, st);
@@ -817,7 +823,7 @@ int fsmn_bwd(const float* x, const float* dy, const float* w, const unsigned cha
   }
   if (dw) {
     const int cpb = (T + kFsmnChunk - 1) / kFsmnChunk;
-    if (!workspace || workspace_floats < fsmn_bwd_workspace(B, T, C, K)) {
+    if (!workspace || workspace_floats < kt_fsmn_bwd_workspace(B, T, C, K)) {
       set_error("fsmn_bwd: workspace too small");
       return KT_ERR_WORKSPACE;
     }
@@ -870,15 +876,18 @@ __global__ void rows_gather_bwd_kernel(const float* __restrict__ dout, const int
   }
 }
 
-int rows_gather_fwd(const float* in, const int* idx, float* out, int B, int T_out, int T_in, int C, cudaStream_t st) {
+extern "C" int kt_rows_gather_fwd(const float* in, const int32_t* idx, float* out, int32_t B, int32_t T_out, int32_t T_in,
+                                  int32_t C, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(in && idx && out && B >= 1 && T_out >= 1 && T_in >= 1 && C >= 1, "rows_gather_fwd: bad arguments");
   rows_gather_fwd_kernel<<<grid_for((long long)B * T_out * C, 256), 256, 0, st>>>(in, idx, out, B, T_out, T_in, C);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
 
-int rows_gather_bwd(const float* dout, const int* idx, const int* start, const int* count, float* din, int B, int T_out,
-                    int T_in, int C, cudaStream_t st) {
+extern "C" int kt_rows_gather_bwd(const float* dout, const int32_t* idx, const int32_t* start, const int32_t* count, float* din,
+                                  int32_t B, int32_t T_out, int32_t T_in, int32_t C, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dout && idx && start && count && din && B >= 1 && T_out >= 1 && T_in >= 1 && C >= 1,
              "rows_gather_bwd: bad arguments");
   rows_gather_bwd_kernel<<<grid_for((long long)B * T_in * C, 256), 256, 0, st>>>(dout, idx, start, count, din, B, T_out,
@@ -1027,8 +1036,9 @@ __global__ void fp_insert_bwd_fp_reduce_kernel(const float* __restrict__ partial
   }
 }
 
-int fp_insert_plan(const void* labels, int label_bytes, const float* fp_p, const int* in_len, int B, int L, int T_cap,
-                   int* codes, int* rows, int* inter, cudaStream_t st) {
+extern "C" int kt_fp_insert_plan(const void* labels, int32_t label_bytes, const float* fp_p, const int32_t* in_len, int32_t B,
+                                 int32_t L, int32_t T_cap, int32_t* codes, int32_t* rows, int32_t* inter, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(in_len && codes && rows && inter && B >= 1 && L >= 1 && T_cap >= L, "fp_insert_plan: bad arguments");
   KT_REQUIRE(label_bytes ? (labels && (label_bytes == 4 || label_bytes == 8)) : (label_bytes == 0 && fp_p != nullptr),
              "fp_insert_plan: give int32 / int64 labels or the (B, L, 4) predictions");
@@ -1042,8 +1052,9 @@ static bool fp_vec4(int C, const void* a, const void* b, const void* c) {
   return C % 4 == 0 && ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
 }
 
-int fp_insert_fwd(const float* text, const float* fp_enc, const int* codes, float* out, int B, int L, int T_cap, int T_ins,
-                  int C, cudaStream_t st) {
+extern "C" int kt_fp_insert_fwd(const float* text, const float* fp_enc, const int32_t* codes, float* out, int32_t B, int32_t L,
+                                int32_t T_cap, int32_t T_ins, int32_t C, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(text && fp_enc && codes && out && B >= 1 && L >= 1 && C >= 1 && T_ins >= L && T_ins <= T_cap,
              "fp_insert_fwd: bad arguments");
   if (fp_vec4(C, text, fp_enc, out))
@@ -1056,8 +1067,10 @@ int fp_insert_fwd(const float* text, const float* fp_enc, const int* codes, floa
   return KT_OK;
 }
 
-int fp_insert_bwd(const float* dout, const int* codes, const int* rows, float* dtext, float* dfp, float* partial,
-                  long long partial_floats, int B, int L, int T_cap, int T_ins, int C, cudaStream_t st) {
+extern "C" int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* rows, float* dtext, float* dfp,
+                                float* partial, int64_t partial_floats, int32_t B, int32_t L, int32_t T_cap, int32_t T_ins,
+                                int32_t C, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dout && codes && rows && B >= 1 && L >= 1 && C >= 1 && T_ins >= L && T_ins <= T_cap,
              "fp_insert_bwd: bad arguments");
   KT_REQUIRE(!dfp || (partial && partial_floats >= 9LL * B * C), "fp_insert_bwd: partials need 9 * batch * c floats");
@@ -1169,9 +1182,11 @@ __global__ void ar_duration_kernel(const ArDurParams p) {
   }
 }
 
-int ar_duration_infer(const float* g0c, const float* w1, const float* b1, const float* w2t, const float* b2, const float* wih0t,
-                      const float* whh0t, const float* wih1t, const float* whh1t, const float* bias1, const float* fcw, float fcb,
-                      float* out, int B, int L, int H, int P1, int P2, cudaStream_t st) {
+extern "C" int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, const float* w2t, const float* b2,
+                                    const float* wih0t, const float* whh0t, const float* wih1t, const float* whh1t,
+                                    const float* bias1, const float* fcw, float fcb, float* out, int32_t B, int32_t L, int32_t H,
+                                    int32_t P1, int32_t P2, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(g0c && w1 && b1 && w2t && b2 && wih0t && whh0t && wih1t && whh1t && bias1 && fcw && out, "ar_duration_infer: null pointer");
   KT_REQUIRE(B >= 1 && L >= 1 && H >= 1 && H <= 256 && P1 >= 1 && P2 >= 1 && P1 <= 1024 && P2 <= 1024, "ar_duration_infer: bad sizes");
   ArDurParams p{g0c, w1, b1, w2t, b2, wih0t, whh0t, wih1t, whh1t, bias1, fcw, fcb, out, L, H, P1, P2};
@@ -1216,8 +1231,10 @@ __global__ void __launch_bounds__(256) fsmn_stream_kernel(const float* __restric
   }
 }
 
-int fsmn_fwd_stream(const KtStreamWin* win, const float* x, const float* w, const int* lengths, const float* resid, float* y,
-                    int B, int rows, int C, int K, int lp, int row0, cudaStream_t st) {
+extern "C" int kt_fsmn_fwd_stream(const KtStreamWin* win, const float* x, const float* w, const int32_t* lengths,
+                                  const float* resid, float* y, int32_t B, int32_t rows, int32_t C, int32_t K, int32_t lp,
+                                  int32_t row0, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(win && x && w && lengths && y, "fsmn_fwd_stream: null pointer");
   KT_REQUIRE(B >= 1 && B <= 65535 && rows >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_fwd_stream: bad sizes");
   KT_REQUIRE(win->in_first >= K - 1 && win->in_first + rows <= win->in_pitch,
@@ -1267,8 +1284,9 @@ __global__ void lstm_stream_kernel(const float* __restrict__ gx, const float* __
   for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
 }
 
-int lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int B, int rows, int H, int gx_pitch, int h_pitch,
-                cudaStream_t st) {
+extern "C" int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t B, int32_t rows, int32_t H,
+                              int32_t gx_pitch, int32_t h_pitch, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(gx && whh_t && state && h, "lstm_stream: null pointer");
   KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream: bad sizes");
   const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);

@@ -187,8 +187,9 @@ static int fill(MelParams& p, const KtMelDesc* d) {
   return KT_OK;
 }
 
-int stft_mel_fwd(const KtMelDesc* d, const float* wav, const float* window, const float* melmat, float* mel,
-                 float* amp, float* spec, cudaStream_t st) {
+extern "C" int kt_stft_mel_fwd(const KtMelDesc* d, const float* wav, const float* window, const float* melmat, float* mel,
+                               float* amp, float* spec, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   MelParams p;
   int rc = fill(p, d);
   if (rc) return rc;
@@ -200,8 +201,9 @@ int stft_mel_fwd(const KtMelDesc* d, const float* wav, const float* window, cons
   return KT_OK;
 }
 
-int stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, const float* spec, const float* window,
-                 const float* melmat, float* dwav, cudaStream_t st) {
+extern "C" int kt_stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, const float* spec, const float* window,
+                               const float* melmat, float* dwav, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   MelParams p;
   int rc = fill(p, d);
   if (rc) return rc;

@@ -282,9 +282,10 @@ static bool weight_tiled_plan(int d0, int d1, int k, int& nblk, int& nsl, int& b
   return true;
 }
 
-int weight_prepare(const float* v, const float* g, const float* inv_sigma, int mode, int d0, int d1, int k,
-                   int transposed, int groups, float* w_fwd, float* w_bwd, float* norm_out, float* w_ref,
-                   cudaStream_t st) {
+extern "C" int kt_weight_prepare(const float* v, const float* g, const float* inv_sigma, int32_t mode, int32_t d0, int32_t d1,
+                                 int32_t k, int32_t transposed, int32_t groups, float* w_fwd, float* w_bwd, float* norm_out,
+                                 float* w_ref, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(v && d0 > 0 && d1 > 0 && k > 0 && groups > 0, "weight_prepare: bad arguments");
   KT_REQUIRE(mode == 0 || (mode == 1 && g && norm_out), "weight_prepare: mode 1 needs g and norm_out");
   KT_REQUIRE(!transposed || groups == 1, "weight_prepare: transposed conv must have groups == 1");
@@ -299,9 +300,9 @@ int weight_prepare(const float* v, const float* g, const float* inv_sigma, int m
   return KT_OK;
 }
 
-int weight_grad(const float* dw, const float* v, const float* g, const float* norm, const float* inv_sigma,
-                int mode, int d0, int d1, int k, int transposed, int groups, float* dv, float* dg, int accumulate,
-                const float* dbias_src, float* dbias_dst, int nbias, cudaStream_t st) {
+static int weight_grad(const float* dw, const float* v, const float* g, const float* norm, const float* inv_sigma,
+                       int mode, int d0, int d1, int k, int transposed, int groups, float* dv, float* dg, int accumulate,
+                       const float* dbias_src, float* dbias_dst, int nbias, cudaStream_t st) {
   KT_REQUIRE(dw && v && dv && d0 > 0 && d1 > 0 && k > 0 && groups > 0, "weight_grad: bad arguments");
   KT_REQUIRE(mode == 0 || (mode == 1 && g && norm && dg), "weight_grad: mode 1 needs g, norm, dg");
   WLayout L{d0, d1, k, transposed, groups};
@@ -315,6 +316,21 @@ int weight_grad(const float* dw, const float* v, const float* g, const float* no
   }
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
+}
+
+extern "C" int kt_weight_grad(const float* dw_fwd, const float* v, const float* g, const float* norm, const float* inv_sigma,
+                              int32_t mode, int32_t d0, int32_t d1, int32_t k, int32_t transposed, int32_t groups, float* dv,
+                              float* dg, void* stream) {
+  return weight_grad(dw_fwd, v, g, norm, inv_sigma, mode, d0, d1, k, transposed, groups, dv, dg, 0, nullptr, nullptr, 0,
+                     static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kt_weight_grad_accum(const float* dw_fwd, const float* v, const float* g, const float* norm, const float* inv_sigma,
+                                    int32_t mode, int32_t d0, int32_t d1, int32_t k, int32_t transposed, int32_t groups,
+                                    float* dv, float* dg, const float* dbias_src, float* dbias_dst, int32_t nbias,
+                                    void* stream) {
+  return weight_grad(dw_fwd, v, g, norm, inv_sigma, mode, d0, d1, k, transposed, groups, dv, dg, 1, dbias_src, dbias_dst, nbias,
+                     static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace kt

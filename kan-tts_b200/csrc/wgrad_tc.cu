@@ -420,8 +420,6 @@ struct WgPlan {
   long long planes_a_off, planes_b_off;   // TMA route: offsets (floats) of the operand planes inside the workspace
 };
 
-Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up);   // conv_ffma.cu
-
 // bytes of one ring stage: the hi / lo planes of the A images (rows_a rows) and of the B images (rows_b rows)
 static size_t wg_stage_bytes(const WgTcParams& p, int rows_a, int rows_b) {
   return 2 * ((size_t)p.a_groups * rows_a * 128 + (size_t)p.b_groups * rows_b * 128);
@@ -565,29 +563,33 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool plan_only = false) {
 // development / test aid (kt_debug_wgrad_plan): the plan of a layer as it would be made on a GPU box
 // out = {ok, tma, tt, R, Rp, nstages, smem bytes, nsplit, NT, unit groups, a_box_t, rows_a_p} (TMA-only entries 0 on the
 // register-staged route)
-void debug_wgrad_plan(const KtConv1dDesc* d, int* out) {
+extern "C" int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out) {
+  KT_REQUIRE(d && out, "kt_debug_wgrad_plan: null pointer");
   const WgPlan pl = make_plan(d, true);
   out[0] = pl.ok; out[1] = pl.tma; out[2] = pl.x.tt; out[3] = pl.x.R; out[4] = pl.x.Rp; out[5] = pl.x.nstages;
   out[6] = (int)pl.smem; out[7] = pl.p.nsplit; out[8] = pl.p.NT; out[9] = pl.p.ngroups;
   out[10] = pl.x.a_box_t; out[11] = pl.x.rows_a_p;
+  return KT_OK;
 }
 
-// floats of workspace needed by conv1d_bwd_weight_tc (0 = layer not supported)
-bool thin_cin1_ok(const KtConv1dDesc* d);   // thin.cu
-
-long long wgrad_tc_workspace(const KtConv1dDesc* d) {
+// floats of workspace needed by kt_conv1d_bwd_weight_tc (0 = layer not supported)
+extern "C" int64_t kt_conv1d_bwd_weight_tc_workspace(const KtConv1dDesc* d) {
+  if (validate_conv(d)) return 0;
   if (d->path != KT_PATH_TC && thin_cin1_ok(d)) return 0;   // waveform-input layers: thin.cu
   const WgPlan pl = make_plan(d);
   return pl.ok ? pl.ws_floats : 0;
 }
 
-int colsum_bias(const Side& s, long long rows, int c, float* out, cudaStream_t st);  // conv_ffma.cu
-
-int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw,
-                         float* dbias, float* ws, long long ws_floats, cudaStream_t st) {
+extern "C" int kt_conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw,
+                                       float* dbias, float* ws, int64_t ws_floats, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_conv(d);
+  if (rc) return rc;
+  KT_REQUIRE(x && dy && dw, "kt_conv1d_bwd_weight_tc: null pointer");
   WgPlan pl = make_plan(d);
   KT_REQUIRE(pl.ok, "conv1d_bwd_weight_tc: layer not supported by the tensor-core path");
-  KT_REQUIRE(ws && ws_floats >= pl.ws_floats, "conv1d_bwd_weight_tc: workspace too small (%lld < %lld floats)", ws_floats, pl.ws_floats);
+  KT_REQUIRE(ws && ws_floats >= pl.ws_floats, "conv1d_bwd_weight_tc: workspace too small (%lld < %lld floats)", (long long)ws_floats,
+             pl.ws_floats);
   KT_REQUIRE(d->act_out == KT_ACT_NONE || y != nullptr, "bwd_weight: y required when act_out != NONE");
   WgTcParams& p = pl.p;
   const Side sx = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
@@ -603,7 +605,7 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
     KT_CHECK_CUDA(split_planes(p.a, na, pa, p.b, nb, pb, st));
-    int rc = encode_plane_map(&x.map_b, pb, p.batch, p.t_b, p.nsub, p.cb, 1, 0, 64, x.tt, "conv1d_bwd_weight_tc (operand B)");
+    rc = encode_plane_map(&x.map_b, pb, p.batch, p.t_b, p.nsub, p.cb, 1, 0, 64, x.tt, "conv1d_bwd_weight_tc (operand B)");
     for (int rho = 0; rc == KT_OK && rho < p.step; ++rho)
       rc = encode_plane_map(&x.map_a[rho], pa, p.batch, p.t_a, p.nsub, p.ca, p.step, rho, 64, x.a_box_t, "conv1d_bwd_weight_tc (operand A)");
     if (rc) return rc;
@@ -629,7 +631,7 @@ int conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy,
   KT_CHECK_CUDA(cudaGetLastError());
   if (dbias) {
     const long long rows = (long long)d->batch * d->nsub * d->t_out;
-    int rc = colsum_bias(sdy, rows, d->c_out, dbias, st);
+    rc = colsum_bias(sdy, rows, d->c_out, dbias, st);
     if (rc) return rc;
   }
   return KT_OK;

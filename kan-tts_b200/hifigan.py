@@ -22,8 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from . import _lib
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, check, ptr, stream_ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, ptr
 from .stream import Windows, WindowTable, own_weight
 
 # --------------------------------------------------------------------------------------------
@@ -572,7 +571,7 @@ class GeneratorStreamer:
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
         win = self._win
-        lib, b, B = _lib.load(), win.buf, self.batch
+        b, B = win.buf, self.batch
         cur = torch.cuda.current_stream()
         forked = False
         for st, place in zip(self.plan.steps, self._places):
@@ -588,16 +587,13 @@ class GeneratorStreamer:
                                     None if st.resid is None else b[st.resid])
             elif type(st) is SinStep:
                 src, dst = b[st.src], b[st.dst]
-                check(lib.kt_sinadd_fwd_win(ptr(src), ptr(dst), B, f * win.rate[st.src], src.shape[2], src.shape[1],
-                                            dst.shape[1], win.first[st.dst], stream_ptr()), "kt_sinadd_fwd_win")
-                ops._count()
+                ops.call("kt_sinadd_fwd_win", ptr(src), ptr(dst), B, f * win.rate[st.src], src.shape[2], src.shape[1],
+                         dst.shape[1], win.first[st.dst])
             else:
                 dst = b[st.dst]
                 srcs = [b[s] for s in st.srcs] + [None] * (3 - len(st.srcs))
-                check(lib.kt_add3_scale_win(ptr(srcs[0]), ptr(srcs[1]), ptr(srcs[2]), st.scale, ptr(dst), B,
-                                            f * win.rate[st.dst], dst.shape[2], srcs[0].shape[1], dst.shape[1],
-                                            win.first[st.dst], stream_ptr()), "kt_add3_scale_win")
-                ops._count()
+                ops.call("kt_add3_scale_win", ptr(srcs[0]), ptr(srcs[1]), ptr(srcs[2]), st.scale, ptr(dst), B,
+                         f * win.rate[st.dst], dst.shape[2], srcs[0].shape[1], dst.shape[1], win.first[st.dst])
         win.advance(f)
 
     def push(self, mel):

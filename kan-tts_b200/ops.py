@@ -26,6 +26,17 @@ def _count(n=1):
     _launches += n
 
 
+def call(fn, *args, launches=1):
+    """Call entry point ``fn`` of the library with ``args`` and the calling thread's current stream (every launching entry
+    point takes its stream last), raise on a failed return code, and count ``launches`` kernel launches.  Eager steps make
+    thousands of these calls from the host, so the success path makes no further Python call."""
+    global _launches
+    rc = getattr(_lib.load(), fn)(*args, stream_ptr())
+    if rc:
+        check(rc, fn)
+    _launches += launches
+
+
 class _Profiler:
     """Optional per-call CUDA-event timing (bench.py's roofline leg): each instrumented library call
     is bracketed by two events on the launching stream and tagged with its algorithmic work."""
@@ -74,16 +85,15 @@ def _sig(spec, d):
 
 
 def _run(name, spec, d, launches, tc, *calls):
-    """Make the library calls ``(entry point, *args)`` as one unit of kernel class ``name``: timed by the profiler
-    (when on) against the work of layer ``spec`` at descriptor ``d``, each checked, and counted as ``launches``
-    kernel launches, ``tc`` of them on the tensor cores."""
+    """Make the library calls ``(entry point, *args)`` through ``call`` as one unit of kernel class ``name``: timed by the
+    profiler (when on) against the work of layer ``spec`` at descriptor ``d``, and counted as ``launches`` kernel
+    launches, ``tc`` of them on the tensor cores."""
     global _tc_launches
-    lib = _lib.load()
     if _profiler is not None:
         e0 = torch.cuda.Event(enable_timing=True)
         e0.record()
     for fn, *args in calls:
-        check(getattr(lib, fn)(*args), fn)
+        call(fn, *args, launches=0)
     if _profiler is not None:
         e1 = torch.cuda.Event(enable_timing=True)
         e1.record()
@@ -234,11 +244,10 @@ class PreparedWeight:
             self.img[key] = img
         img, d = img
         if rb:
-            check(lib.kt_resblock_pack(ctypes.byref(d), ptr(self.w_fwd), ptr(img, True), stream_ptr()), "kt_resblock_pack")
+            call("kt_resblock_pack", ctypes.byref(d), ptr(self.w_fwd), ptr(img, True))
         else:
             src = self.w_fwd if key[0] == 0 else self.w_bwd
-            check(lib.kt_weight_pack_tc(ctypes.byref(d), key[0], ptr(src), ptr(img, True), stream_ptr()), "kt_weight_pack_tc")
-        _count()
+            call("kt_weight_pack_tc", ctypes.byref(d), key[0], ptr(src), ptr(img, True))
         self.img_stale.discard(key)
         return img
 
@@ -266,7 +275,6 @@ def prepare_weight(cache, spec, v, g):
            None if g is None else (g.data_ptr(), g._version, getattr(g, "_kt_epoch", 0))) if cacheable else None
     if key is not None and cache.key == key and cache.w_fwd is not None and cache.w_fwd.device == v.device:
         return cache
-    lib = _lib.load()
     d0 = v.shape[0]
     d1 = v.shape[1]
     k = spec.kernel
@@ -285,10 +293,8 @@ def prepare_weight(cache, spec, v, g):
         cache.norm = torch.empty(d0, device=v.device, dtype=torch.float32) if mode else None
         cache.img = {}
     gd = None if g is None else g.detach().contiguous()
-    check(lib.kt_weight_prepare(ptr(vd), ptr(gd), None, mode, d0, d1, k, int(spec.transposed), spec.groups,
-                                ptr(cache.w_fwd), ptr(cache.w_bwd), ptr(cache.norm), None, stream_ptr()),
-          "kt_weight_prepare")
-    _count()
+    call("kt_weight_prepare", ptr(vd), ptr(gd), None, mode, d0, d1, k, int(spec.transposed), spec.groups, ptr(cache.w_fwd),
+         ptr(cache.w_bwd), ptr(cache.norm), None)
     cache.key = key
     cache.img_stale = set(cache.img)      # packed tensor-core tiles are re-packed (in place) on next use
     return cache
@@ -411,13 +417,11 @@ def _weight_backward(spec, plan, x_, dy, y_, v, g, params, norm, need_v, need_g,
     need_w = need_v or need_g
     if not (need_w or need_b):
         return dbias, dv, dg
-    lib = _lib.load()
     has_g = g is not None
     pv, pg, pb = params
     direct = (need_w and pv.is_leaf and _is_direct(pv) and _is_direct(pg) and (not need_b or _is_direct(pb))
               and need_v and (not has_g or need_g))
     side = _wgrad_stream(x_.device, pv) if (direct and _WGRAD_ASYNC) else None
-    st = stream_ptr()
     if side is not None:
         # nothing of this chain is handed back to autograd (the kernels accumulate into param.grad), so it
         # runs on a side stream; join_wgrad_streams() orders it before the optimizer
@@ -427,7 +431,6 @@ def _weight_backward(spec, plan, x_, dy, y_, v, g, params, norm, need_v, need_g,
                 t.record_stream(side)
         cm = torch.cuda.stream(side)
         cm.__enter__()
-        st = stream_ptr()
     try:
         dw = torch.empty(spec.w_numel, device=x_.device, dtype=torch.float32)
         if need_b:
@@ -436,31 +439,26 @@ def _weight_backward(spec, plan, x_, dy, y_, v, g, params, norm, need_v, need_g,
         if ws_floats:
             ws = torch.empty(ws_floats, device=x_.device, dtype=torch.float32)
             _run("conv_wgrad_tc", spec, d, n, 1, ("kt_conv1d_bwd_weight_tc", ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_),
-                                                  ptr(dw), ptr(dbias), ptr(ws), ws_floats, st))
+                                                  ptr(dw), ptr(dbias), ptr(ws), ws_floats))
         else:
             _run("conv_wgrad_ffma", spec, d, n, 0, ("kt_conv1d_bwd_weight", ctypes.byref(d), ptr(x_), ptr(dy), ptr(y_),
-                                                    ptr(dw), ptr(dbias), st))
+                                                    ptr(dw), ptr(dbias)))
         if need_w:
             vd = v.detach().contiguous()
             gd = None if g is None else g.detach().contiguous()
             mode = 1 if has_g else 0
             if direct:
                 # AccumulateGrad folded into the kernel: param.grad += (train.FlatGrads buffers, pre-zeroed)
-                check(lib.kt_weight_grad_accum(ptr(dw), ptr(vd), ptr(gd), ptr(norm), None, mode, vd.shape[0],
-                                               vd.shape[1], spec.kernel, int(spec.transposed), spec.groups,
-                                               ptr(pv.grad), None if pg is None else ptr(pg.grad),
-                                               ptr(dbias) if need_b else None,
-                                               ptr(pb.grad) if need_b else None, spec.c_out if need_b else 0, st),
-                      "kt_weight_grad_accum")
+                call("kt_weight_grad_accum", ptr(dw), ptr(vd), ptr(gd), ptr(norm), None, mode, vd.shape[0], vd.shape[1],
+                     spec.kernel, int(spec.transposed), spec.groups, ptr(pv.grad), None if pg is None else ptr(pg.grad),
+                     ptr(dbias) if need_b else None, ptr(pb.grad) if need_b else None, spec.c_out if need_b else 0)
                 dbias = None
             else:
                 dv = torch.empty_like(vd)
                 if has_g:
                     dg = torch.empty_like(g)
-                check(lib.kt_weight_grad(ptr(dw), ptr(vd), ptr(gd), ptr(norm), None, mode, vd.shape[0],
-                                         vd.shape[1], spec.kernel, int(spec.transposed), spec.groups, ptr(dv),
-                                         ptr(dg), st), "kt_weight_grad")
-            _count()
+                call("kt_weight_grad", ptr(dw), ptr(vd), ptr(gd), ptr(norm), None, mode, vd.shape[0], vd.shape[1],
+                     spec.kernel, int(spec.transposed), spec.groups, ptr(dv), ptr(dg))
     finally:
         if side is not None:
             cm.__exit__(None, None, None)
@@ -505,10 +503,10 @@ class ConvFn(torch.autograd.Function):
             img = pw.image((0, nt), d)
             ws = _workspace(run.ws_fwd, x.device)
             _run("conv_fwd_tc", spec, d, n + (ws is not None), n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True),
-                                                                   ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd, stream_ptr()))
+                                                                   ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd))
         else:
             _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd", ctypes.byref(d), ptr(x), ptr(pw.w_fwd), ptr(bd),
-                                                  ptr(resid), ptr(y), stream_ptr()))
+                                                  ptr(resid), ptr(y)))
         pw.conv_used = True
         nb = B if _grad_items is None else min(_grad_items, B)     # batch items that carry gradient
         ctx.spec, ctx.nb = spec, nb
@@ -527,7 +525,6 @@ class ConvFn(torch.autograd.Function):
         spec, plan = ctx.spec, ctx.plan
         d = plan.d
         dy = dy.contiguous()
-        st = stream_ptr()
         dx = dres = dbias = dv = dg = None
         dy_full = dy
         if ctx.nb < x.shape[0]:          # grad_items: only the leading items carry gradient (contiguous slices)
@@ -542,21 +539,21 @@ class ConvFn(torch.autograd.Function):
             # there without grad, and its data gradient then runs on the exact kernel
             if ctx.img_bwd is None:
                 _run("conv_dgrad_ffma", spec, d, n, 0, ("kt_conv1d_bwd_data", ctypes.byref(d), ptr(dy), ptr(y_),
-                                                        ptr(ctx.w_bwd), ptr(x_), ptr(dx), st))
+                                                        ptr(ctx.w_bwd), ptr(x_), ptr(dx)))
             elif plan.up_bwd:
                 d2 = plan.d_bwd
                 dxu = torch.empty((ctx.nb, d2.t_in * d2.nsub, spec.c_in), device=x.device, dtype=torch.float32)
                 ws = _workspace(plan.ws_bwd, x.device)
                 _run("conv_dgrad_tc", spec, d, n + 1 + (ws is not None), 1,
                      ("kt_conv1d_bwd_data_tc", ctypes.byref(d2), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), None, ptr(dxu),
-                      ptr(ws), plan.ws_bwd, st),
+                      ptr(ws), plan.ws_bwd),
                      ("kt_upsample_grad_reduce", ptr(dxu), ptr(x_), spec.act_in, spec.act_in_slope, ptr(dx),
-                      ctx.nb * d.t_in * d.nsub, spec.upsample, spec.c_in, st))
+                      ctx.nb * d.t_in * d.nsub, spec.upsample, spec.c_in))
             else:
                 ws = _workspace(plan.ws_bwd, x.device)
                 _run("conv_dgrad_tc", spec, d, n + (ws is not None), 1,
                      ("kt_conv1d_bwd_data_tc", ctypes.byref(d), ptr(dy), ptr(y_), ptr(ctx.img_bwd, True), ptr(x_), ptr(dx),
-                      ptr(ws), plan.ws_bwd, st))
+                      ptr(ws), plan.ws_bwd))
         if ctx.has_resid and ctx.needs_input_grad[1]:
             # NOT the incoming tensor itself: the autograd engine accumulates gradients arriving at the same input IN PLACE
             # into the first arrival when it holds the last reference (input_buffer.cpp: can_accumulate_inplace), and
@@ -584,11 +581,11 @@ def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None):
     if nt:
         img = pw.image((0, nt), d)
         _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(img, True),
-                                            ptr(bias), ptr(resid), ptr(y), stream_ptr()))
+                                            ptr(bias), ptr(resid), ptr(y)))
     else:
         n = spec.stride if spec.transposed else 1
         _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(pw.w_fwd),
-                                              ptr(bias), ptr(resid), ptr(y), stream_ptr()))
+                                              ptr(bias), ptr(resid), ptr(y)))
 
 
 # ---- pair_reuse: one (generated, real) pair batch per phase, the real half computed once per step -----------------------
@@ -674,7 +671,7 @@ class ResblockFn(torch.autograd.Function):
         h = torch.empty_like(x) if need_grad else None
         _run("resblock_fwd_tc", spec1, spec1.plan(B, 1, T).d, 1, 1,
              ("kt_resblock_fwd", ctypes.byref(rd), ptr(x), ptr(img1, True), ptr(None if b1 is None else b1.detach()),
-              ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h), ptr(y), stream_ptr()))
+              ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h), ptr(y)))
         if need_grad:
             nb = B if _grad_items is None else min(_grad_items, B)
             p1, p2 = spec1.plan(nb, 1, T), spec2.plan(nb, 1, T)
@@ -702,7 +699,7 @@ class ResblockFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         _run("conv_dgrad_tc", spec1, p1.d, 3, 2,
              ("kt_resblock_bwd", ctypes.byref(p1.d), ctypes.byref(p2.d), ptr(x_), ptr(h_), ptr(dy), ptr(ctx.img_bwd[0], True),
-              ptr(ctx.img_bwd[1], True), ptr(dh), ptr(dx if ctx.nb == x.shape[0] else dx[:ctx.nb]), stream_ptr()))
+              ptr(ctx.img_bwd[1], True), ptr(dh), ptr(dx if ctx.nb == x.shape[0] else dx[:ctx.nb])))
         ni = ctx.needs_input_grad
         (pv1, pg1, pb1), (pv2, pg2, pb2) = ctx.params
         db2, dv2, dg2 = _weight_backward(spec2, p2, h_, dy, None, v2, g2, (pv2, pg2, pb2), ctx.norms[1], ni[5],
@@ -723,8 +720,7 @@ class SinAddFn(torch.autograd.Function):
     def forward(ctx, x):
         x = x.contiguous()
         y = torch.empty_like(x)
-        check(_lib.load().kt_sinadd_fwd(ptr(x), ptr(y), x.numel(), stream_ptr()), "kt_sinadd_fwd")
-        _count()
+        call("kt_sinadd_fwd", ptr(x), ptr(y), x.numel())
         ctx.save_for_backward(x)
         return y
 
@@ -733,8 +729,7 @@ class SinAddFn(torch.autograd.Function):
         x, = ctx.saved_tensors
         dy = dy.contiguous()
         dx = torch.empty_like(x)
-        check(_lib.load().kt_sinadd_bwd(ptr(x), ptr(dy), ptr(dx), x.numel(), stream_ptr()), "kt_sinadd_bwd")
-        _count()
+        call("kt_sinadd_bwd", ptr(x), ptr(dy), ptr(dx), x.numel())
         return dx
 
 
@@ -747,9 +742,7 @@ class Mean3Fn(torch.autograd.Function):
         b = None if b is None else b.contiguous()
         c = None if c is None else c.contiguous()
         y = torch.empty_like(a)
-        check(_lib.load().kt_add3_scale(ptr(a), ptr(b), ptr(c), float(scale), ptr(y), a.numel(), stream_ptr()),
-              "kt_add3_scale")
-        _count()
+        call("kt_add3_scale", ptr(a), ptr(b), ptr(c), float(scale), ptr(y), a.numel())
         ctx.scale, ctx.nb, ctx.nc = scale, b is not None, c is not None
         return y
 
@@ -757,9 +750,7 @@ class Mean3Fn(torch.autograd.Function):
     def backward(ctx, dy):
         dy = dy.contiguous()
         g = torch.empty_like(dy)
-        check(_lib.load().kt_add3_scale(ptr(dy), None, None, float(ctx.scale), ptr(g), dy.numel(), stream_ptr()),
-              "kt_add3_scale")
-        _count()
+        call("kt_add3_scale", ptr(dy), None, None, float(ctx.scale), ptr(g), dy.numel())
         return None, g, (g if ctx.nb else None), (g if ctx.nc else None)
 
 
@@ -771,8 +762,7 @@ class DwtFn(torch.autograd.Function):
         x = x.contiguous()
         B, T = x.shape
         y = torch.empty(B, (T + 5) // 2, 2, device=x.device, dtype=torch.float32)
-        check(_lib.load().kt_dwt_db3_fwd(ptr(x), ptr(y), B, T, stream_ptr()), "kt_dwt_db3_fwd")
-        _count()
+        call("kt_dwt_db3_fwd", ptr(x), ptr(y), B, T)
         ctx.shape = (B, T)
         return y
 
@@ -781,8 +771,7 @@ class DwtFn(torch.autograd.Function):
         B, T = ctx.shape
         dy = dy.contiguous()
         dx = torch.empty(B, T, device=dy.device, dtype=torch.float32)
-        check(_lib.load().kt_dwt_db3_bwd(ptr(dy), ptr(dx), B, T, stream_ptr()), "kt_dwt_db3_bwd")
-        _count()
+        call("kt_dwt_db3_bwd", ptr(dy), ptr(dx), B, T)
         return dx
 
 
@@ -807,9 +796,7 @@ class StftMelFn(torch.autograd.Function):
             mel = torch.empty(B, n_mels, frames, device=wav.device, dtype=torch.float32)
         else:
             amp = torch.empty(B, frames, nb, device=wav.device, dtype=torch.float32)
-        check(_lib.load().kt_stft_mel_fwd(ctypes.byref(d), ptr(wav), ptr(window), ptr(melmat), ptr(mel), ptr(amp),
-                                         ptr(spec), stream_ptr()), "kt_stft_mel_fwd")
-        _count()
+        call("kt_stft_mel_fwd", ctypes.byref(d), ptr(wav), ptr(window), ptr(melmat), ptr(mel), ptr(amp), ptr(spec))
         ctx.d = d
         ctx.is_mel = melmat is not None
         ctx.save_for_backward(spec, window, melmat)
@@ -822,23 +809,20 @@ class StftMelFn(torch.autograd.Function):
         dout = dout.contiguous()
         dwav = torch.empty(d.batch, d.t, device=dout.device, dtype=torch.float32)
         dmel, damp = (dout, None) if ctx.is_mel else (None, dout)
-        check(_lib.load().kt_stft_mel_bwd(ctypes.byref(d), ptr(dmel), ptr(damp), ptr(spec), ptr(window), ptr(melmat),
-                                         ptr(dwav), stream_ptr()), "kt_stft_mel_bwd")
-        _count(2)
+        call("kt_stft_mel_bwd", ctypes.byref(d), ptr(dmel), ptr(damp), ptr(spec), ptr(window), ptr(melmat), ptr(dwav),
+             launches=2)
         return dwav, None, None, None, None, None, None, None
 
 
 def l1_sum_acc(out, a, b, scale):
     """out += scale * sum|a - b| (0-dim device accumulator zeroed by the caller; one launch)."""
     a, b = a.contiguous(), b.contiguous()
-    check(_lib.load().kt_l1_sum_acc(ptr(a), ptr(b), a.numel(), float(scale), ptr(out), stream_ptr()), "kt_l1_sum_acc")
-    _count()
+    call("kt_l1_sum_acc", ptr(a), ptr(b), a.numel(), float(scale), ptr(out))
 
 
 def l1_sum(a, b, scale=1.0):
     """scale * sum|a - b| -> 0-dim tensor (no autograd; feature-matching value, loss.py:249)."""
     a, b = a.contiguous(), b.contiguous()
     out = torch.empty((), device=a.device, dtype=torch.float32)
-    check(_lib.load().kt_l1_sum(ptr(a), ptr(b), a.numel(), float(scale), ptr(out), stream_ptr()), "kt_l1_sum")
-    _count(2)
+    call("kt_l1_sum", ptr(a), ptr(b), a.numel(), float(scale), ptr(out), launches=2)
     return out

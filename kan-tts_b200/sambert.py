@@ -31,7 +31,7 @@ import torch.nn.functional as F
 
 from . import ops
 from . import sambert_ops as sops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, check, load, ptr, stream_ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, ptr
 from .stream import Windows, WindowTable, own_weight
 
 
@@ -468,9 +468,8 @@ class VarRnnARPredictor(nn.Module):
             args = (g0c, fc1.weight.detach()[:, 0].contiguous(), fc1.bias.detach(), t(fc2.weight), fc2.bias.detach(),
                     t(w_ih0[:, :P2]), t(lstm.weight_hh_l0), t(lstm.weight_ih_l1), t(lstm.weight_hh_l1),
                     (lstm.bias_ih_l1 + lstm.bias_hh_l1).detach().contiguous(), self.fc.weight.detach()[0].contiguous())
-            check(load().kt_ar_duration_infer(*[ptr(a) for a in args], float(self.fc.bias.detach()[0]), ptr(out), B, L, H, P1, P2,
-                                              stream_ptr()), "kt_ar_duration_infer")
-            ops._count(2)
+            ops.call("kt_ar_duration_infer", *[ptr(a) for a in args], float(self.fc.bias.detach()[0]), ptr(out), B, L, H, P1, P2,
+                     launches=2)
         if masks is not None:
             out = out.masked_fill(masks, 0.0)
         return out
@@ -868,7 +867,7 @@ class PostNetStreamer:
 
     def _chunk(self, f):
         """Every launch of one chunk of f decoder rows (already in the "dec" window) -> the final output rows."""
-        lib, b, B, a = load(), self._win.buf, self.batch, self._rows
+        b, B, a = self._win.buf, self.batch, self._rows
         first = a - self.delay                      # frame of the chunk's first output row
         skip = max(0, -first)                       # output rows before frame 0 are not rows of the utterance
         n = f - skip
@@ -883,14 +882,11 @@ class PostNetStreamer:
                 ops.stream_conv(spec, pw, bias, src, dst, rows, place, resid)
             elif st.kind == "fsmn":
                 layer = self.plan.layers[st.layer]
-                check(lib.kt_fsmn_fwd_stream(ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True), ptr(resid),
-                                             ptr(dst), B, rows, src.shape[2], layer["kernel"], layer["lp"],
-                                             a - layer["lag"] - layer["rp"], stream_ptr()), "kt_fsmn_fwd_stream")
-                ops._count()
+                ops.call("kt_fsmn_fwd_stream", ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True), ptr(resid), ptr(dst),
+                         B, rows, src.shape[2], layer["kernel"], layer["lp"], a - layer["lag"] - layer["rp"])
             else:
-                check(lib.kt_lstm_stream(ptr(src), ptr(w), ptr(self._state), ptr(dst), B, rows, self.hidden, src.shape[1],
-                                         dst.shape[1], stream_ptr()), "kt_lstm_stream")
-                ops._count()
+                ops.call("kt_lstm_stream", ptr(src), ptr(w), ptr(self._state), ptr(dst), B, rows, self.hidden, src.shape[1],
+                         dst.shape[1])
         self._win.advance(f)
         self._rows += f
         if n <= 0:

@@ -6,8 +6,8 @@ import ctypes
 import torch
 
 from . import _lib
-from ._lib import KtAttnDesc, check, ptr, stream_ptr
-from .ops import _count
+from ._lib import KtAttnDesc, ptr
+from .ops import call
 
 
 def _u8(mask):
@@ -23,22 +23,19 @@ class LayerNormFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, gamma, beta, eps):
-        lib = _lib.load()
         x = x.contiguous()
         c = x.shape[-1]
         rows = x.numel() // c
         y = torch.empty_like(x)
         mean = torch.empty(rows, device=x.device, dtype=torch.float32)
         rstd = torch.empty(rows, device=x.device, dtype=torch.float32)
-        check(lib.kt_layernorm_fwd(ptr(x), ptr(gamma.detach()), ptr(beta.detach()), ptr(y), ptr(mean), ptr(rstd),
-                                   rows, c, float(eps), stream_ptr()), "kt_layernorm_fwd")
-        _count()
+        call("kt_layernorm_fwd", ptr(x), ptr(gamma.detach()), ptr(beta.detach()), ptr(y), ptr(mean), ptr(rstd), rows, c,
+             float(eps))
         ctx.save_for_backward(x, gamma, mean, rstd)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        lib = _lib.load()
         x, gamma, mean, rstd = ctx.saved_tensors
         c = x.shape[-1]
         rows = x.numel() // c
@@ -46,11 +43,10 @@ class LayerNormFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dgamma = torch.empty_like(gamma)
         dbeta = torch.empty_like(gamma)
-        n = int(lib.kt_layernorm_bwd_workspace(rows, c))
+        n = int(_lib.load().kt_layernorm_bwd_workspace(rows, c))
         ws = torch.empty(n, device=x.device, dtype=torch.float32)
-        check(lib.kt_layernorm_bwd(ptr(dy), ptr(x), ptr(gamma.detach()), ptr(mean), ptr(rstd), ptr(dx), ptr(dgamma),
-                                   ptr(dbeta), ptr(ws), n, rows, c, stream_ptr()), "kt_layernorm_bwd")
-        _count(2)
+        call("kt_layernorm_bwd", ptr(dy), ptr(x), ptr(gamma.detach()), ptr(mean), ptr(rstd), ptr(dx), ptr(dgamma), ptr(dbeta),
+             ptr(ws), n, rows, c, launches=2)
         return dx, dgamma, dbeta, None
 
 
@@ -89,7 +85,6 @@ class SelfAttnFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, qkv, mask, n_head, p_drop=0.0, keep=None):
-        lib = _lib.load()
         qkv = qkv.contiguous()
         B, L, w = qkv.shape
         hd = w // 3
@@ -100,9 +95,8 @@ class SelfAttnFn(torch.autograd.Function):
         probs = torch.empty(n_head * B, L, L, device=qkv.device, dtype=torch.float32)
         keep = _u8(keep) if keep is not None else _keep_mask(p_drop, probs.shape, qkv.device)
         dropped = torch.empty_like(probs) if keep is not None else None
-        check(lib.kt_attention_fwd(ctypes.byref(d), _off(qkv, 0), _off(qkv, hd), _off(qkv, 2 * hd), ptr(m, True), ptr(keep, True),
-                                   ptr(out), ptr(probs), ptr(dropped), stream_ptr()), "kt_attention_fwd")
-        _count()
+        call("kt_attention_fwd", ctypes.byref(d), _off(qkv, 0), _off(qkv, hd), _off(qkv, 2 * hd), ptr(m, True), ptr(keep, True),
+             ptr(out), ptr(probs), ptr(dropped))
         ctx.d, ctx.hd = d, hd
         ctx.save_for_backward(qkv, probs, keep)
         attn = probs if dropped is None else dropped
@@ -111,16 +105,13 @@ class SelfAttnFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout, _dprobs):
-        lib = _lib.load()
         qkv, probs, keep = ctx.saved_tensors
         d, hd = ctx.d, ctx.hd
         dout = dout.contiguous()
         dqkv = torch.empty_like(qkv)
         delta = torch.empty(d.heads * d.batch * d.lq, device=qkv.device, dtype=torch.float32)
-        check(lib.kt_attention_bwd(ctypes.byref(d), _off(qkv, 0), _off(qkv, hd), _off(qkv, 2 * hd), ptr(probs),
-                                   ptr(keep, True), ptr(dout), _off(dqkv, 0), _off(dqkv, hd), _off(dqkv, 2 * hd),
-                                   ptr(delta), 0, stream_ptr()), "kt_attention_bwd")
-        _count(2)
+        call("kt_attention_bwd", ctypes.byref(d), _off(qkv, 0), _off(qkv, hd), _off(qkv, 2 * hd), ptr(probs), ptr(keep, True),
+             ptr(dout), _off(dqkv, 0), _off(dqkv, hd), _off(dqkv, 2 * hd), ptr(delta), 0, launches=2)
         return dqkv, None, None, None, None
 
 
@@ -131,7 +122,6 @@ class PncaAttnFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x_qkv, h_kv, mask_x, mask_h, n_head, p_drop=0.0, keep_x=None, keep_h=None):
-        lib = _lib.load()
         x_qkv, h_kv = x_qkv.contiguous(), h_kv.contiguous()
         B, L, w = x_qkv.shape
         hd = w // 3
@@ -148,12 +138,10 @@ class PncaAttnFn(torch.autograd.Function):
         kh = _u8(keep_h) if keep_h is not None else _keep_mask(p_drop, ph.shape, x_qkv.device)
         pxd = torch.empty_like(px) if kx is not None else None
         phd = torch.empty_like(ph) if kh is not None else None
-        st = stream_ptr()
-        check(lib.kt_attention_fwd(ctypes.byref(dx), _off(x_qkv, 0), _off(x_qkv, hd), _off(x_qkv, 2 * hd), ptr(mx, True),
-                                   ptr(kx, True), ptr(out_x), ptr(px), ptr(pxd), st), "kt_attention_fwd")
-        check(lib.kt_attention_fwd(ctypes.byref(dh), _off(x_qkv, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(mh, True),
-                                   ptr(kh, True), ptr(out_h), ptr(ph), ptr(phd), st), "kt_attention_fwd")
-        _count(2)
+        call("kt_attention_fwd", ctypes.byref(dx), _off(x_qkv, 0), _off(x_qkv, hd), _off(x_qkv, 2 * hd), ptr(mx, True),
+             ptr(kx, True), ptr(out_x), ptr(px), ptr(pxd))
+        call("kt_attention_fwd", ctypes.byref(dh), _off(x_qkv, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(mh, True), ptr(kh, True),
+             ptr(out_h), ptr(ph), ptr(phd))
         ctx.dx, ctx.dh, ctx.hd = dx, dh, hd
         ctx.save_for_backward(x_qkv, h_kv, px, ph, kx, kh)
         ax = px if pxd is None else pxd
@@ -163,21 +151,16 @@ class PncaAttnFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dox, doh, _dpx, _dph):
-        lib = _lib.load()
         x_qkv, h_kv, px, ph, kx, kh = ctx.saved_tensors
         dx, dh, hd = ctx.dx, ctx.dh, ctx.hd
         dox, doh = dox.contiguous(), doh.contiguous()
         dqkv = torch.empty_like(x_qkv)
         dhkv = torch.empty_like(h_kv)
         delta = torch.empty(dx.heads * dx.batch * dx.lq, device=x_qkv.device, dtype=torch.float32)
-        st = stream_ptr()
-        check(lib.kt_attention_bwd(ctypes.byref(dx), _off(x_qkv, 0), _off(x_qkv, hd), _off(x_qkv, 2 * hd), ptr(px),
-                                   ptr(kx, True), ptr(dox), _off(dqkv, 0), _off(dqkv, hd), _off(dqkv, 2 * hd), ptr(delta), 0,
-                                   st), "kt_attention_bwd")
-        check(lib.kt_attention_bwd(ctypes.byref(dh), _off(x_qkv, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(ph),
-                                   ptr(kh, True), ptr(doh), _off(dqkv, 0), _off(dhkv, 0), _off(dhkv, hd), ptr(delta), 1, st),
-              "kt_attention_bwd")
-        _count(4)
+        call("kt_attention_bwd", ctypes.byref(dx), _off(x_qkv, 0), _off(x_qkv, hd), _off(x_qkv, 2 * hd), ptr(px), ptr(kx, True),
+             ptr(dox), _off(dqkv, 0), _off(dqkv, hd), _off(dqkv, 2 * hd), ptr(delta), 0, launches=2)
+        call("kt_attention_bwd", ctypes.byref(dh), _off(x_qkv, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(ph), ptr(kh, True),
+             ptr(doh), _off(dqkv, 0), _off(dhkv, 0), _off(dhkv, hd), ptr(delta), 1, launches=2)
         return dqkv, dhkv, None, None, None, None, None, None
 
 
@@ -188,7 +171,6 @@ def pnca_attn_step(q_row, x_cache, h_kv, mask_x, mask_h, n_head):
     current step are masked by ``mask_x`` (B or 1, 1, Lmax), so the reference's ``torch.cat`` growth is never needed);
     h_kv (B, Lh, 2HD): the memory keys / values projected once; mask_h (B or 1, 1, Lh).
     -> out_x, out_h (B, 1, HD), probs_x (H*B, 1, Lmax), probs_h (H*B, 1, Lh)."""
-    lib = _lib.load()
     assert q_row.is_contiguous() and x_cache.is_contiguous() and h_kv.is_contiguous()
     B, _, w = q_row.shape
     hd = w // 3
@@ -201,12 +183,10 @@ def pnca_attn_step(q_row, x_cache, h_kv, mask_x, mask_h, n_head):
     out_h = torch.empty_like(out_x)
     px = torch.empty(n_head * B, 1, lmax, device=q_row.device, dtype=torch.float32)
     ph = torch.empty(n_head * B, 1, lh, device=q_row.device, dtype=torch.float32)
-    st = stream_ptr()
-    check(lib.kt_attention_fwd(ctypes.byref(dx), _off(q_row, 0), _off(x_cache, hd), _off(x_cache, 2 * hd), ptr(mx, True), None,
-                               ptr(out_x), ptr(px), None, st), "kt_attention_fwd")
-    check(lib.kt_attention_fwd(ctypes.byref(dh), _off(q_row, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(mh, True), None,
-                               ptr(out_h), ptr(ph), None, st), "kt_attention_fwd")
-    _count(2)
+    call("kt_attention_fwd", ctypes.byref(dx), _off(q_row, 0), _off(x_cache, hd), _off(x_cache, 2 * hd), ptr(mx, True), None,
+         ptr(out_x), ptr(px), None)
+    call("kt_attention_fwd", ctypes.byref(dh), _off(q_row, 0), _off(h_kv, 0), _off(h_kv, hd), ptr(mh, True), None, ptr(out_h),
+         ptr(ph), None)
     return out_x, out_h, px, ph
 
 
@@ -215,22 +195,18 @@ class FsmnMemoryFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, w, mask, pad_left):
-        lib = _lib.load()
         x = x.contiguous()
         B, T, C = x.shape
         K = w.shape[-1]
         m = _u8(mask)
         y = torch.empty_like(x)
-        check(lib.kt_fsmn_fwd(ptr(x), ptr(w.detach().contiguous()), ptr(m, True), ptr(y), B, T, C, K, pad_left,
-                              stream_ptr()), "kt_fsmn_fwd")
-        _count()
+        call("kt_fsmn_fwd", ptr(x), ptr(w.detach().contiguous()), ptr(m, True), ptr(y), B, T, C, K, pad_left)
         ctx.pad_left = pad_left
         ctx.save_for_backward(x, w, m)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        lib = _lib.load()
         x, w, m = ctx.saved_tensors
         B, T, C = x.shape
         K = w.shape[-1]
@@ -240,11 +216,10 @@ class FsmnMemoryFn(torch.autograd.Function):
         n = 0
         if ctx.needs_input_grad[1]:
             dw = torch.empty_like(w)
-            n = int(lib.kt_fsmn_bwd_workspace(B, T, C, K))
+            n = int(_lib.load().kt_fsmn_bwd_workspace(B, T, C, K))
             ws = torch.empty(n, device=x.device, dtype=torch.float32)
-        check(lib.kt_fsmn_bwd(ptr(x), ptr(dy), ptr(w.detach().contiguous()), ptr(m, True), ptr(dx), ptr(dw), ptr(ws), n,
-                              B, T, C, K, ctx.pad_left, stream_ptr()), "kt_fsmn_bwd")
-        _count(3)
+        call("kt_fsmn_bwd", ptr(x), ptr(dy), ptr(w.detach().contiguous()), ptr(m, True), ptr(dx), ptr(dw), ptr(ws), n, B, T, C,
+             K, ctx.pad_left, launches=3)
         return dx, dw, None, None
 
 
@@ -254,28 +229,22 @@ class RowsGatherFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, idx, start, count):
-        lib = _lib.load()
         x = x.contiguous()
         B, T_in, C = x.shape
         T_out = idx.shape[1]
         out = torch.empty(B, T_out, C, device=x.device, dtype=torch.float32)
-        check(lib.kt_rows_gather_fwd(ptr(x), ptr(idx, True), ptr(out), B, T_out, T_in, C, stream_ptr()),
-              "kt_rows_gather_fwd")
-        _count()
+        call("kt_rows_gather_fwd", ptr(x), ptr(idx, True), ptr(out), B, T_out, T_in, C)
         ctx.save_for_backward(idx, start, count)
         ctx.t_in = T_in
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        lib = _lib.load()
         idx, start, count = ctx.saved_tensors
         dout = dout.contiguous()
         B, T_out, C = dout.shape
         din = torch.empty(B, ctx.t_in, C, device=dout.device, dtype=torch.float32)
-        check(lib.kt_rows_gather_bwd(ptr(dout), ptr(idx, True), ptr(start, True), ptr(count, True), ptr(din), B, T_out, ctx.t_in, C,
-                                     stream_ptr()), "kt_rows_gather_bwd")
-        _count()
+        call("kt_rows_gather_bwd", ptr(dout), ptr(idx, True), ptr(start, True), ptr(count, True), ptr(din), B, T_out, ctx.t_in, C)
         return din, None, None, None
 
 
@@ -283,7 +252,6 @@ def fp_insert_plan(input_lengths, length, fp_label=None, fp_p=None):
     """Index plan of KanTtsSAMBERT.insert_fp (kantts_sambert.py:766-860, kt_fp_insert_plan): from ``fp_label`` (B, L)
     integer labels (training) or the (B, L, 4) predictions ``fp_p`` (inference).  -> codes (B, t_cap) int32,
     rows (B, L) int32, inter_lengths (B,) int64, t_ins.  Reading t_ins is the one host synchronisation."""
-    lib = _lib.load()
     B = input_lengths.shape[0]
     lens = input_lengths.to(torch.int32).contiguous()
     if fp_label is not None:
@@ -294,9 +262,8 @@ def fp_insert_plan(input_lengths, length, fp_label=None, fp_p=None):
     codes = torch.empty(B, t_cap, device=lens.device, dtype=torch.int32)
     rows = torch.empty(B, length, device=lens.device, dtype=torch.int32)
     inter = torch.empty(B, device=lens.device, dtype=torch.int32)
-    check(lib.kt_fp_insert_plan(ptr(lab, True), nbytes, ptr(p), ptr(lens, True), B, length, t_cap, ptr(codes, True),
-                                ptr(rows, True), ptr(inter, True), stream_ptr()), "kt_fp_insert_plan")
-    _count()
+    call("kt_fp_insert_plan", ptr(lab, True), nbytes, ptr(p), ptr(lens, True), B, length, t_cap, ptr(codes, True),
+         ptr(rows, True), ptr(inter, True))
     t_ins = length + int(inter.max() - lens.max())
     return codes, rows, inter.to(input_lengths.dtype), t_ins
 
@@ -307,21 +274,17 @@ class FpInsertFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, text_hid, fp_enc, codes, rows, t_ins):
-        lib = _lib.load()
         text_hid, fp_enc = text_hid.contiguous(), fp_enc.contiguous()
         B, L, C = text_hid.shape
         assert fp_enc.shape == (3, 3, C), fp_enc.shape
         out = torch.empty(B, t_ins, C, device=text_hid.device, dtype=torch.float32)
-        check(lib.kt_fp_insert_fwd(ptr(text_hid), ptr(fp_enc), ptr(codes, True), ptr(out), B, L, codes.shape[1], t_ins, C,
-                                   stream_ptr()), "kt_fp_insert_fwd")
-        _count()
+        call("kt_fp_insert_fwd", ptr(text_hid), ptr(fp_enc), ptr(codes, True), ptr(out), B, L, codes.shape[1], t_ins, C)
         ctx.save_for_backward(codes, rows)
         ctx.shape = (B, L, C)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        lib = _lib.load()
         codes, rows = ctx.saved_tensors
         B, L, C = ctx.shape
         dout = dout.contiguous()
@@ -329,8 +292,6 @@ class FpInsertFn(torch.autograd.Function):
         dtext = torch.empty(B, L, C, device=dev, dtype=torch.float32) if ctx.needs_input_grad[0] else None
         dfp = torch.empty(3, 3, C, device=dev, dtype=torch.float32) if ctx.needs_input_grad[1] else None
         part = torch.empty(9 * B * C, device=dev, dtype=torch.float32) if dfp is not None else None
-        check(lib.kt_fp_insert_bwd(ptr(dout), ptr(codes, True), ptr(rows, True), ptr(dtext), ptr(dfp), ptr(part),
-                                   0 if part is None else part.numel(), B, L, codes.shape[1], dout.shape[1], C,
-                                   stream_ptr()), "kt_fp_insert_bwd")
-        _count(1 + 2 * (dfp is not None))
+        call("kt_fp_insert_bwd", ptr(dout), ptr(codes, True), ptr(rows, True), ptr(dtext), ptr(dfp), ptr(part),
+             0 if part is None else part.numel(), B, L, codes.shape[1], dout.shape[1], C, launches=1 + 2 * (dfp is not None))
         return dtext, dfp, None, None, None

@@ -5,7 +5,7 @@ any reader of the tensor needs."""
 import torch
 
 from . import ops
-from ._lib import KtStreamWin, KtWindow, check, load, ptr, stream_ptr
+from ._lib import KtStreamWin, KtWindow, ptr
 
 
 class WindowTable:
@@ -81,9 +81,7 @@ class Windows:
     def advance(self, frames):
         """After a chunk of ``frames`` frames, the last H rows of every window become its history (one launch)."""
         if self._ntable:
-            check(load().kt_stream_advance(ptr(self._table, True), self._ntable, self.batch, frames, self._max_c,
-                                           stream_ptr()), "kt_stream_advance")
-            ops._count()
+            ops.call("kt_stream_advance", ptr(self._table, True), self._ntable, self.batch, frames, self._max_c)
 
     def reset(self, slots=None):
         """The history of the given slots (None: all) returns to zeros in every window (one launch)."""
@@ -96,9 +94,7 @@ class Windows:
             mask[slots] = 1
             sel = mask.to(self.device)
         if self._ntable:
-            check(load().kt_stream_reset(ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c,
-                                         stream_ptr()), "kt_stream_reset")
-            ops._count()
+            ops.call("kt_stream_reset", ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c)
 
 
 def own_weight(spec, v, g, bias):

@@ -31,6 +31,36 @@ def test_library_exports_every_declared_symbol(lib):
     assert lib.kt_version() >= 2
 
 
+_CTYPES = {"int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "float": ctypes.c_float}
+_RESTYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "const char*": ctypes.c_char_p}
+
+
+def _accepted_argtypes(param):
+    """The ctypes types that pass one C parameter ("const KtConv1dDesc* d") unchanged."""
+    param = " ".join(param.replace("*", "* ").split())
+    if "*" not in param:
+        return (_CTYPES[param.rsplit(" ", 1)[0]],)
+    struct = re.match(r"const (Kt\w+)\*", param)
+    if struct:
+        return ctypes.POINTER(getattr(_lib, struct.group(1))), ctypes.c_void_p
+    return (ctypes.c_void_p,)
+
+
+def test_every_prototype_matches_header(lib):
+    """Each entry point's argtypes (PROTOTYPES) and the restype load() sets agree with its declaration in the header, argument
+    by argument: a wrong ctypes type would not raise, it would pass corrupted arguments."""
+    header = open(os.path.join(ROOT, "include", "kantts_b200.h")).read()
+    decls = re.findall(r"^(int|int64_t|const char\*)\s+(kt_\w+)\s*\(([^)]*)\);", header, flags=re.M)
+    assert sorted(name for _, name, _ in decls) == sorted(set(_lib.PROTOTYPES) | {"kt_last_error"})
+    for ret, name, params in decls:
+        params = [] if params.strip() == "void" else params.split(",")
+        fn = getattr(lib, name)
+        assert len(fn.argtypes) == len(params), name
+        for i, (param, argtype) in enumerate(zip(params, fn.argtypes)):
+            assert argtype in _accepted_argtypes(param), (name, i, param, argtype)
+        assert fn.restype is _RESTYPES[ret], (name, ret, fn.restype)
+
+
 def test_descriptor_struct_sizes_match_header():
     assert ctypes.sizeof(_lib.KtConv1dDesc) == 18 * 4
     assert ctypes.sizeof(_lib.KtMelDesc) == 14 * 4

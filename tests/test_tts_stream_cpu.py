@@ -1,21 +1,14 @@
 """CPU checks of streamed text-to-speech (PostNet.streamer, infer.stream_synthesize): a chunk-by-chunk restatement of the
 post-net over the oracle's own functions (postnet_stream below) equals the oracle's whole-sequence post-net for every
 chunk schedule, ragged batches and both post-net delays; the stream plan's delay, windows and launch count follow from the
-shapes; bad models are rejected; the new entry points' ctypes signatures match the header."""
-import ctypes
-import os
-import re
-
+shapes; bad models are rejected."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 import kantts_b200 as K
-from kantts_b200 import _lib
 from kantts_b200.sambert import PostNet, PostNetStreamPlan
 from oracle import sambert as O
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # a reduced-width post-net with the shipped filter and layer count; shift 17 gives rp = 3 per layer (D = 12), shift 0
 # gives rp = 20 (D = 80, longer than the utterance: only the flush produces output)
@@ -167,25 +160,3 @@ def test_stream_synthesize_rejects_bad_models(golden):
         K.stream_synthesize(am, _models(golden, nsf_params=dict(nb_harmonics=7, sampling_rate=16000))[1], *inputs)
     with pytest.raises(ValueError, match="mel channels"):
         K.stream_synthesize(am, _models(golden, in_channels=80)[1], *inputs)
-
-
-def _c_args(header, name):
-    """Parameter types of `name` in the header, as ctypes types."""
-    decl = re.search(r"^int\s+" + name + r"\s*\(([^)]*)\)", header, flags=re.M | re.S).group(1)
-    types = []
-    for arg in decl.split(","):
-        arg = " ".join(arg.split())
-        if arg.startswith("const KtStreamWin*"):
-            types.append(ctypes.POINTER(_lib.KtStreamWin))
-        elif "*" in arg:
-            types.append(ctypes.c_void_p)
-        else:
-            assert arg.startswith("int32_t "), arg
-            types.append(ctypes.c_int32)
-    return types
-
-
-@pytest.mark.parametrize("name", ["kt_fsmn_fwd_stream", "kt_lstm_stream"])
-def test_stream_entry_points_match_header(name):
-    header = open(os.path.join(ROOT, "include", "kantts_b200.h")).read()
-    assert _c_args(header, name) == _lib.PROTOTYPES[name]
