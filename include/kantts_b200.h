@@ -403,6 +403,10 @@ int kt_debug_wgrad_plan(const KtConv1dDesc* d, int32_t* out12);
  * out9 = {N tile (0: not on the tensor cores), TMA route, time steps per M tile, rows per M tile, time steps per image box,
  * image stages, weight stages, shared-memory bytes, workspace floats}; tile and stage entries describe the first launch. */
 int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t* out9);
+/* Test aid (no GPU needed): 1 when those launches take the shared-memory staged epilogue (given 16-byte aligned operands),
+ * 0 for the register epilogue (stream chunks, produced channels or channels per N tile % 4 != 0) or a layer off the
+ * tensor cores. */
+int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir);
 
 /* library info */
 const char* kt_last_error(void);

@@ -115,6 +115,7 @@ PROTOTYPES = {
     "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
+    "kt_debug_conv_tc_epilogue": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_version": [],
     "kt_has_tc": [],
 }

@@ -18,7 +18,8 @@
 //              cp.async.bulk (TMA engine) into a ring of shared-memory stages, mbarrier complete_tx.
 //   warpgroups 1 / 2  wgmma (M = 64 rows each, N = NT, K = 16) x 4 k-slices x 3 products per (chunk, tap) into
 //              register accumulators, then the epilogue of their 64 rows: bias / activation / residual (or act'
-//              mask for the data gradient), stores to the channels-last output.
+//              mask for the data gradient), stores to the channels-last output -- staged through a small shared-memory
+//              block per warp into float4 rows when the channel counts allow (TcParams::epi_staged).
 //
 // TMA-fed route (plain convs, channel counts % 8 == 0, see make_tc_plan): warpgroup 0 is the bound of the layers with
 // few taps per image -- every CTA converts its own copy of each image, once per N tile -- so the call first writes the
@@ -134,7 +135,19 @@ struct TcParams {
   int a_box_t;                        // TMA route: time steps per image box = tt + span_q
   // stream instances (kt_conv1d_fwd_tc_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
   int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
+  // 1: the epilogue goes through each consumer warp's shared-memory staging block (kTcEpiWarpBytes) with float4 global
+  // traffic, see conv_tc_kernel; 0: straight from the accumulator registers (stream chunks, channel counts % 4 != 0,
+  // operands not 16-byte aligned)
+  int epi_staged;
 };
+
+// Staged epilogue: each consumer warp turns 32 columns of its 16 accumulator rows at a time into a 16 x 32 fp32 block in
+// shared memory (row pitch 40 floats: the fragment writes conflict at most 2-way, rows stay 16-byte aligned), then reads it
+// back as float4 per lane -- 4 rows x 128 contiguous bytes per warp instruction, like the bias / side-operand loads and the
+// output stores.
+constexpr int kTcEpiPitch = 40;
+constexpr int kTcEpiWarpBytes = 16 * kTcEpiPitch * 4;
+constexpr int kTcEpiBytes = 8 * kTcEpiWarpBytes;   // 8 consumer warps
 
 // TMA route: one tensor map of the gathered operand's planes per input residue class rho (base + rho rows, time stride
 // i_step), as wgrad_tma_kernel's map_a[]
@@ -185,6 +198,8 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
   uint64_t* empty_b = full_b + p.nb_stages;        // [nb]
   // per-tap image row shift in descriptor units (16 bytes)
   uint32_t* s_tapshift = reinterpret_cast<uint32_t*>(empty_b + p.nb_stages);   // [kMaxTaps]
+  // staged epilogue blocks [8][16][kTcEpiPitch] floats, 16-byte aligned, after the tap-shift table (derived from it in the
+  // epilogue: a pointer kept live through the main loop would cost the register-staged instances a register)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mtiles = p.ph_mt0[p.nphases];   // m-tiles of all phases (each: R flattened outputs m * nsub + w)
@@ -358,19 +373,72 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
         const int F = p.ph_M[ph] * p.nsub;
         const int c_tile = nt * p.n_stride;
         const int n_valid = min(p.n_stride, p.c_out - c_tile);   // real output channels of this tile
-        const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;   // row of the M = 128 accumulator tile
+        // Element index of output row r's first column (false: the row is not written).  The residual element is the
+        // output element + rdelta (0 outside streams: the residual has the output's layout); the act' mask and `out` itself
+        // (accumulate) share the output's layout.
+        const long long rdelta = STREAM ? ((long long)bb * (p.res_pitch - p.out_pitch) + p.res_first - p.out_first) * p.c_out : 0;
+        auto row_base = [&](int r, long long& obase) {
           const int f = mt * R + r;
-          if ((TMA && r >= R) || f >= F) continue;
+          if ((TMA && r >= R) || f >= F) return false;
           const int m = p.nsub == 1 ? f : f / p.nsub;
           const int w = f - m * p.nsub;
           const int to = p.ph_ooff[ph] + p.o_step * m;
-          const long long obase = STREAM ? ((long long)bb * p.out_pitch + p.out_first + to) * p.c_out + c_tile
-                                         : ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
-          // residual element = output element + rdelta (0 outside streams: the residual has the output's layout)
-          const long long rdelta = STREAM ? ((long long)bb * (p.res_pitch - p.out_pitch) + p.res_first - p.out_first) * p.c_out : 0;
+          obase = STREAM ? ((long long)bb * p.out_pitch + p.out_first + to) * p.c_out + c_tile
+                         : ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
+          return true;
+        };
+        // Both forms do the same fp32 operations per element in the same order, so they write the same bits.
+        auto finish = [&](float x, float bia, float md, float sd, float od) {
+          x += bia;
+          if (p.out_act == KT_ACT_LRELU) x = x > 0.f ? x : x * p.out_slope;
+          else if (!SIMPLE && p.out_act == KT_ACT_TANH) x = tanhf(x);
+          if (p.mask.p) x = side_apply(x, md, p.mask.mode, p.mask.slope);
+          return x + (sd + od);
+        };
+        if (!STREAM && p.epi_staged) {
+          // Staged: per 32-column chunk, registers -> this warp's shared-memory block -> float4 rows.  A warp waits for its
+          // side operand 16 times per tile instead of 32, every load and store moves whole 128-byte lines, and the unrolled
+          // code per chunk stays small (the register form's code per tile is several times larger).
+          float* blk = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_tapshift + kMaxTaps) + 15) & ~(uintptr_t)15) +
+                       (warp - kConsumer0) * (16 * kTcEpiPitch);
+          const int c4 = (lane & 7) * 4;   // this lane's 4 columns of the chunk; rows it * 4 + lane / 8
+          const float* side = p.resid ? p.resid + rdelta : p.mask.p;   // at most one (run_plan)
+#pragma unroll
+          for (int j = 0; j < (NT + 31) / 32; ++j) {
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii) {
+              const int i = 4 * j + ii;
+              if (i >= NT / 8) break;
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(blk + ((lane >> 2) + 8 * h) * kTcEpiPitch + ii * 8 + 2 * (lane & 3)) =
+                    make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            }
+            __syncwarp();
+            const int col = j * 32 + c4;
+            float4 bia = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (p.bias && col < n_valid) bia = __ldg(reinterpret_cast<const float4*>(p.bias + c_tile + col));
+#pragma unroll
+            for (int it = 0; it < 4; ++it) {
+              long long o;
+              if (col >= n_valid || !row_base(cw * 64 + wq * 16 + it * 4 + (lane >> 3), o)) continue;
+              o += col;
+              const float4 pre = side ? __ldg(reinterpret_cast<const float4*>(side + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
+              const float4 v = *reinterpret_cast<const float4*>(blk + (it * 4 + (lane >> 3)) * kTcEpiPitch + c4);
+              const float4 md = p.resid ? make_float4(0.f, 0.f, 0.f, 0.f) : pre;
+              const float4 sd = p.resid ? pre : make_float4(0.f, 0.f, 0.f, 0.f);
+              *reinterpret_cast<float4*>(p.out + o) = make_float4(finish(v.x, bia.x, md.x, sd.x, 0.f), finish(v.y, bia.y, md.y, sd.y, 0.f),
+                                                                  finish(v.z, bia.z, md.z, sd.z, 0.f), finish(v.w, bia.w, md.w, sd.w, 0.f));
+            }
+            __syncwarp();
+          }
+          continue;
+        }
+        const bool vec2 = ((p.c_out | p.n_stride) & 1) == 0;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          long long obase;
+          if (!row_base(cw * 64 + wq * 16 + (lane >> 2) + 8 * h, obase)) continue;   // row of the M = 128 accumulator tile
 #pragma unroll
           for (int i = 0; i < NT / 8; ++i) {
             const int col = i * 8 + 2 * (lane & 3);
@@ -396,14 +464,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
               }
             }
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              float x = v[e] + bia[e];
-              if (p.out_act == KT_ACT_LRELU) x = x > 0.f ? x : x * p.out_slope;
-              else if (!SIMPLE && p.out_act == KT_ACT_TANH) x = tanhf(x);
-              if (p.mask.p) x = side_apply(x, md[e], p.mask.mode, p.mask.slope);
-              x += sd[e] + od[e];
-              v[e] = x;
-            }
+            for (int e = 0; e < 2; ++e) v[e] = finish(v[e], bia[e], md[e], sd[e], od[e]);
             if (pair) *reinterpret_cast<float2*>(p.out + o) = make_float2(v[0], v[1]);
             else {
               p.out[o] = v[0];
@@ -587,17 +648,23 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
     base.tt = 0; base.R = kTcM;
     if (!plan_launches(phases, d->nsub, P.launches, base)) return P;
   }
+  // staged epilogue: float4 rows need output channel counts and tile offsets % 4 (run_plan also checks the pointers);
+  // accumulating launches keep the register form
+  for (TcParams& lp : P.launches) lp.epi_staged = lp.c_out % 4 == 0 && lp.n_stride % 4 == 0 && !lp.accumulate;
   P.ok = true;
   P.tma = tma;
   P.ws_floats = tma ? plane_floats(base.batch, base.t_in, base.nsub, base.c_in) : 0;
   return P;
 }
 
-// dir: 0 / 1, or KT_PLAN_STREAM (the forward of a stream chunk: register-staged route, nsub == 1)
+// dir: 0 / 1, or KT_PLAN_STREAM (the forward of a stream chunk: register-staged route, nsub == 1, register epilogue: the
+// stream instances have no registers to spare)
 static TcPlan make_tc_plan_flags(const KtConv1dDesc* d, int dir, bool plan_only = false) {
   if (dir == KT_PLAN_STREAM) {
     if (d->nsub != 1) return TcPlan{};
-    return make_tc_plan(d, 0, false, plan_only);
+    TcPlan P = make_tc_plan(d, 0, false, plan_only);
+    for (TcParams& lp : P.launches) lp.epi_staged = 0;
+    return P;
   }
   return make_tc_plan(d, dir, true, plan_only);
 }
@@ -648,7 +715,7 @@ static size_t size_stages(TcParams& p) {
   const int a_stage = 2 * p.rows * 128;
   const int b_stage = 2 * p.NT * 128;
   const int slots = p.ntaps * p.kchunks;                                      // weight tiles of the whole layer
-  const int bar_bytes = tc_fixed_smem(slots);
+  const int bar_bytes = tc_fixed_smem(slots) + (p.epi_staged ? 16 + kTcEpiBytes : 0);
   const int budget = kMaxDynSmem - 1024 /*align slack*/ - bar_bytes;
   p.w_resident = 0;
   if (p.ntiles == 1 && slots <= 160 && 2 * a_stage + slots * b_stage <= budget) {
@@ -681,6 +748,14 @@ extern "C" int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t
   out[0] = P.L.NT; out[1] = P.tma; out[2] = lp.tt; out[3] = lp.R; out[4] = lp.a_box_t;
   out[5] = lp.na_stages; out[6] = lp.nb_stages; out[7] = (int64_t)smem; out[8] = P.ws_floats;
   return KT_OK;
+}
+
+// development / test aid: 1 when the launches of direction dir (0, 1 or KT_PLAN_STREAM) take the staged epilogue given
+// 16-byte aligned operands, 0 for the register epilogue or a layer off the tensor cores
+extern "C" int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir) {
+  if (d == nullptr) return 0;
+  const TcPlan P = make_tc_plan_flags(d, dir, true);
+  return P.ok && P.launches[0].epi_staged ? 1 : 0;
 }
 
 static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, cudaStream_t st) {   // p: phases already planned
@@ -732,6 +807,11 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
     lp.out_act = io.out_act; lp.out_slope = io.out_slope;
     lp.in_pitch = io.in_pitch; lp.in_first = io.in_first; lp.out_pitch = io.out_pitch; lp.out_first = io.out_first;
     lp.res_pitch = io.res_pitch; lp.res_first = io.res_first;
+    auto a16 = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+    // the staged epilogue reads at most one side operand (a forward has no mask, a data gradient no residual): fewer live
+    // values, the register-staged instances are at their cap
+    lp.epi_staged = lp.epi_staged && io.in_pitch == 0 && !(io.resid && io.mask.p) && a16(io.out) && a16(io.bias) &&
+                    a16(io.resid) && a16(io.mask.p);
     for (int rho = 0; P.tma && rho < lp.i_step; ++rho) {
       const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what);
       if (rc) return rc;
