@@ -374,6 +374,26 @@ typedef struct KtWindow {
 int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t frames, int32_t max_channels, void* stream);
 /* ONE launch: rows [0, history) of every window are zeroed for the batch items b with slots[b] != 0 (device uint8 [batch]). */
 int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream);
+/* Streams of a NON-CAUSAL generator: each window trails the pushed mel by `lag` rows (its chunk row t of item b is utterance
+ * row u = frames_done[b] * rows_per_frame - lag + t), and each batch slot holds an utterance of lengths[b] frames.
+ * KtStreamMask describes the input window of one conv call: the _masked conv entry points read a tap of item b as zero
+ * unless 0 <= u < lengths[b] * rows_per_frame -- the whole-utterance forward's zero padding, applied per slot -- and
+ * otherwise take exactly the arguments of kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream.  lengths and frames_done are
+ * device int32 [batch]; the conv calls only read frames_done. */
+typedef struct KtStreamMask {
+  const int32_t* lengths;
+  int32_t* frames_done;
+  int32_t rows_per_frame, lag;
+} KtStreamMask;
+int kt_conv1d_fwd_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                const float* w_fwd, const float* bias, const float* resid, float* y, void* stream);
+int kt_conv1d_fwd_tc_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                   const void* wimg, const float* bias, const float* resid, float* y, void* stream);
+/* ONE launch at the end of a chunk of `frames` frames: rows [first, first + rows) of each item's window y (`ch` channels,
+ * `pitch` rows per item), described by m, are zeroed where their utterance row lies outside the utterance; then
+ * frames_done[b] += frames for every item. */
+int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t pitch,
+                           int32_t first, int32_t frames, void* stream);
 
 /* ---- streaming SAM-BERT post-net (PostNet.streamer: decoder rows in, final post-net rows out, chunk by chunk) ---------------
  * kt_fsmn_fwd_stream: one chunk of MemoryBlockV2 with FsmnEncoderV2's residual fused, seen as a causal depthwise FIR whose

@@ -44,6 +44,11 @@ class KtWindow(ctypes.Structure):
                [(n, ctypes.c_int32) for n in ("pitch", "channels", "history", "rows_per_frame")]
 
 
+class KtStreamMask(ctypes.Structure):
+    _fields_ = [("lengths", ctypes.c_void_p), ("frames_done", ctypes.c_void_p), ("rows_per_frame", ctypes.c_int32),
+                ("lag", ctypes.c_int32)]
+
+
 class KtMelDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("batch", "t", "n_fft", "hop", "n_mels", "frames", "pad_mode")] + \
                [(n, ctypes.c_float) for n in ("eps", "ref_db", "min_db", "norm_scale", "norm_shift", "norm_lo", "norm_hi")]
@@ -111,6 +116,11 @@ PROTOTYPES = {
     "kt_add3_scale_win": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_stream_advance": [_P, _I, _I, _I, _I, _P],
     "kt_stream_reset": [_P, _I, _I, _P, _I, _P],
+    "kt_conv1d_fwd_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask),
+                                    _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_fwd_tc_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin),
+                                       ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P],
+    "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],

@@ -156,11 +156,22 @@ inline ResidueTaps residue_taps(const Phase& ph, int step) {
   return rt;
 }
 
+// Chunk rows [lo, hi) of item b's window described by m (KtStreamMask) that lie inside the item's utterance; clamped to
+// +-2^26 (far beyond any chunk), so bounds scaled by an up-sampling factor <= 32 stay in int range.
+__device__ __forceinline__ void stream_utterance_rows(const KtStreamMask& m, int b, int& lo, int& hi) {
+  const long long l = (long long)m.lag - (long long)__ldg(m.frames_done + b) * m.rows_per_frame;
+  const long long h = l + (long long)__ldg(m.lengths + b) * m.rows_per_frame;
+  lo = (int)max(-(1LL << 26), min(l, 1LL << 26));
+  hi = (int)max(-(1LL << 26), min(h, 1LL << 26));
+}
+
 // ---- host functions shared between files ----
 // conv_ffma.cu
 int validate_conv(const KtConv1dDesc* d);
 // validate_conv plus the window placement of one stream chunk (kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream)
 int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what);
+// the KtStreamMask of a _masked stream call
+int validate_stream_mask(const KtStreamMask* m, const char* what);
 Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up);
 std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir);
 // out[c] = the sum of the Side's values of channel c over `rows` rows, in a fixed order (the bias gradient)

@@ -45,6 +45,8 @@ struct CoreParams {
   Phase ph;
   // stream instances (kt_conv1d_fwd_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
   int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
+  // masked stream instances (kt_conv1d_fwd_stream_masked): the input window's utterance bounds per item
+  KtStreamMask smask;
 };
 
 __device__ __forceinline__ long long row_index(int bb, int t, int T, int nsub) {
@@ -52,7 +54,8 @@ __device__ __forceinline__ long long row_index(int bb, int t, int T, int nsub) {
 }
 
 // STREAM: rows are addressed in the windows of KtStreamWin, and input rows down to -in_first are real data
-template <int RN, int RM, int KC, bool STREAM = false>
+// MASK (with STREAM): of those, only the rows inside item bb's utterance (KtStreamMask) are; the others read as zeros
+template <int RN, int RM, int KC, bool STREAM = false, bool MASK = false>
 __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant__ CoreParams p) {
   constexpr int TN = 32 * RN;
   constexpr int TM = 8 * RM;
@@ -84,6 +87,12 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
 
   const bool vec_in = (p.c_in % 4 == 0) && (p.cin_g % 4 == 0);
   const bool vec_w = (p.c_out % 4 == 0) && (p.cout_g % 4 == 0);
+  int in_lo = 0, in_hi = 0;   // MASK: input rows [in_lo, in_hi) of this item are data
+  if constexpr (MASK) {
+    stream_utterance_rows(p.smask, bb, in_lo, in_hi);
+    in_lo = max(in_lo, -p.in_first);
+    in_hi = min(in_hi, p.t_in);
+  }
 
   for (int c0 = 0; c0 < p.cin_g; c0 += KC) {
     __syncthreads();
@@ -93,7 +102,7 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
       const int tin = row_lo + r;
       const int c = c0 + q * 4;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (tin >= (STREAM ? -p.in_first : 0) && tin < p.t_in && c < p.cin_g) {
+      if ((MASK ? tin >= in_lo && tin < in_hi : tin >= (STREAM ? -p.in_first : 0) && tin < p.t_in) && c < p.cin_g) {
         const long long row = STREAM ? (long long)bb * p.in_pitch + p.in_first + tin : row_index(bb, tin, p.t_in, p.nsub);
         const long long off = row * p.c_in + (long long)g * p.cin_g + c;
         if (vec_in && c + 3 < p.cin_g) {
@@ -218,19 +227,19 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
   }
 }
 
-template <int RN, int RM, int KC, bool STREAM>
+template <int RN, int RM, int KC, bool STREAM, bool MASK>
 static int launch_core(const CoreParams& p, cudaStream_t st) {
   constexpr int TN = 32 * RN, TM = 8 * RM, NTC = 4;
   const size_t smem = ((size_t)p.rmax * KC + (size_t)NTC * KC * TN) * sizeof(float);
   KT_REQUIRE(smem <= 200 * 1024, "conv_core: activation tile too large (%zu bytes shared)", smem);
-  KT_CHECK_CUDA(allow_dyn_smem<conv_core_kernel<RN, RM, KC, STREAM>>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<conv_core_kernel<RN, RM, KC, STREAM, MASK>>(kMaxDynSmem));
   dim3 grid(ceil_div(p.ph.M, TM), p.groups * ceil_div(p.cout_g, TN), p.batch);
-  conv_core_kernel<RN, RM, KC, STREAM><<<grid, 256, smem, st>>>(p);
+  conv_core_kernel<RN, RM, KC, STREAM, MASK><<<grid, 256, smem, st>>>(p);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
 
-template <bool STREAM = false>
+template <bool STREAM = false, bool MASK = false>
 static int run_core(CoreParams p, cudaStream_t st) {
   if (p.ph.M <= 0 || p.ph.ntaps <= 0) return KT_OK;
   const int RN = p.cout_g > 64 ? 4 : (p.cout_g > 32 ? 2 : 1);
@@ -243,7 +252,7 @@ static int run_core(CoreParams p, cudaStream_t st) {
   p.rmax = fdiv((TM - 1) * p.ph.i_step + p.ph.max_ioff - p.ph.min_ioff, p.ph.up) + 2;
   const int KC = p.cin_g <= 4 ? 4 : 16;
 #define KT_CORE_CASE(rn, rm, kc) \
-  if (RN == rn && RM == rm && KC == kc) return launch_core<rn, rm, kc, STREAM>(p, st);
+  if (RN == rn && RM == rm && KC == kc) return launch_core<rn, rm, kc, STREAM, MASK>(p, st);
   KT_CORE_CASE(4, 16, 16) KT_CORE_CASE(4, 8, 16) KT_CORE_CASE(4, 4, 16)
   KT_CORE_CASE(2, 16, 16) KT_CORE_CASE(2, 8, 16) KT_CORE_CASE(2, 4, 16)
   KT_CORE_CASE(1, 16, 16) KT_CORE_CASE(1, 8, 16) KT_CORE_CASE(1, 4, 16)
@@ -569,6 +578,12 @@ int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* re
   return KT_OK;
 }
 
+int validate_stream_mask(const KtStreamMask* m, const char* what) {
+  KT_REQUIRE(m != nullptr && m->lengths != nullptr && m->frames_done != nullptr, "%s: null mask descriptor", what);
+  KT_REQUIRE(m->rows_per_frame > 0 && m->lag >= 0, "%s: bad mask (rows_per_frame %d, lag %d)", what, m->rows_per_frame, m->lag);
+  return KT_OK;
+}
+
 static void finish_phase(Phase& ph) {
   ph.min_ioff = ph.tap_ioff[0];
   ph.max_ioff = ph.tap_ioff[0];
@@ -664,13 +679,9 @@ extern "C" int kt_conv1d_fwd(const KtConv1dDesc* d, const float* x, const float*
   return KT_OK;
 }
 
-// One chunk of a stream (KtStreamWin): the forward's phases over the windows
-extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd,
-                                    const float* bias, const float* resid, float* y, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
-  if (rc) return rc;
-  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
+// The forward's phases over the windows of one stream chunk; m: the input's utterance bounds (masked instances), or null
+static int conv_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x, const float* w_fwd,
+                       const float* bias, const float* resid, float* y, cudaStream_t st) {
   CoreParams p{};
   p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   p.w = w_fwd; p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
@@ -679,12 +690,34 @@ extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w,
   p.out_act = d->act_out; p.out_slope = d->act_out_slope;
   p.in_pitch = w->in_pitch; p.in_first = w->in_first; p.out_pitch = w->out_pitch; p.out_first = w->out_first;
   p.res_pitch = w->res_pitch; p.res_first = w->res_first;
+  if (m) p.smask = *m;
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
-    rc = run_core<true>(p, st);
+    const int rc = m ? run_core<true, true>(p, st) : run_core<true>(p, st);
     if (rc) return rc;
   }
   return KT_OK;
+}
+
+// One chunk of a stream (KtStreamWin): the forward's phases over the windows
+extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd,
+                                    const float* bias, const float* resid, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
+  return conv_stream(d, w, nullptr, x, w_fwd, bias, resid, y, st);
+}
+
+// The same over the utterance rows of each item only (KtStreamMask)
+extern "C" int kt_conv1d_fwd_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                           const float* w_fwd, const float* bias, const float* resid, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream_masked");
+  if (!rc) rc = validate_stream_mask(m, "kt_conv1d_fwd_stream_masked");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream_masked: null pointer");
+  return conv_stream(d, w, m, x, w_fwd, bias, resid, y, st);
 }
 
 extern "C" int kt_conv1d_bwd_data(const KtConv1dDesc* d, const float* dy, const float* y, const float* w_bwd, const float* x,

@@ -139,6 +139,8 @@ struct TcParams {
   // traffic, see conv_tc_kernel; 0: straight from the accumulator registers (stream chunks, channel counts % 4 != 0,
   // operands not 16-byte aligned)
   int epi_staged;
+  // masked stream instances (kt_conv1d_fwd_tc_stream_masked): the input window's utterance bounds per item
+  KtStreamMask smask;
 };
 
 // Staged epilogue: each consumer warp turns 32 columns of its 16 accumulator rows at a time into a 16 x 32 fp32 block in
@@ -173,8 +175,9 @@ enum TcRoute { kTcRegSimple = 0, kTcReg = 1, kTcTma = 2 };
 // Persistent: gridDim.x = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  The activation and
 // weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
 // STREAM (register-staged routes only): one chunk of a stream -- rows live in the windows of KtStreamWin, and the input
-// rows before the chunk (down to -in_first) are real data instead of zero padding.
-template <int ROUTE, bool STREAM = false>
+// rows before the chunk (down to -in_first) are real data instead of zero padding.  MASK (with STREAM): of those, only the
+// rows inside item bb's utterance (KtStreamMask) are, bounded per tile by the row map's t_lo / t_lim.
+template <int ROUTE, bool STREAM = false, bool MASK = false>
 __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
     conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
   static_assert(!(STREAM && ROUTE == kTcTma), "stream chunks take the register-staged route");
@@ -224,6 +227,12 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
       while (gm >= p.ph_mt0[ph + 1]) ++ph;
       const int ch_base = p.grouped ? ((tile / mtiles) % p.ntiles) * p.kg : 0;
       const int f0 = (gm - p.ph_mt0[ph]) * kTcM;
+      int t_lo = 0, t_lim = 0;   // MASK: the item's utterance rows, in the row map's (up-sampled) units
+      if constexpr (MASK) {
+        stream_utterance_rows(p.smask, bb, t_lo, t_lim);
+        t_lo = max(t_lo, -p.in_first) * p.up;
+        t_lim = min(t_lim, p.t_in) * p.up;
+      }
       for (int c = 0; c < p.kchunks; ++c) {
         for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ra.advance(p.na_stages)) {
           const int s = ra.slot();
@@ -238,6 +247,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
           }
           rm.fv0 = f0 + p.grp_qlo[g] * p.nsub;
           rm.nsub = p.nsub; rm.step = p.i_step; rm.rho = p.grp_rho[g]; rm.up = p.up; rm.t_lim = p.t_in * p.up;
+          if constexpr (MASK) { rm.t_lo = t_lo; rm.t_lim = t_lim; }
           stage_rows<5, SIMPLE, 3, STREAM>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
                                    min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
           fence_proxy_async();
@@ -758,7 +768,8 @@ extern "C" int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir) {
   return P.ok && P.launches[0].epi_staged ? 1 : 0;
 }
 
-static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, cudaStream_t st) {   // p: phases already planned
+static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, bool masked,
+                  cudaStream_t st) {   // p: phases already planned
   const size_t smem = size_stages(p);
   KT_REQUIRE(smem > 0, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
   const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
@@ -770,7 +781,13 @@ static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, cuda
     const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
                         (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
                         (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
-    if (stream && simple) {
+    if (masked && simple) {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple, true, true>>(kMaxDynSmem));
+      conv_tc_kernel<kTcRegSimple, true, true><<<grid, kTcThreads, smem, st>>>(p, maps);
+    } else if (masked) {
+      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg, true, true>>(kMaxDynSmem));
+      conv_tc_kernel<kTcReg, true, true><<<grid, kTcThreads, smem, st>>>(p, maps);
+    } else if (stream && simple) {
       KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple, true>>(kMaxDynSmem));
       conv_tc_kernel<kTcRegSimple, true><<<grid, kTcThreads, smem, st>>>(p, maps);
     } else if (stream) {
@@ -807,6 +824,7 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
     lp.out_act = io.out_act; lp.out_slope = io.out_slope;
     lp.in_pitch = io.in_pitch; lp.in_first = io.in_first; lp.out_pitch = io.out_pitch; lp.out_first = io.out_first;
     lp.res_pitch = io.res_pitch; lp.res_first = io.res_first;
+    lp.smask = io.smask;
     auto a16 = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
     // the staged epilogue reads at most one side operand (a forward has no mask, a data gradient no residual): fewer live
     // values, the register-staged instances are at their cap
@@ -816,7 +834,7 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
       const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what);
       if (rc) return rc;
     }
-    const int rc = run_tc(lp, maps, P.tma, io.in_pitch > 0, st);
+    const int rc = run_tc(lp, maps, P.tma, io.in_pitch > 0, io.smask.lengths != nullptr, st);
     if (rc) return rc;
   }
   return KT_OK;
@@ -837,15 +855,12 @@ extern "C" int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const voi
   return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", static_cast<cudaStream_t>(stream));
 }
 
-// One chunk of a stream (KtStreamWin): the register-staged route over the windows
-extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg,
-                                       const float* bias, const float* resid, float* y, void* stream) {
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
-  if (rc) return rc;
-  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
+// The register-staged route over the windows of one stream chunk; m: the input's utterance bounds (masked instances), or null
+static int conv_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x, const void* wimg,
+                          const float* bias, const float* resid, float* y, const char* what, cudaStream_t st) {
   const TcPlan P = make_tc_plan_flags(d, KT_PLAN_STREAM);
-  KT_REQUIRE(P.ok && !P.tma, "conv1d_fwd_tc_stream: layer not supported by the tensor-core path");
-  KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "conv1d_fwd_tc_stream: bad window pitch");
+  KT_REQUIRE(P.ok && !P.tma, "%s: layer not supported by the tensor-core path", what);
+  KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "%s: bad window pitch", what);
   TcParams io{};
   io.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
@@ -853,7 +868,27 @@ extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin*
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
   io.in_pitch = w->in_pitch; io.in_first = w->in_first; io.out_pitch = w->out_pitch; io.out_first = w->out_first;
   io.res_pitch = w->res_pitch; io.res_first = w->res_first;
-  return run_plan(P, io, nullptr, 0, "conv1d_fwd_tc_stream", static_cast<cudaStream_t>(stream));
+  if (m) io.smask = *m;
+  return run_plan(P, io, nullptr, 0, what, st);
+}
+
+// One chunk of a stream (KtStreamWin): the register-staged route over the windows
+extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg,
+                                       const float* bias, const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
+  return conv_tc_stream(d, w, nullptr, x, wimg, bias, resid, y, "conv1d_fwd_tc_stream", static_cast<cudaStream_t>(stream));
+}
+
+// The same over the utterance rows of each item only (KtStreamMask)
+extern "C" int kt_conv1d_fwd_tc_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                              const void* wimg, const float* bias, const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream_masked");
+  if (!rc) rc = validate_stream_mask(m, "kt_conv1d_fwd_tc_stream_masked");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream_masked: null pointer");
+  return conv_tc_stream(d, w, m, x, wimg, bias, resid, y, "conv1d_fwd_tc_stream_masked", static_cast<cudaStream_t>(stream));
 }
 
 int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,

@@ -317,6 +317,34 @@ extern "C" int kt_stream_reset(const KtWindow* wins, int32_t n, int32_t batch, c
   return KT_OK;
 }
 
+// One CTA per batch item: zero the item's chunk rows outside its utterance, then (after every thread has read
+// frames_done[b]) advance the item's frame count.
+__global__ void stream_mask_advance_kernel(const KtStreamMask m, float* __restrict__ y, int rows, int ch, int pitch, int first,
+                                           int frames) {
+  const int b = blockIdx.x;
+  int lo, hi;
+  stream_utterance_rows(m, b, lo, hi);
+  float* base = y + ((long long)b * pitch + first) * ch;
+  for (long long i = threadIdx.x; i < (long long)rows * ch; i += blockDim.x) {
+    const int t = (int)(i / ch);
+    if (t < lo || t >= hi) base[i] = 0.f;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) m.frames_done[b] += frames;
+}
+
+extern "C" int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t pitch,
+                                      int32_t first, int32_t frames, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_stream_mask(m, "stream_mask_advance");
+  if (rc) return rc;
+  KT_REQUIRE(y && batch > 0 && rows > 0 && ch > 0 && frames > 0 && first >= 0 && first + rows <= pitch,
+             "stream_mask_advance: bad arguments");
+  stream_mask_advance_kernel<<<batch, 256, 0, st>>>(*m, y, rows, ch, pitch, first, frames);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
 extern "C" int kt_dwt_db3_fwd(const float* x, float* y, int32_t batch, int32_t t, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && y && batch > 0 && t > 0, "dwt_fwd: bad arguments");

@@ -13,8 +13,10 @@ The NSF branch (``nsf_params``) is module plumbing over the same kernels and has
 of GPU budget: tests/test_gpu_pipeline.py is opt-in).  Out of scope (SURVEY.md section 8a): MultiSpecDiscriminator, PQMF.
 """
 import copy
+import ctypes
 import math
 from collections import namedtuple
+from dataclasses import replace
 
 import numpy as np
 import torch
@@ -22,7 +24,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtStreamMask, ptr
 from .stream import Windows, WindowTable, own_weight
 
 # --------------------------------------------------------------------------------------------
@@ -436,10 +438,11 @@ class Generator(nn.Module):
         y = self.forward_rows(x.transpose(1, 2).contiguous(), excitation)   # (B, T', 1)
         return y.transpose(1, 2)
 
-    def streamer(self, batch, max_frames):
+    def streamer(self, batch, max_frames, lengths=None):
         """-> a GeneratorStreamer that synthesises ``batch`` independent utterances chunk by chunk (at most ``max_frames``
-        mel frames per chunk), giving the waveform of this (causal, non-NSF, eval-mode) generator's forward."""
-        return GeneratorStreamer(self, batch, max_frames)
+        mel frames per chunk), giving the waveform of this (non-NSF, eval-mode) generator's forward.  A non-causal generator
+        needs each slot's utterance ``lengths`` in frames (host list or device tensor (batch,)); a causal one takes none."""
+        return GeneratorStreamer(self, batch, max_frames, lengths)
 
     def remove_weight_norm(self):
         print("Removing weight norm...")
@@ -458,7 +461,7 @@ class Generator(nn.Module):
 
 
 # --------------------------------------------------------------------------------------------
-# Streaming inference of the causal generator
+# Streaming inference of the generator
 # --------------------------------------------------------------------------------------------
 
 
@@ -470,107 +473,195 @@ def stream_history(spec):
     return -(-(spec.kernel - 1) * spec.dilation // spec.upsample)
 
 
-# The steps of a StreamPlan, over windows named by the plan: a conv of ``conv`` (a layer's conv1d or deconv) adding window
-# ``resid`` (or None), on side stream ``side`` of the parallel ResBlocks (None: the current stream); sin(x) + x; a mean.
-ConvStep = namedtuple("ConvStep", "conv src dst resid side")
+def stream_spec(spec):
+    """-> the causal form of a non-causal layer: a conv with all of its padding on the left, a transposed conv without
+    padding and cropped by k - s at the end.  It computes the layer's output ``stream_lag(spec)`` rows late."""
+    if spec.transposed:
+        return replace(spec, pad_left=0, crop=max(spec.kernel - spec.stride, 0))
+    return replace(spec, pad_left=(spec.kernel - 1) * spec.dilation, pad_right=0)
+
+
+def stream_lag(spec):
+    """Output rows by which the causal form of a non-causal layer trails it: the right padding (k-1)*d - pad_left of a
+    conv (in up-sampled rows), the padding p of a transposed conv (its output t reads inputs up to (t + p) / s)."""
+    if spec.transposed:
+        return spec.pad_left
+    return (spec.kernel - 1) * spec.dilation - spec.pad_left
+
+
+# The steps of a StreamPlan, over windows named by the plan: a conv of ``conv`` (a layer's conv1d or deconv), run as ``spec``
+# (the layer's spec, or its causal form), adding the rows of window ``resid`` (or None) that lie ``res_lag`` rows before the
+# chunk, on side stream ``side`` of the parallel ResBlocks (None: the current stream); sin(x) + x; a mean of sources read
+# ``offsets`` rows before the chunk.
+ConvStep = namedtuple("ConvStep", "conv src dst resid side spec res_lag")
 SinStep = namedtuple("SinStep", "src dst")
-MeanStep = namedtuple("MeanStep", "srcs dst scale")
+MeanStep = namedtuple("MeanStep", "srcs dst scale offsets")
 
 
 class StreamPlan:
     """What a GeneratorStreamer runs per chunk, as data (no device needed):
       windows             one entry per tensor of the chunk: {name, channels, rows_per_frame, history}; a tensor read by a
-                          conv keeps the largest history its consumers need, the others keep none
+                          conv keeps the largest history its consumers need, a residual or a mean source read n rows back
+                          keeps n, the others keep none
       layer_history       {layer name (as in named_modules): input rows before the chunk it reads}
+      lags                {window name: rows by which its newest row trails the newest pushed mel row}: all 0 for a causal
+                          generator.  A non-causal one runs every layer in its causal form (stream_spec), whose output
+                          trails the input's lag (times the layer's rate) by stream_lag rows
+      delay               the waveform's lag in samples: a chunk returns the samples ``delay`` before the pushed frames' own
+      causal              whether the generator is causal
       launches_per_chunk  library calls of a full chunk: one per conv (one kernel each on the tensor-core path), one per
-                          sin-add and per mean, one window advance; the mel chunk's copy into its window is not counted
+                          sin-add and per mean, one window advance and, non-causal, one output mask; the mel chunk's copy
+                          into its window is not counted
       steps               ConvStep | SinStep | MeanStep records, in launch order"""
 
     def __init__(self, gen):
         if gen.nsf_enable:
             raise ValueError("streaming needs a generator without NSF: the excitation draws fresh random phases and noise "
                              "per call, so chunks cannot reproduce the whole-utterance forward")
-        if not gen.conv_pre.causal:
-            raise ValueError("streaming needs a causal generator: a non-causal one reads ahead of every output sample")
         if gen.training:
             raise ValueError("streaming runs a generator in eval() mode")
+        self.causal = causal = gen.conv_pre.causal
         names = {m: n for n, m in gen.named_modules()}
         table = WindowTable()
-        self.windows, self.layer_history, self.steps = table.windows, {}, []
+        self.windows, self.layer_history, self.steps, self.lags = table.windows, {}, [], {}
+
+        def add(name, channels, rate=1):
+            self.lags[name] = 0
+            return table.add(name, channels, rate)
+
+        def layer(mod):
+            nc = mod.conv1d if hasattr(mod, "conv1d") else mod.deconv
+            return nc, nc.spec if causal else stream_spec(nc.spec)
+
+        def lag_of(mod, src):
+            """The lag of mod's output when it reads window src."""
+            nc, spec = layer(mod)
+            return 0 if causal else self.lags[src] * (spec.stride if spec.transposed else spec.upsample) + stream_lag(nc.spec)
 
         def conv(mod, src, dst, resid=None, side=None):
-            nc = mod.conv1d if hasattr(mod, "conv1d") else mod.deconv
-            h = stream_history(nc.spec)
+            nc, spec = layer(mod)
+            h = stream_history(spec)
             self.layer_history[names[mod]] = h
             table.read(src, h)
-            self.steps.append(ConvStep(nc, src, dst, resid, side))
+            self.lags[dst] = lag_of(mod, src)
+            res_lag = 0 if resid is None else self.lags[dst] - self.lags[resid]
+            if resid is not None:
+                assert res_lag >= 0
+                table.read(resid, res_lag)
+            self.steps.append(ConvStep(nc, src, dst, resid, side, spec, res_lag))
 
         nk, ch, rate = gen.num_kernels, gen.conv_pre.conv1d.spec.c_out, 1
-        mel = table.add("mel", gen.conv_pre.conv1d.spec.c_in)
-        x = table.add("x", ch)
+        mel = add("mel", gen.conv_pre.conv1d.spec.c_in)
+        x = add("x", ch)
         conv(gen.conv_pre, mel, x)
         for i in range(gen.num_upsamples):
             cin, s = ch >> i, gen.upsample_scales[i]
             cout = cin // 2
-            sx = table.add(f"sin{i}", cin, rate)
+            sx = add(f"sin{i}", cin, rate)
+            self.lags[sx] = self.lags[x]
             self.steps.append(SinStep(x, sx))
             rate *= s
-            rep = table.add(f"rep{i}", cout, rate)
-            conv(gen.repeat_upsamples[i][2], sx, rep)
-            up = table.add(f"up{i}", cout, rate)
-            conv(gen.transpose_upsamples[i][1], sx, up, resid=rep)
+            repm, upm = gen.repeat_upsamples[i][2], gen.transpose_upsamples[i][1]
+            rep = add(f"rep{i}", cout, rate)
+            up = add(f"up{i}", cout, rate)
+            # up + rep: the later of the two adds the other, read as many rows back as it trails (the deconv, unless its
+            # padding is the smaller right reach: k = 4, s = 2 against the k = 7 repeat conv)
+            if lag_of(upm, sx) >= lag_of(repm, sx):
+                conv(repm, sx, rep)
+                conv(upm, sx, up, resid=rep)
+                xin0 = up
+            else:
+                conv(upm, sx, up)
+                conv(repm, sx, rep, resid=up)
+                xin0 = rep
             outs = []
             for j in range(nk):
-                rb, xin = gen.conv_blocks[i * nk + j], up
+                rb, xin = gen.conv_blocks[i * nk + j], xin0
                 side = j if nk > 1 else None
                 for p, (c1, c2) in enumerate(zip(rb.convs1, rb.convs2)):
-                    h = table.add(f"rb{i}.{j}.h{p}", cout, rate)
+                    h = add(f"rb{i}.{j}.h{p}", cout, rate)
                     conv(c1, xin, h, side=side)
-                    xo = table.add(f"rb{i}.{j}.x{p + 1}", cout, rate)
+                    xo = add(f"rb{i}.{j}.x{p + 1}", cout, rate)
                     conv(c2, h, xo, resid=xin, side=side)
                     xin = xo
                 outs.append(xin)
-            x = table.add(f"mean{i}", cout, rate)
-            self.steps.append(MeanStep(outs, x, 1.0 / nk))
-        conv(gen.conv_post, x, table.add("wav", 1, rate))
+            x = add(f"mean{i}", cout, rate)
+            self.lags[x] = max(self.lags[o] for o in outs)
+            # the parallel ResBlocks trail their input by different right reaches: each is read at the mean's lag, and all
+            # keep the same history so that they share one pitch
+            offsets = [self.lags[x] - self.lags[o] for o in outs]
+            for o in outs:
+                table.read(o, max(offsets))
+            self.steps.append(MeanStep(outs, x, 1.0 / nk, offsets))
+        conv(gen.conv_post, x, add("wav", 1, rate))
         self.hop = rate
-        self.launches_per_chunk = table.launches_per_chunk(len(self.steps))
+        self.delay = self.lags["wav"]
+        self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + (not causal)
 
 
 class GeneratorStreamer:
-    """Chunk-by-chunk synthesis with a causal HiFi-GAN generator (Generator.streamer).
+    """Chunk-by-chunk synthesis with a HiFi-GAN generator (Generator.streamer).
 
     ``push(mel)`` takes the next (B, in_channels, f) mel frames of every batch slot (1 <= f <= max_frames, on the
-    generator's GPU) and returns their (B, 1, f * hop) waveform; concatenated, the outputs of any split of a mel equal the
-    generator's forward on the whole mel.  Each batch slot is an independent stream; ``reset(slots)`` starts new utterances
-    in the given slots.  ``push`` never waits for the device.
+    generator's GPU) and returns (B, 1, f * hop) waveform samples.  Each batch slot is an independent stream; ``reset(slots)``
+    starts new utterances in the given slots.  ``push`` never waits for the device.
 
-    Every tensor a causal layer reads lives in a window (stream.py) that its producer writes straight into.  A full-size
-    chunk replays a CUDA graph; a shorter chunk runs the same kernels eagerly.
+    Causal generator: concatenated, the outputs of any split of a mel equal the generator's forward on the whole mel.
+
+    Non-causal generator: a sample depends on mel frames after its own, so the output is delayed.  With p_b the samples of
+    the frames pushed to slot b since its reset, a push returns the samples [p_b - delay, p_b - delay + f * hop) of the
+    slot's utterance, of ``lengths[b]`` frames; positions outside [0, lengths[b] * hop) are 0, and frames pushed past
+    lengths[b] are ignored.  ``finish()`` pushes the ``drain_frames`` frames that bring out an utterance's last sample.
+    The chunks of slot b concatenated and cut to [delay, delay + lengths[b] * hop) equal the forward on the slot's mel of
+    exactly lengths[b] frames: every layer's zero padding at the utterance's end is applied per slot inside the conv
+    kernels (the _masked entry points), from lengths and frame counts kept on the device.  A slot reset before its
+    utterance has drained loses the samples not yet returned.
+
+    Every tensor a layer reads lives in a window (stream.py) that its producer writes straight into.  A full-size chunk
+    replays a CUDA graph; a shorter chunk runs the same kernels eagerly.
 
     The weights are prepared once, when the streamer is created: a generator whose parameters change later needs a new
     streamer.  Creating one also runs a chunk of zeros through every kernel, so that every kernel is loaded, captures the
     full-size chunk's graph, then clears the state; the capture synchronises the device once."""
 
-    def __init__(self, gen, batch, max_frames):
+    def __init__(self, gen, batch, max_frames, lengths=None):
         self.plan = plan = StreamPlan(gen)
+        if plan.causal and lengths is not None:
+            raise ValueError("a causal generator streams without lengths: its output does not depend on where an utterance "
+                             "ends")
+        if not plan.causal and lengths is None:
+            raise ValueError("streaming a non-causal generator needs per-slot lengths (a causal one needs none): its output "
+                             "near an utterance's end depends on where that end is")
         self._win = win = Windows(plan.windows, batch, max_frames, next(gen.parameters()).device, "streamer")
         self.batch, self.max_frames, self.hop, self.device = win.batch, win.max_frames, plan.hop, win.device
+        self.delay = plan.delay
+        self.drain_frames = -(-self.delay // self.hop)
         self.in_channels = plan.windows[0]["channels"]
-        self._places = [win.place(st.src, st.dst, st.resid) if type(st) is ConvStep else None for st in plan.steps]
+        self._places = [win.place(st.src, st.dst, st.resid, res_lag=st.res_lag) if type(st) is ConvStep else None
+                        for st in plan.steps]
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
         with torch.no_grad(), torch.cuda.device(self.device):
-            self._weights = {st.conv: own_weight(st.conv.spec, *st.conv.effective_weight(), st.conv.bias)
+            self._masks = None
+            if not plan.causal:
+                self._len = torch.zeros(self.batch, dtype=torch.int32, device=self.device)
+                self._done = torch.zeros(self.batch, dtype=torch.int32, device=self.device)
+                self._masks = {w["name"]: KtStreamMask(lengths=ptr(self._len, True), frames_done=ptr(self._done, True),
+                                                       rows_per_frame=w["rows_per_frame"], lag=plan.lags[w["name"]])
+                               for w in plan.windows}
+                self._zeros = torch.zeros(self.batch, self.in_channels, self.max_frames, device=self.device)
+            self._weights = {st.conv: own_weight(st.spec, *st.conv.effective_weight(), st.conv.bias)
                              for st in plan.steps if type(st) is ConvStep}
             self._run(self.max_frames)               # warm-up: every kernel and weight image of a full chunk
             self._graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self._graph):
                 self._run(self.max_frames)
             win.reset()
+            if not plan.causal:
+                self._set_lengths(range(self.batch), lengths)
 
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
-        win = self._win
+        win, masks = self._win, self._masks
         b, B = win.buf, self.batch
         cur = torch.cuda.current_stream()
         forked = False
@@ -583,17 +674,22 @@ class GeneratorStreamer:
             if type(st) is ConvStep:
                 pw, bias = self._weights[st.conv]
                 with torch.cuda.stream(self._side[side] if side is not None else cur):
-                    ops.stream_conv(st.conv.spec, pw, bias, b[st.src], b[st.dst], f * win.rate[st.src], place,
-                                    None if st.resid is None else b[st.resid])
+                    ops.stream_conv(st.spec, pw, bias, b[st.src], b[st.dst], f * win.rate[st.src], place,
+                                    None if st.resid is None else b[st.resid], None if masks is None else masks[st.src])
             elif type(st) is SinStep:
                 src, dst = b[st.src], b[st.dst]
                 ops.call("kt_sinadd_fwd_win", ptr(src), ptr(dst), B, f * win.rate[st.src], src.shape[2], src.shape[1],
                          dst.shape[1], win.first[st.dst])
             else:
-                dst = b[st.dst]
-                srcs = [b[s] for s in st.srcs] + [None] * (3 - len(st.srcs))
-                ops.call("kt_add3_scale_win", ptr(srcs[0]), ptr(srcs[1]), ptr(srcs[2]), st.scale, ptr(dst), B,
-                         f * win.rate[st.dst], dst.shape[2], srcs[0].shape[1], dst.shape[1], win.first[st.dst])
+                dst, ch = b[st.dst], b[st.dst].shape[2]
+                # source j's chunk starts `offsets[j]` rows before its own chunk row 0 (4-byte rows of ch floats)
+                srcs = [ptr(b[s]) + (win.first[s] - o) * ch * 4 for s, o in zip(st.srcs, st.offsets)] + [None] * (3 - len(st.srcs))
+                ops.call("kt_add3_scale_win", srcs[0], srcs[1], srcs[2], st.scale, ptr(dst), B, f * win.rate[st.dst], ch,
+                         b[st.srcs[0]].shape[1], dst.shape[1], win.first[st.dst])
+        if masks is not None:
+            wav = b["wav"]
+            ops.call("kt_stream_mask_advance", ctypes.byref(masks["wav"]), ptr(wav), B, f * self.hop, 1, wav.shape[1],
+                     win.first["wav"], f)
         win.advance(f)
 
     def push(self, mel):
@@ -606,10 +702,45 @@ class GeneratorStreamer:
                 self._run(f)
             return self._win.buf["wav"][:, :f * self.hop, 0].unsqueeze(1).clone(memory_format=torch.contiguous_format)
 
-    def reset(self, slots):
-        """The given batch slots start a new utterance: their carried state returns to zeros (one launch)."""
-        with torch.cuda.device(self.device):
+    def finish(self):
+        """Push ``drain_frames`` frames (in chunks of at most max_frames; their content is ignored) -> their (B, 1, n)
+        waveform, which ends with the last sample of every utterance pushed to its end.  (B, 1, 0) for a causal generator."""
+        with torch.no_grad(), torch.cuda.device(self.device):
+            outs, left = [], self.drain_frames
+            while left > 0:
+                f = min(left, self.max_frames)
+                outs.append(self.push(self._zeros[:, :, :f]))
+                left -= f
+            return torch.cat(outs, -1) if outs else torch.zeros(self.batch, 1, 0, device=self.device)
+
+    def reset(self, slots, lengths=None):
+        """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A non-causal
+        generator needs the new utterances' ``lengths`` in frames, in the order of ``slots``."""
+        slots = [int(s) for s in slots]
+        if self.plan.causal and lengths is not None:
+            raise ValueError("reset: a causal generator streams without lengths")
+        if not self.plan.causal and lengths is None:
+            raise ValueError("reset: streaming a non-causal generator needs the new utterances' lengths")
+        with torch.no_grad(), torch.cuda.device(self.device):
             self._win.reset(slots)
+            if not self.plan.causal:
+                self._set_lengths(slots, lengths)
+
+    def _set_lengths(self, slots, lengths):
+        """Slots ``slots`` hold utterances of ``lengths`` frames (host sequence or device tensor), none pushed yet."""
+        slots = list(slots)
+        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
+            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
+        if not (torch.is_tensor(lengths) and lengths.is_cuda):
+            lengths = torch.as_tensor(lengths)
+            if lengths.numel() and int(lengths.min()) < 1:
+                raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
+        n = lengths.to(device=self.device, dtype=torch.int32).reshape(-1)
+        if n.numel() != len(slots):
+            raise ValueError(f"streamer: expected {len(slots)} lengths, got {n.numel()}")
+        idx = torch.tensor(slots, dtype=torch.long).to(self.device)
+        self._len.index_copy_(0, idx, n)
+        self._done.index_fill_(0, idx, 0)
 
 
 # --------------------------------------------------------------------------------------------

@@ -37,7 +37,9 @@ def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_sp
     at ``lengths[b]`` are ``synthesize(...)[0][b]``."""
     if sambert.training or generator.training:
         raise RuntimeError("stream_synthesize() expects both models in eval() mode")
-    StreamPlan(generator)                                          # rejects non-causal and NSF generators
+    StreamPlan(generator)                                          # rejects NSF generators
+    if not generator.conv_pre.causal:                              # the vocoder streams here without a delay
+        raise ValueError("streaming needs a causal generator: a non-causal one reads ahead of every output sample")
     num_mels = sambert.mel_postnet.num_mels
     if generator.conv_pre.conv1d.spec.c_in != num_mels:
         raise ValueError(f"stream_synthesize(): the acoustic model makes {num_mels} mel channels, the generator takes "

@@ -571,21 +571,24 @@ def conv(x, spec, cache, v, g=None, bias=None, resid=None, reuse=None):
     return ConvFn.apply(x, resid, bias, v, g, spec, cache, reuse)
 
 
-def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None):
+def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None, mask=None):
     """One chunk of a causal layer in a stream (no autograd): x, y and resid are the layer's (B, pitch, C) windows, placed
     by ``win`` (a KtStreamWin), and ``t_in`` is the chunk's input rows; the taps before the chunk read the window's history.
     ``pw``: the layer's PreparedWeight, prepared by the caller.  Planned once per chunk shape (ConvSpec.plan, stream=True);
-    the tensor-core image of the plan's N tile is packed from ``pw`` on its first use."""
+    the tensor-core image of the plan's N tile is packed from ``pw`` on its first use.  ``mask`` (a KtStreamMask): the
+    input rows outside each item's utterance read as zeros (the _masked entry points)."""
     plan = spec.plan(x.shape[0], 1, t_in, stream=True)
     d, nt = plan.d, plan.tile(0)
+    m = () if mask is None else (ctypes.byref(mask),)
+    sfx = "" if mask is None else "_masked"
     if nt:
         img = pw.image((0, nt), d)
-        _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(img, True),
-                                            ptr(bias), ptr(resid), ptr(y)))
+        _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream" + sfx, ctypes.byref(d), ctypes.byref(win), *m, ptr(x),
+                                            ptr(img, True), ptr(bias), ptr(resid), ptr(y)))
     else:
         n = spec.stride if spec.transposed else 1
-        _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream", ctypes.byref(d), ctypes.byref(win), ptr(x), ptr(pw.w_fwd),
-                                              ptr(bias), ptr(resid), ptr(y)))
+        _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream" + sfx, ctypes.byref(d), ctypes.byref(win), *m, ptr(x),
+                                              ptr(pw.w_fwd), ptr(bias), ptr(resid), ptr(y)))
 
 
 # ---- pair_reuse: one (generated, real) pair batch per phase, the real half computed once per step -----------------------

@@ -6,7 +6,11 @@ B in {1, 16, 64} slots x F in {1, 4, 16} frames per chunk: the device time per g
 (audio seconds per chunk / chunk time; > 1 is faster than real time), and for comparison the whole-utterance forward of
 the same frames.  Prints the card and its power limit, read in the same run.
 
-    python scripts/stream_latency.py [--chunks 200] [--out DIR]"""
+--config noncausal: the same over the non-causal hifigan_noncausal_v1_16k.yaml generator (hop 200 at 16 kHz), streamed
+with per-slot lengths long enough that no utterance ends during the run; its rows also give the stream's look-ahead
+(delay_ms: the audio a sample waits for) on top of the chunk's own audio.
+
+    python scripts/stream_latency.py [--config causal|noncausal] [--chunks 200] [--out DIR]"""
 import argparse
 import json
 import os
@@ -20,8 +24,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import kantts_b200 as K  # noqa: E402
 
 GENERATORS = {
-    "default_22k": (dict(), 22050),
-    "v1_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),
+    "causal": {
+        "default_22k": (dict(), 22050),
+        "v1_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),
+    },
+    "noncausal": {
+        "noncausal_v1_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
+                                  resblock_dilations=[[1, 3, 5, 7]] * 3, causal=False), 16000),
+    },
 }
 # the whole-utterance forward keeps every activation of the utterance: longer ones are timed at this many frames
 WHOLE_MAX_ROWS = 64 * 256
@@ -34,7 +44,8 @@ def card():
 
 
 def measure(gen, sr, B, F, chunks):
-    st = gen.streamer(batch=B, max_frames=F)
+    lengths = None if gen.conv_pre.causal else [1 << 24] * B
+    st = gen.streamer(batch=B, max_frames=F, lengths=lengths)
     mel = torch.randn(B, 80, F, device="cuda")
     for _ in range(10):                                  # the first push captures the graph
         st.push(mel)
@@ -66,11 +77,12 @@ def measure(gen, sr, B, F, chunks):
     return dict(B=B, F=F, chunk_ms=round(chunk_ms, 4), host_enqueue_ms=round(1e3 * host / chunks, 4),
                 launches_per_chunk=st.plan.launches_per_chunk, rtf=round(audio_s / (chunk_ms / 1e3), 2),
                 latency_audio_ms=round(1e3 * audio_s, 2), whole_frames=frames, whole_ms=round(whole_ms, 3),
-                whole_rtf=round(frames * st.hop / sr / (whole_ms / 1e3), 2))
+                whole_rtf=round(frames * st.hop / sr / (whole_ms / 1e3), 2), delay_ms=round(1e3 * st.delay / sr, 2))
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--config", choices=sorted(GENERATORS), default="causal")
     ap.add_argument("--chunks", type=int, default=200)
     ap.add_argument("--out", default=None, help="also write the rows as DIR/stream_latency.json")
     args = ap.parse_args()
@@ -79,7 +91,7 @@ def main():
     info = card()
     print(f"card: {info}")
     rows = []
-    for name, (cfg, sr) in GENERATORS.items():
+    for name, (cfg, sr) in GENERATORS[args.config].items():
         torch.manual_seed(0)
         gen = K.Generator(**cfg).cuda().eval()
         for B in (1, 16, 64):
@@ -89,7 +101,8 @@ def main():
                 print(json.dumps(r), flush=True)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "stream_latency.json"), "w") as f:
+        suffix = "" if args.config == "causal" else "_" + args.config
+        with open(os.path.join(args.out, f"stream_latency{suffix}.json"), "w") as f:
             json.dump(dict(card=info, rows=rows), f, indent=1)
 
 
