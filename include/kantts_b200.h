@@ -415,6 +415,32 @@ int kt_fsmn_fwd_stream(const KtStreamWin* w, const float* x, const float* weight
 int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t batch, int32_t rows, int32_t hidden,
                    int32_t gx_pitch, int32_t h_pitch, void* stream);
 
+/* ---- seeded NSF excitation (SourceModule, kantts/models/hifigan/layers.py:229-290) ---------------------------------------
+ * kt_nsf_excitation: the sine-plus-noise excitation of `frames` frames of `batch` slots as a deterministic function of each
+ * slot's seed, its f0 / voiced flag and the sample index -- a chunk's rows equal the matching rows of the whole utterance's.
+ *   f0uv  row j of item b at f0uv[(b * f0uv_pitch + f0uv_first + j) * 2]: (f0 in Hz, voiced flag)
+ *   e     row r of item b at e[(b * e_pitch + e_first + r) * (H + 1)], r = j * hop + i, 0 <= i < hop: the H + 1 harmonics
+ *   state seeds [batch] (device int64), phase [batch][H + 1] (device float64), samples_done [batch] (device int64);
+ *         phase and samples_done are advanced by the call (zeros start an utterance), seeds are only read.
+ * With h = 0..H the harmonic, n = samples_done[b] + r the sample index since the slot's reset, seed = (k0 low word, k1 high):
+ *   c_{h,j} = f0_j * (h + 1) / sr                       float64
+ *   P_{h,j+1} = frac(P_{h,j} + hop * c_{h,j})           float64, P_{h,0} = phase[b][h] (the only order-dependent sum)
+ *   theta = (float) 2 pi frac(P_{h,j} + (i + 1) c_{h,j})   (the reference's inclusive cumsum)
+ *   phi_h = (float)(-pi + 2 pi w0 2^-32), (w0..w3) = Philox4x32-10(counter (0, 0, h, 1), key (k0, k1));  phi_0 = 0
+ *   z = (float)(sqrt(-2 log u1) cos(2 pi u2)), u_k = (w_{k-1} + 0.5) 2^-32 in float64, (w0..w3) = Philox4x32-10((n low,
+ *       n high, h, 0), (k0, k1))
+ *   e = (alpha sin(theta + phi) + sigma z) uv + (k (sigma z)) (1 - uv),  k = (float)((double)alpha / 3 / (double)sigma)
+ * in float32, every operation rounded as written (no contraction, no fast-math); sr = sampling_rate.  The reference uses
+ * alpha 0.1, sigma 0.003.  nb_harmonics H < 32.  Two launches (the rows, then the state). */
+typedef struct KtNsfState {
+  const int64_t* seeds;
+  double* phase;
+  int64_t* samples_done;
+} KtNsfState;
+int kt_nsf_excitation(const float* f0uv, int32_t f0uv_pitch, int32_t f0uv_first, const KtNsfState* s, float* e,
+                      int32_t e_pitch, int32_t e_first, int32_t batch, int32_t frames, int32_t hop, int32_t nb_harmonics,
+                      int32_t sampling_rate, float alpha, float sigma, void* stream);
+
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libkantts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu"]
+SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
@@ -47,6 +47,10 @@ class KtWindow(ctypes.Structure):
 class KtStreamMask(ctypes.Structure):
     _fields_ = [("lengths", ctypes.c_void_p), ("frames_done", ctypes.c_void_p), ("rows_per_frame", ctypes.c_int32),
                 ("lag", ctypes.c_int32)]
+
+
+class KtNsfState(ctypes.Structure):
+    _fields_ = [("seeds", ctypes.c_void_p), ("phase", ctypes.c_void_p), ("samples_done", ctypes.c_void_p)]
 
 
 class KtMelDesc(ctypes.Structure):
@@ -123,6 +127,7 @@ PROTOTYPES = {
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_debug_conv_tc_epilogue": [ctypes.POINTER(KtConv1dDesc), _I],
@@ -142,7 +147,7 @@ def nvcc_command(out_path=LIB_PATH):
 def build_library(force=False, verbose=False):
     """Compile libkantts_b200.so in-tree for sm_90a (cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, h) for h in ("common.cuh", "tc_common.cuh", "tma.cuh", "wgmma.cuh")] + [
+    deps = srcs + [os.path.join(CSRC, h) for h in ("common.cuh", "tc_common.cuh", "tma.cuh", "wgmma.cuh", "philox.cuh")] + [
                    os.path.join(os.path.dirname(_HERE), "include", "kantts_b200.h")]
     deps = [d for d in deps if os.path.exists(d)]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
@@ -183,7 +188,7 @@ def check(rc, what):
 
 
 _PTR_DTYPES = (torch.float32,)
-_AUX_DTYPES = (torch.uint8, torch.int32, torch.int64, torch.bfloat16)   # masks / keep-masks, gather indices, filled-pause labels, packed tensor-core weight tiles
+_AUX_DTYPES = (torch.uint8, torch.int32, torch.int64, torch.bfloat16, torch.float64)   # masks / keep-masks, gather indices, filled-pause labels, packed tensor-core weight tiles, NSF phase carry
 
 
 def ptr(t, aux=False):

@@ -24,7 +24,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtStreamMask, ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, KtStreamMask, ptr
 from .stream import Windows, WindowTable, own_weight
 
 # --------------------------------------------------------------------------------------------
@@ -297,8 +297,12 @@ class SourceModule(nn.Module):
         spec.act_out = KT_ACT_TANH
         self.ffn = nn.Sequential(_NormedConv(ref, spec, "weight"), nn.Tanh())    # keys ffn.0.{bias,weight_g,weight_v}
 
-    def excitation(self, pitch, uv):
-        """(B, 1, frames) pitch in Hz and voiced flag -> (B, samples, nb_harmonics + 1) rows (no gradient)."""
+    def excitation(self, pitch, uv, seeds=None):
+        """(B, 1, frames) pitch in Hz and voiced flag -> (B, samples, nb_harmonics + 1) rows (no gradient).  With ``seeds``
+        (one per batch item: a host sequence or a device int64 tensor (B,)) the excitation is kt_nsf_excitation's seeded
+        function of (seed, pitch, uv, sample index) instead of the reference's draw from the global CPU generator."""
+        if seeds is not None:
+            return self._seeded_excitation(pitch, uv, seeds)
         from torch.distributions.normal import Normal
         from torch.distributions.uniform import Uniform
         with torch.no_grad():
@@ -316,14 +320,65 @@ class SourceModule(nn.Module):
             e = e_voice * uv_s + e_unvoice * (1 - uv_s)
             return e.transpose(1, 2).contiguous()
 
-    def forward_rows(self, pitch, uv):
-        return self.ffn[0].run(self.excitation(pitch, uv))          # (B, samples, 1)
+    def _seeded_excitation(self, pitch, uv, seeds):
+        if not pitch.is_cuda:
+            raise RuntimeError("kantts_b200: the seeded NSF excitation runs on a CUDA device (no CPU fallback)")
+        B, _, frames = pitch.shape
+        with torch.no_grad(), torch.cuda.device(pitch.device):
+            state = NsfState(self, nsf_seed_tensor(seeds, B, pitch.device))
+            f0uv = torch.cat([pitch, uv], 1).transpose(1, 2).float().contiguous()         # (B, frames, 2)
+            e = torch.empty(B, frames * self.upsample_ratio, self.nb_harmonics + 1, device=pitch.device)
+            self.run_excitation(f0uv, 0, state, e, 0, frames)
+            return e
 
-    def forward(self, pitch, uv):
-        return self.forward_rows(pitch, uv).transpose(1, 2)
+    def run_excitation(self, f0uv, f0uv_first, state, e, e_first, frames):
+        """kt_nsf_excitation: rows [f0uv_first, + frames) of the (B, pitch, 2) f0 / uv window -> rows [e_first, + frames * hop)
+        of the (B, pitch, nb_harmonics + 1) excitation window; advances ``state`` (an NsfState) on the device."""
+        ops.call("kt_nsf_excitation", ptr(f0uv), f0uv.shape[1], f0uv_first, ctypes.byref(state.desc), ptr(e), e.shape[1],
+                 e_first, f0uv.shape[0], frames, self.upsample_ratio, self.nb_harmonics, int(self.sampling_rate),
+                 float(self.alpha), float(self.sigma), launches=2)
+
+    def forward_rows(self, pitch, uv, seeds=None):
+        return self.ffn[0].run(self.excitation(pitch, uv, seeds))   # (B, samples, 1)
+
+    def forward(self, pitch, uv, seeds=None):
+        return self.forward_rows(pitch, uv, seeds).transpose(1, 2)
 
     def remove_weight_norm(self):
         self.ffn[0].remove_weight_norm()
+
+
+def nsf_seed_tensor(seeds, n, device):
+    """-> ``seeds`` (a host sequence of ints or an int64 tensor) as a device int64 tensor (n,); ValueError on a wrong
+    count or dtype."""
+    if torch.is_tensor(seeds):
+        if seeds.dtype != torch.int64:
+            raise ValueError(f"NSF seeds must be int64, got {seeds.dtype}")
+        s = seeds.reshape(-1)
+    else:
+        s = torch.as_tensor([int(v) for v in seeds], dtype=torch.int64)
+    if s.numel() != n:
+        raise ValueError(f"expected {n} NSF seeds (one per slot), got {s.numel()}")
+    return s.to(device)
+
+
+class NsfState:
+    """The device state of kt_nsf_excitation for a batch: seeds (B,) int64, phase (B, nb_harmonics + 1) float64 and
+    samples_done (B,) int64 (zeros: every slot at the start of its utterance), and the KtNsfState pointing at them."""
+
+    def __init__(self, source, seeds):
+        dev = seeds.device
+        self.seeds = seeds.contiguous()
+        self.phase = torch.zeros(seeds.numel(), source.nb_harmonics + 1, dtype=torch.float64, device=dev)
+        self.samples_done = torch.zeros(seeds.numel(), dtype=torch.int64, device=dev)
+        self.desc = KtNsfState(seeds=ptr(self.seeds, True), phase=ptr(self.phase, True),
+                               samples_done=ptr(self.samples_done, True))
+
+    def reset(self, idx, seeds):
+        """Slots ``idx`` (device long tensor) start new utterances with ``seeds`` (device int64, same length)."""
+        self.seeds.index_copy_(0, idx, seeds)
+        self.phase.index_fill_(0, idx, 0.0)
+        self.samples_done.index_fill_(0, idx, 0)
 
 
 # --------------------------------------------------------------------------------------------
@@ -428,21 +483,26 @@ class Generator(nn.Module):
             x = ops.Mean3Fn.apply(1.0 / self.num_kernels, *rs)               # :170-176
         return self.conv_post.forward_rows(x)                                # :178-180
 
-    def forward(self, x):
+    def forward(self, x, nsf_seeds=None):
         """x: (B, in_channels, T) -> (B, 1, T * prod(scales)); with ``nsf_params`` the last two channels are the
-        pitch (Hz) and the voiced flag (hifigan.py:146-150)."""
+        pitch (Hz) and the voiced flag (hifigan.py:146-150).  ``nsf_seeds`` (NSF only; one per batch item, host sequence
+        or device int64 tensor): the excitation is the seeded kt_nsf_excitation instead of the reference's random draw, so
+        that the output is a function of (x, seeds) -- the one a streamer with the same seeds computes."""
+        if nsf_seeds is not None and not self.nsf_enable:
+            raise ValueError("nsf_seeds: this generator has no NSF source module")
         excitation = None
         if self.nsf_enable:
             x, pitch, uv = x[:, :-2, :], x[:, -2:-1, :], x[:, -1:, :]
-            excitation = self.source_module.forward_rows(pitch, uv)         # (B, samples, 1)
+            excitation = self.source_module.forward_rows(pitch, uv, nsf_seeds)   # (B, samples, 1)
         y = self.forward_rows(x.transpose(1, 2).contiguous(), excitation)   # (B, T', 1)
         return y.transpose(1, 2)
 
-    def streamer(self, batch, max_frames, lengths=None):
+    def streamer(self, batch, max_frames, lengths=None, seeds=None):
         """-> a GeneratorStreamer that synthesises ``batch`` independent utterances chunk by chunk (at most ``max_frames``
-        mel frames per chunk), giving the waveform of this (non-NSF, eval-mode) generator's forward.  A non-causal generator
-        needs each slot's utterance ``lengths`` in frames (host list or device tensor (batch,)); a causal one takes none."""
-        return GeneratorStreamer(self, batch, max_frames, lengths)
+        mel frames per chunk), giving the waveform of this (eval-mode) generator's forward.  A non-causal generator
+        needs each slot's utterance ``lengths`` in frames (host list or device tensor (batch,)); a causal one takes none.
+        An NSF generator needs each slot's excitation ``seeds`` (as ``forward``'s ``nsf_seeds``); others take none."""
+        return GeneratorStreamer(self, batch, max_frames, lengths, seeds)
 
     def remove_weight_norm(self):
         print("Removing weight norm...")
@@ -466,27 +526,40 @@ class Generator(nn.Module):
 
 
 def stream_history(spec):
-    """Input rows before a chunk that one causal layer reads: (k-1)*d for a conv, ceil((k-1)*d / s) for the conv over the
-    nearest-upsampled (by s) input, floor((k-1) / s) for the cropped transposed conv with stride s (1 when k = 2s)."""
+    """Input rows before a chunk that one causal-form layer reads: its left padding for a conv -- (k-1)*d, or less for a
+    strided one (stream_spec) -- ceil((k-1)*d / s) for the conv over the nearest-upsampled (by s) input, floor((k-1) / s)
+    for the cropped transposed conv with stride s (1 when k = 2s)."""
     if spec.transposed:
         return (spec.kernel - 1) // spec.stride
-    return -(-(spec.kernel - 1) * spec.dilation // spec.upsample)
+    return -(-spec.pad_left // spec.upsample)
 
 
-def stream_spec(spec):
-    """-> the causal form of a non-causal layer: a conv with all of its padding on the left, a transposed conv without
-    padding and cropped by k - s at the end.  It computes the layer's output ``stream_lag(spec)`` rows late."""
+def stream_spec(spec, in_lag=0):
+    """-> the causal form of a non-causal layer whose input trails by ``in_lag`` rows: a conv with all of its padding on
+    the left, a transposed conv without padding and cropped by k - s at the end.  It computes the layer's output
+    ``stream_lag(spec, in_lag)`` rows late.  A conv with stride s reads, for output t of the chunk, input rows
+    t*s + j*d - P: with the lag L of stream_lag, P = L*s + pad_left - in_lag lines those rows up with the non-causal layer's
+    (P = (k-1)*d for s = 1), and P + pad_right = (k-1)*d keeps a chunk of n*s input rows at n output rows."""
     if spec.transposed:
         return replace(spec, pad_left=0, crop=max(spec.kernel - spec.stride, 0))
-    return replace(spec, pad_left=(spec.kernel - 1) * spec.dilation, pad_right=0)
+    reach = (spec.kernel - 1) * spec.dilation
+    left = stream_lag(spec, in_lag) * spec.stride + spec.pad_left - in_lag * spec.upsample
+    assert left >= 0, (spec, in_lag)
+    return replace(spec, pad_left=left, pad_right=reach - left)
 
 
-def stream_lag(spec):
-    """Output rows by which the causal form of a non-causal layer trails it: the right padding (k-1)*d - pad_left of a
-    conv (in up-sampled rows), the padding p of a transposed conv (its output t reads inputs up to (t + p) / s)."""
+def stream_lag(spec, in_lag=0):
+    """Output rows by which the causal form of a non-causal layer trails its non-causal output when the input trails by
+    ``in_lag`` rows.  A transposed conv: in_lag*s + its padding p (its output t reads inputs up to (t + p) / s).  A conv with
+    stride s over the input up-sampled by u (s = 1 or u = 1): the input lag in its rows, L_in = in_lag*u, plus the right
+    reach (k-1)*d - pad_left, in whole output rows -- the last output of a chunk may read at most its last input row:
+    ceil((L_in + (k-1)*d - pad_left - (s-1)) / s), and not below 0.  For s = 1 that is L_in + (k-1)*d - pad_left; for the
+    NSF source convs (k = 2s, pad_left = s // 2) from an input of lag 0 it is 1."""
     if spec.transposed:
-        return spec.pad_left
-    return (spec.kernel - 1) * spec.dilation - spec.pad_left
+        return in_lag * spec.stride + spec.pad_left
+    assert spec.stride == 1 or spec.upsample == 1, spec
+    s = spec.stride
+    return max(0, -(-(in_lag * spec.upsample + (spec.kernel - 1) * spec.dilation - spec.pad_left - (s - 1)) // s))
 
 
 # The steps of a StreamPlan, over windows named by the plan: a conv of ``conv`` (a layer's conv1d or deconv), run as ``spec``
@@ -496,6 +569,8 @@ def stream_lag(spec):
 ConvStep = namedtuple("ConvStep", "conv src dst resid side spec res_lag")
 SinStep = namedtuple("SinStep", "src dst")
 MeanStep = namedtuple("MeanStep", "srcs dst scale offsets")
+# the seeded NSF excitation (kt_nsf_excitation) of the chunk's f0 / uv rows in window src into window dst
+ExciteStep = namedtuple("ExciteStep", "src dst")
 
 
 class StreamPlan:
@@ -510,17 +585,20 @@ class StreamPlan:
       delay               the waveform's lag in samples: a chunk returns the samples ``delay`` before the pushed frames' own
       causal              whether the generator is causal
       launches_per_chunk  library calls of a full chunk: one per conv (one kernel each on the tensor-core path), one per
-                          sin-add and per mean, one window advance and, non-causal, one output mask; the mel chunk's copy
-                          into its window is not counted
-      steps               ConvStep | SinStep | MeanStep records, in launch order"""
+                          sin-add and per mean, one window advance and, non-causal, one output mask; NSF adds the
+                          excitation, its 1x1 ffn conv, one source conv per stage and, where the stage sum cannot be chained
+                          in the forward's order, one three-way add per stage; the mel chunk's copy into its window is not
+                          counted
+      nsf                 whether the generator has the NSF source: the last two input channels (f0, uv) go to window
+                          "f0uv", the excitation (kt_nsf_excitation, seeded per slot) to "exc" and its ffn to "source" (rate
+                          hop); stage i adds source_downs[i] of "source", in the forward's order up + (e + rep)
+      steps               ConvStep | SinStep | MeanStep | ExciteStep records, in launch order"""
 
     def __init__(self, gen):
-        if gen.nsf_enable:
-            raise ValueError("streaming needs a generator without NSF: the excitation draws fresh random phases and noise "
-                             "per call, so chunks cannot reproduce the whole-utterance forward")
         if gen.training:
             raise ValueError("streaming runs a generator in eval() mode")
         self.causal = causal = gen.conv_pre.causal
+        self.nsf = nsf = gen.nsf_enable
         names = {m: n for n, m in gen.named_modules()}
         table = WindowTable()
         self.windows, self.layer_history, self.steps, self.lags = table.windows, {}, [], {}
@@ -529,17 +607,17 @@ class StreamPlan:
             self.lags[name] = 0
             return table.add(name, channels, rate)
 
-        def layer(mod):
-            nc = mod.conv1d if hasattr(mod, "conv1d") else mod.deconv
-            return nc, nc.spec if causal else stream_spec(nc.spec)
+        def layer(mod, src):
+            nc = mod.conv1d if hasattr(mod, "conv1d") else getattr(mod, "deconv", mod)     # (the NSF ffn is the conv itself)
+            return nc, nc.spec if causal else stream_spec(nc.spec, self.lags[src])
 
         def lag_of(mod, src):
             """The lag of mod's output when it reads window src."""
-            nc, spec = layer(mod)
-            return 0 if causal else self.lags[src] * (spec.stride if spec.transposed else spec.upsample) + stream_lag(nc.spec)
+            nc, _ = layer(mod, src)
+            return 0 if causal else stream_lag(nc.spec, self.lags[src])
 
         def conv(mod, src, dst, resid=None, side=None):
-            nc, spec = layer(mod)
+            nc, spec = layer(mod, src)
             h = stream_history(spec)
             self.layer_history[names[mod]] = h
             table.read(src, h)
@@ -550,8 +628,24 @@ class StreamPlan:
                 table.read(resid, res_lag)
             self.steps.append(ConvStep(nc, src, dst, resid, side, spec, res_lag))
 
+        def mean(srcs, dst, scale):
+            """dst = scale * (srcs summed in order), read at dst's lag, the latest of theirs: every source keeps the same
+            history, so that they share one pitch"""
+            self.lags[dst] = max(self.lags[o] for o in srcs)
+            offsets = [self.lags[dst] - self.lags[o] for o in srcs]
+            for o in srcs:
+                table.read(o, max(offsets))
+            self.steps.append(MeanStep(srcs, dst, scale, offsets))
+
         nk, ch, rate = gen.num_kernels, gen.conv_pre.conv1d.spec.c_out, 1
+        hop = int(np.prod(gen.upsample_scales))
         mel = add("mel", gen.conv_pre.conv1d.spec.c_in)
+        if nsf:
+            sm = gen.source_module
+            f0uv, exc = add("f0uv", 2), add("exc", sm.nb_harmonics + 1, hop)
+            self.steps.append(ExciteStep(f0uv, exc))
+            source = add("source", 1, hop)
+            conv(sm.ffn[0], exc, source)
         x = add("x", ch)
         conv(gen.conv_pre, mel, x)
         for i in range(gen.num_upsamples):
@@ -564,9 +658,30 @@ class StreamPlan:
             repm, upm = gen.repeat_upsamples[i][2], gen.transpose_upsamples[i][1]
             rep = add(f"rep{i}", cout, rate)
             up = add(f"up{i}", cout, rate)
+            if nsf:
+                # up + (e + rep), e = source_downs[i] of the source: the forward's order, kept bit for bit.  When the deconv
+                # trails the other two, it is last and adds e + rep, itself formed by the later of the two (float addition
+                # commutes); otherwise one three-way add (e + rep) + up at the latest lag
+                dm = gen.source_downs[i]
+                spec = dm.conv1d.spec
+                assert spec.t_out(7 * spec.stride) == 7, f"source_downs[{i}]: {spec} does not bring the source to the stage rate"
+                e = add(f"e{i}", cout, rate)
+                l_rep, l_up, l_e = lag_of(repm, sx), lag_of(upm, sx), lag_of(dm, source)
+                if l_up >= max(l_rep, l_e):
+                    first, second = ((repm, sx, rep), (dm, source, e)) if l_e >= l_rep else ((dm, source, e), (repm, sx, rep))
+                    conv(*first)
+                    conv(*second, resid=first[2])
+                    conv(upm, sx, up, resid=second[2])
+                    xin0 = up
+                else:
+                    conv(repm, sx, rep)
+                    conv(dm, source, e)
+                    conv(upm, sx, up)
+                    xin0 = add(f"sum{i}", cout, rate)
+                    mean([e, rep, up], xin0, 1.0)
             # up + rep: the later of the two adds the other, read as many rows back as it trails (the deconv, unless its
             # padding is the smaller right reach: k = 4, s = 2 against the k = 7 repeat conv)
-            if lag_of(upm, sx) >= lag_of(repm, sx):
+            elif lag_of(upm, sx) >= lag_of(repm, sx):
                 conv(repm, sx, rep)
                 conv(upm, sx, up, resid=rep)
                 xin0 = up
@@ -585,15 +700,14 @@ class StreamPlan:
                     conv(c2, h, xo, resid=xin, side=side)
                     xin = xo
                 outs.append(xin)
+            # the parallel ResBlocks trail their input by different right reaches: each is read at the mean's lag
             x = add(f"mean{i}", cout, rate)
-            self.lags[x] = max(self.lags[o] for o in outs)
-            # the parallel ResBlocks trail their input by different right reaches: each is read at the mean's lag, and all
-            # keep the same history so that they share one pitch
-            offsets = [self.lags[x] - self.lags[o] for o in outs]
-            for o in outs:
-                table.read(o, max(offsets))
-            self.steps.append(MeanStep(outs, x, 1.0 / nk, offsets))
+            mean(outs, x, 1.0 / nk)
         conv(gen.conv_post, x, add("wav", 1, rate))
+        assert rate == hop
+        hist = {w["name"]: w["history"] for w in self.windows}
+        for st in self.steps:                  # kt_add3_scale_win reads its sources at one pitch
+            assert type(st) is not MeanStep or len({hist[o] for o in st.srcs}) == 1, st
         self.hop = rate
         self.delay = self.lags["wav"]
         self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + (not causal)
@@ -617,6 +731,11 @@ class GeneratorStreamer:
     kernels (the _masked entry points), from lengths and frame counts kept on the device.  A slot reset before its
     utterance has drained loses the samples not yet returned.
 
+    NSF generator: ``push`` takes (B, in_channels + 2, f) -- mel, f0 in Hz and the voiced flag, as ``forward`` -- and each
+    slot's excitation is seeded by its ``seeds`` entry (``reset`` takes the new slots' seeds).  The excitation is computed
+    per chunk on the device, its phases and sample count carried per slot, so the output equals ``forward(x, nsf_seeds)``
+    of the slot's whole utterance with that seed.
+
     Every tensor a layer reads lives in a window (stream.py) that its producer writes straight into.  A full-size chunk
     replays a CUDA graph; a shorter chunk runs the same kernels eagerly.
 
@@ -624,8 +743,15 @@ class GeneratorStreamer:
     streamer.  Creating one also runs a chunk of zeros through every kernel, so that every kernel is loaded, captures the
     full-size chunk's graph, then clears the state; the capture synchronises the device once."""
 
-    def __init__(self, gen, batch, max_frames, lengths=None):
+    def __init__(self, gen, batch, max_frames, lengths=None, seeds=None):
         self.plan = plan = StreamPlan(gen)
+        if plan.nsf and seeds is None:
+            raise ValueError("streaming an NSF generator needs per-slot seeds: its excitation is a seeded function of the "
+                             "sample index, so that chunks reproduce the whole-utterance forward(x, nsf_seeds)")
+        if not plan.nsf and seeds is not None:
+            raise ValueError("streamer: seeds are for NSF generators; this one has no NSF source module")
+        if seeds is not None:
+            seeds = nsf_seed_tensor(seeds, int(batch), torch.device("cpu") if not torch.is_tensor(seeds) else seeds.device)
         if plan.causal and lengths is not None:
             raise ValueError("a causal generator streams without lengths: its output does not depend on where an utterance "
                              "ends")
@@ -636,9 +762,10 @@ class GeneratorStreamer:
         self.batch, self.max_frames, self.hop, self.device = win.batch, win.max_frames, plan.hop, win.device
         self.delay = plan.delay
         self.drain_frames = -(-self.delay // self.hop)
-        self.in_channels = plan.windows[0]["channels"]
+        self.in_channels = plan.windows[0]["channels"] + (2 if plan.nsf else 0)
         self._places = [win.place(st.src, st.dst, st.resid, res_lag=st.res_lag) if type(st) is ConvStep else None
                         for st in plan.steps]
+        self._source = gen.source_module if plan.nsf else None
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
         with torch.no_grad(), torch.cuda.device(self.device):
             self._masks = None
@@ -651,6 +778,8 @@ class GeneratorStreamer:
                 self._zeros = torch.zeros(self.batch, self.in_channels, self.max_frames, device=self.device)
             self._weights = {st.conv: own_weight(st.spec, *st.conv.effective_weight(), st.conv.bias)
                              for st in plan.steps if type(st) is ConvStep}
+            self._nsf = NsfState(self._source, torch.zeros(self.batch, dtype=torch.int64, device=self.device)) \
+                if plan.nsf else None
             self._run(self.max_frames)               # warm-up: every kernel and weight image of a full chunk
             self._graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self._graph):
@@ -658,6 +787,8 @@ class GeneratorStreamer:
             win.reset()
             if not plan.causal:
                 self._set_lengths(range(self.batch), lengths)
+            if plan.nsf:
+                self._set_seeds(range(self.batch), seeds)
 
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
@@ -676,6 +807,8 @@ class GeneratorStreamer:
                 with torch.cuda.stream(self._side[side] if side is not None else cur):
                     ops.stream_conv(st.spec, pw, bias, b[st.src], b[st.dst], f * win.rate[st.src], place,
                                     None if st.resid is None else b[st.resid], None if masks is None else masks[st.src])
+            elif type(st) is ExciteStep:
+                self._source.run_excitation(b[st.src], win.first[st.src], self._nsf, b[st.dst], win.first[st.dst], f)
             elif type(st) is SinStep:
                 src, dst = b[st.src], b[st.dst]
                 ops.call("kt_sinadd_fwd_win", ptr(src), ptr(dst), B, f * win.rate[st.src], src.shape[2], src.shape[1],
@@ -693,9 +826,16 @@ class GeneratorStreamer:
         win.advance(f)
 
     def push(self, mel):
-        """mel: (B, in_channels, f), 1 <= f <= max_frames, on the streamer's device -> the (B, 1, f * hop) waveform."""
+        """mel: (B, in_channels, f), 1 <= f <= max_frames, on the streamer's device -> the (B, 1, f * hop) waveform.  NSF:
+        the last two of the in_channels are f0 (Hz) and the voiced flag."""
         with torch.no_grad(), torch.cuda.device(self.device):
-            f = self._win.push("mel", mel, 2, ("a {} mel", "frames", "the mel is"))
+            if self.plan.nsf:
+                if mel.dim() != 3 or mel.shape[1] != self.in_channels:
+                    raise ValueError(f"push: expected a (B, {self.in_channels}, f) chunk of mel + f0 + uv, got {tuple(mel.shape)}")
+                f = self._win.push("mel", mel[:, :-2], 2, ("a {} mel", "frames", "the mel is"))
+                self._win.push("f0uv", mel[:, -2:], 2, ("a {} f0 / uv", "frames", "the f0 / uv is"))
+            else:
+                f = self._win.push("mel", mel, 2, ("a {} mel", "frames", "the mel is"))
             if f == self.max_frames:
                 self._graph.replay()
             else:
@@ -713,18 +853,33 @@ class GeneratorStreamer:
                 left -= f
             return torch.cat(outs, -1) if outs else torch.zeros(self.batch, 1, 0, device=self.device)
 
-    def reset(self, slots, lengths=None):
+    def reset(self, slots, lengths=None, seeds=None):
         """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A non-causal
-        generator needs the new utterances' ``lengths`` in frames, in the order of ``slots``."""
+        generator needs the new utterances' ``lengths`` in frames, an NSF one their excitation ``seeds``, both in the order
+        of ``slots``."""
         slots = [int(s) for s in slots]
         if self.plan.causal and lengths is not None:
             raise ValueError("reset: a causal generator streams without lengths")
         if not self.plan.causal and lengths is None:
             raise ValueError("reset: streaming a non-causal generator needs the new utterances' lengths")
+        if self.plan.nsf and seeds is None:
+            raise ValueError("reset: streaming an NSF generator needs the new utterances' seeds")
+        if not self.plan.nsf and seeds is not None:
+            raise ValueError("reset: seeds are for NSF generators")
         with torch.no_grad(), torch.cuda.device(self.device):
             self._win.reset(slots)
             if not self.plan.causal:
                 self._set_lengths(slots, lengths)
+            if self.plan.nsf:
+                self._set_seeds(slots, seeds)
+
+    def _set_seeds(self, slots, seeds):
+        """Slots ``slots`` start their excitation from ``seeds``: phases and sample counts return to zero."""
+        slots = list(slots)
+        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
+            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
+        idx = torch.tensor(slots, dtype=torch.long).to(self.device)
+        self._nsf.reset(idx, nsf_seed_tensor(seeds, len(slots), self.device))
 
     def _set_lengths(self, slots, lengths):
         """Slots ``slots`` hold utterances of ``lengths`` frames (host sequence or device tensor), none pushed yet."""

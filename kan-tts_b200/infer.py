@@ -7,47 +7,99 @@ forward because its decoder masks only support batch 1), kantts/bin/infer_hifiga
 in one call; every utterance is cut at its own predicted length (frames x product of the up-sampling scales).
 
 ``stream_synthesize`` gives the same waveforms chunk by chunk while the decoder runs: decoder steps -> streamed post-net
-(PostNet.streamer) -> streamed causal vocoder (Generator.streamer)."""
+(PostNet.streamer) -> streamed causal vocoder (Generator.streamer).
+
+An NSF acoustic model (``num_mels`` = mel + f0 + voiced flag) drives an NSF generator with ``nsf_f0`` and ``nsf_seeds``: the
+f0 channel is denormalised and the voiced flag binarised as the reference's hand-off does (kantts/bin/infer_sambert.py:26-56
+``denorm_f0``, infer_hifigan.py:57-63 ``binarize``), and the excitation is seeded per utterance (Generator.forward's
+``nsf_seeds``), so that the streamed and the whole-utterance waveforms agree."""
 import numpy as np
 import torch
 
 from .hifigan import StreamPlan
 
 
+F0_FLOOR, UV_THRESHOLD = 30.0, 0.6          # infer_sambert.py:26 denorm_f0's f0_threshold / uv_threshold
+
+
+def denorm_f0(rows, nsf_f0):
+    """rows (..., num_mels) of an NSF acoustic model -> the same rows with the f0 channel (second to last) denormalised and
+    clamped below at 30 Hz and the voiced flag (last) set to 1 where it is >= 0.6, else 0 (infer_sambert.py:26-56).
+    ``nsf_f0``: ("mean_std", mean, std) -> f0 * std + mean, or ("global", f0_min, f0_max) -> f0 * (f0_max - f0_min) + f0_min.
+    Elementwise torch ops on the rows' device."""
+    kind, a, b = nsf_f0
+    f0, uv = rows[..., -2:-1], rows[..., -1:]
+    if kind == "mean_std":
+        f0 = f0 * float(b) + float(a)
+    else:
+        f0 = f0 * (float(b) - float(a)) + float(a)
+    return torch.cat([rows[..., :-2], f0.clamp_min(F0_FLOOR), (uv >= UV_THRESHOLD).to(rows.dtype)], -1)
+
+
+def _check_nsf(sambert_num_mels, generator, nsf_f0, nsf_seeds, what):
+    """-> whether the NSF hand-off runs: both of nsf_f0 / nsf_seeds given (ValueError when only one is, when the generator
+    has no NSF, or when the acoustic model's channels are not the generator's mel + f0 + uv)."""
+    if nsf_f0 is None and nsf_seeds is None:
+        return False
+    if nsf_f0 is None or nsf_seeds is None:
+        raise ValueError(f"{what}: nsf_f0 and nsf_seeds go together")
+    if not generator.nsf_enable:
+        raise ValueError(f"{what}: nsf_f0 / nsf_seeds need an NSF generator")
+    if len(nsf_f0) != 3 or nsf_f0[0] not in ("mean_std", "global"):
+        raise ValueError(f"{what}: nsf_f0 must be ('mean_std', mean, std) or ('global', f0_min, f0_max), got {nsf_f0!r}")
+    c_in = generator.conv_pre.conv1d.spec.c_in + 2
+    if sambert_num_mels != c_in:
+        raise ValueError(f"{what}: the acoustic model makes {sambert_num_mels} mel channels, the NSF generator takes {c_in} "
+                         "(mel + f0 + uv)")
+    return True
+
+
 @torch.no_grad()
-def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths):
+def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None):
     """sambert: ``KanTtsSAMBERT`` in eval(); generator: ``Generator`` in eval() (``remove_weight_norm()`` optional --
     the prepared weights are cached either way).  Tensors as in ``KanTtsSAMBERT.forward`` (inference branch).
+    ``nsf_f0`` / ``nsf_seeds`` (both or neither): the NSF hand-off, see the module docstring and ``denorm_f0``.
     -> (list of 1-D waveform tensors, dict of the acoustic-model results)."""
     if sambert.training or generator.training:
         raise RuntimeError("synthesize() expects both models in eval() mode")
+    nsf = _check_nsf(sambert.mel_postnet.num_mels, generator, nsf_f0, nsf_seeds, "synthesize()")
     res = sambert(inputs_ling, inputs_emotion, inputs_speaker, input_lengths)
     mel = res["postnet_outputs"]                                   # (B, T, num_mels), zero beyond each length
     frames = res["LR_length_rounded"]
-    wav = generator(mel.transpose(1, 2).contiguous())              # (B, 1, T * hop)
+    if nsf:
+        wav = generator(denorm_f0(mel, nsf_f0).transpose(1, 2).contiguous(), nsf_seeds=nsf_seeds)
+    else:
+        wav = generator(mel.transpose(1, 2).contiguous())          # (B, 1, T * hop)
     hop = int(np.prod(generator.upsample_scales))
     wavs = [wav[b, 0, : int(frames[b]) * hop] for b in range(wav.shape[0])]
     return wavs, res
 
 
-def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps=4):
+def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps=4,
+                      nsf_f0=None, nsf_seeds=None):
     """Streaming ``synthesize``: the encoder, the variance adaptor and the decoder memory run now, then iterating the
     returned TtsStream decodes ``chunk_steps`` decoder steps at a time and yields their audio as soon as the post-net rows
-    are final.  The generator must be causal and without NSF.  For every slot b, the yielded chunks concatenated and cut
-    at ``lengths[b]`` are ``synthesize(...)[0][b]``."""
+    are final.  The generator must be causal; an NSF one needs ``nsf_f0`` and ``nsf_seeds`` (as ``synthesize``), applied to
+    each chunk of post-net rows.  For every slot b, the yielded chunks concatenated and cut at ``lengths[b]`` are
+    ``synthesize(..., nsf_f0, nsf_seeds)[0][b]``."""
     if sambert.training or generator.training:
         raise RuntimeError("stream_synthesize() expects both models in eval() mode")
-    StreamPlan(generator)                                          # rejects NSF generators
+    StreamPlan(generator)
+    if generator.nsf_enable and (nsf_f0 is None or nsf_seeds is None):
+        raise ValueError("stream_synthesize(): an NSF generator streams with nsf_f0 and nsf_seeds: its excitation must be "
+                         "seeded for the chunks to reproduce the whole utterance")
     if not generator.conv_pre.causal:                              # the vocoder streams here without a delay
         raise ValueError("streaming needs a causal generator: a non-causal one reads ahead of every output sample")
     num_mels = sambert.mel_postnet.num_mels
-    if generator.conv_pre.conv1d.spec.c_in != num_mels:
+    nsf = _check_nsf(num_mels, generator, nsf_f0, nsf_seeds, "stream_synthesize()")     # checks the NSF channels
+    if not nsf and generator.conv_pre.conv1d.spec.c_in != num_mels:
         raise ValueError(f"stream_synthesize(): the acoustic model makes {num_mels} mel channels, the generator takes "
                          f"{generator.conv_pre.conv1d.spec.c_in}")
     chunk_steps = int(chunk_steps)
     if chunk_steps < 1:
         raise ValueError(f"stream_synthesize(): chunk_steps must be >= 1, got {chunk_steps}")
-    return TtsStream(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps)
+    return TtsStream(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps, nsf_f0,
+                     nsf_seeds)
 
 
 class TtsStream:
@@ -58,8 +110,9 @@ class TtsStream:
     is padding after that.  From the first chunk to the last no device data is read on the host.  A stream is iterated
     once."""
 
-    def __init__(self, sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps):
-        self.sambert, self.chunk_steps = sambert, chunk_steps
+    def __init__(self, sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps,
+                 nsf_f0=None, nsf_seeds=None):
+        self.sambert, self.chunk_steps, self.nsf_f0 = sambert, chunk_steps, nsf_f0
         dec = sambert.mel_decoder
         self.r, self.d_mel = dec.r, dec.d_mel
         with torch.no_grad():
@@ -70,7 +123,7 @@ class TtsStream:
         self.lengths = [int(n) * self.hop for n in frames.cpu()]
         self.max_frames = F = self.r * chunk_steps
         self._post = sambert.mel_postnet.streamer(B, F, frames)
-        self._voc = generator.streamer(batch=B, max_frames=F)
+        self._voc = generator.streamer(batch=B, max_frames=F, seeds=nsf_seeds)
         self._used = False
 
     def _vocode(self, rows, start):
@@ -104,5 +157,7 @@ class TtsStream:
                 rows = self._post.push(dec)
                 if last:
                     rows = torch.cat([rows, self._post.finish()], 1)
+                if self.nsf_f0 is not None:
+                    rows = denorm_f0(rows, self.nsf_f0)
                 chunks, start = self._vocode(rows, start)
                 yield from chunks

@@ -10,7 +10,11 @@ the same frames.  Prints the card and its power limit, read in the same run.
 with per-slot lengths long enough that no utterance ends during the run; its rows also give the stream's look-ahead
 (delay_ms: the audio a sample waits for) on top of the chunk's own audio.
 
-    python scripts/stream_latency.py [--config causal|noncausal] [--chunks 200] [--out DIR]"""
+--config nsf / nsf_noncausal: the NSF generators hifigan_v1_nsf_24k.yaml (causal, hop 240 at 24 kHz) and
+hifigan_noncausal_nsf_v1_16k.yaml (hop 200 at 16 kHz), streamed with per-slot seeds; each chunk carries f0 and the voiced
+flag after the mel, and the whole-utterance forward takes the same seeds.
+
+    python scripts/stream_latency.py [--config causal|noncausal|nsf|nsf_noncausal] [--chunks 200] [--out DIR]"""
 import argparse
 import json
 import os
@@ -32,7 +36,25 @@ GENERATORS = {
         "noncausal_v1_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
                                   resblock_dilations=[[1, 3, 5, 7]] * 3, causal=False), 16000),
     },
+    "nsf": {
+        "v1_nsf_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4],
+                            nsf_params=dict(nb_harmonics=7, sampling_rate=24000)), 24000),
+    },
+    "nsf_noncausal": {
+        "noncausal_nsf_v1_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
+                                      resblock_dilations=[[1, 3, 5, 7]] * 3, causal=False,
+                                      nsf_params=dict(nb_harmonics=7, sampling_rate=16000)), 16000),
+    },
 }
+
+
+def frames_input(gen, B, F):
+    """(B, in_channels, F) on the device: a random mel, and for an NSF generator f0 in [80, 300) Hz and a voiced flag."""
+    mel = torch.randn(B, 80, F, device="cuda")
+    if not gen.nsf_enable:
+        return mel
+    f0 = 80 + 220 * torch.rand(B, 1, F, device="cuda")
+    return torch.cat([mel, f0, (torch.rand(B, 1, F, device="cuda") > 0.3).float()], 1)
 # the whole-utterance forward keeps every activation of the utterance: longer ones are timed at this many frames
 WHOLE_MAX_ROWS = 64 * 256
 
@@ -45,8 +67,9 @@ def card():
 
 def measure(gen, sr, B, F, chunks):
     lengths = None if gen.conv_pre.causal else [1 << 24] * B
-    st = gen.streamer(batch=B, max_frames=F, lengths=lengths)
-    mel = torch.randn(B, 80, F, device="cuda")
+    seeds = list(range(B)) if gen.nsf_enable else None
+    st = gen.streamer(batch=B, max_frames=F, lengths=lengths, seeds=seeds)
+    mel = frames_input(gen, B, F)
     for _ in range(10):                                  # the first push captures the graph
         st.push(mel)
     torch.cuda.synchronize()
@@ -62,14 +85,15 @@ def measure(gen, sr, B, F, chunks):
     chunk_ms = e0.elapsed_time(e1) / chunks
     # whole-utterance forward of the same frames (capped, see WHOLE_MAX_ROWS)
     frames = min(chunks * F, max(F, WHOLE_MAX_ROWS // B))
-    whole = torch.randn(B, 80, frames, device="cuda")
+    whole = frames_input(gen, B, frames)
+    kw = dict(nsf_seeds=seeds) if seeds else {}
     with torch.no_grad():
-        gen(whole)
+        gen(whole, **kw)
         torch.cuda.synchronize()
         w0, w1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         w0.record()
         for _ in range(3):
-            gen(whole)
+            gen(whole, **kw)
         w1.record()
         torch.cuda.synchronize()
     whole_ms = w0.elapsed_time(w1) / 3
