@@ -414,6 +414,30 @@ int kt_fsmn_fwd_stream(const KtStreamWin* w, const float* x, const float* weight
  * PyTorch gate order (i, f, g, o); exact fp32. */
 int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t batch, int32_t rows, int32_t hidden,
                    int32_t gx_pitch, int32_t h_pitch, void* stream);
+/* Per-slot forms (PostNet.streamer(per_slot=True)): chunk row t of item b is frame frame0[b] + offset + t (frame0: device
+ * int32 [batch]), so each slot can be anywhere in its own utterance.
+ * kt_fsmn_fwd_stream_slots: kt_fsmn_fwd_stream with row0 = frame0[b] + offset per item (same sum, same order).
+ * kt_lstm_stream_slots: kt_lstm_stream where a chunk whose first row is frame 0 or earlier starts from (h, c) = 0 and a later
+ * chunk from the carried state; a row before frame 0 leaves (h, c) as they are (zero) and outputs that zero h, so frame 0
+ * starts from (h, c) = 0. */
+int kt_fsmn_fwd_stream_slots(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths,
+                             const int32_t* frame0, int32_t offset, const float* resid, float* y, int32_t batch, int32_t rows,
+                             int32_t c, int32_t k, int32_t pad_left, void* stream);
+int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const int32_t* frame0, int32_t offset,
+                         int32_t batch, int32_t rows, int32_t hidden, int32_t gx_pitch, int32_t h_pitch, void* stream);
+/* kt_pnca_step_slots: one free-running decoder step of a PNCA layer's two attentions for `batch` slots, each at its own
+ * step s = step[b] (device int32 [batch], as mem_len, x_bw, h_bw; active: device uint8 [batch]).
+ *   q_row  [batch][3 * heads * d_head]: the step's fused Q | K | V projection
+ *   x_kv   [batch][max_steps][2 * heads * d_head]: the self K | V cache; the call writes row s from q_row's K | V (key s
+ *          of this call's attention is read from q_row, rows < s from the cache)
+ *   h_kv   [batch][max_steps][2 * heads * d_head]: the memory K | V rows
+ *   out_x  [batch][heads * d_head]: softmax(q k^T / sqrt(d_head)) v over self keys [max(0, s - x_bw[b]), s]
+ *   out_h  likewise over memory keys [s, min(s + h_bw[b], mem_len[b] - 1)]
+ * Only the band's keys are read; no mask tensor.  A slot with active[b] == 0 (or s outside [0, min(mem_len[b], max_steps)))
+ * gets zero outputs and its cache is not written.  d_head 8, 16 or 32; fp32 (exp from expf). */
+int kt_pnca_step_slots(const float* q_row, float* x_kv, const float* h_kv, const int32_t* step, const int32_t* mem_len,
+                       const int32_t* x_bw, const int32_t* h_bw, const uint8_t* active, float* out_x, float* out_h,
+                       int32_t batch, int32_t heads, int32_t d_head, int32_t max_steps, void* stream);
 
 /* ---- seeded NSF excitation (SourceModule, kantts/models/hifigan/layers.py:229-290) ---------------------------------------
  * kt_nsf_excitation: the sine-plus-noise excitation of `frames` frames of `batch` slots as a deterministic function of each

@@ -9,6 +9,7 @@ Public surface = the reference's own module API for this path:
   train.SambertStep (Sambert_Trainer.train_step)
   infer.synthesize (symbols -> SAM-BERT free-running decode -> HiFi-GAN -> waveforms, no .npy hand-off)
   infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs, causal generators)
+  infer.TtsServer (continuous batching: requests join and leave the slots of one running stream)
   install.install() patches these into an importable KAN-TTS checkout.
 All tensor math runs in libkantts_b200.so (C ABI: include/kantts_b200.h); there is no fallback.
 """
@@ -21,7 +22,7 @@ from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401
                    DiscriminatorAdversarialLoss, FeatureMatchLoss, criterion_builder)
 from .train import GanStep, SambertStep, hifigan_model_builder, sambert_model_builder  # noqa: F401
-from .infer import synthesize, stream_synthesize  # noqa: F401
+from .infer import synthesize, stream_synthesize, TtsServer, slot_schedule  # noqa: F401
 
 
 

@@ -127,6 +127,9 @@ PROTOTYPES = {
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P],
+    "kt_lstm_stream_slots": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],

@@ -1296,4 +1296,209 @@ extern "C" int kt_lstm_stream(const float* gx, const float* whh_t, float* state,
   return KT_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Per-slot post-net streaming: the frame of a slot's chunk row comes from the device (frame0[b] + offset), so every slot of
+// one launch can sit at a different place in its own utterance.
+//
+// fsmn_stream_slots_kernel: fsmn_stream_kernel with row0 = frame0[b] + offset per item; the same sum in the same order.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) fsmn_stream_slots_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                                                const int* __restrict__ lengths, const int* __restrict__ frame0,
+                                                                const float* __restrict__ resid, float* __restrict__ y,
+                                                                KtStreamWin win, int rows, int C, int K, int lp, int offset) {
+  const int b = blockIdx.y;
+  const int len = __ldg(lengths + b);
+  const int row0 = __ldg(frame0 + b) + offset;
+  const long long n = (long long)rows * C;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)(i / C), c = (int)(i - (long long)t * C);
+    const float* xc = x + ((long long)b * win.in_pitch + win.in_first + t - (K - 1)) * C + c;
+    const int a0 = row0 + t - lp;
+    const bool keep_t = row0 + t >= 0 && row0 + t < len;
+    float acc = keep_t ? __ldg(xc + (long long)lp * C) : 0.f;
+    for (int j = 0; j < K; ++j) {
+      const int a = a0 + j;
+      const float v = (a >= 0 && a < len) ? __ldg(xc + (long long)j * C) : 0.f;
+      acc = fmaf(__ldg(w + (long long)c * K + j), v, acc);
+    }
+    float out = keep_t ? acc : 0.f;
+    if (resid) out += __ldg(resid + ((long long)b * win.res_pitch + win.res_first + t) * C + c);
+    y[((long long)b * win.out_pitch + win.out_first + t) * C + c] = out;
+  }
+}
+
+extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const float* x, const float* w, const int32_t* lengths,
+                                        const int32_t* frame0, int32_t offset, const float* resid, float* y, int32_t B,
+                                        int32_t rows, int32_t C, int32_t K, int32_t lp, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(win && x && w && lengths && frame0 && y, "fsmn_fwd_stream_slots: null pointer");
+  KT_REQUIRE(B >= 1 && B <= 65535 && rows >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_fwd_stream_slots: bad sizes");
+  KT_REQUIRE(win->in_first >= K - 1 && win->in_first + rows <= win->in_pitch,
+             "fsmn_fwd_stream_slots: the input window needs K - 1 rows of history before the chunk");
+  KT_REQUIRE(win->out_first >= 0 && win->out_first + rows <= win->out_pitch,
+             "fsmn_fwd_stream_slots: the chunk does not fit its output window");
+  KT_REQUIRE(!resid || (win->res_first >= 0 && win->res_first + rows <= win->res_pitch),
+             "fsmn_fwd_stream_slots: the chunk does not fit its residual window");
+  const long long n = (long long)rows * C;
+  const int blocks = (int)std::min<long long>((n + 255) / 256, 1024);
+  fsmn_stream_slots_kernel<<<dim3(blocks, B), 256, 0, st>>>(x, w, lengths, frame0, resid, y, *win, rows, C, K, lp, offset);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+// lstm_stream_slots_kernel: lstm_stream_kernel where row t of item b is frame frame0[b] + offset + t.  A chunk whose first
+// row is frame 0 or earlier starts from (h, c) = 0, a later chunk from the carried state.  A row before frame 0 leaves
+// (h, c) as they are, i.e. zero, and its output row is that zero h; frame 0 therefore starts from zeros.  The gate sums are
+// lstm_stream_kernel's, in the same order.
+__global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
+                                         float* __restrict__ h_out, const int* __restrict__ frame0, int offset, int rows, int H,
+                                         int gx_pitch, int h_pitch) {
+  extern __shared__ float sm[];
+  const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x;
+  float* h = sm;             // [H]
+  float* c = h + H;          // [H]
+  float* gates = c + H;      // [4H]
+  float* s = state + (long long)b * 2 * H;
+  const int a0 = __ldg(frame0 + b) + offset;
+  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = a0 > 0 ? s[j] : 0.f;
+  __syncthreads();
+  for (int t = 0; t < rows; ++t) {
+    float* out = h_out + ((long long)b * h_pitch + t) * H;
+    if (a0 + t < 0) {
+      for (int j = tid; j < H; j += blockDim.x) out[j] = h[j];
+      continue;                                  // uniform over the CTA: no barrier is skipped by part of it
+    }
+    const float* g = gx + ((long long)b * gx_pitch + t) * G;
+    for (int j = tid; j < G; j += blockDim.x) {
+      float acc = __ldg(g + j);
+      for (int k = 0; k < H; ++k) acc = fmaf(__ldg(whh_t + (long long)k * G + j), h[k], acc);
+      gates[j] = acc;
+    }
+    __syncthreads();
+    for (int j = tid; j < H; j += blockDim.x) {
+      const float ig = sigmoid_f(gates[j]), fg = sigmoid_f(gates[H + j]), gg = tanhf(gates[2 * H + j]), og = sigmoid_f(gates[3 * H + j]);
+      const float cn = fg * c[j] + ig * gg;
+      const float hn = og * tanhf(cn);
+      c[j] = cn;
+      h[j] = hn;
+      out[j] = hn;
+    }
+    __syncthreads();
+  }
+  for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
+}
+
+extern "C" int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const int32_t* frame0,
+                                    int32_t offset, int32_t B, int32_t rows, int32_t H, int32_t gx_pitch, int32_t h_pitch,
+                                    void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(gx && whh_t && state && h && frame0, "lstm_stream_slots: null pointer");
+  KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream_slots: bad sizes");
+  const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
+  const size_t smem = (size_t)6 * H * sizeof(float);
+  lstm_stream_slots_kernel<<<B, threads, smem, st>>>(gx, whh_t, state, h, frame0, offset, rows, H, gx_pitch, h_pitch);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Per-slot free-running decoder step of MultiHeadPNCAAttention (sambert.SlotDecoder): every slot b at its own step
+// s = step[b], with its own bands and memory length, all read on the device.  One CTA of two warps per (head, slot):
+//   warp 0  writes the step's self K / V row into x_kv at s and attends self keys [max(0, s - x_bw[b]), s]; key s is read
+//           from q_row, never from the row this launch writes, and every key / value is loaded with ld.global.cg (L2,
+//           coherent), not through the read-only path, since the cache is written in this launch
+//   warp 1  attends memory keys [s, min(s + h_bw[b], mem_len[b] - 1)] of h_kv
+// Only the band's keys are read (the masked step path scans all Lmax keys).  Each lane takes keys j = lo + lane, lo + lane +
+// 32, ...: the scores' max, then p = exp(score - max) summed into the lane's D accumulators, then one butterfly per
+// accumulator.  An inactive slot (or one outside its memory) writes zero outputs and leaves its cache untouched.
+// ---------------------------------------------------------------------------------------------
+template <int D>
+__global__ void __launch_bounds__(64) pnca_step_slots_kernel(const float* __restrict__ q_row, float* x_kv,
+                                                             const float* __restrict__ h_kv, const int* __restrict__ step,
+                                                             const int* __restrict__ mem_len, const int* __restrict__ x_bw,
+                                                             const int* __restrict__ h_bw, const uint8_t* __restrict__ active,
+                                                             float* __restrict__ out_x, float* __restrict__ out_h, int H,
+                                                             int max_steps, float scale) {
+  const int head = blockIdx.x, b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int hd = H * D;
+  const int s = __ldg(step + b), ml = __ldg(mem_len + b);
+  float* out = (warp ? out_h : out_x) + (long long)b * hd + head * D;
+  const bool live = __ldg(active + b) && s >= 0 && s < max_steps && s < ml;
+  if (!live) {
+    if (lane < D) out[lane] = 0.f;
+    return;
+  }
+  const float* q = q_row + (long long)b * 3 * hd + head * D;
+  const float* kv;
+  int lo, hi;
+  if (warp == 0) {
+    float* row = x_kv + ((long long)b * max_steps + s) * 2 * hd + head * D;
+    if (lane < D) {
+      row[lane] = __ldg(q + hd + lane);
+      row[hd + lane] = __ldg(q + 2 * hd + lane);
+    }
+    kv = x_kv + (long long)b * max_steps * 2 * hd + head * D;
+    lo = max(0, s - __ldg(x_bw + b));
+    hi = s;
+  } else {
+    kv = h_kv + (long long)b * max_steps * 2 * hd + head * D;
+    lo = s;
+    hi = min(s + __ldg(h_bw + b), ml - 1);
+  }
+  float qr[D];
+#pragma unroll
+  for (int d = 0; d < D; ++d) qr[d] = __ldg(q + d) * scale;
+  // key j's K at k[0, D) and V at k[hd, hd + D): a cache row, or for the self key s the step's K | V in q_row
+  const int own = warp == 0 ? s : -1;
+  float m = -INFINITY;
+  for (int j = lo + lane; j <= hi; j += 32) {
+    const float* k = j == own ? q + hd : kv + (long long)j * 2 * hd;
+    float sc = 0.f;
+#pragma unroll
+    for (int d = 0; d < D; ++d) sc = fmaf(qr[d], __ldcg(k + d), sc);
+    m = fmaxf(m, sc);
+  }
+  m = warp_max(m);
+  float acc[D], l = 0.f;
+#pragma unroll
+  for (int d = 0; d < D; ++d) acc[d] = 0.f;
+  for (int j = lo + lane; j <= hi; j += 32) {
+    const float* k = j == own ? q + hd : kv + (long long)j * 2 * hd;
+    float sc = 0.f;
+#pragma unroll
+    for (int d = 0; d < D; ++d) sc = fmaf(qr[d], __ldcg(k + d), sc);
+    const float p = expf(sc - m);
+    l += p;
+#pragma unroll
+    for (int d = 0; d < D; ++d) acc[d] = fmaf(p, __ldcg(k + hd + d), acc[d]);
+  }
+  l = warp_sum(l);
+  float mine = 0.f;
+#pragma unroll
+  for (int d = 0; d < D; ++d) {
+    const float v = warp_sum(acc[d]);
+    if (lane == d) mine = v;
+  }
+  if (lane < D) out[lane] = hi >= lo ? mine / l : 0.f;
+}
+
+extern "C" int kt_pnca_step_slots(const float* q_row, float* x_kv, const float* h_kv, const int32_t* step, const int32_t* mem_len,
+                                  const int32_t* x_bw, const int32_t* h_bw, const uint8_t* active, float* out_x, float* out_h,
+                                  int32_t B, int32_t H, int32_t d_head, int32_t max_steps, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KT_REQUIRE(q_row && x_kv && h_kv && step && mem_len && x_bw && h_bw && active && out_x && out_h,
+             "pnca_step_slots: null pointer");
+  KT_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && H <= 65535 && max_steps >= 1, "pnca_step_slots: bad sizes");
+  const dim3 grid(H, B);
+  const float scale = 1.f / sqrtf((float)d_head);
+  switch (d_head) {
+    case 8: pnca_step_slots_kernel<8><<<grid, 64, 0, st>>>(q_row, x_kv, h_kv, step, mem_len, x_bw, h_bw, active, out_x, out_h, H, max_steps, scale); break;
+    case 16: pnca_step_slots_kernel<16><<<grid, 64, 0, st>>>(q_row, x_kv, h_kv, step, mem_len, x_bw, h_bw, active, out_x, out_h, H, max_steps, scale); break;
+    case 32: pnca_step_slots_kernel<32><<<grid, 64, 0, st>>>(q_row, x_kv, h_kv, step, mem_len, x_bw, h_bw, active, out_x, out_h, H, max_steps, scale); break;
+    default: KT_REQUIRE(false, "pnca_step_slots: d_head must be 8, 16 or 32 (got %d)", d_head);
+  }
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
 }  // namespace kt

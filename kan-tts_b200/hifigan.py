@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, KtStreamMask, ptr
-from .stream import Windows, WindowTable, own_weight
+from .stream import Windows, WindowTable, own_weight, to_device
 
 # --------------------------------------------------------------------------------------------
 # parameter holders (names / shapes == the reference's weight_norm / spectral_norm wrapped convs)
@@ -878,7 +878,7 @@ class GeneratorStreamer:
         slots = list(slots)
         if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
             raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
-        idx = torch.tensor(slots, dtype=torch.long).to(self.device)
+        idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
         self._nsf.reset(idx, nsf_seed_tensor(seeds, len(slots), self.device))
 
     def _set_lengths(self, slots, lengths):

@@ -161,3 +161,147 @@ class TtsStream:
                     rows = denorm_f0(rows, self.nsf_f0)
                 chunks, start = self._vocode(rows, start)
                 yield from chunks
+
+
+def slot_schedule(r, chunk_steps, delay, frames, steps, chunk, max_steps):
+    """Where an utterance of ``frames`` post-net frames and ``steps`` decoder steps, admitted to a TtsServer slot for chunk
+    ``chunk``, runs (decoder rows are counted from row 0 of chunk 0; a chunk holds f = r * chunk_steps rows):
+      start_step  the step of the admission chunk at which the slot decodes the utterance's step 0: ((-delay) mod f) / r,
+                  so that its frame 0, which the post-net returns ``delay`` rows later, is output row 0 of a chunk
+      voc_chunk   that chunk: the slot's vocoder is reset just before it, and its audio starts there
+      last_chunk  the chunk that returns the utterance's last frame (its last audio)
+      free_row    the first decoder row after the last frame became final and after the last decoder step
+      free_chunk  the first chunk that may admit the slot's next utterance: the chunk holding free_row, or the one after
+    ValueError when delay is not a multiple of r (frame 0 could not start a chunk) or steps > max_steps."""
+    if delay % r:
+        raise ValueError(f"serving needs a post-net delay that is a multiple of the decoder's r: delay {delay}, r {r}")
+    if steps > max_steps:
+        raise ValueError(f"an utterance of {steps} decoder steps does not fit max_steps = {max_steps}")
+    f = r * chunk_steps
+    p0 = (-delay) % f
+    first = chunk * f + p0                                       # decoder row of frame 0
+    last_row = first + frames - 1 + delay                        # its arrival makes the last frame final
+    free_row = max(last_row, first + steps * r - 1) + 1
+    return dict(start_step=p0 // r, voc_chunk=(first + delay) // f, last_chunk=last_row // f, free_row=free_row,
+                free_chunk=-(-free_row // f))
+
+
+class TtsServer:
+    """Continuous batching of text-to-speech: requests join and leave the ``slots`` slots of one running stream.
+
+    ``submit(ling, emotion, speaker, length[, nsf_seed])`` queues one utterance (tensors of ``KanTtsSAMBERT.forward``
+    without the batch dimension) and returns its request id.  ``step()`` runs one chunk of ``chunk_steps`` decoder steps
+    -> (audio, finished): ``audio`` lists ``(request id, start sample, wav)`` for every request with audio in this chunk
+    (wav 1-D on the device, cut at the request's end), ``finished`` the ids whose last audio this was.
+
+    Each slot decodes its own utterance (SlotDecoder: its own step, memory length and band), through a per-slot post-net
+    streamer into the causal vocoder streamer.  A request's audio equals ``synthesize`` of that request alone (with its
+    ``nsf_seed`` for an NSF generator), whatever the other slots hold.  Admission (at the start of a ``step``, for the queued
+    requests that fit free slots) runs ``front_half`` per request and reads their frame counts on the host; between
+    admissions no call reads device data.  The alignment of each slot is ``slot_schedule``.  The generator must be causal;
+    ``nsf_f0`` (see ``denorm_f0``) is required for an NSF one."""
+
+    def __init__(self, sambert, generator, slots, chunk_steps, max_steps, nsf_f0=None):
+        from .sambert import PostNetStreamPlan
+        if sambert.training or generator.training:
+            raise RuntimeError("TtsServer expects both models in eval() mode")
+        StreamPlan(generator)
+        if not generator.conv_pre.causal:
+            raise ValueError("serving needs a causal generator: a non-causal one reads ahead of every output sample")
+        num_mels = sambert.mel_postnet.num_mels
+        self.nsf = generator.nsf_enable
+        if self.nsf:
+            _check_nsf(num_mels, generator, nsf_f0, (), "TtsServer")
+        elif nsf_f0 is not None:
+            raise ValueError("TtsServer: nsf_f0 is for NSF generators")
+        elif generator.conv_pre.conv1d.spec.c_in != num_mels:
+            raise ValueError(f"TtsServer: the acoustic model makes {num_mels} mel channels, the generator takes "
+                             f"{generator.conv_pre.conv1d.spec.c_in}")
+        self.chunk_steps, self.max_steps, self.batch = int(chunk_steps), int(max_steps), int(slots)
+        if self.chunk_steps < 1 or self.max_steps < 1 or self.batch < 1:
+            raise ValueError(f"TtsServer: slots ({slots}), chunk_steps ({chunk_steps}) and max_steps ({max_steps}) must be >= 1")
+        dec = sambert.mel_decoder
+        self.r, self.d_mel = dec.r, dec.d_mel
+        self.delay = PostNetStreamPlan(sambert.mel_postnet).delay
+        if self.delay % self.r:
+            raise ValueError(f"TtsServer: the post-net delay ({self.delay}) must be a multiple of the decoder's r ({self.r}) "
+                             "for an utterance's frame 0 to start a chunk")
+        self.sambert, self.nsf_f0 = sambert, nsf_f0
+        self.frames_per_chunk = F = self.r * self.chunk_steps
+        self.hop = int(np.prod(generator.upsample_scales))
+        self.device = next(sambert.parameters()).device
+        self._dec = dec.slots(self.batch, self.max_steps)
+        with torch.no_grad():
+            self._post = sambert.mel_postnet.streamer(self.batch, F, torch.zeros(self.batch, dtype=torch.int32,
+                                                                                 device=self.device), per_slot=True)
+            self._voc = generator.streamer(batch=self.batch, max_frames=F,
+                                           seeds=[0] * self.batch if self.nsf else None)
+        self._queue, self._slots, self._chunk, self._next_id = [], [None] * self.batch, 0, 0
+
+    def submit(self, ling, emotion, speaker, length, nsf_seed=None):
+        """Queue one utterance: ling (L, 4), emotion (L,), speaker (L,) long tensors and its symbol count ``length``;
+        ``nsf_seed`` (an int) for an NSF generator.  -> the request id."""
+        if self.nsf != (nsf_seed is not None):
+            raise ValueError("submit: an NSF generator needs each request's nsf_seed, any other generator none")
+        rid, self._next_id = self._next_id, self._next_id + 1
+        self._queue.append(dict(id=rid, seed=nsf_seed, inputs=(ling.reshape(1, -1, ling.shape[-1]), emotion.reshape(1, -1),
+                                                                speaker.reshape(1, -1), torch.tensor([int(length)]))))
+        return rid
+
+    @property
+    def idle(self):
+        """No request queued or in a slot."""
+        return not self._queue and all(s is None or s["free_chunk"] <= self._chunk for s in self._slots)
+
+    def _admit(self, c):
+        free = [b for b, s in enumerate(self._slots) if s is None or s["free_chunk"] <= c]
+        take = self._queue[:len(free)]
+        if not take:
+            return
+        with torch.no_grad():
+            fronts = [self.sambert.front_half(*(t.to(self.device) for t in req["inputs"])) for req in take]
+        frames = torch.cat([fr["lr_len"].reshape(-1) for fr in fronts]).tolist()       # the one host read
+        sched = []
+        for req, fr, n in zip(take, fronts, frames):
+            try:
+                sched.append(slot_schedule(self.r, self.chunk_steps, self.delay, n, fr["memory"].shape[1], c,
+                                           self.max_steps))
+            except ValueError as e:
+                self._queue.remove(req)
+                raise ValueError(f"request {req['id']}: {e}") from None
+        del self._queue[:len(take)]
+        for b, req, fr, n, s in zip(free, take, fronts, frames, sched):
+            self._dec.admit(b, fr["memory"], fr["band_width_rows"])
+            self._post.reset([n], slots=[b], start_row=s["start_step"] * self.r)
+            seed = None if req["seed"] is None else torch.tensor([int(req["seed"])], dtype=torch.int64).to(self.device)
+            self._slots[b] = dict(s, chunk=c, id=req["id"], samples=n * self.hop, seed=seed)
+
+    def step(self):
+        """Run one chunk -> (audio, finished), see the class docstring."""
+        c, B, F = self._chunk, self.batch, self.frames_per_chunk
+        self._admit(c)
+        live = [(b, s) for b, s in enumerate(self._slots) if s is not None and s["free_chunk"] > c]
+        with torch.no_grad(), torch.cuda.device(self.device):
+            rows = []
+            for k in range(self.chunk_steps):
+                for b, s in live:
+                    if s["chunk"] == c and s["start_step"] == k:
+                        self._dec.start(b)
+                rows.append(self._dec.advance())
+            post = self._post.push(torch.cat(rows, 1).view(B, F, self.d_mel))
+            if self.nsf_f0 is not None:
+                post = denorm_f0(post, self.nsf_f0)
+            due = [(b, s) for b, s in live if s["voc_chunk"] == c]
+            if due:
+                seeds = torch.cat([s["seed"] for _, s in due]) if self.nsf else None
+                self._voc.reset([b for b, _ in due], seeds=seeds)
+            wav = self._voc.push(post.transpose(1, 2))
+        audio, finished = [], []
+        for b, s in live:
+            if s["voc_chunk"] <= c <= s["last_chunk"]:
+                start = (c - s["voc_chunk"]) * F * self.hop
+                audio.append((s["id"], start, wav[b, 0, :min(F * self.hop, s["samples"] - start)]))
+                if c == s["last_chunk"]:
+                    finished.append(s["id"])
+        self._chunk += 1
+        return audio, finished

@@ -740,6 +740,93 @@ class MelPNCADecoder(nn.Module):
         inp = torch.cat([go_frame, target[:, self.r - 1:: self.r, :]], dim=1)[:, :-1, :]
         return self.mel_dec(inp, memory, x_band_width, h_band_width, mask=mask, return_attns=return_attns)
 
+    def slots(self, batch, max_steps):
+        """-> a SlotDecoder: free-running decoding of ``batch`` independent utterances of up to ``max_steps`` steps each."""
+        return SlotDecoder(self, batch, max_steps)
+
+
+class SlotDecoder:
+    """Free-running decoding (MelPNCADecoder.infer_steps) of one utterance per slot, every slot at its own step
+    (MelPNCADecoder.slots).
+
+    Per slot on the device: the memory rows (batch, max_steps, d_mem), each PNCA layer's memory K / V projection and self
+    K / V cache, ``step``, ``mem_len`` (decoder steps), ``x_bw`` / ``h_bw`` (band widths) and ``active``.  ``admit`` places an
+    utterance in a slot (inactive until ``start``); ``advance()`` runs one decoder step of every active slot and returns the
+    (batch, 1, r * d_mel) outputs, zero for the inactive slots.  A slot reads its own memory row at its step and feeds back
+    its own previous output (zeros, the go frame, at its step 0); it goes inactive after its last step.  Each
+    slot's rows equal ``infer_steps`` of its utterance alone.  No call reads device data on the host."""
+
+    def __init__(self, decoder, batch, max_steps):
+        if decoder.training:
+            raise ValueError("slot decoding runs a decoder in eval() mode")
+        dec = decoder.mel_dec
+        self.decoder, self.batch, self.max_steps = decoder, int(batch), int(max_steps)
+        if self.batch < 1 or self.max_steps < 1:
+            raise ValueError(f"slots: batch ({batch}) and max_steps ({max_steps}) must be >= 1")
+        attn = dec.pnca[0].pnca_attn
+        self.n_head, hd = attn.n_head, attn.n_head * attn.d_head
+        self.device = dev = next(decoder.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("kantts_b200: the slot decoder runs on a CUDA device (no CPU fallback)")
+        B, L = self.batch, self.max_steps
+        self.memory = torch.zeros(B, L, attn.d_mem, device=dev)
+        self.h_kv = [torch.zeros(B, L, 2 * hd, device=dev) for _ in dec.pnca]
+        self.x_kv = [torch.zeros(B, L, 2 * hd, device=dev) for _ in dec.pnca]
+        self.step = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.mem_len = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.x_bw = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.h_bw = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.active = torch.zeros(B, dtype=torch.uint8, device=dev)
+        self._inp = torch.zeros(B, 1, decoder.d_mel, device=dev)
+
+    def admit(self, slot, memory, band_width):
+        """Place one utterance in slot ``slot`` (an int): ``memory`` (1, n, d_mem) its decoder memory (n <= max_steps),
+        ``band_width`` its band (an int or a device tensor of one element), for both attentions.  Its memory K / V rows are
+        projected here; the slot stays inactive until ``start``."""
+        b, n = int(slot), memory.shape[1]
+        if not 0 <= b < self.batch:
+            raise ValueError(f"admit: slot must lie in [0, {self.batch}), got {slot}")
+        if memory.dim() != 3 or memory.shape[0] != 1 or memory.shape[2] != self.memory.shape[2]:
+            raise ValueError(f"admit: expected a (1, n, {self.memory.shape[2]}) memory, got {tuple(memory.shape)}")
+        if not 1 <= n <= self.max_steps:
+            raise ValueError(f"admit: an utterance of {n} decoder steps does not fit max_steps = {self.max_steps}")
+        with torch.no_grad():
+            self.memory[b].zero_()
+            self.memory[b, :n].copy_(memory[0])
+            for layer, h_kv in zip(self.decoder.mel_dec.pnca, self.h_kv):
+                h_kv[b, :n].copy_(layer.pnca_attn.w_h_kv(memory)[0])
+            # the go frame: the slot's fed-back input is zero at its step 0 even when its previous utterance ended on the
+            # step before (a copy, since the fed-back rows are a view of the last step's returned output)
+            self._inp = self._inp.clone()
+            self._inp[b].zero_()
+            for t, v in ((self.step, 0), (self.mem_len, n), (self.active, 0)):
+                t[b] = v
+            for t in (self.x_bw, self.h_bw):
+                t[b].copy_(band_width.reshape(())) if torch.is_tensor(band_width) else t[b].fill_(int(band_width))
+
+    def start(self, slot):
+        """Slot ``slot`` decodes its step 0 in the next ``advance()``."""
+        self.active[int(slot)] = 1
+
+    def advance(self):
+        """One decoder step of every active slot -> (batch, 1, r * d_mel), zero rows for the inactive slots."""
+        dec, B = self.decoder.mel_dec, self.batch
+        with torch.no_grad():
+            idx = self.step.long().clamp_(max=self.max_steps - 1).view(B, 1, 1).expand(B, 1, self.memory.shape[2])
+            x = dec.dec_in_proj(torch.cat([torch.gather(self.memory, 1, idx), dec.prenet(self._inp)], dim=-1))
+            x = x * dec.d_model ** 0.5
+            for layer, h_kv, x_kv in zip(dec.pnca, self.h_kv, self.x_kv):
+                attn = layer.pnca_attn
+                q_row = attn.w_x_qkv(attn.layer_norm(x)).contiguous()
+                ox, oh = sops.pnca_step_slots(q_row, x_kv, h_kv, self, attn.n_head)
+                x = layer.pos_ffn(attn.fc_h(oh, resid=attn.fc_x(ox, resid=x)))
+            live = self.active.bool().view(B, 1, 1)
+            out = dec.dec_out_proj(dec.ln(x)).masked_fill(~live, 0)
+            self._inp = out[:, :, -self.decoder.d_mel:]
+            self.step += self.active
+            self.active &= (self.step < self.mem_len).to(torch.uint8)
+        return out
+
 
 class PostNet(nn.Module):
     """kantts_sambert.py:615-649."""
@@ -758,10 +845,11 @@ class PostNet(nn.Module):
         h, _ = self.lstm(self.fsmn(x, mask))
         return self.fc(h, resid=resid)
 
-    def streamer(self, batch, max_frames, lengths):
+    def streamer(self, batch, max_frames, lengths, per_slot=False):
         """-> a PostNetStreamer that runs this (eval-mode) post-net chunk by chunk over ``batch`` utterances of ``lengths``
-        (device tensor (batch,)) frames, at most ``max_frames`` decoder rows per chunk."""
-        return PostNetStreamer(self, batch, max_frames, lengths)
+        (device tensor (batch,)) frames, at most ``max_frames`` decoder rows per chunk.  ``per_slot``: every slot keeps its
+        own frame count on the device and ``reset(slots=...)`` starts an utterance in some slots (see PostNetStreamer)."""
+        return PostNetStreamer(self, batch, max_frames, lengths, per_slot)
 
 
 # One launch of a post-net chunk over named windows.  kind "conv": a k = 1 conv of ``module`` (a Linear, or the nn.LSTM's
@@ -830,16 +918,26 @@ class PostNetStreamer:
 
     A tensor a layer reads before the chunk lives in a window (stream.py); kt_fsmn_fwd_stream masks by each row's frame
     index against the slot lengths kept on the device, and kt_lstm_stream carries the LSTM state.  The weights are
-    prepared once, when the streamer is created."""
+    prepared once, when the streamer is created.
 
-    def __init__(self, postnet, batch, max_frames, lengths):
+    Per-slot mode (``per_slot=True``): each slot's frame count lives on the device, and the chunk's first decoder row is
+    frame ``rows[b]`` of slot b's utterance.  ``push`` then returns all f rows of every slot, output row t being frame
+    rows[b] - delay + t (zero outside [0, lengths[b])).  ``reset(lengths, slots=..., start_row=...)`` starts new
+    utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  The memory
+    blocks (kt_fsmn_fwd_stream_slots) read frames outside [0, lengths[b]) as zeros, the whole-sequence padding, so a slot's
+    window history needs no clearing; the LSTM (kt_lstm_stream_slots) starts from zeros at frame 0.  A slot's new utterance
+    must start after the previous one's last row was returned."""
+
+    def __init__(self, postnet, batch, max_frames, lengths, per_slot=False):
         self.plan = plan = PostNetStreamPlan(postnet)
         self._win = win = Windows(plan.windows, batch, max_frames, next(postnet.parameters()).device, "post-net streamer")
         self.batch, self.max_frames, self.delay, self.device = win.batch, win.max_frames, plan.delay, win.device
         self.num_mels, self.hidden = postnet.num_mels, postnet.lstm.hidden_size
+        self.per_slot = bool(per_slot)
         self._state = torch.zeros(self.batch, 2, self.hidden, device=self.device)
         self._zeros = torch.zeros(self.batch, self.max_frames, self.num_mels, device=self.device)
         self._len = torch.empty(self.batch, dtype=torch.int32, device=self.device)
+        self._row = torch.zeros(self.batch, dtype=torch.int32, device=self.device)     # per-slot mode: rows[b]
         self._steady = [self._place(st, 0) for st in plan.steps]
         with torch.no_grad(), torch.cuda.device(self.device):
             self._weights = [self._own_weight(st) for st in plan.steps]
@@ -865,8 +963,33 @@ class PostNetStreamer:
         o = skip if st.frame0 else 0                    # the chunk row of the step's first output row
         return self._win.place(st.src, st.dst, st.resid, in_offset=o if st.in_skip else 0, res_lag=st.res_lag - o)
 
+    def _chunk_slots(self, f):
+        """Per-slot mode: every launch of one chunk of f decoder rows over all rows of every slot -> the (B, f, num_mels)
+        output rows, zero where a row's frame lies outside its slot's utterance."""
+        b, B = self._win.buf, self.batch
+        for st, w, place in zip(self.plan.steps, self._weights, self._steady):
+            src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
+            if st.kind == "conv":
+                spec, pw, bias = w
+                ops.stream_conv(spec, pw, bias, src, dst, f, place, resid)
+            elif st.kind == "fsmn":
+                layer = self.plan.layers[st.layer]
+                ops.call("kt_fsmn_fwd_stream_slots", ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True),
+                         ptr(self._row, True), -layer["lag"] - layer["rp"], ptr(resid), ptr(dst), B, f, src.shape[2],
+                         layer["kernel"], layer["lp"])
+            else:
+                ops.call("kt_lstm_stream_slots", ptr(src), ptr(w), ptr(self._state), ptr(dst), ptr(self._row, True),
+                         -self.delay, B, f, self.hidden, src.shape[1], dst.shape[1])
+        self._win.advance(f)
+        frames = self._row[:, None] - self.delay + torch.arange(f, device=self.device, dtype=torch.int32)[None, :]
+        pad = (frames < 0) | (frames >= self._len[:, None])
+        self._row += f
+        return b["out"][:, :f].masked_fill(pad.unsqueeze(-1), 0)
+
     def _chunk(self, f):
         """Every launch of one chunk of f decoder rows (already in the "dec" window) -> the final output rows."""
+        if self.per_slot:
+            return self._chunk_slots(f)
         b, B, a = self._win.buf, self.batch, self._rows
         first = a - self.delay                      # frame of the chunk's first output row
         skip = max(0, -first)                       # output rows before frame 0 are not rows of the utterance
@@ -909,9 +1032,16 @@ class PostNetStreamer:
             left -= f
         return torch.cat(outs, 1) if outs else self._zeros[:, :0].clone()
 
-    def reset(self, lengths=None):
+    def reset(self, lengths=None, slots=None, start_row=0):
         """Start a new batch: the carried windows and LSTM state return to zeros; ``lengths`` (device tensor (batch,)),
-        when given, replaces the slots' frame counts."""
+        when given, replaces the slots' frame counts.
+
+        Per-slot mode with ``slots`` (host ints): only those slots start new utterances, of ``lengths`` frames (host ints,
+        in the order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames).
+        Nothing is cleared and no device data is read: every slot's frames restart on the device."""
+        if slots is not None:
+            self._reset_slots(slots, lengths, start_row)
+            return
         with torch.no_grad(), torch.cuda.device(self.device):
             if lengths is not None:
                 if lengths.shape != (self.batch,):
@@ -919,7 +1049,24 @@ class PostNetStreamer:
                 self._len.copy_(lengths)
             self._win.reset()
             self._state.zero_()
+            self._row.zero_()
         self._rows = 0
+
+    def _reset_slots(self, slots, lengths, start_row):
+        slots, start_row = [int(s) for s in slots], int(start_row)
+        if not self.per_slot:
+            raise ValueError("reset: slots are for a per-slot streamer (PostNet.streamer(..., per_slot=True))")
+        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
+            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
+        lengths = [int(n) for n in lengths]
+        if len(lengths) != len(slots) or any(n < 1 for n in lengths):
+            raise ValueError(f"reset: expected {len(slots)} lengths >= 1, got {lengths}")
+        if not 0 <= start_row < self.max_frames:
+            raise ValueError(f"reset: start_row must lie in [0, {self.max_frames}), got {start_row}")
+        with torch.no_grad():
+            for s, n in zip(slots, lengths):
+                self._len[s] = n
+                self._row[s] = -start_row
 
 
 class FP_Predictor(nn.Module):
@@ -1021,12 +1168,17 @@ class KanTtsSAMBERT(nn.Module):
         lfr_spk = lr_spk.contiguous().view(batch_size, -1, r * spk_hid.shape[-1])[:, :, : spk_hid.shape[-1]]
         memory = torch.cat([lfr_text, lfr_spk, lfr_emo], dim=-1)
         if duration_targets is not None:
-            x_band_width = int(duration_targets.float().masked_fill(inter_masks, 0).max() / r + 0.5)
+            dur = duration_targets.float().masked_fill(inter_masks, 0)
+            x_band_width = int(dur.max() / r + 0.5)
         else:
-            x_band_width = int((torch.exp(log_dur_p) - 1).max() / r + 0.5)
+            dur = torch.exp(log_dur_p) - 1
+            x_band_width = int(dur.max() / r + 0.5)
+        # each utterance's own band (the batch-1 rule), on the device: the max over its symbols only
+        band_width_rows = torch.trunc(dur.masked_fill(inter_masks, float("-inf")).amax(1) / r + 0.5).to(torch.int32)
         return dict(enc_attns=enc_attns, fp_p=fp_p, inter_lengths=inter_lengths, output_masks=output_masks,
                     lfr_masks=lfr_masks, lr_text=lr_text, lr_emo=lr_emo, lr_spk=lr_spk, lr_len=lr_len, log_dur_p=log_dur_p,
-                    pitch_p=pitch_p, energy_p=energy_p, memory=memory, x_band_width=x_band_width)
+                    pitch_p=pitch_p, energy_p=energy_p, memory=memory, x_band_width=x_band_width,
+                    band_width_rows=band_width_rows)
 
     def forward(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
                 mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, attn_priors=None,

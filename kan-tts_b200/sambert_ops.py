@@ -164,6 +164,20 @@ class PncaAttnFn(torch.autograd.Function):
         return dqkv, dhkv, None, None, None, None, None, None
 
 
+def pnca_step_slots(q_row, x_kv, h_kv, st, n_head):
+    """One decoder step of MultiHeadPNCAAttention for every slot of a SlotDecoder at its own step (kt_pnca_step_slots):
+    q_row (B, 1, 3HD); x_kv / h_kv (B, max_steps, 2HD), x_kv's row at each active slot's step written here; ``st`` holds
+    the device arrays step, mem_len, x_bw, h_bw (int32) and active (uint8).  -> out_x, out_h (B, 1, HD), zero for an
+    inactive slot."""
+    B, _, w = q_row.shape
+    hd = w // 3
+    out_x = torch.empty(B, 1, hd, device=q_row.device, dtype=torch.float32)
+    out_h = torch.empty_like(out_x)
+    call("kt_pnca_step_slots", ptr(q_row), ptr(x_kv), ptr(h_kv), ptr(st.step, True), ptr(st.mem_len, True), ptr(st.x_bw, True),
+         ptr(st.h_bw, True), ptr(st.active, True), ptr(out_x), ptr(out_h), B, n_head, hd // n_head, x_kv.shape[1])
+    return out_x, out_h
+
+
 def pnca_attn_step(q_row, x_cache, h_kv, mask_x, mask_h, n_head):
     """One free-running decoder step of MultiHeadPNCAAttention (sambert/__init__.py:212-300), inference only.
     q_row (B, 1, 3HD): this step's fused QKV projection (only its q block is read here; the caller has already written

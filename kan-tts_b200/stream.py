@@ -92,9 +92,16 @@ class Windows:
                 raise ValueError(f"reset: slots must lie in [0, {self.batch}), got {slots}")
             mask = torch.zeros(self.batch, dtype=torch.uint8)
             mask[slots] = 1
-            sel = mask.to(self.device)
+            sel = to_device(mask, self.device)
         if self._ntable:
             ops.call("kt_stream_reset", ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c)
+
+
+def to_device(t, device):
+    """A small host tensor on ``device`` without waiting for the device: staged in pinned memory and copied asynchronously
+    (the pinned block is not reused before the copy has run), so that resetting a slot of a running stream does not
+    synchronise the host."""
+    return t.pin_memory().to(device, non_blocking=True)
 
 
 def own_weight(spec, v, g, bias):
