@@ -294,6 +294,45 @@ int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* row
                      float* partials, int64_t partial_floats, int32_t batch, int32_t length, int32_t t_cap, int32_t t_ins,
                      int32_t c, void* stream);
 
+/* Alignment learning (MAS: True, sambert_16k_MAS*.yaml).  Every reduction runs in a fixed order; no float atomics.
+ * kt_align_attn_fwd: the distance attention of ConvAttention (kantts/models/sambert/attention.py:85-125) on the (B, L, C)
+ * rows the convs produce: q [batch][t_q][c], k [batch][t_k][c], c <= 128,
+ *   z[b][i][j] = -0.0005 sum_c (q[b][i][c] - k[b][j][c])^2            (the squares summed directly, exact fp32)
+ *   logprob = prior ? z - logsumexp_j(z) + log(prior + 1e-8) : z      (the log_softmax over ALL t_k keys; prior
+ *                                                                      [batch][t_q][t_k] or NULL)
+ *   soft = softmax over the keys j < key_lengths[b] of logprob, 0 on the other keys.
+ * row_lse [batch][t_q] receives logsumexp_j(z) when a prior is given (kept for the backward).
+ * kt_align_attn_bwd: dq [batch][t_q][c] and dk [batch][t_k][c] from d_soft and / or d_logprob (either may be NULL), with
+ * the softmax backward through soft and, with a prior, the log_softmax backward over all keys; dz [batch][t_q][t_k] is
+ * scratch (the gradient of z).  Two launches: per query row, then per key.
+ *
+ * kt_mas: mas_width1 (kantts/models/sambert/alignment.py:32-71) of every soft[b, :out_lengths[b], :in_lengths[b]], one CTA
+ * per utterance: log_p over the rows with log(soft), row 0 restricted to key 0, the step from key j - 1 taken when its log_p
+ * is >= (ties and -inf included); the backtrack from (T - 1, N - 1) and the reference's final write hard[b][0][0] = 1.
+ * Writes all of hard [batch][t_q][t_k] (0 / 1) and durations [batch][t_k] = sum over the rows of hard.  One decision bit per
+ * cell: in shared memory when they fit, else in `workspace` (kt_mas_workspace_bytes, 0 when they fit).
+ *
+ * kt_attn_ctc_fwd / _bwd: AttentionCTCLoss (kantts/train/loss.py:481-508), one CTA per utterance.  Frame t < T of
+ * utterance b is log_softmax([blank_logprob, logprob[b][t][:N]]), N = in_lengths[b], T = out_lengths[b]; the CTC loss of
+ * the targets 1..N over those frames, divided by N, 0 when infinite (zero_infinity); loss [1] = their mean over the batch.
+ * The backward writes all of d_logprob [batch][t_q][t_k] = d_loss[0] * the gradient of loss.  `workspace` holds the alpha
+ * recursion and the per-frame normalisers between the two calls: kt_attn_ctc_workspace_bytes. */
+int kt_align_attn_fwd(const float* q, const float* k, const float* prior, const int32_t* key_lengths, float* logprob,
+                      float* soft, float* row_lse, int32_t batch, int32_t t_q, int32_t t_k, int32_t c, void* stream);
+int kt_align_attn_bwd(const float* q, const float* k, const float* prior, const float* soft, const float* row_lse,
+                      const float* d_soft, const float* d_logprob, float* dz, float* dq, float* dk, int32_t batch,
+                      int32_t t_q, int32_t t_k, int32_t c, void* stream);
+int64_t kt_mas_workspace_bytes(int32_t batch, int32_t t_q, int32_t t_k);
+int kt_mas(const float* soft, const int32_t* in_lengths, const int32_t* out_lengths, float* hard, float* durations,
+           uint32_t* workspace, int64_t workspace_bytes, int32_t batch, int32_t t_q, int32_t t_k, void* stream);
+int64_t kt_attn_ctc_workspace_bytes(int32_t batch, int32_t t_q, int32_t t_k);
+int kt_attn_ctc_fwd(const float* logprob, const int32_t* in_lengths, const int32_t* out_lengths, float* loss,
+                    void* workspace, int64_t workspace_bytes, int32_t batch, int32_t t_q, int32_t t_k, float blank_logprob,
+                    void* stream);
+int kt_attn_ctc_bwd(const float* logprob, const int32_t* in_lengths, const int32_t* out_lengths, const float* d_loss,
+                    const void* workspace, int64_t workspace_bytes, float* d_logprob, int32_t batch, int32_t t_q,
+                    int32_t t_k, float blank_logprob, void* stream);
+
 /* Autoregressive duration predictor, free-running inference (VarRnnARPredictor.infer, kantts/models/sambert/adaptors.py:67-83):
  * the whole per-symbol recurrence  x -> Prenet(1 -> p1 -> p2, ReLU) -> cat(cond) -> 2-layer LSTM(hidden) -> Linear(hidden, 1) ->
  * ReLU -> next x  in ONE launch (one CTA per batch item) instead of ~10 library launches per symbol from Python.

@@ -16,7 +16,8 @@ All tensor math runs in libkantts_b200.so (C ABI: include/kantts_b200.h); there 
 from . import _lib  # noqa: F401
 from ._lib import build_library  # noqa: F401
 from . import ops, hifigan, audio, loss, sambert_ops, sambert, train, infer, install as _install  # noqa: F401
-from .sambert import KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss  # noqa: F401
+from .sambert import (KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss, AttentionCTCLoss,  # noqa: F401
+                      AttentionBinarizationLoss, ConvAttention)
 from .hifigan import Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator  # noqa: F401
 from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401
@@ -47,6 +48,20 @@ def sambert_fp_8k_config():
     """``Model.KanTtsSAMBERT.params`` of kantts/configs/sambert_fp_8k.yaml: the sambert_24k.yaml network with the
     filled-pause predictor (``FP: True``) and the yaml's six speakers."""
     return dict(sambert_24k_config(), FP=True, speaker=6)
+
+
+def sambert_16k_mas_config():
+    """``Model.KanTtsSAMBERT.params`` of kantts/configs/sambert_16k_MAS.yaml: the sambert_24k.yaml network that learns its
+    phone durations by monotonic alignment search (``MAS: True``), with the same linguistic units."""
+    return dict(sambert_24k_config(), MAS=True)
+
+
+def sambert_16k_mas_byte_config():
+    """``Model.KanTtsSAMBERT.params`` of kantts/configs/sambert_16k_MAS_byte.yaml: the MAS network on byte inputs
+    (``using_byte: True``, lfeat_type_list byte_index,emo_category,speaker_category): ``byte_index`` = 259 embeddings, the
+    256 byte values plus padding, end-of-sentence and mask, in place of the PinYin tables."""
+    cfg = {k: v for k, v in sambert_16k_mas_config().items() if k not in ("sy", "tone", "syllable_flag", "word_segment")}
+    return dict(cfg, using_byte=True, byte_index=259)
 
 
 install = _install.install

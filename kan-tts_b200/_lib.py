@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libkantts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu"]
+SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
@@ -114,6 +114,13 @@ PROTOTYPES = {
     "kt_fp_insert_plan": [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P],
     "kt_fp_insert_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_fp_insert_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _P],
+    "kt_align_attn_fwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "kt_align_attn_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "kt_mas_workspace_bytes": [_I, _I, _I],
+    "kt_mas": [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _P],
+    "kt_attn_ctc_workspace_bytes": [_I, _I, _I],
+    "kt_attn_ctc_fwd": [_P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P],
+    "kt_attn_ctc_bwd": [_P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _F, _P],
     "kt_conv1d_fwd_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
     "kt_conv1d_fwd_tc_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
     "kt_sinadd_fwd_win": [_P, _P, _I, _I, _I, _I, _I, _I, _P],

@@ -11,7 +11,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .audio import MelSpectrogram, stft
-from .sambert import FpCELoss
+from .sambert import AttentionBinarizationLoss, AttentionCTCLoss, FpCELoss
 
 
 def _as_list(outputs):
@@ -232,6 +232,8 @@ loss_dict = {
     "subband_stft_loss": MultiResolutionSTFTLoss,
     "feat_match_loss": FeatureMatchLoss,
     "FpCELoss": FpCELoss,
+    "AttentionCTCLoss": AttentionCTCLoss,
+    "AttentionBinarizationLoss": AttentionBinarizationLoss,
 }
 
 

@@ -18,8 +18,11 @@ Where the arithmetic runs:
     dropout) is torch elementwise / indexing code, as in the reference.
 The filled-pause variant (``FP: True``, sambert_fp_8k.yaml) is built: FP_Predictor on the same conv / LayerNorm
 kernels, and the splice of the predicted or labelled pauses into the text encoding as an index plan plus one
-gather each way (kt_fp_insert_*).  Not built: MAS alignment (``MAS: True``) and the speaker-encoder (``SE``)
-variant -- the shipped sambert_24k.yaml and sambert_fp_8k.yaml disable both.
+gather each way (kt_fp_insert_*).  The alignment-learning variant (``MAS: True``, sambert_16k_MAS*.yaml) is built:
+ConvAttention's projections on the conv kernels, its distance attention fused in kt_align_attn_* (no (B, C, T_mel,
+T_text) difference tensor), monotonic alignment search on the GPU (kt_mas, no host copy) and the forward-sum loss in
+kt_attn_ctc_*.  Not built: the speaker-encoder (``SE``) variant, and MAS together with FP (the reference's two branches
+do not compose: its MAS durations have one entry per symbol before the pause splice).
 """
 import ctypes
 from collections import namedtuple
@@ -1090,6 +1093,64 @@ class FP_Predictor(nn.Module):
         return F.softmax(self.fc(x), dim=2)
 
 
+class ConvNorm(nn.Module):
+    """attention.py:6-39: a "same"-padded Conv1d re-initialised with xavier_uniform_ at the gain of ``w_init_gain``,
+    applied to (B, L, C) rows; ``relu`` fuses the ReLU that follows it in its Sequential."""
+
+    def __init__(self, in_channels, out_channels, kernel_size=1, bias=True, w_init_gain="linear", relu=False):
+        super().__init__()
+        assert kernel_size % 2 == 1
+        self.conv = RowConv1d(in_channels, out_channels, kernel_size, padding=(kernel_size - 1) // 2, bias=bias, relu=relu)
+        nn.init.xavier_uniform_(self.conv.weight, gain=nn.init.calculate_gain(w_init_gain))
+
+    def forward(self, x):
+        return self.conv(x)
+
+
+class ConvAttention(nn.Module):
+    """attention.py:42-125: the alignment attention of the MAS variant.  Same constructor, sub-modules, ``state_dict`` and
+    seeded init as the reference (``attn_proj`` is kept although the forward never uses it).  Unlike the reference's
+    (B, C, T) inputs, ``forward`` takes the model's (B, T, C) rows: queries (B, T_mel, n_mel_channels), keys
+    (B, T_text, n_text_channels), ``mask`` the (B, T_text) key-padding mask of a length vector (True = padding), the
+    optional ``attn_prior`` (B, T_mel, T_text).  -> attn_soft, attn_logprob (B, 1, T_mel, T_text).  The projections run on
+    the conv kernels (ReLUs fused), the distance attention in kt_align_attn_fwd / _bwd."""
+
+    def __init__(self, n_mel_channels=80, n_text_channels=512, n_att_channels=80, temperature=1.0, use_query_proj=True):
+        super().__init__()
+        self.temperature = temperature
+        self.att_scaling_factor = np.sqrt(n_att_channels)
+        self.softmax = nn.Softmax(dim=3)
+        self.log_softmax = nn.LogSoftmax(dim=3)
+        self.attn_proj = nn.Conv2d(n_att_channels, 1, kernel_size=1)
+        self.use_query_proj = bool(use_query_proj)
+        self.key_proj = nn.Sequential(
+            ConvNorm(n_text_channels, n_text_channels * 2, kernel_size=3, bias=True, w_init_gain="relu", relu=True),
+            nn.ReLU(),
+            ConvNorm(n_text_channels * 2, n_att_channels, kernel_size=1, bias=True))
+        self.query_proj = nn.Sequential(
+            ConvNorm(n_mel_channels, n_mel_channels * 2, kernel_size=3, bias=True, w_init_gain="relu", relu=True),
+            nn.ReLU(),
+            ConvNorm(n_mel_channels * 2, n_mel_channels, kernel_size=1, bias=True, relu=True),
+            nn.ReLU(),
+            ConvNorm(n_mel_channels, n_att_channels, kernel_size=1, bias=True))
+
+    @staticmethod
+    def _project(seq, x):
+        for layer in seq:
+            if not isinstance(layer, nn.ReLU):          # the ReLUs are fused into the preceding convs
+                x = layer(x)
+        return x
+
+    def forward(self, queries, keys, mask=None, attn_prior=None):
+        keys_enc = self._project(self.key_proj, keys)
+        queries_enc = self._project(self.query_proj, queries) if self.use_query_proj else queries
+        if mask is None:
+            key_lengths = torch.full((keys.size(0),), keys.size(1), device=keys.device, dtype=torch.int32)
+        else:
+            key_lengths = (~mask).sum(1, dtype=torch.int32)
+        return sops.AlignAttnFn.apply(queries_enc, keys_enc, attn_prior, key_lengths)
+
+
 class KanTtsSAMBERT(nn.Module):
     """kantts_sambert.py:652-1044.  With ``FP: True`` the model builder must set ``fp_dict`` ({1: en, 2: a, 3: e},
     each a (1, 3, 4) long tensor of linguistic ids) before the first forward, as kantts/models/__init__.py:99-105
@@ -1097,9 +1158,10 @@ class KanTtsSAMBERT(nn.Module):
 
     def __init__(self, config):
         super().__init__()
-        for flag in ("SE", "MAS"):
-            if config.get(flag, False):
-                raise NotImplementedError(f"KanTtsSAMBERT variant {flag}=True is not built (see module docstring)")
+        if config.get("SE", False):
+            raise NotImplementedError("KanTtsSAMBERT variant SE=True is not built (see module docstring)")
+        if config.get("MAS", False) and config.get("FP", False):
+            raise NotImplementedError("KanTtsSAMBERT with both MAS=True and FP=True is not built (see module docstring)")
         self.text_encoder = TextFftEncoder(config)
         self.se_enable = False
         self.spk_tokenizer = nn.Embedding(config["speaker"], config["speaker_units"])
@@ -1107,7 +1169,10 @@ class KanTtsSAMBERT(nn.Module):
         self.variance_adaptor = VarianceAdaptor(config)
         self.mel_decoder = MelPNCADecoder(config)
         self.mel_postnet = PostNet(config)
-        self.MAS = False
+        self.MAS = bool(config.get("MAS", False))
+        if self.MAS:
+            self.align_attention = ConvAttention(n_mel_channels=config["num_mels"], n_text_channels=config["embedding_dim"],
+                                                 n_att_channels=config["num_mels"])
         self.fp_enable = bool(config.get("FP", False))
         if self.fp_enable:
             self.FP_predictor = FP_Predictor(config)
@@ -1133,16 +1198,46 @@ class KanTtsSAMBERT(nn.Module):
         r = self.mel_decoder.r
         return get_mask_from_lengths((lengths + r - 1) // r, max_len=max_len // r)
 
+    def align(self, ling_embedding, mel_targets, input_lengths, output_lengths, input_masks, attn_priors, pitch_targets,
+              energy_targets):
+        """The monotonic-alignment-search branch of the teacher-forced forward (kantts_sambert.py:901-925): the alignment
+        attention of the mel targets over the (scaled) symbol embeddings, MAS durations, the frame-level pitch / energy
+        targets averaged per symbol, and the trailing padding symbol input_lengths[b] given the T_mel - output_lengths[b]
+        padding frames.  Validates the lengths on the host (the branch's one host read).  -> dict."""
+        L, T_mel = ling_embedding.size(1), mel_targets.size(1)
+        in_lens, out_lens = torch.stack([input_lengths.long(), output_lengths.long()]).tolist()
+        for b, (n, t) in enumerate(zip(in_lens, out_lens)):
+            if not 1 <= n < L:
+                raise ValueError(f"MAS: input_lengths[{b}] = {n} must lie in [1, {L}): the symbol after the last valid one "
+                                 "(the trailing '~') receives the padding frames")
+            if not 1 <= t <= T_mel:
+                raise ValueError(f"MAS: output_lengths[{b}] = {t} must lie in [1, {T_mel}]")
+        attn_soft, attn_logprob = self.align_attention(mel_targets, ling_embedding, input_masks, attn_priors)
+        attn_hard, durations = sops.mas(attn_soft, input_lengths, output_lengths)
+        pitch = sops.average_frame_feat(pitch_targets, durations)
+        energy = sops.average_frame_feat(energy_targets, durations)
+        pad = (T_mel - output_lengths).to(durations.dtype).unsqueeze(1)
+        durations.scatter_(1, input_lengths.long().unsqueeze(1), pad)
+        return dict(attn_soft=attn_soft, attn_hard=attn_hard, attn_logprob=attn_logprob, duration_targets=durations,
+                    pitch_targets=pitch, energy_targets=energy)
+
     def front_half(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
-                   mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, fp_label=None):
-        """Everything of ``forward`` before the decoder: text encoder, filled-pause insertion (``FP``), variance adaptor,
-        the decoder memory and the band width of its attentions.  -> dict of the intermediate results ``forward`` and
-        ``infer.stream_synthesize`` continue from."""
+                   mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, fp_label=None,
+                   attn_priors=None):
+        """Everything of ``forward`` before the decoder: text encoder, filled-pause insertion (``FP``), alignment search
+        (``MAS``, when ``mel_targets`` is given), variance adaptor, the decoder memory and the band width of its attentions.
+        -> dict of the intermediate results ``forward`` and ``infer.stream_synthesize`` continue from."""
         batch_size = inputs_ling.size(0)
         r = self.mel_decoder.r
         input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
-        text_hid, enc_attns, _ = self.text_encoder(inputs_ling, input_masks, return_attns=True)
+        text_hid, enc_attns, ling_embedding = self.text_encoder(inputs_ling, input_masks, return_attns=True)
         inter_lengths = input_lengths
+        mas = {}
+        if self.MAS and mel_targets is not None:
+            mas = self.align(ling_embedding, mel_targets, input_lengths, output_lengths, input_masks, attn_priors,
+                             pitch_targets, energy_targets)
+            duration_targets, pitch_targets, energy_targets = (mas["duration_targets"], mas["pitch_targets"],
+                                                               mas["energy_targets"])
         fp_p = None
         if self.fp_enable:
             fp_p = self.FP_predictor(text_hid)
@@ -1178,14 +1273,16 @@ class KanTtsSAMBERT(nn.Module):
         return dict(enc_attns=enc_attns, fp_p=fp_p, inter_lengths=inter_lengths, output_masks=output_masks,
                     lfr_masks=lfr_masks, lr_text=lr_text, lr_emo=lr_emo, lr_spk=lr_spk, lr_len=lr_len, log_dur_p=log_dur_p,
                     pitch_p=pitch_p, energy_p=energy_p, memory=memory, x_band_width=x_band_width,
-                    band_width_rows=band_width_rows)
+                    band_width_rows=band_width_rows, duration_targets=duration_targets, pitch_targets=pitch_targets,
+                    energy_targets=energy_targets,
+                    **{k: v for k, v in mas.items() if k.startswith("attn_")})
 
     def forward(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
                 mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, attn_priors=None,
                 fp_label=None):
         batch_size = inputs_ling.size(0)
         f = self.front_half(inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths, mel_targets,
-                            duration_targets, pitch_targets, energy_targets, fp_label)
+                            duration_targets, pitch_targets, energy_targets, fp_label, attn_priors)
         output_masks, lr_len, inter_lengths = f["output_masks"], f["lr_len"], f["inter_lengths"]
         x_band_width = h_band_width = f["x_band_width"]
         dec, ax_lst, ah_lst = self.mel_decoder(f["memory"], x_band_width, h_band_width, target=mel_targets,
@@ -1196,16 +1293,20 @@ class KanTtsSAMBERT(nn.Module):
         postnet_outputs = self.mel_postnet(dec_outputs, output_masks, resid=dec_outputs)
         if output_masks is not None:
             postnet_outputs = postnet_outputs.masked_fill(output_masks.unsqueeze(-1), 0)
-        return {
+        res = {
             "x_band_width": x_band_width, "h_band_width": h_band_width, "enc_slf_attn_lst": f["enc_attns"],
             "pnca_x_attn_lst": ax_lst, "pnca_h_attn_lst": ah_lst, "dec_outputs": dec_outputs,
             "postnet_outputs": postnet_outputs, "LR_length_rounded": lr_len,
             "log_duration_predictions": f["log_dur_p"], "pitch_predictions": f["pitch_p"],
             "energy_predictions": f["energy_p"],
-            "duration_targets": duration_targets, "pitch_targets": pitch_targets, "energy_targets": energy_targets,
+            "duration_targets": f["duration_targets"], "pitch_targets": f["pitch_targets"],
+            "energy_targets": f["energy_targets"],
             "fp_predictions": f["fp_p"], "valid_inter_lengths": inter_lengths,
             "LR_text_outputs": f["lr_text"], "LR_emo_outputs": f["lr_emo"], "LR_spk_outputs": f["lr_spk"],
         }
+        if "attn_hard" in f:
+            res.update(attn_soft=f["attn_soft"], attn_hard=f["attn_hard"], attn_logprob=f["attn_logprob"])
+        return res
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1271,3 +1372,36 @@ class FpCELoss(nn.Module):
         valid = ~get_mask_from_lengths(input_lengths, max_len=fp_label.size(1))
         ce = F.cross_entropy(fp_pd.transpose(2, 1), fp_label, weight=self.weight, reduction="none")
         return torch.sum(ce * valid) / valid.sum()
+
+
+class AttentionCTCLoss(nn.Module):
+    """train/loss.py:481-508: the forward-sum loss of the alignment attention, each utterance's CTC loss of the targets
+    1..in_len over its frames' log_softmax([blank_logprob, keys < in_len]), divided by in_len (0 when infinite), averaged
+    over the batch -- all utterances in one kt_attn_ctc_fwd / _bwd launch instead of a torch.nn.CTCLoss call each."""
+
+    def __init__(self, blank_logprob=-1):
+        super().__init__()
+        self.blank_logprob = blank_logprob
+
+    def forward(self, attn_logprob, in_lens, out_lens):
+        return sops.AttnCtcFn.apply(attn_logprob, in_lens, out_lens, float(self.blank_logprob))
+
+
+class AttentionBinarizationLoss(nn.Module):
+    """train/loss.py:463-478: -sum log(clamp(soft, eps)) over the cells of the hard alignment / their count, scaled by the
+    warm-up ratio min(1, (epoch - start_epoch) / warmup_epoch) (0 before start_epoch).  Written as a masked sum
+    (``hard`` is exactly 0 / 1) instead of the reference's boolean indexing, so it never synchronises with the host."""
+
+    def __init__(self, start_epoch=0, warmup_epoch=100):
+        super().__init__()
+        self.start_epoch = start_epoch
+        self.warmup_epoch = warmup_epoch
+
+    def forward(self, epoch, hard_attention, soft_attention, eps=1e-12):
+        log_sum = (hard_attention * torch.log(torch.clamp(soft_attention, min=eps))).sum()
+        kl_loss = -log_sum / hard_attention.sum()
+        if epoch < self.start_epoch:
+            warmup_ratio = 0
+        else:
+            warmup_ratio = min(1.0, (epoch - self.start_epoch) / self.warmup_epoch)
+        return kl_loss * warmup_ratio

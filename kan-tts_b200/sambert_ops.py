@@ -309,3 +309,108 @@ class FpInsertFn(torch.autograd.Function):
         call("kt_fp_insert_bwd", ptr(dout), ptr(codes, True), ptr(rows, True), ptr(dtext), ptr(dfp), ptr(part),
              0 if part is None else part.numel(), B, L, codes.shape[1], dout.shape[1], C, launches=1 + 2 * (dfp is not None))
         return dtext, dfp, None, None, None
+
+
+# ------------------------------------------------------------------------------------------------
+# alignment learning (MAS: True): kt_align_attn_*, kt_mas, kt_attn_ctc_*
+# ------------------------------------------------------------------------------------------------
+
+
+def _i32(t):
+    return t.to(torch.int32).contiguous()
+
+
+class AlignAttnFn(torch.autograd.Function):
+    """The distance attention of ConvAttention.forward (attention.py:100-125) after its two projections: queries q
+    (B, T_mel, C) and keys k (B, T_text, C), as rows; the optional prior (B, T_mel, T_text); key_lengths (B,) (the padded
+    keys are masked for ``soft`` only).  -> attn_soft, attn_logprob (B, 1, T_mel, T_text).  Both outputs carry gradient:
+    the softmax backward through soft (masked keys excluded), then with a prior the log_softmax backward over all keys."""
+
+    @staticmethod
+    def forward(ctx, q, k, prior, key_lengths):
+        q, k = q.contiguous(), k.contiguous()
+        B, Tq, C = q.shape
+        Tk = k.shape[1]
+        pr = None if prior is None else prior.contiguous()
+        if pr is not None:
+            assert pr.shape == (B, Tq, Tk), (pr.shape, B, Tq, Tk)
+        kl = _i32(key_lengths)
+        logprob = torch.empty(B, Tq, Tk, device=q.device, dtype=torch.float32)
+        soft = torch.empty_like(logprob)
+        lse = torch.empty(B, Tq, device=q.device, dtype=torch.float32) if pr is not None else None
+        call("kt_align_attn_fwd", ptr(q), ptr(k), ptr(pr), ptr(kl, True), ptr(logprob), ptr(soft), ptr(lse), B, Tq, Tk, C)
+        ctx.save_for_backward(q, k, pr, soft, lse)
+        return soft.view(B, 1, Tq, Tk), logprob.view(B, 1, Tq, Tk)
+
+    @staticmethod
+    def backward(ctx, d_soft, d_logprob):
+        q, k, pr, soft, lse = ctx.saved_tensors
+        B, Tq, C = q.shape
+        Tk = k.shape[1]
+        ds = None if d_soft is None else d_soft.reshape(B, Tq, Tk).contiguous()
+        dl = None if d_logprob is None else d_logprob.reshape(B, Tq, Tk).contiguous()
+        dq, dk = torch.empty_like(q), torch.empty_like(k)
+        if ds is None and dl is None:
+            return dq.zero_(), dk.zero_(), None, None
+        dz = torch.empty(B, Tq, Tk, device=q.device, dtype=torch.float32)
+        call("kt_align_attn_bwd", ptr(q), ptr(k), ptr(pr), ptr(soft), ptr(lse), ptr(ds), ptr(dl), ptr(dz), ptr(dq), ptr(dk),
+             B, Tq, Tk, C, launches=2)
+        return dq, dk, None, None
+
+
+def mas(attn_soft, in_lengths, out_lengths):
+    """binarize_attention_parallel (kantts_sambert.py:752-764) on the device, no autograd: mas_width1 of every
+    attn_soft[b, 0, :out_lengths[b], :in_lengths[b]] (kt_mas).  -> attn_hard (B, 1, T_mel, T_text) and the durations
+    attn_hard.sum(2) as (B, T_text) float32."""
+    soft = attn_soft.detach().reshape(attn_soft.shape[0], attn_soft.shape[-2], attn_soft.shape[-1]).contiguous()
+    B, Tq, Tk = soft.shape
+    hard = torch.empty(B, 1, Tq, Tk, device=soft.device, dtype=torch.float32)
+    dur = torch.empty(B, Tk, device=soft.device, dtype=torch.float32)
+    n = int(_lib.load().kt_mas_workspace_bytes(B, Tq, Tk))
+    ws = torch.empty((n + 3) // 4, device=soft.device, dtype=torch.int32) if n else None
+    il, ol = _i32(in_lengths), _i32(out_lengths)          # held until the launch: their memory must not be reused
+    call("kt_mas", ptr(soft), ptr(il, True), ptr(ol, True), ptr(hard), ptr(dur), ptr(ws, True), n, B, Tq, Tk)
+    return hard, dur
+
+
+class AttnCtcFn(torch.autograd.Function):
+    """AttentionCTCLoss.forward (train/loss.py:488-508): attn_logprob (B, 1, T_mel, T_text), in_lengths / out_lengths (B,)
+    -> the scalar mean over the batch of each utterance's CTC loss / in_length (0 when infinite).  The per-frame
+    log_softmax over [blank, valid keys], the alpha / beta recursions and the gradient run in kt_attn_ctc_*."""
+
+    @staticmethod
+    def forward(ctx, attn_logprob, in_lengths, out_lengths, blank_logprob=-1.0):
+        lp = attn_logprob.reshape(attn_logprob.shape[0], attn_logprob.shape[-2], attn_logprob.shape[-1]).contiguous()
+        B, Tq, Tk = lp.shape
+        il, ol = _i32(in_lengths), _i32(out_lengths)
+        n = int(_lib.load().kt_attn_ctc_workspace_bytes(B, Tq, Tk))
+        ws = torch.empty(n // 4, device=lp.device, dtype=torch.float32)
+        loss = torch.empty((), device=lp.device, dtype=torch.float32)
+        call("kt_attn_ctc_fwd", ptr(lp), ptr(il, True), ptr(ol, True), ptr(loss), ptr(ws), n, B, Tq, Tk, float(blank_logprob),
+             launches=2)
+        ctx.save_for_backward(lp, il, ol, ws)
+        ctx.shape, ctx.blank = attn_logprob.shape, float(blank_logprob)
+        return loss
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        lp, il, ol, ws = ctx.saved_tensors
+        B, Tq, Tk = lp.shape
+        d_lp = torch.empty_like(lp)
+        d_loss = d_loss.contiguous()
+        call("kt_attn_ctc_bwd", ptr(lp), ptr(il, True), ptr(ol, True), ptr(d_loss), ptr(ws), ws.numel() * 4,
+             ptr(d_lp), B, Tq, Tk, ctx.blank)
+        return d_lp.view(ctx.shape), None, None, None
+
+
+def average_frame_feat(feat, durs):
+    """average_frame_feat (kantts_sambert.py:652-674) as device torch ops: feat (B, T_frames) frame values, durs (B, L)
+    -> (B, L) the mean of each symbol's frames over its non-zero frames (0 when it has none), from cumulative-sum
+    differences."""
+    ends = torch.cumsum(durs, dim=1).long()
+    starts = torch.nn.functional.pad(ends[:, :-1], (1, 0))
+    nonzero = torch.nn.functional.pad(torch.cumsum(feat != 0.0, dim=1), (1, 0))
+    sums = torch.nn.functional.pad(torch.cumsum(feat, dim=1), (1, 0))
+    total = (torch.gather(sums, 1, ends) - torch.gather(sums, 1, starts)).float()
+    count = (torch.gather(nonzero, 1, ends) - torch.gather(nonzero, 1, starts)).float()
+    return torch.where(count == 0.0, count, total / count)

@@ -392,18 +392,24 @@ class SambertStep:
         self.grad_clip = grad_clip
         self.grads = FlatGrads(model)
         self.steps = 0
+        # the training epoch the caller's loop is in (Sambert_Trainer.epoch): the warm-up of AttentionBinarizationLoss
+        self.epoch = 0
 
     def step(self, batch):
         """batch: dict with the reference collate keys (input_lings, input_emotions, input_speakers,
         valid_input_lengths, valid_output_lengths, mel_targets, durations, pitch_contours, energy_contours),
         tensors already on the model's device; plus ``fp_label`` for a filled-pause (FP) model, whose durations /
-        pitch / energy contours are padded to the length with the pauses inserted."""
+        pitch / energy contours are padded to the length with the pauses inserted.  With the two attention losses in the
+        criterion (a MAS model, the reference's ``with_MAS``) the batch has ``attn_priors`` (B, T_mel, L), frame-level
+        pitch / energy contours and no durations (None or absent): the model finds them by alignment search."""
         fp_label = batch.get("fp_label")
+        with_mas = "AttentionCTCLoss" in self.criterion and "AttentionBinarizationLoss" in self.criterion
         res = self.model(
             batch["input_lings"], batch["input_emotions"], batch["input_speakers"], batch["valid_input_lengths"],
             output_lengths=batch["valid_output_lengths"], mel_targets=batch["mel_targets"],
-            duration_targets=batch["durations"], pitch_targets=batch["pitch_contours"],
-            energy_targets=batch["energy_contours"], fp_label=fp_label)
+            duration_targets=batch.get("durations"), pitch_targets=batch["pitch_contours"],
+            energy_targets=batch["energy_contours"], attn_priors=batch.get("attn_priors") if with_mas else None,
+            fp_label=fp_label)
         mel_loss_, mel_loss = self.criterion["MelReconLoss"](
             batch["valid_output_lengths"], batch["mel_targets"], res["dec_outputs"], res["postnet_outputs"])
         dur_loss, pitch_loss, energy_loss = self.criterion["ProsodyReconLoss"](
@@ -414,6 +420,12 @@ class SambertStep:
         if "FpCELoss" in self.criterion:
             fp_loss = self.criterion["FpCELoss"](batch["valid_input_lengths"], res["fp_predictions"], fp_label)
             loss_total = loss_total + fp_loss
+        attn_ctc_loss = attn_kl_loss = None
+        if with_mas:
+            attn_ctc_loss = self.criterion["AttentionCTCLoss"](res["attn_logprob"], batch["valid_input_lengths"],
+                                                               batch["valid_output_lengths"])
+            attn_kl_loss = self.criterion["AttentionBinarizationLoss"](self.epoch, res["attn_hard"], res["attn_soft"])
+            loss_total = loss_total + attn_ctc_loss + attn_kl_loss
         self.grads.zero()
         loss_total.backward()
         ops.join_wgrad_streams(loss_total.device if loss_total.is_cuda else None)
@@ -429,6 +441,8 @@ class SambertStep:
                "h_band_width": res["h_band_width"]}
         if fp_loss is not None:
             out["fp_loss"] = fp_loss.detach()
+        if attn_ctc_loss is not None:
+            out["attn_ctc_loss"], out["attn_kl_loss"] = attn_ctc_loss.detach(), attn_kl_loss.detach()
         return out
 
 
