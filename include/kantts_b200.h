@@ -504,6 +504,38 @@ int kt_nsf_excitation(const float* f0uv, int32_t f0uv_pitch, int32_t f0uv_first,
                       int32_t e_pitch, int32_t e_first, int32_t batch, int32_t frames, int32_t hop, int32_t nb_harmonics,
                       int32_t sampling_rate, float alpha, float sigma, void* stream);
 
+/* Speaker-embedding extractor (kantts/preprocess/se_processor, csrc/speaker.cu): inference only, exact fp32, fixed-order
+ * reductions.  Item b of a batch owns rows [0, lengths[b]) of its tensors; every kernel writes the rows at or past that as
+ * zeros and reduces over the valid rows only, so an item's results do not depend on the rest of its batch.
+ *
+ * kt_kaldi_fbank: torchaudio.compliance.kaldi.fbank(wav[b, :lengths[b]], num_mel_bins=n_mels) at its other defaults
+ * (400-sample frames every 160 samples, snip_edges, no dither, DC removal, pre-emphasis 0.97, povey window, 512-point power
+ * spectrum, Kaldi mel triangles from low_hz to Nyquist, log(max(e, FLT_EPSILON))), minus each channel's mean over the
+ * utterance's frames.  out [batch][frames][n_mels], frames = 1 + (n_samples - 400) / 160; item b has
+ * 1 + (lengths[b] - 400) / 160 frames (lengths[b] in [400, n_samples]).  Two launches.
+ * kt_se_tap_gather: y[b][fo][t][k][c] (rows of y_pitch floats) = x[b * sb + fi * sf + t * st + c] with
+ * fi = stride * fo + k - pad (zero outside [0, f_in)): the frequency taps of a 2-D conv as the channels of a 1-D one.
+ * kt_se_affine_rows: y[b][r][c] (row pitch y_pitch) = act(scale[c] * x[b][r][c] + shift[c]) (row pitch x_pitch); scale and
+ * shift both NULL for a copy; act = ReLU when relu != 0.
+ * kt_se_gate_stats: per item and `seg`-row segment (the last one partial), the sum and the max of each channel of h
+ * [batch][t][c] over the segment's valid rows into stats [batch][ceil(t / seg)][2][c]; zeroes h's rows past each item.
+ * kt_se_gate_apply: per segment, s = sigmoid(w2 relu(w1 (mean(h) + segmax(h)) + b1) + b2) from those stats (w1 [c_mid][c],
+ * w2 [c_out][c_mid]), then out[b][r][o] (row pitch out_pitch) = y[b][r][o] * s[o], y [batch][t][c_out].
+ * kt_se_stats_pool: out [batch][2c] = the mean and the unbiased std of each channel of x [batch][t][c] over the valid rows. */
+int kt_kaldi_fbank(const float* wav, const int32_t* lengths, float* out, int32_t batch, int32_t n_samples, int32_t frames,
+                   int32_t n_mels, float sample_rate, float low_hz, void* stream);
+int kt_se_tap_gather(const float* x, int64_t sb, int64_t sf, int64_t st, const int32_t* lengths, float* y, int32_t y_pitch,
+                     int32_t batch, int32_t f_in, int32_t t, int32_t c, int32_t f_out, int32_t taps, int32_t stride,
+                     int32_t pad, void* stream);
+int kt_se_affine_rows(const float* x, int32_t x_pitch, const float* scale, const float* shift, int32_t relu,
+                      const int32_t* lengths, float* y, int32_t y_pitch, int32_t batch, int32_t t, int32_t c, void* stream);
+int kt_se_gate_stats(float* h, const int32_t* lengths, float* stats, int32_t batch, int32_t t, int32_t c, int32_t seg,
+                     void* stream);
+int kt_se_gate_apply(const float* y, const float* stats, const float* w1, const float* b1, const float* w2, const float* b2,
+                     const int32_t* lengths, float* out, int32_t out_pitch, int32_t batch, int32_t t, int32_t c,
+                     int32_t c_mid, int32_t c_out, int32_t seg, void* stream);
+int kt_se_stats_pool(const float* x, const int32_t* lengths, float* out, int32_t batch, int32_t t, int32_t c, void* stream);
+
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

@@ -10,12 +10,13 @@ Public surface = the reference's own module API for this path:
   infer.synthesize (symbols -> SAM-BERT free-running decode -> HiFi-GAN -> waveforms, no .npy hand-off)
   infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs, causal generators)
   infer.TtsServer (continuous batching: requests join and leave the slots of one running stream)
+  speaker.DTDNN / kaldi_fbank / speaker_embedding (kantts.preprocess.se_processor: the SE flow's speaker embeddings)
   install.install() patches these into an importable KAN-TTS checkout.
 All tensor math runs in libkantts_b200.so (C ABI: include/kantts_b200.h); there is no fallback.
 """
 from . import _lib  # noqa: F401
 from ._lib import build_library  # noqa: F401
-from . import ops, hifigan, audio, loss, sambert_ops, sambert, train, infer, install as _install  # noqa: F401
+from . import ops, hifigan, audio, loss, sambert_ops, sambert, train, infer, speaker, install as _install  # noqa: F401
 from .sambert import (KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss, AttentionCTCLoss,  # noqa: F401
                       AttentionBinarizationLoss, ConvAttention)
 from .hifigan import Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator  # noqa: F401
@@ -24,6 +25,7 @@ from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversa
                    DiscriminatorAdversarialLoss, FeatureMatchLoss, criterion_builder)
 from .train import GanStep, SambertStep, hifigan_model_builder, sambert_model_builder  # noqa: F401
 from .infer import synthesize, stream_synthesize, TtsServer, slot_schedule  # noqa: F401
+from .speaker import DTDNN, kaldi_fbank, speaker_embedding  # noqa: F401
 
 
 
@@ -62,6 +64,15 @@ def sambert_16k_mas_byte_config():
     256 byte values plus padding, end-of-sentence and mask, in place of the PinYin tables."""
     cfg = {k: v for k, v in sambert_16k_mas_config().items() if k not in ("sy", "tone", "syllable_flag", "word_segment")}
     return dict(cfg, using_byte=True, byte_index=259)
+
+
+def sambert_se_nsf_global_16k_config():
+    """``Model.KanTtsSAMBERT.params`` of kantts/configs/sambert_se_nsf_global_16k.yaml: the sambert_24k.yaml network driven
+    by a 192-d speaker embedding per symbol (``SE: True``, no speaker table) with NSF outputs (80 mels + f0 + voiced flag,
+    f0 normalised globally to [30, 730] Hz), and the PinYin unit sizes."""
+    cfg = {k: v for k, v in sambert_24k_config().items() if k != "speaker"}
+    return dict(cfg, speaker_units=192, num_mels=82, NSF=True, nsf_norm_type="global", nsf_f0_global_minimum=30.0,
+                nsf_f0_global_maximum=730.0, SE=True)
 
 
 install = _install.install

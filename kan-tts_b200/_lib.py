@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libkantts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu"]
+SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
@@ -138,6 +138,12 @@ PROTOTYPES = {
     "kt_lstm_stream_slots": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
+    "kt_kaldi_fbank": [_P, _P, _P, _I, _I, _I, _I, _F, _F, _P],
+    "kt_se_tap_gather": [_P, _L, _L, _L, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
+    "kt_se_affine_rows": [_P, _I, _P, _P, _I, _P, _P, _I, _I, _I, _I, _P],
+    "kt_se_gate_stats": [_P, _P, _P, _I, _I, _I, _I, _P],
+    "kt_se_gate_apply": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    "kt_se_stats_pool": [_P, _P, _P, _I, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_debug_conv_tc_epilogue": [ctypes.POINTER(KtConv1dDesc), _I],
@@ -157,7 +163,7 @@ def nvcc_command(out_path=LIB_PATH):
 def build_library(force=False, verbose=False):
     """Compile libkantts_b200.so in-tree for sm_90a (cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, h) for h in ("common.cuh", "tc_common.cuh", "tma.cuh", "wgmma.cuh", "philox.cuh")] + [
+    deps = srcs + [os.path.join(CSRC, h) for h in ("common.cuh", "tc_common.cuh", "tma.cuh", "wgmma.cuh", "philox.cuh", "fft.cuh")] + [
                    os.path.join(os.path.dirname(_HERE), "include", "kantts_b200.h")]
     deps = [d for d in deps if os.path.exists(d)]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):

@@ -239,13 +239,14 @@ class TtsServer:
         self._queue, self._slots, self._chunk, self._next_id = [], [None] * self.batch, 0, 0
 
     def submit(self, ling, emotion, speaker, length, nsf_seed=None):
-        """Queue one utterance: ling (L, 4), emotion (L,), speaker (L,) long tensors and its symbol count ``length``;
-        ``nsf_seed`` (an int) for an NSF generator.  -> the request id."""
+        """Queue one utterance: ling (L, 4), emotion (L,) long tensors, speaker (L,) ids, or the (L, speaker_units) float
+        embedding rows of a speaker-embedding (SE) model, and its symbol count ``length``; ``nsf_seed`` (an int) for an NSF
+        generator.  -> the request id."""
         if self.nsf != (nsf_seed is not None):
             raise ValueError("submit: an NSF generator needs each request's nsf_seed, any other generator none")
         rid, self._next_id = self._next_id, self._next_id + 1
         self._queue.append(dict(id=rid, seed=nsf_seed, inputs=(ling.reshape(1, -1, ling.shape[-1]), emotion.reshape(1, -1),
-                                                                speaker.reshape(1, -1), torch.tensor([int(length)]))))
+                                                                speaker.unsqueeze(0), torch.tensor([int(length)]))))
         return rid
 
     @property

@@ -1,11 +1,17 @@
 """Patch the H100-native classes into an importable KAN-TTS checkout so that its unchanged
 ``kantts/bin/train_hifigan.py`` / ``kantts.train.trainer.GAN_Trainer`` run on them
 (see INTEGRATION.md).  ``model_builder`` looks classes up by name in ``kantts.models``' globals
-(kantts/models/__init__.py:38,51) and ``criterion_builder`` in ``loss_dict`` (loss.py:512-544)."""
+(kantts/models/__init__.py:38,51) and ``criterion_builder`` in ``loss_dict`` (loss.py:512-544).  The speaker-embedding
+processor (kantts/preprocess/se_processor/se_processor.py) builds its model as ``DTDNN()`` from its module globals, so
+replacing that name runs the unchanged ``SpeakerEmbeddingProcessor`` on speaker.DTDNN."""
+import sys
 
 
-def install(kantts_models=None, kantts_loss=None, kantts_audio=None):
-    from . import audio, hifigan, loss
+def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=None):
+    """``kantts_se``: the speaker-embedding processor module to patch; by default
+    kantts.preprocess.se_processor.se_processor when it is already imported.  It is never imported here: it needs
+    torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want."""
+    from . import audio, hifigan, loss, speaker
     if kantts_models is None:
         import kantts.models as kantts_models
     if kantts_loss is None:
@@ -21,4 +27,8 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None):
         setattr(kantts_loss, cls.__name__, cls)
     kantts_audio.MelSpectrogram = audio.MelSpectrogram
     kantts_audio.stft = audio.stft
+    if kantts_se is None:
+        kantts_se = sys.modules.get("kantts.preprocess.se_processor.se_processor")
+    if kantts_se is not None:
+        kantts_se.DTDNN = speaker.DTDNN
     return kantts_models

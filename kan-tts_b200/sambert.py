@@ -21,8 +21,10 @@ kernels, and the splice of the predicted or labelled pauses into the text encodi
 gather each way (kt_fp_insert_*).  The alignment-learning variant (``MAS: True``, sambert_16k_MAS*.yaml) is built:
 ConvAttention's projections on the conv kernels, its distance attention fused in kt_align_attn_* (no (B, C, T_mel,
 T_text) difference tensor), monotonic alignment search on the GPU (kt_mas, no host copy) and the forward-sum loss in
-kt_attn_ctc_*.  Not built: the speaker-encoder (``SE``) variant, and MAS together with FP (the reference's two branches
-do not compose: its MAS durations have one entry per symbol before the pause splice).
+kt_attn_ctc_*.  The speaker-embedding variant (``SE: True``, sambert_se_nsf_global_16k.yaml) is built: it has no speaker
+table, and ``inputs_speaker`` is the float (B, L, speaker_units) per-symbol embedding (speaker.speaker_embedding) in
+place of the ids.  Not built: MAS together with FP (the reference's two branches do not compose: its MAS durations have
+one entry per symbol before the pause splice), and SE together with FP or MAS.
 """
 import ctypes
 from collections import namedtuple
@@ -1158,13 +1160,14 @@ class KanTtsSAMBERT(nn.Module):
 
     def __init__(self, config):
         super().__init__()
-        if config.get("SE", False):
-            raise NotImplementedError("KanTtsSAMBERT variant SE=True is not built (see module docstring)")
+        if config.get("SE", False) and (config.get("FP", False) or config.get("MAS", False)):
+            raise NotImplementedError("KanTtsSAMBERT with SE=True together with FP or MAS is not built (see module docstring)")
         if config.get("MAS", False) and config.get("FP", False):
             raise NotImplementedError("KanTtsSAMBERT with both MAS=True and FP=True is not built (see module docstring)")
         self.text_encoder = TextFftEncoder(config)
-        self.se_enable = False
-        self.spk_tokenizer = nn.Embedding(config["speaker"], config["speaker_units"])
+        self.se_enable = bool(config.get("SE", False))
+        if not self.se_enable:
+            self.spk_tokenizer = nn.Embedding(config["speaker"], config["speaker_units"])
         self.emo_tokenizer = nn.Embedding(config["emotion"], config["emotion_units"])
         self.variance_adaptor = VarianceAdaptor(config)
         self.mel_decoder = MelPNCADecoder(config)
@@ -1244,7 +1247,7 @@ class KanTtsSAMBERT(nn.Module):
             text_hid, inputs_emotion, inputs_speaker, inter_lengths = self.insert_fp(
                 text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths)
         emo_hid = self.emo_tokenizer(inputs_emotion)
-        spk_hid = self.spk_tokenizer(inputs_speaker)
+        spk_hid = inputs_speaker if self.se_enable else self.spk_tokenizer(inputs_speaker)
         inter_masks = get_mask_from_lengths(inter_lengths, max_len=text_hid.size(1))
         output_masks = None
         if output_lengths is not None:
