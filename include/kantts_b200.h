@@ -435,30 +435,26 @@ int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32
                            int32_t first, int32_t frames, void* stream);
 
 /* ---- streaming SAM-BERT post-net (PostNet.streamer: decoder rows in, final post-net rows out, chunk by chunk) ---------------
- * kt_fsmn_fwd_stream: one chunk of MemoryBlockV2 with FsmnEncoderV2's residual fused, seen as a causal depthwise FIR whose
- * output lags its input by rp = k - 1 - pad_left rows.  x, y and resid are windows placed by `w` (KtStreamWin, c channels):
- * input rows [-(k-1), rows) of the chunk are read (in_first >= k - 1), output rows [0, rows) are written.  Output row t is
- * frame row0 + t of the utterance; its tap j reads input row t + j - (k-1), frame row0 + t + j - pad_left.  With
- * keep(b, a) = (0 <= a < lengths[b]) (lengths: device int32 [batch]) and xm = keep * x:
+ * Chunk row t of item b is frame frame0[b] + offset + t of its utterance (frame0: device int32 [batch]), so each slot can be
+ * anywhere in its own utterance and no chunk reads device data on the host.
+ *
+ * kt_fsmn_fwd_stream_slots: one chunk of MemoryBlockV2 with FsmnEncoderV2's residual fused, seen as a causal depthwise FIR
+ * whose output lags its input by rp = k - 1 - pad_left rows.  x, y and resid are windows placed by `w` (KtStreamWin, c
+ * channels): input rows [-(k-1), rows) of the chunk are read (in_first >= k - 1), output rows [0, rows) are written.  Output
+ * row t is frame row0 + t, row0 = frame0[b] + offset; its tap j reads input row t + j - (k-1), frame row0 + t + j - pad_left.
+ * With keep(b, a) = (0 <= a < lengths[b]) (lengths: device int32 [batch]) and xm = keep * x:
  *   y[t] = keep(row0 + t) * (xm[t - rp] + sum_j weight[c][j] * xm[t + j - (k-1)]) + resid[t]      (resid optional)
- * Frames before 0 and from lengths[b] on read as zeros, so no chunk reads device data on the host.  The taps are summed in
- * kt_fsmn_fwd's order: a streamed row equals the whole-sequence row bit for bit.  weight [c][k] as in kt_fsmn_fwd. */
-int kt_fsmn_fwd_stream(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths, const float* resid, float* y,
-                       int32_t batch, int32_t rows, int32_t c, int32_t k, int32_t pad_left, int32_t row0, void* stream);
-/* kt_lstm_stream: `rows` steps of a 1-layer unidirectional nn.LSTM (hidden <= 256), one CTA per batch item.
+ * xm is a selection, not a product: frames before 0 and from lengths[b] on read as zeros whatever the window holds there.
+ * The skip term first, then the taps in order, each an fma: kt_fsmn_fwd's sum, so a streamed row equals the whole-sequence
+ * row bit for bit.  weight [c][k] as in kt_fsmn_fwd.
+ * kt_lstm_stream_slots: `rows` steps of a 1-layer unidirectional nn.LSTM (hidden <= 256), one CTA per batch item.
  *   gx     row t of item b at gx[(b * gx_pitch + t) * 4 * hidden]: x . weight_ih^T + bias_ih + bias_hh (one k = 1 conv)
  *   whh_t  [hidden][4 * hidden] = weight_hh^T
- *   state  [batch][2][hidden]: (h, c) before the first step, overwritten with (h, c) after the last (zeros start an utterance)
+ *   state  [batch][2][hidden]: (h, c) carried from the previous chunk, overwritten with (h, c) after the last row.  A chunk
+ *          whose first row is frame 0 or earlier ignores it and starts from (h, c) = 0; a row before frame 0 leaves (h, c)
+ *          as they are (zero) and outputs that zero h, so frame 0 starts from (h, c) = 0.
  *   h      row t of item b at h[(b * h_pitch + t) * hidden]: the LSTM output.
  * PyTorch gate order (i, f, g, o); exact fp32. */
-int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t batch, int32_t rows, int32_t hidden,
-                   int32_t gx_pitch, int32_t h_pitch, void* stream);
-/* Per-slot forms (PostNet.streamer(per_slot=True)): chunk row t of item b is frame frame0[b] + offset + t (frame0: device
- * int32 [batch]), so each slot can be anywhere in its own utterance.
- * kt_fsmn_fwd_stream_slots: kt_fsmn_fwd_stream with row0 = frame0[b] + offset per item (same sum, same order).
- * kt_lstm_stream_slots: kt_lstm_stream where a chunk whose first row is frame 0 or earlier starts from (h, c) = 0 and a later
- * chunk from the carried state; a row before frame 0 leaves (h, c) as they are (zero) and outputs that zero h, so frame 0
- * starts from (h, c) = 0. */
 int kt_fsmn_fwd_stream_slots(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths,
                              const int32_t* frame0, int32_t offset, const float* resid, float* y, int32_t batch, int32_t rows,
                              int32_t c, int32_t k, int32_t pad_left, void* stream);

@@ -132,8 +132,6 @@ PROTOTYPES = {
     "kt_conv1d_fwd_tc_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin),
                                        ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P],
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
-    "kt_fsmn_fwd_stream": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
-    "kt_lstm_stream": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P],
     "kt_lstm_stream_slots": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],

@@ -1198,109 +1198,17 @@ extern "C" int kt_ar_duration_infer(const float* g0c, const float* w1, const flo
 }
 
 // ---------------------------------------------------------------------------------------------
-// Streaming post-net (PostNet.streamer): one chunk of MemoryBlockV2 and one chunk of the post-net LSTM.
+// Streaming post-net (PostNet.streamer): one chunk of MemoryBlockV2 and one chunk of the post-net LSTM.  The frame of a
+// slot's chunk row comes from the device (frame0[b] + offset), so every slot of one launch can sit at a different place in
+// its own utterance.
 //
-// fsmn_stream_kernel: the memory block as a causal depthwise FIR whose output lags its input by rp = K-1-lp rows.  Output
-// row t of the chunk is frame row0 + t; its taps j < K read input rows t + j - (K-1) of the chunk (negative: the window's
-// history), frames row0 + t + j - lp.  keep(b, a) = 0 <= a < lengths[b]; xm = keep * x.
+// fsmn_stream_slots_kernel: the memory block as a causal depthwise FIR whose output lags its input by rp = K-1-lp rows.
+// Output row t of item b's chunk is frame row0 + t, row0 = frame0[b] + offset; its taps j < K read input rows t + j - (K-1)
+// of the chunk (negative: the window's history), frames row0 + t + j - lp.  keep(b, a) = 0 <= a < lengths[b]; xm = keep * x,
+// by selection, so whatever a window holds outside the utterance reads as zero.
 //   y[t] = keep(row0 + t) * (xm[t - rp] + sum_j w[c][j] * xm[t + j - (K-1)]) + resid[t]
 // The skip term first, then the taps in order, each an fmaf with the masked value: fsmn_fir_kernel's sum, so a streamed row
 // equals the whole-sequence row bit for bit.  One thread per (row, channel) of one item (blockIdx.y).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) fsmn_stream_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                          const int* __restrict__ lengths, const float* __restrict__ resid,
-                                                          float* __restrict__ y, KtStreamWin win, int rows, int C, int K,
-                                                          int lp, int row0) {
-  const int b = blockIdx.y;
-  const int len = __ldg(lengths + b);
-  const long long n = (long long)rows * C;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const int t = (int)(i / C), c = (int)(i - (long long)t * C);
-    const float* xc = x + ((long long)b * win.in_pitch + win.in_first + t - (K - 1)) * C + c;   // tap j: xc[j * C]
-    const int a0 = row0 + t - lp;                                                              // frame of tap 0
-    const bool keep_t = row0 + t >= 0 && row0 + t < len;
-    float acc = keep_t ? __ldg(xc + (long long)lp * C) : 0.f;
-    for (int j = 0; j < K; ++j) {
-      const int a = a0 + j;
-      const float v = (a >= 0 && a < len) ? __ldg(xc + (long long)j * C) : 0.f;
-      acc = fmaf(__ldg(w + (long long)c * K + j), v, acc);
-    }
-    float out = keep_t ? acc : 0.f;
-    if (resid) out += __ldg(resid + ((long long)b * win.res_pitch + win.res_first + t) * C + c);
-    y[((long long)b * win.out_pitch + win.out_first + t) * C + c] = out;
-  }
-}
-
-extern "C" int kt_fsmn_fwd_stream(const KtStreamWin* win, const float* x, const float* w, const int32_t* lengths,
-                                  const float* resid, float* y, int32_t B, int32_t rows, int32_t C, int32_t K, int32_t lp,
-                                  int32_t row0, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  KT_REQUIRE(win && x && w && lengths && y, "fsmn_fwd_stream: null pointer");
-  KT_REQUIRE(B >= 1 && B <= 65535 && rows >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_fwd_stream: bad sizes");
-  KT_REQUIRE(win->in_first >= K - 1 && win->in_first + rows <= win->in_pitch,
-             "fsmn_fwd_stream: the input window needs K - 1 rows of history before the chunk");
-  KT_REQUIRE(win->out_first >= 0 && win->out_first + rows <= win->out_pitch, "fsmn_fwd_stream: the chunk does not fit its output window");
-  KT_REQUIRE(!resid || (win->res_first >= 0 && win->res_first + rows <= win->res_pitch),
-             "fsmn_fwd_stream: the chunk does not fit its residual window");
-  const long long n = (long long)rows * C;
-  const int blocks = (int)std::min<long long>((n + 255) / 256, 1024);
-  fsmn_stream_kernel<<<dim3(blocks, B), 256, 0, st>>>(x, w, lengths, resid, y, *win, rows, C, K, lp, row0);
-  KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
-}
-
-// lstm_stream_kernel: `rows` steps of a 1-layer unidirectional LSTM, carrying (h, c) of item b in state[b][2][H].  One CTA
-// per item, one thread per gate: gate j of step t = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced
-// over j), then one thread per hidden unit updates c and h.  PyTorch gate order (i, f, g, o); exact fp32.
-__global__ void lstm_stream_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
-                                   float* __restrict__ h_out, int rows, int H, int gx_pitch, int h_pitch) {
-  extern __shared__ float sm[];
-  const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x;
-  float* h = sm;             // [H]
-  float* c = h + H;          // [H]
-  float* gates = c + H;      // [4H]
-  float* s = state + (long long)b * 2 * H;
-  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = s[j];
-  __syncthreads();
-  for (int t = 0; t < rows; ++t) {
-    const float* g = gx + ((long long)b * gx_pitch + t) * G;
-    for (int j = tid; j < G; j += blockDim.x) {
-      float acc = __ldg(g + j);
-      for (int k = 0; k < H; ++k) acc = fmaf(__ldg(whh_t + (long long)k * G + j), h[k], acc);
-      gates[j] = acc;
-    }
-    __syncthreads();
-    float* out = h_out + ((long long)b * h_pitch + t) * H;
-    for (int j = tid; j < H; j += blockDim.x) {
-      const float ig = sigmoid_f(gates[j]), fg = sigmoid_f(gates[H + j]), gg = tanhf(gates[2 * H + j]), og = sigmoid_f(gates[3 * H + j]);
-      const float cn = fg * c[j] + ig * gg;
-      const float hn = og * tanhf(cn);
-      c[j] = cn;
-      h[j] = hn;
-      out[j] = hn;
-    }
-    __syncthreads();
-  }
-  for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
-}
-
-extern "C" int kt_lstm_stream(const float* gx, const float* whh_t, float* state, float* h, int32_t B, int32_t rows, int32_t H,
-                              int32_t gx_pitch, int32_t h_pitch, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  KT_REQUIRE(gx && whh_t && state && h, "lstm_stream: null pointer");
-  KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream: bad sizes");
-  const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
-  const size_t smem = (size_t)6 * H * sizeof(float);
-  lstm_stream_kernel<<<B, threads, smem, st>>>(gx, whh_t, state, h, rows, H, gx_pitch, h_pitch);
-  KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Per-slot post-net streaming: the frame of a slot's chunk row comes from the device (frame0[b] + offset), so every slot of
-// one launch can sit at a different place in its own utterance.
-//
-// fsmn_stream_slots_kernel: fsmn_stream_kernel with row0 = frame0[b] + offset per item; the same sum in the same order.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) fsmn_stream_slots_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                 const int* __restrict__ lengths, const int* __restrict__ frame0,
@@ -1346,10 +1254,12 @@ extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const float* x, 
   return KT_OK;
 }
 
-// lstm_stream_slots_kernel: lstm_stream_kernel where row t of item b is frame frame0[b] + offset + t.  A chunk whose first
-// row is frame 0 or earlier starts from (h, c) = 0, a later chunk from the carried state.  A row before frame 0 leaves
-// (h, c) as they are, i.e. zero, and its output row is that zero h; frame 0 therefore starts from zeros.  The gate sums are
-// lstm_stream_kernel's, in the same order.
+// lstm_stream_slots_kernel: `rows` steps of a 1-layer unidirectional LSTM, carrying (h, c) of item b in state[b][2][H];
+// row t of item b is frame frame0[b] + offset + t.  A chunk whose first row is frame 0 or earlier starts from (h, c) = 0
+// whatever state holds, a later chunk from the carried state.  A row before frame 0 leaves (h, c) as they are, i.e. zero,
+// and its output row is that zero h; frame 0 therefore starts from zeros.  One CTA per item, one thread per gate: gate j of
+// step t = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced over j), then one thread per hidden unit
+// updates c and h.  PyTorch gate order (i, f, g, o); exact fp32.
 __global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
                                          float* __restrict__ h_out, const int* __restrict__ frame0, int offset, int rows, int H,
                                          int gx_pitch, int h_pitch) {

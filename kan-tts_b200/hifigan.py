@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, KtStreamMask, ptr
-from .stream import Windows, WindowTable, own_weight, to_device
+from .stream import Windows, WindowTable, check_slots, own_weight, to_device
 
 # --------------------------------------------------------------------------------------------
 # parameter holders (names / shapes == the reference's weight_norm / spectral_norm wrapped convs)
@@ -784,11 +784,7 @@ class GeneratorStreamer:
             self._graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self._graph):
                 self._run(self.max_frames)
-            win.reset()
-            if not plan.causal:
-                self._set_lengths(range(self.batch), lengths)
-            if plan.nsf:
-                self._set_seeds(range(self.batch), seeds)
+            self.reset(range(self.batch), lengths, seeds)
 
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
@@ -856,8 +852,7 @@ class GeneratorStreamer:
     def reset(self, slots, lengths=None, seeds=None):
         """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A non-causal
         generator needs the new utterances' ``lengths`` in frames, an NSF one their excitation ``seeds``, both in the order
-        of ``slots``."""
-        slots = [int(s) for s in slots]
+        of ``slots``.  All of it is checked before the first launch: a rejected reset leaves every slot as it was."""
         if self.plan.causal and lengths is not None:
             raise ValueError("reset: a causal generator streams without lengths")
         if not self.plan.causal and lengths is None:
@@ -866,36 +861,31 @@ class GeneratorStreamer:
             raise ValueError("reset: streaming an NSF generator needs the new utterances' seeds")
         if not self.plan.nsf and seeds is not None:
             raise ValueError("reset: seeds are for NSF generators")
+        slots = check_slots(slots, self.batch)
         with torch.no_grad(), torch.cuda.device(self.device):
+            if lengths is not None:
+                lengths = self._lengths(lengths, len(slots))
+            if seeds is not None:
+                seeds = nsf_seed_tensor(seeds, len(slots), self.device)
             self._win.reset(slots)
-            if not self.plan.causal:
-                self._set_lengths(slots, lengths)
-            if self.plan.nsf:
-                self._set_seeds(slots, seeds)
+            idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
+            if lengths is not None:                 # none of the new utterances' frames pushed yet
+                self._len.index_copy_(0, idx, lengths)
+                self._done.index_fill_(0, idx, 0)
+            if seeds is not None:                   # excitation phases and sample counts return to zero
+                self._nsf.reset(idx, seeds)
 
-    def _set_seeds(self, slots, seeds):
-        """Slots ``slots`` start their excitation from ``seeds``: phases and sample counts return to zero."""
-        slots = list(slots)
-        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
-            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
-        idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
-        self._nsf.reset(idx, nsf_seed_tensor(seeds, len(slots), self.device))
-
-    def _set_lengths(self, slots, lengths):
-        """Slots ``slots`` hold utterances of ``lengths`` frames (host sequence or device tensor), none pushed yet."""
-        slots = list(slots)
-        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
-            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
+    def _lengths(self, lengths, n):
+        """-> the frame counts of n utterances (host sequence or device tensor) as a device int32 tensor (n,); ValueError
+        on a wrong count or, for host values, a length below 1."""
         if not (torch.is_tensor(lengths) and lengths.is_cuda):
             lengths = torch.as_tensor(lengths)
             if lengths.numel() and int(lengths.min()) < 1:
                 raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
-        n = lengths.to(device=self.device, dtype=torch.int32).reshape(-1)
-        if n.numel() != len(slots):
-            raise ValueError(f"streamer: expected {len(slots)} lengths, got {n.numel()}")
-        idx = torch.tensor(slots, dtype=torch.long).to(self.device)
-        self._len.index_copy_(0, idx, n)
-        self._done.index_fill_(0, idx, 0)
+        lengths = lengths.to(device=self.device, dtype=torch.int32).reshape(-1)
+        if lengths.numel() != n:
+            raise ValueError(f"streamer: expected {n} lengths, got {lengths.numel()}")
+        return lengths
 
 
 # --------------------------------------------------------------------------------------------

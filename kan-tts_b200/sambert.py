@@ -37,7 +37,7 @@ import torch.nn.functional as F
 from . import ops
 from . import sambert_ops as sops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, ptr
-from .stream import Windows, WindowTable, own_weight
+from .stream import Windows, WindowTable, check_slots, own_weight
 
 
 def get_mask_from_lengths(lengths, max_len=None):
@@ -859,10 +859,8 @@ class PostNet(nn.Module):
 
 # One launch of a post-net chunk over named windows.  kind "conv": a k = 1 conv of ``module`` (a Linear, or the nn.LSTM's
 # input projection); "fsmn": the memory block ``module`` of FSMN layer ``layer``; "lstm": the nn.LSTM's recurrence.
-# ``resid`` (or None) is added to the output from ``res_lag`` rows before the output's chunk rows.  A ``frame0`` step runs
-# over the chunk's rows of frame >= 0 only, written from row 0 of ``dst``; with ``in_skip`` its input holds every row.
-PostNetStep = namedtuple("PostNetStep", "kind module src dst resid res_lag frame0 in_skip layer",
-                         defaults=(None, 0, False, False, -1))
+# ``resid`` (or None) is added to the output from ``res_lag`` rows before the output's chunk rows.
+PostNetStep = namedtuple("PostNetStep", "kind module src dst resid res_lag layer", defaults=(None, 0, -1))
 
 
 class PostNetStreamPlan:
@@ -905,10 +903,8 @@ class PostNetStreamPlan:
         table.read("dec", self.delay)                      # the output Linear's residual: the decoder rows D rows back
         gates = table.add("gates", 4 * postnet.lstm.hidden_size)
         h = table.add("h", postnet.lstm.hidden_size)
-        self.steps += [PostNetStep("conv", postnet.lstm, x, gates, frame0=True, in_skip=True),
-                       PostNetStep("lstm", postnet.lstm, gates, h, frame0=True),
-                       PostNetStep("conv", postnet.fc, h, table.add("out", postnet.num_mels), "dec", res_lag=self.delay,
-                                   frame0=True)]
+        self.steps += [PostNetStep("conv", postnet.lstm, x, gates), PostNetStep("lstm", postnet.lstm, gates, h),
+                       PostNetStep("conv", postnet.fc, h, table.add("out", postnet.num_mels), "dec", res_lag=self.delay)]
         self.launches_per_chunk = table.launches_per_chunk(len(self.steps))
 
 
@@ -921,17 +917,17 @@ class PostNetStreamer:
     ``delay`` all-padding rows and returns the rest; the rows returned in order are then the whole-sequence post-net output.
     ``reset(lengths=None)`` starts a new batch.  No call reads device data on the host.
 
-    A tensor a layer reads before the chunk lives in a window (stream.py); kt_fsmn_fwd_stream masks by each row's frame
-    index against the slot lengths kept on the device, and kt_lstm_stream carries the LSTM state.  The weights are
-    prepared once, when the streamer is created.
+    Every chunk runs over all f rows of every slot.  Each slot's frame count and the frame ``rows[b]`` of its utterance at
+    the chunk's first decoder row live on the device.  A tensor a layer reads before the chunk lives in a window
+    (stream.py).  The memory blocks (kt_fsmn_fwd_stream_slots) read frames outside [0, lengths[b]) as zeros, the
+    whole-sequence padding, and the LSTM (kt_lstm_stream_slots) starts from zeros at frame 0, so starting an utterance
+    clears no window history or LSTM state; every other step reads only the frame it writes, and the output is masked
+    outside the utterance.  The weights are prepared once, when the streamer is created.
 
-    Per-slot mode (``per_slot=True``): each slot's frame count lives on the device, and the chunk's first decoder row is
-    frame ``rows[b]`` of slot b's utterance.  ``push`` then returns all f rows of every slot, output row t being frame
+    Per-slot mode (``per_slot=True``): ``push`` returns all f rows of every slot, output row t being frame
     rows[b] - delay + t (zero outside [0, lengths[b])).  ``reset(lengths, slots=..., start_row=...)`` starts new
-    utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  The memory
-    blocks (kt_fsmn_fwd_stream_slots) read frames outside [0, lengths[b]) as zeros, the whole-sequence padding, so a slot's
-    window history needs no clearing; the LSTM (kt_lstm_stream_slots) starts from zeros at frame 0.  A slot's new utterance
-    must start after the previous one's last row was returned."""
+    utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  A slot's new
+    utterance must start after the previous one's last row was returned."""
 
     def __init__(self, postnet, batch, max_frames, lengths, per_slot=False):
         self.plan = plan = PostNetStreamPlan(postnet)
@@ -942,8 +938,10 @@ class PostNetStreamer:
         self._state = torch.zeros(self.batch, 2, self.hidden, device=self.device)
         self._zeros = torch.zeros(self.batch, self.max_frames, self.num_mels, device=self.device)
         self._len = torch.empty(self.batch, dtype=torch.int32, device=self.device)
-        self._row = torch.zeros(self.batch, dtype=torch.int32, device=self.device)     # per-slot mode: rows[b]
-        self._steady = [self._place(st, 0) for st in plan.steps]
+        self._row = torch.zeros(self.batch, dtype=torch.int32, device=self.device)     # rows[b]
+        self._out_frame = torch.arange(self.max_frames, dtype=torch.int32, device=self.device) - self.delay  # row t: + rows[b]
+        self._places = [None if st.kind == "lstm" else win.place(st.src, st.dst, st.resid, res_lag=st.res_lag)
+                        for st in plan.steps]
         with torch.no_grad(), torch.cuda.device(self.device):
             self._weights = [self._own_weight(st) for st in plan.steps]
             self.reset(lengths)
@@ -961,18 +959,11 @@ class PostNetStreamer:
             return (spec, *own_weight(spec, mod.weight_ih_l0.unsqueeze(-1), None, mod.bias_ih_l0 + mod.bias_hh_l0))
         return (mod.spec, *own_weight(mod.spec, mod.weight, None, mod.bias))
 
-    def _place(self, st, skip):
-        """-> the KtStreamWin of step st (None for the LSTM) in a chunk whose first ``skip`` rows lie before frame 0."""
-        if st.kind == "lstm":
-            return None
-        o = skip if st.frame0 else 0                    # the chunk row of the step's first output row
-        return self._win.place(st.src, st.dst, st.resid, in_offset=o if st.in_skip else 0, res_lag=st.res_lag - o)
-
-    def _chunk_slots(self, f):
-        """Per-slot mode: every launch of one chunk of f decoder rows over all rows of every slot -> the (B, f, num_mels)
-        output rows, zero where a row's frame lies outside its slot's utterance."""
+    def _chunk(self, f, skip):
+        """Every launch of one chunk of f decoder rows (already in the "dec" window) -> output rows [skip, f) of every slot,
+        zero where a row's frame lies outside its slot's utterance."""
         b, B = self._win.buf, self.batch
-        for st, w, place in zip(self.plan.steps, self._weights, self._steady):
+        for st, w, place in zip(self.plan.steps, self._weights, self._places):
             src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
             if st.kind == "conv":
                 spec, pw, bias = w
@@ -986,47 +977,19 @@ class PostNetStreamer:
                 ops.call("kt_lstm_stream_slots", ptr(src), ptr(w), ptr(self._state), ptr(dst), ptr(self._row, True),
                          -self.delay, B, f, self.hidden, src.shape[1], dst.shape[1])
         self._win.advance(f)
-        frames = self._row[:, None] - self.delay + torch.arange(f, device=self.device, dtype=torch.int32)[None, :]
+        frames = self._row[:, None] + self._out_frame[None, :f]
         pad = (frames < 0) | (frames >= self._len[:, None])
         self._row += f
-        return b["out"][:, :f].masked_fill(pad.unsqueeze(-1), 0)
-
-    def _chunk(self, f):
-        """Every launch of one chunk of f decoder rows (already in the "dec" window) -> the final output rows."""
-        if self.per_slot:
-            return self._chunk_slots(f)
-        b, B, a = self._win.buf, self.batch, self._rows
-        first = a - self.delay                      # frame of the chunk's first output row
-        skip = max(0, -first)                       # output rows before frame 0 are not rows of the utterance
-        n = f - skip
-        places = self._steady if skip == 0 else [self._place(st, skip) for st in self.plan.steps]
-        for st, w, place in zip(self.plan.steps, self._weights, places):
-            if st.frame0 and n <= 0:
-                continue                            # nothing of the utterance has reached this step yet
-            src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
-            rows = n if st.frame0 else f
-            if st.kind == "conv":
-                spec, pw, bias = w
-                ops.stream_conv(spec, pw, bias, src, dst, rows, place, resid)
-            elif st.kind == "fsmn":
-                layer = self.plan.layers[st.layer]
-                ops.call("kt_fsmn_fwd_stream", ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True), ptr(resid), ptr(dst),
-                         B, rows, src.shape[2], layer["kernel"], layer["lp"], a - layer["lag"] - layer["rp"])
-            else:
-                ops.call("kt_lstm_stream", ptr(src), ptr(w), ptr(self._state), ptr(dst), B, rows, self.hidden, src.shape[1],
-                         dst.shape[1])
-        self._win.advance(f)
-        self._rows += f
-        if n <= 0:
-            return b["out"][:, :0].clone()
-        frames = torch.arange(first + skip, first + f, device=self.device)
-        pad = frames[None, :] >= self._len[:, None]
-        return b["out"][:, :n].masked_fill(pad.unsqueeze(-1), 0)
+        return b["out"][:, skip:f].masked_fill(pad[:, skip:].unsqueeze(-1), 0)
 
     def push(self, dec_rows):
-        """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final."""
+        """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final
+        (per-slot mode: all f rows)."""
         with torch.no_grad(), torch.cuda.device(self.device):
-            return self._chunk(self._win.push("dec", dec_rows, 1, ("{} decoder rows", "rows", "the rows are")))
+            f = self._win.push("dec", dec_rows, 1, ("{} decoder rows", "rows", "the rows are"))
+            skip = 0 if self.per_slot else min(f, max(0, self.delay - self._rows))    # rows before frame 0
+            self._rows += f
+            return self._chunk(f, skip)
 
     def finish(self):
         """Push ``delay`` all-padding rows (the whole-sequence zero padding) -> the remaining (B, n, num_mels) output rows."""
@@ -1038,12 +1001,12 @@ class PostNetStreamer:
         return torch.cat(outs, 1) if outs else self._zeros[:, :0].clone()
 
     def reset(self, lengths=None, slots=None, start_row=0):
-        """Start a new batch: the carried windows and LSTM state return to zeros; ``lengths`` (device tensor (batch,)),
-        when given, replaces the slots' frame counts.
+        """Start a new batch: every slot's frame 0 is row 0 of the next push; ``lengths`` (device tensor (batch,)), when
+        given, replaces the slots' frame counts.
 
         Per-slot mode with ``slots`` (host ints): only those slots start new utterances, of ``lengths`` frames (host ints,
-        in the order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames).
-        Nothing is cleared and no device data is read: every slot's frames restart on the device."""
+        in the order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames); the
+        other slots go on.  Neither form clears a window or the LSTM state, and neither reads device data."""
         if slots is not None:
             self._reset_slots(slots, lengths, start_row)
             return
@@ -1052,17 +1015,13 @@ class PostNetStreamer:
                 if lengths.shape != (self.batch,):
                     raise ValueError(f"reset: expected ({self.batch},) lengths, got {tuple(lengths.shape)}")
                 self._len.copy_(lengths)
-            self._win.reset()
-            self._state.zero_()
             self._row.zero_()
         self._rows = 0
 
     def _reset_slots(self, slots, lengths, start_row):
-        slots, start_row = [int(s) for s in slots], int(start_row)
         if not self.per_slot:
             raise ValueError("reset: slots are for a per-slot streamer (PostNet.streamer(..., per_slot=True))")
-        if len(set(slots)) != len(slots) or any(not 0 <= s < self.batch for s in slots):
-            raise ValueError(f"reset: slots must be distinct and lie in [0, {self.batch}), got {slots}")
+        slots, start_row = check_slots(slots, self.batch), int(start_row)
         lengths = [int(n) for n in lengths]
         if len(lengths) != len(slots) or any(n < 1 for n in lengths):
             raise ValueError(f"reset: expected {len(slots)} lengths >= 1, got {lengths}")

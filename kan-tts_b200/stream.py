@@ -68,12 +68,11 @@ class Windows:
         self.buf[name][:, h:h + f].copy_(x if f_axis == 1 else x.transpose(1, 2))
         return f
 
-    def place(self, src, dst, resid=None, in_offset=0, res_lag=0):
-        """-> the KtStreamWin of a layer reading ``src`` from ``in_offset`` rows into its chunk, writing the chunk of
-        ``dst`` and adding the rows of ``resid`` that lie ``res_lag`` rows before its chunk."""
+    def place(self, src, dst, resid=None, res_lag=0):
+        """-> the KtStreamWin of a layer reading the chunk of ``src``, writing the chunk of ``dst`` and adding the rows of
+        ``resid`` that lie ``res_lag`` rows before its chunk."""
         b, first = self.buf, self.first
-        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=first[src] + in_offset, out_pitch=b[dst].shape[1],
-                        out_first=first[dst])
+        w = KtStreamWin(in_pitch=b[src].shape[1], in_first=first[src], out_pitch=b[dst].shape[1], out_first=first[dst])
         if resid is not None:
             w.res_pitch, w.res_first = b[resid].shape[1], first[resid] - res_lag
         return w
@@ -87,14 +86,19 @@ class Windows:
         """The history of the given slots (None: all) returns to zeros in every window (one launch)."""
         sel = self._all
         if slots is not None:
-            slots = sorted({int(s) for s in slots})
-            if any(not 0 <= s < self.batch for s in slots):
-                raise ValueError(f"reset: slots must lie in [0, {self.batch}), got {slots}")
             mask = torch.zeros(self.batch, dtype=torch.uint8)
-            mask[slots] = 1
+            mask[check_slots(slots, self.batch)] = 1
             sel = to_device(mask, self.device)
         if self._ntable:
             ops.call("kt_stream_reset", ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c)
+
+
+def check_slots(slots, batch):
+    """-> ``slots`` as a list of ints; ValueError unless they are distinct and lie in [0, batch)."""
+    slots = [int(s) for s in slots]
+    if len(set(slots)) != len(slots) or any(not 0 <= s < batch for s in slots):
+        raise ValueError(f"reset: slots must be distinct and lie in [0, {batch}), got {slots}")
+    return slots
 
 
 def to_device(t, device):

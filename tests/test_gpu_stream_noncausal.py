@@ -1,7 +1,7 @@
 """Streaming a non-causal generator on the GPU (Generator.streamer with lengths): each slot's delayed chunks, cut to
 [delay, delay + length * hop), equal the batch-1 forward on the slot's mel of exactly its length, for any chunk schedule and
-ragged lengths; a slot reset after draining starts an exact new utterance without touching the others; graph-replayed
-chunks equal eager ones bit for bit; push and finish never synchronise the host."""
+ragged lengths; a slot reset after draining starts an exact new utterance without touching the others, and a rejected reset
+touches nothing; graph-replayed chunks equal eager ones bit for bit; push and finish never synchronise the host."""
 import pytest
 import torch
 
@@ -106,6 +106,25 @@ def test_reset_after_drain_starts_an_exact_utterance_in_one_slot_only():
     assert float((second[1:2, :, L:L + 9 * hop] - want_u).abs().max()) <= 1e-6
     for b in (0, 2):                                   # drained slots keep streaming silence past their utterance
         assert float(second[b].abs().max()) == 0.0
+
+
+def test_rejected_reset_leaves_the_stream_as_it_was():
+    g, mel = _setup("v1_16k", B=2, T=12)
+    g, mel = g.cuda(), mel.cuda()
+    with torch.no_grad():
+        ops.set_force_ffma(True)
+        try:
+            want, _ = _stream(g, mel, [4, 4, 4], [12, 12])
+            st = g.streamer(batch=2, max_frames=4, lengths=[12, 12])
+            outs = [st.push(mel[:, :, :4])]
+            with pytest.raises(ValueError, match="distinct"):
+                st.reset([0, 0], [12, 12])
+            with pytest.raises(ValueError, match="expected 1 lengths"):
+                st.reset([1], [9, 9])
+            outs += [st.push(mel[:, :, t:t + 4]) for t in (4, 8)] + [st.finish()]
+        finally:
+            ops.set_force_ffma(False)
+    assert torch.equal(torch.cat(outs, -1), want)
 
 
 def test_graph_replay_equals_eager_bitwise():

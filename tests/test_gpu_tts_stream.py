@@ -67,15 +67,23 @@ def test_postnet_streamer_matches_forward(schedule):
 
 def test_postnet_streamer_reset_starts_a_new_batch():
     pn, dec, lengths, mask = _postnet_case()
+    other = torch.randn(dec.shape, generator=torch.Generator().manual_seed(8)).to(DEV)
     with torch.no_grad():
         st = pn.streamer(batch=dec.shape[0], max_frames=6, lengths=lengths)
         first = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
         st.reset(lengths)
         again = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
+        # a batch cut off mid-stream leaves its rows in every window and its LSTM state carried: a reset clears neither
+        st.reset(torch.full_like(lengths, T))
+        for c in torch.split(other[:, :16], 6, 1):
+            st.push(c)
+        st.reset(lengths)
+        after = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
     assert torch.equal(first, again)
+    assert torch.equal(first, after)                  # first: the output of a fresh streamer
 
 
-def test_fsmn_stream_rows_equal_whole_sequence_rows_bitwise():
+def test_fsmn_stream_slots_rows_equal_whole_sequence_rows_bitwise():
     lib = _lib.load()
     B, C, K_, lp = 3, 96, 41, 37
     rp = K_ - 1 - lp
@@ -86,6 +94,7 @@ def test_fsmn_stream_rows_equal_whole_sequence_rows_bitwise():
     lengths = torch.tensor(LENGTHS, device=DEV, dtype=torch.int32)
     mask = (torch.arange(T, device=DEV)[None, :] >= lengths[:, None]).to(torch.uint8)
     y = torch.empty_like(x)
+    frame0 = torch.zeros(B, dtype=torch.int32, device=DEV)
     check(lib.kt_fsmn_fwd(ptr(x), ptr(w), ptr(mask, True), ptr(y), B, T, C, K_, lp, stream_ptr()), "kt_fsmn_fwd")
     # one window holding the whole input after k - 1 history rows (zeros), and rp padding rows at the end; the outputs are
     # frames -rp .. T-1 (the first rp rows are before the utterance)
@@ -97,8 +106,9 @@ def test_fsmn_stream_rows_equal_whole_sequence_rows_bitwise():
         for f in (7, 1, 12, 3, T + rp - 23):
             win = KtStreamWin(in_pitch=xw.shape[1], in_first=K_ - 1 + s, out_pitch=T + rp, out_first=s, res_pitch=T + rp,
                               res_first=s)
-            check(lib.kt_fsmn_fwd_stream(ctypes.byref(win), ptr(xw), ptr(w), ptr(lengths, True), ptr(res), ptr(yw), B, f, C,
-                                         K_, lp, s - rp, stream_ptr()), "kt_fsmn_fwd_stream")
+            check(lib.kt_fsmn_fwd_stream_slots(ctypes.byref(win), ptr(xw), ptr(w), ptr(lengths, True), ptr(frame0, True),
+                                               s - rp, ptr(res), ptr(yw), B, f, C, K_, lp, stream_ptr()),
+                  "kt_fsmn_fwd_stream_slots")
             s += f
         assert s == T + rp
         want = y if res is None else y + resid
@@ -107,7 +117,7 @@ def test_fsmn_stream_rows_equal_whole_sequence_rows_bitwise():
 
 
 @pytest.mark.parametrize("H", [128, 40])
-def test_lstm_stream_carries_state_across_uneven_chunks(H):
+def test_lstm_stream_slots_carries_state_across_uneven_chunks(H):
     lib = _lib.load()
     B, L, D = 3, 37, 64
     torch.manual_seed(11)
@@ -119,10 +129,11 @@ def test_lstm_stream_carries_state_across_uneven_chunks(H):
     whh_t = lstm.weight_hh_l0.detach().t().contiguous().to(DEV)
     state = torch.zeros(B, 2, H, device=DEV)
     h = torch.empty(B, L, H, device=DEV)
+    frame0 = torch.zeros(B, dtype=torch.int32, device=DEV)
     t0 = 0
     for f in (5, 1, 13, 2, 16):
-        check(lib.kt_lstm_stream(ptr(gx) + 4 * t0 * 4 * H, ptr(whh_t), ptr(state), ptr(h) + 4 * t0 * H, B, f, H, L, L,
-                                 stream_ptr()), "kt_lstm_stream")
+        check(lib.kt_lstm_stream_slots(ptr(gx) + 4 * t0 * 4 * H, ptr(whh_t), ptr(state), ptr(h) + 4 * t0 * H,
+                                       ptr(frame0, True), t0, B, f, H, L, L, stream_ptr()), "kt_lstm_stream_slots")
         t0 += f
     assert t0 == L
     err = rel_l2(h.cpu(), want)
