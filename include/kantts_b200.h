@@ -532,6 +532,43 @@ int kt_se_gate_apply(const float* y, const float* stats, const float* w1, const 
                      int32_t c_mid, int32_t c_out, int32_t seg, void* stream);
 int kt_se_stats_pool(const float* x, const int32_t* lengths, float* out, int32_t batch, int32_t t, int32_t c, void* stream);
 
+/* Masked-symbol pretraining of the text encoder (KanTtsTextsyBERT, sybert.yaml; csrc/bert.cu).
+ * kt_seq_ce_fwd: SeqCELoss (kantts/train/loss.py:444-460) of logits [rows][v] (any v >= 1), int64 targets [rows] and float
+ * masks [rows], one warp per row:
+ *   lse[r]  = log sum_j exp(logits[r][j])                       (online max / sum in fp32, written for the backward)
+ *   arg[r]  = the first j with the row's largest logit          (torch.argmax's rule on ties)
+ *   loss[0] = sum_r (lse[r] - logits[r][t_r]) m_r / M,  err[0] = sum_r [arg[r] != t_r] m_r / M,  mask_sum[0] = M = sum_r m_r
+ *                                                               (float32; device scalars)
+ * The sums run in float64: per-CTA partials in `workspace` (kt_seq_ce_workspace_bytes(rows)), then one reducing warp; the
+ * grid depends on `rows` only, so two calls give bit-identical scalars.  M == 0 gives NaN loss and error, as the reference
+ * does; a target outside [0, v) gives a NaN loss.  Two launches, no host read.
+ * kt_seq_ce_bwd: dlogits[r][j] = (d_loss[0] / M) m_r (exp(logits[r][j] - lse[r]) - [j == t_r]), with d_loss (device [1])
+ * and M = mask_sum[0] read on the device.
+ *
+ * kt_bert_mask: BERT_Text_Dataset.bert_masking (kantts/datasets/dataset.py:873-920, 1022-1040) of a batch, one CTA per
+ * utterance.  lings [batch][length][n_feat] int64 with the symbol id in feature 0; valid_lengths [batch] int32 (the
+ * collate's valid_input_lengths: positions from valid_lengths[b] on, the trailing eos and the padding, are never selected).
+ * With key (k0, k1) = (seed low word, seed high word), (c2, c3) = (call low word, call high word) and
+ * (w0..w3) = Philox4x32-10(counter (i, b, c2, c3), key) for position i of utterance b:
+ *   selected    i < valid_lengths[b] and w0 < threshold;  threshold = ceil(mask_ratio 2^32) makes this w0 2^-32 < mask_ratio
+ *               exactly, the float64 compare of the reference's uniform draw
+ *   rank        the position of (w1 2^32 + w2, i) in ascending order among the n selected positions of the utterance
+ *   n_mask = floor(n * 0.8), n_rand = floor(n * 0.1)                     (float64, as math.floor in Python)
+ *   out symbol  mask_id when rank < n_mask; the utterance's replacement id when n_mask <= rank < n_mask + n_rand;
+ *               otherwise the symbol itself
+ *   replacement (w0' n_sy) >> 32 (an id in [0, n_sy - 1]), (w0'..w3') = Philox4x32-10(counter (0xFFFFFFFF, b, c2, c3), key)
+ * Writes out_lings (lings with feature 0 masked), targets [batch][length] (feature 0 unmasked) and bert_masks
+ * [batch][length] (1.0 at the selected positions, else 0.0).  length * 9 bytes of shared memory (length <= 22755).  One
+ * launch. */
+int64_t kt_seq_ce_workspace_bytes(int32_t rows);
+int kt_seq_ce_fwd(const float* logits, const int64_t* targets, const float* masks, float* lse, float* loss, float* err,
+                  float* mask_sum, void* workspace, int64_t workspace_bytes, int32_t rows, int32_t v, void* stream);
+int kt_seq_ce_bwd(const float* logits, const int64_t* targets, const float* masks, const float* lse, const float* mask_sum,
+                  const float* d_loss, float* dlogits, int32_t rows, int32_t v, void* stream);
+int kt_bert_mask(const int64_t* lings, const int32_t* valid_lengths, int64_t* out_lings, int64_t* targets, float* bert_masks,
+                 int32_t batch, int32_t length, int32_t n_feat, int64_t seed, int64_t call, int64_t threshold, int32_t n_sy,
+                 int32_t mask_id, void* stream);
+
 /* Test aid (no GPU needed): the plan kt_conv1d_bwd_weight_tc would make for this layer on a GPU box.
  * out12 = {supported, TMA variant, time steps per chunk, rows per chunk, padded rows, ring stages, shared-memory bytes,
  * split-K factor, N tile, unit groups, time steps per A box, rows of one A image}. */

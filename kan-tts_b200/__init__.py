@@ -7,6 +7,7 @@ Public surface = the reference's own module API for this path:
   train.GanStep (GAN_Trainer.train_step + the data-parallel gradient exchange)
   sambert.KanTtsSAMBERT + MelReconLoss / ProsodyReconLoss                  (kantts.models.sambert, kantts.train.loss)
   train.SambertStep (Sambert_Trainer.train_step)
+  sambert.KanTtsTextsyBERT + SeqCELoss, train.SybertStep, data.BertMasker (sybert.yaml: masked-symbol pretraining)
   infer.synthesize (symbols -> SAM-BERT free-running decode -> HiFi-GAN -> waveforms, no .npy hand-off)
   infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs, causal generators)
   infer.TtsServer (continuous batching: requests join and leave the slots of one running stream)
@@ -18,12 +19,14 @@ from . import _lib  # noqa: F401
 from ._lib import build_library  # noqa: F401
 from . import ops, hifigan, audio, loss, sambert_ops, sambert, train, infer, speaker, install as _install  # noqa: F401
 from .sambert import (KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss, AttentionCTCLoss,  # noqa: F401
-                      AttentionBinarizationLoss, ConvAttention)
+                      AttentionBinarizationLoss, ConvAttention, KanTtsTextsyBERT, SeqCELoss)
 from .hifigan import Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator  # noqa: F401
 from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401
                    DiscriminatorAdversarialLoss, FeatureMatchLoss, criterion_builder)
-from .train import GanStep, SambertStep, hifigan_model_builder, sambert_model_builder  # noqa: F401
+from .train import (GanStep, SambertStep, SybertStep, hifigan_model_builder, sambert_model_builder,  # noqa: F401
+                    sybert_model_builder)
+from .data import BertMasker  # noqa: F401
 from .infer import synthesize, stream_synthesize, TtsServer, slot_schedule  # noqa: F401
 from .speaker import DTDNN, kaldi_fbank, speaker_embedding  # noqa: F401
 
@@ -73,6 +76,16 @@ def sambert_se_nsf_global_16k_config():
     cfg = {k: v for k, v in sambert_24k_config().items() if k != "speaker"}
     return dict(cfg, speaker_units=192, num_mels=82, NSF=True, nsf_norm_type="global", nsf_f0_global_minimum=30.0,
                 nsf_f0_global_maximum=730.0, SE=True)
+
+
+def sybert_config():
+    """``Model.KanTtsTextsyBERT.params`` of kantts/configs/sybert.yaml plus the PinYin unit sizes the trainer injects
+    (bin/train_sybert.py:129-131), as sambert_24k_config.  The sy table ends with pad, eos and the mask symbol, so the mask
+    id is ``sy - 1``."""
+    return dict(
+        max_len=800, embedding_dim=512, encoder_num_layers=8, encoder_num_heads=8, encoder_num_units=128,
+        encoder_ffn_inner_dim=1024, encoder_dropout=0.1, encoder_attention_dropout=0.1, encoder_relu_dropout=0.1,
+        encoder_projection_units=32, mask_ratio=0.3, sy=147, tone=10, syllable_flag=8, word_segment=8)
 
 
 install = _install.install

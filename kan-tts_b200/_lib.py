@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libkantts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu"]
+SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu", "bert.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
@@ -142,6 +142,10 @@ PROTOTYPES = {
     "kt_se_gate_stats": [_P, _P, _P, _I, _I, _I, _I, _P],
     "kt_se_gate_apply": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
     "kt_se_stats_pool": [_P, _P, _P, _I, _I, _I, _P],
+    "kt_seq_ce_workspace_bytes": [_I],
+    "kt_seq_ce_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _P],
+    "kt_seq_ce_bwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _P],
+    "kt_bert_mask": [_P, _P, _P, _P, _P, _I, _I, _I, _L, _L, _L, _I, _I, _P],
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_debug_conv_tc_epilogue": [ctypes.POINTER(KtConv1dDesc), _I],

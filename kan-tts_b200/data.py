@@ -121,3 +121,37 @@ class GpuVocBatcher:
             mel = (mel - self.mel_mean) / self.mel_std
         mel = torch.where((fidx < self.valid_mel_t[ii][:, None])[:, None, :], mel, torch.zeros((), device=self.device))
         return wav, mel.contiguous()
+
+
+class BertMasker:
+    """The BERT masking of the syBERT data path (``BERT_Text_Dataset.bert_masking`` / ``MaskingActor``,
+    kantts/datasets/dataset.py:873-920, and the mask / target columns of its ``collate_fn``, 1022-1100) on the device.
+
+    ``masker(batch)`` takes a batch with the UNMASKED ``input_lings`` (B, L, 4) and ``valid_input_lengths`` (B,) already on
+    the device and returns a new dict with the reference collate's keys: ``input_lings`` with the sy column masked,
+    ``targets`` (the unmasked sy column, (B, L) int64, padded with whatever pads ``input_lings``: the sy pad id, as the
+    collate pads it) and ``bert_masks`` ((B, L) float, 1 at the selected positions), plus the input's other entries.  One
+    kt_bert_mask launch per call and no host synchronisation.
+
+    The rule of the reference, kept exactly: each position before ``valid_input_lengths`` (never the trailing eos nor the
+    padding) is selected with probability ``mask_ratio``; of the n selected, a uniformly random floor(n * 0.8) become
+    ``mask_id``, the next floor(n * 0.1) become ONE id drawn per utterance from [0, n_sy - 1], and the rest keep their
+    symbol.  The draws come from Philox4x32-10 keyed by ``seed`` with a counter of (call index, utterance, position), as
+    include/kantts_b200.h (kt_bert_mask) defines; they replace numpy's and Python's RNG of the dataset workers, so the masks
+    follow the reference's distribution, not its samples.  ``call_index`` advances by one per call and may be set (to
+    resume a run where it stopped)."""
+
+    def __init__(self, mask_ratio, n_sy, seed, mask_id=None):
+        self.mask_ratio = float(mask_ratio)
+        self.n_sy = int(n_sy)
+        # the sy table ends with [pad "_", eos "~", mask "@[MASK]"] (kantts/utils/ling_unit/ling_unit.py:130)
+        self.mask_id = self.n_sy - 1 if mask_id is None else int(mask_id)
+        self.seed = int(seed)
+        self.call_index = 0
+
+    def __call__(self, batch):
+        from .sambert_ops import bert_mask
+        lings, targets, masks = bert_mask(batch["input_lings"], batch["valid_input_lengths"], self.seed, self.call_index,
+                                          self.mask_ratio, self.n_sy, self.mask_id)
+        self.call_index += 1
+        return dict(batch, input_lings=lings, targets=targets, bert_masks=masks)

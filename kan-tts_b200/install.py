@@ -1,7 +1,8 @@
 """Patch the H100-native classes into an importable KAN-TTS checkout so that its unchanged
 ``kantts/bin/train_hifigan.py`` / ``kantts.train.trainer.GAN_Trainer`` run on them
 (see INTEGRATION.md).  ``model_builder`` looks classes up by name in ``kantts.models``' globals
-(kantts/models/__init__.py:38,51) and ``criterion_builder`` in ``loss_dict`` (loss.py:512-544).  The speaker-embedding
+(kantts/models/__init__.py:38,51,131) and ``criterion_builder`` in ``loss_dict`` (loss.py:512-544): the syBERT builder
+finds ``KanTtsTextsyBERT`` there and its SeqCELoss arrives through ``loss_dict``.  The speaker-embedding
 processor (kantts/preprocess/se_processor/se_processor.py) builds its model as ``DTDNN()`` from its module globals, so
 replacing that name runs the unchanged ``SpeakerEmbeddingProcessor`` on speaker.DTDNN."""
 import sys
@@ -11,7 +12,7 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
     """``kantts_se``: the speaker-embedding processor module to patch; by default
     kantts.preprocess.se_processor.se_processor when it is already imported.  It is never imported here: it needs
     torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want."""
-    from . import audio, hifigan, loss, speaker
+    from . import audio, hifigan, loss, sambert, speaker
     if kantts_models is None:
         import kantts.models as kantts_models
     if kantts_loss is None:
@@ -22,6 +23,7 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
         setattr(kantts_models, name, getattr(hifigan, name))
         if hasattr(kantts_models, "hifigan") and hasattr(kantts_models.hifigan, "hifigan"):
             setattr(kantts_models.hifigan.hifigan, name, getattr(hifigan, name))
+    kantts_models.KanTtsTextsyBERT = sambert.KanTtsTextsyBERT
     for key, cls in loss.loss_dict.items():
         kantts_loss.loss_dict[key] = cls
         setattr(kantts_loss, cls.__name__, cls)

@@ -11,7 +11,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .audio import MelSpectrogram, stft
-from .sambert import AttentionBinarizationLoss, AttentionCTCLoss, FpCELoss
+from .sambert import AttentionBinarizationLoss, AttentionCTCLoss, FpCELoss, SeqCELoss
 
 
 def _as_list(outputs):
@@ -234,6 +234,7 @@ loss_dict = {
     "FpCELoss": FpCELoss,
     "AttentionCTCLoss": AttentionCTCLoss,
     "AttentionBinarizationLoss": AttentionBinarizationLoss,
+    "SeqCELoss": SeqCELoss,
 }
 
 

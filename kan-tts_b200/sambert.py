@@ -23,8 +23,9 @@ ConvAttention's projections on the conv kernels, its distance attention fused in
 T_text) difference tensor), monotonic alignment search on the GPU (kt_mas, no host copy) and the forward-sum loss in
 kt_attn_ctc_*.  The speaker-embedding variant (``SE: True``, sambert_se_nsf_global_16k.yaml) is built: it has no speaker
 table, and ``inputs_speaker`` is the float (B, L, speaker_units) per-symbol embedding (speaker.speaker_embedding) in
-place of the ids.  Not built: MAS together with FP (the reference's two branches do not compose: its MAS durations have
-one entry per symbol before the pause splice), and SE together with FP or MAS.
+place of the ids.  The masked-symbol pretraining model of sybert.yaml (KanTtsTextsyBERT) is built on the same text
+encoder, with its loss (SeqCELoss) fused in kt_seq_ce_*.  Not built: MAS together with FP (the reference's two branches
+do not compose: its MAS durations have one entry per symbol before the pause splice), and SE together with FP or MAS.
 """
 import ctypes
 from collections import namedtuple
@@ -1367,3 +1368,43 @@ class AttentionBinarizationLoss(nn.Module):
         else:
             warmup_ratio = min(1.0, (epoch - self.start_epoch) / self.warmup_epoch)
         return kl_loss * warmup_ratio
+
+
+class KanTtsTextsyBERT(nn.Module):
+    """kantts_sambert.py:1047-1068: the masked-symbol pretraining model of sybert.yaml, TextFftEncoder without its output
+    projection followed by a Linear onto the ``sy`` vocabulary.  ``ling_proj`` is constructed and then deleted, as the
+    reference does: its initialiser consumes the torch RNG, so a seeded init equals the reference's, and the state_dict is
+    ``text_encoder.*`` (no ``ling_proj``) then ``fc.*``.  ``fc`` runs on the conv kernels like every other Linear.
+
+    ``forward(inputs_ling, input_lengths)`` -> {"logits": (B, L, sy), "enc_slf_attn_lst": one attention map per encoder
+    layer, in the reference's layout}.  The reference's forward unpacks two of TextFftEncoder's three results and raises
+    ValueError; this one returns what it evidently means to.  Byte input (``using_byte``) is not built: the reference's
+    ``fc`` needs ``config["sy"]``, so it cannot build a byte model either."""
+
+    def __init__(self, config):
+        super().__init__()
+        if config.get("using_byte", False):
+            raise NotImplementedError("KanTtsTextsyBERT: byte input (using_byte) is not built; the output layer is sized by "
+                                      "the PinYin 'sy' vocabulary")
+        self.text_encoder = TextFftEncoder(config)
+        delattr(self.text_encoder, "ling_proj")
+        self.fc = Linear(self.text_encoder.d_model, config["sy"])
+
+    def forward(self, inputs_ling, input_lengths):
+        input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
+        text_hid, enc_slf_attn_lst, _ = self.text_encoder(inputs_ling, input_masks, return_attns=True)
+        return {"logits": self.fc(text_hid), "enc_slf_attn_lst": enc_slf_attn_lst}
+
+
+class SeqCELoss(nn.Module):
+    """train/loss.py:444-460: ``(loss, err)`` of ``logits`` (..., V), int64 ``targets`` and ``masks`` (float, bool or int):
+    the masked mean cross-entropy and the masked argmax error rate.  Both come from one kt_seq_ce_fwd pass over the logits
+    (instead of a log-softmax, a gather, an argmax and two masked reductions); the gradient of ``loss`` is kt_seq_ce_bwd and
+    ``err`` has none.  An all-zero mask gives NaN, as the reference's 0 / 0 does."""
+
+    def __init__(self, loss_type="ce"):
+        super().__init__()
+        self.loss_type = loss_type
+
+    def forward(self, logits, targets, masks):
+        return sops.SeqCEFn.apply(logits, targets, masks)

@@ -2,6 +2,7 @@
 FSMN memory block, LengthRegulator gather, filled-pause insertion).  Same contract as ops.py: CUDA fp32 tensors only, explicit
 stream, RuntimeError on any failure -- no PyTorch / CPU fallback."""
 import ctypes
+import math
 
 import torch
 
@@ -414,3 +415,65 @@ def average_frame_feat(feat, durs):
     total = (torch.gather(sums, 1, ends) - torch.gather(sums, 1, starts)).float()
     count = (torch.gather(nonzero, 1, ends) - torch.gather(nonzero, 1, starts)).float()
     return torch.where(count == 0.0, count, total / count)
+
+
+# masked-symbol pretraining (KanTtsTextsyBERT): kt_seq_ce_*, kt_bert_mask
+# ------------------------------------------------------------------------------------------------
+
+
+class SeqCEFn(torch.autograd.Function):
+    """SeqCELoss.forward (train/loss.py:444-460): logits (..., V), int64 targets (...) and float masks (...) -> the masked
+    mean cross-entropy ``loss`` and the masked argmax error rate ``err``, both 0-d device tensors.  One pass over the logits
+    in kt_seq_ce_fwd (log-sum-exp, target logit, argmax with torch's first-index rule, fixed-order masked sums); ``err`` is
+    not differentiable.  The backward is kt_seq_ce_bwd, with the incoming gradient and the mask sum read on the device."""
+
+    @staticmethod
+    def forward(ctx, logits, targets, masks):
+        V = logits.shape[-1]
+        x = logits.reshape(-1, V).contiguous()
+        rows = x.shape[0]
+        t = targets.reshape(-1).to(torch.int64).contiguous()
+        m = masks.reshape(-1).to(torch.float32).contiguous()
+        assert t.numel() == rows and m.numel() == rows, (logits.shape, targets.shape, masks.shape)
+        dev = x.device
+        lse = torch.empty(rows, device=dev, dtype=torch.float32)
+        loss, err, msum = (torch.empty((), device=dev, dtype=torch.float32) for _ in range(3))
+        n = int(_lib.load().kt_seq_ce_workspace_bytes(rows))
+        ws = torch.empty(n // 8, device=dev, dtype=torch.float64)
+        call("kt_seq_ce_fwd", ptr(x), ptr(t, True), ptr(m), ptr(lse), ptr(loss), ptr(err), ptr(msum), ptr(ws, True), n,
+             rows, V, launches=2)
+        ctx.save_for_backward(x, t, m, lse, msum)
+        ctx.shape = logits.shape
+        ctx.mark_non_differentiable(err)
+        return loss, err
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_err):
+        x, t, m, lse, msum = ctx.saved_tensors
+        dx = torch.empty_like(x)
+        d_loss = d_loss.to(torch.float32).contiguous()
+        call("kt_seq_ce_bwd", ptr(x), ptr(t, True), ptr(m), ptr(lse), ptr(msum), ptr(d_loss), ptr(dx),
+             x.shape[0], x.shape[1])
+        return dx.view(ctx.shape), None, None
+
+
+def bert_mask(lings, valid_lengths, seed, call_index, mask_ratio, n_sy, mask_id):
+    """BERT masking of the symbol column of ``lings`` (B, L, n_feat) int64 on the device (kt_bert_mask), positions
+    [0, valid_lengths[b]) eligible.  -> (masked lings, targets = the unmasked symbol column (B, L) int64, bert_masks (B, L)
+    float32 with 1 at the selected positions).  ``seed`` and ``call_index`` (host ints) key the draw."""
+    x = lings.to(torch.int64).contiguous()
+    B, L, F = x.shape
+    vl = _i32(valid_lengths)
+    out = torch.empty_like(x)
+    targets = torch.empty(B, L, device=x.device, dtype=torch.int64)
+    masks = torch.empty(B, L, device=x.device, dtype=torch.float32)
+    threshold = math.ceil(float(mask_ratio) * 2.0 ** 32)
+    call("kt_bert_mask", ptr(x, True), ptr(vl, True), ptr(out, True), ptr(targets, True), ptr(masks), B, L, F,
+         _wrap64(seed), _wrap64(call_index), threshold, int(n_sy), int(mask_id))
+    return out, targets, masks
+
+
+def _wrap64(v):
+    """A Python int as the int64 whose bits are its low 64 bits (seeds and call counters are unsigned 64-bit words)."""
+    v = int(v) & 0xFFFFFFFFFFFFFFFF
+    return v - (1 << 64) if v >= 1 << 63 else v

@@ -380,6 +380,20 @@ class NoamLR(torch.optim.lr_scheduler.LRScheduler):
         return [base_lr * scale for base_lr in self.base_lrs]
 
 
+def apply_gradients(loss_total, grads, optimizer, scheduler, grad_clip):
+    """The tail of the SAM-BERT and syBERT train steps (Sambert_Trainer.train_step, Textsy_BERT_Trainer.train_step in
+    kantts/train/trainer.py) after the loss: zero the flat gradient buffer, backward, the data-parallel all-reduce (mean)
+    of that buffer, gradient-norm clipping (``grad_clip`` None: none), the optimizer and the scheduler step."""
+    grads.zero()
+    loss_total.backward()
+    ops.join_wgrad_streams(loss_total.device if loss_total.is_cuda else None)
+    grads.all_reduce_mean()
+    if grad_clip is not None:
+        torch.nn.utils.clip_grad_norm_(grads.params, grad_clip)
+    optimizer.step()
+    scheduler.step()
+
+
 class SambertStep:
     """``Sambert_Trainer.train_step`` (kantts/train/trainer.py:898-1005): teacher-forced forward, MelReconLoss +
     ProsodyReconLoss, backward, gradient-norm clipping, Adam, NoamLR.  Data parallel: the batch is sharded by
@@ -426,14 +440,7 @@ class SambertStep:
                                                                batch["valid_output_lengths"])
             attn_kl_loss = self.criterion["AttentionBinarizationLoss"](self.epoch, res["attn_hard"], res["attn_soft"])
             loss_total = loss_total + attn_ctc_loss + attn_kl_loss
-        self.grads.zero()
-        loss_total.backward()
-        ops.join_wgrad_streams(loss_total.device if loss_total.is_cuda else None)
-        self.grads.all_reduce_mean()
-        if self.grad_clip is not None:
-            torch.nn.utils.clip_grad_norm_(self.grads.params, self.grad_clip)
-        self.optimizer.step()
-        self.scheduler.step()
+        apply_gradients(loss_total, self.grads, self.optimizer, self.scheduler, self.grad_clip)
         self.steps += 1
         out = {"TotalLoss": loss_total.detach(), "mel_loss_": mel_loss_.detach(), "mel_loss": mel_loss.detach(),
                "dur_loss": dur_loss.detach(), "pitch_loss": pitch_loss.detach(),
@@ -455,9 +462,52 @@ def sambert_model_builder(config, device, fp_dict=None):
     model = sambert.KanTtsSAMBERT(sect["params"]).to(device)
     if fp_dict is not None:
         model.fp_dict = {k: v.to(device) for k, v in fp_dict.items()}
+    return (model,) + _optimizer_and_scheduler(model, sect)
+
+
+def _optimizer_and_scheduler(model, sect):
+    """The optimizer and scheduler of one ``Model.<name>`` yaml section (kantts/models/__init__.py:107-116, 134-143):
+    NoamLR is this module's, any other scheduler torch's."""
     opt = optimizer_builder(model.parameters(), sect["optimizer"].get("type", "Adam"),
                             dict(sect["optimizer"].get("params", {})))
     sch_t = sect["scheduler"].get("type", "NoamLR")
     sch_p = sect["scheduler"].get("params", {})
     sch = NoamLR(opt, **sch_p) if sch_t == "NoamLR" else getattr(torch.optim.lr_scheduler, sch_t)(opt, **sch_p)
-    return model, opt, sch
+    return opt, sch
+
+
+# ------------------------------------------------------------------------------------------------
+# syBERT
+# ------------------------------------------------------------------------------------------------
+
+
+class SybertStep:
+    """``Textsy_BERT_Trainer.train_step`` (kantts/train/trainer.py:1155-1185): the KanTtsTextsyBERT forward, SeqCELoss over
+    the masked positions, ``loss / V`` as the reference divides by the vocabulary size, then the SAM-BERT step's tail
+    (``apply_gradients``: backward, the flat-gradient all-reduce that replaces DistributedDataParallel, the clip, Adam,
+    NoamLR).  ``step(batch)`` takes the collate's keys (input_lings, valid_input_lengths, targets, bert_masks) on the
+    model's device -- ``data.BertMasker`` makes them there -- and returns device tensors {"TotalLoss", "Error"}."""
+
+    def __init__(self, model, optimizer, scheduler, criterion, grad_clip=1.0):
+        self.model, self.optimizer, self.scheduler, self.criterion = model, optimizer, scheduler, criterion
+        self.grad_clip = grad_clip
+        self.grads = FlatGrads(model)
+        self.steps = 0
+
+    def step(self, batch):
+        res = self.model(batch["input_lings"], batch["valid_input_lengths"])
+        logits = res["logits"]
+        loss, err = self.criterion["SeqCELoss"](logits, batch["targets"], batch["bert_masks"])
+        loss_total = loss / logits.size(-1)
+        apply_gradients(loss_total, self.grads, self.optimizer, self.scheduler, self.grad_clip)
+        self.steps += 1
+        return {"TotalLoss": loss_total.detach(), "Error": err}
+
+
+def sybert_model_builder(config, device):
+    """kantts/models/__init__.py:126-150 without the DDP wrapper: ``config`` is the whole sybert.yaml dict with the
+    linguistic-unit sizes merged into ``Model.KanTtsTextsyBERT.params`` (bin/train_sybert.py:129-131)."""
+    from . import sambert
+    sect = config["Model"]["KanTtsTextsyBERT"]
+    model = sambert.KanTtsTextsyBERT(sect["params"]).to(device)
+    return (model,) + _optimizer_and_scheduler(model, sect)
