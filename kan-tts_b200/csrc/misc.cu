@@ -13,9 +13,15 @@ static inline int stream_grid(long long n_items, int threads) {
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
+// float4 loads only when every pointer is 16-byte aligned (a contiguous view may start at any float): else all scalar
+__device__ __forceinline__ bool aligned16(const void* a, const void* b = nullptr, const void* c = nullptr, const void* d = nullptr) {
+  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
+           reinterpret_cast<uintptr_t>(d)) & 15) == 0;
+}
+
 // hifigan.py:157  x = torch.sin(x) + x
 __global__ void sinadd_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
-  const long long n4 = n / 4;
+  const long long n4 = aligned16(x, y) ? n / 4 : 0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
     v.x += sinf(v.x); v.y += sinf(v.y); v.z += sinf(v.z); v.w += sinf(v.w);
@@ -26,7 +32,7 @@ __global__ void sinadd_fwd_kernel(const float* __restrict__ x, float* __restrict
 }
 
 __global__ void sinadd_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx, long long n) {
-  const long long n4 = n / 4;
+  const long long n4 = aligned16(x, dy, dx) ? n / 4 : 0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
     float4 g = __ldg(reinterpret_cast<const float4*>(dy) + i);
@@ -40,7 +46,7 @@ __global__ void sinadd_bwd_kernel(const float* __restrict__ x, const float* __re
 // hifigan.py:170-176  x = (r0 + r1 + r2) / num_kernels
 __global__ void add3_scale_kernel(const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ c,
                                   float scale, float* __restrict__ y, long long n) {
-  const long long n4 = n / 4;
+  const long long n4 = aligned16(a, b, c, y) ? n / 4 : 0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = __ldg(reinterpret_cast<const float4*>(a) + i);
     if (b) { const float4 t = __ldg(reinterpret_cast<const float4*>(b) + i); v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w; }
@@ -81,6 +87,8 @@ extern "C" int kt_upsample_grad_reduce(const float* dxu, const float* x, int32_t
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(dxu && dx && rows > 0 && up >= 1 && c > 0 && (c & 3) == 0, "upsample_grad_reduce: bad arguments (C %% 4 == 0 required)");
   KT_REQUIRE(act == KT_ACT_NONE || (act == KT_ACT_LRELU && x), "upsample_grad_reduce: act must be NONE or LRELU (with x)");
+  KT_REQUIRE(((reinterpret_cast<uintptr_t>(dxu) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0,
+             "upsample_grad_reduce: dxu, x and dx must be 16-byte aligned (float4 rows)");
   upsample_grad_reduce_kernel<<<stream_grid(rows * (c / 4), 256), 256, 0, st>>>(dxu, x, act, slope, dx, rows, up, c / 4);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
@@ -362,7 +370,7 @@ extern "C" int kt_dwt_db3_bwd(const float* dy, float* dx, int32_t batch, int32_t
   return KT_OK;
 }
 static int l1_sum(const float* a, const float* b, long long n, float scale, float* out, cudaStream_t st, bool accumulate) {
-  KT_REQUIRE(a && b && out && n >= 0, "l1_sum: bad arguments");
+  KT_REQUIRE(out && n >= 0 && (n == 0 || (a && b)), "l1_sum: bad arguments");   // an empty tensor has no data pointer
   if (n == 0) {
     if (!accumulate) KT_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
     return KT_OK;

@@ -580,7 +580,10 @@ static int attn_check(const KtAttnDesc* d) {
   return KT_OK;
 }
 
-// rows per warp: RW*D per-lane accumulators (<= 64) and a [8*RW][Lk] fp32 score buffer in shared memory
+// rows per warp: RW*D per-lane accumulators (<= 64) and a [8*RW][Lk] fp32 score buffer in shared memory.  d_head 32 keeps
+// RW = 2 up to the Lk <= 2048 limit, so the dispatchers have no <32, 1> arm.
+static_assert(((size_t)8 * 2 * 2048 + (size_t)kKeyTile * (32 + 4)) * sizeof(float) <= (size_t)kMaxDynSmem,
+              "attention: d_head 32 at Lk 2048 no longer fits RW = 2; add a <32, 1> dispatch arm");
 static int attn_rows_per_warp(int d_head, int lk) {
   int rw = d_head <= 16 ? 4 : (d_head == 32 ? 2 : 1);
   while (rw > 1 && ((size_t)8 * rw * lk + (size_t)kKeyTile * (d_head + 4)) * sizeof(float) > (size_t)kMaxDynSmem) rw >>= 1;
@@ -615,7 +618,6 @@ extern "C" int kt_attention_fwd(const KtAttnDesc* d, const float* q, const float
     case 16 * 8 + 4: return attn_fwd_launch<16, 4>(d, a, st);
     case 16 * 8 + 2: return attn_fwd_launch<16, 2>(d, a, st);
     case 32 * 8 + 2: return attn_fwd_launch<32, 2>(d, a, st);
-    case 32 * 8 + 1: return attn_fwd_launch<32, 1>(d, a, st);
     case 64 * 8 + 1: return attn_fwd_launch<64, 1>(d, a, st);
     default: break;
   }
@@ -654,7 +656,6 @@ extern "C" int kt_attention_bwd(const KtAttnDesc* d, const float* q, const float
     case 16 * 8 + 4: return attn_bwd_launch<16, 4>(d, a, st);
     case 16 * 8 + 2: return attn_bwd_launch<16, 2>(d, a, st);
     case 32 * 8 + 2: return attn_bwd_launch<32, 2>(d, a, st);
-    case 32 * 8 + 1: return attn_bwd_launch<32, 1>(d, a, st);
     case 64 * 8 + 1: return attn_bwd_launch<64, 1>(d, a, st);
     default: break;
   }

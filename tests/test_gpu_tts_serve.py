@@ -26,7 +26,7 @@ def _attend(q, k, v):
     return p @ v
 
 
-@pytest.mark.parametrize("d_head", [8, 16])
+@pytest.mark.parametrize("d_head", [8, 16, 32])
 def test_pnca_step_slots_matches_torch(d_head):
     B, H, L = 5, 3, 40
     hd = H * d_head
