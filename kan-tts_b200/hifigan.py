@@ -9,8 +9,10 @@ leaf ``nn.Parameter``s so ``torch.optim.Adam`` / ``DistributedDataParallel`` wor
 Every tensor op of the forward and backward runs in libkantts_b200.so (hand-written sm_90a
 kernels) through ``ops.py``; activations are channels-last rows internally and are converted only
 at the module boundary (feature maps are returned as zero-copy permuted views).
-The NSF branch (``nsf_params``) is module plumbing over the same kernels and has NOT run on a GPU yet (round 1 ran out
-of GPU budget: tests/test_gpu_pipeline.py is opt-in).  Out of scope (SURVEY.md section 8a): MultiSpecDiscriminator, PQMF.
+A multi-band generator (``out_channels`` = S > 1) emits S sub-band signals at 1/S of the sample rate; the PQMF filter bank
+(pqmf.py) turns them into the waveform.  Like the reference, the PQMF is not part of the generator: the model builder adds
+it next to the generator, and inference attaches it as ``generator.pqmf`` after loading.  Out of scope (SURVEY.md
+section 8a): MultiSpecDiscriminator, a multi-band NSF generator and streaming a multi-band generator.
 """
 import copy
 import ctypes
@@ -400,8 +402,8 @@ class Generator(nn.Module):
             raise NotImplementedError("kantts_b200: repeat_upsample=False is not used by any shipped config")
         if nonlinear_activation != "LeakyReLU":
             raise NotImplementedError("kantts_b200: only LeakyReLU is fused into the conv kernels")
-        if out_channels != 1:
-            raise NotImplementedError("kantts_b200: multi-band (PQMF) output is out of scope")
+        if out_channels > 1 and nsf_params is not None:
+            raise NotImplementedError("kantts_b200: a multi-band (PQMF) NSF generator is out of scope")
         slope = nonlinear_activation_params.get("negative_slope", 0.01)
         self.upsample_scales = upsample_scales
         self.repeat_upsample = repeat_upsample
@@ -484,7 +486,7 @@ class Generator(nn.Module):
         return self.conv_post.forward_rows(x)                                # :178-180
 
     def forward(self, x, nsf_seeds=None):
-        """x: (B, in_channels, T) -> (B, 1, T * prod(scales)); with ``nsf_params`` the last two channels are the
+        """x: (B, in_channels, T) -> (B, out_channels, T * prod(scales)); with ``nsf_params`` the last two channels are the
         pitch (Hz) and the voiced flag (hifigan.py:146-150).  ``nsf_seeds`` (NSF only; one per batch item, host sequence
         or device int64 tensor): the excitation is the seeded kt_nsf_excitation instead of the reference's random draw, so
         that the output is a function of (x, seeds) -- the one a streamer with the same seeds computes."""
@@ -595,6 +597,9 @@ class StreamPlan:
       steps               ConvStep | SinStep | MeanStep | ExciteStep records, in launch order"""
 
     def __init__(self, gen):
+        if gen.out_channels > 1:
+            raise ValueError("streaming a multi-band (PQMF) generator is not supported: PQMF synthesis reads 31 samples "
+                             "ahead of every output sample")
         if gen.training:
             raise ValueError("streaming runs a generator in eval() mode")
         self.causal = causal = gen.conv_pre.causal

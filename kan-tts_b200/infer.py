@@ -57,11 +57,16 @@ def _check_nsf(sambert_num_mels, generator, nsf_f0, nsf_seeds, what):
 @torch.no_grad()
 def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None):
     """sambert: ``KanTtsSAMBERT`` in eval(); generator: ``Generator`` in eval() (``remove_weight_norm()`` optional --
-    the prepared weights are cached either way).  Tensors as in ``KanTtsSAMBERT.forward`` (inference branch).
+    the prepared weights are cached either way).  A multi-band generator (``out_channels`` > 1) needs its PQMF attached as
+    ``generator.pqmf`` (as infer_hifigan.py:47-53 does after loading), whose synthesis makes the waveform.  Tensors as in
+    ``KanTtsSAMBERT.forward`` (inference branch).
     ``nsf_f0`` / ``nsf_seeds`` (both or neither): the NSF hand-off, see the module docstring and ``denorm_f0``.
     -> (list of 1-D waveform tensors, dict of the acoustic-model results)."""
     if sambert.training or generator.training:
         raise RuntimeError("synthesize() expects both models in eval() mode")
+    pqmf = getattr(generator, "pqmf", None) if generator.out_channels > 1 else None
+    if generator.out_channels > 1 and pqmf is None:
+        raise ValueError("synthesize(): a multi-band generator needs its PQMF attached as generator.pqmf")
     nsf = _check_nsf(sambert.mel_postnet.num_mels, generator, nsf_f0, nsf_seeds, "synthesize()")
     res = sambert(inputs_ling, inputs_emotion, inputs_speaker, input_lengths)
     mel = res["postnet_outputs"]                                   # (B, T, num_mels), zero beyond each length
@@ -69,8 +74,10 @@ def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, 
     if nsf:
         wav = generator(denorm_f0(mel, nsf_f0).transpose(1, 2).contiguous(), nsf_seeds=nsf_seeds)
     else:
-        wav = generator(mel.transpose(1, 2).contiguous())          # (B, 1, T * hop)
-    hop = int(np.prod(generator.upsample_scales))
+        wav = generator(mel.transpose(1, 2).contiguous())          # (B, out_channels, T * prod(scales))
+    if pqmf is not None:
+        wav = pqmf.synthesis(wav)                                  # (B, 1, T * hop)
+    hop = int(np.prod(generator.upsample_scales)) * generator.out_channels
     wavs = [wav[b, 0, : int(frames[b]) * hop] for b in range(wav.shape[0])]
     return wavs, res
 

@@ -12,7 +12,7 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
     """``kantts_se``: the speaker-embedding processor module to patch; by default
     kantts.preprocess.se_processor.se_processor when it is already imported.  It is never imported here: it needs
     torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want."""
-    from . import audio, hifigan, loss, sambert, speaker
+    from . import audio, hifigan, loss, pqmf, sambert, speaker
     if kantts_models is None:
         import kantts.models as kantts_models
     if kantts_loss is None:
@@ -24,6 +24,9 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
         if hasattr(kantts_models, "hifigan") and hasattr(kantts_models.hifigan, "hifigan"):
             setattr(kantts_models.hifigan.hifigan, name, getattr(hifigan, name))
     kantts_models.KanTtsTextsyBERT = sambert.KanTtsTextsyBERT
+    kantts_models.PQMF = pqmf.PQMF                           # hifigan_model_builder (kantts/models/__init__.py:65-67)
+    if hasattr(kantts_models, "pqmf"):                       # infer_hifigan.py:50-52 imports it from there
+        kantts_models.pqmf.PQMF = pqmf.PQMF
     for key, cls in loss.loss_dict.items():
         kantts_loss.loss_dict[key] = cls
         setattr(kantts_loss, cls.__name__, cls)

@@ -239,7 +239,9 @@ loss_dict = {
 
 
 def criterion_builder(config, device="cpu"):
-    """loss.py:528-544"""
+    """loss.py:528-544.  An enabled ``subband_stft_loss`` is also stored as ``"sub_stft"``, the key GAN_Trainer calls it
+    by (trainer.py:495-498) while it checks for the other: the reference builder leaves that key out, so its trainer
+    raises KeyError on the multi-band yamls."""
     criterion = {}
     for key, value in config["Loss"].items():
         if key in loss_dict:
@@ -248,4 +250,6 @@ def criterion_builder(config, device="cpu"):
                 setattr(criterion[key], "weights", value.get("weights", 1.0))
         else:
             raise NotImplementedError("{} is not implemented".format(key))
+    if "subband_stft_loss" in criterion:
+        criterion["sub_stft"] = criterion["subband_stft_loss"]
     return criterion

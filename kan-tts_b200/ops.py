@@ -786,7 +786,7 @@ class StftMelFn(torch.autograd.Function):
     def forward(ctx, wav, window, melmat, n_fft, hop, pad_mode, eps, norm=(20.0, -100.0, 8.0, 4.0, -4.0, 4.0)):
         wav = wav.contiguous()
         B, T = wav.shape
-        frames = T // hop + 1
+        frames = (T - n_fft % 2) // hop + 1           # torch.stft(center=True): n_fft // 2 samples of padding per side
         nb = n_fft // 2 + 1
         n_mels = 0 if melmat is None else melmat.shape[1]
         d = KtMelDesc(batch=B, t=T, n_fft=n_fft, hop=hop, n_mels=n_mels, frames=frames, pad_mode=pad_mode, eps=eps,

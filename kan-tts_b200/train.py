@@ -3,7 +3,9 @@
 ``GanStep.step`` follows ``GAN_Trainer.train_step`` (KAN-TTS kantts/train/trainer.py:469-589)
 statement for statement -- generator phase (mel + adversarial + feature-matching value), Adam,
 then the discriminator phase on a re-generated ``y_`` -- with two scheduling changes that do not
-alter any result (SURVEY.md section 3.1 / 8e):
+alter any result (SURVEY.md section 3.1 / 8e).  With a PQMF in the model (a multi-band generator) both phases
+synthesise the full band from the generator's sub-bands, and the sub-band STFT loss compares them with the PQMF analysis
+of the real waveform (trainer.py:476-505, 559-562).  The scheduling changes:
   * the discriminators' weight gradients of the GENERATOR phase are never computed nor reduced:
     the reference computes, all-reduces and then zeroes them (trainer.py:577-578);
   * losses are kept as device tensors; ``.item()`` is only called by ``losses_to_float``.
@@ -61,6 +63,8 @@ class GanStep:
 
     def __init__(self, model, optimizer, scheduler, criterion, config, skip_unused_d_grads=True, cuda_graph=False,
                  graph_warmup=3, pair_discriminators=True, reuse_real_half=True):
+        if criterion.get("subband_stft_loss", None) and model.get("pqmf", None) is None:
+            raise ValueError("GanStep: the sub-band STFT loss needs a PQMF in the model (a multi-band generator)")
         self.model, self.optimizer, self.scheduler = model, optimizer, scheduler
         self.criterion, self.config = criterion, config
         self.skip_unused_d_grads = skip_unused_d_grads
@@ -95,11 +99,20 @@ class GanStep:
         pre = self._prefetch(list(model["discriminator"].values()), y) if self._d_active() else None
         y_ = model["generator"](x)
         self._prefetch_join(pre)
+        pqmf = model.get("pqmf", None)
+        if pqmf is not None:                                   # the full band from the sub-bands (trainer.py:476-479)
+            y_mb_ = y_
+            y_ = pqmf.synthesis(y_mb_)
         gen_loss = 0.0
         if crit.get("stft_loss", None):
             sc_loss, mag_loss = crit["stft_loss"](y_, y)
             gen_loss = gen_loss + (sc_loss + mag_loss) * crit["stft_loss"].weights
             log["spectral_convergence_loss"], log["log_stft_magnitude_loss"] = sc_loss, mag_loss
+        if crit.get("subband_stft_loss", None):               # trainer.py:496-507: halves the losses so far, unweighted
+            gen_loss = gen_loss * 0.5
+            sub_sc_loss, sub_mag_loss = crit["subband_stft_loss"](y_mb_, pqmf.analysis(y))
+            gen_loss = gen_loss + 0.5 * (sub_sc_loss + sub_mag_loss)
+            log["sub_spectral_convergence_loss"], log["sub_log_stft_magnitude_loss"] = sub_sc_loss, sub_mag_loss
         if crit.get("mel_loss", None):
             mel_loss = crit["mel_loss"](y_, y)
             gen_loss = gen_loss + mel_loss * crit["mel_loss"].weights
@@ -162,6 +175,8 @@ class GanStep:
             self._prefetch_join(self._prefetch([model["generator"]], y))    # generator weights changed just now
             with torch.no_grad():
                 y_ = model["generator"](x)
+                if model.get("pqmf", None) is not None:          # trainer.py:559-562
+                    y_ = model["pqmf"].synthesis(y_)
             dis_loss = 0.0
             real_t, fake_t = 0.0, 0.0
             for name, disc in model["discriminator"].items():
@@ -330,7 +345,8 @@ def optimizer_builder(model_params, opt_name, opt_params):
 
 def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None):
     """kantts/models/__init__.py:28-86 without the DDP wrappers (GanStep reduces the flat gradient
-    buffers itself); scheduler = torch MultiStepLR as in the shipped yamls.  ``capturable=True`` builds
+    buffers itself); scheduler = torch MultiStepLR as in the shipped yamls.  A multi-band generator
+    (``out_channels`` > 1) gets ``model["pqmf"]``, a PQMF with that many sub-bands and the yaml's ``pqmf`` kwargs.  ``capturable=True`` builds
     the Adam optimizers so that ``GanStep(cuda_graph=True)`` can capture their step.  ``fused_optimizer`` (default: on a
     CUDA device) asks torch for its single-kernel Adam (``fused=True``: the same update and the same ``state_dict`` as the
     reference's foreach Adam, ~4 launches per model instead of ~12 multi-tensor passes; ablation: the three Adam steps
@@ -359,6 +375,10 @@ def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None
             model["generator"], optimizer["generator"], scheduler["generator"] = m, opt, sch
         else:
             model["discriminator"][name], optimizer["discriminator"][name], scheduler["discriminator"][name] = m, opt, sch
+    out_channels = config["Model"]["Generator"]["params"].get("out_channels", 1)
+    if out_channels > 1:
+        from .pqmf import PQMF
+        model["pqmf"] = PQMF(subbands=out_channels, **config.get("pqmf", {})).to(device)
     return model, optimizer, scheduler
 
 
