@@ -316,7 +316,21 @@ int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* row
  * utterance b is log_softmax([blank_logprob, logprob[b][t][:N]]), N = in_lengths[b], T = out_lengths[b]; the CTC loss of
  * the targets 1..N over those frames, divided by N, 0 when infinite (zero_infinity); loss [1] = their mean over the batch.
  * The backward writes all of d_logprob [batch][t_q][t_k] = d_loss[0] * the gradient of loss.  `workspace` holds the alpha
- * recursion and the per-frame normalisers between the two calls: kt_attn_ctc_workspace_bytes. */
+ * recursion and the per-frame normalisers between the two calls: kt_attn_ctc_workspace_bytes.
+ *
+ * kt_attn_prior: the alignment prior of a collate batch, beta_binomial_prior_distribution (kantts/datasets/dataset.py:20-31)
+ * per utterance as AM_Dataset.collate_fn pads it (dataset.py:816-827).  valid_input_lengths / valid_output_lengths
+ * [batch] are the collate's int64 device tensors.  With P = valid_input_lengths[b] + 1 (the symbols with the trailing eos),
+ * M = valid_output_lengths[b], n = P, alpha = t + 1, beta = M - t:
+ *   prior[b][t][k] = exp(lnC(n, k) + lnB(k + alpha, n - k + beta) - lnB(alpha, beta))   for t < M, k < P
+ *                  = 0                                                                  elsewhere
+ * with lnB(x, y) = lgamma(x) + lgamma(y) - lgamma(x + y), lnC the log binomial coefficient: the beta-binomial pmf of k
+ * (support 0..n; k = P is left out, as in the reference).  The exponent is summed in float64 with the device lgamma, every
+ * term that depends on t only, on k only or on t + k only computed once per CTA, and rounded to float32 by
+ * __double2float_rn (subnormals kept).  Writes all of prior [batch][t_mel][t_text]; when M > t_mel or P > t_text only the
+ * elements inside the pad are written, with the values of the true P and M.  One launch, no host read. */
+int kt_attn_prior(const int64_t* valid_input_lengths, const int64_t* valid_output_lengths, float* prior, int32_t batch,
+                  int32_t t_mel, int32_t t_text, void* stream);
 int kt_align_attn_fwd(const float* q, const float* k, const float* prior, const int32_t* key_lengths, float* logprob,
                       float* soft, float* row_lse, int32_t batch, int32_t t_q, int32_t t_k, int32_t c, void* stream);
 int kt_align_attn_bwd(const float* q, const float* k, const float* prior, const float* soft, const float* row_lse,

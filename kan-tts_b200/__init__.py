@@ -7,7 +7,7 @@ Public surface = the reference's own module API for this path:
   loss.* + criterion_builder                                              (kantts.train.loss)
   train.GanStep (GAN_Trainer.train_step + the data-parallel gradient exchange)
   sambert.KanTtsSAMBERT + MelReconLoss / ProsodyReconLoss                  (kantts.models.sambert, kantts.train.loss)
-  train.SambertStep (Sambert_Trainer.train_step)
+  train.SambertStep (Sambert_Trainer.train_step); data.AttnPriors (the MAS data path's alignment prior)
   sambert.KanTtsTextsyBERT + SeqCELoss, train.SybertStep, data.BertMasker (sybert.yaml: masked-symbol pretraining)
   infer.synthesize (symbols -> SAM-BERT free-running decode -> HiFi-GAN -> waveforms, no .npy hand-off)
   infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs, causal generators)
@@ -28,7 +28,7 @@ from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversa
                    DiscriminatorAdversarialLoss, FeatureMatchLoss, criterion_builder)
 from .train import (GanStep, SambertStep, SybertStep, hifigan_model_builder, sambert_model_builder,  # noqa: F401
                     sybert_model_builder)
-from .data import BertMasker  # noqa: F401
+from .data import AttnPriors, BertMasker  # noqa: F401
 from .infer import synthesize, stream_synthesize, TtsServer, slot_schedule  # noqa: F401
 from .speaker import DTDNN, kaldi_fbank, speaker_embedding  # noqa: F401
 

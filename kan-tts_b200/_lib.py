@@ -121,6 +121,7 @@ PROTOTYPES = {
     "kt_attn_ctc_workspace_bytes": [_I, _I, _I],
     "kt_attn_ctc_fwd": [_P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P],
     "kt_attn_ctc_bwd": [_P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _F, _P],
+    "kt_attn_prior": [_P, _P, _P, _I, _I, _I, _P],
     "kt_conv1d_fwd_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
     "kt_conv1d_fwd_tc_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
     "kt_sinadd_fwd_win": [_P, _P, _I, _I, _I, _I, _I, _I, _P],

@@ -1,6 +1,7 @@
 // Alignment learning of SAM-BERT with monotonic alignment search (MAS: True, sambert_16k_MAS*.yaml): the distance attention
 // of ConvAttention (kantts/models/sambert/attention.py:85-125), the width-1 MAS of alignment.py:32-71 and the forward-sum
 // loss of AttentionCTCLoss (kantts/train/loss.py:481-508).  Exact fp32 on CUDA cores, fixed-order reductions, no atomics.
+// Also the beta-binomial alignment prior of the data path (kantts/datasets/dataset.py:20-31), evaluated in float64.
 #include <math.h>
 
 #include "common.cuh"
@@ -473,7 +474,75 @@ __global__ void __launch_bounds__(kCtcThreads) ctc_bwd_kernel(const float* __res
   }
 }
 
+// ---- alignment prior ----------------------------------------------------------------------------------------------------
+constexpr int kPriorThreads = 256;
+constexpr int kPriorRows = 32;       // mel frames per CTA
+constexpr int kPriorCols = 128;      // symbols per pass over the CTA's rows
+
+// beta_binomial_prior_distribution (kantts/datasets/dataset.py:20-31) of utterance b = blockIdx.y, rows
+// [t0, t0 + kPriorRows): with n = P = in_len[b] + 1, M = out_len[b], alpha = t + 1, beta = M - t and s = t + k,
+//   ln prior[t][k] = lnC(n, k) + lnB(k + alpha, n - k + beta) - lnB(alpha, beta)
+//                  = col[k] + diag[s] + row[t]
+//   col[k]  = lg(n + 1) - lg(k + 1) - lg(n - k + 1)
+//   diag[s] = lg(s + 1) + lg(n + M - s)                       (k + alpha = s + 1, n - k + beta = n + M - s)
+//   row[t]  = -(lg(t + 1) + lg(M - t) - lg(M + 1)) - lg(n + M + 1)
+// with lg = the float64 lgamma.  Each term is computed once per CTA (the diagonal once per pass), in shared memory; an
+// element costs two adds and an exp.  Zero outside t < M, k < P.
+__global__ void __launch_bounds__(kPriorThreads) attn_prior_kernel(const int64_t* __restrict__ in_len,
+                                                                   const int64_t* __restrict__ out_len,
+                                                                   float* __restrict__ prior, int t_q, int t_k) {
+  __shared__ double row[kPriorRows];
+  __shared__ double col[kPriorCols];
+  __shared__ double diag[kPriorRows + kPriorCols - 1];
+  const int b = blockIdx.y, t0 = blockIdx.x * kPriorRows, tid = threadIdx.x;
+  const long long P = in_len[b] + 1, M = out_len[b];
+  const double n = (double)P, m = (double)M;
+  const double lg_n1 = lgamma(n + 1.0), lg_nm1 = lgamma(n + m + 1.0), lg_m1 = lgamma(m + 1.0);
+  const int rows = min(kPriorRows, t_q - t0);
+  const int live_rows = (int)max(0LL, min((long long)rows, M - t0));     // rows t < M
+  const int live_cols = (int)max(0LL, min((long long)t_k, P));            // columns k < P
+  for (int r = tid; r < live_rows; r += blockDim.x) {
+    const double t = (double)(t0 + r);
+    row[r] = -(lgamma(t + 1.0) + lgamma(m - t) - lg_m1) - lg_nm1;
+  }
+  float* out = prior + ((long long)b * t_q + t0) * t_k;
+  for (int k0 = 0; k0 < t_k; k0 += kPriorCols) {
+    const int cols = min(kPriorCols, t_k - k0);
+    const int live = max(0, min(cols, live_cols - k0));
+    if (live_rows > 0 && live > 0) {
+      __syncthreads();                                  // the previous pass has read col and diag
+      for (int c = tid; c < live; c += blockDim.x) {
+        const double k = (double)(k0 + c);
+        col[c] = lg_n1 - lgamma(k + 1.0) - lgamma(n - k + 1.0);
+      }
+      for (int d = tid; d < live_rows + live - 1; d += blockDim.x) {
+        const double s = (double)(t0 + k0 + d);
+        diag[d] = lgamma(s + 1.0) + lgamma(n + m - s);
+      }
+      __syncthreads();
+    }
+    for (int e = tid; e < rows * cols; e += blockDim.x) {
+      const int r = e / cols, c = e - r * cols;
+      float v = 0.f;
+      if (r < live_rows && c < live) v = __double2float_rn(exp(col[c] + diag[r + c] + row[r]));
+      out[(long long)r * t_k + k0 + c] = v;
+    }
+  }
+}
+
 }  // namespace
+
+extern "C" int kt_attn_prior(const int64_t* valid_input_lengths, const int64_t* valid_output_lengths, float* prior,
+                             int32_t batch, int32_t t_mel, int32_t t_text, void* stream) {
+  KT_REQUIRE(valid_input_lengths && valid_output_lengths && prior, "attn_prior: null argument");
+  KT_REQUIRE(batch > 0 && batch <= 65535 && t_mel > 0 && t_text > 0, "attn_prior: bad shape (batch %d, t_mel %d, t_text %d)",
+             batch, t_mel, t_text);
+  const dim3 grid((unsigned)ceil_div(t_mel, kPriorRows), (unsigned)batch);
+  attn_prior_kernel<<<grid, kPriorThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      valid_input_lengths, valid_output_lengths, prior, t_mel, t_text);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
 
 extern "C" int kt_align_attn_fwd(const float* q, const float* k, const float* prior, const int32_t* key_lengths,
                                  float* logprob, float* soft, float* row_lse, int32_t batch, int32_t t_q, int32_t t_k,

@@ -17,7 +17,7 @@ void set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* kt_last_error(void) { return g_err; }
-extern "C" int kt_version(void) { return 8; }
+extern "C" int kt_version(void) { return 9; }
 extern "C" int kt_has_tc(void) { return 1; }
 
 }  // namespace kt

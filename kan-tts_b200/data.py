@@ -155,3 +155,34 @@ class BertMasker:
                                           self.mask_ratio, self.n_sy, self.mask_id)
         self.call_index += 1
         return dict(batch, input_lings=lings, targets=targets, bert_masks=masks)
+
+
+class AttnPriors:
+    """The alignment prior of the MAS data path (``attn_priors`` of ``AM_Dataset``: ``beta_binomial_prior_distribution``
+    per utterance in ``__getitem__`` and the zero padding of ``collate_fn``, kantts/datasets/dataset.py:20-31, 497-503,
+    816-827) on the device.
+
+    ``priors(batch)`` takes a reference collate batch whose ``valid_input_lengths``, ``valid_output_lengths``,
+    ``mel_targets`` and ``input_lings`` are already on the device and returns a new dict with ``attn_priors`` (B, T, L)
+    float32, T = ``mel_targets.shape[1]``, L = ``input_lings.shape[1]``, the collate's shape; any ``attn_priors`` the batch
+    carries is replaced, never read.  Utterance b holds the beta-binomial pmf of P = valid_input_lengths[b] + 1 symbols
+    (the eos included, as the reference's ``len(ling_data[0])``) over its valid_output_lengths[b] frames, zero elsewhere,
+    evaluated in float64 and rounded to float32 (include/kantts_b200.h, kt_attn_prior).  One launch and no host
+    synchronisation.
+
+    ``install(kantts_dataset=module)`` replaces the dataset's own prior with ``attn_prior_placeholder``, so the workers do
+    no per-frame work; the batches then need this transform before the train step."""
+
+    def __call__(self, batch):
+        from .sambert_ops import attn_prior
+        prior = attn_prior(batch["valid_input_lengths"], batch["valid_output_lengths"], batch["mel_targets"].shape[1],
+                           batch["input_lings"].shape[1])
+        return dict(batch, attn_priors=prior)
+
+
+def attn_prior_placeholder(phoneme_count, mel_count):
+    """Stand-in for the dataset's ``beta_binomial_prior_distribution`` (see ``install``): an (M, P) float32 view of a single
+    NaN with strides (0, 0).  The workers compute and cache nothing per frame, ``collate_fn`` still slices its pad with the
+    shape, and a batch that misses ``AttnPriors`` trains on NaN losses instead of silently without a prior (an all-zero
+    prior would be a constant under the attention's log-softmax)."""
+    return torch.full((), float("nan"), dtype=torch.float32).expand(int(mel_count), int(phoneme_count))

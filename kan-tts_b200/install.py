@@ -8,11 +8,15 @@ replacing that name runs the unchanged ``SpeakerEmbeddingProcessor`` on speaker.
 import sys
 
 
-def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=None):
+def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=None, kantts_dataset=None):
     """``kantts_se``: the speaker-embedding processor module to patch; by default
     kantts.preprocess.se_processor.se_processor when it is already imported.  It is never imported here: it needs
-    torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want."""
-    from . import audio, hifigan, loss, pqmf, sambert, speaker
+    torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want.
+
+    ``kantts_dataset``: the dataset module (kantts.datasets.dataset) whose ``beta_binomial_prior_distribution`` becomes
+    ``data.attn_prior_placeholder``, for a MAS run whose batches go through ``data.AttnPriors`` on the device.  Patched
+    only when passed: without that transform the placeholder's NaN prior would reach the model."""
+    from . import audio, data, hifigan, loss, pqmf, sambert, speaker
     if kantts_models is None:
         import kantts.models as kantts_models
     if kantts_loss is None:
@@ -36,4 +40,6 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
         kantts_se = sys.modules.get("kantts.preprocess.se_processor.se_processor")
     if kantts_se is not None:
         kantts_se.DTDNN = speaker.DTDNN
+    if kantts_dataset is not None:
+        kantts_dataset.beta_binomial_prior_distribution = data.attn_prior_placeholder
     return kantts_models

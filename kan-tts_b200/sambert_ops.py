@@ -313,7 +313,7 @@ class FpInsertFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------------
-# alignment learning (MAS: True): kt_align_attn_*, kt_mas, kt_attn_ctc_*
+# alignment learning (MAS: True): kt_align_attn_*, kt_mas, kt_attn_ctc_*, kt_attn_prior
 # ------------------------------------------------------------------------------------------------
 
 
@@ -402,6 +402,17 @@ class AttnCtcFn(torch.autograd.Function):
         call("kt_attn_ctc_bwd", ptr(lp), ptr(il, True), ptr(ol, True), ptr(d_loss), ptr(ws), ws.numel() * 4,
              ptr(d_lp), B, Tq, Tk, ctx.blank)
         return d_lp.view(ctx.shape), None, None, None
+
+
+def attn_prior(valid_input_lengths, valid_output_lengths, t_mel, t_text):
+    """The collate's ``attn_priors`` on the device (kt_attn_prior): the beta-binomial prior of P = valid_input_lengths[b] + 1
+    symbols over M = valid_output_lengths[b] frames (beta_binomial_prior_distribution, kantts/datasets/dataset.py:20-31),
+    zero-padded to (B, t_mel, t_text) float32.  One launch, no host synchronisation."""
+    il = valid_input_lengths.to(torch.int64).contiguous()
+    ol = valid_output_lengths.to(torch.int64).contiguous()
+    prior = torch.empty(il.shape[0], t_mel, t_text, device=il.device, dtype=torch.float32)
+    call("kt_attn_prior", ptr(il, True), ptr(ol, True), ptr(prior), il.shape[0], int(t_mel), int(t_text))
+    return prior
 
 
 def average_frame_feat(feat, durs):
