@@ -427,12 +427,12 @@ typedef struct KtWindow {
 int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t frames, int32_t max_channels, void* stream);
 /* ONE launch: rows [0, history) of every window are zeroed for the batch items b with slots[b] != 0 (device uint8 [batch]). */
 int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream);
-/* Streams of a NON-CAUSAL generator: each window trails the pushed mel by `lag` rows (its chunk row t of item b is utterance
- * row u = frames_done[b] * rows_per_frame - lag + t), and each batch slot holds an utterance of lengths[b] frames.
- * KtStreamMask describes the input window of one conv call: the _masked conv entry points read a tap of item b as zero
- * unless 0 <= u < lengths[b] * rows_per_frame -- the whole-utterance forward's zero padding, applied per slot -- and
- * otherwise take exactly the arguments of kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream.  lengths and frames_done are
- * device int32 [batch]; the conv calls only read frames_done. */
+/* Streams of a NON-CAUSAL generator and of the post-net: each window trails the pushed frames by `lag` rows (its chunk row t
+ * of item b is utterance row u = frames_done[b] * rows_per_frame - lag + t), and each batch slot holds an utterance of
+ * lengths[b] frames.  KtStreamMask describes the input window of one conv call: the _masked conv entry points read a tap
+ * of item b as zero unless 0 <= u < lengths[b] * rows_per_frame -- the whole-utterance forward's zero padding, applied
+ * per slot -- and otherwise take exactly the arguments of kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream.  lengths and
+ * frames_done are device int32 [batch]; the conv calls only read frames_done. */
 typedef struct KtStreamMask {
   const int32_t* lengths;
   int32_t* frames_done;
@@ -449,19 +449,21 @@ int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32
                            int32_t first, int32_t frames, void* stream);
 
 /* ---- streaming SAM-BERT post-net (PostNet.streamer: decoder rows in, final post-net rows out, chunk by chunk) ---------------
- * Chunk row t of item b is frame frame0[b] + offset + t of its utterance (frame0: device int32 [batch]), so each slot can be
- * anywhere in its own utterance and no chunk reads device data on the host.
+ * `m` (KtStreamMask, one row per frame) describes a window: chunk row u of item b lies inside its utterance iff lo <= u < hi,
+ * lo = lag - frames_done[b] and hi = lo + lengths[b].  So each slot can be anywhere in its own utterance and no chunk reads
+ * device data on the host.
  *
  * kt_fsmn_fwd_stream_slots: one chunk of MemoryBlockV2 with FsmnEncoderV2's residual fused, seen as a causal depthwise FIR
  * whose output lags its input by rp = k - 1 - pad_left rows.  x, y and resid are windows placed by `w` (KtStreamWin, c
- * channels): input rows [-(k-1), rows) of the chunk are read (in_first >= k - 1), output rows [0, rows) are written.  Output
- * row t is frame row0 + t, row0 = frame0[b] + offset; its tap j reads input row t + j - (k-1), frame row0 + t + j - pad_left.
- * With keep(b, a) = (0 <= a < lengths[b]) (lengths: device int32 [batch]) and xm = keep * x:
- *   y[t] = keep(row0 + t) * (xm[t - rp] + sum_j weight[c][j] * xm[t + j - (k-1)]) + resid[t]      (resid optional)
- * xm is a selection, not a product: frames before 0 and from lengths[b] on read as zeros whatever the window holds there.
+ * channels): input rows [-(k-1), rows) of the chunk are read (in_first >= k - 1), output rows [0, rows) are written.  `m`
+ * describes the input window; output row t is the frame of input row t - rp, and its tap j reads input row t + j - (k-1).
+ * With keep(u) = (lo <= u < hi) and xm = keep * x:
+ *   y[t] = keep(t - rp) * (xm[t - rp] + sum_j weight[c][j] * xm[t + j - (k-1)]) + resid[t]      (resid optional)
+ * xm is a selection, not a product: rows outside the utterance read as zeros whatever the window holds there.
  * The skip term first, then the taps in order, each an fma: kt_fsmn_fwd's sum, so a streamed row equals the whole-sequence
  * row bit for bit.  weight [c][k] as in kt_fsmn_fwd.
- * kt_lstm_stream_slots: `rows` steps of a 1-layer unidirectional nn.LSTM (hidden <= 256), one CTA per batch item.
+ * kt_lstm_stream_slots: `rows` steps of a 1-layer unidirectional nn.LSTM (hidden <= 256), one CTA per batch item.  `m`
+ * describes gx: row t of item b is frame t - lo.
  *   gx     row t of item b at gx[(b * gx_pitch + t) * 4 * hidden]: x . weight_ih^T + bias_ih + bias_hh (one k = 1 conv)
  *   whh_t  [hidden][4 * hidden] = weight_hh^T
  *   state  [batch][2][hidden]: (h, c) carried from the previous chunk, overwritten with (h, c) after the last row.  A chunk
@@ -469,11 +471,11 @@ int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32
  *          as they are (zero) and outputs that zero h, so frame 0 starts from (h, c) = 0.
  *   h      row t of item b at h[(b * h_pitch + t) * hidden]: the LSTM output.
  * PyTorch gate order (i, f, g, o); exact fp32. */
-int kt_fsmn_fwd_stream_slots(const KtStreamWin* w, const float* x, const float* weight, const int32_t* lengths,
-                             const int32_t* frame0, int32_t offset, const float* resid, float* y, int32_t batch, int32_t rows,
-                             int32_t c, int32_t k, int32_t pad_left, void* stream);
-int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const int32_t* frame0, int32_t offset,
-                         int32_t batch, int32_t rows, int32_t hidden, int32_t gx_pitch, int32_t h_pitch, void* stream);
+int kt_fsmn_fwd_stream_slots(const KtStreamWin* w, const KtStreamMask* m, const float* x, const float* weight,
+                             const float* resid, float* y, int32_t batch, int32_t rows, int32_t c, int32_t k, int32_t pad_left,
+                             void* stream);
+int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const KtStreamMask* m, int32_t batch,
+                         int32_t rows, int32_t hidden, int32_t gx_pitch, int32_t h_pitch, void* stream);
 /* kt_pnca_step_slots: one free-running decoder step of a PNCA layer's two attentions for `batch` slots, each at its own
  * step s = step[b] (device int32 [batch], as mem_len, x_bw, h_bw; active: device uint8 [batch]).
  *   q_row  [batch][3 * heads * d_head]: the step's fused Q | K | V projection

@@ -133,8 +133,9 @@ PROTOTYPES = {
     "kt_conv1d_fwd_tc_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin),
                                        ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P],
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
-    "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P],
-    "kt_lstm_stream_slots": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _I, _I, _I, _I,
+                                 _I, _P],
+    "kt_lstm_stream_slots": [_P, _P, _P, _P, ctypes.POINTER(KtStreamMask), _I, _I, _I, _I, _I, _P],
     "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
     "kt_kaldi_fbank": [_P, _P, _P, _I, _I, _I, _I, _F, _F, _P],

@@ -1199,35 +1199,35 @@ extern "C" int kt_ar_duration_infer(const float* g0c, const float* w1, const flo
 }
 
 // ---------------------------------------------------------------------------------------------
-// Streaming post-net (PostNet.streamer): one chunk of MemoryBlockV2 and one chunk of the post-net LSTM.  The frame of a
-// slot's chunk row comes from the device (frame0[b] + offset), so every slot of one launch can sit at a different place in
-// its own utterance.
+// Streaming post-net (PostNet.streamer): one chunk of MemoryBlockV2 and one chunk of the post-net LSTM.  Which chunk rows
+// of item b lie inside its utterance comes from the device (KtStreamMask, read by stream_utterance_rows), so every slot of
+// one launch can sit at a different place in its own utterance.
 //
 // fsmn_stream_slots_kernel: the memory block as a causal depthwise FIR whose output lags its input by rp = K-1-lp rows.
-// Output row t of item b's chunk is frame row0 + t, row0 = frame0[b] + offset; its taps j < K read input rows t + j - (K-1)
-// of the chunk (negative: the window's history), frames row0 + t + j - lp.  keep(b, a) = 0 <= a < lengths[b]; xm = keep * x,
-// by selection, so whatever a window holds outside the utterance reads as zero.
-//   y[t] = keep(row0 + t) * (xm[t - rp] + sum_j w[c][j] * xm[t + j - (K-1)]) + resid[t]
+// m describes the input window: input row u of item b's chunk (negative: the window's history) holds a frame iff
+// lo <= u < hi.  Output row t is the frame of input row t - rp; its taps j < K read input rows t + j - (K-1).
+// keep(u) = lo <= u < hi; xm = keep * x, by selection, so whatever a window holds outside the utterance reads as zero.
+//   y[t] = keep(t - rp) * (xm[t - rp] + sum_j w[c][j] * xm[t + j - (K-1)]) + resid[t]
 // The skip term first, then the taps in order, each an fmaf with the masked value: fsmn_fir_kernel's sum, so a streamed row
 // equals the whole-sequence row bit for bit.  One thread per (row, channel) of one item (blockIdx.y).
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) fsmn_stream_slots_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                                const int* __restrict__ lengths, const int* __restrict__ frame0,
-                                                                const float* __restrict__ resid, float* __restrict__ y,
-                                                                KtStreamWin win, int rows, int C, int K, int lp, int offset) {
+__global__ void __launch_bounds__(256) fsmn_stream_slots_kernel(const KtStreamMask m, const float* __restrict__ x,
+                                                                const float* __restrict__ w, const float* __restrict__ resid,
+                                                                float* __restrict__ y, KtStreamWin win, int rows, int C, int K,
+                                                                int lp) {
   const int b = blockIdx.y;
-  const int len = __ldg(lengths + b);
-  const int row0 = __ldg(frame0 + b) + offset;
+  int lo, hi;
+  stream_utterance_rows(m, b, lo, hi);
+  const int rp = K - 1 - lp;
   const long long n = (long long)rows * C;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int t = (int)(i / C), c = (int)(i - (long long)t * C);
     const float* xc = x + ((long long)b * win.in_pitch + win.in_first + t - (K - 1)) * C + c;
-    const int a0 = row0 + t - lp;
-    const bool keep_t = row0 + t >= 0 && row0 + t < len;
+    const bool keep_t = t - rp >= lo && t - rp < hi;
     float acc = keep_t ? __ldg(xc + (long long)lp * C) : 0.f;
     for (int j = 0; j < K; ++j) {
-      const int a = a0 + j;
-      const float v = (a >= 0 && a < len) ? __ldg(xc + (long long)j * C) : 0.f;
+      const int u = t + j - (K - 1);
+      const float v = (u >= lo && u < hi) ? __ldg(xc + (long long)j * C) : 0.f;
       acc = fmaf(__ldg(w + (long long)c * K + j), v, acc);
     }
     float out = keep_t ? acc : 0.f;
@@ -1236,11 +1236,13 @@ __global__ void __launch_bounds__(256) fsmn_stream_slots_kernel(const float* __r
   }
 }
 
-extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const float* x, const float* w, const int32_t* lengths,
-                                        const int32_t* frame0, int32_t offset, const float* resid, float* y, int32_t B,
-                                        int32_t rows, int32_t C, int32_t K, int32_t lp, void* stream) {
+extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const KtStreamMask* m, const float* x, const float* w,
+                                        const float* resid, float* y, int32_t B, int32_t rows, int32_t C, int32_t K,
+                                        int32_t lp, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  KT_REQUIRE(win && x && w && lengths && frame0 && y, "fsmn_fwd_stream_slots: null pointer");
+  int rc = validate_stream_mask(m, "fsmn_fwd_stream_slots");
+  if (rc) return rc;
+  KT_REQUIRE(win && x && w && y, "fsmn_fwd_stream_slots: null pointer");
   KT_REQUIRE(B >= 1 && B <= 65535 && rows >= 1 && C >= 1 && K >= 1 && lp >= 0 && lp < K, "fsmn_fwd_stream_slots: bad sizes");
   KT_REQUIRE(win->in_first >= K - 1 && win->in_first + rows <= win->in_pitch,
              "fsmn_fwd_stream_slots: the input window needs K - 1 rows of history before the chunk");
@@ -1250,32 +1252,33 @@ extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const float* x, 
              "fsmn_fwd_stream_slots: the chunk does not fit its residual window");
   const long long n = (long long)rows * C;
   const int blocks = (int)std::min<long long>((n + 255) / 256, 1024);
-  fsmn_stream_slots_kernel<<<dim3(blocks, B), 256, 0, st>>>(x, w, lengths, frame0, resid, y, *win, rows, C, K, lp, offset);
+  fsmn_stream_slots_kernel<<<dim3(blocks, B), 256, 0, st>>>(*m, x, w, resid, y, *win, rows, C, K, lp);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
 
 // lstm_stream_slots_kernel: `rows` steps of a 1-layer unidirectional LSTM, carrying (h, c) of item b in state[b][2][H];
-// row t of item b is frame frame0[b] + offset + t.  A chunk whose first row is frame 0 or earlier starts from (h, c) = 0
-// whatever state holds, a later chunk from the carried state.  A row before frame 0 leaves (h, c) as they are, i.e. zero,
-// and its output row is that zero h; frame 0 therefore starts from zeros.  One CTA per item, one thread per gate: gate j of
-// step t = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced over j), then one thread per hidden unit
-// updates c and h.  PyTorch gate order (i, f, g, o); exact fp32.
+// with lo from m (stream_utterance_rows), row t of item b is frame t - lo.  A chunk whose first row is frame 0 or earlier
+// (lo >= 0) starts from (h, c) = 0 whatever state holds, a later chunk from the carried state.  A row before frame 0 leaves
+// (h, c) as they are, i.e. zero, and its output row is that zero h; frame 0 therefore starts from zeros.  One CTA per item,
+// one thread per gate: gate j of step t = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced over j),
+// then one thread per hidden unit updates c and h.  PyTorch gate order (i, f, g, o); exact fp32.
 __global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
-                                         float* __restrict__ h_out, const int* __restrict__ frame0, int offset, int rows, int H,
-                                         int gx_pitch, int h_pitch) {
+                                         float* __restrict__ h_out, const KtStreamMask m, int rows, int H, int gx_pitch,
+                                         int h_pitch) {
   extern __shared__ float sm[];
   const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x;
   float* h = sm;             // [H]
   float* c = h + H;          // [H]
   float* gates = c + H;      // [4H]
   float* s = state + (long long)b * 2 * H;
-  const int a0 = __ldg(frame0 + b) + offset;
-  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = a0 > 0 ? s[j] : 0.f;
+  int lo, hi;
+  stream_utterance_rows(m, b, lo, hi);
+  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = lo < 0 ? s[j] : 0.f;
   __syncthreads();
   for (int t = 0; t < rows; ++t) {
     float* out = h_out + ((long long)b * h_pitch + t) * H;
-    if (a0 + t < 0) {
+    if (t < lo) {
       for (int j = tid; j < H; j += blockDim.x) out[j] = h[j];
       continue;                                  // uniform over the CTA: no barrier is skipped by part of it
     }
@@ -1299,15 +1302,16 @@ __global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const flo
   for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
 }
 
-extern "C" int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const int32_t* frame0,
-                                    int32_t offset, int32_t B, int32_t rows, int32_t H, int32_t gx_pitch, int32_t h_pitch,
-                                    void* stream) {
+extern "C" int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const KtStreamMask* m,
+                                    int32_t B, int32_t rows, int32_t H, int32_t gx_pitch, int32_t h_pitch, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  KT_REQUIRE(gx && whh_t && state && h && frame0, "lstm_stream_slots: null pointer");
+  int rc = validate_stream_mask(m, "lstm_stream_slots");
+  if (rc) return rc;
+  KT_REQUIRE(gx && whh_t && state && h, "lstm_stream_slots: null pointer");
   KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream_slots: bad sizes");
   const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
   const size_t smem = (size_t)6 * H * sizeof(float);
-  lstm_stream_slots_kernel<<<B, threads, smem, st>>>(gx, whh_t, state, h, frame0, offset, rows, H, gx_pitch, h_pitch);
+  lstm_stream_slots_kernel<<<B, threads, smem, st>>>(gx, whh_t, state, h, *m, rows, H, gx_pitch, h_pitch);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }

@@ -26,8 +26,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, KtStreamMask, ptr
-from .stream import Windows, WindowTable, check_slots, own_weight, to_device
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, ptr
+from .stream import SlotUtterances, Windows, WindowTable, check_slots, own_weight, to_device
 
 # --------------------------------------------------------------------------------------------
 # parameter holders (names / shapes == the reference's weight_norm / spectral_norm wrapped convs)
@@ -733,7 +733,7 @@ class GeneratorStreamer:
     lengths[b] are ignored.  ``finish()`` pushes the ``drain_frames`` frames that bring out an utterance's last sample.
     The chunks of slot b concatenated and cut to [delay, delay + lengths[b] * hop) equal the forward on the slot's mel of
     exactly lengths[b] frames: every layer's zero padding at the utterance's end is applied per slot inside the conv
-    kernels (the _masked entry points), from lengths and frame counts kept on the device.  A slot reset before its
+    kernels (the _masked entry points), from the slots' utterance record (stream.SlotUtterances).  A slot reset before its
     utterance has drained loses the samples not yet returned.
 
     NSF generator: ``push`` takes (B, in_channels + 2, f) -- mel, f0 in Hz and the voiced flag, as ``forward`` -- and each
@@ -773,13 +773,10 @@ class GeneratorStreamer:
         self._source = gen.source_module if plan.nsf else None
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
         with torch.no_grad(), torch.cuda.device(self.device):
-            self._masks = None
+            self._slots = self._masks = None
             if not plan.causal:
-                self._len = torch.zeros(self.batch, dtype=torch.int32, device=self.device)
-                self._done = torch.zeros(self.batch, dtype=torch.int32, device=self.device)
-                self._masks = {w["name"]: KtStreamMask(lengths=ptr(self._len, True), frames_done=ptr(self._done, True),
-                                                       rows_per_frame=w["rows_per_frame"], lag=plan.lags[w["name"]])
-                               for w in plan.windows}
+                self._slots = SlotUtterances(self.batch, self.device)
+                self._masks = {w["name"]: self._slots.mask(w["rows_per_frame"], plan.lags[w["name"]]) for w in plan.windows}
                 self._zeros = torch.zeros(self.batch, self.in_channels, self.max_frames, device=self.device)
             self._weights = {st.conv: own_weight(st.spec, *st.conv.effective_weight(), st.conv.bias)
                              for st in plan.steps if type(st) is ConvStep}
@@ -821,9 +818,7 @@ class GeneratorStreamer:
                 ops.call("kt_add3_scale_win", srcs[0], srcs[1], srcs[2], st.scale, ptr(dst), B, f * win.rate[st.dst], ch,
                          b[st.srcs[0]].shape[1], dst.shape[1], win.first[st.dst])
         if masks is not None:
-            wav = b["wav"]
-            ops.call("kt_stream_mask_advance", ctypes.byref(masks["wav"]), ptr(wav), B, f * self.hop, 1, wav.shape[1],
-                     win.first["wav"], f)
+            self._slots.mask_advance(masks["wav"], b["wav"], win.first["wav"], f * self.hop, f)
         win.advance(f)
 
     def push(self, mel):
@@ -868,29 +863,13 @@ class GeneratorStreamer:
             raise ValueError("reset: seeds are for NSF generators")
         slots = check_slots(slots, self.batch)
         with torch.no_grad(), torch.cuda.device(self.device):
-            if lengths is not None:
-                lengths = self._lengths(lengths, len(slots))
             if seeds is not None:
                 seeds = nsf_seed_tensor(seeds, len(slots), self.device)
+            if lengths is not None:                 # checks the lengths before its first launch
+                self._slots.reset(slots, lengths)
             self._win.reset(slots)
-            idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
-            if lengths is not None:                 # none of the new utterances' frames pushed yet
-                self._len.index_copy_(0, idx, lengths)
-                self._done.index_fill_(0, idx, 0)
             if seeds is not None:                   # excitation phases and sample counts return to zero
-                self._nsf.reset(idx, seeds)
-
-    def _lengths(self, lengths, n):
-        """-> the frame counts of n utterances (host sequence or device tensor) as a device int32 tensor (n,); ValueError
-        on a wrong count or, for host values, a length below 1."""
-        if not (torch.is_tensor(lengths) and lengths.is_cuda):
-            lengths = torch.as_tensor(lengths)
-            if lengths.numel() and int(lengths.min()) < 1:
-                raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
-        lengths = lengths.to(device=self.device, dtype=torch.int32).reshape(-1)
-        if lengths.numel() != n:
-            raise ValueError(f"streamer: expected {n} lengths, got {lengths.numel()}")
-        return lengths
+                self._nsf.reset(to_device(torch.tensor(slots, dtype=torch.long), self.device), seeds)
 
 
 # --------------------------------------------------------------------------------------------

@@ -38,7 +38,7 @@ import torch.nn.functional as F
 from . import ops
 from . import sambert_ops as sops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, ptr
-from .stream import Windows, WindowTable, check_slots, own_weight
+from .stream import SlotUtterances, Windows, WindowTable, own_weight
 
 
 def get_mask_from_lengths(lengths, max_len=None):
@@ -872,16 +872,17 @@ class PostNetStreamPlan:
       delay               D = the sum of rp: the post-net output of a chunk is its decoder rows shifted back by D rows
       windows             one entry per tensor of a chunk: {name, channels, rows_per_frame (1), history}; a memory block's
                           input keeps k - 1 rows, a residual read lagging its tensor by n rows keeps n, the others keep none
+      lags                {window: rows it trails the decoder rows} of the masked reads: ctx{i} (lag), "gates", "out" (D)
       steps               PostNetStep records, in launch order
-      launches_per_chunk  library calls of a steady chunk: one per step and one window advance; the copy of the decoder rows
-                          into their window and the output mask are not counted"""
+      launches_per_chunk  library calls of a steady chunk: one per step, one window advance and one output mask; the copy of
+                          the decoder rows into their window is not counted"""
 
     def __init__(self, postnet):
         if postnet.training:
             raise ValueError("streaming runs a post-net in eval() mode")
         fsmn = postnet.fsmn
         table = WindowTable()
-        self.windows, self.layers, self.steps = table.windows, [], []
+        self.windows, self.layers, self.steps, self.lags = table.windows, [], [], {}
         x, lag = table.add("dec", postnet.num_mels), 0
         mid = table.add("mid", fsmn.ffn_inner_dim)
         units = fsmn.num_memory_units
@@ -893,6 +894,7 @@ class PostNetStreamPlan:
             self.layers.append(dict(lp=mb.lp, rp=mb.rp, kernel=k, lag=lag))
             ctx = table.add(f"ctx{i}", units)
             table.read(ctx, k - 1)
+            self.lags[ctx] = lag
             resid = x if ffn.w_1.in_channels == units else None
             if resid is not None:
                 table.read(resid, mb.rp)
@@ -906,7 +908,8 @@ class PostNetStreamPlan:
         h = table.add("h", postnet.lstm.hidden_size)
         self.steps += [PostNetStep("conv", postnet.lstm, x, gates), PostNetStep("lstm", postnet.lstm, gates, h),
                        PostNetStep("conv", postnet.fc, h, table.add("out", postnet.num_mels), "dec", res_lag=self.delay)]
-        self.launches_per_chunk = table.launches_per_chunk(len(self.steps))
+        self.lags.update(gates=self.delay, out=self.delay)
+        self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + 1
 
 
 class PostNetStreamer:
@@ -918,15 +921,15 @@ class PostNetStreamer:
     ``delay`` all-padding rows and returns the rest; the rows returned in order are then the whole-sequence post-net output.
     ``reset(lengths=None)`` starts a new batch.  No call reads device data on the host.
 
-    Every chunk runs over all f rows of every slot.  Each slot's frame count and the frame ``rows[b]`` of its utterance at
-    the chunk's first decoder row live on the device.  A tensor a layer reads before the chunk lives in a window
+    Every chunk runs over all f rows of every slot.  Where each slot is in its utterance lives on the device
+    (stream.SlotUtterances, whose frames are the decoder rows).  A tensor a layer reads before the chunk lives in a window
     (stream.py).  The memory blocks (kt_fsmn_fwd_stream_slots) read frames outside [0, lengths[b]) as zeros, the
     whole-sequence padding, and the LSTM (kt_lstm_stream_slots) starts from zeros at frame 0, so starting an utterance
     clears no window history or LSTM state; every other step reads only the frame it writes, and the output is masked
     outside the utterance.  The weights are prepared once, when the streamer is created.
 
     Per-slot mode (``per_slot=True``): ``push`` returns all f rows of every slot, output row t being frame
-    rows[b] - delay + t (zero outside [0, lengths[b])).  ``reset(lengths, slots=..., start_row=...)`` starts new
+    frames_done[b] - delay + t (zero outside [0, lengths[b])).  ``reset(lengths, slots=..., start_row=...)`` starts new
     utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  A slot's new
     utterance must start after the previous one's last row was returned."""
 
@@ -938,9 +941,8 @@ class PostNetStreamer:
         self.per_slot = bool(per_slot)
         self._state = torch.zeros(self.batch, 2, self.hidden, device=self.device)
         self._zeros = torch.zeros(self.batch, self.max_frames, self.num_mels, device=self.device)
-        self._len = torch.empty(self.batch, dtype=torch.int32, device=self.device)
-        self._row = torch.zeros(self.batch, dtype=torch.int32, device=self.device)     # rows[b]
-        self._out_frame = torch.arange(self.max_frames, dtype=torch.int32, device=self.device) - self.delay  # row t: + rows[b]
+        self._slots = SlotUtterances(self.batch, self.device)
+        self._masks = {name: self._slots.mask(1, lag) for name, lag in plan.lags.items()}
         self._places = [None if st.kind == "lstm" else win.place(st.src, st.dst, st.resid, res_lag=st.res_lag)
                         for st in plan.steps]
         with torch.no_grad(), torch.cuda.device(self.device):
@@ -963,7 +965,7 @@ class PostNetStreamer:
     def _chunk(self, f, skip):
         """Every launch of one chunk of f decoder rows (already in the "dec" window) -> output rows [skip, f) of every slot,
         zero where a row's frame lies outside its slot's utterance."""
-        b, B = self._win.buf, self.batch
+        b, B, masks = self._win.buf, self.batch, self._masks
         for st, w, place in zip(self.plan.steps, self._weights, self._places):
             src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
             if st.kind == "conv":
@@ -971,17 +973,14 @@ class PostNetStreamer:
                 ops.stream_conv(spec, pw, bias, src, dst, f, place, resid)
             elif st.kind == "fsmn":
                 layer = self.plan.layers[st.layer]
-                ops.call("kt_fsmn_fwd_stream_slots", ctypes.byref(place), ptr(src), ptr(w), ptr(self._len, True),
-                         ptr(self._row, True), -layer["lag"] - layer["rp"], ptr(resid), ptr(dst), B, f, src.shape[2],
-                         layer["kernel"], layer["lp"])
+                ops.call("kt_fsmn_fwd_stream_slots", ctypes.byref(place), ctypes.byref(masks[st.src]), ptr(src), ptr(w),
+                         ptr(resid), ptr(dst), B, f, src.shape[2], layer["kernel"], layer["lp"])
             else:
-                ops.call("kt_lstm_stream_slots", ptr(src), ptr(w), ptr(self._state), ptr(dst), ptr(self._row, True),
-                         -self.delay, B, f, self.hidden, src.shape[1], dst.shape[1])
+                ops.call("kt_lstm_stream_slots", ptr(src), ptr(w), ptr(self._state), ptr(dst), ctypes.byref(masks[st.src]),
+                         B, f, self.hidden, src.shape[1], dst.shape[1])
+        self._slots.mask_advance(masks["out"], b["out"], self._win.first["out"], f, f)
         self._win.advance(f)
-        frames = self._row[:, None] + self._out_frame[None, :f]
-        pad = (frames < 0) | (frames >= self._len[:, None])
-        self._row += f
-        return b["out"][:, skip:f].masked_fill(pad[:, skip:].unsqueeze(-1), 0)
+        return b["out"][:, skip:f].clone(memory_format=torch.contiguous_format)
 
     def push(self, dec_rows):
         """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final
@@ -1002,36 +1001,20 @@ class PostNetStreamer:
         return torch.cat(outs, 1) if outs else self._zeros[:, :0].clone()
 
     def reset(self, lengths=None, slots=None, start_row=0):
-        """Start a new batch: every slot's frame 0 is row 0 of the next push; ``lengths`` (device tensor (batch,)), when
-        given, replaces the slots' frame counts.
+        """Start a new batch: every slot's frame 0 is row 0 of the next push; ``lengths`` (host ints or a device tensor,
+        (batch,)), when given, replaces the slots' frame counts.
 
-        Per-slot mode with ``slots`` (host ints): only those slots start new utterances, of ``lengths`` frames (host ints,
-        in the order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames); the
+        Per-slot mode with ``slots`` (host ints): only those slots start new utterances, of ``lengths`` frames (in the
+        order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames); the
         other slots go on.  Neither form clears a window or the LSTM state, and neither reads device data."""
-        if slots is not None:
-            self._reset_slots(slots, lengths, start_row)
-            return
-        with torch.no_grad(), torch.cuda.device(self.device):
-            if lengths is not None:
-                if lengths.shape != (self.batch,):
-                    raise ValueError(f"reset: expected ({self.batch},) lengths, got {tuple(lengths.shape)}")
-                self._len.copy_(lengths)
-            self._row.zero_()
-        self._rows = 0
-
-    def _reset_slots(self, slots, lengths, start_row):
-        if not self.per_slot:
+        if slots is None:
+            start_row = 0
+        elif not self.per_slot:
             raise ValueError("reset: slots are for a per-slot streamer (PostNet.streamer(..., per_slot=True))")
-        slots, start_row = check_slots(slots, self.batch), int(start_row)
-        lengths = [int(n) for n in lengths]
-        if len(lengths) != len(slots) or any(n < 1 for n in lengths):
-            raise ValueError(f"reset: expected {len(slots)} lengths >= 1, got {lengths}")
-        if not 0 <= start_row < self.max_frames:
+        elif not 0 <= int(start_row) < self.max_frames:
             raise ValueError(f"reset: start_row must lie in [0, {self.max_frames}), got {start_row}")
-        with torch.no_grad():
-            for s, n in zip(slots, lengths):
-                self._len[s] = n
-                self._row[s] = -start_row
+        self._slots.reset(slots, lengths, start_row)
+        self._rows = 0                                     # (read in lockstep mode only)
 
 
 class FP_Predictor(nn.Module):

@@ -1,11 +1,13 @@
 """The stream window format of the streamed vocoder (hifigan.GeneratorStreamer) and post-net (sambert.PostNetStreamer),
-DESIGN.md §3.7.  A window is a persistent (B, H + F·rows_per_frame, C) buffer: rows [0, H) carry the last H rows of the
-earlier chunks (zeros after a reset: the causal padding), the chunk is written at row H, and H is the largest history
-any reader of the tensor needs."""
+and the per-slot utterance record both keep, DESIGN.md §3.7.  A window is a persistent (B, H + F·rows_per_frame, C)
+buffer: rows [0, H) carry the last H rows of the earlier chunks (zeros after a reset: the causal padding), the chunk is
+written at row H, and H is the largest history any reader of the tensor needs."""
+import ctypes
+
 import torch
 
 from . import ops
-from ._lib import KtStreamWin, KtWindow, ptr
+from ._lib import KtStreamMask, KtStreamWin, KtWindow, ptr
 
 
 class WindowTable:
@@ -91,6 +93,41 @@ class Windows:
             sel = to_device(mask, self.device)
         if self._ntable:
             ops.call("kt_stream_reset", ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c)
+
+
+class SlotUtterances:
+    """Each slot's place in its utterance, on the device: ``lengths`` and ``frames_done`` (frames since frame 0), int32
+    (B,).  Chunk row t of a window trailing by ``lag`` rows is frame frames_done[b] + (t - lag) / rows_per_frame."""
+
+    def __init__(self, batch, device):
+        self.batch, self.device = batch, device
+        self.lengths = torch.zeros(batch, dtype=torch.int32, device=device)
+        self.frames_done = torch.zeros(batch, dtype=torch.int32, device=device)
+
+    def reset(self, slots, lengths, start_row=0):
+        """``slots`` (host ints; None: all) start utterances of ``lengths`` frames (host ints or CUDA tensor; None:
+        kept) at chunk row ``start_row`` of the next push.  All checked before the first launch; none waits."""
+        slots = list(range(self.batch)) if slots is None else check_slots(slots, self.batch)
+        idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
+        if lengths is not None:
+            if not (torch.is_tensor(lengths) and lengths.is_cuda):
+                lengths = torch.as_tensor(lengths, dtype=torch.int32)
+                if lengths.numel() and int(lengths.min()) < 1:
+                    raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
+                lengths = to_device(lengths, self.device)
+            if lengths.numel() != len(slots):
+                raise ValueError(f"streamer: expected {len(slots)} lengths, got {lengths.numel()}")
+            self.lengths.index_copy_(0, idx, lengths.to(self.device, torch.int32).reshape(-1))
+        self.frames_done.index_fill_(0, idx, -int(start_row))
+
+    def mask(self, rows_per_frame, lag):
+        """-> the KtStreamMask of a window of ``rows_per_frame`` rows per frame trailing by ``lag`` rows."""
+        return KtStreamMask(ptr(self.lengths, True), ptr(self.frames_done, True), rows_per_frame, lag)
+
+    def mask_advance(self, mask, window_buf, first, rows, frames):
+        """One launch: zero the chunk rows [first, first + rows) outside each utterance, then frames_done += frames."""
+        ops.call("kt_stream_mask_advance", ctypes.byref(mask), ptr(window_buf), self.batch, rows, window_buf.shape[2],
+                 window_buf.shape[1], first, frames)
 
 
 def check_slots(slots, batch):

@@ -190,6 +190,26 @@ def test_per_slot_postnet_equals_lockstep_alone_bitwise():
             assert torch.equal(got[b, first + lens[b]:], torch.zeros_like(got[b, first + lens[b]:]))
 
 
+def test_rejected_per_slot_postnet_reset_leaves_the_stream_as_it_was():
+    torch.manual_seed(3)
+    pn = PostNet(K.sambert_24k_config()).to(DEV).eval()
+    rows = torch.randn(2, 24, 80, generator=torch.Generator().manual_seed(5)).to(DEV)
+    outs = {}
+    with torch.no_grad(), _exact():
+        for rejected in (False, True):
+            st = pn.streamer(2, 8, torch.zeros(2, dtype=torch.int32, device=DEV), per_slot=True)
+            st.reset([20, 13], slots=[0, 1], start_row=0)
+            got = [st.push(rows[:, :8])]
+            if rejected:
+                with pytest.raises(ValueError, match="distinct"):
+                    st.reset([5, 5], slots=[1, 1], start_row=2)
+                with pytest.raises(ValueError, match="start_row"):
+                    st.reset([5], slots=[1], start_row=8)
+            got += [st.push(rows[:, t:t + 8]) for t in (8, 16)]
+            outs[rejected] = torch.cat(got, 1)
+    assert torch.equal(outs[True], outs[False])
+
+
 # ---- server --------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("chunk_steps", [1, 3, 4])
 def test_server_matches_synthesize_alone_and_isolates_slots(golden, chunk_steps):

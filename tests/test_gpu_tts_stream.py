@@ -10,7 +10,7 @@ import torch.nn.functional as F
 
 import kantts_b200 as K
 from kantts_b200 import _lib, ops
-from kantts_b200._lib import KtStreamWin, check, ptr, stream_ptr
+from kantts_b200._lib import KtStreamMask, KtStreamWin, check, ptr, stream_ptr
 from kantts_b200.sambert import PostNet
 from conftest import rel_l2
 from test_tts_stream_cpu import LENGTHS, SCHEDULES, T
@@ -83,7 +83,7 @@ def test_postnet_streamer_reset_starts_a_new_batch():
     assert torch.equal(first, after)                  # first: the output of a fresh streamer
 
 
-def test_fsmn_stream_slots_rows_equal_whole_sequence_rows_bitwise():
+def test_fsmn_stream_slots_masked_rows_equal_whole_sequence_rows_bitwise():
     lib = _lib.load()
     B, C, K_, lp = 3, 96, 41, 37
     rp = K_ - 1 - lp
@@ -94,7 +94,8 @@ def test_fsmn_stream_slots_rows_equal_whole_sequence_rows_bitwise():
     lengths = torch.tensor(LENGTHS, device=DEV, dtype=torch.int32)
     mask = (torch.arange(T, device=DEV)[None, :] >= lengths[:, None]).to(torch.uint8)
     y = torch.empty_like(x)
-    frame0 = torch.zeros(B, dtype=torch.int32, device=DEV)
+    done = torch.zeros(B, dtype=torch.int32, device=DEV)
+    m = KtStreamMask(lengths=ptr(lengths, True), frames_done=ptr(done, True), rows_per_frame=1, lag=0)
     check(lib.kt_fsmn_fwd(ptr(x), ptr(w), ptr(mask, True), ptr(y), B, T, C, K_, lp, stream_ptr()), "kt_fsmn_fwd")
     # one window holding the whole input after k - 1 history rows (zeros), and rp padding rows at the end; the outputs are
     # frames -rp .. T-1 (the first rp rows are before the utterance)
@@ -106,9 +107,9 @@ def test_fsmn_stream_slots_rows_equal_whole_sequence_rows_bitwise():
         for f in (7, 1, 12, 3, T + rp - 23):
             win = KtStreamWin(in_pitch=xw.shape[1], in_first=K_ - 1 + s, out_pitch=T + rp, out_first=s, res_pitch=T + rp,
                               res_first=s)
-            check(lib.kt_fsmn_fwd_stream_slots(ctypes.byref(win), ptr(xw), ptr(w), ptr(lengths, True), ptr(frame0, True),
-                                               s - rp, ptr(res), ptr(yw), B, f, C, K_, lp, stream_ptr()),
-                  "kt_fsmn_fwd_stream_slots")
+            done.fill_(s)
+            check(lib.kt_fsmn_fwd_stream_slots(ctypes.byref(win), ctypes.byref(m), ptr(xw), ptr(w), ptr(res), ptr(yw), B, f,
+                                               C, K_, lp, stream_ptr()), "kt_fsmn_fwd_stream_slots")
             s += f
         assert s == T + rp
         want = y if res is None else y + resid
@@ -117,7 +118,7 @@ def test_fsmn_stream_slots_rows_equal_whole_sequence_rows_bitwise():
 
 
 @pytest.mark.parametrize("H", [128, 40])
-def test_lstm_stream_slots_carries_state_across_uneven_chunks(H):
+def test_lstm_stream_slots_masked_carries_state_across_uneven_chunks(H):
     lib = _lib.load()
     B, L, D = 3, 37, 64
     torch.manual_seed(11)
@@ -129,11 +130,14 @@ def test_lstm_stream_slots_carries_state_across_uneven_chunks(H):
     whh_t = lstm.weight_hh_l0.detach().t().contiguous().to(DEV)
     state = torch.zeros(B, 2, H, device=DEV)
     h = torch.empty(B, L, H, device=DEV)
-    frame0 = torch.zeros(B, dtype=torch.int32, device=DEV)
+    lengths = torch.full((B,), L, dtype=torch.int32, device=DEV)
+    done = torch.zeros(B, dtype=torch.int32, device=DEV)
+    m = KtStreamMask(lengths=ptr(lengths, True), frames_done=ptr(done, True), rows_per_frame=1, lag=0)
     t0 = 0
     for f in (5, 1, 13, 2, 16):
+        done.fill_(t0)
         check(lib.kt_lstm_stream_slots(ptr(gx) + 4 * t0 * 4 * H, ptr(whh_t), ptr(state), ptr(h) + 4 * t0 * H,
-                                       ptr(frame0, True), t0, B, f, H, L, L, stream_ptr()), "kt_lstm_stream_slots")
+                                       ctypes.byref(m), B, f, H, L, L, stream_ptr()), "kt_lstm_stream_slots")
         t0 += f
     assert t0 == L
     err = rel_l2(h.cpu(), want)

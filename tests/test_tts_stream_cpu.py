@@ -118,11 +118,12 @@ def test_plan_windows_keep_the_history_their_readers_need():
     assert all(win[n]["history"] == 0 for n in ("mid", "gates", "h", "out"))
 
 
-def test_launches_per_chunk_follow_from_the_shapes():
-    # per FSMN layer: two feed-forward convs + the memory block; LSTM input projection, LSTM, output Linear; one advance
-    assert PostNetStreamPlan(_yaml_postnet()).launches_per_chunk == 3 * 4 + 3 + 1
+def test_launches_per_chunk_include_the_output_mask():
+    # per FSMN layer: two feed-forward convs + the memory block; LSTM input projection, LSTM, output Linear; one advance;
+    # one output mask
+    assert PostNetStreamPlan(_yaml_postnet()).launches_per_chunk == 3 * 4 + 3 + 1 + 1
     for layers in (1, 2, 3):
-        assert PostNetStreamPlan(PostNet(dict(SMALL, postnet_fsmn_num_layers=layers)).eval()).launches_per_chunk == 3 * layers + 4
+        assert PostNetStreamPlan(PostNet(dict(SMALL, postnet_fsmn_num_layers=layers)).eval()).launches_per_chunk == 3 * layers + 5
 
 
 def test_plan_rejects_what_it_cannot_stream():
