@@ -199,11 +199,10 @@ int kt_stft_mel_fwd(const KtMelDesc* d, const float* wav, const float* window, c
 int kt_stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, const float* spec,
                     const float* window, const float* melmat, float* dwav, void* stream);
 
-/* out[0] = scale * sum |a - b|  (F.l1_loss numerator; loss.py:249,309); out[0] is overwritten. */
-int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, void* stream);
-/* out[0] += scale * sum |a - b|: one accumulator for a whole feature pyramid (FeatureMatchLoss, loss.py:217-256); the caller
- * zeroes out[0] once. */
-int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float* out, void* stream);
+/* accumulate == 0: out[0] = scale * sum |a - b|  (F.l1_loss numerator; loss.py:249,309); out[0] is overwritten.
+ * accumulate != 0: out[0] += scale * sum |a - b|: one accumulator for a whole feature pyramid (FeatureMatchLoss,
+ * loss.py:217-256); the caller zeroes out[0] once. */
+int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, int32_t accumulate, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * SAM-BERT acoustic model (kantts/models/sambert).  Activations are (B, L, C) rows -- the
@@ -397,15 +396,26 @@ typedef struct KtStreamWin {
   int32_t out_pitch, out_first;
   int32_t res_pitch, res_first;
 } KtStreamWin;
+/* Streams of a NON-CAUSAL generator and of the post-net: each window trails the pushed frames by `lag` rows (its chunk row t
+ * of item b is utterance row u = frames_done[b] * rows_per_frame - lag + t), and each batch slot holds an utterance of
+ * lengths[b] frames.  KtStreamMask describes the input window of one conv call: pass it as `m` to the stream forward, which
+ * then reads a tap of item b as zero unless 0 <= u < lengths[b] * rows_per_frame -- the whole-utterance forward's zero
+ * padding, applied per slot.  lengths and frames_done are device int32 [batch]; the conv calls only read frames_done. */
+typedef struct KtStreamMask {
+  const int32_t* lengths;
+  int32_t* frames_done;
+  int32_t rows_per_frame, lag;
+} KtStreamMask;
 /* Forward of one chunk.  The descriptor is the layer's with t_in / t_out = the chunk's rows (nsub == 1): a tap before the
  * chunk reads the window's earlier rows, down to -in_first, where the whole-sequence forward reads its zero padding; a
  * nearest-upsampled conv reads input row floor(t / upsample) of the same window.  The output goes to rows
- * out_first + [0, t_out) of each item's output window.  _tc_stream: the register-staged tensor-core kernel
- * (kt_conv1d_tc_plan(d, KT_PLAN_STREAM) != 0; no workspace), `wimg` = the forward image of that N tile. */
-int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd, const float* bias,
-                         const float* resid, float* y, void* stream);
-int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg, const float* bias,
-                            const float* resid, float* y, void* stream);
+ * out_first + [0, t_out) of each item's output window.  `m`: the input window's utterance bounds (KtStreamMask), or NULL
+ * for none.  _tc_stream: the register-staged tensor-core kernel (kt_conv1d_tc_plan(d, KT_PLAN_STREAM) != 0; no
+ * workspace), `wimg` = the forward image of that N tile. */
+int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                         const float* w_fwd, const float* bias, const float* resid, float* y, void* stream);
+int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                            const void* wimg, const float* bias, const float* resid, float* y, void* stream);
 /* kt_conv1d_tc_plan / kt_conv1d_tc_workspace / kt_debug_conv_tc_plan: direction flag of the stream forward (OR'd into dir 0):
  * the plan of kt_conv1d_fwd_tc_stream, which always takes the register-staged route. */
 #define KT_PLAN_STREAM 16
@@ -427,21 +437,6 @@ typedef struct KtWindow {
 int kt_stream_advance(const KtWindow* windows, int32_t n, int32_t batch, int32_t frames, int32_t max_channels, void* stream);
 /* ONE launch: rows [0, history) of every window are zeroed for the batch items b with slots[b] != 0 (device uint8 [batch]). */
 int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uint8_t* slots, int32_t max_channels, void* stream);
-/* Streams of a NON-CAUSAL generator and of the post-net: each window trails the pushed frames by `lag` rows (its chunk row t
- * of item b is utterance row u = frames_done[b] * rows_per_frame - lag + t), and each batch slot holds an utterance of
- * lengths[b] frames.  KtStreamMask describes the input window of one conv call: the _masked conv entry points read a tap
- * of item b as zero unless 0 <= u < lengths[b] * rows_per_frame -- the whole-utterance forward's zero padding, applied
- * per slot -- and otherwise take exactly the arguments of kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream.  lengths and
- * frames_done are device int32 [batch]; the conv calls only read frames_done. */
-typedef struct KtStreamMask {
-  const int32_t* lengths;
-  int32_t* frames_done;
-  int32_t rows_per_frame, lag;
-} KtStreamMask;
-int kt_conv1d_fwd_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
-                                const float* w_fwd, const float* bias, const float* resid, float* y, void* stream);
-int kt_conv1d_fwd_tc_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
-                                   const void* wimg, const float* bias, const float* resid, float* y, void* stream);
 /* ONE launch at the end of a chunk of `frames` frames: rows [first, first + rows) of each item's window y (`ch` channels,
  * `pitch` rows per item), described by m, are zeroed where their utterance row lies outside the utterance; then
  * frames_done[b] += frames for every item. */

@@ -85,8 +85,7 @@ PROTOTYPES = {
     "kt_dwt_db3_bwd": [_P, _P, _I, _I, _P],
     "kt_stft_mel_fwd": [ctypes.POINTER(KtMelDesc), _P, _P, _P, _P, _P, _P, _P],
     "kt_stft_mel_bwd": [ctypes.POINTER(KtMelDesc), _P, _P, _P, _P, _P, _P, _P],
-    "kt_l1_sum": [_P, _P, _L, _F, _P, _P],
-    "kt_l1_sum_acc": [_P, _P, _L, _F, _P, _P],
+    "kt_l1_sum": [_P, _P, _L, _F, _P, _I, _P],
     "kt_conv1d_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_conv1d_tc_image_bytes": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_weight_pack_tc": [ctypes.POINTER(KtConv1dDesc), _I, _P, _P, _P],
@@ -122,16 +121,14 @@ PROTOTYPES = {
     "kt_attn_ctc_fwd": [_P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P],
     "kt_attn_ctc_bwd": [_P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _F, _P],
     "kt_attn_prior": [_P, _P, _P, _I, _I, _I, _P],
-    "kt_conv1d_fwd_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
-    "kt_conv1d_fwd_tc_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_fwd_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask),
+                             _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_fwd_tc_stream": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask),
+                                _P, _P, _P, _P, _P, _P],
     "kt_sinadd_fwd_win": [_P, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_add3_scale_win": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_stream_advance": [_P, _I, _I, _I, _I, _P],
     "kt_stream_reset": [_P, _I, _I, _P, _I, _P],
-    "kt_conv1d_fwd_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask),
-                                    _P, _P, _P, _P, _P, _P],
-    "kt_conv1d_fwd_tc_stream_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamWin),
-                                       ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P],
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _I, _I, _I, _I,
                                  _I, _P],

@@ -170,7 +170,7 @@ __device__ __forceinline__ void stream_utterance_rows(const KtStreamMask& m, int
 int validate_conv(const KtConv1dDesc* d);
 // validate_conv plus the window placement of one stream chunk (kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream)
 int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what);
-// the KtStreamMask of a _masked stream call
+// the KtStreamMask of a masked stream call
 int validate_stream_mask(const KtStreamMask* m, const char* what);
 Phase gather_phase(int t_out, int kernel, int stride, int dil, int pad, int up);
 std::vector<Phase> conv_phases(const KtConv1dDesc* d, int dir);

@@ -45,7 +45,7 @@ struct CoreParams {
   Phase ph;
   // stream instances (kt_conv1d_fwd_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
   int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
-  // masked stream instances (kt_conv1d_fwd_stream_masked): the input window's utterance bounds per item
+  // masked stream instances (kt_conv1d_fwd_stream with a mask): the input window's utterance bounds per item
   KtStreamMask smask;
 };
 
@@ -679,9 +679,15 @@ extern "C" int kt_conv1d_fwd(const KtConv1dDesc* d, const float* x, const float*
   return KT_OK;
 }
 
-// The forward's phases over the windows of one stream chunk; m: the input's utterance bounds (masked instances), or null
-static int conv_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x, const float* w_fwd,
-                       const float* bias, const float* resid, float* y, cudaStream_t st) {
+// One chunk of a stream (KtStreamWin): the forward's phases over the windows; m: the input's utterance bounds (masked
+// instances), or null
+extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                    const float* w_fwd, const float* bias, const float* resid, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
+  if (!rc && m) rc = validate_stream_mask(m, "kt_conv1d_fwd_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
   CoreParams p{};
   p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   p.w = w_fwd; p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
@@ -693,31 +699,10 @@ static int conv_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStre
   if (m) p.smask = *m;
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
-    const int rc = m ? run_core<true, true>(p, st) : run_core<true>(p, st);
+    rc = m ? run_core<true, true>(p, st) : run_core<true>(p, st);
     if (rc) return rc;
   }
   return KT_OK;
-}
-
-// One chunk of a stream (KtStreamWin): the forward's phases over the windows
-extern "C" int kt_conv1d_fwd_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const float* w_fwd,
-                                    const float* bias, const float* resid, float* y, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream");
-  if (rc) return rc;
-  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream: null pointer");
-  return conv_stream(d, w, nullptr, x, w_fwd, bias, resid, y, st);
-}
-
-// The same over the utterance rows of each item only (KtStreamMask)
-extern "C" int kt_conv1d_fwd_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
-                                           const float* w_fwd, const float* bias, const float* resid, float* y, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_stream_masked");
-  if (!rc) rc = validate_stream_mask(m, "kt_conv1d_fwd_stream_masked");
-  if (rc) return rc;
-  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_stream_masked: null pointer");
-  return conv_stream(d, w, m, x, w_fwd, bias, resid, y, st);
 }
 
 extern "C" int kt_conv1d_bwd_data(const KtConv1dDesc* d, const float* dy, const float* y, const float* w_bwd, const float* x,

@@ -139,7 +139,7 @@ struct TcParams {
   // traffic, see conv_tc_kernel; 0: straight from the accumulator registers (stream chunks, channel counts % 4 != 0,
   // operands not 16-byte aligned)
   int epi_staged;
-  // masked stream instances (kt_conv1d_fwd_tc_stream_masked): the input window's utterance bounds per item
+  // masked stream instances (kt_conv1d_fwd_tc_stream with a mask): the input window's utterance bounds per item
   KtStreamMask smask;
 };
 
@@ -855,12 +855,17 @@ extern "C" int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const voi
   return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", static_cast<cudaStream_t>(stream));
 }
 
-// The register-staged route over the windows of one stream chunk; m: the input's utterance bounds (masked instances), or null
-static int conv_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x, const void* wimg,
-                          const float* bias, const float* resid, float* y, const char* what, cudaStream_t st) {
+// One chunk of a stream (KtStreamWin): the register-staged route over the windows; m: the input's utterance bounds (masked
+// instances), or null
+extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
+                                       const void* wimg, const float* bias, const float* resid, float* y, void* stream) {
+  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
+  if (!rc && m) rc = validate_stream_mask(m, "kt_conv1d_fwd_tc_stream");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
   const TcPlan P = make_tc_plan_flags(d, KT_PLAN_STREAM);
-  KT_REQUIRE(P.ok && !P.tma, "%s: layer not supported by the tensor-core path", what);
-  KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "%s: bad window pitch", what);
+  KT_REQUIRE(P.ok && !P.tma, "kt_conv1d_fwd_tc_stream: layer not supported by the tensor-core path");
+  KT_REQUIRE(w->in_pitch > 0 && w->out_pitch > 0, "kt_conv1d_fwd_tc_stream: bad window pitch");
   TcParams io{};
   io.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
   io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
@@ -869,26 +874,7 @@ static int conv_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const KtS
   io.in_pitch = w->in_pitch; io.in_first = w->in_first; io.out_pitch = w->out_pitch; io.out_first = w->out_first;
   io.res_pitch = w->res_pitch; io.res_first = w->res_first;
   if (m) io.smask = *m;
-  return run_plan(P, io, nullptr, 0, what, st);
-}
-
-// One chunk of a stream (KtStreamWin): the register-staged route over the windows
-extern "C" int kt_conv1d_fwd_tc_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* x, const void* wimg,
-                                       const float* bias, const float* resid, float* y, void* stream) {
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream");
-  if (rc) return rc;
-  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream: null pointer");
-  return conv_tc_stream(d, w, nullptr, x, wimg, bias, resid, y, "conv1d_fwd_tc_stream", static_cast<cudaStream_t>(stream));
-}
-
-// The same over the utterance rows of each item only (KtStreamMask)
-extern "C" int kt_conv1d_fwd_tc_stream_masked(const KtConv1dDesc* d, const KtStreamWin* w, const KtStreamMask* m, const float* x,
-                                              const void* wimg, const float* bias, const float* resid, float* y, void* stream) {
-  int rc = validate_stream(d, w, resid, "kt_conv1d_fwd_tc_stream_masked");
-  if (!rc) rc = validate_stream_mask(m, "kt_conv1d_fwd_tc_stream_masked");
-  if (rc) return rc;
-  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_stream_masked: null pointer");
-  return conv_tc_stream(d, w, m, x, wimg, bias, resid, y, "conv1d_fwd_tc_stream_masked", static_cast<cudaStream_t>(stream));
+  return run_plan(P, io, nullptr, 0, "kt_conv1d_fwd_tc_stream", static_cast<cudaStream_t>(stream));
 }
 
 int conv1d_bwd_data_tc(const KtConv1dDesc* d, const float* dy, const float* y, const void* wimg, const float* x,

@@ -369,7 +369,9 @@ extern "C" int kt_dwt_db3_bwd(const float* dy, float* dx, int32_t batch, int32_t
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
-static int l1_sum(const float* a, const float* b, long long n, float scale, float* out, cudaStream_t st, bool accumulate) {
+extern "C" int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, int32_t accumulate,
+                         void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(out && n >= 0 && (n == 0 || (a && b)), "l1_sum: bad arguments");   // an empty tensor has no data pointer
   if (n == 0) {
     if (!accumulate) KT_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
@@ -384,12 +386,6 @@ static int l1_sum(const float* a, const float* b, long long n, float scale, floa
   rc = split_sum(part, 1, blocks, 1, out, accumulate, st);
   if (rc) return rc;
   return scratch_free(part, st);
-}
-extern "C" int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, void* stream) {
-  return l1_sum(a, b, n, scale, out, static_cast<cudaStream_t>(stream), false);
-}
-extern "C" int kt_l1_sum_acc(const float* a, const float* b, int64_t n, float scale, float* out, void* stream) {
-  return l1_sum(a, b, n, scale, out, static_cast<cudaStream_t>(stream), true);
 }
 
 }  // namespace kt

@@ -733,8 +733,8 @@ class GeneratorStreamer:
     lengths[b] are ignored.  ``finish()`` pushes the ``drain_frames`` frames that bring out an utterance's last sample.
     The chunks of slot b concatenated and cut to [delay, delay + lengths[b] * hop) equal the forward on the slot's mel of
     exactly lengths[b] frames: every layer's zero padding at the utterance's end is applied per slot inside the conv
-    kernels (the _masked entry points), from the slots' utterance record (stream.SlotUtterances).  A slot reset before its
-    utterance has drained loses the samples not yet returned.
+    kernels (the stream conv's KtStreamMask), from the slots' utterance record (stream.SlotUtterances).  A slot reset
+    before its utterance has drained loses the samples not yet returned.
 
     NSF generator: ``push`` takes (B, in_channels + 2, f) -- mel, f0 in Hz and the voiced flag, as ``forward`` -- and each
     slot's excitation is seeded by its ``seeds`` entry (``reset`` takes the new slots' seeds).  The excitation is computed

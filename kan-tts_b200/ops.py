@@ -576,18 +576,17 @@ def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None, mask=None):
     by ``win`` (a KtStreamWin), and ``t_in`` is the chunk's input rows; the taps before the chunk read the window's history.
     ``pw``: the layer's PreparedWeight, prepared by the caller.  Planned once per chunk shape (ConvSpec.plan, stream=True);
     the tensor-core image of the plan's N tile is packed from ``pw`` on its first use.  ``mask`` (a KtStreamMask): the
-    input rows outside each item's utterance read as zeros (the _masked entry points)."""
+    input rows outside each item's utterance read as zeros."""
     plan = spec.plan(x.shape[0], 1, t_in, stream=True)
     d, nt = plan.d, plan.tile(0)
-    m = () if mask is None else (ctypes.byref(mask),)
-    sfx = "" if mask is None else "_masked"
+    m = None if mask is None else ctypes.byref(mask)
     if nt:
         img = pw.image((0, nt), d)
-        _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream" + sfx, ctypes.byref(d), ctypes.byref(win), *m, ptr(x),
+        _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream", ctypes.byref(d), ctypes.byref(win), m, ptr(x),
                                             ptr(img, True), ptr(bias), ptr(resid), ptr(y)))
     else:
         n = spec.stride if spec.transposed else 1
-        _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream" + sfx, ctypes.byref(d), ctypes.byref(win), *m, ptr(x),
+        _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_stream", ctypes.byref(d), ctypes.byref(win), m, ptr(x),
                                               ptr(pw.w_fwd), ptr(bias), ptr(resid), ptr(y)))
 
 
@@ -820,12 +819,12 @@ class StftMelFn(torch.autograd.Function):
 def l1_sum_acc(out, a, b, scale):
     """out += scale * sum|a - b| (0-dim device accumulator zeroed by the caller; one launch)."""
     a, b = a.contiguous(), b.contiguous()
-    call("kt_l1_sum_acc", ptr(a), ptr(b), a.numel(), float(scale), ptr(out))
+    call("kt_l1_sum", ptr(a), ptr(b), a.numel(), float(scale), ptr(out), 1)
 
 
 def l1_sum(a, b, scale=1.0):
     """scale * sum|a - b| -> 0-dim tensor (no autograd; feature-matching value, loss.py:249)."""
     a, b = a.contiguous(), b.contiguous()
     out = torch.empty((), device=a.device, dtype=torch.float32)
-    call("kt_l1_sum", ptr(a), ptr(b), a.numel(), float(scale), ptr(out), launches=2)
+    call("kt_l1_sum", ptr(a), ptr(b), a.numel(), float(scale), ptr(out), 0, launches=2)
     return out

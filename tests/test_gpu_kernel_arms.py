@@ -31,9 +31,11 @@ def _ops():
     return ops
 
 
-def _profiled(fn, leaves=()):
-    """-> (fn(), names of the CUDA kernels it launched).  Should the profiler deliver no kernel record at all, fn runs
-    again, with the gradients of `leaves` cleared first."""
+def _profiled(fn, kernels, leaves=()):
+    """-> fn(), checked by torch.profiler to launch, for each name in `kernels`, a CUDA kernel whose name contains it.
+    The profiler can deliver a run's kernel records incompletely (none at all, or without some launches), so a run
+    whose records miss one of `kernels` is repeated, up to three runs, with the gradients of `leaves` cleared first.
+    The dispatch is deterministic: a kernel that is not the arm which runs is missing from every run and fails."""
     for _ in range(3):
         for t in leaves:
             t.grad = None
@@ -41,12 +43,8 @@ def _profiled(fn, leaves=()):
             out = fn()
             torch.cuda.synchronize()
         names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
-        if names:
-            break
-    return out, names
-
-
-def _assert_ran(names, *kernels):
+        if all(any(k in n for n in names) for k in kernels):
+            return out
     for k in kernels:
         assert any(k in n for n in names), (k, sorted(n for n in names if k.split("<")[0] in n))
 
@@ -106,8 +104,8 @@ def test_self_attention_arm_matches_float64(D, L, rw):
         (o * r.to(DEV)).sum().backward()
         return o, a
 
-    (o, a), names = _profiled(run, [qg])
-    _assert_ran(names, f"attn_fwd_kernel<{D}, {rw}>", f"attn_bwd_q_kernel<{D}, {rw}>", f"attn_bwd_kv_kernel<{D}>")
+    o, a = _profiled(run, [f"attn_fwd_kernel<{D}, {rw}>", f"attn_bwd_q_kernel<{D}, {rw}>", f"attn_bwd_kv_kernel<{D}>"],
+                     [qg])
     # forward: a D-term dot product, a softmax over Lk and an Lk-term P V sum per output
     assert rel_l2(o.cpu(), o_ref) < 5e-6, rel_l2(o.cpu(), o_ref)
     assert rel_l2(a.cpu(), a_ref) < 5e-6, rel_l2(a.cpu(), a_ref)
@@ -135,8 +133,7 @@ def test_self_attention_dropout_arm_matches_float64():
         (o * r.to(DEV)).sum().backward()
         return o, a
 
-    (o, a), names = _profiled(run, [qg])
-    _assert_ran(names, "attn_fwd_kernel<8, 2>", "attn_bwd_q_kernel<8, 2>")
+    o, a = _profiled(run, ["attn_fwd_kernel<8, 2>", "attn_bwd_q_kernel<8, 2>"], [qg])
     assert rel_l2(o.cpu(), o_ref) < 5e-6
     assert rel_l2(a.cpu(), a_ref) < 5e-6
     assert rel_l2(qg.grad.cpu(), qr.grad) < 2e-5, rel_l2(qg.grad.cpu(), qr.grad)
@@ -167,8 +164,7 @@ def test_pnca_attention_pair_arm_matches_float64(D, Lh, rw):
         ((out[0] * rx.to(DEV)).sum() + (out[1] * rh.to(DEV)).sum()).backward()
         return out
 
-    (ox, oh, ax, ah), names = _profiled(run, [xg, hg])
-    _assert_ran(names, f"attn_fwd_kernel<{D}, {rw}>", f"attn_bwd_q_kernel<{D}, {rw}>")
+    ox, oh, ax, ah = _profiled(run, [f"attn_fwd_kernel<{D}, {rw}>", f"attn_bwd_q_kernel<{D}, {rw}>"], [xg, hg])
     for name, got, want in (("ox", ox, ox_ref), ("oh", oh, oh_ref), ("ax", ax, ax_ref), ("ah", ah, ah_ref)):
         assert rel_l2(got.cpu(), want) < 5e-6, (name, rel_l2(got.cpu(), want))
     for name, got, want in (("dq", xg.grad[..., :hd], xr.grad[..., :hd]), ("dx_kv", xg.grad[..., hd:], xr.grad[..., hd:]),
@@ -198,8 +194,7 @@ def test_layernorm_arm_matches_float64(rows, c, nc):
         (y.view(rows, c) * r.to(DEV)).sum().backward()
         return y
 
-    y, names = _profiled(run, [xg, wg, bg])
-    _assert_ran(names, f"layernorm_fwd_kernel<{nc}>", f"layernorm_bwd_kernel<{nc}>")
+    y = _profiled(run, [f"layernorm_fwd_kernel<{nc}>", f"layernorm_bwd_kernel<{nc}>"], [xg, wg, bg])
     assert rel_l2(y.view(rows, c).cpu(), yr) < 2e-6, rel_l2(y.view(rows, c).cpu(), yr)        # C-term mean / variance
     assert rel_l2(xg.grad.cpu(), xr.grad) < 1e-5, rel_l2(xg.grad.cpu(), xr.grad)
     assert rel_l2(wg.grad.cpu(), wr.grad) < 1e-5, rel_l2(wg.grad.cpu(), wr.grad)              # rows-term column sums
@@ -238,8 +233,7 @@ def test_fsmn_arm_matches_float64(K, lp, tj):
         (y * r.to(DEV)).sum().backward()
         return y
 
-    y, names = _profiled(run, [xg, wg])
-    _assert_ran(names, "fsmn_fir_kernel", f"fsmn_bwd_weight_kernel<{tj}>")
+    y = _profiled(run, ["fsmn_fir_kernel", f"fsmn_bwd_weight_kernel<{tj}>"], [xg, wg])
     assert rel_l2(y.cpu(), yr) < 2e-6, rel_l2(y.cpu(), yr)                        # K-term FIR
     assert rel_l2(xg.grad.cpu(), xr.grad) < 1e-5, rel_l2(xg.grad.cpu(), xr.grad)
     assert rel_l2(wg.grad.cpu(), wr.grad) < 1e-5, rel_l2(wg.grad.cpu(), wr.grad)  # B*T-term sums
@@ -292,8 +286,7 @@ def test_ar_duration_predictor_matches_float64(cu, pre, H, B, L):
     cond = torch.randn(B, L, cu)
     want = _ar_duration_ref(m, cond.to(F64))
     m = m.to(DEV)
-    got, names = _profiled(lambda: m.infer(cond.to(DEV)))
-    _assert_ran(names, "ar_duration_kernel")
+    got = _profiled(lambda: m.infer(cond.to(DEV)), ["ar_duration_kernel"])
     assert float(want.abs().max()) > 0.1
     # each step: P1-, P2- and (P2 + H)-term dot products, an error that the recurrence carries through L steps
     assert rel_l2(got.cpu(), want) < 2e-5, rel_l2(got.cpu(), want)
@@ -375,7 +368,7 @@ def test_thin_conv_arm_matches_float64(name):
     def fwd():
         return ops.conv(xg, spec, ops.PreparedWeight(), vg, g2, bg)
 
-    y, names_f = _profiled(fwd)
+    y = _profiled(fwd, [kernel.format("fwd")])
     if slope is not None:
         # outputs whose sign differs between fp32 and float64 (|y| below the forward error) would switch the LeakyReLU's
         # slope in the gradient: leave exactly those out of the scalar both sides differentiate
@@ -383,9 +376,7 @@ def test_thin_conv_arm_matches_float64(name):
         assert float(flip.double().mean()) < 1e-3
         r = r * (~flip)
     (yo * r.to(F64)).sum().backward()
-    _, names_b = _profiled(lambda: (y * rows(r).to(DEV)).sum().backward(retain_graph=True), [xg, vg, g2, bg])
-    _assert_ran(names_f, kernel.format("fwd"))
-    _assert_ran(names_b, kernel.format("wgrad"))
+    _profiled(lambda: (y * rows(r).to(DEV)).sum().backward(retain_graph=True), [kernel.format("wgrad")], [xg, vg, g2, bg])
     assert rel_l2(unrows(y).cpu(), yo) < 2e-6, rel_l2(unrows(y).cpu(), yo)          # k-term FIR
     assert rel_l2(unrows(xg.grad).cpu(), xo.grad) < 1e-4, rel_l2(unrows(xg.grad).cpu(), xo.grad)
     # B*T_out*nsub-term sums per tap, then the weight-norm backward
@@ -483,8 +474,7 @@ def test_stft_mel_matches_float64(n_fft, hop, win, T, pad_mode, mel):
         (o * r.to(DEV)).sum().backward()
         return o
 
-    out, names = _profiled(run, [wg])
-    _assert_ran(names, "stft_mel_fwd_kernel", "stft_mel_bwd_kernel", "ola_gather_kernel")
+    out = _profiled(run, ["stft_mel_fwd_kernel", "stft_mel_bwd_kernel", "ola_gather_kernel"], [wg])
     keep = ~near
     assert rel_l2(out.cpu()[keep], want[keep]) < 1e-5, rel_l2(out.cpu()[keep], want[keep])
     dw = wg.grad.cpu()
@@ -622,13 +612,11 @@ def test_l1_sum_matches_float64(n, offset, kernel):
     a, b = torch.randn(n, generator=g), torch.randn(n, generator=g)
     ag, bg = _offset_view(a.to(DEV), offset), _offset_view(b.to(DEV), 2 * offset)
     want = 0.37 * float((a.to(F64) - b.to(F64)).abs().sum())
-    got, names = _profiled(lambda: ops.l1_sum(ag, bg, 0.37))
-    _assert_ran(names, "l1_sum_kernel", kernel + "(")
+    got = _profiled(lambda: ops.l1_sum(ag, bg, 0.37), ["l1_sum_kernel", kernel + "("])
     # per-thread running sums of ~n / (blocks * 256) terms, then block and split sums
     assert abs(float(got) - want) <= 1e-6 * want, (float(got), want)
     acc = torch.full((), 2.5, device=DEV)
-    _, names = _profiled(lambda: (acc.fill_(2.5), ops.l1_sum_acc(acc, ag, bg, 0.37)))
-    _assert_ran(names, kernel + "(")
+    _profiled(lambda: (acc.fill_(2.5), ops.l1_sum_acc(acc, ag, bg, 0.37)), [kernel + "("])
     assert abs(float(acc) - (2.5 + want)) <= 1e-6 * (2.5 + want), (float(acc), 2.5 + want)
 
 

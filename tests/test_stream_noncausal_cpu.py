@@ -199,14 +199,20 @@ def test_causal_plan_is_unchanged(name):
     assert {w["name"]: w["history"] for w in plan.windows}["wav"] == 0
 
 
-def test_stream_mask_descriptor_matches_header():
+def test_stream_mask_descriptor_and_argument_match_header():
     assert ctypes.sizeof(_lib.KtStreamMask) == 8 + 8 + 4 + 4
     header = open(os.path.join(ROOT, "include", "kantts_b200.h")).read()
     body = re.search(r"typedef struct KtStreamMask \{([^}]*)\} KtStreamMask;", header).group(1)
     fields = re.findall(r"(\w+)(?:,|;)", body)
     assert fields == [f for f, _ in _lib.KtStreamMask._fields_]
-    for name in ("kt_conv1d_fwd_stream_masked", "kt_conv1d_fwd_tc_stream_masked", "kt_stream_mask_advance"):
-        assert name in _lib.PROTOTYPES and re.search(rf"^int {name}\(", header, flags=re.M)
+    assert "kt_stream_mask_advance" in _lib.PROTOTYPES and re.search(r"^int kt_stream_mask_advance\(", header, flags=re.M)
+    # the utterance mask is the optional third argument of the one stream forward per route
+    for name in ("kt_conv1d_fwd_stream", "kt_conv1d_fwd_tc_stream"):
+        params = re.search(rf"^int {name}\(([^)]*)\);", header, flags=re.M).group(1).split(",")
+        assert " ".join(params[2].split()) == "const KtStreamMask* m", (name, params)
+        assert _lib.PROTOTYPES[name][2] is ctypes.POINTER(_lib.KtStreamMask), name
+    for name in ("kt_conv1d_fwd_stream_masked", "kt_conv1d_fwd_tc_stream_masked", "kt_l1_sum_acc"):
+        assert name not in _lib.PROTOTYPES and not re.search(rf"\b{name}\b", header), name
 
 
 def test_streamer_rejects_what_it_cannot_stream():
