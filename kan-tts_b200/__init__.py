@@ -10,7 +10,8 @@ Public surface = the reference's own module API for this path:
   train.SambertStep (Sambert_Trainer.train_step); data.AttnPriors (the MAS data path's alignment prior)
   sambert.KanTtsTextsyBERT + SeqCELoss, train.SybertStep, data.BertMasker (sybert.yaml: masked-symbol pretraining)
   infer.synthesize (symbols -> SAM-BERT free-running decode -> HiFi-GAN -> waveforms, no .npy hand-off)
-  infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs, causal generators)
+  infer.stream_synthesize (the same waveforms chunk by chunk while the decoder runs; non-causal generators with
+    allow_lookahead=True)
   infer.TtsServer (continuous batching: requests join and leave the slots of one running stream)
   speaker.DTDNN / kaldi_fbank / speaker_embedding (kantts.preprocess.se_processor: the SE flow's speaker embeddings)
   install.install() patches these into an importable KAN-TTS checkout.

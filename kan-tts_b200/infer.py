@@ -7,7 +7,10 @@ forward because its decoder masks only support batch 1), kantts/bin/infer_hifiga
 in one call; every utterance is cut at its own predicted length (frames x product of the up-sampling scales).
 
 ``stream_synthesize`` gives the same waveforms chunk by chunk while the decoder runs: decoder steps -> streamed post-net
-(PostNet.streamer) -> streamed causal vocoder (Generator.streamer).
+(PostNet.streamer) -> streamed vocoder (Generator.streamer).  A non-causal vocoder streams with ``allow_lookahead=True``:
+its output waits for its look-ahead (``lookahead`` samples, 3424 = 214 ms for the 16 kHz yamls), and each utterance's
+audio equals the generator run on exactly that utterance's post-net frames, the reference's hand-off
+(infer_sambert.py:136-138 then infer_hifigan.py).
 
 An NSF acoustic model (``num_mels`` = mel + f0 + voiced flag) drives an NSF generator with ``nsf_f0`` and ``nsf_seeds``: the
 f0 channel is denormalised and the voiced flag binarised as the reference's hand-off does (kantts/bin/infer_sambert.py:26-56
@@ -54,6 +57,17 @@ def _check_nsf(sambert_num_mels, generator, nsf_f0, nsf_seeds, what):
     return True
 
 
+def stream_lookahead(generator, allow_lookahead, what):
+    """-> the samples by which ``generator`` streams each sample late (StreamPlan.delay; 0 for a causal generator).
+    ValueError for a generator that does not stream (StreamPlan: multi-band, training mode), and for a non-causal one
+    unless ``allow_lookahead``: its look-ahead adds to every utterance's time to first audio, so the caller opts in."""
+    plan = StreamPlan(generator)
+    if not plan.causal and not allow_lookahead:
+        raise ValueError(f"{what} needs a causal generator: a non-causal one reads {plan.delay} samples ahead of every "
+                         "output sample; allow_lookahead=True accepts that delay")
+    return plan.delay
+
+
 @torch.no_grad()
 def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None):
     """sambert: ``KanTtsSAMBERT`` in eval(); generator: ``Generator`` in eval() (``remove_weight_norm()`` optional --
@@ -83,20 +97,21 @@ def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, 
 
 
 def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps=4,
-                      nsf_f0=None, nsf_seeds=None):
+                      nsf_f0=None, nsf_seeds=None, allow_lookahead=False):
     """Streaming ``synthesize``: the encoder, the variance adaptor and the decoder memory run now, then iterating the
     returned TtsStream decodes ``chunk_steps`` decoder steps at a time and yields their audio as soon as the post-net rows
-    are final.  The generator must be causal; an NSF one needs ``nsf_f0`` and ``nsf_seeds`` (as ``synthesize``), applied to
-    each chunk of post-net rows.  For every slot b, the yielded chunks concatenated and cut at ``lengths[b]`` are
-    ``synthesize(..., nsf_f0, nsf_seeds)[0][b]``."""
+    are final.  An NSF generator needs ``nsf_f0`` and ``nsf_seeds`` (as ``synthesize``), applied to each chunk of post-net
+    rows.  For every slot b, the yielded chunks concatenated and cut at ``lengths[b]`` are
+    ``synthesize(..., nsf_f0, nsf_seeds)[0][b]`` for a causal generator.
+    A non-causal generator is refused unless ``allow_lookahead``: its audio then comes ``TtsStream.lookahead`` samples
+    later, and slot b's is the generator run on exactly its ``lengths[b] / hop`` post-net frames (the reference's
+    hand-off; ``synthesize`` runs it on the batch's padded mel instead, which changes an utterance's last samples)."""
     if sambert.training or generator.training:
         raise RuntimeError("stream_synthesize() expects both models in eval() mode")
-    StreamPlan(generator)
     if generator.nsf_enable and (nsf_f0 is None or nsf_seeds is None):
         raise ValueError("stream_synthesize(): an NSF generator streams with nsf_f0 and nsf_seeds: its excitation must be "
                          "seeded for the chunks to reproduce the whole utterance")
-    if not generator.conv_pre.causal:                              # the vocoder streams here without a delay
-        raise ValueError("streaming needs a causal generator: a non-causal one reads ahead of every output sample")
+    stream_lookahead(generator, allow_lookahead, "streaming")
     num_mels = sambert.mel_postnet.num_mels
     nsf = _check_nsf(num_mels, generator, nsf_f0, nsf_seeds, "stream_synthesize()")     # checks the NSF channels
     if not nsf and generator.conv_pre.conv1d.spec.c_in != num_mels:
@@ -113,9 +128,12 @@ class TtsStream:
     """The audio of one batch of utterances, chunk by chunk (made by ``stream_synthesize``).
 
     ``lengths``: per-slot sample counts, ``LR_length_rounded[b] * hop`` (read on the host once, before decoding).
-    Iterating yields ``(start_sample, wav)``, ``wav`` (B, 1, n) on the device, n > 0; slot b's audio ends at lengths[b] and
-    is padding after that.  From the first chunk to the last no device data is read on the host.  A stream is iterated
-    once."""
+    ``lookahead``: the vocoder's delay in samples (GeneratorStreamer.delay; 0 for a causal one): the push of the frames
+    [p, p + f) returns the samples [p·hop - lookahead, (p + f)·hop - lookahead), and the samples before 0 are not
+    yielded; after the last decoder step the vocoder's drain (GeneratorStreamer.finish) brings out the rest.
+    Iterating yields ``(start_sample, wav)``, ``wav`` (B, 1, n) on the device, n > 0, with starts contiguous from 0; slot
+    b's audio ends at lengths[b] and is padding after that.  From the first chunk to the last no device data is read on
+    the host.  A stream is iterated once."""
 
     def __init__(self, sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps,
                  nsf_f0=None, nsf_seeds=None):
@@ -130,15 +148,26 @@ class TtsStream:
         self.lengths = [int(n) * self.hop for n in frames.cpu()]
         self.max_frames = F = self.r * chunk_steps
         self._post = sambert.mel_postnet.streamer(B, F, frames)
-        self._voc = generator.streamer(batch=B, max_frames=F, seeds=nsf_seeds)
+        # a non-causal vocoder masks each slot's utterance end on the device, from the lengths the decoder masks by
+        self._voc = generator.streamer(batch=B, max_frames=F, lengths=None if generator.conv_pre.causal else frames,
+                                       seeds=nsf_seeds)
+        self.lookahead = self._voc.delay
         self._used = False
 
+    @staticmethod
+    def _audio(wav, start):
+        """The vocoder's output wav (B, 1, n) for the samples from ``start`` on -> [(start sample, wav)] without the samples
+        before 0 (none when it holds only those)."""
+        lo = max(0, -start)
+        return [(start + lo, wav[..., lo:])] if lo < wav.shape[-1] else []
+
     def _vocode(self, rows, start):
-        """rows (B, n, num_mels) of final post-net output -> [(start sample, wav)] in pieces of at most max_frames frames."""
+        """rows (B, n, num_mels) of final post-net output -> [(start sample, wav)] in pieces of at most max_frames frames,
+        and the start of the next piece."""
         out = []
         for piece in torch.split(rows, self.max_frames, dim=1):
             if piece.shape[1]:
-                out.append((start, self._voc.push(piece.transpose(1, 2))))
+                out += self._audio(self._voc.push(piece.transpose(1, 2)), start)
                 start += piece.shape[1] * self.hop
         return out, start
 
@@ -147,7 +176,7 @@ class TtsStream:
             raise RuntimeError("a TtsStream is iterated once")
         self._used = True
         f = self._front
-        steps, B, start, row = f["memory"].shape[1], self.batch, 0, 0
+        steps, B, start, row = f["memory"].shape[1], self.batch, -self.lookahead, 0
         outs = []
         with torch.no_grad():
             for s, (out, _, _) in enumerate(self.sambert.mel_decoder.infer_steps(f["memory"], f["x_band_width"],
@@ -168,17 +197,26 @@ class TtsStream:
                     rows = denorm_f0(rows, self.nsf_f0)
                 chunks, start = self._vocode(rows, start)
                 yield from chunks
+            if self.lookahead:
+                yield from self._audio(self._voc.finish(), start)
 
 
-def slot_schedule(r, chunk_steps, delay, frames, steps, chunk, max_steps):
+def slot_schedule(r, chunk_steps, delay, frames, steps, chunk, max_steps, hop=1, lookahead=0):
     """Where an utterance of ``frames`` post-net frames and ``steps`` decoder steps, admitted to a TtsServer slot for chunk
-    ``chunk``, runs (decoder rows are counted from row 0 of chunk 0; a chunk holds f = r * chunk_steps rows):
+    ``chunk``, runs (decoder rows are counted from row 0 of chunk 0; a chunk holds f = r * chunk_steps rows), into a
+    vocoder of ``hop`` samples per frame whose output lags by ``lookahead`` samples (0: a causal vocoder):
       start_step  the step of the admission chunk at which the slot decodes the utterance's step 0: ((-delay) mod f) / r,
                   so that its frame 0, which the post-net returns ``delay`` rows later, is output row 0 of a chunk
-      voc_chunk   that chunk: the slot's vocoder is reset just before it, and its audio starts there
-      last_chunk  the chunk that returns the utterance's last frame (its last audio)
+      voc_chunk   that chunk: the slot's vocoder is reset just before it.  Chunk voc_chunk + k returns the samples
+                  [k·f·hop - lookahead, (k + 1)·f·hop - lookahead) (``chunk_audio``): the first audio is in chunk
+                  voc_chunk + lookahead // (f·hop), from its sample lookahead mod (f·hop)
+      last_chunk  the chunk that returns the utterance's last sample: voc_chunk + (frames·hop - 1 + lookahead) // (f·hop),
+                  with no look-ahead the chunk that returns its last frame
       free_row    the first decoder row after the last frame became final and after the last decoder step
-      free_chunk  the first chunk that may admit the slot's next utterance: the chunk holding free_row, or the one after
+      free_chunk  the first chunk that may admit the slot's next utterance: the chunk holding free_row, or the one after,
+                  and late enough that the next utterance's voc_chunk (as far after its admission chunk as this one's) comes
+                  after last_chunk: a vocoder reset before the drain would lose the utterance's last samples.  With a
+                  look-ahead, free_chunk may come before last_chunk: the next utterance decodes while this one drains
     ValueError when delay is not a multiple of r (frame 0 could not start a chunk) or steps > max_steps."""
     if delay % r:
         raise ValueError(f"serving needs a post-net delay that is a multiple of the decoder's r: delay {delay}, r {r}")
@@ -189,8 +227,21 @@ def slot_schedule(r, chunk_steps, delay, frames, steps, chunk, max_steps):
     first = chunk * f + p0                                       # decoder row of frame 0
     last_row = first + frames - 1 + delay                        # its arrival makes the last frame final
     free_row = max(last_row, first + steps * r - 1) + 1
-    return dict(start_step=p0 // r, voc_chunk=(first + delay) // f, last_chunk=last_row // f, free_row=free_row,
-                free_chunk=-(-free_row // f))
+    voc_chunk = (first + delay) // f
+    # with lookahead 0 this is last_row // f (first + delay is a multiple of f), and the reset bound is below free_row's
+    last_chunk = voc_chunk + (frames * hop - 1 + lookahead) // (f * hop)
+    return dict(start_step=p0 // r, voc_chunk=voc_chunk, last_chunk=last_chunk, free_row=free_row,
+                free_chunk=max(-(-free_row // f), last_chunk + 1 - (voc_chunk - chunk)))
+
+
+def chunk_audio(voc_chunk, samples, chunk, chunk_samples, lookahead=0):
+    """The audio of an utterance of ``samples`` samples in chunk ``chunk``'s vocoder output of ``chunk_samples`` samples,
+    the utterance's frame 0 being row 0 of chunk ``voc_chunk`` and the vocoder's output lagging by ``lookahead`` samples
+    -> (start, lo, hi): the chunk's samples [lo, hi) are the utterance's [start, start + hi - lo); None when the chunk
+    holds none of them."""
+    first = (chunk - voc_chunk) * chunk_samples - lookahead
+    lo, hi = max(0, -first), min(chunk_samples, samples - first)
+    return (first + lo, lo, hi) if lo < hi else None
 
 
 class TtsServer:
@@ -202,19 +253,24 @@ class TtsServer:
     (wav 1-D on the device, cut at the request's end), ``finished`` the ids whose last audio this was.
 
     Each slot decodes its own utterance (SlotDecoder: its own step, memory length and band), through a per-slot post-net
-    streamer into the causal vocoder streamer.  A request's audio equals ``synthesize`` of that request alone (with its
+    streamer into the vocoder streamer.  A request's audio equals ``synthesize`` of that request alone (with its
     ``nsf_seed`` for an NSF generator), whatever the other slots hold.  Admission (at the start of a ``step``, for the queued
     requests that fit free slots) runs ``front_half`` per request and reads their frame counts on the host; between
-    admissions no call reads device data.  The alignment of each slot is ``slot_schedule``.  The generator must be causal;
-    ``nsf_f0`` (see ``denorm_f0``) is required for an NSF one."""
+    admissions no call reads device data.  The alignment of each slot is ``slot_schedule``.  ``nsf_f0`` (see
+    ``denorm_f0``) is required for an NSF generator.
 
-    def __init__(self, sambert, generator, slots, chunk_steps, max_steps, nsf_f0=None):
+    A non-causal generator is refused unless ``allow_lookahead``: each request's audio then comes ``lookahead`` samples
+    later (the vocoder's delay; 0 for a causal one) and equals the generator run on exactly that request's post-net
+    frames, the reference's hand-off.  A slot may start decoding its next request while the vocoder still drains the
+    previous one's last samples, timed so that its vocoder reset comes after them.  (``delay`` is the post-net's delay
+    in rows.)"""
+
+    def __init__(self, sambert, generator, slots, chunk_steps, max_steps, nsf_f0=None, allow_lookahead=False):
         from .sambert import PostNetStreamPlan
         if sambert.training or generator.training:
             raise RuntimeError("TtsServer expects both models in eval() mode")
-        StreamPlan(generator)
-        if not generator.conv_pre.causal:
-            raise ValueError("serving needs a causal generator: a non-causal one reads ahead of every output sample")
+        self.lookahead = stream_lookahead(generator, allow_lookahead, "serving")
+        self._causal = generator.conv_pre.causal
         num_mels = sambert.mel_postnet.num_mels
         self.nsf = generator.nsf_enable
         if self.nsf:
@@ -241,9 +297,12 @@ class TtsServer:
         with torch.no_grad():
             self._post = sambert.mel_postnet.streamer(self.batch, F, torch.zeros(self.batch, dtype=torch.int32,
                                                                                  device=self.device), per_slot=True)
-            self._voc = generator.streamer(batch=self.batch, max_frames=F,
+            # every slot is reset, with its request's frame count and seed, before its first audio
+            self._voc = generator.streamer(batch=self.batch, max_frames=F, lengths=None if self._causal else [1] * self.batch,
                                            seeds=[0] * self.batch if self.nsf else None)
-        self._queue, self._slots, self._chunk, self._next_id = [], [None] * self.batch, 0, 0
+        # _slots: each slot's current request (decoder and post-net); _playing: (slot, request) of every request whose
+        # audio has not all come out, which with a vocoder look-ahead can outlast its slot's hold on the decoder
+        self._queue, self._slots, self._playing, self._chunk, self._next_id = [], [None] * self.batch, [], 0, 0
 
     def submit(self, ling, emotion, speaker, length, nsf_seed=None):
         """Queue one utterance: ling (L, 4), emotion (L,) long tensors, speaker (L,) ids, or the (L, speaker_units) float
@@ -258,8 +317,9 @@ class TtsServer:
 
     @property
     def idle(self):
-        """No request queued or in a slot."""
-        return not self._queue and all(s is None or s["free_chunk"] <= self._chunk for s in self._slots)
+        """No request queued, in a slot or with audio still to come."""
+        return not self._queue and not self._playing and all(s is None or s["free_chunk"] <= self._chunk
+                                                               for s in self._slots)
 
     def _admit(self, c):
         free = [b for b, s in enumerate(self._slots) if s is None or s["free_chunk"] <= c]
@@ -273,7 +333,7 @@ class TtsServer:
         for req, fr, n in zip(take, fronts, frames):
             try:
                 sched.append(slot_schedule(self.r, self.chunk_steps, self.delay, n, fr["memory"].shape[1], c,
-                                           self.max_steps))
+                                           self.max_steps, hop=self.hop, lookahead=self.lookahead))
             except ValueError as e:
                 self._queue.remove(req)
                 raise ValueError(f"request {req['id']}: {e}") from None
@@ -282,7 +342,8 @@ class TtsServer:
             self._dec.admit(b, fr["memory"], fr["band_width_rows"])
             self._post.reset([n], slots=[b], start_row=s["start_step"] * self.r)
             seed = None if req["seed"] is None else torch.tensor([int(req["seed"])], dtype=torch.int64).to(self.device)
-            self._slots[b] = dict(s, chunk=c, id=req["id"], samples=n * self.hop, seed=seed)
+            self._slots[b] = dict(s, chunk=c, id=req["id"], frames=n, samples=n * self.hop, seed=seed)
+            self._playing.append((b, self._slots[b]))
 
     def step(self):
         """Run one chunk -> (audio, finished), see the class docstring."""
@@ -302,14 +363,17 @@ class TtsServer:
             due = [(b, s) for b, s in live if s["voc_chunk"] == c]
             if due:
                 seeds = torch.cat([s["seed"] for _, s in due]) if self.nsf else None
-                self._voc.reset([b for b, _ in due], seeds=seeds)
+                lengths = None if self._causal else [s["frames"] for _, s in due]
+                self._voc.reset([b for b, _ in due], lengths, seeds=seeds)
             wav = self._voc.push(post.transpose(1, 2))
         audio, finished = [], []
-        for b, s in live:
-            if s["voc_chunk"] <= c <= s["last_chunk"]:
-                start = (c - s["voc_chunk"]) * F * self.hop
-                audio.append((s["id"], start, wav[b, 0, :min(F * self.hop, s["samples"] - start)]))
+        for b, s in sorted(self._playing, key=lambda p: p[0]):
+            cut = chunk_audio(s["voc_chunk"], s["samples"], c, F * self.hop, self.lookahead)
+            if cut is not None:
+                start, lo, hi = cut
+                audio.append((s["id"], start, wav[b, 0, lo:hi]))
                 if c == s["last_chunk"]:
                     finished.append(s["id"])
+        self._playing = [(b, s) for b, s in self._playing if s["last_chunk"] > c]
         self._chunk += 1
         return audio, finished

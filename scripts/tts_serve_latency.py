@@ -1,8 +1,10 @@
 """Continuous batching (infer.TtsServer) against lockstep batches (infer.stream_synthesize) on the GPU.
 
 SAM-BERT with the sambert_24k.yaml network (seeded weights, about DUR frames per symbol) and the hifigan_v1_24k.yaml
-generator.  N requests of 16..96 symbols arrive at seeded Poisson times (mean gap --gap ms).  Both servers run on one host
-thread and deliver each chunk's audio to the host (a synchronize after each chunk):
+generator, or with ``--vocoder noncausal_16k`` the non-causal hifigan_noncausal_v1_16k.yaml generator (hop 200 at 16 kHz,
+served and streamed with ``allow_lookahead=True``: every request's audio waits for 214 ms of look-ahead).  N requests of
+16..96 symbols arrive at seeded Poisson times (mean gap --gap ms).  Both servers run on one host thread and deliver
+each chunk's audio to the host (a synchronize after each chunk):
   serve     TtsServer with B slots: requests are submitted when their arrival time has passed, one step() per chunk
   lockstep  whenever the previous batch has finished, the arrived requests (up to B) go through stream_synthesize as one batch
 Per server: time to first audio per request (arrival -> the first chunk holding its audio, p50 / p95, ms) and aggregate
@@ -10,7 +12,8 @@ audio seconds per wall second (all requests' audio / time from the first arrival
 cost: front_half of B requests one by one (as TtsServer admits them) against one padded batch.  Prints the card and
 its power limit, read in the same run, and the result as one JSON line.
 
-    python scripts/tts_serve_latency.py [--requests 32] [--slots 8] [--chunk-steps 4] [--gap 150] [--out DIR]"""
+    python scripts/tts_serve_latency.py [--vocoder causal_24k|noncausal_16k] [--requests 32] [--slots 8] [--chunk-steps 4]
+                                        [--gap 150] [--out DIR]"""
 import argparse
 import json
 import os
@@ -22,7 +25,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import kantts_b200 as K  # noqa: E402
-from tts_stream_latency import SR, card, models  # noqa: E402
+from tts_stream_latency import VOCODERS, card, models  # noqa: E402
 
 
 def requests(n, gap_ms, seed=1):
@@ -42,7 +45,7 @@ def requests(n, gap_ms, seed=1):
 
 def run_serve(am, gen, reqs, slots, cs):
     """-> (ttfa per request in s, audio samples, wall s)"""
-    server = K.TtsServer(am, gen, slots=slots, chunk_steps=cs, max_steps=256)
+    server = K.TtsServer(am, gen, slots=slots, chunk_steps=cs, max_steps=256, allow_lookahead=True)   # (no-op for a causal one)
     first, ids, samples, nxt = {}, {}, 0, 0
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -80,7 +83,7 @@ def run_lockstep(am, gen, reqs, slots, cs):
         pad = lambda t: torch.nn.functional.pad(t, (0, 0, 0, L - t.shape[0]) if t.dim() == 2 else (0, L - t.shape[0]))
         x = [torch.stack([pad(reqs[i]["inputs"][k]) for i in batch]).to(dev) for k in range(3)]
         x.append(torch.tensor([reqs[i]["inputs"][3] for i in batch], device=dev))
-        st = K.stream_synthesize(am, gen, *x, chunk_steps=cs)
+        st = K.stream_synthesize(am, gen, *x, chunk_steps=cs, allow_lookahead=True)
         for start, w in st:
             torch.cuda.synchronize()
             now = time.perf_counter() - t0
@@ -113,39 +116,42 @@ def front_half_cost(am, reqs, repeats=5):
     return clock(lambda: [am.front_half(*x) for x in one]), clock(lambda: am.front_half(*batch))
 
 
-def summary(name, ttfa, samples, wall):
+def summary(name, sr, ttfa, samples, wall):
     ms = np.array(ttfa) * 1e3
     return dict(server=name, ttfa_p50_ms=round(float(np.percentile(ms, 50)), 1),
-                ttfa_p95_ms=round(float(np.percentile(ms, 95)), 1), audio_s=round(samples / SR, 2), wall_s=round(wall, 2),
-                audio_s_per_wall_s=round(samples / SR / wall, 2))
+                ttfa_p95_ms=round(float(np.percentile(ms, 95)), 1), audio_s=round(samples / sr, 2), wall_s=round(wall, 2),
+                audio_s_per_wall_s=round(samples / sr / wall, 2))
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--vocoder", choices=sorted(VOCODERS), default="causal_24k")
     ap.add_argument("--requests", type=int, default=32)
     ap.add_argument("--slots", type=int, default=8)
     ap.add_argument("--chunk-steps", type=int, default=4)
     ap.add_argument("--gap", type=float, default=150.0, help="mean gap between arrivals, ms")
-    ap.add_argument("--out", default=None, help="also write the result as DIR/tts_serve_latency.json")
+    ap.add_argument("--out", default=None, help="also write the result as DIR/tts_serve_latency[_<vocoder>].json")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tts_serve_latency: needs a CUDA device")
     info = card()
-    am, gen = models()
+    am, gen, sr = models(args.vocoder)
     reqs = requests(args.requests, args.gap)
     with torch.no_grad():
         warm = requests(args.slots, 0.0, seed=2)                     # plans, weight images, graph captures
         run_serve(am, gen, warm, args.slots, args.chunk_steps)
         run_lockstep(am, gen, warm, args.slots, args.chunk_steps)
-        rows = [summary("serve", *run_serve(am, gen, reqs, args.slots, args.chunk_steps)),
-                summary("lockstep", *run_lockstep(am, gen, reqs, args.slots, args.chunk_steps))]
+        rows = [summary("serve", sr, *run_serve(am, gen, reqs, args.slots, args.chunk_steps)),
+                summary("lockstep", sr, *run_lockstep(am, gen, reqs, args.slots, args.chunk_steps))]
         alone, batched = front_half_cost(am, reqs[:args.slots])
-    result = dict(card=info, requests=args.requests, slots=args.slots, chunk_steps=args.chunk_steps, mean_gap_ms=args.gap,
+    result = dict(card=info, vocoder=args.vocoder, lookahead_ms=round(1e3 * K.hifigan.StreamPlan(gen).delay / sr, 1),
+                  requests=args.requests, slots=args.slots, chunk_steps=args.chunk_steps, mean_gap_ms=args.gap,
                   rows=rows, front_half_ms=dict(requests=args.slots, one_by_one=alone, one_batch=batched))
     print(json.dumps(result), flush=True)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "tts_serve_latency.json"), "w") as f:
+        name = "tts_serve_latency" + ("" if args.vocoder == "causal_24k" else "_" + args.vocoder)
+        with open(os.path.join(args.out, name + ".json"), "w") as f:
             json.dump(result, f, indent=1)
 
 

@@ -1,8 +1,12 @@
 """Latency of streamed text-to-speech (infer.stream_synthesize) on the GPU.
 
 SAM-BERT with the sambert_24k.yaml network (seeded weights) and the hifigan_v1_24k.yaml generator (hop 240 at 24 kHz), over
-B in {1, 8} utterances x chunk_steps in {1, 4, 16} decoder steps (3 frames each) per chunk.  Per setting:
+B in {1, 8} utterances x chunk_steps in {1, 4, 16} decoder steps (3 frames each) per chunk.  ``--vocoder noncausal_16k``:
+the same network (sambert_16k.yaml differs only in its data) into the non-causal hifigan_noncausal_v1_16k.yaml generator
+(hop 200 at 16 kHz), streamed with ``allow_lookahead=True``: its audio waits for 3424 samples (214 ms) of look-ahead.
+Per setting:
   ttfa_ms            time to first audio: host clock from the stream_synthesize call to a synchronize after the first chunk
+                     (with a non-causal vocoder, the first chunk holding audio)
   chunk_ms           device time per chunk after the first (CUDA events at each yielded chunk; includes the device idling
                      while the host runs the per-step decoder loop)
   stream_ms          host clock from the call to a synchronize after the last chunk
@@ -13,7 +17,7 @@ Seeded weights predict near-zero durations, so the duration predictor's output b
 symbol: the utterances are then as long as real ones.  Prints the card and its power limit, read in the same run, and all
 rows as one JSON line.
 
-    python scripts/tts_stream_latency.py [--symbols 64] [--repeats 3] [--out DIR]"""
+    python scripts/tts_stream_latency.py [--vocoder causal_24k|noncausal_16k] [--symbols 64] [--repeats 3] [--out DIR]"""
 import argparse
 import json
 import math
@@ -28,7 +32,13 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import kantts_b200 as K  # noqa: E402
 from kantts_b200 import ops  # noqa: E402
 
-SR, DUR = 24000, 5.0
+DUR = 5.0
+# generator structure and sample rate of each vocoder
+VOCODERS = {
+    "causal_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),    # hifigan_v1_24k.yaml
+    "noncausal_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
+                           resblock_dilations=[[1, 3, 5, 7]] * 3, causal=False), 16000),      # hifigan_noncausal_v1_16k.yaml
+}
 
 
 def card():
@@ -37,13 +47,15 @@ def card():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
-def models():
+def models(vocoder="causal_24k"):
+    """-> (SAM-BERT, the ``vocoder``'s generator, its sample rate)"""
     torch.manual_seed(0)
     am = K.KanTtsSAMBERT(K.sambert_24k_config())
     with torch.no_grad():
         am.variance_adaptor.duration_predictor.fc.bias.fill_(math.log(DUR + 1))
-    gen = K.Generator(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4])
-    return am.cuda().eval(), gen.cuda().eval()
+    gcfg, sr = VOCODERS[vocoder]
+    gen = K.Generator(**gcfg)
+    return am.cuda().eval(), gen.cuda().eval(), sr
 
 
 def inputs(cfg, B, L):
@@ -58,7 +70,7 @@ def run_stream(am, gen, x, cs):
     """-> (ttfa s, per-chunk device ms, stream s, lengths in samples)"""
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    st = K.stream_synthesize(am, gen, *x, chunk_steps=cs)
+    st = K.stream_synthesize(am, gen, *x, chunk_steps=cs, allow_lookahead=True)       # (no-op for a causal generator)
     it = iter(st)
     next(it)
     torch.cuda.synchronize()
@@ -75,7 +87,7 @@ def run_stream(am, gen, x, cs):
     return ttfa, chunk_ms, total, st.lengths
 
 
-def measure(am, gen, B, cs, L, repeats):
+def measure(am, gen, sr, B, cs, L, repeats):
     x = inputs(K.sambert_24k_config(), B, L)
     with torch.no_grad():
         run_stream(am, gen, x, cs)                                  # warm-up: plans, weight images, graph capture
@@ -94,7 +106,7 @@ def measure(am, gen, B, cs, L, repeats):
     ttfa = sorted(r[0] for r in runs)[len(runs) // 2]
     total = sorted(r[2] for r in runs)[len(runs) // 2]
     chunks = [c for r in runs for c in r[1]]
-    audio_s = max(runs[0][3]) / SR
+    audio_s = max(runs[0][3]) / sr
     return dict(B=B, chunk_steps=cs, frames_per_chunk=3 * cs, decoder_steps=steps, audio_s=round(audio_s, 3),
                 ttfa_ms=round(1e3 * ttfa, 2), chunk_ms=round(sum(chunks) / max(1, len(chunks)), 3),
                 chunk_ms_max=round(max(chunks, default=0.0), 3), stream_ms=round(1e3 * total, 1),
@@ -103,23 +115,27 @@ def measure(am, gen, B, cs, L, repeats):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--vocoder", choices=sorted(VOCODERS), default="causal_24k")
     ap.add_argument("--symbols", type=int, default=64)
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--out", default=None, help="also write the result as DIR/tts_stream_latency.json")
+    ap.add_argument("--out", default=None, help="also write the result as DIR/tts_stream_latency[_<vocoder>].json")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tts_stream_latency: needs a CUDA device")
     info = card()
-    am, gen = models()
+    am, gen, sr = models(args.vocoder)
     rows = []
     for B in (1, 8):
         for cs in (1, 4, 16):
-            rows.append(measure(am, gen, B, cs, args.symbols, args.repeats))
-    result = dict(card=info, symbols=args.symbols, rows=rows)
+            rows.append(measure(am, gen, sr, B, cs, args.symbols, args.repeats))
+    lookahead = K.hifigan.StreamPlan(gen).delay
+    result = dict(card=info, vocoder=args.vocoder, sample_rate=sr, lookahead_ms=round(1e3 * lookahead / sr, 1),
+                  symbols=args.symbols, rows=rows)
     print(json.dumps(result), flush=True)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "tts_stream_latency.json"), "w") as f:
+        name = "tts_stream_latency" + ("" if args.vocoder == "causal_24k" else "_" + args.vocoder)
+        with open(os.path.join(args.out, name + ".json"), "w") as f:
             json.dump(result, f, indent=1)
 
 
