@@ -157,7 +157,8 @@ inline ResidueTaps residue_taps(const Phase& ph, int step) {
 }
 
 // Chunk rows [lo, hi) of item b's window described by m (KtStreamMask) that lie inside the item's utterance; clamped to
-// +-2^26 (far beyond any chunk), so bounds scaled by an up-sampling factor <= 32 stay in int range.
+// +-2^26 (far beyond any chunk) to fit an int.  A caller that scales them (by an up-sampling factor) clamps them to its
+// window's rows first: 2^26 * 32 is already past INT_MAX.
 __device__ __forceinline__ void stream_utterance_rows(const KtStreamMask& m, int b, int& lo, int& hi) {
   const long long l = (long long)m.lag - (long long)__ldg(m.frames_done + b) * m.rows_per_frame;
   const long long h = l + (long long)__ldg(m.lengths + b) * m.rows_per_frame;

@@ -230,8 +230,10 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
       int t_lo = 0, t_lim = 0;   // MASK: the item's utterance rows, in the row map's (up-sampled) units
       if constexpr (MASK) {
         stream_utterance_rows(p.smask, bb, t_lo, t_lim);
-        t_lo = max(t_lo, -p.in_first) * p.up;
-        t_lim = min(t_lim, p.t_in) * p.up;
+        // both bounds clamped into the window's rows [-in_first, t_in] before they are scaled: the products stay in int
+        // for every up-sampling factor whose up-sampled window does
+        t_lo = min(max(t_lo, -p.in_first), p.t_in) * p.up;
+        t_lim = max(min(t_lim, p.t_in), -p.in_first) * p.up;
       }
       for (int c = 0; c < p.kchunks; ++c) {
         for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ra.advance(p.na_stages)) {
