@@ -11,8 +11,9 @@ kernels) through ``ops.py``; activations are channels-last rows internally and a
 at the module boundary (feature maps are returned as zero-copy permuted views).
 A multi-band generator (``out_channels`` = S > 1) emits S sub-band signals at 1/S of the sample rate; the PQMF filter bank
 (pqmf.py) turns them into the waveform.  Like the reference, the PQMF is not part of the generator: the model builder adds
-it next to the generator, and inference attaches it as ``generator.pqmf`` after loading.  Out of scope (SURVEY.md
-section 8a): MultiSpecDiscriminator, a multi-band NSF generator and streaming a multi-band generator.
+it next to the generator, and inference attaches it as ``generator.pqmf`` after loading; streaming (GeneratorStreamer)
+runs the attached PQMF's synthesis as its last stage.  Out of scope (SURVEY.md section 8a): MultiSpecDiscriminator and a
+multi-band NSF generator.
 """
 import copy
 import ctypes
@@ -502,7 +503,8 @@ class Generator(nn.Module):
     def streamer(self, batch, max_frames, lengths=None, seeds=None):
         """-> a GeneratorStreamer that synthesises ``batch`` independent utterances chunk by chunk (at most ``max_frames``
         mel frames per chunk), giving the waveform of this (eval-mode) generator's forward.  A non-causal generator
-        needs each slot's utterance ``lengths`` in frames (host list or device tensor (batch,)); a causal one takes none.
+        needs each slot's utterance ``lengths`` in frames (host list or device tensor (batch,)); a causal one takes none,
+        unless it is multi-band: its attached PQMF's synthesis reads ahead, so that it needs them too.
         An NSF generator needs each slot's excitation ``seeds`` (as ``forward``'s ``nsf_seeds``); others take none."""
         return GeneratorStreamer(self, batch, max_frames, lengths, seeds)
 
@@ -575,6 +577,17 @@ MeanStep = namedtuple("MeanStep", "srcs dst scale offsets")
 ExciteStep = namedtuple("ExciteStep", "src dst")
 
 
+class FixedConv:
+    """A conv with fixed weights and no bias that is not a layer of the generator: the PQMF synthesis of a multi-band
+    generator (PQMF._weights()), as a ConvStep runs it."""
+
+    def __init__(self, spec, weight):
+        self.spec, self.weight, self.bias = spec, weight, None
+
+    def effective_weight(self):
+        return self.weight, None
+
+
 class StreamPlan:
     """What a GeneratorStreamer runs per chunk, as data (no device needed):
       windows             one entry per tensor of the chunk: {name, channels, rows_per_frame, history}; a tensor read by a
@@ -586,25 +599,40 @@ class StreamPlan:
                           trails the input's lag (times the layer's rate) by stream_lag rows
       delay               the waveform's lag in samples: a chunk returns the samples ``delay`` before the pushed frames' own
       causal              whether the generator is causal
+      hop                 waveform samples per mel frame: prod(upsample_scales), times S for a multi-band generator
       launches_per_chunk  library calls of a full chunk: one per conv (one kernel each on the tensor-core path), one per
-                          sin-add and per mean, one window advance and, non-causal, one output mask; NSF adds the
+                          sin-add and per mean, one window advance and, with a delay, one output mask; NSF adds the
                           excitation, its 1x1 ffn conv, one source conv per stage and, where the stage sum cannot be chained
                           in the forward's order, one three-way add per stage; the mel chunk's copy into its window is not
                           counted
       nsf                 whether the generator has the NSF source: the last two input channels (f0, uv) go to window
                           "f0uv", the excitation (kt_nsf_excitation, seeded per slot) to "exc" and its ffn to "source" (rate
                           hop); stage i adds source_downs[i] of "source", in the forward's order up + (e + rep)
+      pqmf                the PQMF of a multi-band generator (``out_channels`` = S > 1, attached as ``generator.pqmf`` with
+                          ``subbands`` = S), else None.  conv_post writes the S sub-bands to window "sub"
+                          (prod(upsample_scales) rows per frame), and one more ConvStep (layer "pqmf") runs the causal form
+                          of the synthesis (stream_spec of PQMF.synthesis_spec, weight PQMF._weights()[1]) into "wav".  The
+                          synthesis reads taps / 2 samples ahead, so that even a causal multi-band generator streams with a
+                          delay: lag("sub") * S + taps / 2 samples, 31 for the default 62 taps
       steps               ConvStep | SinStep | MeanStep | ExciteStep records, in launch order"""
 
     def __init__(self, gen):
+        pqmf = None
         if gen.out_channels > 1:
-            raise ValueError("streaming a multi-band (PQMF) generator is not supported: PQMF synthesis reads 31 samples "
-                             "ahead of every output sample")
+            pqmf = getattr(gen, "pqmf", None)
+            if pqmf is None or pqmf.subbands != gen.out_channels:
+                raise ValueError(f"streaming a multi-band (PQMF) generator of {gen.out_channels} sub-bands needs its PQMF "
+                                 f"attached as generator.pqmf with as many sub-bands (got "
+                                 f"{'none' if pqmf is None else pqmf.subbands}), as synthesize() does")
         if gen.training:
             raise ValueError("streaming runs a generator in eval() mode")
         self.causal = causal = gen.conv_pre.causal
         self.nsf = nsf = gen.nsf_enable
+        self.pqmf = pqmf
+        synth = None if pqmf is None else FixedConv(pqmf.synthesis_spec, pqmf._weights()[1])
         names = {m: n for n, m in gen.named_modules()}
+        if synth is not None:
+            names[synth] = "pqmf"
         table = WindowTable()
         self.windows, self.layer_history, self.steps, self.lags = table.windows, {}, [], {}
 
@@ -612,14 +640,19 @@ class StreamPlan:
             self.lags[name] = 0
             return table.add(name, channels, rate)
 
+        def padded(nc):
+            """Whether layer nc reads ahead of its output and runs in causal form: every layer of a non-causal generator,
+            and the PQMF synthesis"""
+            return not causal or nc is synth
+
         def layer(mod, src):
             nc = mod.conv1d if hasattr(mod, "conv1d") else getattr(mod, "deconv", mod)     # (the NSF ffn is the conv itself)
-            return nc, nc.spec if causal else stream_spec(nc.spec, self.lags[src])
+            return nc, stream_spec(nc.spec, self.lags[src]) if padded(nc) else nc.spec
 
         def lag_of(mod, src):
             """The lag of mod's output when it reads window src."""
             nc, _ = layer(mod, src)
-            return 0 if causal else stream_lag(nc.spec, self.lags[src])
+            return stream_lag(nc.spec, self.lags[src]) if padded(nc) else 0
 
         def conv(mod, src, dst, resid=None, side=None):
             nc, spec = layer(mod, src)
@@ -708,14 +741,20 @@ class StreamPlan:
             # the parallel ResBlocks trail their input by different right reaches: each is read at the mean's lag
             x = add(f"mean{i}", cout, rate)
             mean(outs, x, 1.0 / nk)
-        conv(gen.conv_post, x, add("wav", 1, rate))
         assert rate == hop
+        if synth is None:
+            conv(gen.conv_post, x, add("wav", 1, rate))
+        else:
+            sub = add("sub", gen.out_channels, rate)
+            conv(gen.conv_post, x, sub)
+            rate *= gen.out_channels
+            conv(synth, sub, add("wav", 1, rate))
         hist = {w["name"]: w["history"] for w in self.windows}
         for st in self.steps:                  # kt_add3_scale_win reads its sources at one pitch
             assert type(st) is not MeanStep or len({hist[o] for o in st.srcs}) == 1, st
         self.hop = rate
         self.delay = self.lags["wav"]
-        self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + (not causal)
+        self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + (self.delay > 0)
 
 
 class GeneratorStreamer:
@@ -735,6 +774,13 @@ class GeneratorStreamer:
     exactly lengths[b] frames: every layer's zero padding at the utterance's end is applied per slot inside the conv
     kernels (the stream conv's KtStreamMask), from the slots' utterance record (stream.SlotUtterances).  A slot reset
     before its utterance has drained loses the samples not yet returned.
+
+    Multi-band generator (``out_channels`` = S > 1 with its PQMF attached as ``generator.pqmf``): the last stream stage is
+    the PQMF synthesis, run in causal form over the S sub-bands, and a push returns the waveform (B, 1, f * hop) with hop =
+    prod(upsample_scales) * S.  The synthesis reads taps / 2 samples ahead, so that the stream is delayed as above even for
+    a causal generator (delay 31 samples for the default 62 taps, one drain frame), and needs ``lengths``: each slot's
+    sub-bands are masked at its utterance end (lengths[b] * hop / S rows), the synthesis's zero padding.  Slot b's chunks,
+    cut the same way, equal ``pqmf.synthesis(generator(mel_b[..., :lengths[b]]))``.
 
     NSF generator: ``push`` takes (B, in_channels + 2, f) -- mel, f0 in Hz and the voiced flag, as ``forward`` -- and each
     slot's excitation is seeded by its ``seeds`` entry (``reset`` takes the new slots' seeds).  The excitation is computed
@@ -757,10 +803,14 @@ class GeneratorStreamer:
             raise ValueError("streamer: seeds are for NSF generators; this one has no NSF source module")
         if seeds is not None:
             seeds = nsf_seed_tensor(seeds, int(batch), torch.device("cpu") if not torch.is_tensor(seeds) else seeds.device)
-        if plan.causal and lengths is not None:
+        if not plan.delay and lengths is not None:
             raise ValueError("a causal generator streams without lengths: its output does not depend on where an utterance "
                              "ends")
-        if not plan.causal and lengths is None:
+        if plan.delay and lengths is None:
+            if plan.causal:
+                raise ValueError("streaming a multi-band generator needs per-slot lengths: its PQMF synthesis reads "
+                                 f"{plan.delay} samples ahead, so its output near an utterance's end depends on where that "
+                                 "end is")
             raise ValueError("streaming a non-causal generator needs per-slot lengths (a causal one needs none): its output "
                              "near an utterance's end depends on where that end is")
         self._win = win = Windows(plan.windows, batch, max_frames, next(gen.parameters()).device, "streamer")
@@ -774,12 +824,11 @@ class GeneratorStreamer:
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
         with torch.no_grad(), torch.cuda.device(self.device):
             self._slots = self._masks = None
-            if not plan.causal:
+            if plan.delay:
                 self._slots = SlotUtterances(self.batch, self.device)
                 self._masks = {w["name"]: self._slots.mask(w["rows_per_frame"], plan.lags[w["name"]]) for w in plan.windows}
                 self._zeros = torch.zeros(self.batch, self.in_channels, self.max_frames, device=self.device)
-            self._weights = {st.conv: own_weight(st.spec, *st.conv.effective_weight(), st.conv.bias)
-                             for st in plan.steps if type(st) is ConvStep}
+            self._weights = {st.conv: self._own_weight(st) for st in plan.steps if type(st) is ConvStep}
             self._nsf = NsfState(self._source, torch.zeros(self.batch, dtype=torch.int64, device=self.device)) \
                 if plan.nsf else None
             self._run(self.max_frames)               # warm-up: every kernel and weight image of a full chunk
@@ -787,6 +836,12 @@ class GeneratorStreamer:
             with torch.cuda.graph(self._graph):
                 self._run(self.max_frames)
             self.reset(range(self.batch), lengths, seeds)
+
+    def _own_weight(self, st):
+        """The streamer's copy of ConvStep st's weights, on its device (the PQMF synthesis weight lives wherever the PQMF's
+        buffers are)."""
+        v, g = st.conv.effective_weight()
+        return own_weight(st.spec, v.to(self.device), g, st.conv.bias)
 
     def _run(self, f):
         """Every launch of one chunk of f frames (the mel chunk is in its window), on the current stream."""
@@ -840,7 +895,8 @@ class GeneratorStreamer:
 
     def finish(self):
         """Push ``drain_frames`` frames (in chunks of at most max_frames; their content is ignored) -> their (B, 1, n)
-        waveform, which ends with the last sample of every utterance pushed to its end.  (B, 1, 0) for a causal generator."""
+        waveform, which ends with the last sample of every utterance pushed to its end.  (B, 1, 0) without a delay (a
+        causal full-band generator)."""
         with torch.no_grad(), torch.cuda.device(self.device):
             outs, left = [], self.drain_frames
             while left > 0:
@@ -850,13 +906,14 @@ class GeneratorStreamer:
             return torch.cat(outs, -1) if outs else torch.zeros(self.batch, 1, 0, device=self.device)
 
     def reset(self, slots, lengths=None, seeds=None):
-        """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A non-causal
-        generator needs the new utterances' ``lengths`` in frames, an NSF one their excitation ``seeds``, both in the order
-        of ``slots``.  All of it is checked before the first launch: a rejected reset leaves every slot as it was."""
-        if self.plan.causal and lengths is not None:
+        """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A generator
+        streamed with a delay (non-causal or multi-band) needs the new utterances' ``lengths`` in frames, an NSF one their
+        excitation ``seeds``, both in the order of ``slots``.  All of it is checked before the first launch: a rejected reset leaves every slot as it was."""
+        if not self.delay and lengths is not None:
             raise ValueError("reset: a causal generator streams without lengths")
-        if not self.plan.causal and lengths is None:
-            raise ValueError("reset: streaming a non-causal generator needs the new utterances' lengths")
+        if self.delay and lengths is None:
+            raise ValueError("reset: streaming a " + ("multi-band" if self.plan.causal else "non-causal") +
+                             " generator needs the new utterances' lengths")
         if self.plan.nsf and seeds is None:
             raise ValueError("reset: streaming an NSF generator needs the new utterances' seeds")
         if not self.plan.nsf and seeds is not None:

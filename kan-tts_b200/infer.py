@@ -10,7 +10,10 @@ in one call; every utterance is cut at its own predicted length (frames x produc
 (PostNet.streamer) -> streamed vocoder (Generator.streamer).  A non-causal vocoder streams with ``allow_lookahead=True``:
 its output waits for its look-ahead (``lookahead`` samples, 3424 = 214 ms for the 16 kHz yamls), and each utterance's
 audio equals the generator run on exactly that utterance's post-net frames, the reference's hand-off
-(infer_sambert.py:136-138 then infer_hifigan.py).
+(infer_sambert.py:136-138 then infer_hifigan.py).  A multi-band vocoder (its PQMF attached as ``generator.pqmf``) streams
+its PQMF synthesis as the last stage: the synthesis reads taps/2 samples ahead (31 = 1.3 ms at 24 kHz for the default 62
+taps), so that even a causal multi-band vocoder streams late by that look-ahead; being under one frame, it needs no
+``allow_lookahead``.
 
 An NSF acoustic model (``num_mels`` = mel + f0 + voiced flag) drives an NSF generator with ``nsf_f0`` and ``nsf_seeds``: the
 f0 channel is denormalised and the voiced flag binarised as the reference's hand-off does (kantts/bin/infer_sambert.py:26-56
@@ -58,9 +61,11 @@ def _check_nsf(sambert_num_mels, generator, nsf_f0, nsf_seeds, what):
 
 
 def stream_lookahead(generator, allow_lookahead, what):
-    """-> the samples by which ``generator`` streams each sample late (StreamPlan.delay; 0 for a causal generator).
-    ValueError for a generator that does not stream (StreamPlan: multi-band, training mode), and for a non-causal one
-    unless ``allow_lookahead``: its look-ahead adds to every utterance's time to first audio, so the caller opts in."""
+    """-> the samples by which ``generator`` streams each sample late (StreamPlan.delay; 0 for a causal full-band generator,
+    taps/2 of the PQMF for a causal multi-band one).  ValueError for a generator that does not stream (StreamPlan:
+    multi-band without its PQMF attached, training mode), and for a non-causal one unless ``allow_lookahead``: its
+    look-ahead adds to every utterance's time to first audio, so the caller opts in.  A causal multi-band generator
+    streams without it: its PQMF synthesis reads less than a frame ahead."""
     plan = StreamPlan(generator)
     if not plan.causal and not allow_lookahead:
         raise ValueError(f"{what} needs a causal generator: a non-causal one reads {plan.delay} samples ahead of every "
@@ -105,7 +110,11 @@ def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_sp
     ``synthesize(..., nsf_f0, nsf_seeds)[0][b]`` for a causal generator.
     A non-causal generator is refused unless ``allow_lookahead``: its audio then comes ``TtsStream.lookahead`` samples
     later, and slot b's is the generator run on exactly its ``lengths[b] / hop`` post-net frames (the reference's
-    hand-off; ``synthesize`` runs it on the batch's padded mel instead, which changes an utterance's last samples)."""
+    hand-off; ``synthesize`` runs it on the batch's padded mel instead, which changes an utterance's last samples).
+    A multi-band generator streams with its PQMF attached, with or without ``allow_lookahead`` when it is causal: slot b's
+    audio is ``pqmf.synthesis(generator(mel_b))`` of exactly its frames, later by the synthesis's taps/2 samples (plus the
+    generator's own look-ahead when it is non-causal).  Against ``synthesize``, a shorter utterance of the batch differs in
+    its last taps/2 samples, where the padded batch's synthesis reads the generator's output past the utterance's end."""
     if sambert.training or generator.training:
         raise RuntimeError("stream_synthesize() expects both models in eval() mode")
     if generator.nsf_enable and (nsf_f0 is None or nsf_seeds is None):
@@ -128,7 +137,8 @@ class TtsStream:
     """The audio of one batch of utterances, chunk by chunk (made by ``stream_synthesize``).
 
     ``lengths``: per-slot sample counts, ``LR_length_rounded[b] * hop`` (read on the host once, before decoding).
-    ``lookahead``: the vocoder's delay in samples (GeneratorStreamer.delay; 0 for a causal one): the push of the frames
+    ``hop``: the vocoder's samples per frame (GeneratorStreamer.hop: prod(upsample_scales), times S for a multi-band one).
+    ``lookahead``: the vocoder's delay in samples (GeneratorStreamer.delay; 0 for a causal full-band one): the push of the frames
     [p, p + f) returns the samples [p·hop - lookahead, (p + f)·hop - lookahead), and the samples before 0 are not
     yielded; after the last decoder step the vocoder's drain (GeneratorStreamer.finish) brings out the rest.
     Iterating yields ``(start_sample, wav)``, ``wav`` (B, 1, n) on the device, n > 0, with starts contiguous from 0; slot
@@ -143,15 +153,15 @@ class TtsStream:
         with torch.no_grad():
             self._front = f = sambert.front_half(inputs_ling, inputs_emotion, inputs_speaker, input_lengths)
         self.batch = B = f["memory"].shape[0]
-        self.hop = int(np.prod(generator.upsample_scales))
         frames = f["lr_len"]
-        self.lengths = [int(n) * self.hop for n in frames.cpu()]
         self.max_frames = F = self.r * chunk_steps
         self._post = sambert.mel_postnet.streamer(B, F, frames)
-        # a non-causal vocoder masks each slot's utterance end on the device, from the lengths the decoder masks by
-        self._voc = generator.streamer(batch=B, max_frames=F, lengths=None if generator.conv_pre.causal else frames,
+        # a vocoder with a look-ahead (non-causal, or multi-band: the PQMF synthesis) masks each slot's utterance end on the
+        # device, from the lengths the decoder masks by
+        self._voc = generator.streamer(batch=B, max_frames=F, lengths=frames if StreamPlan(generator).delay else None,
                                        seeds=nsf_seeds)
-        self.lookahead = self._voc.delay
+        self.hop, self.lookahead = self._voc.hop, self._voc.delay
+        self.lengths = [int(n) * self.hop for n in frames.cpu()]
         self._used = False
 
     @staticmethod
@@ -261,16 +271,18 @@ class TtsServer:
 
     A non-causal generator is refused unless ``allow_lookahead``: each request's audio then comes ``lookahead`` samples
     later (the vocoder's delay; 0 for a causal one) and equals the generator run on exactly that request's post-net
-    frames, the reference's hand-off.  A slot may start decoding its next request while the vocoder still drains the
-    previous one's last samples, timed so that its vocoder reset comes after them.  (``delay`` is the post-net's delay
-    in rows.)"""
+    frames, the reference's hand-off.  A multi-band generator serves with its PQMF attached (``generator.pqmf``); a
+    causal one needs no ``allow_lookahead``: its look-ahead is the PQMF synthesis's taps/2 samples, and each request's
+    audio is ``pqmf.synthesis(generator(mel))`` of exactly its frames (``synthesize`` of a padded batch differs from it in
+    a shorter utterance's last taps/2 samples).  A slot may start decoding its next request while the vocoder still
+    drains the previous one's last samples, timed so that its vocoder reset comes after them.  (``delay`` is the
+    post-net's delay in rows.)"""
 
     def __init__(self, sambert, generator, slots, chunk_steps, max_steps, nsf_f0=None, allow_lookahead=False):
         from .sambert import PostNetStreamPlan
         if sambert.training or generator.training:
             raise RuntimeError("TtsServer expects both models in eval() mode")
         self.lookahead = stream_lookahead(generator, allow_lookahead, "serving")
-        self._causal = generator.conv_pre.causal
         num_mels = sambert.mel_postnet.num_mels
         self.nsf = generator.nsf_enable
         if self.nsf:
@@ -291,15 +303,15 @@ class TtsServer:
                              "for an utterance's frame 0 to start a chunk")
         self.sambert, self.nsf_f0 = sambert, nsf_f0
         self.frames_per_chunk = F = self.r * self.chunk_steps
-        self.hop = int(np.prod(generator.upsample_scales))
         self.device = next(sambert.parameters()).device
         self._dec = dec.slots(self.batch, self.max_steps)
         with torch.no_grad():
             self._post = sambert.mel_postnet.streamer(self.batch, F, torch.zeros(self.batch, dtype=torch.int32,
                                                                                  device=self.device), per_slot=True)
             # every slot is reset, with its request's frame count and seed, before its first audio
-            self._voc = generator.streamer(batch=self.batch, max_frames=F, lengths=None if self._causal else [1] * self.batch,
+            self._voc = generator.streamer(batch=self.batch, max_frames=F, lengths=[1] * self.batch if self.lookahead else None,
                                            seeds=[0] * self.batch if self.nsf else None)
+        self.hop = self._voc.hop                        # waveform samples per frame (times S for a multi-band vocoder)
         # _slots: each slot's current request (decoder and post-net); _playing: (slot, request) of every request whose
         # audio has not all come out, which with a vocoder look-ahead can outlast its slot's hold on the decoder
         self._queue, self._slots, self._playing, self._chunk, self._next_id = [], [None] * self.batch, [], 0, 0
@@ -363,7 +375,7 @@ class TtsServer:
             due = [(b, s) for b, s in live if s["voc_chunk"] == c]
             if due:
                 seeds = torch.cat([s["seed"] for _, s in due]) if self.nsf else None
-                lengths = None if self._causal else [s["frames"] for _, s in due]
+                lengths = [s["frames"] for _, s in due] if self.lookahead else None
                 self._voc.reset([b for b, _ in due], lengths, seeds=seeds)
             wav = self._voc.push(post.transpose(1, 2))
         audio, finished = [], []

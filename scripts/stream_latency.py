@@ -14,7 +14,16 @@ with per-slot lengths long enough that no utterance ends during the run; its row
 hifigan_noncausal_nsf_v1_16k.yaml (hop 200 at 16 kHz), streamed with per-slot seeds; each chunk carries f0 and the voiced
 flag after the mel, and the whole-utterance forward takes the same seeds.
 
-    python scripts/stream_latency.py [--config causal|noncausal|nsf|nsf_noncausal] [--chunks 200] [--out DIR]"""
+--config multiband: the multi-band generator of scripts/multiband_step.py (G_MB: 4 sub-bands at 6 kHz, upsample_scales
+[5, 3, 2, 2], 512 channels) with its PQMF synthesis as the last stream stage (hop 240 at 24 kHz; the synthesis's 31 samples
+of look-ahead: per-slot lengths, one drain frame), next to the full-band v1_24k generator (hop 240 at 24 kHz).  The
+whole-utterance forward of the multi-band generator includes PQMF.synthesis.
+
+--runs N repeats the config's generators N times, alternating them, so that the spread between runs of one generator can
+be set against the difference between generators.
+
+    python scripts/stream_latency.py [--config causal|noncausal|nsf|nsf_noncausal|multiband] [--chunks 200] [--runs 1]
+                                     [--out DIR]"""
 import argparse
 import json
 import os
@@ -39,6 +48,10 @@ GENERATORS = {
     "nsf": {
         "v1_nsf_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4],
                             nsf_params=dict(nb_harmonics=7, sampling_rate=24000)), 24000),
+    },
+    "multiband": {
+        "v1_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),
+        "multiband_24k": (dict(out_channels=4, upsample_scales=[5, 3, 2, 2], upsample_kernal_sizes=[10, 6, 4, 4]), 24000),
     },
     "nsf_noncausal": {
         "noncausal_nsf_v1_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
@@ -66,7 +79,8 @@ def card():
 
 
 def measure(gen, sr, B, F, chunks):
-    lengths = None if gen.conv_pre.causal else [1 << 24] * B
+    # a generator streamed with a look-ahead (non-causal, or multi-band) takes lengths that outlast the run
+    lengths = [1 << 24] * B if K.hifigan.StreamPlan(gen).delay else None
     seeds = list(range(B)) if gen.nsf_enable else None
     st = gen.streamer(batch=B, max_frames=F, lengths=lengths, seeds=seeds)
     mel = frames_input(gen, B, F)
@@ -87,13 +101,14 @@ def measure(gen, sr, B, F, chunks):
     frames = min(chunks * F, max(F, WHOLE_MAX_ROWS // B))
     whole = frames_input(gen, B, frames)
     kw = dict(nsf_seeds=seeds) if seeds else {}
+    forward = (lambda: gen.pqmf.synthesis(gen(whole))) if gen.out_channels > 1 else (lambda: gen(whole, **kw))
     with torch.no_grad():
-        gen(whole, **kw)
+        forward()
         torch.cuda.synchronize()
         w0, w1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         w0.record()
         for _ in range(3):
-            gen(whole, **kw)
+            forward()
         w1.record()
         torch.cuda.synchronize()
     whole_ms = w0.elapsed_time(w1) / 3
@@ -108,21 +123,28 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", choices=sorted(GENERATORS), default="causal")
     ap.add_argument("--chunks", type=int, default=200)
+    ap.add_argument("--runs", type=int, default=1, help="measure the config's generators this many times, alternating")
     ap.add_argument("--out", default=None, help="also write the rows as DIR/stream_latency.json")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("stream_latency: needs a CUDA device")
     info = card()
     print(f"card: {info}")
-    rows = []
+    rows, gens = [], {}
     for name, (cfg, sr) in GENERATORS[args.config].items():
         torch.manual_seed(0)
-        gen = K.Generator(**cfg).cuda().eval()
-        for B in (1, 16, 64):
-            for F in (1, 4, 16):
-                r = dict(generator=name, **measure(gen, sr, B, F, args.chunks))
-                rows.append(r)
-                print(json.dumps(r), flush=True)
+        gens[name] = K.Generator(**cfg).cuda().eval()
+        if gens[name].out_channels > 1:
+            gens[name].pqmf = K.PQMF(gens[name].out_channels).cuda()
+    for run in range(args.runs):
+        for name, (cfg, sr) in GENERATORS[args.config].items():
+            for B in (1, 16, 64):
+                for F in (1, 4, 16):
+                    r = dict(generator=name, **measure(gens[name], sr, B, F, args.chunks))
+                    if args.runs > 1:
+                        r["run"] = run
+                    rows.append(r)
+                    print(json.dumps(r), flush=True)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         suffix = "" if args.config == "causal" else "_" + args.config

@@ -2,7 +2,9 @@
 
 SAM-BERT with the sambert_24k.yaml network (seeded weights, about DUR frames per symbol) and the hifigan_v1_24k.yaml
 generator, or with ``--vocoder noncausal_16k`` the non-causal hifigan_noncausal_v1_16k.yaml generator (hop 200 at 16 kHz,
-served and streamed with ``allow_lookahead=True``: every request's audio waits for 214 ms of look-ahead).  N requests of
+served and streamed with ``allow_lookahead=True``: every request's audio waits for 214 ms of look-ahead), or with
+``--vocoder multiband_24k`` the causal multi-band generator of scripts/multiband_step.py with its PQMF (hop 240 at 24 kHz,
+1.3 ms of look-ahead: the synthesis's 31 samples).  N requests of
 16..96 symbols arrive at seeded Poisson times (mean gap --gap ms).  Both servers run on one host thread and deliver
 each chunk's audio to the host (a synchronize after each chunk):
   serve     TtsServer with B slots: requests are submitted when their arrival time has passed, one step() per chunk
@@ -12,7 +14,7 @@ audio seconds per wall second (all requests' audio / time from the first arrival
 cost: front_half of B requests one by one (as TtsServer admits them) against one padded batch.  Prints the card and
 its power limit, read in the same run, and the result as one JSON line.
 
-    python scripts/tts_serve_latency.py [--vocoder causal_24k|noncausal_16k] [--requests 32] [--slots 8] [--chunk-steps 4]
+    python scripts/tts_serve_latency.py [--vocoder causal_24k|noncausal_16k|multiband_24k] [--requests 32] [--slots 8] [--chunk-steps 4]
                                         [--gap 150] [--out DIR]"""
 import argparse
 import json

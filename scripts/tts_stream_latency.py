@@ -4,6 +4,8 @@ SAM-BERT with the sambert_24k.yaml network (seeded weights) and the hifigan_v1_2
 B in {1, 8} utterances x chunk_steps in {1, 4, 16} decoder steps (3 frames each) per chunk.  ``--vocoder noncausal_16k``:
 the same network (sambert_16k.yaml differs only in its data) into the non-causal hifigan_noncausal_v1_16k.yaml generator
 (hop 200 at 16 kHz), streamed with ``allow_lookahead=True``: its audio waits for 3424 samples (214 ms) of look-ahead.
+``--vocoder multiband_24k``: the causal multi-band generator of scripts/multiband_step.py (4 sub-bands, hop 240 at 24 kHz)
+with its PQMF, whose synthesis adds 31 samples (1.3 ms) of look-ahead.
 Per setting:
   ttfa_ms            time to first audio: host clock from the stream_synthesize call to a synchronize after the first chunk
                      (with a non-causal vocoder, the first chunk holding audio)
@@ -17,7 +19,8 @@ Seeded weights predict near-zero durations, so the duration predictor's output b
 symbol: the utterances are then as long as real ones.  Prints the card and its power limit, read in the same run, and all
 rows as one JSON line.
 
-    python scripts/tts_stream_latency.py [--vocoder causal_24k|noncausal_16k] [--symbols 64] [--repeats 3] [--out DIR]"""
+    python scripts/tts_stream_latency.py [--vocoder causal_24k|noncausal_16k|multiband_24k] [--symbols 64] [--repeats 3]
+                                         [--out DIR]"""
 import argparse
 import json
 import math
@@ -38,6 +41,8 @@ VOCODERS = {
     "causal_24k": (dict(upsample_scales=[8, 5, 3, 2], upsample_kernal_sizes=[16, 10, 6, 4]), 24000),    # hifigan_v1_24k.yaml
     "noncausal_16k": (dict(channels=256, upsample_scales=[10, 5, 2, 2], upsample_kernal_sizes=[20, 11, 4, 4],
                            resblock_dilations=[[1, 3, 5, 7]] * 3, causal=False), 16000),      # hifigan_noncausal_v1_16k.yaml
+    # G_MB of scripts/multiband_step.py: 4 sub-bands at 6 kHz, with its PQMF (hop 240 at 24 kHz)
+    "multiband_24k": (dict(out_channels=4, upsample_scales=[5, 3, 2, 2], upsample_kernal_sizes=[10, 6, 4, 4]), 24000),
 }
 
 
@@ -54,8 +59,10 @@ def models(vocoder="causal_24k"):
     with torch.no_grad():
         am.variance_adaptor.duration_predictor.fc.bias.fill_(math.log(DUR + 1))
     gcfg, sr = VOCODERS[vocoder]
-    gen = K.Generator(**gcfg)
-    return am.cuda().eval(), gen.cuda().eval(), sr
+    gen = K.Generator(**gcfg).cuda().eval()
+    if gen.out_channels > 1:
+        gen.pqmf = K.PQMF(gen.out_channels).cuda()
+    return am.cuda().eval(), gen, sr
 
 
 def inputs(cfg, B, L):
