@@ -28,7 +28,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, ptr
-from .stream import SlotUtterances, Windows, WindowTable, check_slots, own_weight, to_device
+from .stream import Streamer, WindowTable, check_slots, own_weight, to_device
 
 # --------------------------------------------------------------------------------------------
 # parameter holders (names / shapes == the reference's weight_norm / spectral_norm wrapped convs)
@@ -757,7 +757,7 @@ class StreamPlan:
         self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + (self.delay > 0)
 
 
-class GeneratorStreamer:
+class GeneratorStreamer(Streamer):
     """Chunk-by-chunk synthesis with a HiFi-GAN generator (Generator.streamer).
 
     ``push(mel)`` takes the next (B, in_channels, f) mel frames of every batch slot (1 <= f <= max_frames, on the
@@ -794,40 +794,17 @@ class GeneratorStreamer:
     streamer.  Creating one also runs a chunk of zeros through every kernel, so that every kernel is loaded, captures the
     full-size chunk's graph, then clears the state; the capture synchronises the device once."""
 
+    out, f_axis = "wav", 2
+
     def __init__(self, gen, batch, max_frames, lengths=None, seeds=None):
-        self.plan = plan = StreamPlan(gen)
-        if plan.nsf and seeds is None:
-            raise ValueError("streaming an NSF generator needs per-slot seeds: its excitation is a seeded function of the "
-                             "sample index, so that chunks reproduce the whole-utterance forward(x, nsf_seeds)")
-        if not plan.nsf and seeds is not None:
-            raise ValueError("streamer: seeds are for NSF generators; this one has no NSF source module")
-        if seeds is not None:
-            seeds = nsf_seed_tensor(seeds, int(batch), torch.device("cpu") if not torch.is_tensor(seeds) else seeds.device)
-        if not plan.delay and lengths is not None:
-            raise ValueError("a causal generator streams without lengths: its output does not depend on where an utterance "
-                             "ends")
-        if plan.delay and lengths is None:
-            if plan.causal:
-                raise ValueError("streaming a multi-band generator needs per-slot lengths: its PQMF synthesis reads "
-                                 f"{plan.delay} samples ahead, so its output near an utterance's end depends on where that "
-                                 "end is")
-            raise ValueError("streaming a non-causal generator needs per-slot lengths (a causal one needs none): its output "
-                             "near an utterance's end depends on where that end is")
-        self._win = win = Windows(plan.windows, batch, max_frames, next(gen.parameters()).device, "streamer")
-        self.batch, self.max_frames, self.hop, self.device = win.batch, win.max_frames, plan.hop, win.device
-        self.delay = plan.delay
-        self.drain_frames = -(-self.delay // self.hop)
-        self.in_channels = plan.windows[0]["channels"] + (2 if plan.nsf else 0)
-        self._places = [win.place(st.src, st.dst, st.resid, res_lag=st.res_lag) if type(st) is ConvStep else None
-                        for st in plan.steps]
+        plan = StreamPlan(gen)
+        self._check_utterances(plan, int(batch), lengths, seeds)         # before any device work
+        self.hop, self.in_channels = plan.hop, plan.windows[0]["channels"] + (2 if plan.nsf else 0)
+        super().__init__(plan, batch, max_frames, next(gen.parameters()).device, "streamer", masked=plan.delay > 0,
+                         in_channels=self.in_channels)
         self._source = gen.source_module if plan.nsf else None
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(gen.num_kernels)] if gen.num_kernels > 1 else []
         with torch.no_grad(), torch.cuda.device(self.device):
-            self._slots = self._masks = None
-            if plan.delay:
-                self._slots = SlotUtterances(self.batch, self.device)
-                self._masks = {w["name"]: self._slots.mask(w["rows_per_frame"], plan.lags[w["name"]]) for w in plan.windows}
-                self._zeros = torch.zeros(self.batch, self.in_channels, self.max_frames, device=self.device)
             self._weights = {st.conv: self._own_weight(st) for st in plan.steps if type(st) is ConvStep}
             self._nsf = NsfState(self._source, torch.zeros(self.batch, dtype=torch.int64, device=self.device)) \
                 if plan.nsf else None
@@ -836,6 +813,24 @@ class GeneratorStreamer:
             with torch.cuda.graph(self._graph):
                 self._run(self.max_frames)
             self.reset(range(self.batch), lengths, seeds)
+
+    @staticmethod
+    def _check_utterances(plan, n, lengths, seeds):
+        """-> ``seeds`` as an int64 tensor (n,) where they are (None without NSF), after checking that ``lengths`` are given
+        exactly when the stream has a delay and ``seeds`` exactly when the generator is NSF; ValueError otherwise."""
+        if plan.nsf and seeds is None:
+            raise ValueError("streaming an NSF generator needs per-slot seeds: its excitation is a seeded function of the "
+                             "sample index, so that chunks reproduce the whole-utterance forward(x, nsf_seeds)")
+        if not plan.nsf and seeds is not None:
+            raise ValueError("streamer: seeds are for NSF generators; this one has no NSF source module")
+        if not plan.delay and lengths is not None:
+            raise ValueError("a causal generator streams without lengths: its output does not depend on where an utterance "
+                             "ends")
+        if plan.delay and lengths is None:
+            raise ValueError(f"streaming a {'multi-band' if plan.causal else 'non-causal'} generator needs per-slot lengths: "
+                             f"it reads {plan.delay} samples ahead, so that its output near an utterance's end depends on "
+                             "where that end is")
+        return None if seeds is None else nsf_seed_tensor(seeds, n, seeds.device if torch.is_tensor(seeds) else "cpu")
 
     def _own_weight(self, st):
         """The streamer's copy of ConvStep st's weights, on its device (the PQMF synthesis weight lives wherever the PQMF's
@@ -872,9 +867,7 @@ class GeneratorStreamer:
                 srcs = [ptr(b[s]) + (win.first[s] - o) * ch * 4 for s, o in zip(st.srcs, st.offsets)] + [None] * (3 - len(st.srcs))
                 ops.call("kt_add3_scale_win", srcs[0], srcs[1], srcs[2], st.scale, ptr(dst), B, f * win.rate[st.dst], ch,
                          b[st.srcs[0]].shape[1], dst.shape[1], win.first[st.dst])
-        if masks is not None:
-            self._slots.mask_advance(masks["wav"], b["wav"], win.first["wav"], f * self.hop, f)
-        win.advance(f)
+        self._end_chunk(f)
 
     def push(self, mel):
         """mel: (B, in_channels, f), 1 <= f <= max_frames, on the streamer's device -> the (B, 1, f * hop) waveform.  NSF:
@@ -891,42 +884,21 @@ class GeneratorStreamer:
                 self._graph.replay()
             else:
                 self._run(f)
-            return self._win.buf["wav"][:, :f * self.hop, 0].unsqueeze(1).clone(memory_format=torch.contiguous_format)
-
-    def finish(self):
-        """Push ``drain_frames`` frames (in chunks of at most max_frames; their content is ignored) -> their (B, 1, n)
-        waveform, which ends with the last sample of every utterance pushed to its end.  (B, 1, 0) without a delay (a
-        causal full-band generator)."""
-        with torch.no_grad(), torch.cuda.device(self.device):
-            outs, left = [], self.drain_frames
-            while left > 0:
-                f = min(left, self.max_frames)
-                outs.append(self.push(self._zeros[:, :, :f]))
-                left -= f
-            return torch.cat(outs, -1) if outs else torch.zeros(self.batch, 1, 0, device=self.device)
+            return self._output(f)
 
     def reset(self, slots, lengths=None, seeds=None):
         """The given batch slots start a new utterance: their carried state returns to zeros (one launch).  A generator
         streamed with a delay (non-causal or multi-band) needs the new utterances' ``lengths`` in frames, an NSF one their
-        excitation ``seeds``, both in the order of ``slots``.  All of it is checked before the first launch: a rejected reset leaves every slot as it was."""
-        if not self.delay and lengths is not None:
-            raise ValueError("reset: a causal generator streams without lengths")
-        if self.delay and lengths is None:
-            raise ValueError("reset: streaming a " + ("multi-band" if self.plan.causal else "non-causal") +
-                             " generator needs the new utterances' lengths")
-        if self.plan.nsf and seeds is None:
-            raise ValueError("reset: streaming an NSF generator needs the new utterances' seeds")
-        if not self.plan.nsf and seeds is not None:
-            raise ValueError("reset: seeds are for NSF generators")
+        excitation ``seeds``, both in the order of ``slots``.  All of it is checked before the first launch: a rejected
+        reset leaves every slot as it was."""
         slots = check_slots(slots, self.batch)
+        seeds = self._check_utterances(self.plan, len(slots), lengths, seeds)
         with torch.no_grad(), torch.cuda.device(self.device):
-            if seeds is not None:
-                seeds = nsf_seed_tensor(seeds, len(slots), self.device)
             if lengths is not None:                 # checks the lengths before its first launch
                 self._slots.reset(slots, lengths)
             self._win.reset(slots)
             if seeds is not None:                   # excitation phases and sample counts return to zero
-                self._nsf.reset(to_device(torch.tensor(slots, dtype=torch.long), self.device), seeds)
+                self._nsf.reset(to_device(torch.tensor(slots, dtype=torch.long), self.device), seeds.to(self.device))
 
 
 # --------------------------------------------------------------------------------------------

@@ -73,6 +73,26 @@ def stream_lookahead(generator, allow_lookahead, what):
     return plan.delay
 
 
+def _check_stream(sambert, generator, chunk_steps, nsf_f0, nsf_seeds, allow_lookahead, what):
+    """-> the vocoder's look-ahead (stream_lookahead), after the model checks stream_synthesize and TtsServer share: both
+    models in eval() (RuntimeError), and ValueError unless an NSF generator comes with nsf_f0 and nsf_seeds and any other
+    with neither, the acoustic model makes the mel channels the generator takes, and chunk_steps >= 1.  TtsServer, whose
+    seeds come with each request, passes nsf_seeds = () along with nsf_f0."""
+    if sambert.training or generator.training:
+        raise RuntimeError(f"{what} expects both models in eval() mode")
+    if generator.nsf_enable and (nsf_f0 is None or nsf_seeds is None):
+        raise ValueError(f"{what}: an NSF generator streams with nsf_f0 and nsf_seeds: its excitation must be seeded for "
+                         "the chunks to reproduce the whole utterance")
+    lookahead = stream_lookahead(generator, allow_lookahead, what)
+    num_mels = sambert.mel_postnet.num_mels
+    if not _check_nsf(num_mels, generator, nsf_f0, nsf_seeds, what) and generator.conv_pre.conv1d.spec.c_in != num_mels:
+        raise ValueError(f"{what}: the acoustic model makes {num_mels} mel channels, the generator takes "
+                         f"{generator.conv_pre.conv1d.spec.c_in}")
+    if int(chunk_steps) < 1:
+        raise ValueError(f"{what}: chunk_steps must be >= 1, got {chunk_steps}")
+    return lookahead
+
+
 @torch.no_grad()
 def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None):
     """sambert: ``KanTtsSAMBERT`` in eval(); generator: ``Generator`` in eval() (``remove_weight_norm()`` optional --
@@ -115,22 +135,9 @@ def stream_synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_sp
     audio is ``pqmf.synthesis(generator(mel_b))`` of exactly its frames, later by the synthesis's taps/2 samples (plus the
     generator's own look-ahead when it is non-causal).  Against ``synthesize``, a shorter utterance of the batch differs in
     its last taps/2 samples, where the padded batch's synthesis reads the generator's output past the utterance's end."""
-    if sambert.training or generator.training:
-        raise RuntimeError("stream_synthesize() expects both models in eval() mode")
-    if generator.nsf_enable and (nsf_f0 is None or nsf_seeds is None):
-        raise ValueError("stream_synthesize(): an NSF generator streams with nsf_f0 and nsf_seeds: its excitation must be "
-                         "seeded for the chunks to reproduce the whole utterance")
-    stream_lookahead(generator, allow_lookahead, "streaming")
-    num_mels = sambert.mel_postnet.num_mels
-    nsf = _check_nsf(num_mels, generator, nsf_f0, nsf_seeds, "stream_synthesize()")     # checks the NSF channels
-    if not nsf and generator.conv_pre.conv1d.spec.c_in != num_mels:
-        raise ValueError(f"stream_synthesize(): the acoustic model makes {num_mels} mel channels, the generator takes "
-                         f"{generator.conv_pre.conv1d.spec.c_in}")
-    chunk_steps = int(chunk_steps)
-    if chunk_steps < 1:
-        raise ValueError(f"stream_synthesize(): chunk_steps must be >= 1, got {chunk_steps}")
-    return TtsStream(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps, nsf_f0,
-                     nsf_seeds)
+    lookahead = _check_stream(sambert, generator, chunk_steps, nsf_f0, nsf_seeds, allow_lookahead, "stream_synthesize()")
+    return TtsStream(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, int(chunk_steps),
+                     lookahead, nsf_f0, nsf_seeds)
 
 
 class TtsStream:
@@ -138,16 +145,17 @@ class TtsStream:
 
     ``lengths``: per-slot sample counts, ``LR_length_rounded[b] * hop`` (read on the host once, before decoding).
     ``hop``: the vocoder's samples per frame (GeneratorStreamer.hop: prod(upsample_scales), times S for a multi-band one).
-    ``lookahead``: the vocoder's delay in samples (GeneratorStreamer.delay; 0 for a causal full-band one): the push of the frames
-    [p, p + f) returns the samples [p·hop - lookahead, (p + f)·hop - lookahead), and the samples before 0 are not
-    yielded; after the last decoder step the vocoder's drain (GeneratorStreamer.finish) brings out the rest.
+    ``delay`` / ``lookahead``: the post-net's delay in rows and the vocoder's in samples (GeneratorStreamer.delay; 0 for a
+    causal full-band one).  The post-net's push of the decoder rows [p, p + f) returns the frames [p - delay, p + f -
+    delay), the vocoder's push of the frames [p, p + f) the samples [p·hop - lookahead, (p + f)·hop - lookahead); what
+    lies before 0 is dropped, and after the last decoder step each streamer's drain (``finish``) brings out the rest.
     Iterating yields ``(start_sample, wav)``, ``wav`` (B, 1, n) on the device, n > 0, with starts contiguous from 0; slot
     b's audio ends at lengths[b] and is padding after that.  From the first chunk to the last no device data is read on
     the host.  A stream is iterated once."""
 
     def __init__(self, sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, chunk_steps,
-                 nsf_f0=None, nsf_seeds=None):
-        self.sambert, self.chunk_steps, self.nsf_f0 = sambert, chunk_steps, nsf_f0
+                 lookahead, nsf_f0=None, nsf_seeds=None):
+        self.sambert, self.chunk_steps, self.lookahead, self.nsf_f0 = sambert, chunk_steps, lookahead, nsf_f0
         dec = sambert.mel_decoder
         self.r, self.d_mel = dec.r, dec.d_mel
         with torch.no_grad():
@@ -156,29 +164,28 @@ class TtsStream:
         frames = f["lr_len"]
         self.max_frames = F = self.r * chunk_steps
         self._post = sambert.mel_postnet.streamer(B, F, frames)
+        self.delay = self._post.delay
         # a vocoder with a look-ahead (non-causal, or multi-band: the PQMF synthesis) masks each slot's utterance end on the
         # device, from the lengths the decoder masks by
-        self._voc = generator.streamer(batch=B, max_frames=F, lengths=frames if StreamPlan(generator).delay else None,
-                                       seeds=nsf_seeds)
-        self.hop, self.lookahead = self._voc.hop, self._voc.delay
+        self._voc = generator.streamer(batch=B, max_frames=F, lengths=frames if lookahead else None, seeds=nsf_seeds)
+        self.hop = self._voc.hop
         self.lengths = [int(n) * self.hop for n in frames.cpu()]
         self._used = False
 
     @staticmethod
-    def _audio(wav, start):
-        """The vocoder's output wav (B, 1, n) for the samples from ``start`` on -> [(start sample, wav)] without the samples
-        before 0 (none when it holds only those)."""
+    def _from_zero(x, start, dim):
+        """x, a delayed streamer's output whose entries along ``dim`` are the stream's positions from ``start`` on ->
+        [(its first position from 0 on, x without the positions before 0)], [] when x holds only those."""
         lo = max(0, -start)
-        return [(start + lo, wav[..., lo:])] if lo < wav.shape[-1] else []
+        return [(start + lo, x.narrow(dim, lo, x.shape[dim] - lo))] if lo < x.shape[dim] else []
 
     def _vocode(self, rows, start):
         """rows (B, n, num_mels) of final post-net output -> [(start sample, wav)] in pieces of at most max_frames frames,
         and the start of the next piece."""
         out = []
         for piece in torch.split(rows, self.max_frames, dim=1):
-            if piece.shape[1]:
-                out += self._audio(self._voc.push(piece.transpose(1, 2)), start)
-                start += piece.shape[1] * self.hop
+            out += self._from_zero(self._voc.push(piece.transpose(1, 2)), start, 2)
+            start += piece.shape[1] * self.hop
         return out, start
 
     def __iter__(self):
@@ -199,16 +206,17 @@ class TtsStream:
                 outs = []
                 frames = torch.arange(row, row + dec.shape[1], device=dec.device)
                 dec = dec.masked_fill((frames[None, :] >= f["lr_len"][:, None]).unsqueeze(-1), 0)
-                row += dec.shape[1]
                 rows = self._post.push(dec)
                 if last:
                     rows = torch.cat([rows, self._post.finish()], 1)
-                if self.nsf_f0 is not None:
-                    rows = denorm_f0(rows, self.nsf_f0)
-                chunks, start = self._vocode(rows, start)
-                yield from chunks
+                for _, mel in self._from_zero(rows, row - self.delay, 1):
+                    if self.nsf_f0 is not None:
+                        mel = denorm_f0(mel, self.nsf_f0)
+                    chunks, start = self._vocode(mel, start)
+                    yield from chunks
+                row += dec.shape[1]
             if self.lookahead:
-                yield from self._audio(self._voc.finish(), start)
+                yield from self._from_zero(self._voc.finish(), start, 2)
 
 
 def slot_schedule(r, chunk_steps, delay, frames, steps, chunk, max_steps, hop=1, lookahead=0):
@@ -280,21 +288,12 @@ class TtsServer:
 
     def __init__(self, sambert, generator, slots, chunk_steps, max_steps, nsf_f0=None, allow_lookahead=False):
         from .sambert import PostNetStreamPlan
-        if sambert.training or generator.training:
-            raise RuntimeError("TtsServer expects both models in eval() mode")
-        self.lookahead = stream_lookahead(generator, allow_lookahead, "serving")
-        num_mels = sambert.mel_postnet.num_mels
+        self.lookahead = _check_stream(sambert, generator, chunk_steps, nsf_f0, None if nsf_f0 is None else (),
+                                       allow_lookahead, "TtsServer")
         self.nsf = generator.nsf_enable
-        if self.nsf:
-            _check_nsf(num_mels, generator, nsf_f0, (), "TtsServer")
-        elif nsf_f0 is not None:
-            raise ValueError("TtsServer: nsf_f0 is for NSF generators")
-        elif generator.conv_pre.conv1d.spec.c_in != num_mels:
-            raise ValueError(f"TtsServer: the acoustic model makes {num_mels} mel channels, the generator takes "
-                             f"{generator.conv_pre.conv1d.spec.c_in}")
         self.chunk_steps, self.max_steps, self.batch = int(chunk_steps), int(max_steps), int(slots)
-        if self.chunk_steps < 1 or self.max_steps < 1 or self.batch < 1:
-            raise ValueError(f"TtsServer: slots ({slots}), chunk_steps ({chunk_steps}) and max_steps ({max_steps}) must be >= 1")
+        if self.max_steps < 1 or self.batch < 1:
+            raise ValueError(f"TtsServer: slots ({slots}) and max_steps ({max_steps}) must be >= 1")
         dec = sambert.mel_decoder
         self.r, self.d_mel = dec.r, dec.d_mel
         self.delay = PostNetStreamPlan(sambert.mel_postnet).delay
@@ -307,7 +306,7 @@ class TtsServer:
         self._dec = dec.slots(self.batch, self.max_steps)
         with torch.no_grad():
             self._post = sambert.mel_postnet.streamer(self.batch, F, torch.zeros(self.batch, dtype=torch.int32,
-                                                                                 device=self.device), per_slot=True)
+                                                                                 device=self.device))
             # every slot is reset, with its request's frame count and seed, before its first audio
             self._voc = generator.streamer(batch=self.batch, max_frames=F, lengths=[1] * self.batch if self.lookahead else None,
                                            seeds=[0] * self.batch if self.nsf else None)
@@ -352,7 +351,7 @@ class TtsServer:
         del self._queue[:len(take)]
         for b, req, fr, n, s in zip(free, take, fronts, frames, sched):
             self._dec.admit(b, fr["memory"], fr["band_width_rows"])
-            self._post.reset([n], slots=[b], start_row=s["start_step"] * self.r)
+            self._post.reset([b], [n], start_row=s["start_step"] * self.r)
             seed = None if req["seed"] is None else torch.tensor([int(req["seed"])], dtype=torch.int64).to(self.device)
             self._slots[b] = dict(s, chunk=c, id=req["id"], frames=n, samples=n * self.hop, seed=seed)
             self._playing.append((b, self._slots[b]))

@@ -38,7 +38,7 @@ import torch.nn.functional as F
 from . import ops
 from . import sambert_ops as sops
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, ptr
-from .stream import SlotUtterances, Windows, WindowTable, own_weight
+from .stream import Streamer, WindowTable, own_weight
 
 
 def get_mask_from_lengths(lengths, max_len=None):
@@ -851,11 +851,12 @@ class PostNet(nn.Module):
         h, _ = self.lstm(self.fsmn(x, mask))
         return self.fc(h, resid=resid)
 
-    def streamer(self, batch, max_frames, lengths, per_slot=False):
+    def streamer(self, batch, max_frames, lengths):
         """-> a PostNetStreamer that runs this (eval-mode) post-net chunk by chunk over ``batch`` utterances of ``lengths``
-        (device tensor (batch,)) frames, at most ``max_frames`` decoder rows per chunk.  ``per_slot``: every slot keeps its
-        own frame count on the device and ``reset(slots=...)`` starts an utterance in some slots (see PostNetStreamer)."""
-        return PostNetStreamer(self, batch, max_frames, lengths, per_slot)
+        (host ints or device tensor (batch,)) frames, at most ``max_frames`` decoder rows per chunk.  Its output trails
+        the decoder rows by ``delay`` rows; ``reset(slots, lengths, start_row)`` starts utterances in some slots (see
+        PostNetStreamer)."""
+        return PostNetStreamer(self, batch, max_frames, lengths)
 
 
 # One launch of a post-net chunk over named windows.  kind "conv": a k = 1 conv of ``module`` (a Linear, or the nn.LSTM's
@@ -912,42 +913,35 @@ class PostNetStreamPlan:
         self.launches_per_chunk = table.launches_per_chunk(len(self.steps)) + 1
 
 
-class PostNetStreamer:
+class PostNetStreamer(Streamer):
     """Chunk-by-chunk PostNet (PostNet.streamer) over decoder rows that arrive step by step.
 
     ``push(dec_rows)`` takes the next (B, f, num_mels) decoder rows of every slot (de-LFR'd and masked, 1 <= f <=
-    max_frames) and returns the post-net output rows ``fc(lstm(fsmn(x))) + x``, masked beyond each slot's length, that have
-    become final: f rows in the steady state, fewer while the first ``delay`` rows are held back.  ``finish()`` pushes
-    ``delay`` all-padding rows and returns the rest; the rows returned in order are then the whole-sequence post-net output.
-    ``reset(lengths=None)`` starts a new batch.  No call reads device data on the host.
+    max_frames) and returns f rows of the post-net output ``fc(lstm(fsmn(x))) + x``: row t of slot b is frame
+    frames_done[b] - delay + t of its utterance (frames_done counts the decoder rows since its frame 0), zero outside
+    [0, lengths[b]).  ``finish()`` pushes ``delay`` all-padding rows and returns their output.  The rows returned in
+    order from frame 0 on are then the whole-sequence post-net output.  ``reset(slots, lengths, start_row)`` starts new
+    utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  A slot's
+    new utterance must start after the previous one's last row was returned.  No call reads device data on the host.
 
     Every chunk runs over all f rows of every slot.  Where each slot is in its utterance lives on the device
     (stream.SlotUtterances, whose frames are the decoder rows).  A tensor a layer reads before the chunk lives in a window
     (stream.py).  The memory blocks (kt_fsmn_fwd_stream_slots) read frames outside [0, lengths[b]) as zeros, the
     whole-sequence padding, and the LSTM (kt_lstm_stream_slots) starts from zeros at frame 0, so starting an utterance
     clears no window history or LSTM state; every other step reads only the frame it writes, and the output is masked
-    outside the utterance.  The weights are prepared once, when the streamer is created.
+    outside the utterance.  The weights are prepared once, when the streamer is created."""
 
-    Per-slot mode (``per_slot=True``): ``push`` returns all f rows of every slot, output row t being frame
-    frames_done[b] - delay + t (zero outside [0, lengths[b])).  ``reset(lengths, slots=..., start_row=...)`` starts new
-    utterances in the given slots with frame 0 at row ``start_row`` of the next push; the other slots go on.  A slot's new
-    utterance must start after the previous one's last row was returned."""
+    out, f_axis = "out", 1
 
-    def __init__(self, postnet, batch, max_frames, lengths, per_slot=False):
-        self.plan = plan = PostNetStreamPlan(postnet)
-        self._win = win = Windows(plan.windows, batch, max_frames, next(postnet.parameters()).device, "post-net streamer")
-        self.batch, self.max_frames, self.delay, self.device = win.batch, win.max_frames, plan.delay, win.device
-        self.num_mels, self.hidden = postnet.num_mels, postnet.lstm.hidden_size
-        self.per_slot = bool(per_slot)
+    def __init__(self, postnet, batch, max_frames, lengths):
+        plan = PostNetStreamPlan(postnet)
+        super().__init__(plan, batch, max_frames, next(postnet.parameters()).device, "post-net streamer", masked=True,
+                         in_channels=postnet.num_mels)
+        self.hidden = postnet.lstm.hidden_size
         self._state = torch.zeros(self.batch, 2, self.hidden, device=self.device)
-        self._zeros = torch.zeros(self.batch, self.max_frames, self.num_mels, device=self.device)
-        self._slots = SlotUtterances(self.batch, self.device)
-        self._masks = {name: self._slots.mask(1, lag) for name, lag in plan.lags.items()}
-        self._places = [None if st.kind == "lstm" else win.place(st.src, st.dst, st.resid, res_lag=st.res_lag)
-                        for st in plan.steps]
         with torch.no_grad(), torch.cuda.device(self.device):
             self._weights = [self._own_weight(st) for st in plan.steps]
-            self.reset(lengths)
+            self.reset(range(self.batch), lengths)
 
     @staticmethod
     def _own_weight(st):
@@ -962,9 +956,8 @@ class PostNetStreamer:
             return (spec, *own_weight(spec, mod.weight_ih_l0.unsqueeze(-1), None, mod.bias_ih_l0 + mod.bias_hh_l0))
         return (mod.spec, *own_weight(mod.spec, mod.weight, None, mod.bias))
 
-    def _chunk(self, f, skip):
-        """Every launch of one chunk of f decoder rows (already in the "dec" window) -> output rows [skip, f) of every slot,
-        zero where a row's frame lies outside its slot's utterance."""
+    def _chunk(self, f):
+        """Every launch of one chunk of f decoder rows (already in the "dec" window)."""
         b, B, masks = self._win.buf, self.batch, self._masks
         for st, w, place in zip(self.plan.steps, self._weights, self._places):
             src, dst, resid = b[st.src], b[st.dst], None if st.resid is None else b[st.resid]
@@ -978,43 +971,23 @@ class PostNetStreamer:
             else:
                 ops.call("kt_lstm_stream_slots", ptr(src), ptr(w), ptr(self._state), ptr(dst), ctypes.byref(masks[st.src]),
                          B, f, self.hidden, src.shape[1], dst.shape[1])
-        self._slots.mask_advance(masks["out"], b["out"], self._win.first["out"], f, f)
-        self._win.advance(f)
-        return b["out"][:, skip:f].clone(memory_format=torch.contiguous_format)
+        self._end_chunk(f)
 
     def push(self, dec_rows):
-        """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, n, num_mels) post-net rows that became final
-        (per-slot mode: all f rows)."""
+        """dec_rows: (B, f, num_mels), 1 <= f <= max_frames -> the (B, f, num_mels) post-net rows ``delay`` rows behind
+        them."""
         with torch.no_grad(), torch.cuda.device(self.device):
             f = self._win.push("dec", dec_rows, 1, ("{} decoder rows", "rows", "the rows are"))
-            skip = 0 if self.per_slot else min(f, max(0, self.delay - self._rows))    # rows before frame 0
-            self._rows += f
-            return self._chunk(f, skip)
+            self._chunk(f)
+            return self._output(f)
 
-    def finish(self):
-        """Push ``delay`` all-padding rows (the whole-sequence zero padding) -> the remaining (B, n, num_mels) output rows."""
-        outs, left = [], self.delay
-        while left > 0:
-            f = min(left, self.max_frames)
-            outs.append(self.push(self._zeros[:, :f]))
-            left -= f
-        return torch.cat(outs, 1) if outs else self._zeros[:, :0].clone()
-
-    def reset(self, lengths=None, slots=None, start_row=0):
-        """Start a new batch: every slot's frame 0 is row 0 of the next push; ``lengths`` (host ints or a device tensor,
-        (batch,)), when given, replaces the slots' frame counts.
-
-        Per-slot mode with ``slots`` (host ints): only those slots start new utterances, of ``lengths`` frames (in the
-        order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames); the
-        other slots go on.  Neither form clears a window or the LSTM state, and neither reads device data."""
-        if slots is None:
-            start_row = 0
-        elif not self.per_slot:
-            raise ValueError("reset: slots are for a per-slot streamer (PostNet.streamer(..., per_slot=True))")
-        elif not 0 <= int(start_row) < self.max_frames:
+    def reset(self, slots, lengths, start_row=0):
+        """The given slots (host ints) start new utterances of ``lengths`` frames (host ints or a device tensor, in the
+        order of ``slots``), with frame 0 at row ``start_row`` of the next push (0 <= start_row < max_frames); the other
+        slots go on.  Clears no window or LSTM state and reads no device data."""
+        if not 0 <= int(start_row) < self.max_frames:
             raise ValueError(f"reset: start_row must lie in [0, {self.max_frames}), got {start_row}")
         self._slots.reset(slots, lengths, start_row)
-        self._rows = 0                                     # (read in lockstep mode only)
 
 
 class FP_Predictor(nn.Module):

@@ -1,5 +1,5 @@
 """The stream window format of the streamed vocoder (hifigan.GeneratorStreamer) and post-net (sambert.PostNetStreamer),
-and the per-slot utterance record both keep, DESIGN.md §3.7.  A window is a persistent (B, H + F·rows_per_frame, C)
+the per-slot utterance record both keep, and the scaffolding both build on (Streamer), DESIGN.md §3.7.  A window is a persistent (B, H + F·rows_per_frame, C)
 buffer: rows [0, H) carry the last H rows of the earlier chunks (zeros after a reset: the causal padding), the chunk is
 written at row H, and H is the largest history any reader of the tensor needs."""
 import ctypes
@@ -52,7 +52,6 @@ class Windows:
                                                   rows_per_frame=w["rows_per_frame"]) for w in kept])
         self._table = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(device)
         self._ntable, self._max_c = len(kept), max([w["channels"] for w in kept], default=1)
-        self._all = torch.ones(batch, dtype=torch.uint8, device=device)
 
     def push(self, name, x, f_axis, what):
         """Check the chunk x, (B, C, f) for f_axis 2 or (B, f, C) for f_axis 1, and write it into window ``name`` -> f.
@@ -84,13 +83,11 @@ class Windows:
         if self._ntable:
             ops.call("kt_stream_advance", ptr(self._table, True), self._ntable, self.batch, frames, self._max_c)
 
-    def reset(self, slots=None):
-        """The history of the given slots (None: all) returns to zeros in every window (one launch)."""
-        sel = self._all
-        if slots is not None:
-            mask = torch.zeros(self.batch, dtype=torch.uint8)
-            mask[check_slots(slots, self.batch)] = 1
-            sel = to_device(mask, self.device)
+    def reset(self, slots):
+        """The history of the given slots returns to zeros in every window (one launch)."""
+        mask = torch.zeros(self.batch, dtype=torch.uint8)
+        mask[check_slots(slots, self.batch)] = 1
+        sel = to_device(mask, self.device)
         if self._ntable:
             ops.call("kt_stream_reset", ptr(self._table, True), self._ntable, self.batch, ptr(sel, True), self._max_c)
 
@@ -105,19 +102,18 @@ class SlotUtterances:
         self.frames_done = torch.zeros(batch, dtype=torch.int32, device=device)
 
     def reset(self, slots, lengths, start_row=0):
-        """``slots`` (host ints; None: all) start utterances of ``lengths`` frames (host ints or CUDA tensor; None:
-        kept) at chunk row ``start_row`` of the next push.  All checked before the first launch; none waits."""
-        slots = list(range(self.batch)) if slots is None else check_slots(slots, self.batch)
+        """``slots`` (host ints) start utterances of ``lengths`` frames (host ints or CUDA tensor) at chunk row
+        ``start_row`` of the next push.  All checked before the first launch; none waits."""
+        slots = check_slots(slots, self.batch)
         idx = to_device(torch.tensor(slots, dtype=torch.long), self.device)
-        if lengths is not None:
-            if not (torch.is_tensor(lengths) and lengths.is_cuda):
-                lengths = torch.as_tensor(lengths, dtype=torch.int32)
-                if lengths.numel() and int(lengths.min()) < 1:
-                    raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
-                lengths = to_device(lengths, self.device)
-            if lengths.numel() != len(slots):
-                raise ValueError(f"streamer: expected {len(slots)} lengths, got {lengths.numel()}")
-            self.lengths.index_copy_(0, idx, lengths.to(self.device, torch.int32).reshape(-1))
+        if not (torch.is_tensor(lengths) and lengths.is_cuda):
+            lengths = torch.as_tensor(lengths, dtype=torch.int32)
+            if lengths.numel() and int(lengths.min()) < 1:
+                raise ValueError(f"streamer: lengths must be >= 1 frame, got {lengths.tolist()}")
+            lengths = to_device(lengths, self.device)
+        if lengths.numel() != len(slots):
+            raise ValueError(f"streamer: expected {len(slots)} lengths, got {lengths.numel()}")
+        self.lengths.index_copy_(0, idx, lengths.to(self.device, torch.int32).reshape(-1))
         self.frames_done.index_fill_(0, idx, -int(start_row))
 
     def mask(self, rows_per_frame, lag):
@@ -128,6 +124,57 @@ class SlotUtterances:
         """One launch: zero the chunk rows [first, first + rows) outside each utterance, then frames_done += frames."""
         ops.call("kt_stream_mask_advance", ctypes.byref(mask), ptr(window_buf), self.batch, rows, window_buf.shape[2],
                  window_buf.shape[1], first, frames)
+
+
+class Streamer:
+    """What a streamer of a plan keeps besides its own steps: the plan's windows, the KtStreamWin of every step record
+    with src / dst / resid / res_lag fields (others: None), and when ``masked`` the slots' utterances with one
+    KtStreamMask per window of ``plan.lags``.  A subclass names its output window ``out`` and the frame axis ``f_axis``
+    of the chunks it takes and returns (2: (B, C, f), 1: (B, f, C)).
+
+    A push of f frames returns f frames' output rows, ``delay`` (the plan's) rows behind the pushed frames; a masked
+    stream zeroes the rows outside each slot's utterance, those before its frame 0 included.  ``finish()`` pushes the
+    ``drain_frames`` frames of zeros (``in_channels`` wide) that bring out the last ``delay`` rows."""
+
+    out = f_axis = None
+
+    def __init__(self, plan, batch, max_frames, device, what, masked, in_channels):
+        self.plan = plan
+        self._win = win = Windows(plan.windows, batch, max_frames, device, what)
+        self.batch, self.max_frames, self.device, self.delay = win.batch, win.max_frames, win.device, plan.delay
+        self.drain_frames = -(-self.delay // win.rate[self.out])
+        self._places = [win.place(st.src, st.dst, st.resid, res_lag=st.res_lag) if hasattr(st, "res_lag") else None
+                        for st in plan.steps]
+        self._slots = self._masks = self._zeros = None
+        if masked:
+            self._slots = SlotUtterances(self.batch, self.device)
+            self._masks = {name: self._slots.mask(win.rate[name], lag) for name, lag in plan.lags.items()}
+        if self.drain_frames:
+            self._zeros = torch.zeros(self.batch, self.max_frames, in_channels, device=self.device).movedim(1, self.f_axis)
+
+    def _end_chunk(self, f):
+        """After the steps of a chunk of f frames: zero the output rows outside each slot's utterance and advance its
+        frames_done (masked only), then move every window's history (one launch each)."""
+        win, out = self._win, self.out
+        if self._slots is not None:
+            self._slots.mask_advance(self._masks[out], win.buf[out], win.first[out], f * win.rate[out], f)
+        win.advance(f)
+
+    def _output(self, f):
+        """-> a copy of the output window's rows of a chunk of f frames, frames on axis f_axis."""
+        win, out = self._win, self.out
+        rows = win.buf[out][:, win.first[out]:win.first[out] + f * win.rate[out]]
+        return rows.movedim(1, self.f_axis).clone(memory_format=torch.contiguous_format)
+
+    def finish(self):
+        """Push ``drain_frames`` frames of zeros, at most max_frames at a time -> their output, which ends with the last
+        row of every utterance pushed to its end (none without a delay)."""
+        outs, left = [], self.drain_frames
+        while left > 0:
+            f = min(left, self.max_frames)
+            outs.append(self.push(self._zeros.narrow(self.f_axis, 0, f)))
+            left -= f
+        return torch.cat(outs, self.f_axis) if outs else self._output(0)
 
 
 def check_slots(slots, batch):

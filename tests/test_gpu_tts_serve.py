@@ -1,7 +1,8 @@
 """Continuous-batching text-to-speech on the GPU: kt_pnca_step_slots equals plain torch attention over each slot's bands;
-the slot decoder gives each utterance's batch-1 infer_steps rows with staggered starts; the per-slot post-net gives each
-slot's lockstep rows bit for bit; TtsServer gives every request synthesize()'s audio of that request alone, bit for bit
-whether the other slots are busy or idle, for plain and NSF generators, without synchronising between admissions."""
+the slot decoder gives each utterance's batch-1 infer_steps rows with staggered starts; the post-net with staggered slot
+resets gives each slot the rows of that utterance streamed alone, bit for bit; TtsServer gives every request
+synthesize()'s audio of that request alone, bit for bit whether the other slots are busy or idle, for plain and NSF
+generators, without synchronising between admissions."""
 import pytest
 import torch
 
@@ -158,8 +159,8 @@ def test_slot_decoder_matches_batch1_infer_steps(golden):
         assert err <= 1e-5
 
 
-# ---- per-slot post-net ---------------------------------------------------------------------------------------------------
-def test_per_slot_postnet_equals_lockstep_alone_bitwise():
+# ---- post-net slot resets ------------------------------------------------------------------------------------------------
+def test_postnet_slot_resets_give_each_utterance_its_rows_alone_bitwise():
     torch.manual_seed(3)
     pn = PostNet(K.sambert_24k_config()).to(DEV).eval()
     lens, starts, T = [30, 7, 22], [0, 5, 13], 30
@@ -168,7 +169,7 @@ def test_per_slot_postnet_equals_lockstep_alone_bitwise():
     chunks = [4, 7, 1, 9, 12, 3, 12, 12, 12]
     total = sum(chunks)
     with torch.no_grad(), _exact():
-        st = pn.streamer(3, max(chunks), torch.zeros(3, dtype=torch.int32, device=DEV), per_slot=True)
+        st = pn.streamer(3, max(chunks), torch.zeros(3, dtype=torch.int32, device=DEV))
         rows = torch.zeros(3, total, 80, device=DEV)
         for b in range(3):
             rows[b, starts[b]:starts[b] + lens[b]] = dec[b][0]
@@ -176,7 +177,7 @@ def test_per_slot_postnet_equals_lockstep_alone_bitwise():
         for f in chunks:
             for b in range(3):
                 if r0 <= starts[b] < r0 + f:
-                    st.reset([lens[b]], slots=[b], start_row=starts[b] - r0)
+                    st.reset([b], [lens[b]], start_row=starts[b] - r0)
             outs.append(st.push(rows[:, r0:r0 + f]))
             r0 += f
         got = torch.cat(outs, 1)
@@ -184,27 +185,30 @@ def test_per_slot_postnet_equals_lockstep_alone_bitwise():
         for b in range(3):
             one = pn.streamer(1, 6, torch.tensor([lens[b]], device=DEV))
             want = torch.cat([one.push(c) for c in torch.split(dec[b], 6, 1)] + [one.finish()], 1)
+            assert want.shape[1] == one.delay + lens[b]
+            assert torch.equal(want[:, :one.delay], torch.zeros_like(want[:, :one.delay]))     # the rows before frame 0
+            want = want[:, one.delay:]
             first = starts[b] + st.delay                 # output row of frame 0
             assert torch.equal(got[b, first:first + lens[b]], want[0]), b
             assert torch.equal(got[b, :first], torch.zeros_like(got[b, :first]))
             assert torch.equal(got[b, first + lens[b]:], torch.zeros_like(got[b, first + lens[b]:]))
 
 
-def test_rejected_per_slot_postnet_reset_leaves_the_stream_as_it_was():
+def test_rejected_postnet_slot_reset_leaves_the_stream_as_it_was():
     torch.manual_seed(3)
     pn = PostNet(K.sambert_24k_config()).to(DEV).eval()
     rows = torch.randn(2, 24, 80, generator=torch.Generator().manual_seed(5)).to(DEV)
     outs = {}
     with torch.no_grad(), _exact():
         for rejected in (False, True):
-            st = pn.streamer(2, 8, torch.zeros(2, dtype=torch.int32, device=DEV), per_slot=True)
-            st.reset([20, 13], slots=[0, 1], start_row=0)
+            st = pn.streamer(2, 8, torch.zeros(2, dtype=torch.int32, device=DEV))
+            st.reset([0, 1], [20, 13], start_row=0)
             got = [st.push(rows[:, :8])]
             if rejected:
                 with pytest.raises(ValueError, match="distinct"):
-                    st.reset([5, 5], slots=[1, 1], start_row=2)
+                    st.reset([1, 1], [5, 5], start_row=2)
                 with pytest.raises(ValueError, match="start_row"):
-                    st.reset([5], slots=[1], start_row=8)
+                    st.reset([1], [5], start_row=8)
             got += [st.push(rows[:, t:t + 8]) for t in (8, 16)]
             outs[rejected] = torch.cat(got, 1)
     assert torch.equal(outs[True], outs[False])

@@ -43,14 +43,19 @@ def _postnet_case():
 
 
 def _stream_postnet(pn, dec, lengths, schedule):
+    """-> the streamed rows from frame 0 on, after checking that every push returns its f rows, the first ``delay`` (before
+    frame 0) zero."""
     st = pn.streamer(batch=dec.shape[0], max_frames=max(schedule), lengths=lengths)
     outs = [st.push(c) for c in torch.split(dec, schedule, 1)]
-    assert sum(o.shape[1] for o in outs) == max(0, T - st.delay)
-    return torch.cat(outs + [st.finish()], 1)
+    assert [o.shape[1] for o in outs] == list(schedule)
+    got = torch.cat(outs + [st.finish()], 1)
+    assert got.shape[1] == T + st.delay
+    assert torch.equal(got[:, :st.delay], torch.zeros_like(got[:, :st.delay]))
+    return got[:, st.delay:]
 
 
 @pytest.mark.parametrize("schedule", sorted(SCHEDULES))
-def test_postnet_streamer_matches_forward(schedule):
+def test_postnet_streamer_rows_from_frame_0_match_forward(schedule):
     pn, dec, lengths, mask = _postnet_case()
     with torch.no_grad():
         with _exact():
@@ -65,20 +70,22 @@ def test_postnet_streamer_matches_forward(schedule):
         assert rel_l2(got.cpu(), want.cpu()) <= 1e-4
 
 
-def test_postnet_streamer_reset_starts_a_new_batch():
+def test_postnet_streamer_reset_of_every_slot_starts_a_new_batch():
     pn, dec, lengths, mask = _postnet_case()
     other = torch.randn(dec.shape, generator=torch.Generator().manual_seed(8)).to(DEV)
     with torch.no_grad():
         st = pn.streamer(batch=dec.shape[0], max_frames=6, lengths=lengths)
         first = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
-        st.reset(lengths)
+        slots = range(dec.shape[0])
+        st.reset(slots, lengths)
         again = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
         # a batch cut off mid-stream leaves its rows in every window and its LSTM state carried: a reset clears neither
-        st.reset(torch.full_like(lengths, T))
+        st.reset(slots, torch.full_like(lengths, T))
         for c in torch.split(other[:, :16], 6, 1):
             st.push(c)
-        st.reset(lengths)
+        st.reset(slots, lengths)
         after = torch.cat([st.push(c) for c in torch.split(dec, 6, 1)] + [st.finish()], 1)
+    assert torch.equal(first[:, :st.delay], torch.zeros_like(first[:, :st.delay]))      # the rows before frame 0
     assert torch.equal(first, again)
     assert torch.equal(first, after)                  # first: the output of a fresh streamer
 
