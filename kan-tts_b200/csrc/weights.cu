@@ -100,7 +100,8 @@ __global__ void weight_grad_kernel(const float* __restrict__ dw, const float* __
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       long long i_fwd, i_bwd;
       L.map(a, i / L.k, i % L.k, i_fwd, i_bwd);
-      const float r = dw[L.transposed ? i_bwd : i_fwd] * scale;
+      // rounded before the accumulate (no fused multiply-add into dv): the sum is param.grad += grad of the plain kernel
+      const float r = __fmul_rn(dw[L.transposed ? i_bwd : i_fwd], scale);
       dvs[i] = accumulate ? dvs[i] + r : r;
     }
   }
@@ -264,7 +265,8 @@ __global__ void __launch_bounds__(256) weight_grad_tiled_kernel(const float* __r
       const long long row = (long long)(a0 + warp) * n + (long long)b0 * L.k;
       const float c1 = c1_s[warp], c2 = c2_s[warp];
       for (int i = lane; i < bt * L.k; i += 32) {
-        const float r = mode == 1 ? c1 * tile[warp][i] - c2 * v[row + i] : c1 * tile[warp][i];
+        // (mode 0 rounds the product before the accumulate, as weight_grad_kernel does)
+        const float r = mode == 1 ? c1 * tile[warp][i] - c2 * v[row + i] : __fmul_rn(c1, tile[warp][i]);
         dv[row + i] = accumulate ? dv[row + i] + r : r;
       }
     }

@@ -280,23 +280,43 @@ def tc_instance(c):
     return None if route is None else f"conv_tc_kernel<{route}, true, {'true' if c.masked else 'false'}>"
 
 
+def conv_phase_rows(spec, t_in, direction):
+    """The output rows M of each phase conv_phases makes for direction 0 (forward) or 1 (data gradient) of layer spec over
+    t_in input rows: a scatter (transposed forward, strided data gradient) has one phase per output residue mod stride,
+    an up-sampled data gradient one accumulating phase per up-sampled row."""
+    t_out = spec.t_out(t_in)
+    s = spec.stride
+
+    def scatter(n):
+        return [(n - r + s - 1) // s for r in range(min(s, n))]
+
+    if direction == 0:
+        return scatter(t_out) if spec.transposed else [t_out]
+    if spec.transposed:
+        return [t_in]
+    return scatter(t_in) if spec.upsample == 1 else [t_in] * spec.upsample
+
+
+def core_instance(M, cin_g, cout_g, groups, batch, stream=False, masked=False):
+    """The conv_core_kernel instance run_core launches for one phase of M output rows: cin_g / cout_g channels per group on
+    the contracted / produced side, batch items (x sub-sequences)."""
+    rn = 4 if cout_g > 64 else (2 if cout_g > 32 else 1)
+    kc = 4 if cin_g <= 4 else 16
+
+    def ctas(rm):
+        return -(-M // (8 * rm)) * groups * -(-cout_g // (32 * rn)) * batch
+
+    rm = 16
+    while rm > 4 and (ctas(rm) < 296 or M <= 4 * rm):
+        rm >>= 1
+    return f"conv_core_kernel<{rn}, {rm}, {kc}, {'true' if stream else 'false'}, {'true' if masked else 'false'}>"
+
+
 def core_instances(c):
     """The conv_core_kernel instances run_core launches for case c, one per phase (a transposed conv has `stride`)."""
     s = c.spec
-    t_out = s.t_out(c.t_in)
-    Ms = [(t_out - r + s.stride - 1) // s.stride for r in range(min(s.stride, t_out))] if s.transposed else [t_out]
-    cin_g, cout_g = s.c_in // s.groups, s.c_out // s.groups
-    rn = 4 if cout_g > 64 else (2 if cout_g > 32 else 1)
-    kc = 4 if cin_g <= 4 else 16
-    out = set()
-    for M in Ms:
-        def ctas(rm):
-            return -(-M // (8 * rm)) * s.groups * -(-cout_g // (32 * rn)) * c.B
-        rm = 16
-        while rm > 4 and (ctas(rm) < 296 or M <= 4 * rm):
-            rm >>= 1
-        out.add(f"conv_core_kernel<{rn}, {rm}, {kc}, true, {'true' if c.masked else 'false'}>")
-    return sorted(out)
+    return sorted({core_instance(M, s.c_in // s.groups, s.c_out // s.groups, s.groups, c.B, True, c.masked)
+                   for M in conv_phase_rows(s, c.t_in, 0)})
 
 
 def _spec_key(spec):
