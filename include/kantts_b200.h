@@ -204,6 +204,23 @@ int kt_stft_mel_bwd(const KtMelDesc* d, const float* dmel, const float* damp, co
  * loss.py:217-256); the caller zeroes out[0] once. */
 int kt_l1_sum(const float* a, const float* b, int64_t n, float scale, float* out, int32_t accumulate, void* stream);
 
+/* Feature-map columns of the multi-resolution spectrogram discriminator (SpecDiscriminator, hifigan.py:481-582).  Its
+ * (k, 1) convs also pad the width-1 frequency axis by p_l per side, so after layer l the map is
+ * [class_l x p_l | previous columns | class_l x p_l] around the centre (signal) column, and all columns of one class are
+ * the same sequence for every item.  rows [batch + classes][t][c]: the signal rows of the items, then one row block per
+ * class in birth order.  reach[k]: how far class k extends from the centre (the sum of the paddings up to its birth layer,
+ * strictly increasing from 1); width = 2 * reach[classes - 1] + 1 (1 without classes). */
+#define KT_SPEC_MAX_CLASSES 8
+typedef struct KtSpecColumnsDesc {
+  int32_t batch, t, c, classes;
+  int32_t reach[KT_SPEC_MAX_CLASSES];
+} KtSpecColumnsDesc;
+/* out [batch][t][width][c] (channels-last; the module returns its (batch, c, t, width) view) from rows. */
+int kt_spec_columns_fwd(const KtSpecColumnsDesc* d, const float* rows, float* out, void* stream);
+/* drows [batch + classes][t][c] (overwritten) = the gradient of rows: each item's centre column, and each class summed over
+ * its columns and the items in a fixed order (no atomics: reproducible bits). */
+int kt_spec_columns_bwd(const KtSpecColumnsDesc* d, const float* dout, float* drows, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * SAM-BERT acoustic model (kantts/models/sambert).  Activations are (B, L, C) rows -- the
  * reference's own layout for this model -- so nn.Linear and the transposed nn.Conv1d pairs

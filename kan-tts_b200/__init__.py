@@ -2,6 +2,7 @@
 
 Public surface = the reference's own module API for this path:
   hifigan.Generator / MultiPeriodDiscriminator / MultiScaleDiscriminator   (kantts.models)
+    / SpecDiscriminator / MultiSpecDiscriminator
   pqmf.PQMF (the multi-band generator's filter bank)                      (kantts.models.pqmf)
   audio.MelSpectrogram / stft                                             (kantts.utils.audio_torch)
   loss.* + criterion_builder                                              (kantts.train.loss)
@@ -22,7 +23,8 @@ from ._lib import build_library  # noqa: F401
 from . import ops, hifigan, pqmf, audio, loss, sambert_ops, sambert, train, infer, speaker, install as _install  # noqa: F401
 from .sambert import (KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss, AttentionCTCLoss,  # noqa: F401
                       AttentionBinarizationLoss, ConvAttention, KanTtsTextsyBERT, SeqCELoss)
-from .hifigan import Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator  # noqa: F401
+from .hifigan import (Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator, SpecDiscriminator,  # noqa: F401
+                      MultiSpecDiscriminator)
 from .pqmf import PQMF  # noqa: F401
 from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401

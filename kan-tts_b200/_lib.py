@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libkantts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu", "bert.cu"]
+SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu", "bert.cu", "spec_disc.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
 KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
@@ -58,6 +58,14 @@ class KtMelDesc(ctypes.Structure):
                [(n, ctypes.c_float) for n in ("eps", "ref_db", "min_db", "norm_scale", "norm_shift", "norm_lo", "norm_hi")]
 
 
+KT_SPEC_MAX_CLASSES = 8
+
+
+class KtSpecColumnsDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("batch", "t", "c", "classes")] + \
+               [("reach", ctypes.c_int32 * KT_SPEC_MAX_CLASSES)]
+
+
 class KtAttnDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("batch", "heads", "d_head", "lq", "lk", "q_stride", "k_stride",
                                               "v_stride", "o_stride", "mask_q_stride")] + \
@@ -86,6 +94,8 @@ PROTOTYPES = {
     "kt_stft_mel_fwd": [ctypes.POINTER(KtMelDesc), _P, _P, _P, _P, _P, _P, _P],
     "kt_stft_mel_bwd": [ctypes.POINTER(KtMelDesc), _P, _P, _P, _P, _P, _P, _P],
     "kt_l1_sum": [_P, _P, _L, _F, _P, _I, _P],
+    "kt_spec_columns_fwd": [ctypes.POINTER(KtSpecColumnsDesc), _P, _P, _P],
+    "kt_spec_columns_bwd": [ctypes.POINTER(KtSpecColumnsDesc), _P, _P, _P],
     "kt_conv1d_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_conv1d_tc_image_bytes": [ctypes.POINTER(KtConv1dDesc), _I],
     "kt_weight_pack_tc": [ctypes.POINTER(KtConv1dDesc), _I, _P, _P, _P],

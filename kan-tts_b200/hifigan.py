@@ -1,7 +1,8 @@
 """H100-native HiFi-GAN modules with the reference's module API.
 
 Drop-in replacements for ``kantts.models.hifigan.hifigan.{Generator, MultiPeriodDiscriminator,
-MultiScaleDiscriminator}`` (KAN-TTS kantts/models/hifigan/hifigan.py:22-478, layers.py:15-226):
+MultiScaleDiscriminator, SpecDiscriminator, MultiSpecDiscriminator}`` (KAN-TTS kantts/models/hifigan/hifigan.py:22-617,
+layers.py:15-226):
 same class names, constructor kwargs (yaml ``params``), forward signatures / return structure,
 ``state_dict`` keys and shapes, ``remove_weight_norm()`` and ``nsf_enable``; parameters are plain
 leaf ``nn.Parameter``s so ``torch.optim.Adam`` / ``DistributedDataParallel`` work unchanged.
@@ -12,8 +13,9 @@ at the module boundary (feature maps are returned as zero-copy permuted views).
 A multi-band generator (``out_channels`` = S > 1) emits S sub-band signals at 1/S of the sample rate; the PQMF filter bank
 (pqmf.py) turns them into the waveform.  Like the reference, the PQMF is not part of the generator: the model builder adds
 it next to the generator, and inference attaches it as ``generator.pqmf`` after loading; streaming (GeneratorStreamer)
-runs the attached PQMF's synthesis as its last stage.  Out of scope (SURVEY.md section 8a): MultiSpecDiscriminator and a
-multi-band NSF generator.
+runs the attached PQMF's synthesis as its last stage.  ``MultiSpecDiscriminator`` (the multi-resolution spectrogram
+discriminator, hifigan.py:481-617) trains on the STFT and conv kernels plus kt_spec_columns_fwd / _bwd.  Out of scope
+(SURVEY.md section 8a): a multi-band NSF generator.
 """
 import copy
 import ctypes
@@ -27,6 +29,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
+from .audio import stft
 from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, ptr
 from .stream import Streamer, WindowTable, check_slots, own_weight, to_device
 
@@ -76,6 +79,73 @@ def prefetch_weights(module, streams):
             for m in share:
                 v, g = m.effective_weight()
                 ops.prefetch_weight(m._cache, m.spec, v, g)
+
+
+def _spectral(d):
+    """Is any conv of sub-discriminator ``d`` spectral-normed?"""
+    return any(getattr(l[0], "norm", "") == "spectral" for l in d.convs)
+
+
+def _run_halves(forward, x, pair_nb):
+    """A spectral-normed sub-discriminator on a pair batch: the two calls of the reference, in ITS order (the power iteration
+    makes the order observable).  The discriminator phase evaluates the real waveforms first (trainer.py:560-561) -- with
+    pair_state("reuse") the batch is [re-generated | real], so the second half goes first.  -> ((out_a, out_b), (fmap_a,
+    fmap_b)), which _split_runs takes apart."""
+    st = ops._pair_state
+    if st is not None and st[0] == "reuse":
+        ob, fb = forward(x[pair_nb:])
+        oa, fa = forward(x[:pair_nb])
+    else:
+        oa, fa = forward(x[:pair_nb])
+        ob, fb = forward(x[pair_nb:])
+    return (oa, ob), (fa, fb)
+
+
+def _split_runs(outs, fmaps, nb, detach_b):
+    """Results of one pair-batch run over cat([ya, yb]) whose sub-discriminators either ran on the whole batch or per half
+    (_run_halves) -> ((outs_a, fmaps_a), (outs_b, fmaps_b)); ``detach_b``: the second result is returned detached."""
+    det = (lambda t: t.detach()) if detach_b else (lambda t: t)
+    ra, rb = ([], []), ([], [])
+    for o, fm in zip(outs, fmaps):
+        if isinstance(o, tuple):                       # a sub-discriminator that ran per half
+            (oa, ob), (fa, fb) = o, fm
+            fb = [det(f) for f in fb]
+            ob = det(ob)
+        else:
+            oa, ob = o[:nb], det(o[nb:])
+            fa, fb = [f[:nb] for f in fm], [det(f[nb:]) for f in fm]
+        ra[0].append(oa); ra[1].append(fa)
+        rb[0].append(ob); rb[1].append(fb)
+    return ra, rb
+
+
+def _run_parallel(y, jobs):
+    """Run the independent sub-discriminator calls ``jobs`` [(fn, may_take_side_stream)] -> ([outputs], [feature maps]).
+    On the GPU each call that may runs on a side stream of its own (fork / join around the loop; autograd replays the
+    same streams in backward, and CUDA-graph capture records the branches as parallel graph paths).  A spectral-normed
+    sub-discriminator stays on the calling stream: its parameters receive their gradients through autograd (w / sigma is
+    recomputed per forward), and with that chain on a side stream the gradient of the first layer's weight_orig was
+    intermittently lost when the sub-discriminator is used twice in one backward."""
+    par = y.is_cuda and _PARALLEL_STREAMS and len(jobs) > 1
+    if par:
+        cur = torch.cuda.current_stream()
+        streams = _side_streams(y.device, len(jobs))
+    outs, fmaps, forked = [], [], []
+    for i, (fn, side) in enumerate(jobs):
+        if par and side:
+            streams[i].wait_stream(cur)
+            forked.append(streams[i])
+            with torch.cuda.stream(streams[i]):
+                o, fm = fn()
+        else:
+            o, fm = fn()
+        outs.append(o)
+        fmaps.append(fm)
+    # join only the streams this call forked: under CUDA-graph capture, waiting on a pool stream whose last work was
+    # not captured (a spectral-normed job's slot that nothing else in the graph used) invalidates the capture
+    for s in forked:
+        cur.wait_stream(s)
+    return outs, fmaps
 
 
 def _split_pair(outs, fmaps, nb, detach_b):
@@ -1144,22 +1214,9 @@ class MultiScaleDiscriminator(nn.Module):
         assert ya.shape == yb.shape
         nb = ya.shape[0]
         outs, fmaps = self._run(torch.cat([ya, yb], 0), nb)
-        det = (lambda t: t.detach()) if detach_b else (lambda t: t)
-        ra, rb = ([], []), ([], [])
-        for o, fm in zip(outs, fmaps):
-            if isinstance(o, tuple):                       # a scale that ran per half
-                (oa, ob), (fa, fb) = o, fm
-                fb = [det(f) for f in fb]
-                ob = det(ob)
-            else:
-                oa, ob = o[:nb], det(o[nb:])
-                fa, fb = [f[:nb] for f in fm], [det(f[nb:]) for f in fm]
-            ra[0].append(oa); ra[1].append(fa)
-            rb[0].append(ob); rb[1].append(fb)
-        return ra, rb
+        return _split_runs(outs, fmaps, nb, detach_b)
 
     def _run(self, y, pair_nb):
-        y_d_rs, fmap_rs = [], []
         rows = y.transpose(1, 2).contiguous()                                 # (B, T, 1)
         inputs = [rows]
         for i in range(1, len(self.discriminators)):                          # the pooling chain is cheap and serial
@@ -1169,40 +1226,124 @@ class MultiScaleDiscriminator(nn.Module):
                 cat = ops.DwtFn.apply(rows.reshape(rows.shape[0], -1))        # (B, T2, 2) = cat([yl, yh], 1)
                 rows = self.aux_convs[i - 1].run(cat)                          # (B, T2, 1), lrelu fused
             inputs.append(rows)
-        par = y.is_cuda and _PARALLEL_STREAMS and len(self.discriminators) > 1
-        if par:                                                               # the scales themselves are independent
-            cur = torch.cuda.current_stream()
-            streams = _side_streams(y.device, len(self.discriminators))
 
         def run_scale(d, x):
-            if pair_nb is not None and any(getattr(l[0], "norm", "") == "spectral" for l in d.convs):
-                # the two calls of the reference, in ITS order (the power iteration makes the order observable): the
-                # discriminator phase evaluates the real waveforms first (trainer.py:560-561) -- with pair_state("reuse") the
-                # batch is [re-generated | real], so the second half goes first
-                st = ops._pair_state
-                if st is not None and st[0] == "reuse":
-                    ob, fb = d.forward_rows(x[pair_nb:])
-                    oa, fa = d.forward_rows(x[:pair_nb])
-                else:
-                    oa, fa = d.forward_rows(x[:pair_nb])
-                    ob, fb = d.forward_rows(x[pair_nb:])
-                return (oa, ob), (fa, fb)
+            if pair_nb is not None and _spectral(d):
+                return _run_halves(d.forward_rows, x, pair_nb)
             return d.forward_rows(x)
 
-        for i, d in enumerate(self.discriminators):
-            # a spectral-normed scale stays on the calling stream: its parameters receive their gradients through autograd
-            # (w / sigma is recomputed per forward), and with that chain on a side stream the gradient of the first layer's
-            # weight_orig was intermittently lost when the scale is used twice in one backward
-            side = par and not any(getattr(l[0], "norm", "") == "spectral" for l in d.convs)
-            if side:
-                streams[i].wait_stream(cur)
-                with torch.cuda.stream(streams[i]):
-                    y_d_r, fmap_r = run_scale(d, inputs[i])
-            else:
-                y_d_r, fmap_r = run_scale(d, inputs[i])
-            y_d_rs.append(y_d_r)
-            fmap_rs.append(fmap_r)
-        if par:
-            for s in streams:
-                cur.wait_stream(s)
-        return y_d_rs, fmap_rs
+        # the scales themselves are independent
+        return _run_parallel(y, [(lambda d=d, x=x: run_scale(d, x), not _spectral(d))
+                                 for d, x in zip(self.discriminators, inputs)])
+
+
+# --------------------------------------------------------------------------------------------
+# MultiSpecDiscriminator (hifigan.py:481-617)
+# --------------------------------------------------------------------------------------------
+
+
+class _SpecConv(_NormedConv):
+    """``norm_f(nn.Conv2d(cin, cout, (k, 1), (stride, 1), padding))`` of the spectrogram discriminator, computed as a Conv1d
+    over frames on channels-last rows.  ``pad_width``: the zero columns the layer adds on each side of the frequency axis
+    (the reference passes ``padding=(k-1)//2`` as an int, which pads that width-1 axis too; conv_post pads frames only)."""
+
+    def __init__(self, cin, cout, k, stride, pad_width, norm, act_out_slope=None):
+        pad = (k - 1) // 2
+        ref = nn.Conv2d(cin, cout, (k, 1), (stride, 1), padding=(pad, pad_width))
+        spec = ops.ConvSpec(c_in=cin, c_out=cout, kernel=k, stride=stride, pad_left=pad, pad_right=pad)
+        if act_out_slope is not None:
+            spec.act_out, spec.act_out_slope = KT_ACT_LRELU, float(act_out_slope)
+        super().__init__(ref, spec, norm)
+        self.pad_width = pad_width
+
+
+class SpecDiscriminator(nn.Module):
+    """One resolution of the multi-resolution spectrogram discriminator (hifigan.py:481-582).  ``forward(wav)`` takes the
+    magnitude spectrogram without gradient (the generator learns nothing from this discriminator; only its own weights do)
+    and runs the (k, 1) convs over frames with F = fft_size//2+1 input channels.
+
+    Every conv also pads the width-1 frequency axis, so the maps grow by 2p columns per layer.  All columns born as zeros
+    at one layer (a "column class") hold the same sequence for every item: the module computes each class once, as one
+    extra batch item after the signal items (a zero item appended to the layer's input becomes lrelu(bias) at its birth),
+    and kt_spec_columns_fwd expands the rows into the reference's maps, returned as (B, C, frames, width) views of
+    channels-last (B, frames, width, C) buffers."""
+
+    def __init__(self, channels=32, init_kernel=15, kernel_size=11, stride=2, use_spectral_norm=False, fft_size=1024,
+                 shift_size=120, win_length=600, window="hann_window", nonlinear_activation="LeakyReLU",
+                 nonlinear_activation_params={"negative_slope": 0.1}):
+        super().__init__()
+        if nonlinear_activation != "LeakyReLU":
+            raise NotImplementedError("kantts_b200: only LeakyReLU is fused into the conv kernels")
+        slope = nonlinear_activation_params.get("negative_slope", 0.01)
+        self.fft_size, self.shift_size, self.win_length = fft_size, shift_size, win_length
+        norm = "spectral" if use_spectral_norm else "weight"
+        act = lambda: getattr(nn, nonlinear_activation)(**nonlinear_activation_params)  # noqa: E731
+        layers = [(fft_size // 2 + 1, init_kernel, 1)] + [(channels, kernel_size, stride)] * 3 + [(channels, 5, 1)]
+        self.convs = nn.ModuleList(
+            nn.Sequential(_SpecConv(cin, channels, k, s, (k - 1) // 2, norm, slope), act()) for cin, k, s in layers)
+        self.conv_post = _SpecConv(channels, 1, 3, 1, 0, norm)
+        self.register_buffer("window", getattr(torch, window)(win_length))
+
+    def magnitude(self, wav):
+        """(B, 1, T) -> the magnitude rows (B, frames, F) of audio_torch.stft, without gradient (hifigan.py:566-571)."""
+        with torch.no_grad():
+            return stft(torch.squeeze(wav, 1), self.fft_size, self.shift_size, self.win_length, self.window)
+
+    def forward_rows(self, mag):
+        """mag (B, frames, F) -> (output (B, 1, frames', width), [six (B, C, frames_l, width_l) feature maps])"""
+        n = mag.shape[0]
+        x, reach, fmap = mag, [], []
+        for conv in [l[0] for l in self.convs] + [self.conv_post]:
+            if conv.pad_width:
+                # the columns this layer pads in: their input is zeros at every frame
+                x = torch.cat([x, x.new_zeros((1,) + tuple(x.shape[1:]))])
+                reach.append((reach[-1] if reach else 0) + conv.pad_width)
+            x = conv.run(x)
+            fmap.append(ops.SpecColumnsFn.apply(x, n, tuple(reach)).permute(0, 3, 1, 2))
+        return fmap[-1].squeeze(-1), fmap
+
+    def forward(self, wav):
+        return self.forward_rows(self.magnitude(wav))
+
+
+class MultiSpecDiscriminator(nn.Module):
+    """hifigan.py:585-617: one SpecDiscriminator per (fft size, hop, window length).  The default ``discriminator_params``
+    are the reference's, whose ``kernel_sizes`` key SpecDiscriminator does not take: like the reference,
+    ``MultiSpecDiscriminator()`` raises TypeError, and a usable config passes ``kernel_size``."""
+
+    def __init__(self, fft_sizes=[1024, 2048, 512], hop_sizes=[120, 240, 50], win_lengths=[600, 1200, 240],
+                 discriminator_params={
+                     "channels": 15, "init_kernel": 1, "kernel_sizes": 11, "stride": 2, "use_spectral_norm": False,
+                     "window": "hann_window", "nonlinear_activation": "LeakyReLU",
+                     "nonlinear_activation_params": {"negative_slope": 0.1}}):
+        super().__init__()
+        self.discriminators = nn.ModuleList()
+        for fft_size, hop_size, win_length in zip(fft_sizes, hop_sizes, win_lengths):
+            params = copy.deepcopy(discriminator_params)
+            params["fft_size"] = fft_size
+            params["shift_size"] = hop_size
+            params["win_length"] = win_length
+            self.discriminators += [SpecDiscriminator(**params)]
+
+    def forward(self, y):
+        """y: (B, 1, T) -> (list of (B, 1, frames, width), list of lists of (B, C, frames_l, width_l) feature maps)"""
+        return self._run(y, None)
+
+    def forward_pair(self, ya, yb, detach_b=False):
+        """== (self(ya), self(yb)) evaluated as one batch of 2B (see MultiPeriodDiscriminator.forward_pair): the column
+        classes follow the 2B signal items, so ops.grad_items(B) keeps them out of the gradient of a generator-phase pair
+        (nothing there needs it), and pair_state("reuse") reuses them with the real half.  A spectral-normed resolution
+        runs per half in the reference's order, as in MultiScaleDiscriminator.forward_pair."""
+        assert ya.shape == yb.shape
+        nb = ya.shape[0]
+        outs, fmaps = self._run(torch.cat([ya, yb], 0), nb)
+        return _split_runs(outs, fmaps, nb, detach_b)
+
+    def _run(self, y, pair_nb):
+        def run_resolution(d):
+            mag = d.magnitude(y)
+            if pair_nb is not None and _spectral(d):
+                return _run_halves(d.forward_rows, mag, pair_nb)
+            return d.forward_rows(mag)
+
+        return _run_parallel(y, [(lambda d=d: run_resolution(d), not _spectral(d)) for d in self.discriminators])

@@ -23,7 +23,8 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
         import kantts.train.loss as kantts_loss
     if kantts_audio is None:
         import kantts.utils.audio_torch as kantts_audio
-    for name in ("Generator", "MultiPeriodDiscriminator", "MultiScaleDiscriminator"):
+    for name in ("Generator", "MultiPeriodDiscriminator", "MultiScaleDiscriminator", "SpecDiscriminator",
+                 "MultiSpecDiscriminator"):
         setattr(kantts_models, name, getattr(hifigan, name))
         if hasattr(kantts_models, "hifigan") and hasattr(kantts_models.hifigan, "hifigan"):
             setattr(kantts_models.hifigan.hifigan, name, getattr(hifigan, name))

@@ -777,6 +777,37 @@ class DwtFn(torch.autograd.Function):
         return dx
 
 
+def spec_columns_desc(batch, t, c, reach):
+    """-> the KtSpecColumnsDesc of ``batch`` items whose column classes reach ``reach`` (increasing) from the centre."""
+    assert len(reach) <= _lib.KT_SPEC_MAX_CLASSES, reach
+    return _lib.KtSpecColumnsDesc(batch, t, c, len(reach), (ctypes.c_int32 * _lib.KT_SPEC_MAX_CLASSES)(*reach))
+
+
+class SpecColumnsFn(torch.autograd.Function):
+    """rows (batch + classes, T, C) -> the spectrogram discriminator's feature map (batch, T, width, C), see
+    kt_spec_columns_fwd."""
+
+    @staticmethod
+    def forward(ctx, rows, batch, reach):
+        rows = rows.contiguous()
+        _, t, c = rows.shape
+        assert rows.shape[0] == batch + len(reach), (rows.shape, batch, reach)
+        d = spec_columns_desc(batch, t, c, reach)
+        width = 2 * reach[-1] + 1 if reach else 1
+        out = torch.empty(batch, t, width, c, device=rows.device, dtype=torch.float32)
+        call("kt_spec_columns_fwd", ctypes.byref(d), ptr(rows), ptr(out))
+        ctx.d = d
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        d = ctx.d
+        dout = dout.contiguous()
+        drows = torch.empty(d.batch + d.classes, d.t, d.c, device=dout.device, dtype=torch.float32)
+        call("kt_spec_columns_bwd", ctypes.byref(d), ptr(dout), ptr(drows))
+        return drows, None, None
+
+
 class StftMelFn(torch.autograd.Function):
     """Fused framing/window/rFFT/magnitude(/mel/log-normalise).  Returns mel (B, n_mels, frames)
     when ``melmat`` is given, else the magnitude (B, frames, n_bins)."""
