@@ -609,6 +609,10 @@ int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t* out9);
  * 0 for the register epilogue (stream chunks, produced channels or channels per N tile % 4 != 0) or a layer off the
  * tensor cores. */
 int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir);
+/* Test aid (no GPU needed): how those launches pack the items of a batch into M tiles when an item has few output rows.
+ * out5 = {items per M tile (1: not packed), image rows of one item's block, MMA rows issued per N tile over all launches,
+ * the same with one item per tile, output rows produced per N tile}. */
+int kt_debug_conv_tc_pack(const KtConv1dDesc* d, int32_t dir, int64_t* out5);
 
 /* library info */
 const char* kt_last_error(void);

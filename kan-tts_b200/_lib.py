@@ -158,6 +158,7 @@ PROTOTYPES = {
     "kt_debug_wgrad_plan": [ctypes.POINTER(KtConv1dDesc), _P],
     "kt_debug_conv_tc_plan": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_debug_conv_tc_epilogue": [ctypes.POINTER(KtConv1dDesc), _I],
+    "kt_debug_conv_tc_pack": [ctypes.POINTER(KtConv1dDesc), _I, _P],
     "kt_version": [],
     "kt_has_tc": [],
 }

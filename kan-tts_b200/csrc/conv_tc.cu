@@ -133,6 +133,13 @@ struct TcParams {
   // output rows per m-tile: kTcM on the register-staged route; tt whole time steps x nsub on the TMA route
   int R, tt;
   int a_box_t;                        // TMA route: time steps per image box = tt + span_q
+  // Packed tiles (register-staged route, layers whose items have few output rows): one m-tile holds `pack` consecutive items
+  // of the batch, item b of the tile in image rows [b * pack_rows, (b + 1) * pack_rows) -- its M * nsub output rows and the
+  // span_q * nsub halo rows their taps read, so every tap stays inside the item's block -- and output row r belongs to item
+  // r / pack_rows, flattened output r % pack_rows (dropped past the phase's M * nsub).  pack_magic: the RowMap divisor of
+  // pack_rows.  pack = 1, pack_magic = 0: one item per tile.  The m-tile index space is per group of `pack` items.
+  int pack, pack_rows;
+  uint32_t pack_magic;
   // stream instances (kt_conv1d_fwd_tc_stream, nsub == 1): windows of the input / output / residual, see KtStreamWin
   int in_pitch, in_first, out_pitch, out_first, res_pitch, res_first;
   // 1: the epilogue goes through each consumer warp's shared-memory staging block (kTcEpiWarpBytes) with float4 global
@@ -206,7 +213,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mtiles = p.ph_mt0[p.nphases];   // m-tiles of all phases (each: R flattened outputs m * nsub + w)
-  const int total_tiles = mtiles * p.ntiles * p.batch;
+  const int total_tiles = mtiles * p.ntiles * ((p.batch + p.pack - 1) / p.pack);   // bb below: a group of p.pack items
 
   if (tid == 0) {
     for (int s = 0; s < p.na_stages; ++s) { mbar_init(&full_a[s], TMA ? 1 : 128); mbar_init(&empty_a[s], kTcConsumerArrivals); }
@@ -245,12 +252,14 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
             rm.base_row = (long long)bb * p.in_pitch + p.in_first;
             rm.t_lo = -p.in_first * p.up;
           } else {
-            rm.base_row = (long long)bb * p.t_in * p.nsub;
+            rm.base_row = (long long)bb * p.pack * p.t_in * p.nsub;
+            rm.pack_magic = p.pack_magic; rm.pack_rows = p.pack_rows; rm.pack_items = min(p.pack, p.batch - bb * p.pack);
+            rm.item_rows = (long long)p.t_in * p.nsub;
           }
           rm.fv0 = f0 + p.grp_qlo[g] * p.nsub;
           rm.nsub = p.nsub; rm.step = p.i_step; rm.rho = p.grp_rho[g]; rm.up = p.up; rm.t_lim = p.t_in * p.up;
           if constexpr (MASK) { rm.t_lo = t_lo; rm.t_lim = t_lim; }
-          stage_rows<5, SIMPLE, 3, STREAM>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
+          stage_rows<5, SIMPLE, 3, STREAM, !STREAM>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
                                    min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
           fence_proxy_async();
           mbar_arrive(&full_a[s]);
@@ -389,14 +398,19 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
         // output element + rdelta (0 outside streams: the residual has the output's layout); the act' mask and `out` itself
         // (accumulate) share the output's layout.
         const long long rdelta = STREAM ? ((long long)bb * (p.res_pitch - p.out_pitch) + p.res_first - p.out_first) * p.c_out : 0;
+        // packed tiles: row r is row r - b * pack_rows of item b's block (RowMap); the TMA and stream instances never pack
+        constexpr bool PACKED = !TMA && !STREAM;
         auto row_base = [&](int r, long long& obase) {
+          const int b = PACKED ? (int)(((uint32_t)r * p.pack_magic) >> 16) : 0;
+          const int item = PACKED ? bb * p.pack + b : bb;
+          r -= b * p.pack_rows;
           const int f = mt * R + r;
-          if ((TMA && r >= R) || f >= F) return false;
+          if ((TMA && r >= R) || f >= F || (PACKED && (b >= p.pack || item >= p.batch))) return false;
           const int m = p.nsub == 1 ? f : f / p.nsub;
           const int w = f - m * p.nsub;
           const int to = p.ph_ooff[ph] + p.o_step * m;
           obase = STREAM ? ((long long)bb * p.out_pitch + p.out_first + to) * p.c_out + c_tile
-                         : ((long long)(bb * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
+                         : ((long long)(item * p.t_out + to) * p.nsub + w) * p.c_out + c_tile;
           return true;
         };
         // Both forms do the same fp32 operations per element in the same order, so they write the same bits.
@@ -501,6 +515,7 @@ struct TcLayerPlan {
   int NT;        // padded N tile (multiple of 16, <= 128: the accumulators live in registers)
   int ntiles, kchunks, grouped;
   int kin_g, pout_g;   // grouped: channels of ONE group on the contraction / produced side (kg = gt * kin_g)
+  int pack, pack_rows; // items per packed m-tile and rows of one item's block (pack_shape); pack = 1: not packed
 };
 
 struct TcParams;
@@ -508,8 +523,33 @@ struct TcParams;
 // shared memory outside the activation / weight stages: barriers and the tap-shift table (see the carve-up in conv_tc_kernel)
 static int tc_fixed_smem(int slots) { return (2 * 3 + 2 * std::max(6, slots)) * 8 + kMaxTaps * 4; }
 
+// Packing of a layer whose items have few output rows (TcParams::pack): with M output time steps per item (the largest phase)
+// and taps spanning span_q steps of one residue class (the widest), an item's block is pack_rows = (M + span_q) * nsub image
+// rows, and the last item's M * nsub output rows must lie in the 128-row tile: pack = (128 - M * nsub) / pack_rows + 1 items,
+// at most the batch.  The last block's taps then read at most 128 + span_q * nsub rows, which every launch of the layer
+// stages.  Items of more than 64 output rows never pack (pack = 1).
+static void pack_shape(const KtConv1dDesc* d, const std::vector<Phase>& phases, int& pack, int& pack_rows) {
+  int M = 0, span_q = 0;
+  for (const Phase& ph : phases) {
+    if (ph.M <= 0) continue;
+    M = std::max(M, ph.M);
+    const ResidueTaps rt = residue_taps(ph, ph.i_step);
+    for (int r = 0; r < ph.i_step; ++r) {
+      int qlo = 1 << 30, qhi = -(1 << 30);
+      for (int n = rt.first[r]; n < rt.first[r + 1]; ++n) { qlo = std::min(qlo, rt.q[n]); qhi = std::max(qhi, rt.q[n]); }
+      if (rt.first[r + 1] > rt.first[r]) span_q = std::max(span_q, qhi - qlo);
+    }
+  }
+  pack = 1; pack_rows = 0;
+  if (M == 0 || 2 * M * d->nsub > kTcM) return;
+  pack_rows = (M + span_q) * d->nsub;
+  pack = std::min(d->batch, (kTcM - M * d->nsub) / pack_rows + 1);
+  if (pack < 2) { pack = 1; pack_rows = 0; }
+}
+
 static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
   TcLayerPlan L{};
+  pack_shape(d, conv_phases(d, dir), L.pack, L.pack_rows);
   const int g = d->groups;
   const int kin = (dir == 0 ? d->c_in : d->c_out) / g;     // contraction channels per group
   const int pout = (dir == 0 ? d->c_out : d->c_in) / g;    // produced channels per group
@@ -517,11 +557,21 @@ static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
   L.n_total = pout * g;
   L.kchunks = ceil_div(kin, kTcKC);
   L.grouped = g > 1;
+  // M tiles per N tile of the launch (packed: one per group of L.pack items)
+  const long long mtiles = L.pack > 1 ? ceil_div(d->batch, L.pack)
+                                      : (long long)ceil_div((dir == 0 ? d->t_out : d->t_in) * d->nsub, kTcM) * d->batch;
   if (g > 1) {
     if (pout > kWgmmaMaxN) return L;
     // groups per tile: fill one 64-channel K chunk, keep the N tile <= 128 (block-diagonal tile, see tc_pack_weights_kernel)
     int gt = 1;
     while (gt * 2 <= g && g % (gt * 2) == 0 && kin * gt * 2 <= kTcKC && pout * gt * 2 <= 128) gt *= 2;
+    // Under-filled grids (short sequences): fewer groups per tile.  A tile's MMAs grow with gt^2 (K and N both gt-fold) of
+    // which only 1 / gt is off the zero blocks, so halving gt quarters each tile's MMA time and doubles the tiles.  Each
+    // output still gets its own group's K = 16 slices in the same order (the dropped slices only added zero products): the
+    // same bits.  The halving keeps the N tile >= 16 (so the N tile still identifies the image layout, PreparedWeight's
+    // key) and the alignment of kg and n_stride the kernel instances depend on.
+    while (gt > 1 && mtiles * (g / gt) < 120 && (gt / 2) * pout >= 16 && (gt / 2) * kin % 8 == 0 && (gt / 2) * pout % 4 == 0)
+      gt /= 2;
     L.kin_g = kin; L.pout_g = pout;
     L.kg = gt * kin;
     L.kchunks = ceil_div(L.kg, kTcKC);
@@ -531,7 +581,6 @@ static TcLayerPlan layer_plan(const KtConv1dDesc* d, int dir) {
     L.ntiles = ceil_div(pout, kWgmmaMaxN);
     L.n_stride = (ceil_div(pout, L.ntiles) + 15) & ~15; L.NT = L.n_stride;
     // under-filled grids (short sequences x wide layers): split N so that >= ~1 tile per SM exists
-    const long long mtiles = (long long)ceil_div((dir == 0 ? d->t_out : d->t_in) * d->nsub, kTcM) * d->batch;
     while (mtiles * L.ntiles < 120 && L.NT >= 128 && L.NT % 32 == 0 && pout % (L.NT / 2) == 0) {
       L.NT /= 2; L.n_stride = L.NT; L.ntiles = pout / L.NT;
     }
@@ -628,7 +677,8 @@ static bool tma_pays(const TcParams& lp) {
   return !lp.grouped && elems >= (1LL << 19) && (lp.ntiles >= 2 || elems < (1LL << 22));
 }
 
-static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true, bool plan_only = false) {
+// allow_pack: false for stream chunks, whose rows live in per-slot windows (one item per tile)
+static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true, bool plan_only = false, bool allow_pack = true) {
   TcPlan P{};
   if (dir == 0 && d->path != KT_PATH_TC && thin_cin1_ok(d)) return P;   // waveform-input layers: HBM-bound FIR kernel
   if (dir == 1 && d->upsample > 1) return P;   // no direct plan: ops.ConvPlan runs it as the plain conv over the
@@ -638,7 +688,7 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   if (!L.ok) return P;
   TcParams base{};
   base.NT = L.NT; base.ntiles = L.ntiles; base.kchunks = L.kchunks; base.kg = L.kg; base.grouped = L.grouped; base.n_stride = L.n_stride;
-  base.batch = d->batch; base.nsub = d->nsub;
+  base.batch = d->batch; base.nsub = d->nsub; base.pack = 1;
   // roles swap for the data gradient: the gathered tensor is dy, the product is dx
   base.t_in = dir == 0 ? d->t_in : d->t_out; base.t_out = dir == 0 ? d->t_out : d->t_in;
   base.c_in = dir == 0 ? d->c_in : d->c_out; base.c_out = dir == 0 ? d->c_out : d->c_in;
@@ -658,6 +708,11 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   if (!tma) {
     P.launches.clear();
     base.tt = 0; base.R = kTcM;
+    if (allow_pack && L.pack > 1) {
+      // packed tiles (register-staged route only: a TMA box holds one item); every phase is one m-tile per item group
+      base.pack = L.pack; base.pack_rows = L.pack_rows;
+      base.pack_magic = (1u << 16) / (unsigned)L.pack_rows + 1;
+    }
     if (!plan_launches(phases, d->nsub, P.launches, base)) return P;
   }
   // staged epilogue: float4 rows need output channel counts and tile offsets % 4 (run_plan also checks the pointers);
@@ -674,7 +729,7 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
 static TcPlan make_tc_plan_flags(const KtConv1dDesc* d, int dir, bool plan_only = false) {
   if (dir == KT_PLAN_STREAM) {
     if (d->nsub != 1) return TcPlan{};
-    TcPlan P = make_tc_plan(d, 0, false, plan_only);
+    TcPlan P = make_tc_plan(d, 0, false, plan_only, false);
     for (TcParams& lp : P.launches) lp.epi_staged = 0;
     return P;
   }
@@ -762,6 +817,25 @@ extern "C" int kt_debug_conv_tc_plan(const KtConv1dDesc* d, int32_t dir, int64_t
   return KT_OK;
 }
 
+// development / test aid (kt_debug_conv_tc_pack): the tile packing of direction dir (0, 1 or KT_PLAN_STREAM) as it would be
+// planned on a GPU box.  out = {items per m-tile, rows of one item's block, MMA rows issued per N tile over all launches,
+// the same without packing, output rows produced per N tile}; {1, 0, 0, 0, 0} for a layer off the tensor cores
+extern "C" int kt_debug_conv_tc_pack(const KtConv1dDesc* d, int32_t dir, int64_t* out) {
+  KT_REQUIRE(d && out, "kt_debug_conv_tc_pack: null pointer");
+  const TcPlan P = make_tc_plan_flags(d, dir, true);
+  out[0] = 1;
+  for (int i = 1; i < 5; ++i) out[i] = 0;
+  if (!P.ok) return KT_OK;
+  out[0] = P.launches[0].pack; out[1] = P.launches[0].pack_rows;
+  for (const TcParams& lp : P.launches) {
+    const int mt = lp.ph_mt0[lp.nphases];
+    out[2] += (int64_t)kTcM * mt * ceil_div(lp.batch, lp.pack);
+    out[3] += (int64_t)kTcM * mt * lp.batch;
+    for (int i = 0; i < lp.nphases; ++i) out[4] += (int64_t)lp.ph_M[i] * lp.nsub * lp.batch;
+  }
+  return KT_OK;
+}
+
 // development / test aid: 1 when the launches of direction dir (0, 1 or KT_PLAN_STREAM) take the staged epilogue given
 // 16-byte aligned operands, 0 for the register epilogue or a layer off the tensor cores
 extern "C" int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir) {
@@ -774,7 +848,7 @@ static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, bool
                   cudaStream_t st) {   // p: phases already planned
   const size_t smem = size_stages(p);
   KT_REQUIRE(smem > 0, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
-  const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * p.batch;
+  const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * ceil_div(p.batch, p.pack);
   const int grid = (int)std::min<long long>(tiles, device_sm_count());
   if (tma) {
     KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcTma>>(kMaxDynSmem));

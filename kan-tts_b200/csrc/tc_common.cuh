@@ -213,26 +213,48 @@ static inline cudaError_t split_planes(const Side& a, long long na, __nv_bfloat1
 // period, so every M = 128 tile is a dense run of flattened outputs.
 // STREAM (a chunk of a stream, nsub == 1): base_row is the row of time step 0 in the item's window, and the rows before it
 // are real data down to tv >= t_lo (= -history * up); negative up-sampled times take the floor.
+// PACK (packed tiles of the conv kernel, see TcParams::pack): the image holds consecutive blocks of pack_rows rows, block b
+// belonging to item b of the tile (item_rows source rows further on); row r is row r - b * pack_rows of its block, and
+// blocks past the tile's pack_items items are zero.  pack_magic = floor(2^16 / pack_rows) + 1, so that b = (r * pack_magic)
+// >> 16 = r / pack_rows exactly for r * pack_rows < 2^16 (rows < 256, pack_rows <= 128); 0 when the tile holds one item.
 struct RowMap {
   long long base_row;
   int fv0, nsub, step, rho, up, t_lim;
   int t_lo;   // STREAM only
-  // nsub == 1 && up == 1 (every layer but the period discriminator's and the nearest-upsampled convs): no divisions
-  template <bool STREAM = false>
-  __device__ __forceinline__ bool map_simple(int r, long long& row) const {
-    const int tv = (fv0 + r) * step + rho;
-    if (tv < (STREAM ? t_lo : 0) || tv >= t_lim) return false;
-    row = base_row + tv;
+  uint32_t pack_magic;
+  int pack_rows, pack_items;
+  long long item_rows;
+  // PACK: image row r -> (row of its item's block, source-row offset of the item); false past the tile's items
+  template <bool PACK>
+  __device__ __forceinline__ bool block_row(int& r, long long& item) const {
+    if constexpr (PACK) {
+      const int b = (int)(((uint32_t)r * pack_magic) >> 16);
+      if (b >= pack_items) return false;
+      r -= b * pack_rows;
+      item = b * item_rows;
+    }
     return true;
   }
-  template <bool STREAM = false>
+  // nsub == 1 && up == 1 (every layer but the period discriminator's and the nearest-upsampled convs): no divisions
+  template <bool STREAM = false, bool PACK = false>
+  __device__ __forceinline__ bool map_simple(int r, long long& row) const {
+    long long item = 0;
+    if (!block_row<PACK>(r, item)) return false;
+    const int tv = (fv0 + r) * step + rho;
+    if (tv < (STREAM ? t_lo : 0) || tv >= t_lim) return false;
+    row = base_row + item + tv;
+    return true;
+  }
+  template <bool STREAM = false, bool PACK = false>
   __device__ __forceinline__ bool map(int r, long long& row) const {
+    long long item = 0;
+    if (!block_row<PACK>(r, item)) return false;
     const int fv = fv0 + r;
     const int mp = nsub == 1 ? fv : fdiv(fv, nsub);
     const int w = fv - mp * nsub;
     const int tv = mp * step + rho;
     if (tv < (STREAM ? t_lo : 0) || tv >= t_lim) return false;
-    row = base_row + (long long)(up == 1 ? tv : (STREAM ? fdiv(tv, up) : tv / up)) * nsub + w;
+    row = base_row + item + (long long)(up == 1 ? tv : (STREAM ? fdiv(tv, up) : tv / up)) * nsub + w;
     return true;
   }
 };
@@ -242,7 +264,7 @@ struct RowMap {
 // converts and stores.  The two phases are separate fully-unrolled loops without early exits: with one
 // CTA per SM the staging loop is pure DRAM/L2 latency, and a fused load->convert->store loop measured
 // ~1 load in flight per thread.
-template <int NB, bool VEC, bool AUX, bool SIMPLE = false, bool STREAM = false>
+template <int NB, bool VEC, bool AUX, bool SIMPLE = false, bool STREAM = false, bool PACK = false>
 __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                                 const float* aux_base, int c_total, int ch0, int nv, const RowMap& rm,
                                                 int rows, int tid, int r_begin = 0) {
@@ -255,7 +277,7 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
     for (int i = 0; i < NB; ++i) {
       const int r = r0 + 16 * i;
       long long srow = 0;
-      ok[i] = r < rows && nv > 0 && (SIMPLE ? rm.template map_simple<STREAM>(r, srow) : rm.template map<STREAM>(r, srow));
+      ok[i] = r < rows && nv > 0 && (SIMPLE ? rm.template map_simple<STREAM, PACK>(r, srow) : rm.template map<STREAM, PACK>(r, srow));
       off[i] = ok[i] ? srow * c_total + ch0 + q * 8 : 0;   // offset 0 is always a readable address
     }
 #pragma unroll
@@ -310,7 +332,7 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
 // SIMPLE: the host guarantees nsub == 1, up == 1 and 16-byte-aligned 8-channel chunks (c_valid % 8 == 0, c_total % 4
 // == 0): only the vectorised instantiations exist in that kernel variant, which roughly halves its code size -- the
 // generic kernel (~140 KB of SASS shared by four concurrently running warp roles) does not fit the instruction cache.
-template <int NB, bool SIMPLE = false, int NB_AUX = NB, bool STREAM = false>
+template <int NB, bool SIMPLE = false, int NB_AUX = NB, bool STREAM = false, bool PACK = false>
 __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                            const float* aux_base, int c_total, int ch0, int c_valid, bool fill_all,
                                            const RowMap& rm, int rows, int tid, int r_begin = 0) {
@@ -337,16 +359,16 @@ __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, con
   const bool vec = nv == 8 && (c_total & 3) == 0 && ((ch0 + q * 8) & 3) == 0;
   const bool has_aux = s.mode >= SIDE_DLRELU;
   if constexpr (SIMPLE) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true, true, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false, true, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, true, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, true, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
     return;
   }
   if (vec) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   } else {
-    if (has_aux) stage_rows_impl<2, false, true, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<2, false, false, false, STREAM>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<2, false, true, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<2, false, false, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   }
 }
 

@@ -17,6 +17,19 @@ LAYERS = {
     "mpd_512_1024_k5s3_p3": (dict(c_in=512, c_out=1024, kernel=5, stride=3, pad_left=2, pad_right=2), 16, 102, 3),
     "mpd_128_512_k5s3_p5": (dict(c_in=128, c_out=512, kernel=5, stride=3, pad_left=2, pad_right=2), 16, 547, 5),
     "msd_1024_1024_k5": (dict(c_in=1024, c_out=1024, kernel=5, pad_left=2, pad_right=2), 16, 33, 0),
+    # scale discriminator at its shorter scales and pair batch (32 items): packed M tiles, several items per tile
+    "msd_1024_1024_k5_t17": (dict(c_in=1024, c_out=1024, kernel=5, pad_left=2, pad_right=2), 32, 17, 0),
+    "msd_1024_1024_k5_t9": (dict(c_in=1024, c_out=1024, kernel=5, pad_left=2, pad_right=2), 32, 9, 0),
+    "msd_1024_1024_k41_g16_t33": (dict(c_in=1024, c_out=1024, kernel=41, groups=16, pad_left=20, pad_right=20), 32, 33, 0),
+    "msd_1024_1024_k41_g16_t17": (dict(c_in=1024, c_out=1024, kernel=41, groups=16, pad_left=20, pad_right=20), 32, 17, 0),
+    "msd_1024_1024_k41_g16_t9": (dict(c_in=1024, c_out=1024, kernel=41, groups=16, pad_left=20, pad_right=20), 32, 9, 0),
+    "msd_512_1024_k41_g16_s4_t9": (dict(c_in=512, c_out=1024, kernel=41, stride=4, groups=16, pad_left=20, pad_right=20),
+                                   32, 33, 0),
+    "msd_512_1024_k41_g16_s4_t32": (dict(c_in=512, c_out=1024, kernel=41, stride=4, groups=16, pad_left=20, pad_right=20),
+                                    16, 128, 0),
+    "msd_256_512_k41_g16_s4_t128": (dict(c_in=256, c_out=512, kernel=41, stride=4, groups=16, pad_left=20, pad_right=20),
+                                    16, 512, 0),
+    "gen_conv_pre_80_512_k7": (dict(c_in=80, c_out=512, kernel=7, pad_left=3, pad_right=3), 16, 32, 0),
     "gen_128_128_k11": (dict(c_in=128, c_out=128, kernel=11, pad_left=10, pad_right=0), 16, 2048, 0),
     "gen_32_32_k7": (dict(c_in=32, c_out=32, kernel=7, pad_left=6, pad_right=0), 16, 8192, 0),
     # one shape per MMA tile width N: 16 (single-channel output; the data gradient of a 1-channel input layer),
