@@ -45,6 +45,11 @@ extern "C" {
 #define KT_PATH_AUTO 0  /* tensor-core where the shape qualifies, FFMA otherwise */
 #define KT_PATH_FFMA 1  /* exact-fp32 CUDA-core kernels */
 #define KT_PATH_TC 2    /* tensor-core split-bf16 (bf16x3) tensor-core kernels; error if unsupported */
+/* opt-in single-pass bf16: each operand rounded once to bf16 (round to nearest), ONE wgmma per K = 16 slice, fp32
+ * accumulation; a shape without a tensor-core route runs the FFMA kernels, as KT_PATH_AUTO.  Every tensor-core query and
+ * entry point (plans, workspaces, image sizes and packing, forward, data / weight gradient, stream, fused resblock) answers
+ * for, and runs, the precision of the descriptor it is given: an image packed for one precision is not valid for the other. */
+#define KT_PATH_BF16 3
 
 /* One 1-D convolution layer (forward semantics; the backward entry points take the
  * SAME descriptor).  Replaces F.conv1d / F.conv_transpose1d / F.conv2d((k,1)) as

@@ -24,7 +24,7 @@ from . import ops, hifigan, pqmf, audio, loss, sambert_ops, sambert, train, infe
 from .sambert import (KanTtsSAMBERT, MelReconLoss, ProsodyReconLoss, FpCELoss, AttentionCTCLoss,  # noqa: F401
                       AttentionBinarizationLoss, ConvAttention, KanTtsTextsyBERT, SeqCELoss)
 from .hifigan import (Generator, MultiPeriodDiscriminator, MultiScaleDiscriminator, SpecDiscriminator,  # noqa: F401
-                      MultiSpecDiscriminator)
+                      MultiSpecDiscriminator, set_precision)
 from .pqmf import PQMF  # noqa: F401
 from .audio import MelSpectrogram, stft  # noqa: F401
 from .loss import (MelSpectrogramLoss, MultiResolutionSTFTLoss, GeneratorAdversarialLoss,  # noqa: F401

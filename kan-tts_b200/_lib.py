@@ -18,7 +18,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_ffma.cu", "conv_tc.cu", "resblock_tc.cu", "wgrad_tc.cu", "weights.cu", "misc.cu", "stft_mel.cu", "sambert.cu", "thin.cu", "nsf.cu", "align.cu", "speaker.cu", "bert.cu", "spec_disc.cu"]
 
 KT_ACT_NONE, KT_ACT_LRELU, KT_ACT_TANH = 0, 1, 2
-KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC = 0, 1, 2
+KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC, KT_PATH_BF16 = 0, 1, 2, 3
 KT_PLAN_STREAM = 16
 
 

@@ -4,6 +4,9 @@
 // and the product is accumulated in fp32 registers as hi*hi + hi*lo + lo*hi (the dropped lo*lo term is
 // ~2^-18 relative).  A single-pass TF32/BF16 MMA does not meet the path's tolerance (mel-L1 <= 1e-4,
 // SURVEY.md "hard parts"); three bf16 MMAs do, at twice the rate of 3xTF32.
+// Single-pass bf16 (KT_PATH_BF16, opt-in): every operand is rounded once to bf16 (the hi plane alone) and each K = 16
+// slice is ONE wgmma hi * hi into the same fp32 accumulators.  Those instances (template argument PL = 1, "planes") stage,
+// pack and move one plane per operand; PL = 2 is the bf16x3 route.
 //
 // Tile = 128 consecutive FLATTENED outputs (time m, sub-sequence w) of one batch item x NT (<= 128) channels.
 // Data flow per CTA:
@@ -46,7 +49,7 @@ constexpr int kTcMaxGroups = 8;  // residue classes (= input step) per phase
 
 // ---------------------------------------------------------------------------------------------
 // weight packing: fp32 W[taps][K][N] (kernel layout of conv_ffma.cu) -> bf16 hi/lo SWIZZLE_128B tiles
-//   block (j, kc, nt) = [hi tile | lo tile], tile = NT rows (n) x 64 (k) bf16, row = 128 bytes
+//   block (j, kc, nt) = [hi tile | lo tile], tile = NT rows (n) x 64 (k) bf16, row = 128 bytes (PL = 1: the hi tile only)
 // ---------------------------------------------------------------------------------------------
 // K (contraction rows of W) is zero-padded to a multiple of 64 and every N tile to NT rows, so thin
 // (C_in = 1, 32, 80, ...), single-output and GROUPED layers use the same kernel: tile nt covers the
@@ -61,12 +64,13 @@ constexpr int kTcMaxGroups = 8;  // residue classes (= input step) per phase
 // One thread = one 16-byte chunk (8 consecutive k) of one tile row r: the 8 source loads are coalesced across the warp (lanes =
 // consecutive produced channels n), the hi / lo chunks are written with two 16-byte stores (round 1 wrote single bf16
 // elements: 2-byte scattered stores and five 64-bit divisions per element made this the 4th largest kernel of the step).
+template <int PL>
 __global__ void tc_pack_weights_kernel(const float* __restrict__ w, int taps, int K, int N, int NT, int n_stride,
                                        int ntiles, int kin_g, int pout_g, __nv_bfloat16* __restrict__ out) {
   const int kchunks = (K + kTcKC - 1) / kTcKC;
   const int block = blockIdx.x;                                   // (j, kc, nt)
   const int nt = block % ntiles, kc = (block / ntiles) % kchunks, j = block / (ntiles * kchunks);
-  uint8_t* tile = reinterpret_cast<uint8_t*>(out) + (size_t)block * (2u * NT * kTcKC * 2u);
+  uint8_t* tile = reinterpret_cast<uint8_t*>(out) + (size_t)block * ((uint32_t)PL * NT * kTcKC * 2u);
   for (int idx = blockIdx.y * blockDim.x + threadIdx.x; idx < NT * 8; idx += gridDim.y * blockDim.x) {
     const int q = idx / NT, r = idx - q * NT;
     const int n = nt * n_stride + r;
@@ -85,11 +89,7 @@ __global__ void tc_pack_weights_kernel(const float* __restrict__ w, int taps, in
       }
       x[e] = ok ? __ldg(w + src) : 0.f;
     }
-    uint4 hi, lo;
-    split8(x, hi, lo);
-    const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)q);
-    *reinterpret_cast<uint4*>(tile + o) = hi;
-    *reinterpret_cast<uint4*>(tile + (size_t)NT * kTcKC * 2 + o) = lo;
+    store_planes8<PL>(x, tile, tile + (size_t)NT * kTcKC * 2, sw128_offset((uint32_t)r, (uint32_t)q));
   }
 }
 
@@ -107,6 +107,7 @@ struct TcParams {
   int out_act;
   float out_slope;
   int NT, ntiles, kchunks, rows, na_stages, nb_stages;
+  int planes;    // bf16 planes per operand: 2 bf16x3, 1 single-pass bf16 (the kernel instance's PL)
   // 1: every (K chunk, tap) weight tile of the layer has its own shared-memory slot (slot = c * ntaps + n), loaded
   // ONCE per CTA and reused by all of its tiles -- thin layers otherwise re-stream all taps per 128-row tile through
   // a ring whose refill round trip (release -> empty -> bulk copy -> full) bounds the MMA issue rate
@@ -183,10 +184,10 @@ enum TcRoute { kTcRegSimple = 0, kTcReg = 1, kTcTma = 2 };
 // weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
 // STREAM (register-staged routes only): one chunk of a stream -- rows live in the windows of KtStreamWin, and the input
 // rows before the chunk (down to -in_first) are real data instead of zero padding.  MASK (with STREAM): of those, only the
-// rows inside item bb's utterance (KtStreamMask) are, bounded per tile by the row map's t_lo / t_lim.
-template <int ROUTE, bool STREAM = false, bool MASK = false>
-__global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
-    conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
+// rows inside item bb's utterance (KtStreamMask) are, bounded per tile by the row map's t_lo / t_lim.  PL: bf16 planes per
+// operand (2: bf16x3, three wgmma per K = 16 slice; 1: single-pass bf16, one): conv_tc_kernel / conv_tc_bf16_kernel.
+template <int ROUTE, bool STREAM, bool MASK, int PL>
+__device__ __forceinline__ void conv_tc_body(const TcParams& p, const TcTmaMaps& maps) {
   static_assert(!(STREAM && ROUTE == kTcTma), "stream chunks take the register-staged route");
   constexpr bool SIMPLE = ROUTE == kTcRegSimple;
   constexpr bool TMA = ROUTE == kTcTma;
@@ -197,8 +198,8 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);          // carve-up: all image / tile bases 1024-byte aligned
   const int img_bytes = p.rows * 128;                 // one plane of one activation stage
-  const int a_stage_bytes = 2 * img_bytes;            // hi + lo
-  const int b_stage_bytes = 2 * p.NT * 128;           // hi + lo weight tile
+  const int a_stage_bytes = PL * img_bytes;           // hi (+ lo)
+  const int b_stage_bytes = PL * p.NT * 128;          // hi (+ lo) weight tile
   uint8_t* a_base = smem;
   uint8_t* b_base = a_base + (size_t)p.na_stages * a_stage_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(b_base + (size_t)p.nb_stages * b_stage_bytes);
@@ -259,7 +260,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
           rm.fv0 = f0 + p.grp_qlo[g] * p.nsub;
           rm.nsub = p.nsub; rm.step = p.i_step; rm.rho = p.grp_rho[g]; rm.up = p.up; rm.t_lim = p.t_in * p.up;
           if constexpr (MASK) { rm.t_lo = t_lo; rm.t_lim = t_lim; }
-          stage_rows<5, SIMPLE, 3, STREAM, !STREAM>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
+          stage_rows<5, SIMPLE, 3, STREAM, !STREAM, PL>(img_hi, img_hi + img_bytes, p.in, p.in.p, p.in.aux, p.c_in, ch_base + c * kTcKC,
                                    min(kTcKC, p.kg - c * kTcKC), false, rm, p.rows, ptid);
           fence_proxy_async();
           mbar_arrive(&full_a[s]);
@@ -289,9 +290,9 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
             mbar_wait(&empty_a[s], ra.phase() ^ 1u);
             uint8_t* img_hi = a_base + (size_t)s * a_stage_bytes;
             const CUtensorMap* map = &maps.map[p.grp_rho[g]];
-            mbar_arrive_expect_tx(&full_a[s], 2u * box_bytes);
+            mbar_arrive_expect_tx(&full_a[s], (uint32_t)PL * box_bytes);
             tma_load_5d(img_hi, map, ch_base + c * kTcKC, 0, m0 + p.grp_qlo[g], bb, 0, &full_a[s]);
-            tma_load_5d(img_hi + img_bytes, map, ch_base + c * kTcKC, 0, m0 + p.grp_qlo[g], bb, 1, &full_a[s]);
+            if constexpr (PL == 2) tma_load_5d(img_hi + img_bytes, map, ch_base + c * kTcKC, 0, m0 + p.grp_qlo[g], bb, 1, &full_a[s]);
           }
         }
       }
@@ -378,7 +379,7 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
               const uint32_t b_hi = b_base16 + (uint32_t)sb * b_stage16;
               wgmma_fence();
               for (int ks = 0; ks < kslices; ++ks) {
-                wgmma_x3<NT, 0, 0>(acc, a_hi + 2u * ks, img16, b_hi + 2u * ks, bplane16, scale_d);
+                wgmma_slice<PL, NT, 0, 0>(acc, a_hi + 2u * ks, img16, b_hi + 2u * ks, bplane16, scale_d);
                 scale_d = 1;
               }
               wgmma_commit();
@@ -501,6 +502,17 @@ __global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 
       }
     });
   }
+}
+
+template <int ROUTE, bool STREAM = false, bool MASK = false>
+__global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
+    conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
+  conv_tc_body<ROUTE, STREAM, MASK, 2>(p, maps);
+}
+template <int ROUTE, bool STREAM = false, bool MASK = false>
+__global__ void __launch_bounds__(ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, 1)
+    conv_tc_bf16_kernel(const __grid_constant__ TcParams p, const __grid_constant__ TcTmaMaps maps) {
+  conv_tc_body<ROUTE, STREAM, MASK, 1>(p, maps);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -689,6 +701,7 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   TcParams base{};
   base.NT = L.NT; base.ntiles = L.ntiles; base.kchunks = L.kchunks; base.kg = L.kg; base.grouped = L.grouped; base.n_stride = L.n_stride;
   base.batch = d->batch; base.nsub = d->nsub; base.pack = 1;
+  base.planes = d->path == KT_PATH_BF16 ? 1 : 2;
   // roles swap for the data gradient: the gathered tensor is dy, the product is dx
   base.t_in = dir == 0 ? d->t_in : d->t_out; base.t_out = dir == 0 ? d->t_out : d->t_in;
   base.c_in = dir == 0 ? d->c_in : d->c_out; base.c_out = dir == 0 ? d->c_out : d->c_in;
@@ -720,7 +733,7 @@ static TcPlan make_tc_plan(const KtConv1dDesc* d, int dir, bool allow_tma = true
   for (TcParams& lp : P.launches) lp.epi_staged = lp.c_out % 4 == 0 && lp.n_stride % 4 == 0 && !lp.accumulate;
   P.ok = true;
   P.tma = tma;
-  P.ws_floats = tma ? plane_floats(base.batch, base.t_in, base.nsub, base.c_in) : 0;
+  P.ws_floats = tma ? plane_floats(base.batch, base.t_in, base.nsub, base.c_in, base.planes) : 0;
   return P;
 }
 
@@ -751,13 +764,14 @@ extern "C" int64_t kt_conv1d_tc_workspace(const KtConv1dDesc* d, int32_t dir) {
   return make_tc_plan_flags(d, dir).ws_floats;
 }
 
-// bytes of the packed split-bf16 weight image of direction `dir` (0 when unsupported)
+// bytes of the packed weight image of direction `dir` (0 when unsupported): two bf16 planes, one for KT_PATH_BF16
 extern "C" int64_t kt_conv1d_tc_image_bytes(const KtConv1dDesc* d, int32_t dir) {
   if (validate_conv(d)) return 0;
   if (dir != 0 && dir != 1) return 0;
   if (tc_plan(d, dir) == 0) return 0;
   const TcLayerPlan L = layer_plan(d, dir);
-  return (long long)d->kernel * L.kchunks * L.ntiles * 2LL * L.NT * kTcKC * 2LL;
+  const long long planes = d->path == KT_PATH_BF16 ? 1 : 2;
+  return (long long)d->kernel * L.kchunks * L.ntiles * planes * L.NT * kTcKC * 2LL;
 }
 
 // w = the fp32 kernel-layout weight of this direction (w_fwd for dir 0, w_bwd for dir 1): [taps][K][N]
@@ -765,8 +779,13 @@ int tc_pack_layer(const KtConv1dDesc* d, int dir, const float* w, void* out, cud
   KT_REQUIRE(w && out && tc_plan(d, dir) > 0, "tc_pack_layer: layer not supported by the tensor-core path");
   const TcLayerPlan L = layer_plan(d, dir);
   const dim3 grid((unsigned)(d->kernel * L.kchunks * L.ntiles), (unsigned)ceil_div(L.NT * 8, 256));
-  tc_pack_weights_kernel<<<grid, 256, 0, st>>>(w, d->kernel, L.kg, L.n_total, L.NT, L.n_stride, L.ntiles,
-                                               L.grouped ? L.kin_g : 0, L.pout_g, reinterpret_cast<__nv_bfloat16*>(out));
+  auto* img = reinterpret_cast<__nv_bfloat16*>(out);
+  if (d->path == KT_PATH_BF16)
+    tc_pack_weights_kernel<1><<<grid, 256, 0, st>>>(w, d->kernel, L.kg, L.n_total, L.NT, L.n_stride, L.ntiles, L.grouped ? L.kin_g : 0,
+                                                    L.pout_g, img);
+  else
+    tc_pack_weights_kernel<2><<<grid, 256, 0, st>>>(w, d->kernel, L.kg, L.n_total, L.NT, L.n_stride, L.ntiles, L.grouped ? L.kin_g : 0,
+                                                    L.pout_g, img);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
@@ -778,9 +797,11 @@ extern "C" int kt_weight_pack_tc(const KtConv1dDesc* d, int32_t dir, const float
 }
 
 // Ring sizes of one launch -> its shared-memory bytes (0: the stages do not fit)
+// (single-pass bf16 stages are half the bytes: the same rule gives those layers resident weights or deeper rings where they
+// fit, up to the same stage caps)
 static size_t size_stages(TcParams& p) {
-  const int a_stage = 2 * p.rows * 128;
-  const int b_stage = 2 * p.NT * 128;
+  const int a_stage = p.planes * p.rows * 128;
+  const int b_stage = p.planes * p.NT * 128;
   const int slots = p.ntaps * p.kchunks;                                      // weight tiles of the whole layer
   const int bar_bytes = tc_fixed_smem(slots) + (p.epi_staged ? 16 + kTcEpiBytes : 0);
   const int budget = kMaxDynSmem - 1024 /*align slack*/ - bar_bytes;
@@ -844,39 +865,39 @@ extern "C" int kt_debug_conv_tc_epilogue(const KtConv1dDesc* d, int32_t dir) {
   return P.ok && P.launches[0].epi_staged ? 1 : 0;
 }
 
+template <int ROUTE, bool STREAM, bool MASK, int PL>
+static int launch_tc(const TcParams& p, const TcTmaMaps& maps, int grid, size_t smem, cudaStream_t st) {
+  constexpr auto kernel = PL == 1 ? conv_tc_bf16_kernel<ROUTE, STREAM, MASK> : conv_tc_kernel<ROUTE, STREAM, MASK>;
+  KT_CHECK_CUDA(allow_dyn_smem<kernel>(kMaxDynSmem));
+  kernel<<<grid, ROUTE == kTcTma ? kTcTmaThreads : kTcThreads, smem, st>>>(p, maps);
+  return KT_OK;
+}
+
+// the instance of one launch, PL = p.planes
+template <int PL>
+static int launch_route(const TcParams& p, const TcTmaMaps& maps, bool tma, bool stream, bool masked, int grid, size_t smem,
+                        cudaStream_t st) {
+  if (tma) return launch_tc<kTcTma, false, false, PL>(p, maps, grid, smem, st);
+  const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
+                      (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
+                      (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
+  if (masked && simple) return launch_tc<kTcRegSimple, true, true, PL>(p, maps, grid, smem, st);
+  if (masked) return launch_tc<kTcReg, true, true, PL>(p, maps, grid, smem, st);
+  if (stream && simple) return launch_tc<kTcRegSimple, true, false, PL>(p, maps, grid, smem, st);
+  if (stream) return launch_tc<kTcReg, true, false, PL>(p, maps, grid, smem, st);
+  if (simple) return launch_tc<kTcRegSimple, false, false, PL>(p, maps, grid, smem, st);
+  return launch_tc<kTcReg, false, false, PL>(p, maps, grid, smem, st);
+}
+
 static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, bool masked,
                   cudaStream_t st) {   // p: phases already planned
   const size_t smem = size_stages(p);
   KT_REQUIRE(smem > 0, "conv_tc: shared memory budget exceeded (rows=%d NT=%d)", p.rows, p.NT);
   const long long tiles = (long long)p.ph_mt0[p.nphases] * p.ntiles * ceil_div(p.batch, p.pack);
   const int grid = (int)std::min<long long>(tiles, device_sm_count());
-  if (tma) {
-    KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcTma>>(kMaxDynSmem));
-    conv_tc_kernel<kTcTma><<<grid, kTcTmaThreads, smem, st>>>(p, maps);
-  } else {
-    const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
-                        (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
-                        (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
-    if (masked && simple) {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple, true, true>>(kMaxDynSmem));
-      conv_tc_kernel<kTcRegSimple, true, true><<<grid, kTcThreads, smem, st>>>(p, maps);
-    } else if (masked) {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg, true, true>>(kMaxDynSmem));
-      conv_tc_kernel<kTcReg, true, true><<<grid, kTcThreads, smem, st>>>(p, maps);
-    } else if (stream && simple) {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple, true>>(kMaxDynSmem));
-      conv_tc_kernel<kTcRegSimple, true><<<grid, kTcThreads, smem, st>>>(p, maps);
-    } else if (stream) {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg, true>>(kMaxDynSmem));
-      conv_tc_kernel<kTcReg, true><<<grid, kTcThreads, smem, st>>>(p, maps);
-    } else if (simple) {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcRegSimple>>(kMaxDynSmem));
-      conv_tc_kernel<kTcRegSimple><<<grid, kTcThreads, smem, st>>>(p, maps);
-    } else {
-      KT_CHECK_CUDA(allow_dyn_smem<conv_tc_kernel<kTcReg>>(kMaxDynSmem));
-      conv_tc_kernel<kTcReg><<<grid, kTcThreads, smem, st>>>(p, maps);
-    }
-  }
+  const int rc = p.planes == 1 ? launch_route<1>(p, maps, tma, stream, masked, grid, smem, st)
+                               : launch_route<2>(p, maps, tma, stream, masked, grid, smem, st);
+  if (rc) return rc;
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
@@ -893,7 +914,7 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
     }
     const TcParams& g = P.launches[0];
     KT_CHECK_CUDA(split_planes(io.in, (long long)g.batch * g.t_in * g.nsub * g.c_in, planes, Side{nullptr, nullptr, 0, 0.f}, 0,
-                               nullptr, st));
+                               nullptr, g.planes, st));
   }
   for (TcParams lp : P.launches) {
     lp.in = io.in; lp.wimg = io.wimg; lp.bias = io.bias; lp.resid = io.resid; lp.mask = io.mask; lp.out = io.out;
@@ -907,7 +928,8 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
     lp.epi_staged = lp.epi_staged && io.in_pitch == 0 && !(io.resid && io.mask.p) && a16(io.out) && a16(io.bias) &&
                     a16(io.resid) && a16(io.mask.p);
     for (int rho = 0; P.tma && rho < lp.i_step; ++rho) {
-      const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what);
+      const int rc = encode_plane_map(&maps.map[rho], planes, lp.batch, lp.t_in, lp.nsub, lp.c_in, lp.i_step, rho, kTcKC, lp.a_box_t, what,
+                                      lp.planes);
       if (rc) return rc;
     }
     const int rc = run_tc(lp, maps, P.tma, io.in_pitch > 0, io.smask.lengths != nullptr, st);

@@ -14,6 +14,9 @@
 // conv_tc.cu.  C = 32 packs TWO taps per 64-wide K chunk: image row r holds [act(x[r]) | act(x[r + d])], so a tap pair is
 // one dense K = 64 step and the resident weights halve (k = 11: 96 KB for both convs).
 //
+// Single-pass bf16 (KT_PATH_BF16): the PL = 1 instances keep one bf16 plane per image and weight tile and issue the hi * hi
+// wgmma alone; the layout, the tiling and the pipeline are the bf16x3 ones (PL = 2).
+//
 // Warp roles: see resblock_tc_kernel.
 
 #include <algorithm>
@@ -48,7 +51,8 @@ struct RbParams {
   int nsteps;                       // MMA steps per conv: k, or ceil(k / 2) when pair
   int last_kslices;                 // K = 16 slices of the last step (pair with odd k: 2, else 4)
   int resident, nb;                 // weights: all tiles resident | ring of nb stages
-  int tile_bytes;                   // one weight tile: [hi NT rows | lo NT rows] x 128 B
+  int tile_bytes;                   // one weight tile: [hi NT rows | lo NT rows] x 128 B (single-pass bf16: hi only)
+  int planes;                       // bf16 planes per image / tile: 2 bf16x3, 1 single-pass bf16 (the instance's PL)
   // TMA-staged input: the fp32 x tile [rows_box][C] of every tile -- halo included, rows outside [0, T) zero-filled by the
   // TMA unit itself -- is brought into shared memory with cp.async.bulk.tensor (one box of 32 channels x rows_box rows per
   // 32 channels, nx landing stages); the producer warps then only CONVERT shared -> shared (LeakyReLU, hi / lo split,
@@ -60,7 +64,8 @@ struct RbParams {
 
 // ---- weight packing for the paired (C = 32) layout: tile p = taps (2p, 2p + 1) along K -----------------------------
 // w: kernel layout [k][ci][co] (kt_weight_prepare's w_fwd).  Tile p: NT = 32 rows n = co, k index c: c < 32 -> tap 2p,
-// ci = c; c >= 32 -> tap 2p + 1, ci = c - 32 (zero when 2p + 1 == k).  [hi tile | lo tile], SWIZZLE_128B rows.
+// ci = c; c >= 32 -> tap 2p + 1, ci = c - 32 (zero when 2p + 1 == k).  [hi tile | lo tile] (PL = 1: hi), SWIZZLE_128B rows.
+template <int PL>
 __global__ void rb_pack_pair_kernel(const float* __restrict__ w, int k, int npairs, __nv_bfloat16* __restrict__ out) {
   const int total = npairs * 32 * 64;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
@@ -69,17 +74,17 @@ __global__ void rb_pack_pair_kernel(const float* __restrict__ w, int k, int npai
     const float v = tap < k ? w[((long long)tap * 32 + ci) * 32 + n] : 0.f;
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    const long long base = (long long)p * (2 * 32 * 64);
+    const long long base = (long long)p * (PL * 32 * 64);
     const uint32_t off = (sw128_offset((uint32_t)n, (uint32_t)(c >> 3)) >> 1) + (uint32_t)(c & 7);
     out[base + off] = hi;
-    out[base + 32 * 64 + off] = lo;
+    if constexpr (PL == 2) out[base + 32 * 64 + off] = lo;
   }
 }
 
 // ---- shared fp32 landing tile -> split-bf16 SWIZZLE_128B image (fused LeakyReLU), rows [r_begin, r_end), 128 threads.
 // ft: boxes of [rows_box][32 floats] (128-byte rows, linear).  PAIR (C = 32): image row r = [x[r] | x[r + d]];
 // else (C = 64): image row r = channels 0..63 of row r, box q / 4.  Rows outside [0, T) arrive as zeros.
-template <bool PAIR>
+template <bool PAIR, int PL>
 __device__ __forceinline__ void rb_convert_tile(uint8_t* img_hi, uint8_t* img_lo, const float* ft, int box_floats, int d, float slope,
                                                 int r_begin, int r_end, int tid) {
   const int q = tid & 7;
@@ -91,11 +96,7 @@ __device__ __forceinline__ void rb_convert_tile(uint8_t* img_hi, uint8_t* img_lo
     float e[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
     for (int z = 0; z < 8; ++z) e[z] = e[z] > 0.f ? e[z] : e[z] * slope;
-    uint4 hi, lo;
-    split8(e, hi, lo);
-    const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)q);
-    *reinterpret_cast<uint4*>(img_hi + o) = hi;
-    *reinterpret_cast<uint4*>(img_lo + o) = lo;
+    store_planes8<PL>(e, img_hi, img_lo, sw128_offset((uint32_t)r, (uint32_t)q));
   }
 }
 
@@ -109,16 +110,17 @@ constexpr int kRbConsumerBar = 1;        // named barrier of the 256 consumer th
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync %0, 256;" ::"n"(kRbConsumerBar) : "memory"); }
 
-// NT = C (32 or 64): the MMA width is a compile-time constant of each instance
-template <int NT>
-__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) {
+// NT = C (32 or 64): the MMA width is a compile-time constant of each instance; PL: bf16 planes (2 bf16x3: resblock_tc_kernel,
+// 1 single-pass: resblock_tc_bf16_kernel)
+template <int NT, int PL>
+__device__ __forceinline__ void resblock_tc_body(const RbParams& p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   const int ximg = p.rows_x * 128, himg = p.rows_h * 128;            // one plane
   const int nslots = p.resident ? 2 * p.nsteps : p.nb;
   uint8_t* x_base = smem;                                            // nx stages x (hi | lo)
-  uint8_t* h_base = x_base + (size_t)p.nx * 2 * ximg;                // (hi | lo)
-  uint8_t* w_base = h_base + 2 * (size_t)himg;
+  uint8_t* h_base = x_base + (size_t)p.nx * PL * ximg;               // (hi | lo)
+  uint8_t* w_base = h_base + PL * (size_t)himg;
   uint8_t* f_base = w_base + (size_t)nslots * p.tile_bytes;          // nx fp32 landing stages of the TMA-staged x tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(f_base + (size_t)p.nx * p.fstage_bytes);
   uint64_t* x_full = bars;                 // [2]
@@ -142,7 +144,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
   }
   // the H image starts as zeros: rows >= 128 (read only by discarded output rows) and, in the paired layout, the
   // second half of row 127 are never written
-  for (int i = tid; i < 2 * himg / 16; i += kRbThreads) reinterpret_cast<uint4*>(h_base)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < PL * himg / 16; i += kRbThreads) reinterpret_cast<uint4*>(h_base)[i] = make_uint4(0u, 0u, 0u, 0u);
   for (int i = tid; i < 2 * NT; i += kRbThreads) s_bias[i] = i < NT ? (p.b1 ? p.b1[i] : 0.f) : (p.b2 ? p.b2[i - NT] : 0.f);
   fence_proxy_async();
   __syncthreads();
@@ -169,10 +171,10 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
       const int s = rx.slot();
       mbar_wait(&x_empty[s], rx.phase() ^ 1u);
       mbar_wait(&f_full[s], rx.phase());
-      uint8_t* img_hi = x_base + (size_t)s * 2 * ximg;
+      uint8_t* img_hi = x_base + (size_t)s * PL * ximg;
       const float* ft = reinterpret_cast<const float*>(f_base + (size_t)s * p.fstage_bytes);
-      if (p.pair) rb_convert_tile<true>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
-      else rb_convert_tile<false>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+      if (p.pair) rb_convert_tile<true, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+      else rb_convert_tile<false, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
       fence_proxy_async();
       mbar_arrive(&x_full[s]);
       asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
@@ -242,7 +244,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
         const int ks = warp_uniform((s == p.nsteps - 1) ? p.last_kslices : 4);
         wgmma_fence();
         for (int k = 0; k < ks; ++k) {
-          wgmma_x3<NT, 0, 0>(acc, a_hi + 2u * k, plane16, b_hi + 2u * k, bplane16, scale_d);
+          wgmma_slice<PL, NT, 0, 0>(acc, a_hi + 2u * k, plane16, b_hi + 2u * k, bplane16, scale_d);
           scale_d = 1;
         }
         wgmma_commit();
@@ -261,7 +263,7 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
       const int s = rx.slot();
       // ---------- c1 ----------
       mbar_wait(&x_full[s], rx.phase());
-      run_conv(0, x16 + (uint32_t)s * 2u * ximg16 + half16, ximg16, step1, ti == 0);
+      run_conv(0, x16 + (uint32_t)s * (uint32_t)PL * ximg16 + half16, ximg16, step1, ti == 0);
       if (lane == 0) mbar_arrive(&x_empty[s]);
       // ---------- epilogue 1: h = acc + b1 -> [global] -> lrelu -> split -> H image ----------
       const int h0 = it * p.to - p.p2;
@@ -301,11 +303,11 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
           const uint32_t bo = 4u * (uint32_t)(lane & 3);                // byte offset of this thread's 2 channels in the 16-byte chunk
           const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)i) + bo;
           *reinterpret_cast<__nv_bfloat162*>(h_base + o) = hb;
-          *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o) = lb;
+          if constexpr (PL == 2) *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o) = lb;
           if (p.pair && r > 0) {   // second half of the previous row: act(h[r]) = "row r - 1, + 1"
             const uint32_t o2 = sw128_offset((uint32_t)(r - 1), (uint32_t)i + 4u) + bo;
             *reinterpret_cast<__nv_bfloat162*>(h_base + o2) = hb;
-            *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o2) = lb;
+            if constexpr (PL == 2) *reinterpret_cast<__nv_bfloat162*>(h_base + himg + o2) = lb;
           }
         }
       }
@@ -333,6 +335,11 @@ __global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid
   }
 }
 
+template <int NT>
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) { resblock_tc_body<NT, 2>(p); }
+template <int NT>
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_bf16_kernel(const __grid_constant__ RbParams p) { resblock_tc_body<NT, 1>(p); }
+
 // ---------------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------------
@@ -355,6 +362,7 @@ static RbPlan rb_plan(const KtResblockDesc* d) {
   if (d->pad_left1 < 0 || d->pad_left1 > span1 || d->pad_left2 < 0 || d->pad_left2 > span2) return pl;
   p.batch = d->batch; p.t = d->t; p.c = d->channels; p.k = d->kernel; p.d1 = d->dilation;
   p.p1 = d->pad_left1; p.p2 = d->pad_left2; p.slope = d->slope;
+  p.planes = d->path == KT_PATH_BF16 ? 1 : 2;
   p.to = kRbM - span2;
   p.tiles_per_item = ceil_div(p.t, p.to);
   p.total_tiles = p.tiles_per_item * p.batch;
@@ -363,12 +371,12 @@ static RbPlan rb_plan(const KtResblockDesc* d) {
   p.last_kslices = (p.pair && (p.k & 1)) ? 2 : 4;
   p.rows_x = (kRbM + span1 + 7) & ~7;
   p.rows_h = (kRbM + span2 + 7) & ~7;
-  p.tile_bytes = 2 * p.c * 128;
-  const int himg2 = 2 * p.rows_h * 128;
+  p.tile_bytes = p.planes * p.c * 128;
+  const int himg2 = p.planes * p.rows_h * 128;
   p.rows_box = p.rows_x + (p.pair ? p.d1 : 0);
   p.fstage_bytes = (p.c / 32) * p.rows_box * 128;
   if (p.rows_box > 256) return pl;                 // TMA box limit (k >= 13 with dilation >= 9): the pair runs as two convs
-  const int ximg2 = 2 * p.rows_x * 128 + p.fstage_bytes;   // one x stage: (hi | lo) image + its fp32 landing stage
+  const int ximg2 = p.planes * p.rows_x * 128 + p.fstage_bytes;   // one x stage: (hi | lo) image + its fp32 landing stage
   const int cap = kMaxDynSmem - 1024;
   // preference: resident weights + 2 x stages; resident + 1; ring (>= 3 stages) + 2 x stages; ring + 1
   const int res_bytes = 2 * p.nsteps * p.tile_bytes;
@@ -405,16 +413,31 @@ extern "C" int kt_resblock_pack(const KtResblockDesc* d, const float* w, void* i
   KT_REQUIRE(pl.ok && w && img, "resblock_pack: shape not supported by the fused kernel");
   if (pl.p.pair) {
     const int total = pl.p.nsteps * 32 * 64;
-    rb_pack_pair_kernel<<<std::min((total + 255) / 256, 132 * 4), 256, 0, st>>>(w, d->kernel, pl.p.nsteps,
-                                                                                reinterpret_cast<__nv_bfloat16*>(img));
+    const int blocks = std::min((total + 255) / 256, 132 * 4);
+    auto* out = reinterpret_cast<__nv_bfloat16*>(img);
+    if (pl.p.planes == 1) rb_pack_pair_kernel<1><<<blocks, 256, 0, st>>>(w, d->kernel, pl.p.nsteps, out);
+    else rb_pack_pair_kernel<2><<<blocks, 256, 0, st>>>(w, d->kernel, pl.p.nsteps, out);
     KT_CHECK_CUDA(cudaGetLastError());
     return KT_OK;
   }
-  // C = 64: one [hi 64 rows | lo 64 rows] tile per tap == conv_tc's packed forward image of a 64 -> 64 layer
+  // C = 64: one [hi 64 rows | lo 64 rows] tile per tap (hi only in single-pass bf16) == conv_tc's packed forward image of a
+  // 64 -> 64 layer of the same precision
   KtConv1dDesc cd{};
   cd.batch = d->batch; cd.nsub = 1; cd.t_in = d->t; cd.t_out = d->t; cd.c_in = 64; cd.c_out = 64; cd.groups = 1;
-  cd.kernel = d->kernel; cd.stride = 1; cd.dilation = 1; cd.pad_left = d->kernel - 1; cd.upsample = 1; cd.path = KT_PATH_TC;
+  cd.kernel = d->kernel; cd.stride = 1; cd.dilation = 1; cd.pad_left = d->kernel - 1; cd.upsample = 1;
+  cd.path = d->path == KT_PATH_BF16 ? KT_PATH_BF16 : KT_PATH_TC;
   return tc_pack_layer(&cd, 0, w, img, st);
+}
+
+template <int PL>
+static int launch_resblock(const RbParams& p, int grid, size_t smem, cudaStream_t st) {
+  constexpr auto k32 = PL == 1 ? resblock_tc_bf16_kernel<32> : resblock_tc_kernel<32>;
+  constexpr auto k64 = PL == 1 ? resblock_tc_bf16_kernel<64> : resblock_tc_kernel<64>;
+  KT_CHECK_CUDA(allow_dyn_smem<k32>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<k64>(kMaxDynSmem));
+  if (p.c == 32) k32<<<grid, kRbThreads, smem, st>>>(p);
+  else k64<<<grid, kRbThreads, smem, st>>>(p);
+  return KT_OK;
 }
 
 extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
@@ -434,11 +457,9 @@ extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const vo
   const int rc = encode_tensor_map(&p.tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, x, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "resblock_fwd");
   if (rc) return rc;
-  KT_CHECK_CUDA(allow_dyn_smem<resblock_tc_kernel<32>>(kMaxDynSmem));
-  KT_CHECK_CUDA(allow_dyn_smem<resblock_tc_kernel<64>>(kMaxDynSmem));
   const int grid = std::min(p.total_tiles, device_sm_count());
-  if (p.c == 32) resblock_tc_kernel<32><<<grid, kRbThreads, pl.smem, st>>>(p);
-  else resblock_tc_kernel<64><<<grid, kRbThreads, pl.smem, st>>>(p);
+  const int rc2 = p.planes == 1 ? launch_resblock<1>(p, grid, pl.smem, st) : launch_resblock<2>(p, grid, pl.smem, st);
+  if (rc2) return rc2;
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }

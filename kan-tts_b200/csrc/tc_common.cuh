@@ -128,6 +128,16 @@ __device__ __forceinline__ void wgmma_x3(float (&d)[kWgmmaMaxRegs], uint32_t a_h
   wgmma_bf16_n<N, TA, TB>(d, desc_lo(a_hi), desc_lo(b_hi), 1u);
 }
 
+// One K = 16 slice of a product whose operands are PL bf16 planes (hi, then lo, plane distances a_pl / b_pl): PL = 2 the
+// split-bf16 product above, PL = 1 the single-pass bf16 product hi * hi (KT_PATH_BF16)
+template <int PL, int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_slice(float (&d)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t a_pl, uint32_t b_hi, uint32_t b_pl,
+                                            uint32_t scale_d) {
+  static_assert(PL == 1 || PL == 2, "wgmma_slice: one or two planes");
+  if constexpr (PL == 2) wgmma_x3<N, TA, TB>(d, a_hi, a_pl, b_hi, b_pl, scale_d);
+  else wgmma_bf16_n<N, TA, TB>(d, desc_lo(a_hi), desc_lo(b_hi), scale_d);
+}
+
 // A value every lane of the warp already holds, in a form ptxas can prove warp-uniform.  ptxas serialises EVERY wgmma of a
 // kernel (a wait for completion after each one; ptxas info C7520) when it cannot prove that all threads run the same
 // number of them, and it cannot for a loop bound derived from the counter of a loop that waits on an mbarrier: the MMA
@@ -152,11 +162,22 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo
   lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
+// Store the planes of 8 values at byte offset o of a hi image (and of its lo image when PL = 2): PL = 1 keeps hi only, the
+// round-to-nearest bf16 of each value
+template <int PL>
+__device__ __forceinline__ void store_planes8(const float (&x)[8], uint8_t* img_hi, uint8_t* img_lo, size_t o) {
+  uint4 hi, lo;
+  split8(x, hi, lo);
+  *reinterpret_cast<uint4*>(img_hi + o) = hi;
+  if constexpr (PL == 2) *reinterpret_cast<uint4*>(img_lo + o) = lo;
+}
+
 // fp32 operand -> hi / lo bf16 planes ([plane][batch][time][sub-sequence][channel], the activation layout), with the
 // operand's fused transform (pre-activation / activation-derivative mask) -- the same arithmetic as stage_rows, so a tile
 // pulled from the planes by the TMA unit holds the bits a register-staged tile would.  Two operands in ONE launch: CTAs
 // [0, blocks_a) convert operand A, the rest operand B (n8b = 0: none).  Static: every kernel file that feeds its tiles
-// from planes compiles its own instance of this one definition.
+// from planes compiles its own instance of this one definition.  PL = 1 (single-pass bf16): the hi plane only.
+template <int PL>
 static __global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16* __restrict__ hia, Side sb, long long n8b,
                                            __nv_bfloat16* __restrict__ hib, int blocks_a) {
   const bool first = (int)blockIdx.x < blocks_a;
@@ -178,20 +199,18 @@ static __global__ void split_planes_kernel(Side sa, long long n8a, __nv_bfloat16
 #pragma unroll
       for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : x[e] * s.slope;
     }
-    uint4 h, l;
-    split8(x, h, l);
-    reinterpret_cast<uint4*>(hi)[i] = h;
-    reinterpret_cast<uint4*>(lo)[i] = l;
+    store_planes8<PL>(x, reinterpret_cast<uint8_t*>(hi), reinterpret_cast<uint8_t*>(lo), (size_t)i * 16);
   }
 }
 
 // Launch split_planes_kernel over na elements of operand a into the planes at pa and nb elements of b into pb (na, nb
-// multiples of 8; nb = 0: one operand).
+// multiples of 8; nb = 0: one operand), `planes` (1 or 2) planes each.
 static inline cudaError_t split_planes(const Side& a, long long na, __nv_bfloat16* pa, const Side& b, long long nb,
-                                       __nv_bfloat16* pb, cudaStream_t st) {
+                                       __nv_bfloat16* pb, int planes, cudaStream_t st) {
   auto blocks_for = [](long long n8) { return (int)std::max<long long>(1, std::min<long long>((n8 + 255) / 256, 132LL * 16)); };
   const int ba = blocks_for(na / 8), bb = nb > 0 ? blocks_for(nb / 8) : 0;
-  split_planes_kernel<<<ba + bb, 256, 0, st>>>(a, na / 8, pa, b, nb / 8, pb, ba);
+  if (planes == 1) split_planes_kernel<1><<<ba + bb, 256, 0, st>>>(a, na / 8, pa, b, nb / 8, pb, ba);
+  else split_planes_kernel<2><<<ba + bb, 256, 0, st>>>(a, na / 8, pa, b, nb / 8, pb, ba);
   return cudaGetLastError();
 }
 
@@ -264,7 +283,7 @@ struct RowMap {
 // converts and stores.  The two phases are separate fully-unrolled loops without early exits: with one
 // CTA per SM the staging loop is pure DRAM/L2 latency, and a fused load->convert->store loop measured
 // ~1 load in flight per thread.
-template <int NB, bool VEC, bool AUX, bool SIMPLE = false, bool STREAM = false, bool PACK = false>
+template <int NB, bool VEC, bool AUX, bool SIMPLE = false, bool STREAM = false, bool PACK = false, int PL = 2>
 __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                                 const float* aux_base, int c_total, int ch0, int nv, const RowMap& rm,
                                                 int rows, int tid, int r_begin = 0) {
@@ -318,13 +337,7 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
 #pragma unroll
         for (int e = 0; e < 8; ++e) x[e] = side_apply(x[e], ax[e], s.mode, s.slope);
       }
-      uint4 hi, lo;
-      tc::split8(x, hi, lo);
-      if (r < rows) {
-        const uint32_t o = tc::sw128_offset((uint32_t)r, (uint32_t)q);
-        *reinterpret_cast<uint4*>(img_hi + o) = hi;
-        *reinterpret_cast<uint4*>(img_lo + o) = lo;
-      }
+      if (r < rows) tc::store_planes8<PL>(x, img_hi, img_lo, tc::sw128_offset((uint32_t)r, (uint32_t)q));
     }
   }
 }
@@ -332,7 +345,8 @@ __device__ __forceinline__ void stage_rows_impl(uint8_t* img_hi, uint8_t* img_lo
 // SIMPLE: the host guarantees nsub == 1, up == 1 and 16-byte-aligned 8-channel chunks (c_valid % 8 == 0, c_total % 4
 // == 0): only the vectorised instantiations exist in that kernel variant, which roughly halves its code size -- the
 // generic kernel (~140 KB of SASS shared by four concurrently running warp roles) does not fit the instruction cache.
-template <int NB, bool SIMPLE = false, int NB_AUX = NB, bool STREAM = false, bool PACK = false>
+// PL: bf16 planes written per image (2: hi / lo split, 1: hi only, img_lo unused)
+template <int NB, bool SIMPLE = false, int NB_AUX = NB, bool STREAM = false, bool PACK = false, int PL = 2>
 __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, const Side& s, const float* base,
                                            const float* aux_base, int c_total, int ch0, int c_valid, bool fill_all,
                                            const RowMap& rm, int rows, int tid, int r_begin = 0) {
@@ -352,23 +366,23 @@ __device__ __forceinline__ void stage_rows(uint8_t* img_hi, uint8_t* img_lo, con
     for (int r = r_begin + (tid >> 3); r < rows; r += 16) {
       const uint32_t o = tc::sw128_offset((uint32_t)r, (uint32_t)q);
       *reinterpret_cast<uint4*>(img_hi + o) = z;
-      *reinterpret_cast<uint4*>(img_lo + o) = z;
+      if constexpr (PL == 2) *reinterpret_cast<uint4*>(img_lo + o) = z;
     }
     return;
   }
   const bool vec = nv == 8 && (c_total & 3) == 0 && ((ch0 + q * 8) & 3) == 0;
   const bool has_aux = s.mode >= SIDE_DLRELU;
   if constexpr (SIMPLE) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true, true, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false, true, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, true, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, true, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
     return;
   }
   if (vec) {
-    if (has_aux) stage_rows_impl<NB_AUX, true, true, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<NB, true, false, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<NB_AUX, true, true, false, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<NB, true, false, false, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   } else {
-    if (has_aux) stage_rows_impl<2, false, true, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
-    else stage_rows_impl<2, false, false, false, STREAM, PACK>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    if (has_aux) stage_rows_impl<2, false, true, false, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
+    else stage_rows_impl<2, false, false, false, STREAM, PACK, PL>(img_hi, img_lo, s, base, aux_base, c_total, ch0, nv, rm, rows, tid, r_begin);
   }
 }
 

@@ -39,16 +39,20 @@ inline int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int ra
   return KT_OK;
 }
 
-// Split-bf16 planes of a [batch][t][nsub][c] fp32 tensor (split_planes, tc_common.cuh): [hi | lo][batch][t][nsub][c] bf16.
-// plane_floats: workspace floats they occupy (one per element), rounded up to 256 bytes.
-inline long long plane_floats(long long batch, long long t, long long nsub, long long c) { return (batch * t * nsub * c + 63) & ~63LL; }
+// Split-bf16 planes of a [batch][t][nsub][c] fp32 tensor (split_planes, tc_common.cuh): [hi | lo][batch][t][nsub][c] bf16
+// (single-pass bf16: the hi plane only).  plane_floats: workspace floats that `planes` planes occupy (half a float per element
+// per plane), rounded up to 256 bytes.
+inline long long plane_floats(long long batch, long long t, long long nsub, long long c, int planes = 2) {
+  return ((batch * t * nsub * c * planes + 1) / 2 + 63) & ~63LL;
+}
 
 // Tensor map of residue class rho of such planes, time steps rho, rho + step, ...: 5-D boxes of box_c channels x nsub x box_t
-// of those steps, SWIZZLE_128B; coordinates (channel, sub-sequence, step of the class, batch, plane)
+// of those steps, SWIZZLE_128B; coordinates (channel, sub-sequence, step of the class, batch, plane), `nplanes` planes
 inline int encode_plane_map(CUtensorMap* map, const __nv_bfloat16* planes, int batch, int t, int nsub, int c, int step, int rho,
-                            int box_c, int box_t, const char* what) {
+                            int box_c, int box_t, const char* what, int nplanes = 2) {
   const long long n = (long long)batch * t * nsub * c;
-  const cuuint64_t dims[5] = {(cuuint64_t)c, (cuuint64_t)nsub, (cuuint64_t)ceil_div(t - rho, step), (cuuint64_t)batch, 2};
+  const cuuint64_t dims[5] = {(cuuint64_t)c, (cuuint64_t)nsub, (cuuint64_t)ceil_div(t - rho, step), (cuuint64_t)batch,
+                              (cuuint64_t)nplanes};
   const cuuint64_t strides[4] = {(cuuint64_t)c * 2, (cuuint64_t)step * nsub * c * 2, (cuuint64_t)t * nsub * c * 2, (cuuint64_t)n * 2};
   const cuuint32_t box[5] = {(cuuint32_t)box_c, (cuuint32_t)nsub, (cuuint32_t)box_t, 1, 1};
   return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, planes + (long long)rho * nsub * c, dims, strides, box,

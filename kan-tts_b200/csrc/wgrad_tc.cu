@@ -14,6 +14,8 @@
 // Each CTA owns (ca tile, cb tile, a group of <= U "units" of one residue class = U*NT <= 128 accumulator
 // columns) for a slice of the (batch, flattened time) range (split-K); partial tiles go to a workspace
 // with plain stores and a second kernel reduces over the splits in order (deterministic, and cheaper than ~10^7 atomics).
+// Single-pass bf16 (KT_PATH_BF16): the instances with PL = 1 stage / load one bf16 plane per operand and issue the hi * hi
+// wgmma alone; the split-K partials, their reduces and the summation order are those of bf16x3 (PL = 2).
 #include <algorithm>
 
 #include "common.cuh"
@@ -39,6 +41,7 @@ struct WgTcParams {
   int M;                       // base rows m per sub-sequence
   int step, up;
   int mode, NT, n_cb_tiles, n_ca_tiles;
+  int planes;                  // bf16 planes per operand image: 2 bf16x3, 1 single-pass bf16 (the instance's PL)
   int nsplit, chunks_per_batch;   // chunk = kWgTK flattened rows (register-staged) or tt base time steps (TMA)
   int a_groups, b_groups;      // 64-channel images per stage on each side
   int rows_a;                  // register-staged route: A image rows (max over unit groups), multiple of 8
@@ -78,26 +81,29 @@ struct WgCta {
 constexpr int kWgConsumerArrivals = 8;   // one per consumer warp
 
 // MMAs of one staged chunk for one unit (accumulators acc[OFF, OFF + NT / 2)): A (M = 64 channels x K rows) and B (K rows x
-// NT channels) are MN-major images, the hi / lo planes img16 apart, K = 16 rows = 128 descriptor units per slice
-template <int NT, int OFF>
+// NT channels) are MN-major images, the hi / lo planes img16 apart, K = 16 rows = 128 descriptor units per slice (PL = 1: the
+// hi * hi product only)
+template <int NT, int OFF, int PL>
 __device__ __forceinline__ void wg_unit_mma(float (&acc)[kWgmmaMaxRegs], uint32_t a_hi, uint32_t img_a16, uint32_t b_hi, uint32_t img_b16,
                                             int kslices) {
   for (int ks = 0; ks < kslices; ++ks) {
     const uint32_t ko = (uint32_t)ks * 128u;
-    wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko + img_a16), desc_lo(b_hi + ko), 1u);
-    wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko), desc_lo(b_hi + ko + img_b16), 1u);
+    if constexpr (PL == 2) {
+      wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko + img_a16), desc_lo(b_hi + ko), 1u);
+      wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko), desc_lo(b_hi + ko + img_b16), 1u);
+    }
     wgmma_bf16_n<NT, 1, 1, OFF>(acc, desc_lo(a_hi + ko), desc_lo(b_hi + ko), 1u);
   }
 }
 
 // all units of one staged chunk, then wait for the MMAs (the stage is released by the caller)
-template <int NT>
+template <int NT, int PL>
 __device__ __forceinline__ void wg_chunk_mma(float (&acc)[kWgmmaMaxRegs], uint32_t sbase16, uint32_t b_hi, uint32_t img_a16, uint32_t img_b16,
                                              const uint32_t* s_shift, const uint32_t* s_half, int nu, int cw, int kslices) {
   wgmma_fence();
-  wg_unit_mma<NT, 0>(acc, sbase16 + s_shift[0] + (cw ? s_half[0] : 0u), img_a16, b_hi, img_b16, kslices);
+  wg_unit_mma<NT, 0, PL>(acc, sbase16 + s_shift[0] + (cw ? s_half[0] : 0u), img_a16, b_hi, img_b16, kslices);
   if constexpr (kWgmmaMaxN / NT > 1) {
-    if (nu > 1) wg_unit_mma<NT, NT / 2>(acc, sbase16 + s_shift[1] + (cw ? s_half[1] : 0u), img_a16, b_hi, img_b16, kslices);
+    if (nu > 1) wg_unit_mma<NT, NT / 2, PL>(acc, sbase16 + s_shift[1] + (cw ? s_half[1] : 0u), img_a16, b_hi, img_b16, kslices);
   }
   wgmma_commit();
   wgmma_wait<0>();
@@ -151,11 +157,12 @@ __device__ __forceinline__ void wg_store(const WgTcParams& p, const WgCta& cta, 
 }
 
 // per unit of this CTA: A-side row shift and the offset of the second warpgroup's 64 rows, in 16-byte descriptor units
+// (img_a: bytes of ALL planes of one A image, the distance of two 64-channel images)
 __device__ __forceinline__ void wg_unit_table(const WgTcParams& p, const WgCta& cta, int img_a, uint32_t* s_shift, uint32_t* s_half) {
   for (int u = threadIdx.x; u < cta.nu; u += blockDim.x) {
     const int n_a = p.unit_tap0[cta.u0 + u];
     uint32_t half;
-    if (p.mode == 0) half = 2u * (uint32_t)img_a;
+    if (p.mode == 0) half = (uint32_t)img_a;
     // mode 1: second half of M = the next tap of the same residue (rows 64..127 are discarded when the unit has one tap)
     else half = p.unit_ntaps[cta.u0 + u] == 2 ? (uint32_t)((p.tap_q[n_a + 1] - p.tap_q[n_a]) * p.nsub) * 128u : 128u;
     s_shift[u] = ((uint32_t)((p.tap_q[n_a] - cta.qlo) * p.nsub) * 128u) >> 4;
@@ -167,13 +174,14 @@ __device__ __forceinline__ void wg_unit_table(const WgTcParams& p, const WgCta& 
 // by the ISSUE rate of the fp32 -> split-bf16 staging (~80 instructions per 8 elements), so the producers are 8 warps.
 constexpr int kWgThreads = 512;
 
-template <int NT>
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgTcParams p) {
+// (PL: bf16 planes per operand image; kernels wgrad_tc_kernel / wgrad_tc_bf16_kernel)
+template <int NT, int PL>
+__device__ __forceinline__ void wgrad_tc_body(const WgTcParams& p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   const int img_a = p.rows_a * 128;            // one plane of one A image
   const int img_b = kWgTK * 128;               // one plane of one B image
-  const int stage_bytes = 2 * (p.a_groups * img_a + p.b_groups * img_b);
+  const int stage_bytes = PL * (p.a_groups * img_a + p.b_groups * img_b);
   uint8_t* stage0 = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * (size_t)stage_bytes);
   uint64_t* full = bars;        // [2] producers -> MMA
@@ -189,7 +197,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     mbar_fence_init();
     fence_proxy_async();
   }
-  wg_unit_table(p, cta, img_a, s_shift, s_half);
+  wg_unit_table(p, cta, PL * img_a, s_shift, s_half);
   __syncthreads();
 
   if (warp < 4 || warp >= 12) {
@@ -209,19 +217,19 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       ra.fv0 = f0 + cta.qlo * p.nsub;
       ra.nsub = p.nsub; ra.step = p.step; ra.rho = p.grp_rho[cta.grp]; ra.up = p.up; ra.t_lim = p.t_a * p.up;
       for (int g = 0; g < p.a_groups; ++g) {
-        uint8_t* hi = st + (size_t)g * 2 * img_a;
+        uint8_t* hi = st + (size_t)g * PL * img_a;
         const int c_lo = cta.ca_tile * (p.mode == 0 ? 128 : 64) + g * 64;           // channel offset inside the group
-        stage_rows<4, false, 2>(hi, hi + img_a, p.a, p.a.p, p.a.aux, p.ca, cta.cgrp * p.ca_g + c_lo, min(64, p.ca_g - c_lo), true, ra,
+        stage_rows<4, false, 2, false, false, PL>(hi, hi + img_a, p.a, p.a.p, p.a.aux, p.ca, cta.cgrp * p.ca_g + c_lo, min(64, p.ca_g - c_lo), true, ra,
                                 p.rows_a, ptid);
       }
       RowMap rb;  // base side: rows m (flattened with w), zero beyond M
       rb.base_row = (long long)bb * p.t_b * p.nsub;
       rb.fv0 = f0; rb.nsub = p.nsub; rb.step = 1; rb.rho = 0; rb.up = 1; rb.t_lim = min(p.M, p.t_b);
-      uint8_t* bst = st + (size_t)p.a_groups * 2 * img_a;
+      uint8_t* bst = st + (size_t)p.a_groups * PL * img_a;
       for (int g = 0; g < p.b_groups; ++g) {
-        uint8_t* hi = bst + (size_t)g * 2 * img_b;
+        uint8_t* hi = bst + (size_t)g * PL * img_b;
         const int c_lo = cta.cb_tile * NT + g * 64;
-        stage_rows<2, false, 2>(hi, hi + img_b, p.b, p.b.p, p.b.aux, p.cb, cta.cgrp * p.cb_g + c_lo, min(64, p.cb_g - c_lo), true, rb,
+        stage_rows<2, false, 2, false, false, PL>(hi, hi + img_b, p.b, p.b.p, p.b.aux, p.cb, cta.cgrp * p.cb_g + c_lo, min(64, p.cb_g - c_lo), true, rb,
                                 kWgTK, ptid);
       }
       fence_proxy_async();
@@ -230,10 +238,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   } else {
     // ===================== consumers =====================
     const int cw = (warp - 4) >> 2, wq = warp & 3;
-    const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
+    const uint32_t lbo_b16 = (((uint32_t)PL * (uint32_t)img_b) >> 4) << 16;
     const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
     const uint32_t st16[2] = {smem_u32(stage0) >> 4, smem_u32(stage0 + stage_bytes) >> 4};
-    const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
+    const uint32_t boff16 = (uint32_t)(p.a_groups * PL * img_a) >> 4;
     float acc[kWgmmaMaxRegs];
 #pragma unroll
     for (int i = 0; i < kWgmmaMaxRegs; ++i) acc[i] = 0.f;
@@ -241,12 +249,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     for (long long c = cta.c_begin; c < cta.c_end; ++c, ++it) {
       const int s = it & 1;
       mbar_wait(&full[s], (it >> 1) & 1);
-      wg_chunk_mma<NT>(acc, st16[s], (st16[s] + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kWgTK / 16);
+      wg_chunk_mma<NT, PL>(acc, st16[s], (st16[s] + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kWgTK / 16);
       if (lane == 0) mbar_arrive(&empty[s]);
     }
     wg_store<NT>(p, cta, acc, cw, wq, lane);
   }
 }
+
+template <int NT>
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgTcParams p) { wgrad_tc_body<NT, 2>(p); }
+template <int NT>
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_bf16_kernel(const __grid_constant__ WgTcParams p) { wgrad_tc_body<NT, 1>(p); }
 
 // ---- TMA-fed variant (plain convs, no nearest-upsampling, channel counts % 8 == 0) -------------------------------------
 // The register-staged kernel above is bound by its producers: every CTA converts its fp32 operand rows to split bf16
@@ -271,13 +284,14 @@ struct WgTmaExtra {
 };
 
 // (the operand planes are written by split_planes, tc_common.cuh)
-template <int NT>
-__global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __grid_constant__ WgTcParams p, const __grid_constant__ WgTmaExtra x) {
+// (kernels wgrad_tma_kernel / wgrad_tma_bf16_kernel)
+template <int NT, int PL>
+__device__ __forceinline__ void wgrad_tma_body(const WgTcParams& p, const WgTmaExtra& x) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   const int img_a = x.rows_a_p * 128;          // one plane of one A image
   const int img_b = x.Rp * 128;                // one plane of one B image
-  const int stage_bytes = 2 * (p.a_groups * img_a + p.b_groups * img_b);
+  const int stage_bytes = PL * (p.a_groups * img_a + p.b_groups * img_b);
   uint8_t* stage0 = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)x.nstages * stage_bytes);
   uint64_t* full = bars;                        // [nstages] TMA -> MMA
@@ -294,23 +308,23 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   }
   {  // padding rows of every image (never written by the TMA boxes): zero, so that a partial last K slice contributes nothing
     const int a_box_rows = x.a_box_t * p.nsub;
-    const int n_img = 2 * (p.a_groups + p.b_groups);
+    const int n_img = PL * (p.a_groups + p.b_groups);
     for (int s = 0; s < x.nstages; ++s)
       for (int i = 0; i < n_img; ++i) {
-        const bool is_a = i < 2 * p.a_groups;
-        uint8_t* img = stage0 + (size_t)s * stage_bytes + (is_a ? (size_t)i * img_a : (size_t)2 * p.a_groups * img_a + (size_t)(i - 2 * p.a_groups) * img_b);
+        const bool is_a = i < PL * p.a_groups;
+        uint8_t* img = stage0 + (size_t)s * stage_bytes + (is_a ? (size_t)i * img_a : (size_t)PL * p.a_groups * img_a + (size_t)(i - PL * p.a_groups) * img_b);
         const int r0 = is_a ? a_box_rows : x.R, r1 = is_a ? x.rows_a_p : x.Rp;
         for (int o = r0 * 128 + tid * 16; o < r1 * 128; o += kWgTmaThreads * 16) *reinterpret_cast<uint4*>(img + o) = make_uint4(0u, 0u, 0u, 0u);
       }
   }
-  wg_unit_table(p, cta, img_a, s_shift, s_half);
+  wg_unit_table(p, cta, PL * img_a, s_shift, s_half);
   fence_proxy_async();
   __syncthreads();
 
   if (warp == 8) {
     // ===================== TMA producer =====================
     if (elect_one()) {
-      const uint32_t tx = 2u * (uint32_t)(p.a_groups * x.a_box_t * p.nsub + p.b_groups * x.R) * 128u;
+      const uint32_t tx = (uint32_t)PL * (uint32_t)(p.a_groups * x.a_box_t * p.nsub + p.b_groups * x.R) * 128u;
       const CUtensorMap* ma = &x.map_a[p.grp_rho[cta.grp]];
       const int ca0 = cta.cgrp * p.ca_g + cta.ca_tile * (p.mode == 0 ? 128 : 64);
       const int cb0 = cta.cgrp * p.cb_g + cta.cb_tile * NT;
@@ -323,12 +337,12 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
         uint8_t* st = stage0 + (size_t)s * stage_bytes;
         mbar_arrive_expect_tx(&full[s], tx);
         for (int g = 0; g < p.a_groups; ++g)
-          for (int pl = 0; pl < 2; ++pl)
-            tma_load_5d(st + (size_t)(2 * g + pl) * img_a, ma, ca0 + g * 64, 0, m0 + cta.qlo, bb, pl, &full[s]);
-        uint8_t* bst = st + (size_t)p.a_groups * 2 * img_a;
+          for (int pl = 0; pl < PL; ++pl)
+            tma_load_5d(st + (size_t)(PL * g + pl) * img_a, ma, ca0 + g * 64, 0, m0 + cta.qlo, bb, pl, &full[s]);
+        uint8_t* bst = st + (size_t)p.a_groups * PL * img_a;
         for (int g = 0; g < p.b_groups; ++g)
-          for (int pl = 0; pl < 2; ++pl)
-            tma_load_5d(bst + (size_t)(2 * g + pl) * img_b, &x.map_b, cb0 + g * 64, 0, m0, bb, pl, &full[s]);
+          for (int pl = 0; pl < PL; ++pl)
+            tma_load_5d(bst + (size_t)(PL * g + pl) * img_b, &x.map_b, cb0 + g * 64, 0, m0, bb, pl, &full[s]);
       }
       // every issued box has landed before the CTA may exit: the consumers waited for all of them
     }
@@ -336,10 +350,10 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
   } else {
     // ===================== consumers =====================
     const int cw = warp >> 2, wq = warp & 3;
-    const uint32_t lbo_b16 = ((2u * (uint32_t)img_b) >> 4) << 16;
+    const uint32_t lbo_b16 = (((uint32_t)PL * (uint32_t)img_b) >> 4) << 16;
     const uint32_t img_a16 = (uint32_t)img_a >> 4, img_b16 = (uint32_t)img_b >> 4;
     const uint32_t st0_16 = smem_u32(stage0) >> 4, stage16 = (uint32_t)stage_bytes >> 4;
-    const uint32_t boff16 = (uint32_t)(p.a_groups * 2 * img_a) >> 4;
+    const uint32_t boff16 = (uint32_t)(p.a_groups * PL * img_a) >> 4;
     const int kslices = x.Rp >> 4;
     float acc[kWgmmaMaxRegs];
 #pragma unroll
@@ -349,11 +363,21 @@ __global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __gri
       const int s = r.slot();
       mbar_wait(&full[s], r.phase());
       const uint32_t sbase = st0_16 + (uint32_t)s * stage16;
-      wg_chunk_mma<NT>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kslices);
+      wg_chunk_mma<NT, PL>(acc, sbase, (sbase + boff16) | lbo_b16, img_a16, img_b16, s_shift, s_half, cta.nu, cw, kslices);
       if (lane == 0) mbar_arrive(&empty[s]);
     }
     wg_store<NT>(p, cta, acc, cw, wq, lane);
   }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_kernel(const __grid_constant__ WgTcParams p, const __grid_constant__ WgTmaExtra x) {
+  wgrad_tma_body<NT, 2>(p, x);
+}
+template <int NT>
+__global__ void __launch_bounds__(kWgTmaThreads, 1) wgrad_tma_bf16_kernel(const __grid_constant__ WgTcParams p,
+                                                                          const __grid_constant__ WgTmaExtra x) {
+  wgrad_tma_body<NT, 1>(p, x);
 }
 
 // sums the split-K partials: ws = [nsplit][stride] with stride >= n; elements [0, n) -> dw
@@ -420,9 +444,9 @@ struct WgPlan {
   long long planes_a_off, planes_b_off;   // TMA route: offsets (floats) of the operand planes inside the workspace
 };
 
-// bytes of one ring stage: the hi / lo planes of the A images (rows_a rows) and of the B images (rows_b rows)
+// bytes of one ring stage: the planes of the A images (rows_a rows) and of the B images (rows_b rows)
 static size_t wg_stage_bytes(const WgTcParams& p, int rows_a, int rows_b) {
-  return 2 * ((size_t)p.a_groups * rows_a * 128 + (size_t)p.b_groups * rows_b * 128);
+  return (size_t)p.planes * ((size_t)p.a_groups * rows_a * 128 + (size_t)p.b_groups * rows_b * 128);
 }
 
 // split-K factor: the ns in [1, min(units, 296)] of least cost(waves, chunks per CTA, ns), the smaller on a tie.  `ctas`
@@ -453,6 +477,7 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool plan_only = false) {
     while (p.groups % 2 == 0 && p.ca_g * 2 <= 64 && p.cb_g * 2 <= 256) { p.groups /= 2; p.ca_g *= 2; p.cb_g *= 2; p.gt *= 2; }
   }
   p.batch = d->batch; p.nsub = d->nsub; p.ca = ca; p.cb = cb; p.taps_total = d->kernel;
+  p.planes = d->path == KT_PATH_BF16 ? 1 : 2;
   p.t_a = tr ? d->t_out : d->t_in;
   p.t_b = tr ? d->t_in : d->t_out;
   p.M = p.t_b;
@@ -536,15 +561,16 @@ static WgPlan make_plan(const KtConv1dDesc* d, bool plan_only = false) {
     // and the reduce pass itself (~5 us) which a single split does not need at all (the kernel then writes dw directly)
     int u_max = 1;
     for (int g = 0; g < p.ngroups; ++g) u_max = std::max(u_max, p.grp_first_unit[g + 1] - p.grp_first_unit[g]);
-    const double stage_kb = 2.0 * (p.a_groups * x.rows_a_p + p.b_groups * x.Rp) * 128 / 1024.0;
-    const double chunk_us = std::max(stage_kb / 45.0, u_max * 3.0 * (x.Rp / 16) * (p.NT / 2) / 1900.0);
+    const double stage_kb = (double)p.planes * (p.a_groups * x.rows_a_p + p.b_groups * x.Rp) * 128 / 1024.0;
+    const double mmas = p.planes == 2 ? 3.0 : 1.0;   // wgmma per unit, K = 16 slice and 64 rows
+    const double chunk_us = std::max(stage_kb / 45.0, u_max * mmas * (x.Rp / 16) * (p.NT / 2) / 1900.0);
     const double out_us = out_bytes / 4e12 * 1e6;
     p.nsplit = split_k((long long)p.batch * p.chunks_per_batch, ctas, [&](double waves, double chunks, long long ns) {
       return waves * chunks * chunk_us + (ns > 1 ? 5.0 + (double)ns * out_us : 0.0);
     });
     pl.planes_a_off = (p.nsplit * p.split_stride + 63) & ~63LL;
-    pl.planes_b_off = pl.planes_a_off + plane_floats(p.batch, p.t_a, p.nsub, ca);
-    pl.ws_floats = pl.planes_b_off + plane_floats(p.batch, p.t_b, p.nsub, cb);
+    pl.planes_b_off = pl.planes_a_off + plane_floats(p.batch, p.t_a, p.nsub, ca, p.planes);
+    pl.ws_floats = pl.planes_b_off + plane_floats(p.batch, p.t_b, p.nsub, cb, p.planes);
   } else {
     p.rows_a = rows_a;
     p.chunks_per_batch = ceil_div(p.M * p.nsub, kWgTK);
@@ -580,6 +606,27 @@ extern "C" int64_t kt_conv1d_bwd_weight_tc_workspace(const KtConv1dDesc* d) {
   return pl.ok ? pl.ws_floats : 0;
 }
 
+// the weight-gradient instance of one call: TMA-fed or register-staged, N tile 64 / 128, PL planes
+template <int PL, bool TMA>
+static int launch_wgrad(const WgTcParams& p, const WgTmaExtra& x, dim3 grid, size_t smem, cudaStream_t st) {
+  if constexpr (TMA) {
+    constexpr auto k64 = PL == 1 ? wgrad_tma_bf16_kernel<64> : wgrad_tma_kernel<64>;
+    constexpr auto k128 = PL == 1 ? wgrad_tma_bf16_kernel<128> : wgrad_tma_kernel<128>;
+    KT_CHECK_CUDA(allow_dyn_smem<k64>(kMaxDynSmem));
+    KT_CHECK_CUDA(allow_dyn_smem<k128>(kMaxDynSmem));
+    if (p.NT == 64) k64<<<grid, kWgTmaThreads, smem, st>>>(p, x);
+    else k128<<<grid, kWgTmaThreads, smem, st>>>(p, x);
+  } else {
+    constexpr auto k64 = PL == 1 ? wgrad_tc_bf16_kernel<64> : wgrad_tc_kernel<64>;
+    constexpr auto k128 = PL == 1 ? wgrad_tc_bf16_kernel<128> : wgrad_tc_kernel<128>;
+    KT_CHECK_CUDA(allow_dyn_smem<k64>(kMaxDynSmem));
+    KT_CHECK_CUDA(allow_dyn_smem<k128>(kMaxDynSmem));
+    if (p.NT == 64) k64<<<grid, kWgThreads, smem, st>>>(p);
+    else k128<<<grid, kWgThreads, smem, st>>>(p);
+  }
+  return KT_OK;
+}
+
 extern "C" int kt_conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, const float* dy, const float* y, float* dw,
                                        float* dbias, float* ws, int64_t ws_floats, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -604,21 +651,17 @@ extern "C" int kt_conv1d_bwd_weight_tc(const KtConv1dDesc* d, const float* x, co
     __nv_bfloat16* pa = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_a_off);
     __nv_bfloat16* pb = reinterpret_cast<__nv_bfloat16*>(ws + pl.planes_b_off);
     const long long na = (long long)p.batch * p.t_a * p.nsub * p.ca, nb = (long long)p.batch * p.t_b * p.nsub * p.cb;
-    KT_CHECK_CUDA(split_planes(p.a, na, pa, p.b, nb, pb, st));
-    rc = encode_plane_map(&x.map_b, pb, p.batch, p.t_b, p.nsub, p.cb, 1, 0, 64, x.tt, "conv1d_bwd_weight_tc (operand B)");
+    KT_CHECK_CUDA(split_planes(p.a, na, pa, p.b, nb, pb, p.planes, st));
+    rc = encode_plane_map(&x.map_b, pb, p.batch, p.t_b, p.nsub, p.cb, 1, 0, 64, x.tt, "conv1d_bwd_weight_tc (operand B)", p.planes);
     for (int rho = 0; rc == KT_OK && rho < p.step; ++rho)
-      rc = encode_plane_map(&x.map_a[rho], pa, p.batch, p.t_a, p.nsub, p.ca, p.step, rho, 64, x.a_box_t, "conv1d_bwd_weight_tc (operand A)");
+      rc = encode_plane_map(&x.map_a[rho], pa, p.batch, p.t_a, p.nsub, p.ca, p.step, rho, 64, x.a_box_t, "conv1d_bwd_weight_tc (operand A)",
+                            p.planes);
     if (rc) return rc;
-    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<64>>(kMaxDynSmem));
-    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tma_kernel<128>>(kMaxDynSmem));
-    if (p.NT == 64) wgrad_tma_kernel<64><<<grid, kWgTmaThreads, pl.smem, st>>>(p, x);
-    else wgrad_tma_kernel<128><<<grid, kWgTmaThreads, pl.smem, st>>>(p, x);
+    rc = p.planes == 1 ? launch_wgrad<1, true>(p, x, grid, pl.smem, st) : launch_wgrad<2, true>(p, x, grid, pl.smem, st);
   } else {
-    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<64>>(kMaxDynSmem));
-    KT_CHECK_CUDA(allow_dyn_smem<wgrad_tc_kernel<128>>(kMaxDynSmem));
-    if (p.NT == 64) wgrad_tc_kernel<64><<<grid, kWgThreads, pl.smem, st>>>(p);
-    else wgrad_tc_kernel<128><<<grid, kWgThreads, pl.smem, st>>>(p);
+    rc = p.planes == 1 ? launch_wgrad<1, false>(p, pl.x, grid, pl.smem, st) : launch_wgrad<2, false>(p, pl.x, grid, pl.smem, st);
   }
+  if (rc) return rc;
   KT_CHECK_CUDA(cudaGetLastError());
   const long long n = (long long)p.taps_total * p.ca_g0 * p.cb;
   if (p.nsplit >= 16) {

@@ -30,7 +30,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .audio import stft
-from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KtNsfState, ptr
+from ._lib import KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_BF16, KtNsfState, ptr
 from .stream import Streamer, WindowTable, check_slots, own_weight, to_device
 
 # --------------------------------------------------------------------------------------------
@@ -79,6 +79,31 @@ def prefetch_weights(module, streams):
             for m in share:
                 v, g = m.effective_weight()
                 ops.prefetch_weight(m._cache, m.spec, v, g)
+
+
+# tensor-core precisions of set_precision: the compute path of a conv that may take the tensor cores
+PRECISIONS = {"bf16x3": KT_PATH_AUTO, "bf16": KT_PATH_BF16}
+
+
+def set_precision(module, precision):
+    """Run every tensor-core conv of a HiFi-GAN ``module`` tree (Generator, discriminators, PQMF) in ``precision``:
+    "bf16x3" (the default: split-bf16 operands, three MMAs per product, near-fp32 results) or "bf16" (each operand rounded
+    once to bf16, one MMA, fp32 accumulation).  Layers without a tensor-core route keep their exact-fp32 kernels in either.
+    The precision is not state: parameters, checkpoints and the optimizer are fp32 in both, and switching back gives the
+    bits of a model never switched.  Streamers made afterwards run in the new precision.  SAM-BERT, syBERT and the speaker
+    model (DTDNN) have no single-pass bf16 kernels: a tree containing one raises ValueError.  -> ``module``."""
+    if precision not in PRECISIONS:
+        raise ValueError(f"set_precision: precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
+    mods = list(module.modules())
+    for m in mods:
+        if type(m).__module__.rsplit(".", 1)[-1] in ("sambert", "speaker"):
+            raise ValueError(f"set_precision: {type(m).__name__} has no single-pass bf16 kernels (HiFi-GAN models only)")
+    new = PRECISIONS[precision]
+    for m in mods:
+        for spec in vars(m).values():
+            if isinstance(spec, ops.ConvSpec) and spec.path in PRECISIONS.values():
+                spec.path = new
+    return module
 
 
 def _spectral(d):

@@ -8,8 +8,22 @@ replacing that name runs the unchanged ``SpeakerEmbeddingProcessor`` on speaker.
 import sys
 
 
-def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=None, kantts_dataset=None):
-    """``kantts_se``: the speaker-embedding processor module to patch; by default
+def _with_precision(cls, precision):
+    """-> a subclass of HiFi-GAN module class ``cls`` whose instances are built in tensor-core ``precision``
+    (hifigan.set_precision), under the same name: the reference's model builder constructs it unchanged."""
+    from .hifigan import set_precision
+
+    def __init__(self, *args, **kwargs):
+        cls.__init__(self, *args, **kwargs)
+        set_precision(self, precision)
+    return type(cls.__name__, (cls,), {"__init__": __init__, "__module__": cls.__module__, "__qualname__": cls.__qualname__})
+
+
+def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=None, kantts_dataset=None, precision=None):
+    """``precision`` ("bf16" or "bf16x3"; None: the default bf16x3): the tensor-core precision of every HiFi-GAN model and
+    PQMF the patched checkout builds, so that its unchanged GAN_Trainer trains in single-pass bf16 with "bf16".
+
+    ``kantts_se``: the speaker-embedding processor module to patch; by default
     kantts.preprocess.se_processor.se_processor when it is already imported.  It is never imported here: it needs
     torchaudio and configures logging at import, which the HiFi-GAN and SAM-BERT flows do not want.
 
@@ -17,6 +31,9 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
     ``data.attn_prior_placeholder``, for a MAS run whose batches go through ``data.AttnPriors`` on the device.  Patched
     only when passed: without that transform the placeholder's NaN prior would reach the model."""
     from . import audio, data, hifigan, loss, pqmf, sambert, speaker
+    if precision is not None and precision not in hifigan.PRECISIONS:
+        raise ValueError(f"install: precision must be one of {sorted(hifigan.PRECISIONS)}, got {precision!r}")
+    wrap = (lambda cls: cls) if precision is None else (lambda cls: _with_precision(cls, precision))
     if kantts_models is None:
         import kantts.models as kantts_models
     if kantts_loss is None:
@@ -25,13 +42,15 @@ def install(kantts_models=None, kantts_loss=None, kantts_audio=None, kantts_se=N
         import kantts.utils.audio_torch as kantts_audio
     for name in ("Generator", "MultiPeriodDiscriminator", "MultiScaleDiscriminator", "SpecDiscriminator",
                  "MultiSpecDiscriminator"):
-        setattr(kantts_models, name, getattr(hifigan, name))
+        cls = wrap(getattr(hifigan, name))
+        setattr(kantts_models, name, cls)
         if hasattr(kantts_models, "hifigan") and hasattr(kantts_models.hifigan, "hifigan"):
-            setattr(kantts_models.hifigan.hifigan, name, getattr(hifigan, name))
+            setattr(kantts_models.hifigan.hifigan, name, cls)
     kantts_models.KanTtsTextsyBERT = sambert.KanTtsTextsyBERT
-    kantts_models.PQMF = pqmf.PQMF                           # hifigan_model_builder (kantts/models/__init__.py:65-67)
+    pqmf_cls = wrap(pqmf.PQMF)
+    kantts_models.PQMF = pqmf_cls                            # hifigan_model_builder (kantts/models/__init__.py:65-67)
     if hasattr(kantts_models, "pqmf"):                       # infer_hifigan.py:50-52 imports it from there
-        kantts_models.pqmf.PQMF = pqmf.PQMF
+        kantts_models.pqmf.PQMF = pqmf_cls
     for key, cls in loss.loss_dict.items():
         kantts_loss.loss_dict[key] = cls
         setattr(kantts_loss, cls.__name__, cls)

@@ -11,7 +11,8 @@ from dataclasses import dataclass, field, replace
 import torch
 
 from . import _lib
-from ._lib import (KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_FFMA, KT_PATH_TC, KT_PLAN_STREAM, KtConv1dDesc,
+from ._lib import (KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_BF16, KT_PATH_FFMA, KT_PATH_TC, KT_PLAN_STREAM,
+                   KtConv1dDesc,
                    KtMelDesc, KtResblockDesc, check, ptr, stream_ptr)
 
 _launches = 0          # kernels-launched counter (bench.py reports it as gpu_launches)
@@ -117,7 +118,8 @@ def _conv_work(spec, d):
 
 @dataclass
 class ConvSpec:
-    """Static description of one conv layer (forward semantics), see KtConv1dDesc."""
+    """Static description of one conv layer (forward semantics), see KtConv1dDesc.  ``path`` KT_PATH_BF16 runs the layer's
+    tensor-core passes in single-pass bf16 (hifigan.set_precision sets it for a whole model)."""
     c_in: int
     c_out: int
     kernel: int
@@ -145,9 +147,9 @@ class ConvSpec:
 
     def plan(self, batch, nsub, t_in, stream=False):
         """-> the ConvPlan of this layer for one input shape, cached per shape, exact-path flag (the tests toggle
-        set_force_ffma at run time) and stream flag (the forward of a stream chunk, see stream_conv).  Every field of the
-        spec must be set before its first plan."""
-        key = (batch, nsub, t_in, _exact(self), stream)
+        set_force_ffma at run time), stream flag (the forward of a stream chunk, see stream_conv) and compute path (the
+        precision a model is switched to).  Every other field of the spec must be set before its first plan."""
+        key = (batch, nsub, t_in, _exact(self), stream, self.path)
         p = self._plans.get(key)
         if p is None:
             p = self._plans[key] = ConvPlan(self, batch, nsub, t_in, key[3], stream)
@@ -191,7 +193,7 @@ class ConvPlan:
             return
         self.nt_fwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 0)
         self.nt_bwd = lib.kt_conv1d_tc_plan(ctypes.byref(d), 1)
-        if (not self.nt_bwd and spec.path == KT_PATH_AUTO and spec.upsample > 1 and spec.c_in % 4 == 0
+        if (not self.nt_bwd and spec.path in (KT_PATH_AUTO, KT_PATH_BF16) and spec.upsample > 1 and spec.c_in % 4 == 0
                 and not spec.transposed):
             # the nearest-upsampled conv has no tensor-core data gradient of its own: run the same conv over the
             # up-sampled rows (upsample = 1, no fused pre-activation) and fold it back with kt_upsample_grad_reduce
@@ -228,9 +230,10 @@ class PreparedWeight:
         self.conv_used = False  # a ConvFn forward ran on it: hifigan.prefetch_weights re-prepares it
 
     def image(self, key, d):
-        """A packed split-bf16 weight image: hi/lo SWIZZLE_128B tiles for the tensor-core conv kernels
-        (kt_weight_pack_tc, key (direction, N tile): the tiling can depend on the sequence length, hence the key on the
-        N tile) or the fused resblock's (kt_resblock_pack, key ("rb", C, k), d a KtResblockDesc).  Packed for
+        """A packed weight image: hi/lo SWIZZLE_128B tiles for the tensor-core conv kernels (kt_weight_pack_tc, key
+        (direction, N tile, path): the tiling can depend on the sequence length, hence the key on the N tile, and a
+        single-pass bf16 image holds the hi tiles only, hence the key on the descriptor's path) or the fused resblock's
+        (kt_resblock_pack, key ("rb", C, k, path), d a KtResblockDesc).  Packed for
         descriptor d on first use and re-packed in place once the weights changed; the image depends on its key only,
         so a re-pack reuses that first descriptor (prefetch_weight passes none)."""
         img = self.img.get(key)
@@ -500,7 +503,7 @@ class ConvFn(torch.autograd.Function):
         bd = None if bias is None else bias.detach()
         d, nt, n = run.d, run.tile(0), (spec.stride if spec.transposed else 1)
         if nt:
-            img = pw.image((0, nt), d)
+            img = pw.image((0, nt, d.path), d)
             ws = _workspace(run.ws_fwd, x.device)
             _run("conv_fwd_tc", spec, d, n + (ws is not None), n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True),
                                                                    ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd))
@@ -513,7 +516,7 @@ class ConvFn(torch.autograd.Function):
         ctx.plan = full if nb == B else spec.plan(nb, nsub, t_in)
         ctx.w_bwd, ctx.norm = pw.w_bwd, pw.norm
         nt_b = ctx.plan.tile(1) if x.requires_grad else 0
-        ctx.img_bwd = pw.image((1, nt_b), ctx.plan.d_bwd) if nt_b else None
+        ctx.img_bwd = pw.image((1, nt_b, ctx.plan.d_bwd.path), ctx.plan.d_bwd) if nt_b else None
         ctx.has_resid, ctx.has_bias, ctx.has_g = resid is not None, bias is not None, g is not None
         ctx.params = (v, g, bias)
         ctx.save_for_backward(x, y if spec.act_out != KT_ACT_NONE else None, v, g)
@@ -581,7 +584,7 @@ def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None, mask=None):
     d, nt = plan.d, plan.tile(0)
     m = None if mask is None else ctypes.byref(mask)
     if nt:
-        img = pw.image((0, nt), d)
+        img = pw.image((0, nt, d.path), d)
         _run("conv_fwd_tc", spec, d, 1, 1, ("kt_conv1d_fwd_tc_stream", ctypes.byref(d), ctypes.byref(win), m, ptr(x),
                                             ptr(img, True), ptr(bias), ptr(resid), ptr(y)))
     else:
@@ -634,10 +637,10 @@ def pair_conv(owner, x, spec, cache, v, g, bias, resid=None):
 def resblock_desc(spec1, spec2, batch, t):
     """-> KtResblockDesc when the pair (dilated conv, dilation-1 conv; same channels / kernel; fused input LeakyReLU, no
     output activation) can run on the fused kernel for this shape, else None (also on the exact path).  Cached per
-    shape on spec1."""
+    shape and path on spec1; the pair runs in single-pass bf16 when both convs do (set_precision)."""
     if _exact(spec1) or _exact(spec2):
         return None
-    key = (batch, t)
+    key = (batch, t, spec1.path, spec2.path)
     d = spec1._rb_cache.get(key, False)
     if d is not False:
         return d
@@ -649,7 +652,8 @@ def resblock_desc(spec1, spec2, batch, t):
           and spec1.t_out(t) == t and spec2.t_out(t) == t)
     if ok:
         cand = KtResblockDesc(batch=batch, t=t, channels=spec1.c_in, kernel=spec1.kernel, dilation=spec1.dilation,
-                              pad_left1=spec1.pad_left, pad_left2=spec2.pad_left, slope=spec1.act_in_slope, path=KT_PATH_AUTO)
+                              pad_left1=spec1.pad_left, pad_left2=spec2.pad_left, slope=spec1.act_in_slope,
+                              path=KT_PATH_BF16 if spec1.path == spec2.path == KT_PATH_BF16 else KT_PATH_AUTO)
         if _lib.load().kt_resblock_plan(ctypes.byref(cand)) == 1:
             d = cand
     spec1._rb_cache[key] = d
@@ -666,7 +670,7 @@ class ResblockFn(torch.autograd.Function):
         B, T = x.shape[0], x.shape[1]
         pw1 = prepare_weight(cache1, spec1, v1, g1)
         pw2 = prepare_weight(cache2, spec2, v2, g2)
-        key = ("rb", rd.channels, rd.kernel)
+        key = ("rb", rd.channels, rd.kernel, rd.path)
         img1, img2 = pw1.image(key, rd), pw2.image(key, rd)
         need_grad = any(ctx.needs_input_grad[:7])
         y = torch.empty_like(x)
@@ -680,7 +684,7 @@ class ResblockFn(torch.autograd.Function):
             ctx.nb, ctx.plans, ctx.specs = nb, (p1, p2), (spec1, spec2)
             nt1, nt2 = p1.tile(1), p2.tile(1)
             assert nt1 and nt2, "fused resblock: the data gradients run on the tensor-core kernels"
-            ctx.img_bwd = (pw1.image((1, nt1), p1.d), pw2.image((1, nt2), p2.d))
+            ctx.img_bwd = (pw1.image((1, nt1, p1.d.path), p1.d), pw2.image((1, nt2, p2.d.path), p2.d))
             ctx.norms = (pw1.norm, pw2.norm)
             ctx.params = ((v1, g1, b1), (v2, g2, b2))
             ctx.save_for_backward(x, h, v1, g1, v2, g2)

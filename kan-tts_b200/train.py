@@ -343,14 +343,14 @@ def optimizer_builder(model_params, opt_name, opt_params):
     return getattr(torch.optim, opt_name)(model_params, **opt_params)
 
 
-def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None):
+def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None, precision="bf16x3"):
     """kantts/models/__init__.py:28-86 without the DDP wrappers (GanStep reduces the flat gradient
     buffers itself); scheduler = torch MultiStepLR as in the shipped yamls.  A multi-band generator
     (``out_channels`` > 1) gets ``model["pqmf"]``, a PQMF with that many sub-bands and the yaml's ``pqmf`` kwargs.  ``capturable=True`` builds
     the Adam optimizers so that ``GanStep(cuda_graph=True)`` can capture their step.  ``fused_optimizer`` (default: on a
     CUDA device) asks torch for its single-kernel Adam (``fused=True``: the same update and the same ``state_dict`` as the
     reference's foreach Adam, ~4 launches per model instead of ~12 multi-tensor passes; ablation: the three Adam steps
-    cost 1.4 ms of a 36 ms step)."""
+    cost 1.4 ms of a 36 ms step).  ``precision``: the tensor-core precision of every model (hifigan.set_precision)."""
     if fused_optimizer is None:
         fused_optimizer = torch.device(device).type == "cuda"
     from . import hifigan
@@ -362,6 +362,7 @@ def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None
             m = hifigan.Generator(**sect["params"]).to(device)
         else:
             m = getattr(hifigan, name)(**sect["params"]).to(device)
+        hifigan.set_precision(m, precision)
         oparams = dict(sect["optimizer"].get("params", {}))
         if capturable:
             oparams["capturable"] = True
@@ -378,7 +379,7 @@ def hifigan_model_builder(config, device, capturable=False, fused_optimizer=None
     out_channels = config["Model"]["Generator"]["params"].get("out_channels", 1)
     if out_channels > 1:
         from .pqmf import PQMF
-        model["pqmf"] = PQMF(subbands=out_channels, **config.get("pqmf", {})).to(device)
+        model["pqmf"] = hifigan.set_precision(PQMF(subbands=out_channels, **config.get("pqmf", {})).to(device), precision)
     return model, optimizer, scheduler
 
 
