@@ -379,6 +379,18 @@ int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, con
                          const float* wih0t, const float* whh0t, const float* wih1t, const float* whh1t,
                          const float* bias1, const float* fcw, float fcb, float* out, int32_t batch, int32_t length,
                          int32_t hidden, int32_t p1, int32_t p2, void* stream);
+/* kt_blstm_ragged: inference of a 1-layer bidirectional nn.LSTM (hidden <= 256) over a padded batch of ragged sequences,
+ * both directions in ONE launch (one CTA per (item, direction), one thread per gate): pack_padded_sequence -> nn.LSTM
+ * (bidirectional=True) -> pad_packed_sequence(total_length = length).  lengths: device int32 [batch], never read on the host.
+ *   gx     [batch][length][8 * hidden]: x . [weight_ih_l0; weight_ih_l0_reverse]^T + the two directions' bias_ih + bias_hh
+ *          (one k = 1 conv over the concatenated weights)
+ *   whh_t  [2][hidden][4 * hidden]: weight_hh_l0^T, weight_hh_l0_reverse^T
+ *   h      [batch][length][2 * hidden]: forward | backward outputs.  The forward direction runs rows [0, len_b), the
+ *          backward one starts from zeros at row len_b - 1 and runs down to row 0; rows >= len_b are zero.
+ * An item's rows depend on its own gx rows, its length and the weights only (the same sums in the same order for any batch
+ * or length).  PyTorch gate order (i, f, g, o); exact fp32. */
+int kt_blstm_ragged(const float* gx, const float* whh_t, const int32_t* lengths, float* h, int32_t batch, int32_t length,
+                    int32_t hidden, void* stream);
 
 /* ---- fused ResidualBlock unit (kantts/models/hifigan/layers.py:213-220, one (convs1[i], convs2[i]) pair) ----------
  *   h = conv(leaky_relu(x); w1, dilation d, pad_left1) + b1

@@ -143,6 +143,7 @@ PROTOTYPES = {
     "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _I, _I, _I, _I,
                                  _I, _P],
     "kt_lstm_stream_slots": [_P, _P, _P, _P, ctypes.POINTER(KtStreamMask), _I, _I, _I, _I, _I, _P],
+    "kt_blstm_ragged": [_P, _P, _P, _P, _I, _I, _I, _P],
     "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
     "kt_kaldi_fbank": [_P, _P, _P, _I, _I, _I, _I, _F, _F, _P],

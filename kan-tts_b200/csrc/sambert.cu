@@ -1257,38 +1257,54 @@ extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const KtStreamMa
   return KT_OK;
 }
 
-// lstm_stream_slots_kernel: `rows` steps of a 1-layer unidirectional LSTM, carrying (h, c) of item b in state[b][2][H];
-// with lo from m (stream_utterance_rows), row t of item b is frame t - lo.  A chunk whose first row is frame 0 or earlier
-// (lo >= 0) starts from (h, c) = 0 whatever state holds, a later chunk from the carried state.  A row before frame 0 leaves
-// (h, c) as they are, i.e. zero, and its output row is that zero h; frame 0 therefore starts from zeros.  One CTA per item,
-// one thread per gate: gate j of step t = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced over j),
-// then one thread per hidden unit updates c and h.  PyTorch gate order (i, f, g, o); exact fp32.
-__global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
-                                         float* __restrict__ h_out, const KtStreamMask m, int rows, int H, int gx_pitch,
-                                         int h_pitch) {
+// lstm_rows_kernel: the recurrence of a 1-layer LSTM over `rows` rows of one (item b = blockIdx.x, direction d = blockIdx.y)
+// per CTA, one thread per gate: gate j of a step = gx[t][j] + sum_k W_hh^T[k][j] h[k] (W_hh^T streamed from L2, coalesced
+// over j), then one thread per hidden unit updates c and h.  The CTA runs rows [lo, hi) upwards (d = 0) or downwards (d = 1)
+// and writes zeros to the rows outside them.  Row t of item b, direction d, reads gx at ((b * gx_pitch + t) * D + d) * 4H
+// and writes h at ((b * h_pitch + t) * D + d) * H, D = gridDim.y; W_hh^T of direction d at whh_t + d * H * 4H.
+//   lengths != NULL (kt_blstm_ragged): lo = 0, hi = min(lengths[b], rows), from (h, c) = 0; nothing is carried.
+//   lengths == NULL (kt_lstm_stream_slots, D = 1): with lo from m (stream_utterance_rows), row t is frame t - lo, and hi =
+//   rows.  A chunk whose first row is frame 0 or earlier (lo >= 0) starts from (h, c) = 0 whatever state holds, a later
+//   chunk from the carried state[b][2][H]; the rows before frame 0 are zero and (h, c) after the last row go to state.
+// Each step's sums run in the same order whatever the launch shape, so an item's rows depend on its own gx rows, its
+// length and the weights only.  PyTorch gate order (i, f, g, o); exact fp32.
+__global__ void lstm_rows_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
+                                 float* __restrict__ h_out, const int32_t* __restrict__ lengths, const KtStreamMask m, int rows,
+                                 int H, int gx_pitch, int h_pitch) {
   extern __shared__ float sm[];
-  const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x;
+  const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x, d = blockIdx.y, D = gridDim.y;
   float* h = sm;             // [H]
   float* c = h + H;          // [H]
   float* gates = c + H;      // [4H]
-  float* s = state + (long long)b * 2 * H;
-  int lo, hi;
-  stream_utterance_rows(m, b, lo, hi);
-  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = lo < 0 ? s[j] : 0.f;
-  __syncthreads();
+  whh_t += (long long)d * H * G;
+  int lo = 0, hi, carry = 0;
+  if (lengths) {
+    hi = min(max(__ldg(lengths + b), 0), rows);
+  } else {
+    int uhi;
+    stream_utterance_rows(m, b, lo, uhi);
+    carry = lo < 0;
+    lo = max(lo, 0);
+    hi = rows;
+  }
+  float* s = lengths ? nullptr : state + (long long)b * 2 * H;
+  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = carry ? s[j] : 0.f;
   for (int t = 0; t < rows; ++t) {
-    float* out = h_out + ((long long)b * h_pitch + t) * H;
-    if (t < lo) {
-      for (int j = tid; j < H; j += blockDim.x) out[j] = h[j];
-      continue;                                  // uniform over the CTA: no barrier is skipped by part of it
-    }
-    const float* g = gx + ((long long)b * gx_pitch + t) * G;
+    if (t >= lo && t < hi) continue;
+    float* out = h_out + (((long long)b * h_pitch + t) * D + d) * H;
+    for (int j = tid; j < H; j += blockDim.x) out[j] = 0.f;
+  }
+  __syncthreads();
+  for (int n = 0; n < hi - lo; ++n) {
+    const int t = d ? hi - 1 - n : lo + n;
+    const float* g = gx + (((long long)b * gx_pitch + t) * D + d) * G;
     for (int j = tid; j < G; j += blockDim.x) {
       float acc = __ldg(g + j);
       for (int k = 0; k < H; ++k) acc = fmaf(__ldg(whh_t + (long long)k * G + j), h[k], acc);
       gates[j] = acc;
     }
     __syncthreads();
+    float* out = h_out + (((long long)b * h_pitch + t) * D + d) * H;
     for (int j = tid; j < H; j += blockDim.x) {
       const float ig = sigmoid_f(gates[j]), fg = sigmoid_f(gates[H + j]), gg = tanhf(gates[2 * H + j]), og = sigmoid_f(gates[3 * H + j]);
       const float cn = fg * c[j] + ig * gg;
@@ -1299,21 +1315,33 @@ __global__ void lstm_stream_slots_kernel(const float* __restrict__ gx, const flo
     }
     __syncthreads();
   }
-  for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
+  if (s)
+    for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
+}
+
+static int launch_lstm_rows(const float* gx, const float* whh_t, float* state, float* h, const int32_t* lengths,
+                            const KtStreamMask& m, int B, int dirs, int rows, int H, int gx_pitch, int h_pitch, cudaStream_t st) {
+  const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
+  const size_t smem = (size_t)6 * H * sizeof(float);
+  lstm_rows_kernel<<<dim3(B, dirs), threads, smem, st>>>(gx, whh_t, state, h, lengths, m, rows, H, gx_pitch, h_pitch);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
 }
 
 extern "C" int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* state, float* h, const KtStreamMask* m,
                                     int32_t B, int32_t rows, int32_t H, int32_t gx_pitch, int32_t h_pitch, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = validate_stream_mask(m, "lstm_stream_slots");
   if (rc) return rc;
   KT_REQUIRE(gx && whh_t && state && h, "lstm_stream_slots: null pointer");
   KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream_slots: bad sizes");
-  const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
-  const size_t smem = (size_t)6 * H * sizeof(float);
-  lstm_stream_slots_kernel<<<B, threads, smem, st>>>(gx, whh_t, state, h, *m, rows, H, gx_pitch, h_pitch);
-  KT_CHECK_CUDA(cudaGetLastError());
-  return KT_OK;
+  return launch_lstm_rows(gx, whh_t, state, h, nullptr, *m, B, 1, rows, H, gx_pitch, h_pitch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kt_blstm_ragged(const float* gx, const float* whh_t, const int32_t* lengths, float* h, int32_t B, int32_t L,
+                               int32_t H, void* stream) {
+  KT_REQUIRE(gx && whh_t && lengths && h, "blstm_ragged: null pointer");
+  KT_REQUIRE(B >= 1 && L >= 1 && H >= 1 && H <= 256, "blstm_ragged: bad sizes");
+  return launch_lstm_rows(gx, whh_t, nullptr, h, lengths, KtStreamMask{}, B, 2, L, H, L, L, static_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -262,6 +262,15 @@ def chunk_audio(voc_chunk, samples, chunk, chunk_samples, lookahead=0):
     return (first + lo, lo, hi) if lo < hi else None
 
 
+def pad_requests(inputs):
+    """[(ling (1, L_i, 4), emotion (1, L_i), speaker (1, L_i) or (1, L_i, units), length (1,))] of TtsServer requests -> the
+    (ling, emotion, speaker, lengths) of ONE ``KanTtsSAMBERT`` batch: each request right-padded with zeros to the longest
+    L_i, lengths (k,).  ``front_half(..., per_item=True)`` of the batch gives request i its results alone."""
+    L = max(x[0].shape[1] for x in inputs)
+    pad = lambda t: torch.cat([t, t.new_zeros(1, L - t.shape[1], *t.shape[2:])], 1)
+    return tuple(torch.cat([pad(x[j]) for x in inputs]) for j in range(3)) + (torch.cat([x[3] for x in inputs]),)
+
+
 class TtsServer:
     """Continuous batching of text-to-speech: requests join and leave the ``slots`` slots of one running stream.
 
@@ -273,9 +282,11 @@ class TtsServer:
     Each slot decodes its own utterance (SlotDecoder: its own step, memory length and band), through a per-slot post-net
     streamer into the vocoder streamer.  A request's audio equals ``synthesize`` of that request alone (with its
     ``nsf_seed`` for an NSF generator), whatever the other slots hold.  Admission (at the start of a ``step``, for the queued
-    requests that fit free slots) runs ``front_half`` per request and reads their frame counts on the host; between
-    admissions no call reads device data.  The alignment of each slot is ``slot_schedule``.  ``nsf_f0`` (see
-    ``denorm_f0``) is required for an NSF generator.
+    requests that fit free slots) right-pads the round's requests into one batch (``pad_requests``) and runs ``front_half``
+    ONCE with ``per_item=True``: each request's memory rows, frame count and band are bit for bit those of the request
+    alone, so each slot takes its request's slices.  The round's host reads are that one call's, however many requests it
+    admits; between admissions no call reads device data.  The alignment of each slot is ``slot_schedule``.  ``nsf_f0``
+    (see ``denorm_f0``) is required for an NSF generator.
 
     A non-causal generator is refused unless ``allow_lookahead``: each request's audio then comes ``lookahead`` samples
     later (the vocoder's delay; 0 for a causal one) and equals the generator run on exactly that request's post-net
@@ -338,19 +349,20 @@ class TtsServer:
         if not take:
             return
         with torch.no_grad():
-            fronts = [self.sambert.front_half(*(t.to(self.device) for t in req["inputs"])) for req in take]
-        frames = torch.cat([fr["lr_len"].reshape(-1) for fr in fronts]).tolist()       # the one host read
+            fr = self.sambert.front_half(*(t.to(self.device) for t in pad_requests([req["inputs"] for req in take])),
+                                         per_item=True)
+        frames = fr["lr_len"].tolist()                                                  # the round's one host read
         sched = []
-        for req, fr, n in zip(take, fronts, frames):
+        for req, n in zip(take, frames):
             try:
-                sched.append(slot_schedule(self.r, self.chunk_steps, self.delay, n, fr["memory"].shape[1], c,
+                sched.append(slot_schedule(self.r, self.chunk_steps, self.delay, n, -(-n // self.r), c,
                                            self.max_steps, hop=self.hop, lookahead=self.lookahead))
             except ValueError as e:
                 self._queue.remove(req)
                 raise ValueError(f"request {req['id']}: {e}") from None
         del self._queue[:len(take)]
-        for b, req, fr, n, s in zip(free, take, fronts, frames, sched):
-            self._dec.admit(b, fr["memory"], fr["band_width_rows"])
+        for j, (b, req, n, s) in enumerate(zip(free, take, frames, sched)):
+            self._dec.admit(b, fr["memory"][j:j + 1, :-(-n // self.r)], fr["band_width_rows"][j])
             self._post.reset([b], [n], start_row=s["start_step"] * self.r)
             seed = None if req["seed"] is None else torch.tensor([int(req["seed"])], dtype=torch.int64).to(self.device)
             self._slots[b] = dict(s, chunk=c, id=req["id"], frames=n, samples=n * self.hop, seed=seed)

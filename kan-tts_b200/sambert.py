@@ -13,9 +13,10 @@ Where the arithmetic runs:
     through ops.ConvFn, on the model's native (B, L, C) rows, with bias / ReLU / residual fused;
   * LayerNorm, multi-head attention (both PNCA attentions, probabilities materialised like the reference),
     the FSMN memory block and the LengthRegulator expansion -> the kernels in csrc/sambert.cu;
-  * the four LSTMs stay on cuDNN (``nn.LSTM``) -- SURVEY.md section 2c rules them out of scope for custom
-    kernels -- and the remaining glue (embedding lookups, concatenations, padding masks, sinusoid tables,
-    dropout) is torch elementwise / indexing code, as in the reference.
+  * the four LSTMs stay on cuDNN (``nn.LSTM``) in training -- SURVEY.md section 2c rules them out of scope for custom
+    kernels; inference runs the duration predictor's in kt_ar_duration_infer, the pitch / energy predictors' BiLSTMs in
+    kt_blstm_ragged and the streamed post-net's in kt_lstm_stream_slots -- and the remaining glue (embedding lookups,
+    concatenations, padding masks, sinusoid tables, dropout) is torch elementwise / indexing code, as in the reference.
 The filled-pause variant (``FP: True``, sambert_fp_8k.yaml) is built: FP_Predictor on the same conv / LayerNorm
 kernels, and the splice of the predicted or labelled pauses into the text encoding as an index plan plus one
 gather each way (kt_fp_insert_*).  The alignment-learning variant (``MAS: True``, sambert_16k_MAS*.yaml) is built:
@@ -162,8 +163,13 @@ class PositionwiseConvFeedForward(nn.Module):
         self.dropout_inner = nn.Dropout(dropout_inner)
         self.dropout = nn.Dropout(dropout)
 
-    def forward(self, x, mask=None):
-        h = self.w_1(self.layer_norm(x))
+    def forward(self, x, mask=None, per_item=False):
+        """``per_item``: w_1 reads the LayerNorm of the padding rows as zeros, the zero padding an item has run alone
+        (in a padded batch a padding row's LayerNorm is its bias, which a k > 1 w_1 reads at the item's last rows)."""
+        h = self.layer_norm(x)
+        if per_item and mask is not None:
+            h = h.masked_fill(mask.unsqueeze(-1), 0)
+        h = self.w_1(h)
         if mask is not None:
             h = h.masked_fill(mask.unsqueeze(-1), 0)
         h = self.dropout_inner(h)
@@ -182,11 +188,11 @@ class FFTBlock(nn.Module):
         self.pos_ffn = PositionwiseConvFeedForward(d_model, d_inner, kernel_size, dropout_inner=dropout_relu,
                                                    dropout=dropout)
 
-    def forward(self, input, mask=None, slf_attn_mask=None):
+    def forward(self, input, mask=None, slf_attn_mask=None, per_item=False):
         out, attn = self.slf_attn(input, mask=slf_attn_mask)
         if mask is not None:
             out = out.masked_fill(mask.unsqueeze(-1), 0)
-        out = self.pos_ffn(out, mask=mask)
+        out = self.pos_ffn(out, mask=mask, per_item=per_item)
         if mask is not None:
             out = out.masked_fill(mask.unsqueeze(-1), 0)
         return out, attn
@@ -307,10 +313,12 @@ class SinusoidalPositionEncoder(nn.Module):
         return torch.FloatTensor(table)
 
 
-def _duration_spans(durations, t_out, masks, r):
+def _duration_spans(durations, t_out, masks, r, per_item=False):
     """Shared index arithmetic of LengthRegulator / DurSinusoidalPositionEncoder (adaptors.py:16-25,
     positions.py:77-90): for every output frame the symbol it copies (-1: none) and its 1-based position inside
-    that symbol's span.  Integer glue on (B, L)/(B, T) tensors; no host synchronisation when t_out is given."""
+    that symbol's span.  Integer glue on (B, L)/(B, T) tensors; no host synchronisation when t_out is given.
+    ``per_item``: the frames that pad an item's own frame count up to a multiple of r take position 0, as they do when the
+    item runs alone, instead of the padded batch's t + 1."""
     reps = (durations + 0.5).long()
     cums = torch.cumsum(reps, dim=1)
     total = cums[:, -1:]
@@ -322,6 +330,8 @@ def _duration_spans(durations, t_out, masks, r):
     valid = t < total
     pos = (t - torch.gather(start, 1, idx) + 1).float()
     pos = torch.where(valid, pos, t.float() + 1)        # frames past the last span: offsets == 0 in the reference
+    if per_item:
+        pos = pos.masked_fill((t >= total) & (t < (total + r - 1) // r * r), 0.0)
     if masks is not None:
         valid = valid & ~masks
         pos = pos.masked_fill(masks, 0.0)
@@ -494,7 +504,9 @@ class VarFsmnRnnNARPredictor(nn.Module):
 
     def forward(self, inputs, masks=None):
         x = self.fsmn(inputs, masks)
-        if masks is not None:
+        if not self.training and not torch.is_grad_enabled():
+            x = self.blstm_infer(x, masks)
+        elif masks is not None:
             lengths = torch.sum((~masks).float(), dim=1).long()
             x = nn.utils.rnn.pack_padded_sequence(x, lengths.tolist(), batch_first=True, enforce_sorted=False)
             x, _ = self.blstm(x)
@@ -505,6 +517,47 @@ class VarFsmnRnnNARPredictor(nn.Module):
         if masks is not None:
             x = x.masked_fill(masks, 0.0)
         return x
+
+    def blstm_infer(self, x, masks=None):
+        """The packed BiLSTM of ``forward`` for inference (no autograd): both directions over each item's own rows
+        [0, len_b) in ONE kernel (kt_blstm_ragged), with the lengths taken from ``masks`` on the device (no host read);
+        rows >= len_b are zero.  The input projection of both directions is one k = 1 conv over the concatenated [8H]
+        weights.  An item's rows do not depend on the other items of the batch or on its padding.  Training keeps
+        nn.LSTM (cuDNN)."""
+        lstm, (B, L) = self.blstm, x.shape[:2]
+        H = lstm.hidden_size
+        if not x.is_cuda:
+            raise RuntimeError("kantts_b200: VarFsmnRnnNARPredictor.blstm_infer needs CUDA tensors (no CPU fallback)")
+        with torch.no_grad():
+            spec, pw, w, bias, whh_t = self._blstm_weights()
+            gx = ops.conv(x.contiguous(), spec, pw, w, None, bias)
+            if masks is None:
+                lengths = torch.full((B,), L, device=x.device, dtype=torch.int32)
+            else:
+                lengths = (~masks).sum(1, dtype=torch.int32)
+            h = torch.empty(B, L, 2 * H, device=x.device, dtype=torch.float32)
+            ops.call("kt_blstm_ragged", ptr(gx), ptr(whh_t), ptr(lengths, True), ptr(h), B, L, H)
+        return h
+
+    def _blstm_weights(self):
+        """-> (spec, PreparedWeight, w, bias, whh_t) of blstm_infer: the input projection of both directions as one
+        k = 1 conv (w (8H, C, 1), bias (8H,)) and W_hh^T of both directions (2, H, 4H).  Built once and kept until a
+        parameter of the LSTM changes; w is a Parameter so that its prepared (tensor-core) layouts are kept with it."""
+        lstm = self.blstm
+        params = [lstm.weight_ih_l0, lstm.weight_ih_l0_reverse, lstm.bias_ih_l0, lstm.bias_hh_l0,
+                  lstm.bias_ih_l0_reverse, lstm.bias_hh_l0_reverse, lstm.weight_hh_l0, lstm.weight_hh_l0_reverse]
+        key = tuple((p.data_ptr(), p._version, getattr(p, "_kt_epoch", 0)) for p in params)
+        cache = self.__dict__.get("_blstm_cache")
+        if cache is None or cache[0] != key:
+            H = lstm.hidden_size
+            w = nn.Parameter(torch.cat([lstm.weight_ih_l0, lstm.weight_ih_l0_reverse]).unsqueeze(-1).detach(),
+                             requires_grad=False)
+            bias = torch.cat([lstm.bias_ih_l0 + lstm.bias_hh_l0, lstm.bias_ih_l0_reverse + lstm.bias_hh_l0_reverse])
+            whh_t = torch.stack([lstm.weight_hh_l0.t(), lstm.weight_hh_l0_reverse.t()]).contiguous()
+            spec = ops.ConvSpec(c_in=lstm.input_size, c_out=8 * H, kernel=1)
+            cache = (key, (spec, ops.PreparedWeight(), w, bias.detach(), whh_t.detach()))
+            self.__dict__["_blstm_cache"] = cache
+        return cache[1]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -525,7 +578,7 @@ class SelfAttentionEncoder(nn.Module):
         self.ln = LayerNorm(d_model, eps=1e-6)
         self.position_enc = position_encoder
 
-    def forward(self, input, mask=None, return_attns=False):
+    def forward(self, input, mask=None, return_attns=False, per_item=False):
         input *= self.d_model ** 0.5                      # in place, like kantts_sambert.py:62
         if not isinstance(self.position_enc, SinusoidalPositionEncoder):
             raise NotImplementedError
@@ -534,7 +587,7 @@ class SelfAttentionEncoder(nn.Module):
         attns = []
         for layer in self.fft:
             # the (B, L) key-padding mask is broadcast over the queries inside the kernel
-            x, attn = layer(x, mask=mask, slf_attn_mask=mask)
+            x, attn = layer(x, mask=mask, slf_attn_mask=mask, per_item=per_item)
             if return_attns:
                 attns += [attn]
         return self.ln(x), attns
@@ -637,13 +690,13 @@ class TextFftEncoder(nn.Module):
             config["encoder_relu_dropout"], position_enc)
         self.ling_proj = Linear(d_model, config["encoder_projection_units"], bias=False)
 
-    def forward(self, inputs_ling, masks=None, return_attns=False):
+    def forward(self, inputs_ling, masks=None, return_attns=False, per_item=False):
         if self.using_byte:
             ling_embedding = self.byte_index_emb(inputs_ling[:, :, 0])
         else:
             ling_embedding = (self.sy_emb(inputs_ling[:, :, 0]) + self.tone_emb(inputs_ling[:, :, 1])
                               + self.syllable_flag_emb(inputs_ling[:, :, 2]) + self.ws_emb(inputs_ling[:, :, 3]))
-        enc_output, attns = self.ling_enc(ling_embedding, masks, return_attns)
+        enc_output, attns = self.ling_enc(ling_embedding, masks, return_attns, per_item)
         if hasattr(self, "ling_proj"):
             enc_output = self.ling_proj(enc_output)
         return enc_output, attns, ling_embedding
@@ -669,7 +722,7 @@ class VarianceAdaptor(nn.Module):
         self.energy_emb = RowConv1d(1, d_proj, 9, padding=4)
 
     def forward(self, inputs_text_embedding, inputs_emo_embedding, inputs_spk_embedding, masks=None,
-                output_masks=None, duration_targets=None, pitch_targets=None, energy_targets=None):
+                output_masks=None, duration_targets=None, pitch_targets=None, energy_targets=None, per_item=False):
         batch_size = inputs_text_embedding.size(0)
         var_in = torch.cat([inputs_text_embedding, inputs_spk_embedding, inputs_emo_embedding], dim=-1)
         pitch_predictions = self.pitch_predictor(var_in, masks)
@@ -690,7 +743,7 @@ class VarianceAdaptor(nn.Module):
         # one index computation serves the three expansions and the duration position encoding
         r = self.length_regulator.r
         t_out = None if output_masks is None else output_masks.size(1)
-        idx, start, count, pos, lr_len = _duration_spans(durations, t_out, output_masks, r)
+        idx, start, count, pos, lr_len = _duration_spans(durations, t_out, output_masks, r, per_item)
         lr_text = sops.RowsGatherFn.apply(text_aug, idx, start, count) + self.dur_position_encoder.encode(pos)
         lr_emo = sops.RowsGatherFn.apply(inputs_emo_embedding, idx, start, count)
         lr_spk = sops.RowsGatherFn.apply(inputs_spk_embedding, idx, start, count)
@@ -1097,10 +1150,11 @@ class KanTtsSAMBERT(nn.Module):
             self.FP_predictor = FP_Predictor(config)
         self.fp_dict = None
 
-    def insert_fp(self, text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths):
+    def insert_fp(self, text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths, per_item=False):
         """kantts_sambert.py:766-860: splice the encodings of the filled pauses (labelled, or predicted when
         ``fp_label`` is None) in front of their symbols.  The three pause sequences go through the text encoder as one
-        unmasked batch; the emotion / speaker ids are only extended (row t takes row t mod L)."""
+        unmasked batch; the emotion / speaker ids are only extended (row t takes row t mod L, or with ``per_item`` row t mod
+        the item's own length, as when it runs alone)."""
         if self.fp_dict is None:
             raise RuntimeError("KanTtsSAMBERT(FP=True) needs model.fp_dict = {1: en, 2: a, 3: e} (each a (1, 3, 4) "
                                "long tensor of linguistic ids) before the forward, as the reference model builder sets")
@@ -1109,8 +1163,10 @@ class KanTtsSAMBERT(nn.Module):
         L = text_hid.size(1)
         codes, rows, inter_lengths, t_ins = sops.fp_insert_plan(input_lengths, L, fp_label=fp_label, fp_p=fp_p)
         text_hid = sops.FpInsertFn.apply(text_hid, fp_enc, codes, rows, t_ins)
-        ext = torch.arange(t_ins, device=text_hid.device) % L
-        return text_hid, inputs_emotion[:, ext], inputs_speaker[:, ext], inter_lengths
+        n = input_lengths.clamp_min(1)[:, None] if per_item else L
+        ext = torch.arange(t_ins, device=text_hid.device)[None, :] % n
+        items = torch.arange(text_hid.size(0), device=text_hid.device)[:, None]
+        return text_hid, inputs_emotion[items, ext], inputs_speaker[items, ext], inter_lengths
 
     def get_lfr_mask_from_lengths(self, lengths, max_len):
         """kantts_sambert.py:681-695 without the per-item host loop: ceil(len / r) frames are valid."""
@@ -1142,14 +1198,24 @@ class KanTtsSAMBERT(nn.Module):
 
     def front_half(self, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths=None,
                    mel_targets=None, duration_targets=None, pitch_targets=None, energy_targets=None, fp_label=None,
-                   attn_priors=None):
+                   attn_priors=None, per_item=False):
         """Everything of ``forward`` before the decoder: text encoder, filled-pause insertion (``FP``), alignment search
         (``MAS``, when ``mel_targets`` is given), variance adaptor, the decoder memory and the band width of its attentions.
-        -> dict of the intermediate results ``forward`` and ``infer.stream_synthesize`` continue from."""
+        -> dict of the intermediate results ``forward`` and ``infer.stream_synthesize`` continue from.
+        ``per_item`` (inference): every item gets what it gets run alone, the reference's batch-1 inference, bit for bit on
+        both compute paths: ``memory`` rows [0, ceil(lr_len / r)), ``lr_len``, ``band_width_rows`` and ``log_dur_p`` /
+        ``pitch_p`` / ``energy_p`` on its ``inter_lengths`` rows.  The kernels already give an item's rows independently
+        of the batch (in inference the BiLSTMs run in kt_blstm_ragged); what the flag changes is the rules by which the
+        reference's padded batch differs from one item alone: the k = 3 convs of the encoder's feed-forward blocks and of
+        the ``FP`` predictor read an item's padding rows as zeros (in the padded batch a padding row's LayerNorm is its
+        bias), the frames that pad an item's last decoder step take position code 0 (t + 1 in the padded batch), and with
+        ``FP`` the emotion / speaker rows are extended mod the item's length, not mod the padded length.
+        ``x_band_width``, the batch-max band, is batch-dependent by definition."""
         batch_size = inputs_ling.size(0)
         r = self.mel_decoder.r
         input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
-        text_hid, enc_attns, ling_embedding = self.text_encoder(inputs_ling, input_masks, return_attns=True)
+        text_hid, enc_attns, ling_embedding = self.text_encoder(inputs_ling, input_masks, return_attns=True,
+                                                                per_item=per_item)
         inter_lengths = input_lengths
         mas = {}
         if self.MAS and mel_targets is not None:
@@ -1159,9 +1225,11 @@ class KanTtsSAMBERT(nn.Module):
                                                                mas["energy_targets"])
         fp_p = None
         if self.fp_enable:
-            fp_p = self.FP_predictor(text_hid)
+            # per_item: the predictor's k = 3 w_1 reads zeros past an item's last symbol, as run alone (the encoder's
+            # padding rows are its final LayerNorm bias through ling_proj)
+            fp_p = self.FP_predictor(text_hid.masked_fill(input_masks.unsqueeze(-1), 0) if per_item else text_hid)
             text_hid, inputs_emotion, inputs_speaker, inter_lengths = self.insert_fp(
-                text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths)
+                text_hid, fp_p, fp_label, inputs_emotion, inputs_speaker, input_lengths, per_item)
         emo_hid = self.emo_tokenizer(inputs_emotion)
         spk_hid = inputs_speaker if self.se_enable else self.spk_tokenizer(inputs_speaker)
         inter_masks = get_mask_from_lengths(inter_lengths, max_len=text_hid.size(1))
@@ -1170,7 +1238,7 @@ class KanTtsSAMBERT(nn.Module):
             output_masks = get_mask_from_lengths(output_lengths, max_len=mel_targets.size(1))
         (lr_text, lr_emo, lr_spk, lr_len, log_dur_p, pitch_p, energy_p) = self.variance_adaptor(
             text_hid, emo_hid, spk_hid, masks=inter_masks, output_masks=output_masks,
-            duration_targets=duration_targets, pitch_targets=pitch_targets, energy_targets=energy_targets)
+            duration_targets=duration_targets, pitch_targets=pitch_targets, energy_targets=energy_targets, per_item=per_item)
         if output_lengths is not None:
             lfr_masks = self.get_lfr_mask_from_lengths(output_lengths, max_len=lr_text.size(1))
         else:
