@@ -477,6 +477,21 @@ int kt_stream_reset(const KtWindow* windows, int32_t n, int32_t batch, const uin
 int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t batch, int32_t rows, int32_t ch, int32_t pitch,
                            int32_t first, int32_t frames, void* stream);
 
+/* ---- ragged batches through the whole-utterance forward (Generator.forward(..., lengths=)) ---------------------------------
+ * A whole-utterance mask is a KtStreamMask with frames_done = NULL and lag = 0: item b's rows [0, lengths[b] *
+ * rows_per_frame) of the layer's input are data, and the masked forward reads every later row as zero -- the zero padding the
+ * item meets run alone.  rows_per_frame counts the input tensor's rows (before a nearest-upsampled conv's up-sampling).
+ * kt_conv1d_fwd_masked / kt_conv1d_fwd_tc_masked / kt_resblock_fwd_masked: the forwards above (nsub == 1), same routes, N
+ * tiles, images and workspaces, masked; the fused ResBlock masks both its input and its intermediate.
+ * kt_rows_mask: rows t >= lengths[b] * rows_per_frame of item b of y [batch][rows][ch] are set to zero. */
+int kt_conv1d_fwd_masked(const KtConv1dDesc* d, const KtStreamMask* m, const float* x, const float* w_fwd, const float* bias,
+                         const float* resid, float* y, void* stream);
+int kt_conv1d_fwd_tc_masked(const KtConv1dDesc* d, const KtStreamMask* m, const float* x, const void* wimg, const float* bias,
+                            const float* resid, float* y, float* workspace, int64_t workspace_floats, void* stream);
+int kt_resblock_fwd_masked(const KtResblockDesc* d, const KtStreamMask* m, const float* x, const void* img1, const float* b1,
+                           const void* img2, const float* b2, float* h, float* y, void* stream);
+int kt_rows_mask(const KtStreamMask* m, float* y, int32_t batch, int32_t rows, int32_t ch, void* stream);
+
 /* ---- streaming SAM-BERT post-net (PostNet.streamer: decoder rows in, final post-net rows out, chunk by chunk) ---------------
  * `m` (KtStreamMask, one row per frame) describes a window: chunk row u of item b lies inside its utterance iff lo <= u < hi,
  * lo = lag - frames_done[b] and hi = lo + lengths[b].  So each slot can be anywhere in its own utterance and no chunk reads

@@ -140,6 +140,11 @@ PROTOTYPES = {
     "kt_stream_advance": [_P, _I, _I, _I, _I, _P],
     "kt_stream_reset": [_P, _I, _I, _P, _I, _P],
     "kt_stream_mask_advance": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _I, _I, _I, _P],
+    "kt_conv1d_fwd_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P],
+    "kt_conv1d_fwd_tc_masked": [ctypes.POINTER(KtConv1dDesc), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P, _L, _P],
+    "kt_resblock_fwd_masked": [ctypes.POINTER(KtResblockDesc), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _P, _P, _P,
+                               _P],
+    "kt_rows_mask": [ctypes.POINTER(KtStreamMask), _P, _I, _I, _I, _P],
     "kt_fsmn_fwd_stream_slots": [ctypes.POINTER(KtStreamWin), ctypes.POINTER(KtStreamMask), _P, _P, _P, _P, _I, _I, _I, _I,
                                  _I, _P],
     "kt_lstm_stream_slots": [_P, _P, _P, _P, ctypes.POINTER(KtStreamMask), _I, _I, _I, _I, _I, _P],

@@ -166,9 +166,18 @@ __device__ __forceinline__ void stream_utterance_rows(const KtStreamMask& m, int
   hi = (int)max(-(1LL << 26), min(h, 1LL << 26));
 }
 
+// Whole-utterance masked forwards (kt_conv1d_fwd_masked and friends): item b's input rows [0, the returned bound) are data,
+// the bound being lengths[b] * rows_per_frame clamped into [0, t] (the lengths are device data the host never checks: a
+// negative one means no rows, never a row before the item's first)
+__device__ __forceinline__ int utterance_rows(const KtStreamMask& m, int b, int t) {
+  return (int)max(0LL, min((long long)__ldg(m.lengths + b) * m.rows_per_frame, (long long)t));
+}
+
 // ---- host functions shared between files ----
 // conv_ffma.cu
 int validate_conv(const KtConv1dDesc* d);
+// the KtStreamMask of a whole-utterance masked forward: lengths and rows_per_frame only (no frames_done, lag 0)
+int validate_utterance_mask(const KtStreamMask* m, const char* what);
 // validate_conv plus the window placement of one stream chunk (kt_conv1d_fwd_stream / kt_conv1d_fwd_tc_stream)
 int validate_stream(const KtConv1dDesc* d, const KtStreamWin* w, const float* resid, const char* what);
 // the KtStreamMask of a masked stream call

@@ -55,6 +55,7 @@ __device__ __forceinline__ long long row_index(int bb, int t, int T, int nsub) {
 
 // STREAM: rows are addressed in the windows of KtStreamWin, and input rows down to -in_first are real data
 // MASK (with STREAM): of those, only the rows inside item bb's utterance (KtStreamMask) are; the others read as zeros
+// MASK (without STREAM, kt_conv1d_fwd_masked): input rows [0, lengths[bb] * rows_per_frame) of item bb are data
 template <int RN, int RM, int KC, bool STREAM = false, bool MASK = false>
 __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant__ CoreParams p) {
   constexpr int TN = 32 * RN;
@@ -88,10 +89,12 @@ __global__ void __launch_bounds__(256, 2) conv_core_kernel(const __grid_constant
   const bool vec_in = (p.c_in % 4 == 0) && (p.cin_g % 4 == 0);
   const bool vec_w = (p.c_out % 4 == 0) && (p.cout_g % 4 == 0);
   int in_lo = 0, in_hi = 0;   // MASK: input rows [in_lo, in_hi) of this item are data
-  if constexpr (MASK) {
+  if constexpr (MASK && STREAM) {
     stream_utterance_rows(p.smask, bb, in_lo, in_hi);
     in_lo = max(in_lo, -p.in_first);
     in_hi = min(in_hi, p.t_in);
+  } else if constexpr (MASK) {
+    in_hi = utterance_rows(p.smask, bb, p.t_in);
   }
 
   for (int c0 = 0; c0 < p.cin_g; c0 += KC) {
@@ -584,6 +587,13 @@ int validate_stream_mask(const KtStreamMask* m, const char* what) {
   return KT_OK;
 }
 
+int validate_utterance_mask(const KtStreamMask* m, const char* what) {
+  KT_REQUIRE(m != nullptr && m->lengths != nullptr, "%s: null mask descriptor", what);
+  KT_REQUIRE(m->frames_done == nullptr && m->lag == 0, "%s: a whole-utterance mask has no frames_done and lag 0", what);
+  KT_REQUIRE(m->rows_per_frame > 0, "%s: bad mask (rows_per_frame %d)", what, m->rows_per_frame);
+  return KT_OK;
+}
+
 static void finish_phase(Phase& ph) {
   ph.min_ioff = ph.tap_ioff[0];
   ph.max_ioff = ph.tap_ioff[0];
@@ -674,6 +684,30 @@ extern "C" int kt_conv1d_fwd(const KtConv1dDesc* d, const float* x, const float*
   for (const Phase& ph : conv_phases(d, 0)) {
     p.ph = ph;
     rc = run_core(p, st);
+    if (rc) return rc;
+  }
+  return KT_OK;
+}
+
+// kt_conv1d_fwd with item b's input rows at or past lengths[b] * rows_per_frame read as zeros (its zero padding alone)
+extern "C" int kt_conv1d_fwd_masked(const KtConv1dDesc* d, const KtStreamMask* m, const float* x, const float* w_fwd,
+                                    const float* bias, const float* resid, float* y, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_conv(d);
+  if (!rc) rc = validate_utterance_mask(m, "kt_conv1d_fwd_masked");
+  if (rc) return rc;
+  KT_REQUIRE(x && w_fwd && y, "kt_conv1d_fwd_masked: null pointer");
+  KT_REQUIRE(d->nsub == 1, "kt_conv1d_fwd_masked: masked forwards need nsub == 1");
+  CoreParams p{};
+  p.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
+  p.w = w_fwd; p.bias = bias; p.resid = resid; p.mask = Side{nullptr, nullptr, 0, 0.f}; p.out = y;
+  p.batch = d->batch; p.nsub = 1; p.t_in = d->t_in; p.t_out = d->t_out;
+  p.c_in = d->c_in; p.c_out = d->c_out; p.groups = d->groups; p.cin_g = d->c_in / d->groups; p.cout_g = d->c_out / d->groups;
+  p.out_act = d->act_out; p.out_slope = d->act_out_slope;
+  p.smask = *m;
+  for (const Phase& ph : conv_phases(d, 0)) {
+    p.ph = ph;
+    rc = run_core<false, true>(p, st);
     if (rc) return rc;
   }
   return KT_OK;

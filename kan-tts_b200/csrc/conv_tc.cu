@@ -184,7 +184,9 @@ enum TcRoute { kTcRegSimple = 0, kTcReg = 1, kTcTma = 2 };
 // weight pipelines run continuously ACROSS tiles, so staging of tile i+1 overlaps the MMAs and the epilogue of tile i.
 // STREAM (register-staged routes only): one chunk of a stream -- rows live in the windows of KtStreamWin, and the input
 // rows before the chunk (down to -in_first) are real data instead of zero padding.  MASK (with STREAM): of those, only the
-// rows inside item bb's utterance (KtStreamMask) are, bounded per tile by the row map's t_lo / t_lim.  PL: bf16 planes per
+// rows inside item bb's utterance (KtStreamMask) are, bounded per tile by the row map's t_lo / t_lim.  MASK without STREAM
+// (kt_conv1d_fwd_tc_masked, one item per tile): item bb's input rows [0, lengths[bb] * rows_per_frame) are data, the row
+// map's t_lim.  PL: bf16 planes per
 // operand (2: bf16x3, three wgmma per K = 16 slice; 1: single-pass bf16, one): conv_tc_kernel / conv_tc_bf16_kernel.
 template <int ROUTE, bool STREAM, bool MASK, int PL>
 __device__ __forceinline__ void conv_tc_body(const TcParams& p, const TcTmaMaps& maps) {
@@ -236,12 +238,14 @@ __device__ __forceinline__ void conv_tc_body(const TcParams& p, const TcTmaMaps&
       const int ch_base = p.grouped ? ((tile / mtiles) % p.ntiles) * p.kg : 0;
       const int f0 = (gm - p.ph_mt0[ph]) * kTcM;
       int t_lo = 0, t_lim = 0;   // MASK: the item's utterance rows, in the row map's (up-sampled) units
-      if constexpr (MASK) {
+      if constexpr (MASK && STREAM) {
         stream_utterance_rows(p.smask, bb, t_lo, t_lim);
         // both bounds clamped into the window's rows [-in_first, t_in] before they are scaled: the products stay in int
         // for every up-sampling factor whose up-sampled window does
         t_lo = min(max(t_lo, -p.in_first), p.t_in) * p.up;
         t_lim = max(min(t_lim, p.t_in), -p.in_first) * p.up;
+      } else if constexpr (MASK) {
+        t_lim = utterance_rows(p.smask, bb, p.t_in) * p.up;   // one item per tile: the masked plan never packs
       }
       for (int c = 0; c < p.kchunks; ++c) {
         for (int g = p.ph_g0[ph]; g < p.ph_g0[ph + 1]; ++g, ra.advance(p.na_stages)) {
@@ -881,6 +885,8 @@ static int launch_route(const TcParams& p, const TcTmaMaps& maps, bool tma, bool
   const bool simple = p.nsub == 1 && p.up == 1 && (p.kg & 7) == 0 && (p.c_in & 3) == 0 && (p.c_out & 3) == 0 &&
                       (p.n_stride & 3) == 0 && p.out_act != KT_ACT_TANH && !p.accumulate &&
                       (p.in.mode < SIDE_DLRELU || p.in.aux != nullptr) && !(p.resid && p.mask.p);
+  if (masked && !stream && simple) return launch_tc<kTcRegSimple, false, true, PL>(p, maps, grid, smem, st);
+  if (masked && !stream) return launch_tc<kTcReg, false, true, PL>(p, maps, grid, smem, st);
   if (masked && simple) return launch_tc<kTcRegSimple, true, true, PL>(p, maps, grid, smem, st);
   if (masked) return launch_tc<kTcReg, true, true, PL>(p, maps, grid, smem, st);
   if (stream && simple) return launch_tc<kTcRegSimple, true, false, PL>(p, maps, grid, smem, st);
@@ -902,8 +908,31 @@ static int run_tc(TcParams p, const TcTmaMaps& maps, bool tma, bool stream, bool
   return KT_OK;
 }
 
+// split_planes_kernel of one operand [batch][t][c] (nsub == 1, c % 8 == 0) for a whole-utterance masked forward: item b's rows
+// at or past lengths[b] * rows_per_frame are written as zeros, so the TMA route's images need no mask of their own.  The
+// other rows get split_planes_kernel's bits.
+template <int PL>
+__global__ void split_planes_masked_kernel(Side s, long long n8, __nv_bfloat16* __restrict__ hi, const __grid_constant__ KtStreamMask m,
+                                           int t, int c) {
+  __nv_bfloat16* lo = hi + n8 * 8;
+  const int c8 = c / 8;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / c8;
+    const int b = (int)(row / t), tr = (int)(row - (long long)b * t);
+    float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (tr < utterance_rows(m, b, t)) {
+      const float4 v0 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i), v1 = __ldg(reinterpret_cast<const float4*>(s.p) + 2 * i + 1);
+      x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
+      if (s.mode == SIDE_LRELU)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : x[e] * s.slope;
+    }
+    store_planes8<PL>(x, reinterpret_cast<uint8_t*>(hi), reinterpret_cast<uint8_t*>(lo), (size_t)i * 16);
+  }
+}
+
 // Every launch of plan P with the operands of `io` (in, wimg, bias, resid, mask, out, out_act, out_slope).  The TMA route
-// first writes the gathered operand's planes into ws.
+// first writes the gathered operand's planes into ws (masked per item when io.smask is a whole-utterance mask).
 static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws_floats, const char* what, cudaStream_t st) {
   TcTmaMaps maps{};
   __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(ws);
@@ -913,8 +942,15 @@ static int run_plan(const TcPlan& P, const TcParams& io, float* ws, long long ws
       return KT_ERR_WORKSPACE;
     }
     const TcParams& g = P.launches[0];
-    KT_CHECK_CUDA(split_planes(io.in, (long long)g.batch * g.t_in * g.nsub * g.c_in, planes, Side{nullptr, nullptr, 0, 0.f}, 0,
-                               nullptr, g.planes, st));
+    const long long n = (long long)g.batch * g.t_in * g.nsub * g.c_in;
+    if (io.smask.lengths != nullptr) {   // (stream chunks never take the TMA route)
+      const int blocks = (int)std::max<long long>(1, std::min<long long>((n / 8 + 255) / 256, 132LL * 16));
+      if (g.planes == 1) split_planes_masked_kernel<1><<<blocks, 256, 0, st>>>(io.in, n / 8, planes, io.smask, g.t_in, g.c_in);
+      else split_planes_masked_kernel<2><<<blocks, 256, 0, st>>>(io.in, n / 8, planes, io.smask, g.t_in, g.c_in);
+      KT_CHECK_CUDA(cudaGetLastError());
+    } else {
+      KT_CHECK_CUDA(split_planes(io.in, n, planes, Side{nullptr, nullptr, 0, 0.f}, 0, nullptr, g.planes, st));
+    }
   }
   for (TcParams lp : P.launches) {
     lp.in = io.in; lp.wimg = io.wimg; lp.bias = io.bias; lp.resid = io.resid; lp.mask = io.mask; lp.out = io.out;
@@ -951,6 +987,27 @@ extern "C" int kt_conv1d_fwd_tc(const KtConv1dDesc* d, const float* x, const voi
   io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
   io.out_act = d->act_out; io.out_slope = d->act_out_slope;
   return run_plan(P, io, ws, ws_floats, "conv1d_fwd_tc", static_cast<cudaStream_t>(stream));
+}
+
+// kt_conv1d_fwd_tc with item b's input rows at or past lengths[b] * rows_per_frame read as zeros: the same route, N tile and
+// workspace as the unmasked call, except that the register-staged route keeps one item per tile (the bound is per tile)
+extern "C" int kt_conv1d_fwd_tc_masked(const KtConv1dDesc* d, const KtStreamMask* m, const float* x, const void* wimg,
+                                       const float* bias, const float* resid, float* y, float* ws, int64_t ws_floats,
+                                       void* stream) {
+  int rc = validate_conv(d);
+  if (!rc) rc = validate_utterance_mask(m, "kt_conv1d_fwd_tc_masked");
+  if (rc) return rc;
+  KT_REQUIRE(x && wimg && y, "kt_conv1d_fwd_tc_masked: null pointer");
+  KT_REQUIRE(d->nsub == 1, "kt_conv1d_fwd_tc_masked: masked forwards need nsub == 1");
+  const TcPlan P = make_tc_plan(d, 0, true, false, false);
+  KT_REQUIRE(P.ok, "kt_conv1d_fwd_tc_masked: layer not supported by the tensor-core path");
+  TcParams io{};
+  io.in = make_side(x, nullptr, d->act_in, d->act_in_slope, false);
+  io.wimg = reinterpret_cast<const __nv_bfloat16*>(wimg);
+  io.bias = bias; io.resid = resid; io.mask = Side{nullptr, nullptr, 0, 0.f}; io.out = y;
+  io.out_act = d->act_out; io.out_slope = d->act_out_slope;
+  io.smask = *m;
+  return run_plan(P, io, ws, ws_floats, "kt_conv1d_fwd_tc_masked", static_cast<cudaStream_t>(stream));
 }
 
 // One chunk of a stream (KtStreamWin): the register-staged route over the windows; m: the input's utterance bounds (masked

@@ -353,6 +353,25 @@ extern "C" int kt_stream_mask_advance(const KtStreamMask* m, float* y, int32_t b
   return KT_OK;
 }
 
+// rows t >= lengths[b] * rows_per_frame of item b of y [batch][rows][ch] -> 0; grid (blocks per item, batch)
+__global__ void rows_mask_kernel(const KtStreamMask m, float* __restrict__ y, int rows, int ch) {
+  const int b = blockIdx.y;
+  const long long first = (long long)utterance_rows(m, b, rows) * ch, end = (long long)rows * ch;
+  float* base = y + (long long)b * end;
+  for (long long i = first + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (long long)gridDim.x * blockDim.x)
+    base[i] = 0.f;
+}
+
+extern "C" int kt_rows_mask(const KtStreamMask* m, float* y, int32_t batch, int32_t rows, int32_t ch, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = validate_utterance_mask(m, "kt_rows_mask");
+  if (rc) return rc;
+  KT_REQUIRE(y && batch > 0 && batch <= 65535 && rows > 0 && ch > 0, "kt_rows_mask: bad arguments");
+  rows_mask_kernel<<<dim3((unsigned)std::min<long long>(((long long)rows * ch + 255) / 256, 64), batch), 256, 0, st>>>(*m, y, rows, ch);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
+}
+
 extern "C" int kt_dwt_db3_fwd(const float* x, float* y, int32_t batch, int32_t t, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   KT_REQUIRE(x && y && batch > 0 && t > 0, "dwt_fwd: bad arguments");

@@ -62,6 +62,13 @@ struct RbParams {
   alignas(64) CUtensorMap tmx;      // 3-D map of x: (C, T, B), box (32, rows_box, 1), no swizzle, zero OOB fill
 };
 
+// Parameters of the masked instances (kt_resblock_fwd_masked): RbParams and each item's utterance rows.  A struct of its own,
+// so that the unmasked instances keep their parameter block.
+struct RbMaskedParams {
+  RbParams p;
+  KtStreamMask smask;
+};
+
 // ---- weight packing for the paired (C = 32) layout: tile p = taps (2p, 2p + 1) along K -----------------------------
 // w: kernel layout [k][ci][co] (kt_weight_prepare's w_fwd).  Tile p: NT = 32 rows n = co, k index c: c < 32 -> tap 2p,
 // ci = c; c >= 32 -> tap 2p + 1, ci = c - 32 (zero when 2p + 1 == k).  [hi tile | lo tile] (PL = 1: hi), SWIZZLE_128B rows.
@@ -100,6 +107,25 @@ __device__ __forceinline__ void rb_convert_tile(uint8_t* img_hi, uint8_t* img_lo
   }
 }
 
+// rb_convert_tile of the masked instances: source rows of the tile at or past lim_r (the item's utterance end, in
+// landing-stage rows) convert as zeros
+template <bool PAIR, int PL>
+__device__ __forceinline__ void rb_convert_tile_masked(uint8_t* img_hi, uint8_t* img_lo, const float* ft, int box_floats, int d,
+                                                       float slope, int r_begin, int r_end, int tid, int lim_r) {
+  const int q = tid & 7;
+  const float* base = PAIR ? ft + (q >> 2) * d * 32 + (q & 3) * 8 : ft + (q >> 2) * box_floats + (q & 3) * 8;
+  if (PAIR) lim_r -= (q >> 2) * d;   // the second half of a paired row holds source row r + d
+#pragma unroll 2
+  for (int r = r_begin + (tid >> 3); r < r_end; r += 16) {
+    const float4 a = *reinterpret_cast<const float4*>(base + r * 32);
+    const float4 b = *reinterpret_cast<const float4*>(base + r * 32 + 4);
+    float e[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int z = 0; z < 8; ++z) e[z] = r >= lim_r ? 0.f : (e[z] > 0.f ? e[z] : e[z] * slope);
+    store_planes8<PL>(e, img_hi, img_lo, sw128_offset((uint32_t)r, (uint32_t)q));
+  }
+}
+
 // Warp roles (416 threads): warpgroup 0 produces the x images, warpgroups 1 / 2 are the consumers (each: the 64-row half
 // of both convs' wgmma and of both epilogues), warp 12 streams weights (bulk async copies).  (Warps hold registers in
 // groups of four: 13 warps keep the 128 registers per thread the consumers' accumulators need.)
@@ -111,9 +137,10 @@ constexpr int kRbConsumerBar = 1;        // named barrier of the 256 consumer th
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync %0, 256;" ::"n"(kRbConsumerBar) : "memory"); }
 
 // NT = C (32 or 64): the MMA width is a compile-time constant of each instance; PL: bf16 planes (2 bf16x3: resblock_tc_kernel,
-// 1 single-pass: resblock_tc_bf16_kernel)
-template <int NT, int PL>
-__device__ __forceinline__ void resblock_tc_body(const RbParams& p) {
+// 1 single-pass: resblock_tc_bf16_kernel).  MASK (resblock_tc[_bf16]_masked_kernel): item bb's rows at or past
+// lengths[bb] * rows_per_frame read as zeros, both in the x tile (c1's input) and in the H image (c2's input)
+template <int NT, int PL, bool MASK = false>
+__device__ __forceinline__ void resblock_tc_body(const RbParams& p, const KtStreamMask& smask) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   const int ximg = p.rows_x * 128, himg = p.rows_h * 128;            // one plane
@@ -173,8 +200,16 @@ __device__ __forceinline__ void resblock_tc_body(const RbParams& p) {
       mbar_wait(&f_full[s], rx.phase());
       uint8_t* img_hi = x_base + (size_t)s * PL * ximg;
       const float* ft = reinterpret_cast<const float*>(f_base + (size_t)s * p.fstage_bytes);
-      if (p.pair) rb_convert_tile<true, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
-      else rb_convert_tile<false, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+      if constexpr (MASK) {
+        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+        const int bb = tile / p.tiles_per_item, it = tile - bb * p.tiles_per_item;
+        const int lim_r = utterance_rows(smask, bb, p.t) - (it * p.to - p.p2 - p.p1);   // landing-stage row of the item's end
+        if (p.pair) rb_convert_tile_masked<true, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid, lim_r);
+        else rb_convert_tile_masked<false, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid, lim_r);
+      } else {
+        if (p.pair) rb_convert_tile<true, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+        else rb_convert_tile<false, PL>(img_hi, img_hi + ximg, ft, box_floats, p.d1, p.slope, r0, r1, ptid);
+      }
       fence_proxy_async();
       mbar_arrive(&x_full[s]);
       asm volatile("bar.sync 2, 128;" ::: "memory");          // every producer thread has read the landing stage
@@ -287,7 +322,8 @@ __device__ __forceinline__ void resblock_tc_body(const RbParams& p) {
       for (int hh = 0; hh < 2; ++hh) {
         const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
         const int t = h0 + r;
-        const bool in_range = t >= 0 && t < p.t;                       // else: c2's zero padding
+        // else: c2's zero padding (masked: also the rows past the item's end)
+        const bool in_range = t >= 0 && t < (MASK ? utterance_rows(smask, bb, p.t) : p.t);
 #pragma unroll
         for (int i = 0; i < kWgmmaMaxRegs / 4; ++i) {
           if (i * 8 >= NT) continue;
@@ -336,9 +372,21 @@ __device__ __forceinline__ void resblock_tc_body(const RbParams& p) {
 }
 
 template <int NT>
-__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) { resblock_tc_body<NT, 2>(p); }
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_kernel(const __grid_constant__ RbParams p) {
+  resblock_tc_body<NT, 2>(p, KtStreamMask{});
+}
 template <int NT>
-__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_bf16_kernel(const __grid_constant__ RbParams p) { resblock_tc_body<NT, 1>(p); }
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_bf16_kernel(const __grid_constant__ RbParams p) {
+  resblock_tc_body<NT, 1>(p, KtStreamMask{});
+}
+template <int NT>
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_masked_kernel(const __grid_constant__ RbMaskedParams mp) {
+  resblock_tc_body<NT, 2, true>(mp.p, mp.smask);
+}
+template <int NT>
+__global__ void __launch_bounds__(kRbThreads, 1) resblock_tc_bf16_masked_kernel(const __grid_constant__ RbMaskedParams mp) {
+  resblock_tc_body<NT, 1, true>(mp.p, mp.smask);
+}
 
 // ---------------------------------------------------------------------------------------------
 // host
@@ -440,9 +488,19 @@ static int launch_resblock(const RbParams& p, int grid, size_t smem, cudaStream_
   return KT_OK;
 }
 
-extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
-                               const float* b2, float* h, float* y, void* stream) {
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+template <int PL>
+static int launch_resblock_masked(const RbMaskedParams& mp, int grid, size_t smem, cudaStream_t st) {
+  constexpr auto k32 = PL == 1 ? resblock_tc_bf16_masked_kernel<32> : resblock_tc_masked_kernel<32>;
+  constexpr auto k64 = PL == 1 ? resblock_tc_bf16_masked_kernel<64> : resblock_tc_masked_kernel<64>;
+  KT_CHECK_CUDA(allow_dyn_smem<k32>(kMaxDynSmem));
+  KT_CHECK_CUDA(allow_dyn_smem<k64>(kMaxDynSmem));
+  if (mp.p.c == 32) k32<<<grid, kRbThreads, smem, st>>>(mp);
+  else k64<<<grid, kRbThreads, smem, st>>>(mp);
+  return KT_OK;
+}
+
+static int resblock_fwd(const KtResblockDesc* d, const KtStreamMask* m, const float* x, const void* img1, const float* b1,
+                        const void* img2, const float* b2, float* h, float* y, cudaStream_t st) {
   KT_REQUIRE(d, "kt_resblock_fwd: null descriptor");
   RbPlan pl = rb_plan(d);
   KT_REQUIRE(pl.ok, "resblock_fwd: shape not supported by the fused kernel (see kt_resblock_plan)");
@@ -458,10 +516,31 @@ extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const vo
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "resblock_fwd");
   if (rc) return rc;
   const int grid = std::min(p.total_tiles, device_sm_count());
-  const int rc2 = p.planes == 1 ? launch_resblock<1>(p, grid, pl.smem, st) : launch_resblock<2>(p, grid, pl.smem, st);
+  int rc2;
+  if (m) {
+    RbMaskedParams mp{};
+    mp.p = p;
+    mp.smask = *m;
+    rc2 = p.planes == 1 ? launch_resblock_masked<1>(mp, grid, pl.smem, st) : launch_resblock_masked<2>(mp, grid, pl.smem, st);
+  } else {
+    rc2 = p.planes == 1 ? launch_resblock<1>(p, grid, pl.smem, st) : launch_resblock<2>(p, grid, pl.smem, st);
+  }
   if (rc2) return rc2;
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
+}
+
+extern "C" int kt_resblock_fwd(const KtResblockDesc* d, const float* x, const void* img1, const float* b1, const void* img2,
+                               const float* b2, float* h, float* y, void* stream) {
+  return resblock_fwd(d, nullptr, x, img1, b1, img2, b2, h, y, static_cast<cudaStream_t>(stream));
+}
+
+// kt_resblock_fwd with item b's rows at or past lengths[b] * rows_per_frame read as zeros by both convs
+extern "C" int kt_resblock_fwd_masked(const KtResblockDesc* d, const KtStreamMask* m, const float* x, const void* img1,
+                                      const float* b1, const void* img2, const float* b2, float* h, float* y, void* stream) {
+  const int rc = validate_utterance_mask(m, "kt_resblock_fwd_masked");
+  if (rc) return rc;
+  return resblock_fwd(d, m, x, img1, b1, img2, b2, h, y, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int kt_resblock_bwd(const KtConv1dDesc* d1, const KtConv1dDesc* d2, const float* x, const float* h, const float* dy,

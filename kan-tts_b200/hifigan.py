@@ -245,10 +245,10 @@ class _NormedConv(nn.Module):
             return w / sigma, None
         return self.weight, None
 
-    def run(self, x, resid=None):
+    def run(self, x, resid=None, mask=None):
         v, g = self.effective_weight()
-        if self.norm == "spectral":      # sigma changes with every forward: never part of pair_reuse
-            return ops.conv(x, self.spec, self._cache, v, g, self.bias, resid)
+        if self.norm == "spectral" or mask is not None:    # sigma changes with every forward: never part of pair_reuse
+            return ops.conv(x, self.spec, self._cache, v, g, self.bias, resid, mask=mask)
         return ops.pair_conv(self, x, self.spec, self._cache, v, g, self.bias, resid)
 
     def remove_weight_norm(self):
@@ -286,8 +286,8 @@ class Conv1d(nn.Module):
             spec.act_in, spec.act_in_slope = KT_ACT_LRELU, float(act_in)
         self.conv1d = _NormedConv(ref, spec, "weight", init_weights=True)
 
-    def forward_rows(self, x, resid=None):
-        return self.conv1d.run(x, resid)
+    def forward_rows(self, x, resid=None, mask=None):
+        return self.conv1d.run(x, resid, mask)
 
     def forward(self, x):
         """(B, C, T) -> (B, C', T'); the reference signature."""
@@ -319,8 +319,8 @@ class ConvTranspose1d(nn.Module):
         self.stride = stride
         self.pad = kernel_size - stride
 
-    def forward_rows(self, x, resid=None):
-        return self.deconv.run(x, resid)
+    def forward_rows(self, x, resid=None, mask=None):
+        return self.deconv.run(x, resid, mask)
 
     def forward(self, x):
         return self.forward_rows(x.transpose(1, 2).contiguous()).transpose(1, 2)
@@ -354,7 +354,9 @@ class ResidualBlock(nn.Module):
                      act_in=slope) for i in range(len(dilation))])
         self.activation = getattr(nn, nonlinear_activation)(**nonlinear_activation_params)
 
-    def forward_rows(self, x):
+    def forward_rows(self, x, mask=None):
+        """``mask`` (ops.utterance_mask of x's rows): each item's rows past its utterance read as zeros in both convs of every
+        pair (c2 reads the intermediate under the same mask: it has x's rows)."""
         for c1, c2 in zip(self.convs1, self.convs2):
             n1, n2 = c1.conv1d, c2.conv1d
             rd = ops.resblock_desc(n1.spec, n2.spec, x.shape[0], x.shape[1]) \
@@ -363,10 +365,10 @@ class ResidualBlock(nn.Module):
                 # thin stages (32 / 64 channels): the pair is ONE launch, the intermediate stays on the SM (kt_resblock_fwd)
                 v1, g1 = n1.effective_weight()
                 v2, g2 = n2.effective_weight()
-                x = ops.resblock(x, n1.spec, n1._cache, v1, g1, n1.bias, n2.spec, n2._cache, v2, g2, n2.bias, rd)
+                x = ops.resblock(x, n1.spec, n1._cache, v1, g1, n1.bias, n2.spec, n2._cache, v2, g2, n2.bias, rd, mask)
             else:
-                xt = c1.forward_rows(x)
-                x = c2.forward_rows(xt, resid=x)
+                xt = c1.forward_rows(x, mask=mask)
+                x = c2.forward_rows(xt, resid=x, mask=mask)
         return x
 
     def forward(self, x):
@@ -556,14 +558,23 @@ class Generator(nn.Module):
                 else:
                     self.source_downs.append(conv_cls(1, channels // (2 ** (i + 1)), u * 2, u, padding=u // 2))
 
-    def forward_rows(self, x, excitation=None):
-        x = self.conv_pre.forward_rows(x)
+    def forward_rows(self, x, excitation=None, lengths=None):
+        """``lengths`` (device int32 (B,), see ``forward``): every conv reads item b's input rows at or past lengths[b] times
+        the input's rows per frame as zeros, and the output rows past lengths[b] * hop are zeroed.  The element-wise steps
+        (SinAddFn, Mean3Fn, the fused residual adds) run unmasked: only a masked conv reads their rows past an item's end."""
+        mask = (lambda rate: None) if lengths is None else (lambda rate: ops.utterance_mask(lengths, rate))
+        rate = 1                                                             # x's rows per mel frame
+        x = self.conv_pre.forward_rows(x, mask=mask(rate))
+        hop = int(np.prod(self.upsample_scales))
         for i in range(self.num_upsamples):
             x = ops.SinAddFn.apply(x)                                        # hifigan.py:157
-            rep = self.repeat_upsamples[i][2].forward_rows(x)                # :158
+            m = mask(rate)
+            rep = self.repeat_upsamples[i][2].forward_rows(x, mask=m)        # :158
             if excitation is not None:                                       # :162-166  x = rep + e + up (adds fused)
-                rep = self.source_downs[i].forward_rows(excitation, resid=rep)
-            x = self.transpose_upsamples[i][1].forward_rows(x, resid=rep)    # :160,168 (crop fused: t_out)
+                rep = self.source_downs[i].forward_rows(excitation, resid=rep, mask=mask(hop))
+            x = self.transpose_upsamples[i][1].forward_rows(x, resid=rep, mask=m)    # :160,168 (crop fused: t_out)
+            rate *= int(self.upsample_scales[i])
+            m = mask(rate)
             par = x.is_cuda and _PARALLEL_STREAMS and self.num_kernels > 1
             if par:                                                           # the parallel resblocks are independent
                 cur = torch.cuda.current_stream()
@@ -572,27 +583,39 @@ class Generator(nn.Module):
                 for j in range(self.num_kernels):
                     streams[j].wait_stream(cur)
                     with torch.cuda.stream(streams[j]):
-                        rs.append(self.conv_blocks[i * self.num_kernels + j].forward_rows(x))
+                        rs.append(self.conv_blocks[i * self.num_kernels + j].forward_rows(x, m))
                 for s in streams[: self.num_kernels]:
                     cur.wait_stream(s)
             else:
-                rs = [self.conv_blocks[i * self.num_kernels + j].forward_rows(x) for j in range(self.num_kernels)]
+                rs = [self.conv_blocks[i * self.num_kernels + j].forward_rows(x, m) for j in range(self.num_kernels)]
             rs += [None] * (3 - len(rs))
             x = ops.Mean3Fn.apply(1.0 / self.num_kernels, *rs)               # :170-176
-        return self.conv_post.forward_rows(x)                                # :178-180
+        y = self.conv_post.forward_rows(x, mask=mask(hop))                   # :178-180
+        return y if lengths is None else ops.rows_mask(y, mask(hop))
 
-    def forward(self, x, nsf_seeds=None):
+    def forward(self, x, nsf_seeds=None, lengths=None):
         """x: (B, in_channels, T) -> (B, out_channels, T * prod(scales)); with ``nsf_params`` the last two channels are the
         pitch (Hz) and the voiced flag (hifigan.py:146-150).  ``nsf_seeds`` (NSF only; one per batch item, host sequence
         or device int64 tensor): the excitation is the seeded kt_nsf_excitation instead of the reference's random draw, so
-        that the output is a function of (x, seeds) -- the one a streamer with the same seeds computes."""
+        that the output is a function of (x, seeds) -- the one a streamer with the same seeds computes.
+        ``lengths`` (inference only: eval() mode, no autograd): each item's mel frames, a host sequence or a device int
+        tensor (B,), 1 <= lengths[b] <= T (a device tensor's values are not read on the host).  Item b's output samples
+        [0, lengths[b] * prod(scales)) are then ``self(x[b:b+1, :, :lengths[b]])`` (an NSF generator needs ``nsf_seeds``:
+        the same seed) and its later samples are zero."""
         if nsf_seeds is not None and not self.nsf_enable:
             raise ValueError("nsf_seeds: this generator has no NSF source module")
+        if lengths is not None:
+            if self.training:
+                raise RuntimeError("Generator.forward(lengths=...) is inference only: call eval() first")
+            if self.nsf_enable and nsf_seeds is None:
+                raise ValueError("Generator.forward(lengths=...): an NSF generator needs nsf_seeds for each item's excitation "
+                                 "to be its own")
+            lengths = ops.ragged_lengths(lengths, x.shape[0], x.shape[2], x.device)
         excitation = None
         if self.nsf_enable:
             x, pitch, uv = x[:, :-2, :], x[:, -2:-1, :], x[:, -1:, :]
             excitation = self.source_module.forward_rows(pitch, uv, nsf_seeds)   # (B, samples, 1)
-        y = self.forward_rows(x.transpose(1, 2).contiguous(), excitation)   # (B, T', 1)
+        y = self.forward_rows(x.transpose(1, 2).contiguous(), excitation, lengths)   # (B, T', 1)
         return y.transpose(1, 2)
 
     def streamer(self, batch, max_frames, lengths=None, seeds=None):

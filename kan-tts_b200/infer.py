@@ -94,12 +94,17 @@ def _check_stream(sambert, generator, chunk_steps, nsf_f0, nsf_seeds, allow_look
 
 
 @torch.no_grad()
-def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None):
+def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, input_lengths, nsf_f0=None, nsf_seeds=None,
+               per_item=False):
     """sambert: ``KanTtsSAMBERT`` in eval(); generator: ``Generator`` in eval() (``remove_weight_norm()`` optional --
     the prepared weights are cached either way).  A multi-band generator (``out_channels`` > 1) needs its PQMF attached as
     ``generator.pqmf`` (as infer_hifigan.py:47-53 does after loading), whose synthesis makes the waveform.  Tensors as in
     ``KanTtsSAMBERT.forward`` (inference branch).
     ``nsf_f0`` / ``nsf_seeds`` (both or neither): the NSF hand-off, see the module docstring and ``denorm_f0``.
+    ``per_item``: the vocoder runs the padded batch with each utterance's ``LR_length_rounded`` frames as its lengths
+    (Generator.forward(lengths=), PQMF.synthesis(lengths=)), so each waveform is the generator (and PQMF) on exactly its own
+    post-net frames -- the reference's and TtsServer's hand-off.  Without it the vocoder runs the padded batch as is, which
+    changes a shorter utterance's last samples when the generator is non-causal or multi-band.
     -> (list of 1-D waveform tensors, dict of the acoustic-model results)."""
     if sambert.training or generator.training:
         raise RuntimeError("synthesize() expects both models in eval() mode")
@@ -110,12 +115,16 @@ def synthesize(sambert, generator, inputs_ling, inputs_emotion, inputs_speaker, 
     res = sambert(inputs_ling, inputs_emotion, inputs_speaker, input_lengths)
     mel = res["postnet_outputs"]                                   # (B, T, num_mels), zero beyond each length
     frames = res["LR_length_rounded"]
+    # per_item: the frame counts as host ints (read here anyway to cut the waveforms), so the generator checks each one
+    # against the post-net's rows
+    lengths = [int(n) for n in frames.tolist()] if per_item else None
     if nsf:
-        wav = generator(denorm_f0(mel, nsf_f0).transpose(1, 2).contiguous(), nsf_seeds=nsf_seeds)
+        wav = generator(denorm_f0(mel, nsf_f0).transpose(1, 2).contiguous(), nsf_seeds=nsf_seeds, lengths=lengths)
     else:
-        wav = generator(mel.transpose(1, 2).contiguous())          # (B, out_channels, T * prod(scales))
+        wav = generator(mel.transpose(1, 2).contiguous(), lengths=lengths)   # (B, out_channels, T * prod(scales))
     if pqmf is not None:
-        wav = pqmf.synthesis(wav)                                  # (B, 1, T * hop)
+        scale = int(np.prod(generator.upsample_scales))
+        wav = pqmf.synthesis(wav, None if lengths is None else [n * scale for n in lengths])   # (B, 1, T * hop)
     hop = int(np.prod(generator.upsample_scales)) * generator.out_channels
     wavs = [wav[b, 0, : int(frames[b]) * hop] for b in range(wav.shape[0])]
     return wavs, res

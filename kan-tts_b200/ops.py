@@ -13,7 +13,7 @@ import torch
 from . import _lib
 from ._lib import (KT_ACT_LRELU, KT_ACT_NONE, KT_ACT_TANH, KT_PATH_AUTO, KT_PATH_BF16, KT_PATH_FFMA, KT_PATH_TC, KT_PLAN_STREAM,
                    KtConv1dDesc,
-                   KtMelDesc, KtResblockDesc, check, ptr, stream_ptr)
+                   KtMelDesc, KtResblockDesc, KtStreamMask, check, ptr, stream_ptr)
 
 _launches = 0          # kernels-launched counter (bench.py reports it as gpu_launches)
 
@@ -475,11 +475,52 @@ def _workspace(floats, device):
     return torch.empty(floats, device=device, dtype=torch.float32) if floats else None
 
 
+def ragged_lengths(lengths, n, t, device):
+    """-> ``lengths`` (each item's rows: a host sequence of ints, or a device integer tensor (n,)) as a contiguous device
+    int32 tensor (n,).  ValueError on a wrong count, dtype or device, or a host value outside [1, t]."""
+    if torch.is_tensor(lengths):
+        if lengths.dtype not in (torch.int32, torch.int64) or lengths.dim() != 1 or lengths.numel() != n:
+            raise ValueError(f"lengths: expected an int32 / int64 tensor of shape ({n},), got {lengths.dtype} "
+                             f"{tuple(lengths.shape)}")
+        if lengths.device != device:
+            raise ValueError(f"lengths: expected a tensor on {device}, got {lengths.device}")
+        return lengths.to(torch.int32).contiguous()
+    vals = [int(v) for v in lengths]
+    if len(vals) != n:
+        raise ValueError(f"lengths: expected {n} values (one per batch item), got {len(vals)}")
+    bad = [v for v in vals if not 1 <= v <= t]
+    if bad:
+        raise ValueError(f"lengths: every value must lie in [1, {t}], got {bad}")
+    return torch.tensor(vals, dtype=torch.int32).to(device)
+
+
+def utterance_mask(lengths, rows_per_frame):
+    """-> the whole-utterance KtStreamMask of a ragged batch: item b's input rows [0, lengths[b] * rows_per_frame) are data,
+    later rows read as zeros (kt_conv1d_fwd_masked).  ``lengths``: device int32 (B,), kept alive by the caller."""
+    return KtStreamMask(ptr(lengths, True), None, int(rows_per_frame), 0)
+
+
+def _refuse_masked_grad(what, *tensors):
+    """A masked forward has no backward: refuse it where autograd would record it (an autograd.Function's forward always runs
+    without grad mode, so the check belongs to the caller)."""
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+        raise RuntimeError(f"kantts_b200: a masked {what} forward is inference only (run it under torch.no_grad())")
+
+
+def rows_mask(y, mask):
+    """Zero rows t >= lengths[b] * rows_per_frame of each item b of the (B, T, C) rows ``y``, in place (kt_rows_mask)."""
+    call("kt_rows_mask", ctypes.byref(mask), ptr(y), y.shape[0], y.shape[1], y.shape[2])
+    return y
+
+
 class ConvFn(torch.autograd.Function):
-    """y = act_out(conv(act_in(x)) + bias) + resid   on channels-last rows."""
+    """y = act_out(conv(act_in(x)) + bias) + resid   on channels-last rows.  ``mask`` (utterance_mask, inference only):
+    each item's input rows past its utterance read as zeros."""
 
     @staticmethod
-    def forward(ctx, x, resid, bias, v, g, spec, cache, reuse=None):
+    def forward(ctx, x, resid, bias, v, g, spec, cache, reuse=None, mask=None):
+        if mask is not None:
+            assert reuse is None and x.dim() == 3, "a masked conv runs whole batches of (B, T, C) rows"
         x = x.contiguous()
         nsub = x.shape[2] if x.dim() == 4 else 1
         B, t_in = x.shape[0], x.shape[1]
@@ -502,15 +543,21 @@ class ConvFn(torch.autograd.Function):
             assert resid.shape == y.shape, (resid.shape, y.shape)
         bd = None if bias is None else bias.detach()
         d, nt, n = run.d, run.tile(0), (spec.stride if spec.transposed else 1)
+        # the masked calls take the unmasked call's route, N tile, image and workspace (kt_conv1d_fwd_tc_masked), so the plan
+        # and image caches need no key on the mask
+        m = () if mask is None else (ctypes.byref(mask),)
         if nt:
             img = pw.image((0, nt, d.path), d)
             ws = _workspace(run.ws_fwd, x.device)
-            _run("conv_fwd_tc", spec, d, n + (ws is not None), n, ("kt_conv1d_fwd_tc", ctypes.byref(d), ptr(x), ptr(img, True),
-                                                                   ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd))
+            _run("conv_fwd_tc", spec, d, n + (ws is not None), n,
+                 ("kt_conv1d_fwd_tc_masked" if m else "kt_conv1d_fwd_tc", ctypes.byref(d), *m, ptr(x), ptr(img, True),
+                  ptr(bd), ptr(resid), ptr(y), ptr(ws), run.ws_fwd))
         else:
-            _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd", ctypes.byref(d), ptr(x), ptr(pw.w_fwd), ptr(bd),
-                                                  ptr(resid), ptr(y)))
+            _run("conv_fwd_ffma", spec, d, n, 0, ("kt_conv1d_fwd_masked" if m else "kt_conv1d_fwd", ctypes.byref(d), *m, ptr(x),
+                                                  ptr(pw.w_fwd), ptr(bd), ptr(resid), ptr(y)))
         pw.conv_used = True
+        if mask is not None:
+            return y
         nb = B if _grad_items is None else min(_grad_items, B)     # batch items that carry gradient
         ctx.spec, ctx.nb = spec, nb
         ctx.plan = full if nb == B else spec.plan(nb, nsub, t_in)
@@ -567,11 +614,13 @@ class ConvFn(torch.autograd.Function):
             dres = dy_full.clone()
         dbias, dv, dg = _weight_backward(spec, plan, x_, dy, y_, v, g, ctx.params, ctx.norm, ctx.needs_input_grad[3],
                                          ctx.has_g and ctx.needs_input_grad[4], ctx.has_bias and ctx.needs_input_grad[2])
-        return dx, dres, dbias, dv, dg, None, None, None
+        return dx, dres, dbias, dv, dg, None, None, None, None
 
 
-def conv(x, spec, cache, v, g=None, bias=None, resid=None, reuse=None):
-    return ConvFn.apply(x, resid, bias, v, g, spec, cache, reuse)
+def conv(x, spec, cache, v, g=None, bias=None, resid=None, reuse=None, mask=None):
+    if mask is not None:
+        _refuse_masked_grad("conv", x, v, g, bias, resid)
+    return ConvFn.apply(x, resid, bias, v, g, spec, cache, reuse, mask)
 
 
 def stream_conv(spec, pw, bias, x, y, t_in, win, resid=None, mask=None):
@@ -665,7 +714,7 @@ class ResblockFn(torch.autograd.Function):
     gradients) + the two convs' weight-gradient chains, from the saved (x, h)."""
 
     @staticmethod
-    def forward(ctx, x, b1, v1, g1, b2, v2, g2, spec1, cache1, spec2, cache2, rd):
+    def forward(ctx, x, b1, v1, g1, b2, v2, g2, spec1, cache1, spec2, cache2, rd, mask=None):
         x = x.contiguous()
         B, T = x.shape[0], x.shape[1]
         pw1 = prepare_weight(cache1, spec1, v1, g1)
@@ -675,9 +724,11 @@ class ResblockFn(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad[:7])
         y = torch.empty_like(x)
         h = torch.empty_like(x) if need_grad else None
+        m = () if mask is None else (ctypes.byref(mask),)
         _run("resblock_fwd_tc", spec1, spec1.plan(B, 1, T).d, 1, 1,
-             ("kt_resblock_fwd", ctypes.byref(rd), ptr(x), ptr(img1, True), ptr(None if b1 is None else b1.detach()),
-              ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h), ptr(y)))
+             ("kt_resblock_fwd_masked" if m else "kt_resblock_fwd", ctypes.byref(rd), *m, ptr(x), ptr(img1, True),
+              ptr(None if b1 is None else b1.detach()), ptr(img2, True), ptr(None if b2 is None else b2.detach()), ptr(h),
+              ptr(y)))
         if need_grad:
             nb = B if _grad_items is None else min(_grad_items, B)
             p1, p2 = spec1.plan(nb, 1, T), spec2.plan(nb, 1, T)
@@ -712,11 +763,13 @@ class ResblockFn(torch.autograd.Function):
                                          g2 is not None and ni[6], pb2 is not None and ni[4])
         db1, dv1, dg1 = _weight_backward(spec1, p1, x_, dh, None, v1, g1, (pv1, pg1, pb1), ctx.norms[0], ni[2],
                                          g1 is not None and ni[3], pb1 is not None and ni[1])
-        return (dx if ni[0] else None), db1, dv1, dg1, db2, dv2, dg2, None, None, None, None, None
+        return (dx if ni[0] else None), db1, dv1, dg1, db2, dv2, dg2, None, None, None, None, None, None
 
 
-def resblock(x, spec1, cache1, v1, g1, b1, spec2, cache2, v2, g2, b2, rd):
-    return ResblockFn.apply(x, b1, v1, g1, b2, v2, g2, spec1, cache1, spec2, cache2, rd)
+def resblock(x, spec1, cache1, v1, g1, b1, spec2, cache2, v2, g2, b2, rd, mask=None):
+    if mask is not None:
+        _refuse_masked_grad("resblock", x, v1, g1, b1, v2, g2, b2)
+    return ResblockFn.apply(x, b1, v1, g1, b2, v2, g2, spec1, cache1, spec2, cache2, rd, mask)
 
 
 class SinAddFn(torch.autograd.Function):

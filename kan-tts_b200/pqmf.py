@@ -83,10 +83,18 @@ class PQMF(nn.Module):
         rows = x.reshape(x.shape[0], x.shape[2], 1)                    # (B, T, 1): the same memory
         return ops.conv(rows, self.analysis_spec, self._caches[0], wa).transpose(1, 2)
 
-    def synthesis(self, x):
-        """(B, subbands, n) -> (B, 1, subbands * n)"""
+    def synthesis(self, x, lengths=None):
+        """(B, subbands, n) -> (B, 1, subbands * n).  ``lengths`` (inference only): each item's sub-band samples, a host
+        sequence or a device int tensor (B,), 1 <= lengths[b] <= n; item b's output samples [0, subbands * lengths[b]) are
+        then ``synthesis(x[b:b+1, :, :lengths[b]])`` and its later samples are zero."""
         if x.dim() != 3 or x.shape[1] != self.subbands:
             raise ValueError(f"PQMF.synthesis expects (B, {self.subbands}, n), got {tuple(x.shape)}")
         _, ws = self._weights()
-        y = ops.conv(x.transpose(1, 2).contiguous(), self.synthesis_spec, self._caches[1], ws)   # (B, S * n, 1)
+        rows = x.transpose(1, 2).contiguous()
+        if lengths is None:
+            y = ops.conv(rows, self.synthesis_spec, self._caches[1], ws)   # (B, S * n, 1)
+        else:
+            lengths = ops.ragged_lengths(lengths, x.shape[0], x.shape[2], x.device)
+            y = ops.conv(rows, self.synthesis_spec, self._caches[1], ws, mask=ops.utterance_mask(lengths, 1))
+            ops.rows_mask(y, ops.utterance_mask(lengths, self.subbands))
         return y.reshape(y.shape[0], 1, y.shape[1])
