@@ -391,6 +391,30 @@ int kt_ar_duration_infer(const float* g0c, const float* w1, const float* b1, con
  * or length).  PyTorch gate order (i, f, g, o); exact fp32. */
 int kt_blstm_ragged(const float* gx, const float* whh_t, const int32_t* lengths, float* h, int32_t batch, int32_t length,
                     int32_t hidden, void* stream);
+/* kt_lstm_train_fwd / kt_lstm_train_bwd: one layer of a uni- (dirs = 1) or bidirectional (dirs = 2) nn.LSTM (hidden <= 256)
+ * in training, one CTA per (item, direction).  lengths: device int32 [batch] or NULL.  With lengths, the packed semantics
+ * of pack_padded_sequence: the forward direction runs rows [0, len_b), the backward one from row len_b - 1 down to row 0,
+ * both from zeros, and rows >= len_b of h are zero.  Without, every row runs (nn.LSTM over the padded rows).
+ *   gx      [batch][length][dirs * 4 * hidden]: x . weight_ih^T + bias_ih + bias_hh of each direction (one k = 1 conv)
+ *   whh_t   [dirs][hidden][4 * hidden]: weight_hh^T of each direction (forward)
+ *   whh     [dirs][4 * hidden][hidden]: weight_hh of each direction (backward)
+ *   init    [batch][dirs][2][hidden] or NULL: the initial h then c of each (item, direction), zeros when NULL
+ *   h       [batch][length][dirs * hidden]: the output;  c [batch][length][dirs * hidden]: the cell states, zero on rows >=
+ *           len_b (optional in the forward);  acts [batch][length][dirs * 4 * hidden]: the gate activations sigmoid(i), sigmoid(f), tanh(g),
+ *           sigmoid(o) (optional in the forward).  The backward reads the h, c and acts of a forward with the same lengths.
+ *   dh, dc  [batch][length][dirs * hidden]: the gradients of h and c (dc may be NULL: zero)
+ *   dgates  [batch][length][dirs * 4 * hidden]: the gradient of gx (zero on rows >= len_b)
+ *   h_prev  [batch][length][dirs * hidden]: each row's recurrent input (h of the row before it in its direction's order, zero
+ *           at the direction's first row (init's h when given) and on rows >= len_b): dW_hh = sum over rows of
+ *           dgates^T h_prev, per direction.
+ *   dstate  init's layout or NULL: the gradient of the initial (h, c).
+ * Both recurrences are exact fp32 with a fixed summation order: an item's rows depend on its own rows, its length and the
+ * weights only.  PyTorch gate order (i, f, g, o). */
+int kt_lstm_train_fwd(const float* gx, const float* whh_t, const int32_t* lengths, const float* init, float* h, float* c,
+                      float* acts, int32_t batch, int32_t length, int32_t dirs, int32_t hidden, void* stream);
+int kt_lstm_train_bwd(const float* dh, const float* dc, const float* whh, const int32_t* lengths, const float* init,
+                      const float* h, const float* c, const float* acts, float* dgates, float* h_prev, float* dstate,
+                      int32_t batch, int32_t length, int32_t dirs, int32_t hidden, void* stream);
 
 /* ---- fused ResidualBlock unit (kantts/models/hifigan/layers.py:213-220, one (convs1[i], convs2[i]) pair) ----------
  *   h = conv(leaky_relu(x); w1, dilation d, pad_left1) + b1

@@ -149,6 +149,8 @@ PROTOTYPES = {
                                  _I, _P],
     "kt_lstm_stream_slots": [_P, _P, _P, _P, ctypes.POINTER(KtStreamMask), _I, _I, _I, _I, _I, _P],
     "kt_blstm_ragged": [_P, _P, _P, _P, _I, _I, _I, _P],
+    "kt_lstm_train_fwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "kt_lstm_train_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_pnca_step_slots": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "kt_nsf_excitation": [_P, _I, _I, ctypes.POINTER(KtNsfState), _P, _I, _I, _I, _I, _I, _I, _I, _F, _F, _P],
     "kt_kaldi_fbank": [_P, _P, _P, _I, _I, _I, _I, _F, _F, _P],

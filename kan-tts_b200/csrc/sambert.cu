@@ -1262,49 +1262,59 @@ extern "C" int kt_fsmn_fwd_stream_slots(const KtStreamWin* win, const KtStreamMa
 // over j), then one thread per hidden unit updates c and h.  The CTA runs rows [lo, hi) upwards (d = 0) or downwards (d = 1)
 // and writes zeros to the rows outside them.  Row t of item b, direction d, reads gx at ((b * gx_pitch + t) * D + d) * 4H
 // and writes h at ((b * h_pitch + t) * D + d) * H, D = gridDim.y; W_hh^T of direction d at whh_t + d * H * 4H.
-//   lengths != NULL (kt_blstm_ragged): lo = 0, hi = min(lengths[b], rows), from (h, c) = 0; nothing is carried.
-//   lengths == NULL (kt_lstm_stream_slots, D = 1): with lo from m (stream_utterance_rows), row t is frame t - lo, and hi =
+//   lengths != NULL (kt_blstm_ragged, kt_lstm_train_fwd): lo = 0, hi = min(lengths[b], rows), from (h, c) = 0.
+//   m.lengths != NULL (kt_lstm_stream_slots, D = 1): with lo from m (stream_utterance_rows), row t is frame t - lo, and hi =
 //   rows.  A chunk whose first row is frame 0 or earlier (lo >= 0) starts from (h, c) = 0 whatever state holds, a later
 //   chunk from the carried state[b][2][H]; the rows before frame 0 are zero and (h, c) after the last row go to state.
+//   neither (kt_lstm_train_fwd without lengths): every row, from (h, c) = 0.
+// init (kt_lstm_train_fwd, optional): the initial (h, c) of each (item, direction) at init[((b * D + d) * 2) * H], h then c,
+// in place of zeros.  c_out / act_out (training, optional): the cell state c at h's offsets (zero outside [lo, hi), as h)
+// and the gate activations (sigmoid i, f, tanh g, sigmoid o) at gx's, for kt_lstm_train_bwd (not written outside [lo, hi)).
 // Each step's sums run in the same order whatever the launch shape, so an item's rows depend on its own gx rows, its
 // length and the weights only.  PyTorch gate order (i, f, g, o); exact fp32.
 __global__ void lstm_rows_kernel(const float* __restrict__ gx, const float* __restrict__ whh_t, float* __restrict__ state,
-                                 float* __restrict__ h_out, const int32_t* __restrict__ lengths, const KtStreamMask m, int rows,
-                                 int H, int gx_pitch, int h_pitch) {
+                                 const float* __restrict__ init, float* __restrict__ h_out, float* __restrict__ c_out,
+                                 float* __restrict__ act_out, const int32_t* __restrict__ lengths, const KtStreamMask m,
+                                 int rows, int H, int gx_pitch, int h_pitch) {
   extern __shared__ float sm[];
   const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x, d = blockIdx.y, D = gridDim.y;
   float* h = sm;             // [H]
   float* c = h + H;          // [H]
   float* gates = c + H;      // [4H]
   whh_t += (long long)d * H * G;
-  int lo = 0, hi, carry = 0;
+  int lo = 0, hi = rows, carry = 0;
   if (lengths) {
     hi = min(max(__ldg(lengths + b), 0), rows);
-  } else {
+  } else if (m.lengths) {
     int uhi;
     stream_utterance_rows(m, b, lo, uhi);
     carry = lo < 0;
     lo = max(lo, 0);
-    hi = rows;
   }
-  float* s = lengths ? nullptr : state + (long long)b * 2 * H;
-  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = carry ? s[j] : 0.f;
+  float* s = state ? state + (long long)b * 2 * H : nullptr;
+  const float* i0 = init ? init + ((long long)b * D + d) * 2 * H : nullptr;
+  for (int j = tid; j < 2 * H; j += blockDim.x) sm[j] = carry ? s[j] : (i0 ? __ldg(i0 + j) : 0.f);
   for (int t = 0; t < rows; ++t) {
     if (t >= lo && t < hi) continue;
-    float* out = h_out + (((long long)b * h_pitch + t) * D + d) * H;
-    for (int j = tid; j < H; j += blockDim.x) out[j] = 0.f;
+    const long long orow = ((long long)b * h_pitch + t) * D + d;
+    for (int j = tid; j < H; j += blockDim.x) {
+      h_out[orow * H + j] = 0.f;
+      if (c_out) c_out[orow * H + j] = 0.f;
+    }
   }
   __syncthreads();
   for (int n = 0; n < hi - lo; ++n) {
     const int t = d ? hi - 1 - n : lo + n;
-    const float* g = gx + (((long long)b * gx_pitch + t) * D + d) * G;
+    const long long row = ((long long)b * gx_pitch + t) * D + d;
+    const float* g = gx + row * G;
     for (int j = tid; j < G; j += blockDim.x) {
       float acc = __ldg(g + j);
       for (int k = 0; k < H; ++k) acc = fmaf(__ldg(whh_t + (long long)k * G + j), h[k], acc);
       gates[j] = acc;
     }
     __syncthreads();
-    float* out = h_out + (((long long)b * h_pitch + t) * D + d) * H;
+    const long long orow = ((long long)b * h_pitch + t) * D + d;
+    float* out = h_out + orow * H;
     for (int j = tid; j < H; j += blockDim.x) {
       const float ig = sigmoid_f(gates[j]), fg = sigmoid_f(gates[H + j]), gg = tanhf(gates[2 * H + j]), og = sigmoid_f(gates[3 * H + j]);
       const float cn = fg * c[j] + ig * gg;
@@ -1312,6 +1322,14 @@ __global__ void lstm_rows_kernel(const float* __restrict__ gx, const float* __re
       c[j] = cn;
       h[j] = hn;
       out[j] = hn;
+      if (c_out) c_out[orow * H + j] = cn;
+      if (act_out) {
+        float* a = act_out + row * G;
+        a[j] = ig;
+        a[H + j] = fg;
+        a[2 * H + j] = gg;
+        a[3 * H + j] = og;
+      }
     }
     __syncthreads();
   }
@@ -1319,11 +1337,13 @@ __global__ void lstm_rows_kernel(const float* __restrict__ gx, const float* __re
     for (int j = tid; j < 2 * H; j += blockDim.x) s[j] = sm[j];
 }
 
-static int launch_lstm_rows(const float* gx, const float* whh_t, float* state, float* h, const int32_t* lengths,
-                            const KtStreamMask& m, int B, int dirs, int rows, int H, int gx_pitch, int h_pitch, cudaStream_t st) {
+static int launch_lstm_rows(const float* gx, const float* whh_t, float* state, const float* init, float* h, float* c,
+                            float* acts, const int32_t* lengths, const KtStreamMask& m, int B, int dirs, int rows, int H,
+                            int gx_pitch, int h_pitch, cudaStream_t st) {
   const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
   const size_t smem = (size_t)6 * H * sizeof(float);
-  lstm_rows_kernel<<<dim3(B, dirs), threads, smem, st>>>(gx, whh_t, state, h, lengths, m, rows, H, gx_pitch, h_pitch);
+  lstm_rows_kernel<<<dim3(B, dirs), threads, smem, st>>>(gx, whh_t, state, init, h, c, acts, lengths, m, rows, H,
+                                                         gx_pitch, h_pitch);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;
 }
@@ -1334,14 +1354,115 @@ extern "C" int kt_lstm_stream_slots(const float* gx, const float* whh_t, float* 
   if (rc) return rc;
   KT_REQUIRE(gx && whh_t && state && h, "lstm_stream_slots: null pointer");
   KT_REQUIRE(B >= 1 && rows >= 1 && H >= 1 && H <= 256 && gx_pitch >= rows && h_pitch >= rows, "lstm_stream_slots: bad sizes");
-  return launch_lstm_rows(gx, whh_t, state, h, nullptr, *m, B, 1, rows, H, gx_pitch, h_pitch, static_cast<cudaStream_t>(stream));
+  return launch_lstm_rows(gx, whh_t, state, nullptr, h, nullptr, nullptr, nullptr, *m, B, 1, rows, H, gx_pitch, h_pitch,
+                          static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int kt_blstm_ragged(const float* gx, const float* whh_t, const int32_t* lengths, float* h, int32_t B, int32_t L,
                                int32_t H, void* stream) {
   KT_REQUIRE(gx && whh_t && lengths && h, "blstm_ragged: null pointer");
   KT_REQUIRE(B >= 1 && L >= 1 && H >= 1 && H <= 256, "blstm_ragged: bad sizes");
-  return launch_lstm_rows(gx, whh_t, nullptr, h, lengths, KtStreamMask{}, B, 2, L, H, L, L, static_cast<cudaStream_t>(stream));
+  return launch_lstm_rows(gx, whh_t, nullptr, nullptr, h, nullptr, nullptr, lengths, KtStreamMask{}, B, 2, L, H, L, L,
+                          static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kt_lstm_train_fwd(const float* gx, const float* whh_t, const int32_t* lengths, const float* init, float* h,
+                                 float* c, float* acts, int32_t B, int32_t L, int32_t dirs, int32_t H, void* stream) {
+  KT_REQUIRE(gx && whh_t && h, "lstm_train_fwd: null pointer");
+  KT_REQUIRE(B >= 1 && L >= 1 && (dirs == 1 || dirs == 2) && H >= 1 && H <= 256,
+             "lstm_train_fwd: bad sizes (batch %d, length %d, dirs %d, hidden %d)", B, L, dirs, H);
+  return launch_lstm_rows(gx, whh_t, nullptr, init, h, c, acts, lengths, KtStreamMask{}, B, dirs, L, H, L, L,
+                          static_cast<cudaStream_t>(stream));
+}
+
+// lstm_bwd_kernel: the backward recurrence of lstm_rows_kernel for one (item b = blockIdx.x, direction d = blockIdx.y), over
+// the same rows [lo, hi) in the reverse of their forward order.  With t' the row before t in the forward order ((h, c) =
+// init, or 0, there at the direction's first row), from the upstream dh[t] and dc[t] (dc optional) and the carried
+// (dh_rec, dc_rec) of the row after:
+//   dh = dh[t] + dh_rec;  dc = (dc_rec + dc[t]) + dh * o * (1 - tanh(c_t)^2)
+//   dgates[t] = (dc * g * i (1 - i), dc * c_t' * f (1 - f), dc * i * (1 - g^2), dh * tanh(c_t) * o (1 - o))
+//   dc_rec = dc * f;  dh_rec[k] = sum_j dgates[t][j] W_hh[j][k]
+// The last sum runs as four partial sums over the gate blocks (one thread per (block, k), W_hh streamed from L2, coalesced
+// over k), added in block order: a fixed order, so an item's rows depend on its own rows, its length and the weights only.
+// Rows outside [lo, hi) get dgates = 0.  h_prev[t] = h[t'] (init's h, or 0, at the direction's first row; 0 outside [lo, hi)):
+// the operand of the weight gradient dW_hh = sum_t dgates[t]^T h_prev[t].  dstate (optional, init's layout): the gradient
+// of the initial (h, c), the (dh_rec, dc_rec) left after the direction's first row.
+__global__ void lstm_bwd_kernel(const float* __restrict__ dh_out, const float* __restrict__ dc_out,
+                                const float* __restrict__ whh, const int32_t* __restrict__ lengths,
+                                const float* __restrict__ init, const float* __restrict__ h_in, const float* __restrict__ c_in,
+                                const float* __restrict__ acts, float* __restrict__ dgates, float* __restrict__ h_prev,
+                                float* __restrict__ dstate, int rows, int H) {
+  extern __shared__ float sm[];
+  const int G = 4 * H, tid = threadIdx.x, b = blockIdx.x, d = blockIdx.y, D = gridDim.y;
+  float* dc = sm;            // [H]  dc_rec
+  float* dg = dc + H;        // [4H] this row's gate gradients
+  float* part = dg + G;      // [4H] partial sums of dh_rec, one H block per gate block
+  whh += (long long)d * G * H;
+  const int hi = lengths ? min(max(__ldg(lengths + b), 0), rows) : rows;
+  const long long sbase = ((long long)b * D + d) * 2 * H;
+  const float* i0 = init ? init + sbase : nullptr;
+  for (int j = tid; j < H; j += blockDim.x) dc[j] = 0.f;
+  for (int j = tid; j < G; j += blockDim.x) part[j] = 0.f;
+  for (int t = hi; t < rows; ++t) {
+    const long long row = ((long long)b * rows + t) * D + d;
+    for (int j = tid; j < G; j += blockDim.x) dgates[row * G + j] = 0.f;
+    for (int j = tid; j < H; j += blockDim.x) h_prev[row * H + j] = 0.f;
+  }
+  __syncthreads();
+  for (int n = 0; n < hi; ++n) {
+    const int t = d ? n : hi - 1 - n;
+    const int tp = d ? t + 1 : t - 1;
+    const bool first = d ? tp >= hi : tp < 0;
+    const long long row = ((long long)b * rows + t) * D + d, prow = ((long long)b * rows + tp) * D + d;
+    const float* a = acts + row * G;
+    for (int j = tid; j < H; j += blockDim.x) {
+      const float dh = __ldg(dh_out + row * H + j) + (((part[j] + part[H + j]) + part[2 * H + j]) + part[3 * H + j]);
+      const float ig = __ldg(a + j), fg = __ldg(a + H + j), gg = __ldg(a + 2 * H + j), og = __ldg(a + 3 * H + j);
+      const float tc = tanhf(__ldg(c_in + row * H + j));
+      const float cp = first ? (i0 ? __ldg(i0 + H + j) : 0.f) : __ldg(c_in + prow * H + j);
+      const float dcn = fmaf(dh * og, 1.f - tc * tc, dc_out ? dc[j] + __ldg(dc_out + row * H + j) : dc[j]);
+      const float gi = dcn * gg * (ig * (1.f - ig)), gf = dcn * cp * (fg * (1.f - fg));
+      const float gc = dcn * ig * (1.f - gg * gg), go = dh * tc * (og * (1.f - og));
+      dc[j] = dcn * fg;
+      dg[j] = gi;
+      dg[H + j] = gf;
+      dg[2 * H + j] = gc;
+      dg[3 * H + j] = go;
+      float* o = dgates + row * G;
+      o[j] = gi;
+      o[H + j] = gf;
+      o[2 * H + j] = gc;
+      o[3 * H + j] = go;
+      h_prev[row * H + j] = first ? (i0 ? __ldg(i0 + j) : 0.f) : __ldg(h_in + prow * H + j);
+    }
+    __syncthreads();
+    for (int e = tid; e < G; e += blockDim.x) {
+      const int q = e / H, k = e - q * H;
+      float acc = 0.f;
+      for (int j = q * H; j < (q + 1) * H; ++j) acc = fmaf(__ldg(whh + (long long)j * H + k), dg[j], acc);
+      part[e] = acc;
+    }
+    __syncthreads();
+  }
+  if (dstate)
+    for (int j = tid; j < H; j += blockDim.x) {
+      dstate[sbase + j] = ((part[j] + part[H + j]) + part[2 * H + j]) + part[3 * H + j];
+      dstate[sbase + H + j] = dc[j];
+    }
+}
+
+extern "C" int kt_lstm_train_bwd(const float* dh, const float* dc, const float* whh, const int32_t* lengths,
+                                 const float* init, const float* h, const float* c, const float* acts, float* dgates,
+                                 float* h_prev, float* dstate, int32_t B, int32_t L, int32_t dirs, int32_t H, void* stream) {
+  KT_REQUIRE(dh && whh && h && c && acts && dgates && h_prev, "lstm_train_bwd: null pointer");
+  KT_REQUIRE(B >= 1 && L >= 1 && (dirs == 1 || dirs == 2) && H >= 1 && H <= 256,
+             "lstm_train_bwd: bad sizes (batch %d, length %d, dirs %d, hidden %d)", B, L, dirs, H);
+  const int threads = std::min(1024, ((4 * H + 31) / 32) * 32);
+  const size_t smem = (size_t)9 * H * sizeof(float);
+  lstm_bwd_kernel<<<dim3(B, dirs), threads, smem, static_cast<cudaStream_t>(stream)>>>(dh, dc, whh, lengths, init, h, c, acts,
+                                                                                       dgates, h_prev, dstate, L, H);
+  KT_CHECK_CUDA(cudaGetLastError());
+  return KT_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

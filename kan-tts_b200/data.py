@@ -186,3 +186,47 @@ def attn_prior_placeholder(phoneme_count, mel_count):
     shape, and a batch that misses ``AttnPriors`` trains on NaN losses instead of silently without a prior (an all-zero
     prior would be a constant under the attention's log-softmax)."""
     return torch.full((), float("nan"), dtype=torch.float32).expand(int(mel_count), int(phoneme_count))
+
+
+def pad_sambert_batch(batch, symbol_multiple, frame_multiple, r, ling_pad, emotion_pad, speaker_pad):
+    """Right-pad a SAM-BERT collate batch (``AM_Dataset.collate_fn``'s keys, tensors on the device) to L' symbols, L' the
+    symbol count rounded up to a multiple of ``symbol_multiple``, and T' frames, T' the frame count rounded up to a multiple
+    of ``frame_multiple`` (itself a multiple of ``r``), with the collate's pad values: ``ling_pad`` per linguistic column
+    and ``emotion_pad`` / ``speaker_pad``, the linguistic unit's "_" ids (``KanTtsLinguisticUnit._sub_unit_pad``; a float
+    speaker embedding pads with 0.0 and ignores ``speaker_pad``),
+    ``fp_label`` 0, mel / pitch / energy 0.0, durations 0 -- except that the T' - T new frames go to the symbol after each
+    item's last one (index valid_input_lengths + 1, or the last column), as the collate gives an item its padding frames.
+    Batches with durations only (not MAS).  -> a new dict; the lengths are unchanged.  Device ops only, no host synchronisation.
+
+    Fewer distinct batch shapes mean fewer CUDA graphs (SambertStep(cuda_graph=True) captures one per shape).  Padding is
+    not free of consequence: past a batch's own longest item, a padding symbol's encoder row reads as its LayerNorm bias in
+    the k = 3 feed-forward convs (see KanTtsSAMBERT.front_half), so the longest item's results change.  Padding is the
+    caller's choice; the train step trains on exactly what it is given."""
+    import torch.nn.functional as F
+    if frame_multiple % r:
+        raise ValueError(f"pad_sambert_batch: frame_multiple ({frame_multiple}) must be a multiple of r ({r})")
+    if symbol_multiple < 1 or frame_multiple < 1:
+        raise ValueError("pad_sambert_batch: the multiples must be >= 1")
+    if batch.get("durations") is None:
+        raise ValueError("pad_sambert_batch: a batch without durations (MAS: frame-level contours) is not padded here")
+    lings = batch["input_lings"]
+    L, T = lings.shape[1], batch["mel_targets"].shape[1]
+    dl, dt = -L % symbol_multiple, -T % frame_multiple
+    out = dict(batch)
+    if lings.shape[2] != len(ling_pad):
+        raise ValueError(f"pad_sambert_batch: {lings.shape[2]} linguistic columns but {len(ling_pad)} pad ids")
+    out["input_lings"] = torch.stack([F.pad(lings[:, :, i], (0, dl), value=int(v)) for i, v in enumerate(ling_pad)], -1)
+    out["input_emotions"] = F.pad(batch["input_emotions"], (0, dl), value=int(emotion_pad))
+    spk = batch["input_speakers"]
+    out["input_speakers"] = F.pad(spk, (0, 0, 0, dl)) if spk.dim() == 3 else F.pad(spk, (0, dl), value=int(speaker_pad))
+    if batch.get("fp_label") is not None:
+        out["fp_label"] = F.pad(batch["fp_label"], (0, dl), value=0)
+    out["mel_targets"] = F.pad(batch["mel_targets"], (0, 0, 0, dt))
+    for k in ("pitch_contours", "energy_contours"):
+        out[k] = F.pad(batch[k], (0, dl))
+    dur = F.pad(batch["durations"], (0, dl))
+    if dt:
+        at = (batch["valid_input_lengths"].long() + 1).clamp_max(dur.shape[1] - 1).unsqueeze(1)
+        dur = dur.scatter_add(1, at, torch.full_like(at, dt, dtype=dur.dtype))
+    out["durations"] = dur
+    return out

@@ -13,8 +13,9 @@ Where the arithmetic runs:
     through ops.ConvFn, on the model's native (B, L, C) rows, with bias / ReLU / residual fused;
   * LayerNorm, multi-head attention (both PNCA attentions, probabilities materialised like the reference),
     the FSMN memory block and the LengthRegulator expansion -> the kernels in csrc/sambert.cu;
-  * the four LSTMs stay on cuDNN (``nn.LSTM``) in training -- SURVEY.md section 2c rules them out of scope for custom
-    kernels; inference runs the duration predictor's in kt_ar_duration_infer, the pitch / energy predictors' BiLSTMs in
+  * the four LSTMs (the ``nn.LSTM`` modules hold their parameters) -> in training sambert_ops.lstm_layer: the input
+    projection on the conv kernels, the recurrence and its backward in kt_lstm_train_fwd / _bwd, lengths on the device;
+    inference runs the duration predictor's in kt_ar_duration_infer, the pitch / energy predictors' BiLSTMs in
     kt_blstm_ragged and the streamed post-net's in kt_lstm_stream_slots -- and the remaining glue (embedding lookups,
     concatenations, padding masks, sinusoid tables, dropout) is torch elementwise / indexing code, as in the reference.
 The filled-pause variant (``FP: True``, sambert_fp_8k.yaml) is built: FP_Predictor on the same conv / LayerNorm
@@ -457,8 +458,15 @@ class VarRnnARPredictor(nn.Module):
         self.fc = Linear(rnn_units, 1, relu=True)
 
     def forward(self, inputs, cond, h=None, masks=None):
+        """Over all rows from ``h`` (nn.LSTM's initial (h_0, c_0), or None: zeros), one sambert_ops.lstm_layer per layer
+        -> (x, h_new = (h_n, c_n)), (num_layers, B, H) each."""
         x = torch.cat([self.prenet(inputs), cond], dim=-1)
-        x, h_new = self.lstm(x, h)
+        h_n, c_n = [], []
+        for layer in range(self.lstm.num_layers):
+            x, c = sops.lstm_layer(x, self.lstm, layer, state=h)
+            h_n.append(x[:, -1])
+            c_n.append(c[:, -1])
+        h_new = (torch.stack(h_n), torch.stack(c_n))
         x = self.fc(x).squeeze(-1)
         if masks is not None:
             x = x.masked_fill(masks, 0.0)
@@ -506,13 +514,10 @@ class VarFsmnRnnNARPredictor(nn.Module):
         x = self.fsmn(inputs, masks)
         if not self.training and not torch.is_grad_enabled():
             x = self.blstm_infer(x, masks)
-        elif masks is not None:
-            lengths = torch.sum((~masks).float(), dim=1).long()
-            x = nn.utils.rnn.pack_padded_sequence(x, lengths.tolist(), batch_first=True, enforce_sorted=False)
-            x, _ = self.blstm(x)
-            x, _ = nn.utils.rnn.pad_packed_sequence(x, batch_first=True, total_length=inputs.size(1))
         else:
-            x, _ = self.blstm(x)
+            # pack_padded_sequence -> BiLSTM -> pad_packed_sequence, with each item's length on the device
+            lengths = None if masks is None else (~masks).sum(1, dtype=torch.int32)
+            x, _ = sops.lstm_layer(x, self.blstm, 0, lengths)
         x = self.fc(x).squeeze(-1)
         if masks is not None:
             x = x.masked_fill(masks, 0.0)
@@ -522,8 +527,8 @@ class VarFsmnRnnNARPredictor(nn.Module):
         """The packed BiLSTM of ``forward`` for inference (no autograd): both directions over each item's own rows
         [0, len_b) in ONE kernel (kt_blstm_ragged), with the lengths taken from ``masks`` on the device (no host read);
         rows >= len_b are zero.  The input projection of both directions is one k = 1 conv over the concatenated [8H]
-        weights.  An item's rows do not depend on the other items of the batch or on its padding.  Training keeps
-        nn.LSTM (cuDNN)."""
+        weights.  An item's rows do not depend on the other items of the batch or on its padding.  Training runs
+        sambert_ops.lstm_layer."""
         lstm, (B, L) = self.blstm, x.shape[:2]
         H = lstm.hidden_size
         if not x.is_cuda:
@@ -612,7 +617,7 @@ class HybridAttentionDecoder(nn.Module):
             layer.reset_state()
 
     def get_pnca_attn_mask(self, device, max_len, x_band_width, h_band_width, mask=None):
-        """kantts_sambert.py:137-168.  True = masked.  x: keys [i - x_bw, i]; h: keys [i, i + h_bw]; padded keys are
+        """kantts_sambert.py:137-168.  True = masked.  The band widths are ints or 0-d device tensors.  x: keys [i - x_bw, i]; h: keys [i, i + h_bw]; padded keys are
         masked except on padded QUERY rows, which stay fully open so that their softmax is finite."""
         i = torch.arange(max_len, device=device)[:, None]
         j = torch.arange(max_len, device=device)[None, :]
@@ -901,7 +906,7 @@ class PostNet(nn.Module):
         self.fc = Linear(config["postnet_lstm_units"], self.num_mels)
 
     def forward(self, x, mask=None, resid=None):
-        h, _ = self.lstm(self.fsmn(x, mask))
+        h, _ = sops.lstm_layer(self.fsmn(x, mask), self.lstm, 0)
         return self.fc(h, resid=resid)
 
     def streamer(self, batch, max_frames, lengths):
@@ -1210,7 +1215,8 @@ class KanTtsSAMBERT(nn.Module):
         the ``FP`` predictor read an item's padding rows as zeros (in the padded batch a padding row's LayerNorm is its
         bias), the frames that pad an item's last decoder step take position code 0 (t + 1 in the padded batch), and with
         ``FP`` the emotion / speaker rows are extended mod the item's length, not mod the padded length.
-        ``x_band_width``, the batch-max band, is batch-dependent by definition."""
+        ``x_band_width``, the batch-max band (a 0-d int64 device tensor: ``forward`` makes it the reference's int), is
+        batch-dependent by definition."""
         batch_size = inputs_ling.size(0)
         r = self.mel_decoder.r
         input_masks = get_mask_from_lengths(input_lengths, max_len=inputs_ling.size(1))
@@ -1251,10 +1257,10 @@ class KanTtsSAMBERT(nn.Module):
         memory = torch.cat([lfr_text, lfr_spk, lfr_emo], dim=-1)
         if duration_targets is not None:
             dur = duration_targets.float().masked_fill(inter_masks, 0)
-            x_band_width = int(dur.max() / r + 0.5)
         else:
             dur = torch.exp(log_dur_p) - 1
-            x_band_width = int(dur.max() / r + 0.5)
+        # the reference's int(dur.max() / r + 0.5), kept on the device (0-d int64)
+        x_band_width = torch.trunc(dur.max() / r + 0.5).long()
         # each utterance's own band (the batch-1 rule), on the device: the max over its symbols only
         band_width_rows = torch.trunc(dur.masked_fill(inter_masks, float("-inf")).amax(1) / r + 0.5).to(torch.int32)
         return dict(enc_attns=enc_attns, fp_p=fp_p, inter_lengths=inter_lengths, output_masks=output_masks,
@@ -1271,7 +1277,11 @@ class KanTtsSAMBERT(nn.Module):
         f = self.front_half(inputs_ling, inputs_emotion, inputs_speaker, input_lengths, output_lengths, mel_targets,
                             duration_targets, pitch_targets, energy_targets, fp_label, attn_priors)
         output_masks, lr_len, inter_lengths = f["output_masks"], f["lr_len"], f["inter_lengths"]
-        x_band_width = h_band_width = f["x_band_width"]
+        # the reference's Python int, read on the host -- except under CUDA-graph capture, where it stays a 0-d device tensor
+        x_band_width = f["x_band_width"]
+        if not (x_band_width.is_cuda and torch.cuda.is_current_stream_capturing()):
+            x_band_width = int(x_band_width)
+        h_band_width = x_band_width
         dec, ax_lst, ah_lst = self.mel_decoder(f["memory"], x_band_width, h_band_width, target=mel_targets,
                                                mask=f["lfr_masks"], return_attns=True)
         dec_outputs = dec.contiguous().view(batch_size, -1, self.mel_decoder.d_mel)

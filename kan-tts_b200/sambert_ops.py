@@ -1,12 +1,12 @@
 """autograd wrappers of the SAM-BERT entry points of libkantts_b200.so (LayerNorm, multi-head attention,
-FSMN memory block, LengthRegulator gather, filled-pause insertion).  Same contract as ops.py: CUDA fp32 tensors only, explicit
+FSMN memory block, LengthRegulator gather, LSTM recurrence, filled-pause insertion).  Same contract as ops.py: CUDA fp32 tensors only, explicit
 stream, RuntimeError on any failure -- no PyTorch / CPU fallback."""
 import ctypes
 import math
 
 import torch
 
-from . import _lib
+from . import _lib, ops
 from ._lib import KtAttnDesc, ptr
 from .ops import call
 
@@ -261,6 +261,93 @@ class RowsGatherFn(torch.autograd.Function):
         din = torch.empty(B, ctx.t_in, C, device=dout.device, dtype=torch.float32)
         call("kt_rows_gather_bwd", ptr(dout), ptr(idx, True), ptr(start, True), ptr(count, True), ptr(din), B, T_out, ctx.t_in, C)
         return din, None, None, None
+
+
+class LstmFn(torch.autograd.Function):
+    """The recurrence of one nn.LSTM layer (kt_lstm_train_fwd / _bwd), uni- or bidirectional: gx (B, T, D * 4H), the input
+    projection x . W_ih^T + b_ih + b_hh of each direction, and whh (D * 4H, H), each direction's W_hh, -> h and the cell
+    states c, (B, T, D * H) each.  ``lengths`` (device int32 (B,) or None): the packed semantics of pack_padded_sequence
+    (rows >= lengths[b] of h and c are zero), or every row.  ``h0`` / ``c0`` (B, D, H) or None: the initial state of each
+    direction (zeros when None).  ``grad``: whether the caller records autograd (the forward then keeps the cell states and
+    gate activations for the backward).  The backward recurrence gives dgx and the initial state's gradient; dW_hh is the
+    k = 1 weight gradient of the grouped (one group per direction) conv whose input is each row's recurrent input h_prev."""
+
+    @staticmethod
+    def forward(ctx, gx, whh, lengths, dirs, h0, c0, grad):
+        gx = gx.contiguous()
+        B, T, G = gx.shape
+        H = G // (4 * dirs)
+        w = whh.detach()
+        whh_t = w.view(dirs, 4 * H, H).transpose(1, 2).contiguous()
+        init = None if h0 is None else torch.stack([h0.detach(), c0.detach()], 2).contiguous()
+        h = torch.empty(B, T, dirs * H, device=gx.device, dtype=torch.float32)
+        c = torch.empty_like(h)
+        save = grad and any(ctx.needs_input_grad[:2] + ctx.needs_input_grad[4:6])
+        acts = torch.empty_like(gx) if save else None
+        call("kt_lstm_train_fwd", ptr(gx), ptr(whh_t), ptr(lengths, True), ptr(init), ptr(h), ptr(c), ptr(acts), B, T, dirs, H)
+        ctx.dirs = dirs
+        # an unused c (the usual case) then reaches the backward as None, and the kernel reads no dc rows
+        ctx.set_materialize_grads(False)
+        if save:
+            ctx.save_for_backward(h, c, acts, whh, lengths, init)
+        return h, c
+
+    @staticmethod
+    def backward(ctx, dh, dc):
+        h, c, acts, whh, lengths, init = ctx.saved_tensors
+        B, T, DH = h.shape
+        dirs = ctx.dirs
+        H = DH // dirs
+        dh = torch.zeros_like(h) if dh is None else dh.contiguous()
+        dc = None if dc is None else dc.contiguous()
+        w = whh.detach().contiguous()
+        dgx = torch.empty_like(acts)
+        h_prev = torch.empty_like(h)
+        dstate = torch.empty_like(init) if init is not None and any(ctx.needs_input_grad[4:6]) else None
+        call("kt_lstm_train_bwd", ptr(dh), ptr(dc), ptr(w), ptr(lengths, True), ptr(init), ptr(h), ptr(c), ptr(acts), ptr(dgx),
+             ptr(h_prev), ptr(dstate), B, T, dirs, H)
+        dwhh = None
+        if ctx.needs_input_grad[1]:
+            spec = _whh_spec(dirs, H)
+            _, dwhh, _ = ops._weight_backward(spec, spec.plan(B, 1, T), h_prev, dgx, None, w, None, (whh, None, None), None,
+                                              True, False, False)
+            dwhh = dwhh.view_as(whh)
+        dh0 = dc0 = None
+        if dstate is not None:
+            dh0, dc0 = dstate[:, :, 0], dstate[:, :, 1]
+        return dgx, dwhh, None, None, dh0, dc0, None
+
+
+_WHH_SPECS = {}
+
+
+def _whh_spec(dirs, H):
+    """The recurrent term h_prev . W_hh^T of all directions as one grouped k = 1 conv (its weight gradient is dW_hh)."""
+    spec = _WHH_SPECS.get((dirs, H))
+    if spec is None:
+        spec = _WHH_SPECS[(dirs, H)] = ops.ConvSpec(c_in=dirs * H, c_out=dirs * 4 * H, kernel=1, groups=dirs)
+    return spec
+
+
+def lstm_layer(x, lstm, layer, lengths=None, state=None):
+    """Layer ``layer`` of the nn.LSTM ``lstm`` (batch_first, its parameters as they are) over x (B, T, C) -> h (B, T, D * H),
+    c (B, T, D * H).  The input projection of all directions is one k = 1 conv (ops.conv: dx, dW_ih and the biases' gradient
+    come from its backward), the recurrence LstmFn.  ``lengths``: see LstmFn.  ``state``: None (zeros) or nn.LSTM's initial
+    (h_0, c_0), each (num_layers * D, B, H)."""
+    sfx = [f"_l{layer}"] + ([f"_l{layer}_reverse"] if lstm.bidirectional else [])
+    p = lambda name: [getattr(lstm, name + s) for s in sfx]
+    H, D = lstm.hidden_size, len(sfx)
+    w_ih = torch.cat(p("weight_ih")).unsqueeze(-1)
+    bias = torch.cat([bi + bh for bi, bh in zip(p("bias_ih"), p("bias_hh"))])
+    specs = lstm.__dict__.setdefault("_kt_specs", {})
+    spec = specs.get(layer)
+    if spec is None:
+        spec = specs[layer] = ops.ConvSpec(c_in=w_ih.shape[1], c_out=D * 4 * H, kernel=1)
+    gx = ops.conv(x.contiguous(), spec, ops.PreparedWeight(), w_ih, None, bias)
+    h0 = c0 = None
+    if state is not None:
+        h0, c0 = (t[layer * D:(layer + 1) * D].transpose(0, 1) for t in state)
+    return LstmFn.apply(gx, torch.cat(p("weight_hh")), lengths, D, h0, c0, torch.is_grad_enabled())
 
 
 def fp_insert_plan(input_lengths, length, fp_label=None, fp_p=None):

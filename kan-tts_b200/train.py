@@ -57,6 +57,17 @@ class FlatGrads:
             p.requires_grad_(flag)
 
 
+def invalidate_weight_caches(modules):
+    """Forget every prepared (kernel-layout) weight of ``modules``, so that the next forward re-runs kt_weight_prepare /
+    kt_weight_pack_tc (in place, into the same persistent buffers).  A CUDA-graph step calls it before a capture, so that the
+    graph re-prepares the weights its eager optimizer step changed."""
+    for m in modules:
+        for sub in m.modules():
+            c = getattr(sub, "_cache", None)
+            if isinstance(c, ops.PreparedWeight):
+                c.key = None
+
+
 class GanStep:
     """model = {"generator": G, "discriminator": {name: D}}, optimizer / scheduler dicts of the same
     shape and ``criterion`` as built by the reference's builders (or this package's)."""
@@ -268,11 +279,7 @@ class GanStep:
         re-runs kt_weight_prepare / kt_weight_pack_tc (in place, into the same persistent buffers)."""
         if mods is None:
             mods = [self.model["generator"], *self.model["discriminator"].values()]
-        for m in mods:
-            for sub in m.modules():
-                c = getattr(sub, "_cache", None)
-                if isinstance(c, ops.PreparedWeight):
-                    c.key = None
+        invalidate_weight_caches(mods)
 
     # ---- CUDA-graph replay -----------------------------------------------------------------------------------
     def _capture(self, y, x):
@@ -405,9 +412,19 @@ def apply_gradients(loss_total, grads, optimizer, scheduler, grad_clip):
     """The tail of the SAM-BERT and syBERT train steps (Sambert_Trainer.train_step, Textsy_BERT_Trainer.train_step in
     kantts/train/trainer.py) after the loss: zero the flat gradient buffer, backward, the data-parallel all-reduce (mean)
     of that buffer, gradient-norm clipping (``grad_clip`` None: none), the optimizer and the scheduler step."""
+    _backward(loss_total, grads)
+    _update(grads, optimizer, scheduler, grad_clip)
+
+
+def _backward(loss_total, grads):
+    """Zero the flat gradient buffer, backward into it, and join the weight-gradient streams."""
     grads.zero()
     loss_total.backward()
     ops.join_wgrad_streams(loss_total.device if loss_total.is_cuda else None)
+
+
+def _update(grads, optimizer, scheduler, grad_clip):
+    """The data-parallel all-reduce (mean) of the flat gradient buffer, the clip, the optimizer and the scheduler step."""
     grads.all_reduce_mean()
     if grad_clip is not None:
         torch.nn.utils.clip_grad_norm_(grads.params, grad_clip)
@@ -420,15 +437,37 @@ class SambertStep:
     ProsodyReconLoss, backward, gradient-norm clipping, Adam, NoamLR.  Data parallel: the batch is sharded by
     utterance and the only exchange is ONE in-place NCCL all-reduce (mean) of the flat gradient buffer
     (49.2 MB for sambert_24k.yaml) between backward and the clip -- replacing the DistributedDataParallel
-    wrapper of kantts/models/__init__.py:120-127.  Losses stay on the device (``losses_to_float`` syncs)."""
+    wrapper of kantts/models/__init__.py:120-127.  Losses stay on the device (``losses_to_float`` syncs).
 
-    def __init__(self, model, optimizer, scheduler, criterion, grad_clip=1.0):
+    ``cuda_graph=True``: the forward, the losses and the backward into the flat gradient buffer run as a replayed CUDA graph;
+    the all-reduce, the clip, the optimizer and the scheduler stay eager after the replay, as in ``GanStep``.  The collate
+    pads each batch to its own longest item, so one graph is captured per distinct batch shape (the shapes and dtypes of
+    the batch's tensors, and the model's train() / eval() mode), after ``graph_warmup`` eager steps of that shape; each graph replays from its own static copies
+    of the batch, and all graphs share one memory pool (they never run concurrently).  The step never pads a batch: it
+    trains on exactly the tensors it is given, as the eager step does.  To bound the number of graphs, pad the batches
+    before the step with ``data.pad_sambert_batch`` -- which changes the longest item's results (see there).
+    In graph mode the returned losses are copies of the graph's outputs (one device copy each, no host synchronisation), as
+    independent of later steps as the eager step's, and ``x_band_width`` / ``h_band_width`` are 0-d int64 device tensors
+    (the eager step returns the reference's Python ints).
+    Filled-pause (FP) and alignment-search (MAS) models read the host during their forward and are refused."""
+
+    def __init__(self, model, optimizer, scheduler, criterion, grad_clip=1.0, cuda_graph=False, graph_warmup=3):
+        if cuda_graph and getattr(model, "fp_enable", False):
+            raise ValueError("SambertStep(cuda_graph=True): a filled-pause (FP) model cannot be captured -- the forward "
+                             "reads the output length of fp_insert_plan (the spliced symbol count) on the host")
+        if cuda_graph and getattr(model, "MAS", False):
+            raise ValueError("SambertStep(cuda_graph=True): an alignment-search (MAS) model cannot be captured -- align's "
+                             "length validation reads input_lengths / output_lengths on the host")
         self.model, self.optimizer, self.scheduler, self.criterion = model, optimizer, scheduler, criterion
         self.grad_clip = grad_clip
         self.grads = FlatGrads(model)
         self.steps = 0
         # the training epoch the caller's loop is in (Sambert_Trainer.epoch): the warm-up of AttentionBinarizationLoss
         self.epoch = 0
+        self.cuda_graph, self.graph_warmup = bool(cuda_graph), int(graph_warmup)
+        self._graphs = {}          # batch shape -> (static batch, CUDAGraph, output dict)
+        self._warm = {}            # batch shape -> eager steps run
+        self._pool = None
 
     def step(self, batch):
         """batch: dict with the reference collate keys (input_lings, input_emotions, input_speakers,
@@ -437,6 +476,55 @@ class SambertStep:
         pitch / energy contours are padded to the length with the pauses inserted.  With the two attention losses in the
         criterion (a MAS model, the reference's ``with_MAS``) the batch has ``attn_priors`` (B, T_mel, L), frame-level
         pitch / energy contours and no durations (None or absent): the model finds them by alignment search."""
+        if not self.cuda_graph:
+            return self._eager_step(batch)
+        key = (self.model.training,) + tuple((k, tuple(v.shape), v.dtype) for k, v in sorted(batch.items())
+                                             if torch.is_tensor(v))
+        entry = self._graphs.get(key)
+        if entry is None:
+            done = self._warm.get(key, 0)
+            if done < self.graph_warmup:
+                # eager warm-up of this shape on a side stream (allocator, optimizer state and kernel plans settle)
+                self._warm[key] = done + 1
+                cur = torch.cuda.current_stream()
+                s = torch.cuda.Stream()
+                s.wait_stream(cur)
+                with torch.cuda.stream(s):
+                    out = self._eager_step(batch)
+                cur.wait_stream(s)
+                return out
+            entry = self._capture(key, batch)
+        static, graph, out = entry
+        for k, v in static.items():
+            v.copy_(batch[k], non_blocking=True)
+        graph.replay()
+        # copies: the graphs share one memory pool, so a later replay of another graph may reuse the outputs' blocks
+        res = {k: v.clone() for k, v in out.items()}
+        _update(self.grads, self.optimizer, self.scheduler, self.grad_clip)
+        self.steps += 1
+        return res
+
+    def _capture(self, key, batch):
+        static = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
+        invalidate_weight_caches([self.model])
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=self._pool):
+            out = self._losses(dict(batch, **static))
+            _backward(out["TotalLoss"], self.grads)
+        if self._pool is None:
+            self._pool = graph.pool()
+        entry = self._graphs[key] = (static, graph, {k: v.detach() for k, v in out.items()})
+        return entry
+
+    def _eager_step(self, batch):
+        out = self._losses(batch)
+        apply_gradients(out["TotalLoss"], self.grads, self.optimizer, self.scheduler, self.grad_clip)
+        self.steps += 1
+        return {k: (v.detach() if torch.is_tensor(v) else v) for k, v in out.items()}
+
+    def _losses(self, batch):
+        """The forward and the losses -> the step's result dict (TotalLoss still attached to the autograd graph)."""
         fp_label = batch.get("fp_label")
         with_mas = "AttentionCTCLoss" in self.criterion and "AttentionBinarizationLoss" in self.criterion
         res = self.model(
@@ -461,9 +549,7 @@ class SambertStep:
                                                                batch["valid_output_lengths"])
             attn_kl_loss = self.criterion["AttentionBinarizationLoss"](self.epoch, res["attn_hard"], res["attn_soft"])
             loss_total = loss_total + attn_ctc_loss + attn_kl_loss
-        apply_gradients(loss_total, self.grads, self.optimizer, self.scheduler, self.grad_clip)
-        self.steps += 1
-        out = {"TotalLoss": loss_total.detach(), "mel_loss_": mel_loss_.detach(), "mel_loss": mel_loss.detach(),
+        out = {"TotalLoss": loss_total, "mel_loss_": mel_loss_.detach(), "mel_loss": mel_loss.detach(),
                "dur_loss": dur_loss.detach(), "pitch_loss": pitch_loss.detach(),
                "energy_loss": energy_loss.detach(), "x_band_width": res["x_band_width"],
                "h_band_width": res["h_band_width"]}
