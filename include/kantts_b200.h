@@ -336,8 +336,11 @@ int kt_fp_insert_bwd(const float* dout, const int32_t* codes, const int32_t* row
  * kt_attn_ctc_fwd / _bwd: AttentionCTCLoss (kantts/train/loss.py:481-508), one CTA per utterance.  Frame t < T of
  * utterance b is log_softmax([blank_logprob, logprob[b][t][:N]]), N = in_lengths[b], T = out_lengths[b]; the CTC loss of
  * the targets 1..N over those frames, divided by N, 0 when infinite (zero_infinity); loss [1] = their mean over the batch.
- * The backward writes all of d_logprob [batch][t_q][t_k] = d_loss[0] * the gradient of loss.  `workspace` holds the alpha
- * recursion and the per-frame normalisers between the two calls: kt_attn_ctc_workspace_bytes.
+ * The backward writes all of d_logprob [batch][t_q][t_k] = d_loss[0] * the gradient of loss.  The alpha / beta recursions
+ * run in float64 (their values reach thousands at training lengths and the posteriors cancel them); the frame normalisers,
+ * loss and gradient are fp32.  The two float64 state rows live in shared memory: t_k <= 3071.  `workspace` holds the
+ * float64 alpha recursion and per-utterance -log p, then the fp32 per-frame normalisers, between the two calls:
+ * kt_attn_ctc_workspace_bytes.
  *
  * kt_attn_prior: the alignment prior of a collate batch, beta_binomial_prior_distribution (kantts/datasets/dataset.py:20-31)
  * per utterance as AM_Dataset.collate_fn pads it (dataset.py:816-827).  valid_input_lengths / valid_output_lengths

@@ -1,6 +1,7 @@
 // Alignment learning of SAM-BERT with monotonic alignment search (MAS: True, sambert_16k_MAS*.yaml): the distance attention
 // of ConvAttention (kantts/models/sambert/attention.py:85-125), the width-1 MAS of alignment.py:32-71 and the forward-sum
-// loss of AttentionCTCLoss (kantts/train/loss.py:481-508).  Exact fp32 on CUDA cores, fixed-order reductions, no atomics.
+// loss of AttentionCTCLoss (kantts/train/loss.py:481-508).  Exact fp32 on CUDA cores (the forward-sum recursions in float64),
+// fixed-order reductions, no atomics.
 // Also the beta-binomial alignment prior of the data path (kantts/datasets/dataset.py:20-31), evaluated in float64.
 #include <math.h>
 
@@ -309,41 +310,49 @@ __global__ void __launch_bounds__(kMasThreads) mas_kernel(const float* __restric
 }
 
 // ---- forward-sum (CTC) loss ---------------------------------------------------------------------------------------------
+// The alpha / beta recursions run in float64.  Their log-probabilities grow like -(frames x per-frame cost), thousands at
+// a training utterance's length, and each gradient element's posterior exp(alpha + beta - y + nll) cancels them: in fp32
+// that cancellation leaves a relative error near 1e-3 at 1000 frames x 200 symbols.  The frame normalisers and the
+// log-softmax inputs stay fp32; a normaliser's rounding shifts every path through its frame alike, so it cancels in the
+// posteriors.  Loss and gradient are stored as fp32.
 constexpr int kCtcThreads = 256;
+constexpr int kCtcSmemMax = 96 * 1024;       // the two state rows of 2 t_k + 1 doubles: t_k <= 3071
 
 struct CtcWs {
-  float* alpha;    // [batch][t_q][2 t_k + 1]
+  double* alpha;   // [batch][t_q][2 t_k + 1]   first, so that the doubles are 8-byte aligned
+  double* nll;     // [batch]        -log p of each utterance
   float* lse;      // [batch][t_q]   log-sum-exp of the frame's [blank, keys < N]
-  float* nll;      // [batch]        -log p of each utterance
   float* losses;   // [batch]        nll / N, 0 when infinite
 };
 
-inline long long ctc_ws_floats(int batch, int t_q, int t_k) {
-  return (long long)batch * t_q * (2LL * t_k + 1) + (long long)batch * t_q + 2LL * batch;
+inline long long ctc_ws_bytes(int batch, int t_q, int t_k) {
+  return 8 * ((long long)batch * t_q * (2LL * t_k + 1) + batch) + 4 * ((long long)batch * t_q + batch);
 }
 
 inline CtcWs ctc_ws(void* ws, int batch, int t_q, int t_k) {
   CtcWs w;
-  w.alpha = static_cast<float*>(ws);
-  w.lse = w.alpha + (long long)batch * t_q * (2LL * t_k + 1);
-  w.nll = w.lse + (long long)batch * t_q;
-  w.losses = w.nll + batch;
+  w.alpha = static_cast<double*>(ws);
+  w.nll = w.alpha + (long long)batch * t_q * (2LL * t_k + 1);
+  w.lse = reinterpret_cast<float*>(w.nll + batch);
+  w.losses = w.lse + (long long)batch * t_q;
   return w;
 }
 
-__device__ __forceinline__ float lse2(float a, float b) {
-  const float m = fmaxf(a, b);
-  return m == -INFINITY ? -INFINITY : m + logf(expf(a - m) + expf(b - m));
+inline size_t ctc_smem_bytes(int t_k) { return (size_t)2 * (2 * t_k + 1) * sizeof(double); }
+
+__device__ __forceinline__ double lse2(double a, double b) {
+  const double m = fmax(a, b);
+  return m == -INFINITY ? -INFINITY : m + log(exp(a - m) + exp(b - m));
 }
 
-__device__ __forceinline__ float lse3(float a, float b, float c) {
-  const float m = fmaxf(fmaxf(a, b), c);
-  return m == -INFINITY ? -INFINITY : m + logf(expf(a - m) + expf(b - m) + expf(c - m));
+__device__ __forceinline__ double lse3(double a, double b, double c) {
+  const double m = fmax(fmax(a, b), c);
+  return m == -INFINITY ? -INFINITY : m + log(exp(a - m) + exp(b - m) + exp(c - m));
 }
 
 // log-probability of extended label s (even: the blank column, odd: key (s - 1) / 2) at frame row `lp`
-__device__ __forceinline__ float ctc_y(const float* lp, int s, float blank, float lse) {
-  return ((s & 1) ? __ldg(lp + (s >> 1)) : blank) - lse;
+__device__ __forceinline__ double ctc_y(const float* lp, int s, float blank, float lse) {
+  return (double)((s & 1) ? __ldg(lp + (s >> 1)) : blank) - (double)lse;
 }
 
 // One CTA per utterance: the frame log-softmax normalisers, then the alpha recursion over S = 2N + 1 states (stored for the
@@ -352,14 +361,14 @@ __global__ void __launch_bounds__(kCtcThreads) ctc_fwd_kernel(const float* __res
                                                               const int32_t* __restrict__ in_len,
                                                               const int32_t* __restrict__ out_len, CtcWs w, int t_q,
                                                               int t_k, float blank) {
-  extern __shared__ float smem[];
+  extern __shared__ double ctc_state[];
   const int S_max = 2 * t_k + 1;
-  float* a0 = smem;
-  float* a1 = smem + S_max;
+  double* a0 = ctc_state;
+  double* a1 = ctc_state + S_max;
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = min(out_len[b], t_q), N = min(in_len[b], t_k), S = 2 * N + 1;
   const float* lpb = logprob + (long long)b * t_q * t_k;
-  float* alpha = w.alpha + (long long)b * t_q * S_max;
+  double* alpha = w.alpha + (long long)b * t_q * S_max;
   float* lse = w.lse + (long long)b * t_q;
   if (T < 1 || N < 1) {
     if (tid == 0) {
@@ -380,33 +389,33 @@ __global__ void __launch_bounds__(kCtcThreads) ctc_fwd_kernel(const float* __res
   }
   __syncthreads();
   for (int s = tid; s < S; s += blockDim.x) {
-    const float v = s < 2 ? ctc_y(lpb, s, blank, lse[0]) : -INFINITY;
+    const double v = s < 2 ? ctc_y(lpb, s, blank, lse[0]) : -INFINITY;
     a0[s] = v;
     alpha[s] = v;
   }
   __syncthreads();
-  float* prev = a0;
-  float* cur = a1;
+  double* prev = a0;
+  double* cur = a1;
   for (int t = 1; t < T; ++t) {
     const float* row = lpb + (long long)t * t_k;
     const float l = lse[t];
     for (int s = tid; s < S; s += blockDim.x) {
-      const float x = prev[s];
-      const float y1 = s >= 1 ? prev[s - 1] : -INFINITY;
-      const float y2 = ((s & 1) && s >= 3) ? prev[s - 2] : -INFINITY;
-      const float v = ctc_y(row, s, blank, l) + lse3(x, y1, y2);
+      const double x = prev[s];
+      const double y1 = s >= 1 ? prev[s - 1] : -INFINITY;
+      const double y2 = ((s & 1) && s >= 3) ? prev[s - 2] : -INFINITY;
+      const double v = ctc_y(row, s, blank, l) + lse3(x, y1, y2);
       cur[s] = v;
       alpha[(long long)t * S_max + s] = v;
     }
     __syncthreads();
-    float* tmp = prev;
+    double* tmp = prev;
     prev = cur;
     cur = tmp;
   }
   if (tid == 0) {
-    const float nll = -lse2(prev[S - 1], prev[S - 2]);
+    const double nll = -lse2(prev[S - 1], prev[S - 2]);
     w.nll[b] = nll;
-    w.losses[b] = isinf(nll) ? 0.f : nll / (float)N;
+    w.losses[b] = isinf(nll) ? 0.f : (float)(nll / N);
   }
 }
 
@@ -428,47 +437,47 @@ __global__ void __launch_bounds__(kCtcThreads) ctc_bwd_kernel(const float* __res
                                                               const float* __restrict__ d_loss, CtcWs w,
                                                               float* __restrict__ d_logprob, int batch, int t_q, int t_k,
                                                               float blank) {
-  extern __shared__ float smem[];
+  extern __shared__ double ctc_state[];
   const int S_max = 2 * t_k + 1;
-  float* b0 = smem;
-  float* b1 = smem + S_max;
+  double* b0 = ctc_state;
+  double* b1 = ctc_state + S_max;
   const int b = blockIdx.x, tid = threadIdx.x;
   const int T = min(out_len[b], t_q), N = min(in_len[b], t_k), S = 2 * N + 1;
-  const float nll = w.nll[b];
-  const bool live = T >= 1 && N >= 1 && !isinf(nll);
+  const double nll = (T >= 1 && N >= 1) ? w.nll[b] : INFINITY;
+  const bool live = !isinf(nll);
   float* gb = d_logprob + (long long)b * t_q * t_k;
   for (long long e = tid; e < (long long)t_q * t_k; e += blockDim.x) {
     const int t = (int)(e / t_k), j = (int)(e - (long long)t * t_k);
     if (!live || t >= T || j >= N) gb[e] = 0.f;
   }
   if (!live) return;
-  const float g = d_loss[0] / ((float)batch * (float)N);
+  const double g = (double)d_loss[0] / ((double)batch * (double)N);
   const float* lpb = logprob + (long long)b * t_q * t_k;
-  const float* alpha = w.alpha + (long long)b * t_q * S_max;
+  const double* alpha = w.alpha + (long long)b * t_q * S_max;
   const float* lse = w.lse + (long long)b * t_q;
-  float* next = b0;
-  float* cur = b1;
+  double* next = b0;
+  double* cur = b1;
   for (int t = T - 1; t >= 0; --t) {
     const float* row = lpb + (long long)t * t_k;
     const float l = lse[t];
     for (int s = tid; s < S; s += blockDim.x) {
-      const float y = ctc_y(row, s, blank, l);
-      float v;
+      const double y = ctc_y(row, s, blank, l);
+      double v;
       if (t == T - 1) {
         v = s >= S - 2 ? y : -INFINITY;
       } else {
-        const float x1 = s + 1 < S ? next[s + 1] : -INFINITY;
-        const float x2 = ((s & 1) && s + 2 < S) ? next[s + 2] : -INFINITY;
+        const double x1 = s + 1 < S ? next[s + 1] : -INFINITY;
+        const double x2 = ((s & 1) && s + 2 < S) ? next[s + 2] : -INFINITY;
         v = y + lse3(next[s], x1, x2);
       }
       cur[s] = v;
       if (s & 1) {
-        const float post = expf(alpha[(long long)t * S_max + s] + v - y + nll);
-        gb[(long long)t * t_k + (s >> 1)] = g * (expf(y) - post);
+        const double post = exp(alpha[(long long)t * S_max + s] + v - y + nll);
+        gb[(long long)t * t_k + (s >> 1)] = (float)(g * (exp(y) - post));
       }
     }
     __syncthreads();
-    float* tmp = next;
+    double* tmp = next;
     next = cur;
     cur = tmp;
   }
@@ -605,7 +614,7 @@ extern "C" int kt_mas(const float* soft, const int32_t* in_lengths, const int32_
 
 extern "C" int64_t kt_attn_ctc_workspace_bytes(int32_t batch, int32_t t_q, int32_t t_k) {
   if (batch <= 0 || t_q <= 0 || t_k <= 0) return 0;
-  return (int64_t)ctc_ws_floats(batch, t_q, t_k) * 4;
+  return (int64_t)ctc_ws_bytes(batch, t_q, t_k);
 }
 
 static int ctc_check(const float* logprob, const int32_t* in_lengths, const int32_t* out_lengths, const void* workspace,
@@ -613,8 +622,9 @@ static int ctc_check(const float* logprob, const int32_t* in_lengths, const int3
   KT_REQUIRE(logprob && in_lengths && out_lengths && workspace, "%s: null argument", what);
   KT_REQUIRE(batch > 0 && batch <= 65535 && t_q > 0 && t_k > 0, "%s: bad shape (batch %d, t_q %d, t_k %d)", what, batch,
              t_q, t_k);
-  KT_REQUIRE((2LL * (2 * t_k + 1)) * 4 <= 96 * 1024, "%s: %d keys exceed the shared-memory state rows", what, t_k);
-  const long long need = ctc_ws_floats(batch, t_q, t_k) * 4;
+  KT_REQUIRE(ctc_smem_bytes(t_k) <= (size_t)kCtcSmemMax, "%s: %d keys exceed the shared-memory state rows (at most %d)",
+             what, t_k, (kCtcSmemMax / (int)sizeof(double) / 2 - 1) / 2);
+  const long long need = ctc_ws_bytes(batch, t_q, t_k);
   if (workspace_bytes < need) {
     set_error("%s: workspace too small (%lld < %lld bytes)", what, (long long)workspace_bytes, need);
     return KT_ERR_WORKSPACE;
@@ -630,9 +640,8 @@ extern "C" int kt_attn_ctc_fwd(const float* logprob, const int32_t* in_lengths, 
   KT_REQUIRE(loss, "attn_ctc_fwd: null loss");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const CtcWs w = ctc_ws(workspace, batch, t_q, t_k);
-  const size_t smem = (size_t)2 * (2 * t_k + 1) * sizeof(float);
-  KT_CHECK_CUDA(allow_dyn_smem<ctc_fwd_kernel>(96 * 1024));
-  ctc_fwd_kernel<<<batch, kCtcThreads, smem, st>>>(logprob, in_lengths, out_lengths, w, t_q, t_k, blank_logprob);
+  KT_CHECK_CUDA(allow_dyn_smem<ctc_fwd_kernel>(kCtcSmemMax));
+  ctc_fwd_kernel<<<batch, kCtcThreads, ctc_smem_bytes(t_k), st>>>(logprob, in_lengths, out_lengths, w, t_q, t_k, blank_logprob);
   KT_CHECK_CUDA(cudaGetLastError());
   ctc_mean_kernel<<<1, 32, 0, st>>>(w, loss, batch);
   KT_CHECK_CUDA(cudaGetLastError());
@@ -646,9 +655,8 @@ extern "C" int kt_attn_ctc_bwd(const float* logprob, const int32_t* in_lengths, 
   if (rc != KT_OK) return rc;
   KT_REQUIRE(d_loss && d_logprob, "attn_ctc_bwd: null argument");
   const CtcWs w = ctc_ws(const_cast<void*>(workspace), batch, t_q, t_k);
-  const size_t smem = (size_t)2 * (2 * t_k + 1) * sizeof(float);
-  KT_CHECK_CUDA(allow_dyn_smem<ctc_bwd_kernel>(96 * 1024));
-  ctc_bwd_kernel<<<batch, kCtcThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+  KT_CHECK_CUDA(allow_dyn_smem<ctc_bwd_kernel>(kCtcSmemMax));
+  ctc_bwd_kernel<<<batch, kCtcThreads, ctc_smem_bytes(t_k), static_cast<cudaStream_t>(stream)>>>(
       logprob, in_lengths, out_lengths, d_loss, w, d_logprob, batch, t_q, t_k, blank_logprob);
   KT_CHECK_CUDA(cudaGetLastError());
   return KT_OK;

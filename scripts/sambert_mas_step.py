@@ -3,7 +3,8 @@ to 1000 frames) against the same model with MAS off on a batch with given durati
 (attention forward + backward, MAS, forward-sum loss forward + backward) against the reference formulation run through the
 oracle on the same GPU tensors: the materialised (B, C, T_mel, T_text) difference tensor, one torch.nn.CTCLoss call per
 utterance and the host DP.  Reports torch.cuda.max_memory_allocated of each and whether both gave the same hard
-alignments and durations.  Prints one JSON line with the card name and power limit.
+alignments and durations, and the device time of the forward-sum loss kernels alone (kt_attn_ctc_fwd, kt_attn_ctc_bwd)
+on the batch's attention log-probabilities.  Prints one JSON line with the card name and power limit.
 
     python scripts/sambert_mas_step.py [--steps 10] [--warmup 3]
 """
@@ -45,6 +46,36 @@ def _time(fn, steps, warmup):
         fn()
     torch.cuda.synchronize()
     return (time.perf_counter() - t0) / steps * 1e3, (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+
+
+def _event_ms(fn, steps, warmup):
+    """Mean device time of ``fn`` between CUDA events over ``steps`` calls, after ``warmup``."""
+    for _ in range(warmup):
+        fn()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(steps):
+        fn()
+    end.record()
+    end.synchronize()
+    return start.elapsed_time(end) / steps
+
+
+def _ctc_kernel_ms(lp, in_len, out_len, steps, warmup):
+    """Device time of kt_attn_ctc_fwd (with its batch-mean launch) and of kt_attn_ctc_bwd, each called on its own."""
+    from kantts_b200 import _lib
+    from kantts_b200._lib import ptr
+    from kantts_b200.ops import call
+    B, Tq, Tk = lp.shape
+    n = int(_lib.load().kt_attn_ctc_workspace_bytes(B, Tq, Tk))
+    ws = torch.empty(n // 4, device=DEV)
+    loss, d_loss, grad = torch.empty(1, device=DEV), torch.ones(1, device=DEV), torch.empty_like(lp)
+    il, ol = in_len.to(torch.int32).contiguous(), out_len.to(torch.int32).contiguous()
+    fwd = lambda: call("kt_attn_ctc_fwd", ptr(lp), ptr(il, True), ptr(ol, True), ptr(loss), ptr(ws), n, B, Tq, Tk, -1.0)
+    bwd = lambda: call("kt_attn_ctc_bwd", ptr(lp), ptr(il, True), ptr(ol, True), ptr(d_loss), ptr(ws), n, ptr(grad), B,
+                       Tq, Tk, -1.0)
+    fwd_ms = _event_ms(fwd, steps, warmup)
+    return fwd_ms, _event_ms(bwd, steps, warmup)
 
 
 def _step(cfg, batch, mas):
@@ -111,6 +142,10 @@ def main():
         out["reference"] = (hard, hard.sum(2)[:, 0, :])
 
     res["align_kernels_ms"], res["align_kernels_peak_mib"] = _time(kernels, args.steps, args.warmup)
+    with torch.no_grad():
+        _, lp = sambert_ops.AlignAttnFn.apply(q, k, prior, in_len)
+    res["attn_ctc_fwd_ms"], res["attn_ctc_bwd_ms"] = _ctc_kernel_ms(lp[:, 0].contiguous(), in_len, out_len,
+                                                                    max(20, args.steps), args.warmup)
     res["align_reference_ms"], res["align_reference_peak_mib"] = _time(reference, max(1, args.steps // 5), 1)
     res["hard_alignments_equal"] = torch.equal(out["kernels"][0], out["reference"][0])
     res["durations_equal"] = torch.equal(out["kernels"][1], out["reference"][1])
